@@ -2,19 +2,23 @@
 """bench.py - BASELINE.json's metric on BASELINE.json's config: LLaMA-7B w4-s45 decode tokens/s at batch 1
 (QuantLinear layers), plus the per-layer HBM roofline fraction.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload llama7b-w4-s45] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload llama7b-w4-s45] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" is one decode token's pass over the hot path: the 7 QuantLinearLUT matvecs (q, k, v, o, gate, up, down) of
 each of the model's decoder layers, in model order, chained through their real shapes (x -> q,k,v ; v -> o ; o -> gate,up ;
 gate -> down -> next layer's x), on synthetic random-init weights in the reference's buffer format (distinct per layer:
-3.6 GB per token for 7B w4-s45, far beyond the 126 MB L2, so every step streams from HBM).  Attention, norms, rotary,
+3.6 GB per token for 7B w4-s45, far beyond the 50 MB L2 of an H100, so every step streams from HBM).  Attention, norms, rotary,
 lm_head and the KV cache are NOT part of the step (they are not on the path this repo replaces) and that is stated in
 `config`.  As `llama.py --include_sparse` always runs (llama.py:301-306), sparse layers use the hybrid symbol with
 topX=10 dense rows that are zero (a checkpoint without them, llama.py:182).
 
-  value  : tokens/s, device-timed, inputs resident in HBM, one CUDA-graph replay per step; --steps K steps per timed block,
-           5 blocks, the MEDIAN block is reported (ms_per_step = median block / K; all block times are in `blocks_ms`).
+  value  : tokens/s, device-timed, inputs resident in HBM, one CUDA-graph replay per step; --steps K timed steps in all, cut
+           into --blocks (5) blocks as even as K allows; ms_per_step = the median over blocks of block time / its steps
+           (all block times are in `blocks_ms`).
+  --dump-outputs DIR: after the timed steps, what the timed step returned in its last step (the token's output vector)
+           as DIR/step_output.npy (float32), and DIR/step_output_lut_fp16.npy for the fp16 pair-table run.  Weights and
+           inputs come from fixed seeds, so two builds run with the same arguments can be compared output for output.
   lut_fp16: the same measurement with the fp16 pair-table mode of the kernel (quant_cuda.set_lut_mode("fp16"), north_star's
            "per-channel fp16 LUT"); the headline `value` always uses the exact fp32 codebook.  `--lut fp16` makes it the only run.
   parity_check: outside the timed region, one sampled layer group per rank against the fp64 CPU oracle on the same buffers.
@@ -69,7 +73,10 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, bf16 copy read+write)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return NOMINAL_HBM_GBS, "nominal (H100 SXM data sheet: 3.35 TB/s HBM3)"
+
+
+NOMINAL_HBM_GBS = 3350.0
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -316,7 +323,7 @@ def cpu_layer_sample(cfg, reps, seed=0):
 
 def leave(world):
     """Multi-rank exit.  destroy_process_group() can block for ever while CUDA graphs that captured NCCL kernels are alive
-    (seen on 2 x B200: both ranks stuck after the JSON line was out), so ranks leave without tearing the communicator down."""
+    (seen on two GPUs: both ranks stuck after the JSON line was out), so ranks leave without tearing the communicator down."""
     sys.stdout.flush()
     sys.stderr.flush()
     if world > 1:
@@ -381,19 +388,24 @@ def main():
     ap.add_argument("--launch", default="auto", choices=["auto", "seq", "graph"],
                     help="graph: one launch per (stacked) matvec, chained with PDL inside a CUDA graph; seq: the whole token as ONE persistent "
                          "kernel launch (runtime.DecodeSequence, csrc/lutgemv_seq.cuh; on several GPUs its input poll is the exchange); "
-                         "auto (default): what measured faster - graph on one GPU (547 vs 481 tokens/s), seq on several (509 vs 371 at N=2)")
+                         "auto (default): graph on one GPU, seq on several")
     ap.add_argument("--no-fuse", action="store_true", help="one launch per QuantLinearLUT (no q/k/v and gate/up sibling stacking)")
     ap.add_argument("--lut", default="both", choices=["both", "exact", "fp16"],
                     help="codebook precision: exact = fp32 as stored (headline), fp16 = pair tables; both = headline exact + a lut_fp16 object")
-    ap.add_argument("--blocks", type=int, default=5, help="timed blocks of --steps steps each; the median block is reported")
+    ap.add_argument("--blocks", type=int, default=5, help="timed blocks the --steps steps are cut into; the median per-step time of a block is reported")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="--impl ours only: write the timed step's output of its last step as DIR/<name>.npy (float32)")
     ap.add_argument("--per-shape", action="store_true",
                     help="also time each of the step's launch types on its own (one CUDA graph of `layers` launches over every layer's "
                          "distinct weights, CUDA events) and add a per_shape object: us per launch, GB/s and roofline fraction per type")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes what the GPU path computed; it applies to --impl ours only")
     cfg = dict(WORKLOADS[args.workload])
     if args.layers:
         cfg["layers"] = args.layers
     assert args.warmup >= 3, "timing rules: at least 3 warm-up steps"
+    assert args.steps >= 1, "--steps: at least one timed step"
 
     if args.impl == "reference":
         run_reference_arm(args, cfg)
@@ -482,7 +494,9 @@ def main():
 
     from squeezellm_b200.quant import quant_cuda
     from squeezellm_b200.runtime import GraphedDecodeStep
-    xh = torch.randn(cfg["hidden"]).half().pin_memory()
+    nblk = max(1, min(args.blocks, args.steps))
+    block_steps = [args.steps // nblk + (b < args.steps % nblk) for b in range(nblk)]  # --steps timed steps in all
+    xh = torch.randn(cfg["hidden"], generator=torch.Generator().manual_seed(98)).half().pin_memory()
     sampler = ClockSampler(torch.cuda.current_device() if "CUDA_VISIBLE_DEVICES" not in os.environ else local)
 
     def measure(lut_mode, sample_clocks):
@@ -506,10 +520,7 @@ def main():
             torch.cuda.synchronize()
 
         def one_step():
-            if graphed:
-                runner.replay()
-            else:
-                step(x0)
+            return runner.replay() if graphed else step(x0)
 
         for _ in range(args.warmup):
             one_step()
@@ -522,15 +533,16 @@ def main():
             barrier()
         if sample_clocks and rank == 0:
             sampler.start()
-        evs = [torch.cuda.Event(enable_timing=True) for _ in range(args.blocks + 1)]
+        evs = [torch.cuda.Event(enable_timing=True) for _ in range(len(block_steps) + 1)]
         evs[0].record()
-        for b in range(args.blocks):
-            for _ in range(args.steps):
-                one_step()
+        for b, n in enumerate(block_steps):
+            for _ in range(n):
+                y = one_step()
             evs[b + 1].record()
         barrier()
-        blocks = [evs[b].elapsed_time(evs[b + 1]) for b in range(args.blocks)]
+        blocks = [evs[b].elapsed_time(evs[b + 1]) for b in range(len(block_steps))]
         clocks = sampler.stop() if (sample_clocks and rank == 0) else None
+        y_last = y.float().cpu().numpy().reshape(-1)  # the timed step's output of its last step (before e2e reuses the buffers)
         # end to end from host memory through the public API
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         if graphed:
@@ -557,7 +569,7 @@ def main():
             t = torch.tensor(blocks + [e2e_ms], device=dev, dtype=torch.float64)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)  # every block: max over ranks
             blocks, e2e_ms = t.tolist()[:-1], t.tolist()[-1]
-        ms = statistics.median(blocks)
+        ms_step = statistics.median(b / n for b, n in zip(blocks, block_steps))
         quant_cuda.set_lut_mode("exact")
         seq_timeout = False
         if seq is not None:
@@ -566,8 +578,8 @@ def main():
                 print(f"[bench] rank {rank}: the sequence kernel's error word is set after the timed region - THIS RUN'S NUMBERS ARE VOID", file=sys.stderr)
             del runner, seq
             torch.cuda.empty_cache()
-        return {"seq_timeout": seq_timeout, "warm_timeout": warm_timeout, "ms_step": ms / args.steps, "e2e_ms_step": e2e_ms / args.steps, "blocks_ms": [round(b, 4) for b in blocks],
-                "graphed": graphed, "clocks": clocks}
+        return {"seq_timeout": seq_timeout, "warm_timeout": warm_timeout, "ms_step": ms_step, "e2e_ms_step": e2e_ms / args.steps, "blocks_ms": [round(b, 4) for b in blocks],
+                "graphed": graphed, "clocks": clocks, "y_last": y_last}
 
     def per_shape(lut_mode):
         """us per launch for each launch type of the step: a graph with one launch per decoder layer (every layer's own weights, LUT
@@ -579,7 +591,7 @@ def main():
                   ("down", ("down_proj",), "ffn")]
         out = {}
         for gname, names, kin in groups:
-            xin = torch.randn(cfg[kin], device=dev).half()
+            xin = torch.randn(cfg[kin], device=dev, generator=torch.Generator(device=dev).manual_seed(5)).half()
 
             def run():
                 for L in layers:
@@ -656,18 +668,19 @@ def main():
         leave(world)
         return
 
+    if args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "step_output.npy" if head_mode == "exact" else "step_output_lut_fp16.npy"), main_run["y_last"])
+        if extra_run is not None:
+            np.save(os.path.join(args.dump_outputs, "step_output_lut_fp16.npy"), extra_run["y_last"])
     ms_step = main_run["ms_step"]
     tok_s = 1e3 / ms_step
     e2e_tok_s = 1e3 / main_run["e2e_ms_step"]
     graphed = main_run["graphed"]
     peak, peak_src = peaks()
     achieved = nbytes / (ms_step * 1e-3) / 1e9  # per GPU: this rank's bytes over the step time
-    traffic = None
-    if world == 1:  # measured with ncu on the default single-GPU command (profiles/); not meaningful for column shards
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(args.workload)
-        except Exception:
-            pass
+    l2_mb = torch.cuda.get_device_properties(dev).L2_cache_size / 2**20
     kern = f"{'lutgemv_seq_kernel' if use_seq else 'lutgemv2_kernel'}<{cfg['bits']}, {'fp16 pair table' if head_mode == 'fp16' else 'exact fp32 table'}{'' if use_seq else ', fused'}>"
     launches = 2 if use_seq else nlaunch  # seq: token counter + the persistent kernel
     out = {
@@ -678,20 +691,21 @@ def main():
                   "f32 accumulate (fp32 LUT x fp16->fp32 activations, fp16 outputs)"), "data": "synthetic",
         "config": {**base_config(args, cfg), "launches_per_step": launches, "matvec_items_per_step": nlaunch,
                    "sibling_fusion": "q/k/v and gate/up stacked (squeezellm_b200.fusion)" if nlaunch != nmat else "off",
-                   "l2": f"{nbytes_all / 1e9:.2f} GB of distinct weights per step >> 126 MB L2 (inputs larger than L2)",
+                   "l2": f"{nbytes_all / 1e9:.2f} GB of distinct weights per step >> {l2_mb:.0f} MB L2 (inputs larger than L2)",
                    "parallelism": "single GPU" if world == 1 else f"column-sharded x{world}, {nlaunch} launches per step", "exchange": exchange_used,
                    "launch": ("one CUDA-graph replay per step" if graphed else "eager launches (graph capture unavailable)") +
                              (": ONE persistent kernel runs all matvecs of the token (runtime.DecodeSequence)" if use_seq else ": one PDL-chained launch per (stacked) matvec"),
-                   "lut": head_mode, "timing": f"median of {args.blocks} blocks of {args.steps} steps", "layers_timed": cfg["layers"]},
+                   "lut": head_mode, "timing": f"{args.steps} timed steps in {len(block_steps)} blocks, median per-step time of a block",
+                   "layers_timed": cfg["layers"]},
         "blocks_ms": main_run["blocks_ms"],
         "e2e": {"value": e2e_tok_s, "unit": "tokens/s", "h2d_bytes_per_step": cfg["hidden"] * 2, "d2h_bytes_per_step": cfg["hidden"] * 2,
                 "api": ("squeezellm_b200.runtime.GraphedDecodeStep over runtime.DecodeSequence (QuantLinearLUT modules)" if use_seq else
                         "squeezellm_b200.runtime.GraphedDecodeStep over QuantLinearLUT.forward") if graphed else "QuantLinearLUT.forward eager"},
         "gpu_launches": launches * args.steps,
         "clocks": main_run["clocks"],
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "peak_source": peak_src, "kernel": kern,
-                     "algorithmic_bytes_per_step_per_gpu": nbytes, "frac_of_nominal_8000": achieved / 8000.0},
+                     "algorithmic_bytes_per_step_per_gpu": nbytes, "frac_of_nominal": achieved / NOMINAL_HBM_GBS},
         "parity_check": parity,
     }
     if shapes is not None:

@@ -1,5 +1,5 @@
 /*
- * sqllm_b200.h - C ABI of the B200-native (sm_100a) dense-and-sparse LUT GEMV library
+ * sqllm_b200.h - C ABI of the H100-native (sm_90a) dense-and-sparse LUT GEMV library
  *                (libsqllm_b200.so), a from-scratch replacement for the hot path of
  *                SqueezeAILab/SqueezeLLM:  squeezellm/quant_cuda_kernel.cu + quant_cuda.cpp.
  *

@@ -9,12 +9,12 @@ Recipe for `oracle/_ref/` (git-ignored, travels to the GPU box with gpurun):
     `AT_DISPATCH_FLOATING_TYPES(mat.type(), ...)` at quant_cuda_kernel.cu:261,307,367,421,474,545,
     618,699 needs `mat.scalar_type()`.  The patch is applied by `sed` into a scratch directory
     under /tmp (8 sites, a dtype-dispatch macro argument only; no arithmetic is touched);
-  * the module is built under the name `quant_cuda_ref` (TORCH_EXTENSION_NAME) for sm_100 so it
+  * the module is built under the name `quant_cuda_ref` (TORCH_EXTENSION_NAME) for sm_90 (H100) so it
     can live in the same process as our own `quant_cuda`;
   * only the resulting `.so` is written to oracle/_ref/.
 
-The product (squeezellm_b200/, bench.py's own arm) never imports this.  Users: tests/ (parity vs the
-reference kernel on the B200), tests/golden/make_golden_gpu.py, oracle/ref_gpu_timing.py.
+The product (squeezellm_b200/, bench.py's own arm) never imports this.  Users: tests/golden/make_golden_gpu.py
+(stores the reference kernel's outputs as golden data for tests/), oracle/ref_gpu_timing.py.
 """
 import glob
 import os
@@ -66,7 +66,7 @@ def build(force=False):
         with open(os.path.join(tmp, "setup.py"), "w") as f:
             f.write(SETUP)
         env = dict(os.environ)
-        env["TORCH_CUDA_ARCH_LIST"] = "10.0"
+        env["TORCH_CUDA_ARCH_LIST"] = "9.0"
         env.setdefault("MAX_JOBS", "4")
         subprocess.check_call([sys.executable, "setup.py", "build_ext", "--inplace"], cwd=tmp, env=env)
         built = glob.glob(os.path.join(tmp, "quant_cuda_ref*.so"))

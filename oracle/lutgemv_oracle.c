@@ -11,7 +11,7 @@
  *       QuantLinearLUT.pack2 (squeezellm/quant.py:97-208) run in this container; the unpack below
  *       must reproduce the packed indices bit-exactly (tests/test_oracle_golden.py);
  *   (2) arithmetic: tests/golden/refkernel_*.npz are outputs of the reference's own kernels
- *       (oracle/_ref, built by oracle/build_ref.py) executed on a B200; the fp64 results below must
+ *       (oracle/_ref, built by oracle/build_ref.py) executed on an H100; the fp64 results below must
  *       agree with them to fp32-accumulation tolerance.
  *
  * Every function cites the reference lines it restates (paths relative to /root/reference).

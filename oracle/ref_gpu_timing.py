@@ -21,7 +21,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import build_ref  # noqa: E402
 from squeezellm_b200.quant import quant_cuda as qc  # noqa: E402
 
-PEAK = 6489.9
+PEAK = 3350.0  # H100 SXM data-sheet HBM3 bandwidth (GB/s), unless a measured peak is present
 try:
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:

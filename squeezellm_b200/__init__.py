@@ -1,4 +1,4 @@
-"""squeezellm_b200 - B200-native (sm_100a) drop-in for SqueezeLLM's dense-and-sparse LUT-GEMV hot path.
+"""squeezellm_b200 - H100-native (sm_90a) drop-in for SqueezeLLM's dense-and-sparse LUT-GEMV hot path.
 
 Public surface (mirrors the reference's squeezellm/quant.py):
     QuantLinearLUT, make_quant_lut, round_to_nearest_pole_sim      -> squeezellm_b200.quant

@@ -1,6 +1,6 @@
 """In-tree build of the two native artefacts (no JIT cache, so the .so files travel with the tree):
 
-  squeezellm_b200/libsqllm_b200.so                 CUDA kernels + C ABI   (nvcc, sm_100a only)
+  squeezellm_b200/libsqllm_b200.so                 CUDA kernels + C ABI   (nvcc, sm_90a only)
   squeezellm_b200/quant_cuda.<abi>.so              pybind11 adapter        (g++, links the above)
 
 `python -m squeezellm_b200.build` or `__graft_entry__.build()`.
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 INCLUDE = os.path.join(ROOT, "include")
 
-NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC"]  # fast-math deliberately NOT used
 
 

@@ -209,8 +209,8 @@ __global__ void csr_batched_kernel(const int *__restrict__ rows, const int *__re
 
 // topX dense rows for a batch: mul[b][fri[j]] += sum_k full_rows[k][j] * x[b][k].  One CTA per batch row; thread = (k-slice, dense row j):
 // 256 / topX slices of K walk their part with four independent fp32 chains, the slices' sums are added in fixed order through shared
-// memory (deterministic), one atomicAdd per (b, j).  (First build: one thread per (b, j) walking all K terms in fp64 - 0.37 ms of pure
-// latency whatever the batch, 3x SLOWER than the reference's kernels at batch 16: profiles/r02_batched_vs_reference_kernel.jsonl.)
+// memory (deterministic), one atomicAdd per (b, j).  (One thread per (b, j) walking all K terms in fp64 instead is pure
+// latency whatever the batch, slower than the reference's kernels at small batches.)
 __global__ void dense_rows_batched_kernel(const float *__restrict__ full_rows, const int *__restrict__ fri, int topX,
                                           const float *__restrict__ x, float *__restrict__ mul, int K, int N, int B) {
     __shared__ float part[256];

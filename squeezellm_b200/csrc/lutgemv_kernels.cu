@@ -1,4 +1,4 @@
-// lutgemv_kernels.cu - B200 (sm_100a) dense-and-sparse LUT GEMV, written from scratch.
+// lutgemv_kernels.cu - H100 (sm_90a) dense-and-sparse LUT GEMV, written from scratch.
 //
 // Replaces (behaviour, not code) squeezellm/quant_cuda_kernel.cu of SqueezeAILab/SqueezeLLM:
 //   VecQuant{3,4}MatMulKernelNUQPerChannel[Batched]  (:741-1038)   LUT GEMV
@@ -17,7 +17,7 @@
 //         the weight traffic of GEMV n+1 overlaps the tail of GEMV n), pulls the word-quad into registers and turns every
 //         4-bit index into an LDS address with a single PRMT (the per-strip LUT is staged transposed
 //         [value][column-slot] in a 4 KB aligned table so that every lane owns one shared-memory bank: conflict-free
-//         gathers); products go into packed fma.rn.f32x2 accumulators.  No tensor cores: this is a gather-bound GEMV.
+//         gathers); products go into pairs of fp32 accumulators (two fma.rn.f32 per pair).  No tensor cores: this is a gather-bound GEMV.
 //         (SQLLM_LDG=1: register ring fed by LDG.128; SQLLM_LDG=0: TMA producer warp + mbarrier ring - measured, not faster.)
 //       - sparse warp: CSR rows spread evenly over all CTAs, staged with 16-byte cp.async, x gathered in batches,
 //         per-row sums in storage order; plus a k-slice of the topX dense rows.
@@ -52,7 +52,7 @@ namespace {
 #endif
 #ifndef SQLLM_MINB4
 #define SQLLM_MINB4 3   // resident CTAs per SM the register budget must allow (shared memory admits 3; at 4 the 56-register
-                        // cap makes the compiler rematerialise table addresses inside the loop: 6-13 % slower, profiles/r01)
+                        // cap makes the compiler rematerialise table addresses inside the loop: measured slower)
 #endif
 #ifndef SQLLM_MINB3
 #define SQLLM_MINB3 3
@@ -204,8 +204,13 @@ __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
     return r;
 }
-__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) {  // Blackwell packed fp32 FMA
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
+// Two fp32 FMAs on a register pair.  Hopper has no packed fp32 FMA, so each half is one fma.rn.f32: the same rounding,
+// lane for lane, as a packed instruction would give, and the pair keeps two independent accumulation chains per column.
+__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) {
+    asm("{\n.reg .f32 a0, a1, b0, b1, c0, c1;\n"
+        "mov.b64 {a0, a1}, %1;\nmov.b64 {b0, b1}, %2;\nmov.b64 {c0, c1}, %0;\n"
+        "fma.rn.f32 c0, a0, b0, c0;\nfma.rn.f32 c1, a1, b1, c1;\n"
+        "mov.b64 %0, {c0, c1};\n}" : "+l"(acc) : "l"(a), "l"(b));
 }
 __device__ __forceinline__ float sum2(uint64_t v) {
     float lo, hi;
@@ -221,7 +226,7 @@ __device__ __forceinline__ float ldcg_f32(const float *p) { return __ldcg(p); }
 // Ticket: one gpu-scope acq_rel atomic.  The release half publishes everything the calling thread wrote - and, by
 // cumulativity, what the threads it synchronised with (bar.sync / __syncwarp) wrote before that barrier; the acquire half makes
 // the other contributors' published partials visible to whoever draws the last ticket (and, through the next barrier, to its
-// whole group).  This replaces the fence / atomic / fence triple (~1 us per fence on a busy B200).
+// whole group).  This replaces the fence / atomic / fence triple (a fence costs about a microsecond on a busy GPU).
 __device__ __forceinline__ int ticket_take(int *counter) {
     int old;
     asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(counter) : "memory");
@@ -893,7 +898,7 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
         }
         // ---- consumers: stage the LUTs of this CTA's strips, transposed to [value][slot].  One 128-bit load per (column, value
         //      quad); a warp takes 32 columns whose slots fall in 32 different banks, so the four scalar stores are conflict-free.
-        //      (4-byte cp.async would cost 16 shared-memory wavefronts per warp instruction - measured, profiles/r01.) ----
+        //      (4-byte cp.async would cost 16 shared-memory wavefronts per warp instruction - measured.) ----
         constexpr int IPS = STRIP * C::L / 4;                 // (column, quad) items per strip: 256 (w4) / 128 (w3)
         constexpr int LQ = (MAXSEG * IPS + NW * 32 - 1) / (NW * 32);  // items per thread at most
         float4 lq[LQ];
@@ -1151,7 +1156,7 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
         // Fast fused mode.  Every CTA announces "my red.adds are out" with one fire-and-forget red.release on a gpu-scope counter
         // and leaves.  The last `nfin` CTAs of the grid (by index - they are dispatched last) stay, wait until the counter reaches
         // the grid size, and each turns its 1/nfin slice of the accumulator into y (+ bias, converted) and re-zeroes it.  One CTA
-        // alone moves ~125 GB/s: 3.6 us for a 22016-wide layer (trace in profiles/r01); 16 of them need one L2 round trip.
+        // alone is too slow for a wide layer; 16 of them need one L2 round trip.
         // All CTAs of a launch are co-resident by construction (make_plan sizes the grid to the occupancy), so the wait cannot
         // deadlock; the counter is reset by the last finisher for the next launch (kernel boundary orders it).
         __syncthreads();  // all red.adds of this CTA issued

@@ -2,9 +2,9 @@
 // matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Included by lutgemv_kernels.cu after lutgemv_v2.cuh;
 // the per-position math, table builders, outlier warps and mailboxes are v2's (namespace v2), what is new is everything BETWEEN two GEMVs.
 //
-// Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer took 8.9 us in the chain for 1.5 us of HBM time; a fit over the
-// four 7B shapes gave ~6 us of fixed cost per launch (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
-// map fetch, x staging, ring fill from cold) - 128 launches per token, 40 % of the step (profiles/r02_bench_llama7b_w4_s45.json).  Here
+// Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
+// carries a fixed cost (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
+// map fetch, x staging, ring fill from cold) - 128 launches per token.  Here
 //   * grid = #SMs, launched ONCE per token; every CTA walks the same list of GEMV descriptors (global memory, written at create time);
 //   * the TMA producer warp never stops at a GEMV boundary: while the consumers finish GEMV g and wait for its result, the ring already
 //     holds the first 128 KB per SM of GEMV g+1 - weights do not depend on activations;
@@ -13,7 +13,7 @@
 //     straight out of L2 and repack them into fp16 in shared memory.  A stale word carries the previous token's tag, so nothing is ever
 //     reset.  The cross-CTA mailboxes of v2 carry a (token, GEMV) tag the same way.
 //   * on several GPUs (column shards) the owner of a strip stores its tagged words into EVERY rank's arena over NVLink; the poll of the
-//     next GEMV is the whole exchange - no collective, no flag round trip (v2's exchange waited ~10 us per launch on a system-scope flag).
+//     next GEMV is the whole exchange - no collective, no flag round trip (v2's exchange waits on a system-scope flag per launch).
 #pragma once
 
 #ifndef SQLLM_SEQ_POLL_NS
@@ -98,9 +98,9 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
 // ---------------------------------------------------------------------------------------------------------------------------
 // Outlier warps of the sequence kernel.  v2::sparse2 stages the (col, val) chunks in shared memory, forms the products in place and sums
 // rows from there: four or more DEPENDENT shared-memory round trips per chunk, each queueing for hundreds of cycles behind the consumers'
-// gathers (the LSU is what bounds the kernel) - the timeline of a 4096x4096 layer showed the outlier warps finishing 7 us after x arrived
-// for 510 non-zeros per CTA, 2.3 us after the last consumer warp: they, not the weights, set the layer's critical path
-// (profiles/r02_seq_trace_1.txt).  Here nothing but x goes through shared memory:
+// gathers (the LSU is what bounds the kernel) - the timeline of a 4096x4096 layer showed the outlier warps finishing well after x arrived
+// and after the last consumer warp: they, not the weights, set the layer's critical path
+// (tests/perf/seq_trace.cu).  Here nothing but x goes through shared memory:
 //   * LPR lanes share a row (LPR from the average row length), 32 / LPR rows per pass; a lane keeps its <= 8 (col, val) pairs of the
 //     pass in REGISTERS, loaded straight from global memory (L2: prefetched at entry) - everything static, so the first pass is in
 //     registers before x arrives and the loads of pass k+1 are issued before pass k is summed;
@@ -133,7 +133,7 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
     int r = 0, rb = 0;
     if (p.rows) {
         const int ca = min(N, (int)blockIdx.x * p.csr_rpc), cb = min(N, ca + p.csr_rpc);
-        // warp 0 has the dense rows (atomics + a fence before its announcement: ~2-3 us) and then takes no CSR rows: outlier sums are what
+        // warp 0 has the dense rows (atomics + a fence before its announcement) and then takes no CSR rows: outlier sums are what
         // the owners of ALL strips wait for, they must not queue behind that fence
         const int tot = cb - ca, w0 = p.full_rows ? 0 : tot / NSPW, rest = tot - w0;
         r = spw == 0 ? ca : ca + w0 + (int)((long long)rest * (spw - 1) / (NSPW - 1));
@@ -393,7 +393,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             // Strip sums of segment s go to the strip's owner: another CTA (mailbox row) if the strip started before our range, else ourselves -
             // and then they never leave the SM: sown[u][column] for the u-th owned strip (a strip inside one CTA is exactly one segment).
             // (v2 and the first sequence build sent them through the global accumulator - a RED and, in the finishing pass, a load that has to
-            // wait for it: 1.5 us of L2 round trips on the critical path between the last weight and y, profiles/r02_seq_trace_2.txt.)
+            // wait for it: L2 round trips on the critical path between the last weight and y.)
             const uint32_t sown = base + OFF_SROW;  // float [SOWN][64] (the row arrays of v2's outlier warps are not used by the sequence kernel)
             constexpr int SOWN = (2 * (SP_ROWS + 1) * 4) / (STRIP * 4);
             const int ofs = r0 != 0 ? 1 : 0;        // segment s is owned strip s - ofs
@@ -439,7 +439,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             int *const sdj = reinterpret_cast<int *>(sm + OFF_CSR);
             const uint32_t sden = base + OFF_CSR + 4 * 128, sdn_a = base + OFF_CSR + 8 * 128;
             if (p.full_rows) {
-                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads = 6 us for the 30
+                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads for the 30
                 //  dense rows of a stacked q/k/v layer - on every CTA, before its first mailbox row went out)
                 const int topX = p.topX;
                 if (bt == 0) sts_u32(sdn_a, 0u);

@@ -3,21 +3,20 @@
 //
 // Same job as lutgemv_kernel (v1): y[c] (+)= sum_k LUT[c][idx(k,c)] * x[k]  (+ CSR outliers + topX dense rows), replacing
 // squeezellm/quant_cuda_kernel.cu:741-880 (LUT GEMV), :1040-1059 (SPMV_ATOMIC), :1092-1123 (DenseMatVecKernel).
-// What changed and why (measurements: profiles/r02_*; [*] = measured on an intermediate build in the first session of round 2, whose container and raw logs were lost):
+// What changed and why:
 //   * grid = #SMs, 23 warps per CTA: 16 consumer warps, 1 TMA producer warp, 2 table-builder warps, 4 sparse warps.  v1 ran 3 CTAs x 8 consumer warps per SM;
-//     two thirds of its executed instructions on a 4096x4096 layer were per-CTA prologue/epilogue bookkeeping (ncu, r01).
+//     most of its executed instructions on a 4096x4096 layer were per-CTA prologue/epilogue bookkeeping.
 //   * weights arrive as 2-D TMA boxes (cp.async.bulk.tensor.2d): stages are aligned to the CTA's strip segments, so a full stage is
 //     ONE box of 64 columns x 32 units (8 KB / 24 KB) issued by one lane of the producer warp; the ragged last stage of a segment
-//     goes out as 2-unit boxes, one per lane (second tensor map), so nothing is over-fetched.  (First attempt: one 256-byte
-//     cp.async.bulk per row - 2.5x SLOWER than v1, the TMA unit retires a small copy every ~80 clocks: first session of round 2, log lost [*].)
+//     goes out as 2-unit boxes, one per lane (second tensor map), so nothing is over-fetched.  (One 256-byte cp.async.bulk
+//     per row instead was much slower: the TMA unit retires small copies slowly.)
 //     Nothing of this touches the LSU pipe, which bounds the gather loop (32 gathers + 4 word reads + 2-4 x reads per 1024 weights).
 //   * the CTA walks its strips one after the other with TWO table buffers in shared memory: the builder warps prepare the next strip's
 //     table in the background and move each finished strip's sums (red.shared.add by the consumer warps) on to global memory; the
 //     consumers never meet a CTA-wide barrier inside the loop.  Only two tables resident is what makes room for the
 //   * fp16 PAIR table (MODE 1): entry [a | b<<BITS] = half2(LUT[a], LUT[b]) - one PRMT-built (4-bit: the byte of the packed word IS
-//     the entry number) shared-memory lookup serves TWO weights, and the products go through fma.rn.f32.f16 (SASS FHFMA:
-//     fp16 x fp16 -> fp32 accumulate, exact products).  Measured 48.9 (49.5 on another box) weights/clk/SM against 27.0 for the exact fp32 table
-//     (tests/perf/microbench2.cu).  The only rounding is LUT -> fp16 (2^-11 relative per centroid); it needs fp16 x.
+//     the entry number) shared-memory lookup serves TWO weights, and the products are fp16 x fp16 -> fp32 accumulate with
+//     exact products (fhfma2; tests/perf/microbench2.cu measures the loop).  The only rounding is LUT -> fp16 (2^-11 relative per centroid); it needs fp16 x.
 //   * x is staged whole (as fp16 when it is given as fp16), the sparse warps gather it from shared memory.
 #pragma once
 
@@ -107,9 +106,12 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
     return v;
 }
 __device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-// acc_lo += lo16(w) * lo16(x) ; acc_hi += hi16(w) * hi16(x)   (fp16 x fp16 products are exact in fp32; SASS: FHFMA with .H0/.H1 selectors)
+// acc_lo += lo16(w) * lo16(x) ; acc_hi += hi16(w) * hi16(x).  Hopper has no fp16 x fp16 -> fp32 FMA: the halves are widened
+// (exact) and go through fma.rn.f32.  An fp16 x fp16 product is exact in fp32, so the single rounding is the accumulation's.
 __device__ __forceinline__ void fhfma2(float &acc_lo, float &acc_hi, uint32_t w, uint32_t x) {
-    asm("{\n.reg .b16 wl, wh, xl, xh;\nmov.b32 {wl, wh}, %2;\nmov.b32 {xl, xh}, %3;\nfma.rn.f32.f16 %0, wl, xl, %0;\nfma.rn.f32.f16 %1, wh, xh, %1;\n}"
+    asm("{\n.reg .b16 wl, wh, xl, xh;\n.reg .f32 fwl, fwh, fxl, fxh;\nmov.b32 {wl, wh}, %2;\nmov.b32 {xl, xh}, %3;\n"
+        "cvt.f32.f16 fwl, wl;\ncvt.f32.f16 fwh, wh;\ncvt.f32.f16 fxl, xl;\ncvt.f32.f16 fxh, xh;\n"
+        "fma.rn.f32 %0, fwl, fxl, %0;\nfma.rn.f32 %1, fwh, fxh, %1;\n}"
         : "+f"(acc_lo), "+f"(acc_hi) : "r"(w), "r"(x));
 }
 __device__ __forceinline__ uint64_t half2_to_f32x2(uint32_t h) {
@@ -131,19 +133,19 @@ __device__ __forceinline__ uint32_t f32x2_to_half2(float lo, float hi) {
 // Tables are built by the two builder warps (thread = slot = one column of the strip) from the strip's raw LUT rows, which they stage
 // in shared memory first (lut_prefetch, zero-filled past N): a build never waits on global memory, and it runs in the background -
 // the consumers only ever wait on an mbarrier that is normally long complete.  (First v2 build: the consumers rebuilt the table
-// themselves at every strip boundary; ncu showed 24 % of all stall samples on the LUT loads and a 0.8 / 2.3 us bubble per switch.)
+// themselves at every strip boundary; that left a bubble per switch with the warps stalled on the LUT loads.)
 // ---------------------------------------------------------------------------------------------------------------------------
 // Mailboxes (fused mode, SQLLM_BOX).  A sum that one CTA produces and another CTA needs - the partial strip sums of a CTA whose first
 // segment continues a strip started earlier, and every outlier row sum (the CSR rows are spread evenly over the CTAs) - is written
 // ONCE, as one 64-bit word {fp32 value, valid = 1}, and the strip's owner polls that word.  A 64-bit access is single-copy atomic, so
 // the value needs no fence and no separate flag: the word validates itself.  Before: red.add into the accumulator, MEMBAR, flag
 // increment on the producer; acquire-poll of the flag, then a second round trip for the accumulator on the owner - three L2 round
-// trips (~2.5 us under load) between the last weight of a launch and its last y, now one.  The owner writes the word back to zero
+// trips under load between the last weight of a launch and its last y, now one.  The owner writes the word back to zero
 // (next launch's producers only write after the grid dependency resolved).  The dense-row sums travel the same way since the second
 // half of round 2: one word per (contributing CTA, dense row) - rows that feed the same channel are combined in the contributing warp -
 // summed by the owner of the channel's strip; and the owner's OWN strip sums never leave the SM (sown, a shared-memory row per owned
 // strip).  Before: red.add into the global accumulator + MEMBAR.GPU + one announcement per strip on the producers, an acquire-poll and a
-// load of the accumulator behind it on the owner (7B w4-s45: 519.7 -> 547.0 tokens/s, profiles/r02_bench_llama7b_w4_s45.json).
+// load of the accumulator behind it on the owner.
 // ---------------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long *p) {
     unsigned long long v;
@@ -174,8 +176,7 @@ __device__ __forceinline__ float box_take(unsigned long long w, unsigned long lo
 
 // Staging layout: the row of column c sits at slot(c) * (L*4 + 16) bytes.  The builders read it with 16-byte loads, lane = slot: with the
 // rows packed by column (stride 4 columns x 64 B = 256 B between adjacent lanes) every LDS.128 was an 8-way bank conflict, and the
-// pair-table build re-reads the row for each of its 16 outer steps - ncu: 1.18 M of the fp16 kernel's 3.69 M shared-memory wavefronts
-// were these conflicts (first session of round 2, log lost [*]), as much LSU time as a third of the gathers.  With an 80-byte
+// pair-table build re-reads the row for each of its 16 outer steps, so these conflicts cost LSU time the gathers need.  With an 80-byte
 // (4-bit) / 48-byte (3-bit) stride the 8 lanes of each 128-byte phase cover all 32 banks.
 template <int BITS>
 __device__ __forceinline__ void lut_prefetch(const P2 &p, const uint32_t lutbuf, const int strip, const int bt) {
@@ -423,7 +424,7 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
     }
     int r, rb;
     {
-        // warp 0 also has the dense rows (atomics, a fence, the announcement: 2-3 us after x arrives).  sp_w0 = 0 (default): it then takes no CSR
+        // warp 0 also has the dense rows (atomics, a fence, the announcement after x arrives).  sp_w0 = 0 (default): it then takes no CSR
         // rows at all - the outlier sums are what the owners of ALL strips wait for, they must not queue behind that fence; 1: half a share (round-2
         // first build; A/B with SQLLM_SP_W0=1)
         const int tot = cb - ca, w0 = p.full_rows ? (p.sp_w0 ? tot / (2 * NSPW) : 0) : tot / NSPW, rest = tot - w0;
@@ -451,10 +452,10 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
         e_hi = __ldg(p.rows + rb);
     }
     // This warp's non-zeros [e_lo, e_hi) go to L2 right away (a CTA has ~5-25 KB of outliers and only two small chunks per warp fit the
-    // staging buffers: under a saturated HBM every further chunk would otherwise cost a DRAM round trip of 2-3 us), and are then walked
+    // staging buffers: under a saturated HBM every further chunk would otherwise cost a DRAM round trip), and are then walked
     // in chunks of SP_CH staged with 16-byte cp.async into two buffers.  Shared-memory accesses of these warps queue behind the
     // consumers' (the LSU pipe is what bounds the kernel), i.e. each dependent access costs hundreds of cycles: that is why there are
-    // NSPW warps with independent chains (one warp: 14 us for 3200 non-zeros) and why every step below batches independent loads.
+    // NSPW warps with independent chains (one warp alone sets the critical path) and why every step below batches independent loads.
     for (int e = (e_lo & ~31) + 32 * lane; e < e_hi; e += 32 * 32) {
         asm volatile("prefetch.global.L2 [%0];" ::"l"(p.cols + e));
         asm volatile("prefetch.global.L2 [%0];" ::"l"(p.vals + e));
@@ -531,7 +532,7 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
             if constexpr (BOX) {
                 // this CTA's part of dense row j: one self-validating word, no RED + fence + flag (the owner of the channel's strip sums the hc words of
                 // row j, lutgemv2_kernel's finishers); before: atomics into the accumulator, a MEMBAR.GPU and an announcement per strip - the fence
-                // alone held this warp for 1-2 us, and with it every owner that waited for the announcement
+                // alone held this warp, and with it every owner that waited for the announcement
                 if (j < p.topX) st_relaxed_u64(p.ws_dbox + (size_t)j * MAX_GRID_V2 + blockIdx.x, box_word(a));
             } else if (j < p.topX) {
                 const int c = __ldg(p.fri + j);
@@ -709,8 +710,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     pdl_launch_dependents();
     if (warp == WARP_PROD) {
         // Cold-start latencies (a decode step finds none of a layer's arrays in L2): ask for the two tensor-map descriptors now, and let
-        // every CTA pull a 1/grid slice of the layer's look-up table and row pointers into L2 - the CTAs of a launch start up to ~4 us
-        // apart (they inherit their SM from the previous kernel's CTAs), so the late ones find what the early ones asked for.
+        // every CTA pull a 1/grid slice of the layer's look-up table and row pointers into L2 - the CTAs of a launch start at different
+        // times (they inherit their SM from the previous kernel's CTAs), so the late ones find what the early ones asked for.
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_big)) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_small)) : "memory");
@@ -742,8 +743,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     if (warp == WARP_PROD) {
         // =========================== TMA producer: weights never depend on the previous kernel ===========================
         // Stages never straddle a strip: segment `seg` (the CTA's part of strip s0+seg) is cut into stages of SU2 units from its own start.
-        // (Also tried: cp.async.bulk.prefetch.tensor into L2 16-24 stages ahead of the ring - 5-10 % slower on every shape, like the
-        // L2 prefetch experiment of round 1: first session of round 2, log lost [*].)
+        // (Also tried: cp.async.bulk.prefetch.tensor into L2 16-24 stages ahead of the ring - slower on every shape, like the
+        // L2 prefetch experiment of round 1.)
         const uint64_t pol = l2_evict_first_policy();
         int slot = 0;
         uint32_t ph = 0;
@@ -799,7 +800,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                 // (that can only be its first segment) hands its sums to that owner through its mailbox row.
                 // ... or to ourselves: then they never leave the SM (sown[u][column] for the u-th owned strip; a strip inside one CTA is exactly
                 // one segment).  Through the global accumulator (first round-2 build) that was a RED and, in the finishing pass, a load that had to
-                // wait for it - two L2 round trips of 1-2.5 us each between the last weight and y when the last segment is short.
+                // wait for it - two L2 round trips between the last weight and y when the last segment is short.
                 if (s == 0 && r0 != 0) st_relaxed_u64(p.ws_hbox + (size_t)blockIdx.x * STRIP + bt, box_word(v));
                 else if (s - (r0 != 0 ? 1 : 0) < SOWN) sts_u32(sown + 4u * (uint32_t)((s - (r0 != 0 ? 1 : 0)) * STRIP + bt), __float_as_uint(v));
                 else if (col < N) atomicAdd(acc_out + col, v);
@@ -860,7 +861,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             int *const sdj = reinterpret_cast<int *>(sm + OFF_FIN + 2048);
             const uint32_t sden = base + OFF_FIN + 2048 + 4 * 128, sdn_a = base + OFF_FIN + 2048 + 8 * 128;
             if (p.full_rows) {
-                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads = 6 us for the 30
+                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads for the 30
                 //  dense rows of a stacked q/k/v layer - on every CTA, before its first mailbox row went out)
                 const int topX = p.topX;
                 if (bt == 0) sts_u32(sdn_a, 0u);
@@ -1248,7 +1249,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
 #else
             // one stage per trip, no look-ahead: the smallest loop body.  (The two-stage ping-pong variant above hides the word fetch
             // behind the previous position's gathers but doubles the body to ~290 instructions; with 23 warps in five roles on the SM
-            // the instruction cache misses ate the gain - ncu: 18 % of the stall samples "no instruction" - see profiles/r02_*.)
+            // the instruction cache misses ate the gain - ncu showed many stall samples on "no instruction".)
             for (int k = 0; k < nstg; ++k) {
                 mbar_wait(bar_u32 + 8 * slot, par);
                 if (k < mine) {

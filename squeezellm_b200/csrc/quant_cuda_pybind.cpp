@@ -344,7 +344,7 @@ torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-    m.doc() = "B200-native drop-in for SqueezeLLM's quant_cuda extension";
+    m.doc() = "H100-native drop-in for SqueezeLLM's quant_cuda extension";
     // the reference's 12 symbols (squeezellm/quant_cuda.cpp:258-269), same names and positional order
     m.def("vecquant3matmul_nuq_perchannel", &dense<3, false>, "3-bit per-channel LUT matvec (accumulates into mul)");
     m.def("vecquant4matmul_nuq_perchannel", &dense<4, false>, "4-bit per-channel LUT matvec (accumulates into mul)");

@@ -1,5 +1,5 @@
 """QuantLinearLUT / make_quant_lut - host-side mirror of the reference's module interface
-(squeezellm/quant.py:28-435) on top of the B200-native `quant_cuda` extension.
+(squeezellm/quant.py:28-435) on top of the H100-native `quant_cuda` extension.
 
 Same class name, constructor signature, buffer names (= checkpoint keys: qweight, lookup_table, bias,
 rows, cols, vals, full_rows, full_row_indices, startrows), `pack2`, `forward` and `make_quant_lut`
@@ -43,7 +43,7 @@ def _load_extension():
     if not cands:
         raise ImportError(
             "squeezellm_b200: the compiled CUDA extension `quant_cuda` is missing; build it with "
-            "`python -m squeezellm_b200.build` (needs nvcc, sm_100a). No CPU fallback exists.")
+            "`python -m squeezellm_b200.build` (needs nvcc, sm_90a). No CPU fallback exists.")
     spec = importlib.util.spec_from_file_location("quant_cuda", cands[0])
     mod = importlib.util.module_from_spec(spec)
     try:

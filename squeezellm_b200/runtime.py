@@ -1,14 +1,14 @@
 """Decode-time runtime helpers around QuantLinearLUT (public API).
 
 `GraphedDecodeStep` turns a token step made of QuantLinearLUT calls (224 of them per LLaMA-7B token, each a
-~2-10 us kernel) into ONE CUDA-graph replay with static device buffers and pinned host staging:
+short kernel) into ONE CUDA-graph replay with static device buffers and pinned host staging:
 
     runner = GraphedDecodeStep(step_fn, example_x)      # captures step_fn(x_dev) -> y_dev
     y_host = runner(x_host)                             # H2D copy, replay, D2H copy, all on one stream
 
 It exists because the reference drives the path from Python one launch at a time on the legacy stream
-(llama.py:226-234, quant_cuda_kernel.cu:147), which costs more host time per call than the kernels take on a
-B200; our kernels launch on the current stream precisely so that they can be captured.
+(llama.py:226-234, quant_cuda_kernel.cu:147), which costs more host time per call than the kernels take on an
+H100; our kernels launch on the current stream precisely so that they can be captured.
 """
 import torch
 

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

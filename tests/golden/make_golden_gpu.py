@@ -1,14 +1,19 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/refkernel_*.npz on a B200: outputs of the REFERENCE's own CUDA kernels
-(oracle/_ref/quant_cuda_ref*.so, built by oracle/build_ref.py from /root/reference with the 8-site dtype patch).
+"""Generate golden outputs of the REFERENCE's own CUDA kernels on an H100 (oracle/_ref/quant_cuda_ref*.so, built by
+oracle/build_ref.py from a reference checkout with the 8-site dtype patch):
 
-    gpurun -- 'python tests/golden/make_golden_gpu.py'      # writes gpurun_out/golden/*.npz; copy them to tests/golden/
+    python tests/golden/make_golden_gpu.py [--out DIR]      # default DIR: tests/golden
 
-Each file holds the inputs (reference buffer format), the initial `mul`, and `mul_out` after calling the
-reference symbol that squeezellm/quant.py would pick.  They pin the CPU oracle's arithmetic
-(tests/test_oracle_golden.py::test_oracle_matches_reference_kernel_outputs).  Shapes respect the reference's
-unchecked preconditions (in % 128 == 0, out % 128 == 0).  Kept small so the fixtures stay a few hundred KB.
+refkernel_<case>.npz: the inputs (reference buffer format), the initial `mul`, and `mul_out` after calling the reference
+symbol that squeezellm/quant.py would pick.  They pin the CPU oracle's arithmetic
+(tests/test_oracle_golden.py::test_oracle_matches_reference_kernel_outputs).  Kept small so the fixtures stay a few hundred KB.
+
+reference_outputs.npz: for every case of tests/test_gpu_parity.py that compares with the reference kernels, the reference's
+output at the positions tests/util.py:sample_idx keeps, and max |output| over the whole output (key + "__absmax").  The inputs
+are not stored: the tests rebuild them from the same seeds (matvec_inputs / batched_inputs).
+Shapes respect the reference's unchecked preconditions (in % 128 == 0, out % 128 == 0).
 """
+import argparse
 import os
 import sys
 
@@ -20,6 +25,8 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import build_ref  # noqa: E402
 import oracle as orc  # noqa: E402
+import test_gpu_parity as t  # noqa: E402
+from util import sample_idx, to_torch  # noqa: E402
 
 CASES = [  # name, bits, K, N, sparsity, topX, nonzero_full_rows, batch
     ("w4_dense", 4, 256, 128, 0.0, 0, False, 1),
@@ -33,26 +40,20 @@ CASES = [  # name, bits, K, N, sparsity, topX, nonzero_full_rows, batch
 ]
 
 
-def main():
-    ref = build_ref.load()
-    out = os.path.join(ROOT, "gpurun_out", "golden")
-    os.makedirs(out, exist_ok=True)
+def call(ref, L, xv, mul, batched):
+    """The reference symbol squeezellm/quant.py would pick, chosen exactly as the parity tests choose it."""
+    t._module_call(ref, to_torch(L), xv, mul, batched)
+    torch.cuda.synchronize()
+
+
+def oracle_cases(ref, out):
     for name, bits, K, N, sp, topx, nz, batch in CASES:
         L = orc.make_layer(bits, K, N, sparsity=sp, topX=topx, seed=100 + CASES.index((name, bits, K, N, sp, topx, nz, batch)), nonzero_full_rows=nz)
         x = orc.make_vec(K, batch=batch, seed=17)
         init = (np.random.default_rng(5).standard_normal((batch, N)) * 0.5).astype(np.float32)
-        T = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) else v) for k, v in L.items()}
         xv = torch.from_numpy(x).cuda() if batch > 1 else torch.from_numpy(x).cuda().reshape(-1)
         mul = torch.from_numpy(init.copy()).cuda() if batch > 1 else torch.from_numpy(init.copy()).cuda().reshape(-1)
-        sfx = "_batched" if batch > 1 else ""
-        if L["rows"] is not None and L["full_rows"] is not None:
-            getattr(ref, f"vecquant{bits}matmul_spmv_hybrid_nuq_perchannel{sfx}")(
-                T["rows"], T["cols"], T["vals"], xv, T["full_rows"], T["full_row_indices"], mul, N, T["qweight"], T["lookup_table"])
-        elif L["rows"] is not None:
-            getattr(ref, f"vecquant{bits}matmul_spmv_nuq_perchannel{sfx}")(T["rows"], T["cols"], T["vals"], xv, mul, N, T["qweight"], T["lookup_table"])
-        else:
-            getattr(ref, f"vecquant{bits}matmul_nuq_perchannel{sfx}")(xv, T["qweight"], mul, T["lookup_table"])
-        torch.cuda.synchronize()
+        call(ref, L, xv, mul, batch > 1)
         d = dict(bits=bits, K=K, N=N, vec=x, mul_init=init, mul_out=mul.cpu().numpy().reshape(batch, N))
         for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices"):
             if L[k] is not None:
@@ -60,6 +61,42 @@ def main():
         np.savez_compressed(os.path.join(out, f"refkernel_{name}.npz"), **d)
         e = np.abs(d["mul_out"] - orc.forward_f64(L, x, mul_init=init)).max()
         print(f"{name}: max |ref_kernel - oracle_f64| = {e:.3e}")
+
+
+def parity_cases(ref, out):
+    g = {}
+
+    def keep(key, y):
+        y = y.cpu().numpy().reshape(-1)
+        g[key] = y[sample_idx(y.size)].astype(np.float32)
+        g[key + "__absmax"] = np.float64(np.abs(y).max())
+
+    for shape, sid in zip(t.SHAPES, t.IDS):
+        if t.ref_comparable(shape):
+            L, x = t.matvec_inputs(shape)
+            y = torch.zeros(shape[2], device="cuda")
+            call(ref, L, torch.from_numpy(x).cuda(), y, False)
+            keep("mv__" + sid, y)
+    for shape in t.BATCHED_SHAPES:
+        if t.ref_comparable(shape):
+            for batch in t.BATCHES:
+                L, x = t.batched_inputs(shape, batch)
+                y = torch.zeros((batch, shape[2]), device="cuda")
+                call(ref, L, torch.from_numpy(x).cuda(), y, True)
+                keep(f"b{batch}__{t.batched_id(shape)}", y)
+    np.savez_compressed(os.path.join(out, "reference_outputs.npz"), **g)
+    print(f"reference_outputs.npz: {len(g) // 2} outputs")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=os.path.join(ROOT, "tests", "golden"))
+    args = ap.parse_args()
+    os.makedirs(args.out, exist_ok=True)
+    ref = build_ref.load()
+    print(torch.cuda.get_device_name(0))
+    oracle_cases(ref, args.out)
+    parity_cases(ref, args.out)
 
 
 if __name__ == "__main__":

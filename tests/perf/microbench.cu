@@ -1,9 +1,9 @@
-// microbench.cu - isolates the two halves of the LUT GEMV on a B200 (standalone, no torch):
+// microbench.cu - isolates the two halves of the LUT GEMV (standalone, no torch; sm_90a):
 //   stream : read a [rows x N] int32 matrix with the kernel's access pattern (strip-major stream-K chunks,
 //            STRIPW-column row segments), LDG.128 with U loads in flight per lane, no compute
 //   lookup : the 4-bit gather + packed-FMA inner loop on register-resident words (no global traffic),
 //            tables and x in shared memory, W warps per CTA, B CTAs per SM
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o microbench microbench.cu
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o microbench microbench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -72,9 +72,12 @@ __global__ void flat_kernel(const uint4 *__restrict__ q, size_t n4, uint32_t *ou
 __device__ __forceinline__ float lds_f32(uint32_t a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a)); return v; }
 __device__ __forceinline__ float4 lds_v4(uint32_t a) { float4 v; asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a)); return v; }
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) { uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b)); }
+__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) {  // two fma.rn.f32: Hopper has no packed fp32 FMA
+    asm("{\n.reg .f32 a0, a1, b0, b1, c0, c1;\nmov.b64 {a0, a1}, %1;\nmov.b64 {b0, b1}, %2;\nmov.b64 {c0, c1}, %0;\n"
+        "fma.rn.f32 c0, a0, b0, c0;\nfma.rn.f32 c1, a1, b1, c1;\nmov.b64 %0, {c0, c1};\n}" : "+l"(acc) : "l"(a), "l"(b));
+}
 
-template <int MODE>  // 0: PRMT + LDS + FFMA2 (the kernel's loop) ; 1: LDS only (no FMA) ; 2: scalar FFMA instead of FFMA2
+template <int MODE>  // 0: PRMT + LDS + ffma2 pairs (the kernel's loop) ; 1: LDS only (no FMA) ; 2: scalar FFMA chains
 __global__ void lookup_kernel(int iters, float *out) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char *sm = (unsigned char *)(((uintptr_t)smem_raw + 4095) & ~(uintptr_t)4095);

@@ -1,10 +1,10 @@
-// microbench2.cu - round-2 design probes on a B200 (standalone, no torch):
-//   pair    : the fp16 pair-table gather loop (one PRMT + one LDS.32 per TWO 4-bit weights, two mixed-precision
-//             fma.rn.f32.f16 = SASS FHFMA per pair) against the exact loop (one PRMT + LDS.32 per weight, FFMA2)
-//   fhfma   : issue rate of FHFMA alone (is it a full-rate FMA-pipe instruction?)
+// microbench2.cu - design probes (standalone, no torch; sm_90a):
+//   pair    : the fp16 pair-table gather loop (one PRMT + one LDS.32 per TWO 4-bit weights, two fp16 -> fp32
+//             widenings + fma.rn.f32 per weight) against the exact loop (one PRMT + LDS.32 per weight, FFMA)
+//   fhfma   : issue rate of the widen + FMA pair alone
 //   stream  : LDG.128 stream with 32- / 64- / 128-column row segments (DRAM efficiency of narrow strips)
 //   cluster : how many SMs a cluster launch can use (cudaOccupancyMaxActiveClusters for sizes 2, 4, 8)
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o microbench2 microbench2.cu
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o microbench2 microbench2.cu
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -18,21 +18,25 @@ __device__ __forceinline__ float lds_f32(uint32_t a) { float v; asm volatile("ld
 __device__ __forceinline__ float4 lds_v4(uint32_t a) { float4 v; asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a)); return v; }
 __device__ __forceinline__ uint4 lds_u4(uint32_t a) { uint4 v; asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; }
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) { uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b)); }
-// d += lo16(a)*lo16(b) ; d += hi16(a)*hi16(b)   (fp16 x fp16 -> fp32 accumulate: SASS FHFMA with .H0/.H1 operand selectors)
+__device__ __forceinline__ void ffma2(uint64_t &acc, uint64_t a, uint64_t b) {  // two fma.rn.f32: Hopper has no packed fp32 FMA
+    asm("{\n.reg .f32 a0, a1, b0, b1, c0, c1;\nmov.b64 {a0, a1}, %1;\nmov.b64 {b0, b1}, %2;\nmov.b64 {c0, c1}, %0;\n"
+        "fma.rn.f32 c0, a0, b0, c0;\nfma.rn.f32 c1, a1, b1, c1;\nmov.b64 %0, {c0, c1};\n}" : "+l"(acc) : "l"(a), "l"(b));
+}
+// d += lo16(a)*lo16(b) ; d += hi16(a)*hi16(b)   (fp16 x fp16 -> fp32 accumulate; Hopper: widen (exact) + fma.rn.f32)
+#define FH_WIDEN "{\n.reg .b16 al, ah, bl, bh;\n.reg .f32 fal, fah, fbl, fbh;\nmov.b32 {al, ah}, %2;\nmov.b32 {bl, bh}, %3;\n" \
+                 "cvt.f32.f16 fal, al;\ncvt.f32.f16 fah, ah;\ncvt.f32.f16 fbl, bl;\ncvt.f32.f16 fbh, bh;\n"
 __device__ __forceinline__ void fhfma_pair(float &acc, uint32_t a, uint32_t b) {
-    asm("{\n.reg .b16 al, ah, bl, bh;\nmov.b32 {al, ah}, %1;\nmov.b32 {bl, bh}, %2;\nfma.rn.f32.f16 %0, al, bl, %0;\nfma.rn.f32.f16 %0, ah, bh, %0;\n}"
-        : "+f"(acc) : "r"(a), "r"(b));
+    float unused = 0.f;
+    asm(FH_WIDEN "fma.rn.f32 %0, fal, fbl, %0;\nfma.rn.f32 %0, fah, fbh, %0;\n}" : "+f"(acc), "+f"(unused) : "r"(a), "r"(b));
 }
 __device__ __forceinline__ void fhfma_pair2(float &acc0, float &acc1, uint32_t a, uint32_t b) {  // two chains
-    asm("{\n.reg .b16 al, ah, bl, bh;\nmov.b32 {al, ah}, %2;\nmov.b32 {bl, bh}, %3;\nfma.rn.f32.f16 %0, al, bl, %0;\nfma.rn.f32.f16 %1, ah, bh, %1;\n}"
-        : "+f"(acc0), "+f"(acc1) : "r"(a), "r"(b));
+    asm(FH_WIDEN "fma.rn.f32 %0, fal, fbl, %0;\nfma.rn.f32 %1, fah, fbh, %1;\n}" : "+f"(acc0), "+f"(acc1) : "r"(a), "r"(b));
 }
 
-// MODE 0: exact   - per word 8 x (PRMT + LDS.32) + 4 FFMA2, x as 2 LDS.128 of fp32            (the round-1 loop)
-// MODE 1: pair16  - per word 4 x (PRMT + LDS.32) + 8 FHFMA,  x as 1 LDS.128 of 8 halves       (table [256][64 slots] half2 = 64 KB)
+// MODE 0: exact   - per word 8 x (PRMT + LDS.32) + 8 FFMA, x as 2 LDS.128 of fp32             (the round-1 loop)
+// MODE 1: pair16  - per word 4 x (PRMT + LDS.32) + 8 x (widen + FFMA), x as 1 LDS.128 of 8 halves (table [256][64 slots] half2 = 64 KB)
 // MODE 2: pair16 lookups only (no FMA)                                                          (LSU bound of the pair gather)
-// MODE 3: pair16 with cvt + FFMA2 instead of FHFMA (2 HADD2.F32 + FFMA2 per pair, x fp32)
+// MODE 3: pair16 with the table pair converted once + FFMA against fp32 x
 template <int MODE>
 __global__ void lookup_kernel(int iters, float *out) {
     extern __shared__ unsigned char smem_raw[];
@@ -101,8 +105,8 @@ __global__ void lookup_kernel(int iters, float *out) {
     if (s == 1234.5f) out[0] = s;
 }
 
-// FHFMA issue rate: 16 independent chains per thread, no memory
-template <int KIND>  // 0: FHFMA  1: FFMA  2: FFMA2
+// FMA rate of the three product helpers: 16 independent chains per thread, no memory
+template <int KIND>  // 0: fhfma_pair2 (fp16 widen + FFMA)  1: FFMA  2: ffma2 (two FFMA on a register pair)
 __global__ void fma_kernel(int iters, float *out, uint32_t a0, uint32_t b0) {
     float f[16];
     uint64_t g[8];
@@ -185,8 +189,8 @@ void run_lookup(const char *name, int sms, float *dout) {
         if (real < occ) continue;
         float ms = time_ms([&] { lookup_kernel<MODE><<<sms * occ, warps * 32, smem>>>(iters, dout); }, 3);
         const double weights = (double)sms * occ * warps * 32 * 32.0 * iters;
-        printf("%-28s CTAs/SM=%d warps/CTA=%2d : %6.2f Tweights/s = %5.1f weights/clk/SM @1.965 GHz\n", name, occ, warps, weights / ms / 1e9,
-               weights / ms / sms / 1.965e6);
+        printf("%-30s CTAs/SM=%d warps/CTA=%2d : %6.2f Tweights/s = %6.1f Gweights/s/SM\n", name, occ, warps, weights / ms / 1e9,
+               weights / ms / sms / 1e6);
     }
 }
 
@@ -197,10 +201,10 @@ int main() {
     printf("SMs %d\n", sms);
     float *dout; CK(cudaMalloc(&dout, 64));
 
-    run_lookup<0>("exact PRMT+LDS+FFMA2", sms, dout);
-    run_lookup<1>("pair16 PRMT+LDS+2xFHFMA", sms, dout);
+    run_lookup<0>("exact PRMT+LDS+FFMA", sms, dout);
+    run_lookup<1>("pair16 PRMT+LDS+widen+FFMA", sms, dout);
     run_lookup<2>("pair16 lookups only", sms, dout);
-    run_lookup<3>("pair16 cvt+FFMA2", sms, dout);
+    run_lookup<3>("pair16 cvt once+FFMA", sms, dout);
 
     for (int warps : {4, 8, 16}) {
         const int iters = 20000;
@@ -208,8 +212,8 @@ int main() {
         float m1 = time_ms([&] { fma_kernel<1><<<sms, warps * 32>>>(iters, dout, 0x3f800000u, 0x3f800000u); }, 3);
         float m2 = time_ms([&] { fma_kernel<2><<<sms, warps * 32>>>(iters, dout, 0x3f800000u, 0x3f800000u); }, 3);
         const double n = (double)sms * warps * 32 * iters;
-        printf("fma issue, %2d warps/SM: FHFMA %.1f  FFMA %.1f  FFMA2 %.1f  thread-instr/clk/SM (16 / 16 / 8 instr per iteration)\n", warps,
-               n * 16 / m0 / 1e3 / sms / 1.965e6, n * 16 / m1 / 1e3 / sms / 1.965e6, n * 8 / m2 / 1e3 / sms / 1.965e6);
+        printf("fma rate, %2d warps/SM: fp16 widen+FFMA %.1f  FFMA %.1f  FFMA pair helper %.1f  G products/s/SM (16 per thread and iteration)\n", warps,
+               n * 16 / m0 / 1e6 / sms, n * 16 / m1 / 1e6 / sms, n * 16 / m2 / 1e6 / sms);
     }
 
     {

@@ -1,6 +1,6 @@
 // trace_harness.cu - timeline of a chain of back-to-back GEMVs (C ABI, PDL, CUDA graph).  Links a -DSQLLM_TRACE build of
 // lutgemv_kernels.cu.  Prints, per launch, min/max over CTAs of each phase stamp relative to the chain start (ns).
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -DSQLLM_TRACE -I include -o trace_harness \
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -DSQLLM_TRACE -I include -o trace_harness \
 //        tests/perf/trace_harness.cu squeezellm_b200/csrc/lutgemv_kernels.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -21,12 +21,12 @@ int main(int argc, char **argv) {
     const int sparse = argc > 6 ? atoi(argv[6]) : 0;  // 1: CSR (0.45 %) + 10 zero dense rows, accumulate; 2: same, fused fp16
 
     const size_t qwords = (size_t)K / 32 * bits * N;
-    // enough distinct copies that the chain never finds a matrix in the 126 MB L2 (>= 400 MB in rotation)
+    // enough distinct copies that the chain never finds a matrix in L2 (>= 400 MB in rotation, 8x the 50 MB L2 of an H100)
     const int copies = (int)std::min<size_t>(40, std::max<size_t>(3, (400u << 20) / (qwords * 4) + 1));
     uint32_t *q; float *lut, *x, *y; unsigned long long *trace;
     CK(cudaMalloc(&q, qwords * 4 * copies)); CK(cudaMemset(q, 0x5a, qwords * 4 * copies));
     // every launch of the chain gets its own weights AND its own look-up table / outlier arrays: a decode step never finds a layer's small
-    // arrays in L2 either (one shared table made the chain ~3 us per launch faster than the real step: r02 notes in profiles/)
+    // arrays in L2 either (one shared table made the chain faster per launch than the real step)
     const size_t lutn = (size_t)N * 16;
     CK(cudaMalloc(&lut, lutn * 4 * copies)); CK(cudaMemset(lut, 0, lutn * 4 * copies));
     CK(cudaMalloc(&x, K * 4)); CK(cudaMemset(x, 0, K * 4));

@@ -5,7 +5,7 @@ import ctypes
 
 import pytest
 
-from util import Args, header_symbols, load_lib
+from util import GOLDEN, Args, header_symbols, load_lib
 
 REFERENCE_SYMBOLS = [
     "vecquant3matmul_nuq_perchannel", "vecquant4matmul_nuq_perchannel",
@@ -105,23 +105,20 @@ def test_exchange_descriptor_validation_without_gpu(change, frag):
 
 
 def test_reference_quant_py_imports_against_our_extension():
-    """Option A of INTEGRATION.md: the reference's own squeezellm/quant.py, unmodified, imports `quant_cuda` by name and finds every
-    symbol it calls in OUR extension (except the *_balanced_* ones, which the reference's extension does not define either).
-    Needs the reference checkout; skipped where it is absent (e.g. on the GPU box)."""
-    import importlib.util
+    """Option A of INTEGRATION.md: the reference's own squeezellm/quant.py imports `quant_cuda` by name and must find every
+    symbol it calls in OUR extension (except the *_balanced_* ones, which the reference's extension does not define either), and its
+    QuantLinearLUT must hold the same buffers as ours.  What the reference asks for is recorded in
+    tests/golden/reference_quant_py.json (tests/golden/make_golden_quant_py.py)."""
+    import json
     import os
-    import re
-    ref = "/root/reference/squeezellm/quant.py"
-    if not os.path.exists(ref):
-        pytest.skip("reference checkout not present")
+    import sys
     import squeezellm_b200.quant as ours            # puts the in-tree extension directory on sys.path, imports quant_cuda
-    spec = importlib.util.spec_from_file_location("reference_quant", ref)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)                     # runs `import quant_cuda` (quant.py:5)
-    assert mod.quant_cuda is ours.quant_cuda
-    called = set(re.findall(r"quant_cuda\.(\w+)", open(ref).read()))
-    missing = {n for n in called if not hasattr(mod.quant_cuda, n)}
+    assert sys.modules["quant_cuda"] is ours.quant_cuda   # what the reference's `import quant_cuda` (quant.py:5) resolves to
+    g = json.load(open(os.path.join(GOLDEN, "reference_quant_py.json")))
+    called = set(g["called_symbols"])
+    missing = {n for n in called if not hasattr(ours.quant_cuda, n)}
     assert len(called - missing) == 12
     assert missing and all("balanced" in n for n in missing), missing
-    m = mod.QuantLinearLUT(4, 128, 128, False, include_sparse=True, numvals=5, topX=10)   # the reference's module over our extension
-    assert set(m.state_dict()) == set(ours.QuantLinearLUT(4, 128, 128, False, include_sparse=True, numvals=5, topX=10).state_dict())
+    m = ours.QuantLinearLUT(4, 128, 128, False, include_sparse=True, numvals=5, topX=10)
+    got = {k: [list(v.shape), str(v.dtype).replace("torch.", "")] for k, v in m.state_dict().items()}
+    assert got == g["quantlinearlut_w4_128x128_sparse5_topx10"]

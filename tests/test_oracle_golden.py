@@ -1,6 +1,6 @@
 """CPU tests: the oracle (C restatement + numpy restatement) against fixtures produced by the
 REFERENCE's own code - tests/golden/pack2_*.npz (reference pack2 run on CPU, make_golden_pack2.py) and
-tests/golden/refkernel_*.npz (reference CUDA kernels run on a B200, make_golden_gpu.py)."""
+tests/golden/refkernel_*.npz (reference CUDA kernels run on an H100, make_golden_gpu.py)."""
 import numpy as np
 import pytest
 import torch
@@ -104,7 +104,7 @@ def test_cpu_baseline_fp16_dequant_within_north_star_tolerance():
 @pytest.mark.skipif(not REFK, reason="tests/golden/refkernel_*.npz not generated yet (needs one GPU run)")
 @pytest.mark.parametrize("path", REFK, ids=lambda p: p.split("refkernel_")[-1][:-4])
 def test_oracle_matches_reference_kernel_outputs(path):
-    """Pins the oracle's arithmetic: outputs of the reference's own CUDA kernels (oracle/_ref, run on a B200)
+    """Pins the oracle's arithmetic: outputs of the reference's own CUDA kernels (oracle/_ref, run on an H100)
     for the inputs stored next to them."""
     g = np.load(path, allow_pickle=False)
     L = {k: (g[k] if k in g.files else None) for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices")}

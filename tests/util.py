@@ -24,12 +24,22 @@ FLOOR = 1e-2
 TIGHT_TOL = 5e-5
 
 
-def rel_err(a, b):
+def rel_err(a, b, b_absmax=None):
+    """b_absmax: max|b| over the whole vector when a and b are a sample of it (the floor stays that of the whole vector)."""
     a = np.asarray(a, dtype=np.float64).ravel()
     b = np.asarray(b, dtype=np.float64).ravel()
     assert a.shape == b.shape
-    den = np.maximum(np.abs(b), FLOOR * max(np.abs(b).max(), 1e-30))
+    den = np.maximum(np.abs(b), FLOOR * max(np.abs(b).max() if b_absmax is None else b_absmax, 1e-30))
     return float((np.abs(a - b) / den).max())
+
+
+def sample_idx(n, cap=2048):
+    """The output positions kept in golden data of large outputs: all of them up to `cap`, else `cap` positions spread over
+    the vector by a prime stride (7919 divides none of the sizes used)."""
+    if n <= cap:
+        return np.arange(n)
+    assert n % 7919
+    return (np.arange(cap, dtype=np.int64) * 7919 + 13) % n
 
 
 def golden_files(prefix):
