@@ -6,19 +6,21 @@
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.
 //
-// Design (DESIGN.md has the full story and the measurements):
+// Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every layer of 64 or more output columns in the
+// accumulate and the default (fast) fused mode.  lutgemv_kernel below ("v1") runs the deterministic fused mode
+// (sqllm_set_deterministic / SQLLM_DETERMINISTIC=1) and layers narrower than one strip (out_features < 64) in every mode.
+// v1 (DESIGN.md has the full story and the measurements):
 //   * ONE launch per GEMV.  The [units x strips] iteration space (unit = one packed row for 4-bit,
 //     one 3-row / 32-input group for 3-bit; strip = 64 output columns) is flattened strip-major and
 //     cut into equal contiguous chunks, one per CTA (stream-K): every SM gets the same number of
 //     bytes whatever the shape.  A CTA touches at most MAXSEG strips.
-//   * Warp roles (default build, SQLLM_LDG=2): 8 consumer warps + 1 sparse warp, 72 registers, 3 CTAs per SM.
+//   * Warp roles: 8 consumer warps + 1 sparse warp, 72 registers, 3 CTAs per SM.
 //       - consumers: each lane streams its own 16 bytes per unit row with cp.async into a private ring in shared memory,
 //         PF positions ahead (the first PF before the programmatic dependency on the previous kernel resolves - PDL - so
 //         the weight traffic of GEMV n+1 overlaps the tail of GEMV n), pulls the word-quad into registers and turns every
 //         4-bit index into an LDS address with a single PRMT (the per-strip LUT is staged transposed
 //         [value][column-slot] in a 4 KB aligned table so that every lane owns one shared-memory bank: conflict-free
 //         gathers); products go into pairs of fp32 accumulators (two fma.rn.f32 per pair).  No tensor cores: this is a gather-bound GEMV.
-//         (SQLLM_LDG=1: register ring fed by LDG.128; SQLLM_LDG=0: TMA producer warp + mbarrier ring - measured, not faster.)
 //       - sparse warp: CSR rows spread evenly over all CTAs, staged with 16-byte cp.async, x gathered in batches,
 //         per-row sums in storage order; plus a k-slice of the topX dense rows.
 //   * Only the slice of x a CTA needs is staged (fp32, converted from fp16 on the way in).
@@ -44,37 +46,22 @@
 
 namespace {
 
-#ifndef SQLLM_NW
-#define SQLLM_NW 8
-#endif
-#ifndef SQLLM_LDG
-#define SQLLM_LDG 2   // 2: per-thread private cp.async ring in shared memory (default); 1: LDG.128 register ring; 0: TMA producer warp + mbarrier ring
-#endif
-#ifndef SQLLM_MINB4
-#define SQLLM_MINB4 3   // resident CTAs per SM the register budget must allow (shared memory admits 3; at 4 the 56-register
-                        // cap makes the compiler rematerialise table addresses inside the loop: measured slower)
-#endif
-#ifndef SQLLM_MINB3
-#define SQLLM_MINB3 3
-#endif
-#ifndef SQLLM_PF4
-#define SQLLM_PF4 8   // 128-bit loads in flight per lane, 4-bit path (LDG / cp.async modes)
-#endif
-#ifndef SQLLM_PF3
-#define SQLLM_PF3 3   // 3-row groups in flight per lane, 3-bit path (LDG / cp.async modes)
-#endif
-constexpr bool LDG_MODE = SQLLM_LDG != 0;   // no producer warp
-constexpr bool CPA_MODE = SQLLM_LDG == 2;   // weights staged by each consumer thread into its own cp.async ring
-constexpr int NW = SQLLM_NW;              // consumer warps per CTA (multiple of 8)
-constexpr int WARP_PRODUCER = LDG_MODE ? -1 : NW;            // warp index of the TMA producer (TMA mode only)
-constexpr int WARP_SPARSE = LDG_MODE ? NW : NW + 1;          // warp index of the CSR / dense-row warp
-constexpr int THREADS = (NW + (LDG_MODE ? 1 : 2)) * 32;
+constexpr int NW = 8;                     // consumer warps per CTA
+constexpr int WARP_SPARSE = NW;           // warp index of the CSR / dense-row warp
+constexpr int THREADS = (NW + 1) * 32;
+constexpr int CTAS_PER_SM = 3;            // resident CTAs per SM the register budget must allow and the plan asks for (shared memory
+                                          // admits 3; at 4 the 56-register cap makes the compiler rematerialise table addresses inside
+                                          // the loop: measured slower)
+constexpr int PF4 = 8;                    // 128-bit loads in flight per lane, 4-bit path
+constexpr int PF3 = 3;                    // 3-row groups in flight per lane, 3-bit path
 constexpr int MAXSEG = 4;                 // strips a CTA may touch
 constexpr int STRIP = 64;                 // output columns per strip (16 lanes x 4 columns)
 constexpr int SU = 2 * NW;                // units per pipeline stage (one pair per consumer warp)
 constexpr int CSR_CH = 1024;              // CSR elements staged per chunk
 constexpr int SROWS_LD = 68;              // padded row-pointer slice per segment (65 used)
 constexpr int MAX_TOPX_FUSED = 128;
+constexpr int NFIN_COLS = 1024;           // fast fused mode: about this many columns per finishing CTA ...
+constexpr int NFIN_MAX = 16;              // ... and at most this many finishers
 constexpr int HYB_R = 11;                 // dense rows: k-rows per lane slot requested before the dependency wait
 constexpr int MAX_STRIPS = 16320;         // per-strip tickets in the workspace header (out_features <= 1,044,480)
 constexpr int MAX_N_FUSED = 262144;        // fused path: the scratch accumulator lives at a fixed place in the workspace
@@ -84,7 +71,6 @@ constexpr size_t WS_HBOX_OFF = WS_ACC_OFF + (size_t)MAX_N_FUSED * 4;       // v2
 constexpr size_t WS_CBOX_OFF = WS_HBOX_OFF + (size_t)MAX_GRID_V2 * 64 * 8;  // ... and [MAX_N_FUSED] x 8 bytes (outlier row sums); zero between launches
 constexpr size_t WS_DBOX_OFF = WS_CBOX_OFF + (size_t)MAX_N_FUSED * 8;          // ... and [MAX_TOPX_FUSED][MAX_GRID_V2] x 8 bytes (dense-row parts, one per contributing CTA)
 constexpr size_t WS_HEADER = WS_DBOX_OFF + (size_t)MAX_TOPX_FUSED * MAX_GRID_V2 * 8;  // tickets + accumulator + mailboxes: never shared with data of any shape
-constexpr int MAX_NSTAGE = 16;            // weight stages per CTA (runtime count, fills the shared-memory budget)
 
 struct Params {
     const uint32_t *qw;
@@ -103,8 +89,6 @@ struct Params {
     int T;        // strips * R
     int chunk;    // units per CTA (even)
     int maxseg;   // strips a CTA of this launch can touch (sizes the LUT tables)
-    int nstage;   // weight stages in the TMA ring
-    int tma2d;    // 1: stages are fetched with 2-D tensor-map TMA boxes, 0: row-by-row bulk copies (odd shapes)
     int x_direct; // 1: x staged at its natural index (CTA covers whole strips), 0: compact, indexed by unit offset
     int xfloats;  // floats in the x staging buffer
     int hc;       // CTAs that take a slice of the dense rows
@@ -127,7 +111,6 @@ struct Params {
     unsigned long long xw_out_off, xw_flag_off, xw_state_off, xw_err_off;
     int nfin;        // fast fused mode: CTAs (the last ones of the grid) that share the final conversion
     int det;         // fused mode: 1 = deterministic per-strip tickets, 0 = red.add into ws_acc + one global ticket per CTA
-    int dbg;                    // debug: 1 = skip the gather/FMA math, 2 = no work at all, 4 = skip LUT staging (SQLLM_DEBUG_FLAGS)
     unsigned long long *trace;  // debug timeline (only written when built with -DSQLLM_TRACE and non-null)
 };
 
@@ -138,29 +121,21 @@ struct Cfg {
     static constexpr int TAB = L * STRIP * 4;              // 4096 (w4) / 2048 (w3) bytes per strip table
     static constexpr int ROWS_PER_UNIT = BITS == 4 ? 1 : 3;
     static constexpr int XU = BITS == 4 ? 8 : 32;          // inputs per unit
-    static constexpr int UNIT_BYTES = ROWS_PER_UNIT * STRIP * 4;
-    static constexpr int STAGE_BYTES = SU * UNIT_BYTES;    // 4 KB (w4) / 12 KB (w3)
-    // 2-D TMA box: BU units tall (w4: a whole stage of 16 rows; w3: 4 groups = 12 rows), 64 columns wide.
-    // in_features % 128 == 0 (the reference's own precondition) makes every box lie inside one strip.
-    static constexpr int BU = BITS == 4 ? SU : 4;
-    static constexpr int BOX_ROWS = BU * ROWS_PER_UNIT;
-    static constexpr int BOX_BYTES = BOX_ROWS * STRIP * 4;
-    // cp.async mode: every consumer thread owns PF slots of POS_BYTES (its 4 columns of one unit), laid out [slot][row-in-unit][thread]
-    static constexpr int PF = BITS == 4 ? SQLLM_PF4 : SQLLM_PF3;
+    // every consumer thread owns PF slots of POS_BYTES (its 4 columns of one unit) in the weight ring, laid out [slot][row-in-unit][thread]
+    static constexpr int PF = BITS == 4 ? PF4 : PF3;
     static constexpr int POS_BYTES = ROWS_PER_UNIT * 16;
     static constexpr int RING_BYTES = PF * NW * 32 * POS_BYTES;
-    // layout: [tables maxseg*TAB][part maxseg][misc][x][csr stage][weight stages ...]
+    // layout: [tables maxseg*TAB][part maxseg][misc][x][csr stage][weight ring]
     __host__ __device__ static int off_part(int maxseg) { return maxseg * TAB; }
     __host__ __device__ static int off_misc(int maxseg) { return off_part(maxseg) + maxseg * NW * STRIP * 4; }
-    // misc: 2 x MAX_NSTAGE mbarriers (256 B) + 16 ints (64 B) + dense-row totals float[maxseg + 1][MAX_TOPX_FUSED]
+    // misc: 256 B unused (kept so that the carve-up - and with it occupancy, plan and workspace size - stays as it was measured)
+    // + 16 ints (64 B) + dense-row totals float[maxseg + 1][MAX_TOPX_FUSED]
     __host__ __device__ static int off_x(int maxseg) { return off_misc(maxseg) + 256 + 64 + (maxseg + 1) * MAX_TOPX_FUSED * 4; }
     __host__ __device__ static int off_cstage(int maxseg, int xfloats) { return off_x(maxseg) + ((xfloats * 4 + 15) & ~15); }
     __host__ __device__ static int off_stage(int maxseg, int xfloats, int csr) {  // csr: bytes of staging (CSR 8 KB [+ dense-row partials 8 KB])
         return (off_cstage(maxseg, xfloats) + csr + 127) & ~127;
     }
-    __host__ __device__ static int total(int maxseg, int xfloats, int csr, int nstage) {
-        return 4096 + off_stage(maxseg, xfloats, csr) + (CPA_MODE ? RING_BYTES : nstage * STAGE_BYTES);
-    }
+    __host__ __device__ static int total(int maxseg, int xfloats, int csr) { return 4096 + off_stage(maxseg, xfloats, csr) + RING_BYTES; }
 };
 
 // ---- small PTX helpers -------------------------------------------------------------------------
@@ -232,11 +207,6 @@ __device__ __forceinline__ int ticket_take(int *counter) {
     asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(counter) : "memory");
     return old;
 }
-#if defined(SQLLM_TRACE) || defined(SQLLM_DEBUG)
-#define DBG(p) ((p).dbg)
-#else
-#define DBG(p) 0
-#endif
 #ifdef SQLLM_TRACE
 __device__ __forceinline__ void trace_mark(unsigned long long *trace, int slot) {
     if (trace) {
@@ -263,23 +233,14 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     do {
-#ifdef SQLLM_SPIN_WAIT
-        asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-#else
         asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
                      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-#endif
     } while (!ok);
 }
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
     uint64_t pol;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     return pol;
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void tma_tile2d_g2s(uint32_t dst, const CUtensorMap *map, int col, int row, uint32_t bar, uint64_t pol) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;"
@@ -290,22 +251,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-
-// Maps a unit offset `o` (from the CTA's first unit) to (segment, unit-in-strip); advanced incrementally.
-struct UnitIt {
-    int o, rr, seg;
-    __device__ __forceinline__ void init(int first, int r0, int R) {
-        o = first;
-        rr = r0 + first;
-        seg = 0;
-        while (rr >= R) { rr -= R; ++seg; }
-    }
-    __device__ __forceinline__ void advance(int step, int R) {
-        o += step;
-        rr += step;
-        while (rr >= R) { rr -= R; ++seg; }
-    }
-};
 
 // Walks, in order, the positions (unit pairs) one consumer warp owns: offset 2*warp + SU*p from the CTA's first unit.  Within a
 // segment (= strip) consecutive positions are SU units apart, so callers keep running pointers and only `seek` at segment ends.
@@ -412,20 +357,6 @@ __device__ __forceinline__ void consume(const Words<3> &g, const int jsel, const
     const uint32_t c[4] = {jsel ? g.c.y : g.c.x, jsel ? g.c.x : g.c.y, jsel ? g.c.w : g.c.z, jsel ? g.c.z : g.c.w};
 #pragma unroll
     for (int t = 0; t < 4; ++t) consume3_col(a[t], b[t], c[t], lsv[t], xp, acc[t]);
-}
-__device__ __forceinline__ void gload_words(Words<4> &g, const uint32_t *q, size_t) { g.a = ldg_stream(q); }
-__device__ __forceinline__ void gload_words(Words<3> &g, const uint32_t *q, size_t N) {
-    g.a = ldg_stream(q);
-    g.b = ldg_stream(q + N);
-    g.c = ldg_stream(q + 2 * N);
-}
-__device__ __forceinline__ void zero_words(Words<4> &g) { g.a = make_uint4(0u, 0u, 0u, 0u); }
-__device__ __forceinline__ void zero_words(Words<3> &g) { g.a = g.b = g.c = make_uint4(0u, 0u, 0u, 0u); }
-__device__ __forceinline__ void load_words(Words<4> &g, uint32_t unit_addr) { g.a = lds_u4(unit_addr); }
-__device__ __forceinline__ void load_words(Words<3> &g, uint32_t unit_addr) {
-    g.a = lds_u4(unit_addr);
-    g.b = lds_u4(unit_addr + STRIP * 4);
-    g.c = lds_u4(unit_addr + 2 * STRIP * 4);
 }
 
 // ---- fused mode: who contributes to a strip, and the per-column final reduction ----------------------
@@ -580,12 +511,8 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
     if (r < rb) group_begin();
 
     TRACE(13, lane == 0);
-#ifdef SQLLM_WAIT_ALL
-    pdl_wait();
-#else
     if (lane == 0) pdl_wait();
     __syncwarp();
-#endif
     TRACE(14, lane == 0);
 
     // ---------------- phase B: needs x (and, in fused mode, the workspace) ----------------
@@ -716,7 +643,7 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
 // The kernel
 // =================================================================================================
 template <int BITS, bool FUSED>
-__global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3) lutgemv_kernel(const Params p, const __grid_constant__ CUtensorMap tmap) {
+__global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Params p) {
     using C = Cfg<BITS>;
     extern __shared__ unsigned char smem_raw[];
     // 4 KB aligned base, computed in the 32-bit shared window and pinned in a register (an opaque mov: otherwise the
@@ -727,13 +654,11 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
     unsigned char *sm = smem_raw + (sm_u32 - raw_u32);
     const int maxseg = p.maxseg;
     float *part = reinterpret_cast<float *>(sm + C::off_part(maxseg));
-    const uint32_t bar_u32 = sm_u32 + C::off_misc(maxseg);          // full[s] at +8s, empty[s] at +128+8s
     int *misc = reinterpret_cast<int *>(sm + C::off_misc(maxseg) + 256);
     float *hyb_tot = reinterpret_cast<float *>(sm + C::off_misc(maxseg) + 320);
     float *xs = reinterpret_cast<float *>(sm + C::off_x(maxseg));
     const uint32_t xs_u32 = sm_u32 + C::off_x(maxseg);
     const uint32_t stage_u32 = sm_u32 + C::off_stage(maxseg, p.xfloats, p.has_stage);
-    const int nstage = p.nstage;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int i16 = lane & 15, jsel = lane >> 4;  // column group (4 columns) and unit-of-the-pair of this lane
@@ -741,41 +666,22 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
 
     // ---- this CTA's chunk of the flattened [strip][unit] space ----
     const int g0 = min((int)blockIdx.x * p.chunk, p.T);
-    const int g1 = (DBG(p) & 2) ? g0 : min(g0 + p.chunk, p.T);
+    const int g1 = min(g0 + p.chunk, p.T);
     const int len = g1 - g0;
     const int s0 = g0 / R;
     const int r0 = g0 - s0 * R;
     const int nseg = len > 0 ? (g1 - 1) / R - s0 + 1 : 0;
-    const int nst = (len + SU - 1) / SU;  // pipeline stages this CTA will consume
 
     TRACE(0, tid == 0);
 #ifdef SQLLM_TRACE
     if (p.trace && tid == 0) { unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid)); p.trace[(size_t)blockIdx.x * 32 + 12] = smid + 1; }
 #endif
-    if (!LDG_MODE && tid == 0) {
-        for (int s = 0; s < nstage; ++s) {
-            mbar_init(bar_u32 + 8 * s, 1);          // full: the producer's arrive.expect_tx
-            mbar_init(bar_u32 + 128 + 8 * s, NW);   // empty: one arrive per consumer warp
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     pdl_launch_dependents();  // the next kernel in the stream may start its own (independent) prologue now
     __syncthreads();
     TRACE(1, tid == 0);
 
-    // ---- LDG mode: the first PF packed-word loads of every lane go out before anything else.  They do not depend on the
-    //      previous kernel, so under PDL the register file of the next GEMV fills while this SM is still busy. ----
-    constexpr int PF = LDG_MODE ? C::PF : 1;
-    Words<BITS> ring[(LDG_MODE && !CPA_MODE) ? PF : 1];
-    UnitIt ld;
-    ld.init(2 * warp, r0, R);
-    auto gload = [&](Words<BITS> &w) {  // fetch the pair `ld` points at (this lane's unit and 4 columns), then advance
-        const int col0 = (s0 + ld.seg) * STRIP + 4 * (lane & 15);
-        if (ld.o < len && col0 < N) gload_words(w, p.qw + (size_t)((ld.rr + (lane >> 4)) * C::ROWS_PER_UNIT) * N + col0, (size_t)N);
-        else zero_words(w);
-        ld.advance(SU, R);
-    };
-    // cp.async mode: slot u of this thread lives at ring_u32 + ((u * ROWS_PER_UNIT + row) * NW*32 + tid) * 16 (consecutive threads are
+    constexpr int PF = C::PF;
+    // ---- weight ring: slot u of this thread lives at ring_u32 + ((u * ROWS_PER_UNIT + row) * NW*32 + tid) * 16 (consecutive threads are
     // contiguous: coalesced fills, conflict-free 128-bit reads).  Exactly one group is committed per position, valid or not,
     // so "at most PF-1 groups pending" always means "the oldest position has landed".  A running global pointer follows the
     // load cursor; it is re-derived only when the cursor enters a new segment.
@@ -813,89 +719,16 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
             w.c = lds_u4(src + 2 * NW * 32 * 16);
         }
     };
-    if (warp == WARP_PRODUCER) {
-        // =========================== TMA producer ===========================
-        // Weights never depend on the previous kernel, so this runs ahead of pdl_wait().
-        const uint64_t pol = l2_evict_first_policy();
-        if (p.tma2d) {
-            // One tensor-map box per BU units: hardware address generation.  The loop is a single latency-bound warp, so it
-            // carries no divisions or re-derivations: ring slot, phase and box coordinates are all advanced incrementally.
-            constexpr int BOXES = SU / C::BU;  // 1 (w4) / 4 (w3): lane b owns box b of every stage
-            if (lane < BOXES) {
-                constexpr uint32_t MASK = (1u << BOXES) - 1u;
-                UnitIt it;
-                it.init(lane * C::BU, r0, R);
-                uint32_t full = bar_u32, empty = bar_u32 + 128, dst = stage_u32 + lane * C::BOX_BYTES;
-                int s = 0;
-                uint32_t ph = 0;
-                bool refill = false;
-                for (int n = 0; n < nst; ++n) {
-                    if (refill) mbar_wait(empty, ph);
-                    if (lane == 0) mbar_expect_tx(full, (uint32_t)min(BOXES, (len - it.o + C::BU - 1) / C::BU) * C::BOX_BYTES);
-                    if (BOXES > 1) __syncwarp(MASK);
-                    if (it.o < len) tma_tile2d_g2s(dst, &tmap, (s0 + it.seg) * STRIP, it.rr * C::ROWS_PER_UNIT, full, pol);
-                    TRACE(8, lane == 0 && n == 0);
-                    it.advance(SU, R);
-                    full += 8; empty += 8; dst += C::STAGE_BYTES;
-                    if (++s == nstage) {
-                        s = 0;
-                        full = bar_u32; empty = bar_u32 + 128; dst = stage_u32 + lane * C::BOX_BYTES;
-                        if (refill) ph ^= 1u;
-                        refill = true;
-                    }
-                }
-            }
-        } else {
-            constexpr int COPIES = SU * C::ROWS_PER_UNIT;  // 16 (w4) / 48 (w3) row copies per stage
-            for (int n = 0; n < nst; ++n) {
-                const int use = n / nstage, s = n - use * nstage;
-                const uint32_t full = bar_u32 + 8 * s, empty = bar_u32 + 128 + 8 * s;
-                if (use > 0) mbar_wait(empty, (use - 1) & 1);
-                // each lane describes up to 2 copies: copy id -> (unit, row-in-unit)
-                uint32_t bytes[2] = {0u, 0u}, dst[2] = {0u, 0u};
-                const uint32_t *src[2] = {nullptr, nullptr};
-                uint32_t tot = 0;
-    #pragma unroll
-                for (int h = 0; h < (COPIES + 31) / 32; ++h) {
-                    const int cid = lane + 32 * h;
-                    if (cid < COPIES) {
-                        const int u = cid / C::ROWS_PER_UNIT, rowin = cid - u * C::ROWS_PER_UNIT;
-                        const int o = n * SU + u;
-                        if (o < len) {
-                            UnitIt it;
-                            it.init(o, r0, R);
-                            const int c0 = (s0 + it.seg) * STRIP;
-                            bytes[h] = (uint32_t)min(STRIP, N - c0) * 4u;
-                            src[h] = p.qw + (size_t)(it.rr * C::ROWS_PER_UNIT + rowin) * N + c0;
-                            dst[h] = stage_u32 + s * C::STAGE_BYTES + cid * (STRIP * 4);
-                        }
-                    }
-                    tot += bytes[h];
-                }
-                tot = __reduce_add_sync(0xffffffffu, tot);
-                if (lane == 0) mbar_expect_tx(full, tot);
-                __syncwarp();
-    #pragma unroll
-                for (int h = 0; h < (COPIES + 31) / 32; ++h)
-                    if (bytes[h]) tma_bulk_g2s(dst[h], src[h], bytes[h], full, pol);
-                TRACE(8, lane == 0 && n == 0);
-            }
-        }
-        TRACE(9, lane == 0);
-    } else if (warp == WARP_SPARSE) {
+    if (warp == WARP_SPARSE) {
         sparse_warp<BITS, FUSED>(p, sm, sm_u32, lane, hyb_tot + maxseg * MAX_TOPX_FUSED, nseg, s0);
         TRACE(10, lane == 0);
     } else {
-        // ---- LDG mode: the first PF packed-word loads of every lane go out before anything else ----
-        if (CPA_MODE) {
-            cl.seek(0, warp2, r0, R, len, nseg);
-            cl_setup();
+        // ---- the first PF weight fetches of every lane go out before anything else.  They do not depend on the previous
+        //      kernel, so under PDL the ring of the next GEMV fills while this SM is still busy. ----
+        cl.seek(0, warp2, r0, R, len, nseg);
+        cl_setup();
 #pragma unroll
-            for (int u = 0; u < PF; ++u) cpa_issue(ring_u32 + u * SLOT_STRIDE);
-        } else if (LDG_MODE) {
-#pragma unroll
-            for (int u = 0; u < PF; ++u) gload(ring[u]);
-        }
+        for (int u = 0; u < PF; ++u) cpa_issue(ring_u32 + u * SLOT_STRIDE);
         // ---- consumers: stage the LUTs of this CTA's strips, transposed to [value][slot].  One 128-bit load per (column, value
         //      quad); a warp takes 32 columns whose slots fall in 32 different banks, so the four scalar stores are conflict-free.
         //      (4-byte cp.async would cost 16 shared-memory wavefronts per warp instruction - measured.) ----
@@ -907,8 +740,8 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
             const int it = tid + n * (NW * 32), seg = it / IPS, vw = (it % IPS) >> 5;
             const int c = ((lane >> 1) << 2) | ((vw & 1) << 1) | (lane & 1), q = vw >> 1;
             const int col = (s0 + seg) * STRIP + c;
-            lq[n] = (seg < nseg && col < N && !(DBG(p) & 4)) ? __ldg(reinterpret_cast<const float4 *>(p.lut + (size_t)col * C::L) + q)
-                                                            : make_float4(0.f, 0.f, 0.f, 0.f);
+            lq[n] = (seg < nseg && col < N) ? __ldg(reinterpret_cast<const float4 *>(p.lut + (size_t)col * C::L) + q)
+                                            : make_float4(0.f, 0.f, 0.f, 0.f);
         }
         for (int e = tid; e < maxseg * NW * STRIP; e += NW * 32) part[e] = 0.f;
 #pragma unroll
@@ -925,12 +758,8 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
         TRACE(2, tid == 0);
         // Everything below reads data the previous kernel may have produced (x, mul, workspace).  One thread waits on the
         // programmatic dependency; the other consumers sleep on a hardware barrier instead of each polling it.
-#ifdef SQLLM_WAIT_ALL
-        pdl_wait();
-#else
         if (tid == 0) pdl_wait();
         named_bar_sync(6, NW * 32);
-#endif
         TRACE(3, tid == 0);
 
         // ---- stage the slice(s) of x this CTA needs, as fp32 ----
@@ -966,7 +795,6 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
         uint64_t acc[4] = {0ull, 0ull, 0ull, 0ull};
         uint32_t lsb = 0u, segc = 0u;
         uint32_t lsv[4] = {0u, 0u, 0u, 0u};
-        int cur_seg = -1;
         const uint32_t part_u32 = sm_u32 + C::off_part(maxseg) + (warp * STRIP + 4 * i16) * 4;
         const uint32_t lane_slot = (uint32_t)((jsel << 6) | (i16 << 2));  // column 0 of this lane: slot ((0^jsel)<<4 | i16), x4 bytes
 
@@ -1003,88 +831,29 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
 
         const uint32_t xlane = xs_u32 + (C::XU * 4) * jsel;
         const bool xdir = p.x_direct != 0;
-        UnitIt it;
-        it.init(2 * warp, r0, R);
-        if constexpr (CPA_MODE) {
-            // private cp.async ring.  Outer loop: the segments (strips) this warp has positions in; inner loop: a fixed trip
-            // count of positions with nothing but running pointers: wait for the slot, pull it into registers, do the math,
-            // refill the slot PF positions ahead.
-            Cursor cc;
-            cc.seek(0, warp2, r0, R, len, nseg);
-            uint32_t slot = ring_u32;
-            const uint32_t slot_end = ring_u32 + PF * SLOT_STRIDE;
-            while (cc.seg < nseg) {
-                set_seg(cc.seg);
-                uint32_t xptr = xlane + (C::XU * 4) * (xdir ? cc.rr : cc.rr + cc.seg * R - r0);
-                for (int i = cc.left; i > 0; --i) {
-                    cp_async_wait_pending<PF - 1>();
-                    Words<BITS> cur;
-                    cpa_fetch(cur, slot);
-                    if (!(DBG(p) & 1)) consume(cur, jsel, lsb, segc, lsv, xptr, acc);
-                    else acc[0] ^= cur.a.x;
-                    cpa_issue(slot);  // the words are in registers (consumed above): the slot can be overwritten
-                    slot += SLOT_STRIDE;
-                    if (slot == slot_end) slot = ring_u32;
-                    xptr += SU * C::XU * 4;
-                }
-                deposit(cc.seg);
-                cc.seek(cc.seg + 1, warp2, r0, R, len, nseg);
+        // Outer loop: the segments (strips) this warp has positions in; inner loop: a fixed trip
+        // count of positions with nothing but running pointers: wait for the slot, pull it into registers, do the math,
+        // refill the slot PF positions ahead.
+        Cursor cc;
+        cc.seek(0, warp2, r0, R, len, nseg);
+        uint32_t slot = ring_u32;
+        const uint32_t slot_end = ring_u32 + PF * SLOT_STRIDE;
+        while (cc.seg < nseg) {
+            set_seg(cc.seg);
+            uint32_t xptr = xlane + (C::XU * 4) * (xdir ? cc.rr : cc.rr + cc.seg * R - r0);
+            for (int i = cc.left; i > 0; --i) {
+                cp_async_wait_pending<PF - 1>();
+                Words<BITS> cur;
+                cpa_fetch(cur, slot);
+                consume(cur, jsel, lsb, segc, lsv, xptr, acc);
+                cpa_issue(slot);  // the words are in registers (consumed above): the slot can be overwritten
+                slot += SLOT_STRIDE;
+                if (slot == slot_end) slot = ring_u32;
+                xptr += SU * C::XU * 4;
             }
-            cur_seg = -1;  // everything already deposited
-        } else if constexpr (LDG_MODE) {
-            // register ring: consume slot u, immediately refill it with the pair PF positions ahead
-            while (it.o < len) {
-#pragma unroll
-                for (int u = 0; u < PF; ++u) {
-                    if (it.o < len) {  // warp-uniform: len and o are even, a pair never straddles the end
-                        if (it.seg != cur_seg) {
-                            if (cur_seg >= 0) deposit(cur_seg);
-                            cur_seg = it.seg;
-                            set_seg(cur_seg);
-                        }
-                        if (!(DBG(p) & 1)) consume(ring[u], jsel, lsb, segc, lsv, xlane + (C::XU * 4) * (xdir ? it.rr : it.o), acc);
-                        else acc[0] ^= ring[u].a.x;
-                        gload(ring[u]);
-                        it.advance(SU, R);
-                    }
-                }
-            }
-        } else {
-            // this lane's unit inside a stage: 2*warp + jsel ; its 16 bytes at column group i16
-            const uint32_t lane_off = stage_u32 + (2 * warp + jsel) * C::UNIT_BYTES + i16 * 16;
-            Words<BITS> cur = {}, nxt = {};
-            int s = 0;               // ring slot of the stage being fetched
-            uint32_t par = 0;        // its phase parity
-            auto fetch = [&](Words<BITS> &dst) {  // wait for ring slot s, pull this lane's words, release the slot, advance
-                mbar_wait(bar_u32 + 8 * s, par);
-                load_words(dst, lane_off + s * C::STAGE_BYTES);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * s);
-                if (++s == nstage) { s = 0; par ^= 1u; }
-            };
-            if (nst > 0) {
-                fetch(cur);
-                TRACE(5, tid == 0);
-            }
-            for (int n = 0; n < nst; ++n) {
-                if (n + 1 < nst) {  // pull the next stage into registers before computing on this one
-                    fetch(nxt);
-                    TRACE(16 + (n + 1 < 15 ? n + 1 : 15), tid == 0);
-                }
-                if (it.o < len) {  // warp-uniform: len and o are even, a pair never straddles the end
-                    if (it.seg != cur_seg) {
-                        if (cur_seg >= 0) deposit(cur_seg);
-                        cur_seg = it.seg;
-                        set_seg(cur_seg);
-                    }
-                    if (!(DBG(p) & 1)) consume(cur, jsel, lsb, segc, lsv, xlane + (C::XU * 4) * (xdir ? it.rr : it.o), acc);
-                    else acc[0] ^= cur.a.x;
-                }
-                it.advance(SU, R);
-                cur = nxt;
-            }
+            deposit(cc.seg);
+            cc.seek(cc.seg + 1, warp2, r0, R, len, nseg);
         }
-        if (cur_seg >= 0) deposit(cur_seg);
         TRACE(6, tid == 0);
     }
 
@@ -1172,7 +941,7 @@ __global__ void __launch_bounds__(THREADS, BITS == 4 ? SQLLM_MINB4 : SQLLM_MINB3
                 } while (seen < G);
             }
         }
-        TRACE(8, tid == 0);  // (slots 8 / 9 double as "announced / all arrived" and "finalizer done" outside the TMA mode)
+        TRACE(8, tid == 0);  // announced (finishers: all arrived)
         if (fidx < 0) return;
         __syncthreads();
         {
@@ -1318,7 +1087,6 @@ struct DevInfo {
 // being captured.
 std::recursive_mutex g_state_mu;
 DevInfo g_dev[64];
-int g_use_pdl = -1;
 int g_det = -1;
 int det_mode() {
     std::lock_guard<std::recursive_mutex> lk(g_state_mu);
@@ -1375,7 +1143,7 @@ int get_tensor_map(const void *qweight, int rows, int cols, int box_rows, CUtens
 }
 
 struct Plan {
-    int R, strips, T, chunk, G, maxc, hc, hrows, smem, maxseg, nstage, x_direct, xfloats, tma2d, box_rows;
+    int R, strips, T, chunk, G, maxc, hc, hrows, smem, maxseg, x_direct, xfloats;
     size_t ws_cnt_off, ws_hybcnt_off, ws_hyb_off, ws_part_off, ws_csr_off, ws_acc_off, ws_bytes;
     int csr_rpc, has_stage;
 };
@@ -1410,30 +1178,13 @@ int make_plan(int bits, int K, int N, int topX, bool has_csr_in, bool fused, Pla
     pl.T = (int)T;
     if (pl.strips > MAX_STRIPS || (fused && N > MAX_N_FUSED)) return fail(SQLLM_EINVAL, "out_features=%d exceeds the workspace header (max %d)", N, MAX_N_FUSED);
 
-    // Each kernel takes only CPS CTA slots per SM (default 2 of the 4 that fit): the rest of the SM is left to the NEXT
-    // GEMV in the stream, which - launched with programmatic dependent launch - streams its weights into shared memory
-    // while this one is still computing.  All of a CTA's shared memory beyond the fixed part holds weight stages.
-    static int cps = 0, budget = 0;
-    if (!cps) {
-        const char *e1 = getenv("SQLLM_CTAS_PER_SM"), *e2 = getenv("SQLLM_SMEM_BUDGET_KB");
-        cps = e1 ? atoi(e1) : (LDG_MODE ? 3 : 2);
-        if (cps < 1 || cps > 8) cps = LDG_MODE ? 3 : 2;
-        budget = (e2 ? atoi(e2) : 56) * 1024;
-        if (budget < 16 * 1024 || budget > 227 * 1024) budget = 56 * 1024;
-    }
-    // The grid must be co-resident: a plan whose shared memory lets fewer than `cps` CTAs onto an SM would run a second wave.
-    // Plan for cps CTAs/SM, ask the occupancy calculator, and fall back to fewer CTAs per SM if it disagrees.
-    int use_cps = cps;
+    // The grid must be co-resident (the fast fused mode's finishers wait for every CTA): a plan whose shared memory lets fewer
+    // than CTAS_PER_SM CTAs onto an SM would run a second wave.  Plan for CTAS_PER_SM, ask the occupancy calculator, and fall
+    // back to fewer CTAs per SM if it disagrees.
+    int use_cps = CTAS_PER_SM;
 replan:
     const int G0 = d.sm * use_cps;
-    // 2-D TMA boxes need every box inside one strip and one CTA range: units per box BU divides R and the chunk.
-    const int BU = bits == 4 ? Cfg<4>::BU : Cfg<3>::BU;
-    static int no_tma2d = -1;
-    if (no_tma2d < 0) { const char *e = getenv("SQLLM_NO_TMA2D"); no_tma2d = (e && e[0] == '1') ? 1 : 0; }
-    pl.tma2d = (!LDG_MODE && !no_tma2d && K % 128 == 0 && pl.R % BU == 0) ? 1 : 0;
-    pl.box_rows = bits == 4 ? Cfg<4>::BOX_ROWS : Cfg<3>::BOX_ROWS;
-    const int gran = pl.tma2d ? (BU % 2 ? 2 * BU : BU) : 2;
-    int chunk = (int)(gran * ((T + (long long)gran * G0 - 1) / ((long long)gran * G0)));
+    int chunk = (int)(2 * ((T + 2LL * G0 - 1) / (2LL * G0)));  // an even number of units: a consumer warp's pair never straddles the end
     if (chunk > 3 * pl.R) chunk = 3 * pl.R;  // a CTA may touch at most MAXSEG strips
     if (chunk < 2) chunk = 2;
     int maxseg = (chunk - 2) / pl.R + 2;      // worst case over start offsets (even offsets, even R)
@@ -1441,15 +1192,7 @@ replan:
     const bool direct = (long long)chunk * XU >= K;
     const int xfl = direct ? K : chunk * XU;
     pl.x_direct = direct ? 1 : 0;
-    const int stage_bytes = bits == 4 ? Cfg<4>::STAGE_BYTES : Cfg<3>::STAGE_BYTES;
-    const int fixed = bits == 4 ? Cfg<4>::total(maxseg, xfl, pl.has_stage, 0) : Cfg<3>::total(maxseg, xfl, pl.has_stage, 0);
-    const int need = (chunk + SU - 1) / SU;
-    int nstage = (budget - fixed) / stage_bytes;
-    if (nstage > need) nstage = need;
-    if (nstage > MAX_NSTAGE) nstage = MAX_NSTAGE;
-    if (nstage < 2) nstage = 2;
-    if (LDG_MODE) nstage = 0;  // weights go straight to registers
-    const int smem = fixed + nstage * stage_bytes;
+    const int smem = bits == 4 ? Cfg<4>::total(maxseg, xfl, pl.has_stage) : Cfg<3>::total(maxseg, xfl, pl.has_stage);
     if (smem > 227 * 1024) return fail(SQLLM_EINVAL, "in_features=%d needs %d B of shared memory (> 227 KB)", K, smem);
     {
         static std::mutex occ_mu;
@@ -1477,7 +1220,6 @@ replan:
     }
     pl.smem = smem;
     pl.maxseg = maxseg;
-    pl.nstage = nstage;
     pl.xfloats = xfl;
     pl.chunk = chunk;
     pl.G = (int)((T + chunk - 1) / chunk);
@@ -1531,12 +1273,8 @@ int check_common(const sqllm_lutgemv_args *a) {
 }
 
 template <int BITS, bool FUSED>
-cudaError_t launch_kernel(const Plan &pl, const Params &p, const CUtensorMap &tm, cudaStream_t st) {
+cudaError_t launch_kernel(const Plan &pl, const Params &p, cudaStream_t st) {
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
-    if (g_use_pdl < 0) {
-        const char *e = getenv("SQLLM_NO_PDL");
-        g_use_pdl = (e && e[0] == '1') ? 0 : 1;
-    }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     g_last_grid = pl.G;
@@ -1548,8 +1286,8 @@ cudaError_t launch_kernel(const Plan &pl, const Params &p, const CUtensorMap &tm
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, lutgemv_kernel<BITS, FUSED>, p, tm);
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, lutgemv_kernel<BITS, FUSED>, p);
 }
 
 template <bool FUSED>
@@ -1564,34 +1302,19 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
     p.topX = hyb ? a->topX : 0;
     p.K = a->in_features; p.N = a->out_features;
     p.R = pl.R; p.strips = pl.strips; p.T = pl.T; p.chunk = pl.chunk;
-    p.maxseg = pl.maxseg; p.nstage = pl.nstage; p.tma2d = pl.tma2d; p.x_direct = pl.x_direct; p.xfloats = pl.xfloats;
+    p.maxseg = pl.maxseg; p.x_direct = pl.x_direct; p.xfloats = pl.xfloats;
     p.hc = hyb ? pl.hc : 0; p.hrows = pl.hrows; p.maxc = pl.maxc;
     p.has_csr = a->rows ? 1 : 0;
     p.has_stage = pl.has_stage;
     p.csr_rpc = pl.csr_rpc;
-    {   // ~1024 columns per finishing CTA, at most 16 of them (SQLLM_NFIN_COLS / SQLLM_NFIN_MAX override, for experiments)
-        static int cols_per = 0, nmax = 0;
-        if (!cols_per) {
-            const char *e1 = getenv("SQLLM_NFIN_COLS"), *e2 = getenv("SQLLM_NFIN_MAX");
-            cols_per = e1 && atoi(e1) > 0 ? atoi(e1) : 1024;
-            nmax = e2 && atoi(e2) > 0 ? atoi(e2) : 16;
-        }
-        p.nfin = (a->out_features + cols_per - 1) / cols_per;
-        if (p.nfin > nmax) p.nfin = nmax;
-    }
+    p.nfin = (a->out_features + NFIN_COLS - 1) / NFIN_COLS;
+    if (p.nfin > NFIN_MAX) p.nfin = NFIN_MAX;
     if (p.nfin > pl.G) p.nfin = pl.G;
     if (p.nfin < 1) p.nfin = 1;
     p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
     p.trace = g_trace;
-    { static int dbg = -1; if (dbg < 0) { const char *e = getenv("SQLLM_DEBUG_FLAGS"); dbg = e ? atoi(e) : 0; } p.dbg = dbg; }
     if (g_trace) g_trace += g_trace_stride;
-    CUtensorMap tm;
-    memset(&tm, 0, sizeof(tm));
-    if (pl.tma2d) {
-        const int rc = get_tensor_map(a->qweight, a->in_features / 32 * a->bits, a->out_features, pl.box_rows, tm);
-        if (rc) return rc;
-    }
-    const cudaError_t e = a->bits == 4 ? launch_kernel<4, FUSED>(pl, p, tm, st) : launch_kernel<3, FUSED>(pl, p, tm, st);
+    const cudaError_t e = a->bits == 4 ? launch_kernel<4, FUSED>(pl, p, st) : launch_kernel<3, FUSED>(pl, p, st);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1602,7 +1325,6 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
 // =================================================================================================
 bool g_v2_attr[64] = {};
 int g_lut_mode = -1;     // 0: exact fp32 table, 1: fp16 pair table when x is fp16 (SQLLM_LUT_MODE=fp16 / sqllm_set_lut_mode)
-int g_kernel_sel = -1;   // 2: v2 (default), 1: v1 everywhere (SQLLM_KERNEL=v1; kept for A/B runs and as the deterministic mode's kernel)
 
 int lut_mode() {
     std::lock_guard<std::recursive_mutex> lk(g_state_mu);
@@ -1611,14 +1333,6 @@ int lut_mode() {
         g_lut_mode = (e && (!strcmp(e, "fp16") || !strcmp(e, "pair") || !strcmp(e, "1"))) ? 1 : 0;
     }
     return g_lut_mode;
-}
-int kernel_sel() {
-    std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-    if (g_kernel_sel < 0) {
-        const char *e = getenv("SQLLM_KERNEL");
-        g_kernel_sel = (e && !strcmp(e, "v1")) ? 1 : 2;
-    }
-    return g_kernel_sel;
 }
 
 typedef void (*K2)(const v2::P2, const CUtensorMap, const CUtensorMap);
@@ -1746,22 +1460,6 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
         p.trace = g_trace;
         if (g_trace) g_trace += g_trace_stride;
         g_last_grid = pl.G;
-        if (g_use_pdl < 0) {
-            const char *e = getenv("SQLLM_NO_PDL");
-            g_use_pdl = (e && e[0] == '1') ? 0 : 1;
-        }
-        static int l2pf = -1;
-        if (l2pf < 0) {
-            const char *e = getenv("SQLLM_L2PF");
-            l2pf = e ? (e[0] == '1') : 0;
-        }
-        p.l2pf = l2pf;
-        static int sp_w0 = -1;
-        if (sp_w0 < 0) {
-            const char *e = getenv("SQLLM_SP_W0");
-            sp_w0 = e ? (e[0] == '1') : 0;
-        }
-        p.sp_w0 = sp_w0;
     }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -1773,7 +1471,7 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     // two tensor maps over the packed matrix: 64 columns x (32 units | 2 units) boxes
     const int rows_per_unit = a->bits == 4 ? 1 : 3, qrows = a->in_features / 32 * a->bits;
     CUtensorMap tm_big, tm_small;
@@ -1811,7 +1509,7 @@ size_t seq_item_len(const sqllm_seq_item &it) {  // elements of the item's full-
 }  // namespace
 
 struct sqllm_sequence {
-    int dev = 0, n = 0, bits = 0, mode = 0, world = 1, rank = 0, grid = 0, smem = 0, coop = 1;
+    int dev = 0, n = 0, bits = 0, mode = 0, world = 1, rank = 0, grid = 0, smem = 0;
     seq::SeqCfg cfg;
     KSeq fn = nullptr;
     void *d_descs = nullptr, *d_exports = nullptr, *d_ws = nullptr, *d_arena = nullptr;
@@ -1898,17 +1596,12 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
     if (hi_room < 0) return fail(SQLLM_EINVAL, "sequence: in_features=%d does not fit the shared-memory carve-up of this table mode", kmax);
     const int lo_cap = (int)((tab0 - lo_base) / (unsigned)ki.stage), hi_cap = (int)(hi_room / ki.stage);
     int nst = std::min(v2::MAXD, lo_cap + hi_cap);
-    if (const char *e = getenv("SQLLM_SEQ_STAGES")) nst = std::max(2, std::min(nst, atoi(e)));  // experiments: a shallower weight ring
     if (nst < 2) return fail(SQLLM_EINVAL, "sequence: in_features=%d leaves no room for a weight ring in shared memory", kmax);
     const int n_lo = std::min(nst, lo_cap);
     const int smem = (int)((long long)tab0 + (long long)ki.ntb * ki.tab + (long long)(nst - n_lo) * ki.stage - raw);
 
     sqllm_sequence *s = new sqllm_sequence();
     s->dev = dev; s->n = n_items; s->bits = bits; s->mode = mode; s->world = world; s->rank = rank; s->grid = sm; s->smem = smem; s->fn = ki.fn;
-    {
-        const char *e = getenv("SQLLM_SEQ_COOP");
-        s->coop = (e && e[0] == '0') ? 0 : 1;
-    }
     // workspace: [0,4) token counter, [64,68) error word, per parity {flags [64 + MAX_STRIPS] ints, accumulator [MAX_N_FUSED] floats} (only
     // used by CTAs that own more than 8 strips), then EVERY item's own mailboxes: outlier row sums [N], partial strip sums [grid][64],
     // dense-row parts [topX][MAX_GRID_V2].  Mailboxes are not shared between items: an item may read only a slice of its predecessor's
@@ -2040,7 +1733,7 @@ extern "C" int sqllm_sequence_run(sqllm_sequence *s, void *stream) {
     attr[0].id = cudaLaunchAttributeCooperative;  // every CTA waits on every other one: they must all be resident
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = s->coop ? 1 : 0;
+    cfg.numAttrs = 1;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, s->fn, s->cfg);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "sequence launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
@@ -2176,38 +1869,23 @@ int sqllm_lutgemv(const sqllm_lutgemv_args *a, void *stream) {
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch must be >= 1");
     if (reinterpret_cast<uintptr_t>(a->vec) & 15) return fail(SQLLM_EINVAL, "vec must be 16-byte aligned");
     const bool hyb = a->full_rows && a->topX > 0;
-    if (a->batch >= 2) {
-        static int loop_mode = -1;  // SQLLM_BATCHED=loop: one batch-1 launch per row, as in round 1 (A/B runs)
-        {
-            std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-            if (loop_mode < 0) { const char *e = getenv("SQLLM_BATCHED"); loop_mode = (e && !strcmp(e, "loop")) ? 1 : 0; }
-        }
-        if (!loop_mode) return launch_batched(a, static_cast<cudaStream_t>(stream));
-    }
-    if (kernel_sel() == 2 && a->out_features >= STRIP) {
+    if (a->batch >= 2) return launch_batched(a, static_cast<cudaStream_t>(stream));
+    if (a->out_features >= STRIP) {
         v2::P2 q;
         memset(&q, 0, sizeof(q));
-        for (int b = 0; b < a->batch; ++b) {  // serial over batch rows, like the reference's in-kernel `for b` (:1011)
-            q.x = a->vec + (size_t)b * a->in_features;
-            q.out = a->mul + (size_t)b * a->out_features;
-            rc = launch2(a, 0, false, q, static_cast<cudaStream_t>(stream));
-            if (rc) return rc;
-        }
-        return SQLLM_OK;
+        q.x = a->vec;
+        q.out = a->mul;
+        return launch2(a, 0, false, q, static_cast<cudaStream_t>(stream));
     }
     Plan pl;
     rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, false, pl);
     if (rc) return rc;
     Params p;
     memset(&p, 0, sizeof(p));
-    for (int b = 0; b < a->batch; ++b) {  // serial over batch rows, like the reference's in-kernel `for b` (:1011)
-        p.x = a->vec + (size_t)b * a->in_features;
-        p.out = a->mul + (size_t)b * a->out_features;
-        p.x_is_half = 0;
-        rc = launch<false>(a, pl, p, static_cast<cudaStream_t>(stream));
-        if (rc) return rc;
-    }
-    return SQLLM_OK;
+    p.x = a->vec;
+    p.out = a->mul;
+    p.x_is_half = 0;
+    return launch<false>(a, pl, p, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half,
@@ -2220,7 +1898,7 @@ int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_hal
     const bool hyb = a->full_rows && a->topX > 0;
     if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
     unsigned char *ws = static_cast<unsigned char *>(workspace);
-    if (det_mode() == 0 && kernel_sel() == 2 && a->out_features >= STRIP) {
+    if (det_mode() == 0 && a->out_features >= STRIP) {
         if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
         v2::P2 q;
         memset(&q, 0, sizeof(q));
@@ -2269,7 +1947,7 @@ int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int
     const bool hyb = a->full_rows && a->topX > 0;
     if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
     unsigned char *ws = static_cast<unsigned char *>(workspace);
-    if (kernel_sel() == 2 && a->out_features >= STRIP) {
+    if (a->out_features >= STRIP) {
         if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
         v2::P2 q;
         memset(&q, 0, sizeof(q));

@@ -16,14 +16,6 @@
 //     next GEMV is the whole exchange - no collective, no flag round trip (v2's exchange waits on a system-scope flag per launch).
 #pragma once
 
-#ifndef SQLLM_SEQ_POLL_NS
-#define SQLLM_SEQ_POLL_NS 0   // pause between two reads of an x word that is not there yet
-#endif
-
-#ifndef SQLLM_SEQ_PREFETCH
-#define SQLLM_SEQ_PREFETCH 0  // 1: consumer loop fetches the next stage's words before the current stage's gathers (register rotation); measured: no gain (4-bit), spills (3-bit)
-#endif
-
 namespace seq {
 using namespace v2;
 
@@ -80,9 +72,6 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
             const int i = i0 + j * nthr;
             if (i < n4) {
                 while (!tags_ok(w[j], want)) {
-#if SQLLM_SEQ_POLL_NS > 0
-                    __nanosleep(SQLLM_SEQ_POLL_NS);
-#endif
                     w[j] = ld_relaxed_v4<SYS>(src + 4 * (size_t)i);
                     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
                     if (t0 == 0ull) t0 = t1;
@@ -656,31 +645,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;
                 mbar_wait(bar_u32 + 256 + 8 * b, (uint32_t)((q / NTB) & 1));
                 TRACE(16 + (seg < 7 ? seg : 7), tid == 0);
-#if SQLLM_SEQ_PREFETCH
-                // The words (and x slice) of stage k+1 are requested BEFORE the gathers of stage k are issued: one of the two serialized
-                // shared-memory round trips per position (word fetch, then gathers - each queues behind the other warps' gathers in the LSU)
-                // disappears from a warp's critical path.  One copy of the math, the look-ahead lives in a second register set that is
-                // moved over at the end of the trip (8 / 12 MOVs per ~140 instructions); the loop is kept rolled (i-cache: see v2).
-                {
-                    Fetch<BITS, XH> F, Fn;
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (0 < mine) fetch2<BITS, XH>(F, stage_of(slot), xaddr);
-#pragma unroll 1
-                    for (int k = 0; k < nstg; ++k) {
-                        const int cur = slot;
-                        advance();
-                        if (k + 1 < nstg) {
-                            mbar_wait(bar_u32 + 8 * slot, par);
-                            if (k + 1 < mine) fetch2<BITS, XH>(Fn, stage_of(slot), xaddr + XBS);
-                        }
-                        if (k < mine) math2<BITS, MODE, XH>(F, jsel, l, segc, xaddr, A);
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * cur);
-                        F = Fn;
-                        xaddr += XBS;
-                    }
-                }
-#else
                 for (int k = 0; k < nstg; ++k) {
                     mbar_wait(bar_u32 + 8 * slot, par);
                     if (k < mine) {
@@ -693,7 +657,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                     advance();
                     xaddr += XBS;
                 }
-#endif
                 {
                     float s[4];
 #pragma unroll

@@ -20,16 +20,6 @@
 //   * x is staged whole (as fp16 when it is given as fp16), the sparse warps gather it from shared memory.
 #pragma once
 
-#ifndef SQLLM_CSR_LOCAL
-#define SQLLM_CSR_LOCAL 0   // 1: a CTA sums the CSR rows of the strips it owns, in shared memory; 0: rows spread evenly over all CTAs (see sparse2)
-#endif
-#ifndef SQLLM_BOX
-#define SQLLM_BOX 1         // 1: contributions to another CTA's strip travel as self-validating {value, valid} words (see "mailboxes" below); 0: red.add + flags
-#endif
-#ifndef SQLLM_V2_PIPE
-#define SQLLM_V2_PIPE 0   // 1: two-stage ping-pong word fetch in the consumer loop (measured, not faster: see the loop)
-#endif
-
 namespace v2 {
 
 constexpr int NWC = 16;                         // consumer warps
@@ -75,17 +65,15 @@ struct P2 {
     int y_is_half;
     int hc, hrows, csr_rpc, csr_al16;
     float *ws_acc;       // fused: [N] fp32 accumulator, zero between launches
-    unsigned long long *ws_hbox;  // fused, SQLLM_BOX: [grid][64] partial strip sums of a CTA's first segment when the strip starts in an earlier CTA
-    unsigned long long *ws_cbox;  // fused, SQLLM_BOX: [N] outlier (CSR) row sums; both {float value, u32 valid}, all zero between launches
+    unsigned long long *ws_hbox;  // fused: [grid][64] partial strip sums of a CTA's first segment when the strip starts in an earlier CTA
+    unsigned long long *ws_cbox;  // fused: [N] outlier (CSR) row sums; both {float value, u32 valid}, all zero between launches
     unsigned long long *ws_dbox;  // sequence kernel: [topX][MAX_GRID_V2] dense-row partial sums, one tagged word per (dense row, contributing CTA)
-    int *ws_cnt;         // fused: [16] error flag (a bounded wait gave up; sqllm_workspace_error), [64 + s] arrivals on strip s (zero between launches)
+    int *ws_cnt;         // fused: [16] error flag (a bounded wait gave up; sqllm_workspace_error)
     int strips;          // output strips of 64 columns
     int nown_ctas;       // exchange: CTAs that own at least one strip (each announces itself once on every rank)
     int xw_world, xw_rank, xw_members, xw_nfull;
     const unsigned long long *xw_base;
     unsigned long long xw_out_off, xw_flag_off, xw_state_off, xw_err_off;
-    int sp_w0; // 1: sparse warp 0 takes half a share of the CSR rows next to the dense rows (see sparse2)
-    int l2pf;  // 1: prefetch the CTA's chunk of weights into L2 at entry
     unsigned long long *trace;
 };
 
@@ -135,7 +123,7 @@ __device__ __forceinline__ uint32_t f32x2_to_half2(float lo, float hi) {
 // the consumers only ever wait on an mbarrier that is normally long complete.  (First v2 build: the consumers rebuilt the table
 // themselves at every strip boundary; that left a bubble per switch with the warps stalled on the LUT loads.)
 // ---------------------------------------------------------------------------------------------------------------------------
-// Mailboxes (fused mode, SQLLM_BOX).  A sum that one CTA produces and another CTA needs - the partial strip sums of a CTA whose first
+// Mailboxes (fused mode).  A sum that one CTA produces and another CTA needs - the partial strip sums of a CTA whose first
 // segment continues a strip started earlier, and every outlier row sum (the CSR rows are spread evenly over the CTAs) - is written
 // ONCE, as one 64-bit word {fp32 value, valid = 1}, and the strip's owner polls that word.  A 64-bit access is single-copy atomic, so
 // the value needs no fence and no separate flag: the word validates itself.  Before: red.add into the accumulator, MEMBAR, flag
@@ -232,7 +220,6 @@ struct Acc {
 };
 
 // What a lane pulls out of a stage for one position: its 16 bytes (x 3 rows for 3-bit) and - 4-bit only, 8 inputs - its slice of x.
-// Fetched one stage AHEAD of the math (software pipeline): the LDS.128 latency hides behind the previous position's gathers.
 template <int BITS, bool XH> struct Fetch;
 template <> struct Fetch<4, true> { uint4 q, xh; };
 template <> struct Fetch<4, false> { uint4 q; float4 xa, xb; };
@@ -364,10 +351,10 @@ __device__ __forceinline__ void math2(const Fetch<BITS, XH> &F, const int jsel, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// Sparse warp(s) (NSPW per CTA).  CSR rows (= output channels) are spread evenly over the CTAs (csr_rpc consecutive rows each; split
-// between the CTA's sparse warps if there are several); warp 0 also takes the CTA's k-slice of the topX dense rows.  Everything static (row
-// pointers, the first cols/vals group, dense-row values) is requested before the x barrier; x comes from shared memory.
-// Per-row sums are taken in storage order; results go out as one red.add per row.
+// Sparse warp(s) (NSPW per CTA).  CSR rows (= output channels) are spread evenly over the CTAs (csr_rpc consecutive rows each, split
+// between the CTA's sparse warps); warp 0 also takes the CTA's k-slice of the topX dense rows.  Everything static (row pointers, the
+// first cols/vals group, dense-row values) is requested before the x barrier; x comes from shared memory.  Per-row sums are taken in
+// storage order; results go out as one red.add per row (accumulate mode) or as mailbox words (fused mode).
 // ---------------------------------------------------------------------------------------------------------------------------
 template <bool XH>
 __device__ __forceinline__ float xs_load(const uint32_t xs_u32, const int k) {
@@ -383,7 +370,6 @@ __device__ __forceinline__ float xs_load(const uint32_t xs_u32, const int k) {
 template <bool XH, bool FUSED>
 __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const uint32_t base, const int spw, const int lane, float *acc_out, const uint32_t boxtag = 1u) {
     const int N = p.N;
-    constexpr bool BOX = FUSED && SQLLM_BOX && !SQLLM_CSR_LOCAL;  // cross-CTA sums travel as mailbox words
     const uint32_t xs_u32 = base + OFF_X;
     const uint32_t stage_u32 = base + OFF_CSR + spw * SP_BYTES;       // this warp's chunk buffer b: cols at +b*SP_CH*8, vals SP_CH*4 further
     int *srow = reinterpret_cast<int *>(sm + OFF_SROW);               // [SP_ROWS + 1] row pointers of the CTA's rows (FUSED, when they fit)
@@ -405,40 +391,28 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
             hfr[i] = (rs < nsl && k < ke) ? __ldg(p.full_rows + (size_t)k * p.topX + hj) : 0.f;
         }
     }
-    // FUSED: the CSR rows of the strips this CTA OWNS (those that start in its range - it also finishes them), so that outlier sums
-    // never leave the CTA: they go into a shared-memory row accumulator that the builders add when they write y.  (Earlier v2 builds
-    // spread the rows evenly over all CTAs and announced them on the strips' flags: a MEMBAR.GPU per announcement, and every strip owner
-    // waited for some other CTA's sparse warp - the critical path of the kernel on layers with outliers.)
-    // Accumulate mode (the 12 symbols, no owner): rows spread evenly over the CTAs, one red.add per row into `mul`.
-    // The CTA's rows [ca, cb) are split over its NSPW sparse warps (warp 0, which also has the dense rows, takes half a share).
+    // This CTA's CSR rows [ca, cb): csr_rpc consecutive rows, the same share for every CTA, whichever strips they fall in.  Accumulate mode
+    // (the 12 symbols) adds each row sum into `mul` with one red.add; fused mode publishes it as a mailbox word that the owner of the row's
+    // strip (the CTA in whose range the strip starts) collects when it writes y.  The rows are split over the NSPW sparse warps.
     int ca = 0, cb = 0;
     if (p.rows) {
-        if constexpr (FUSED && SQLLM_CSR_LOCAL) {
-            const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
-            ca = min(N, (int)((cb0 + p.R - 1) / p.R) * STRIP);
-            cb = min(N, (int)((cb1 + p.R - 1) / p.R) * STRIP);
-        } else {
-            ca = min(N, (int)blockIdx.x * p.csr_rpc);
-            cb = min(N, ca + p.csr_rpc);
-        }
+        ca = min(N, (int)blockIdx.x * p.csr_rpc);
+        cb = min(N, ca + p.csr_rpc);
     }
     int r, rb;
     {
-        // warp 0 also has the dense rows (atomics, a fence, the announcement after x arrives).  sp_w0 = 0 (default): it then takes no CSR
-        // rows at all - the outlier sums are what the owners of ALL strips wait for, they must not queue behind that fence; 1: half a share (round-2
-        // first build; A/B with SQLLM_SP_W0=1)
-        const int tot = cb - ca, w0 = p.full_rows ? (p.sp_w0 ? tot / (2 * NSPW) : 0) : tot / NSPW, rest = tot - w0;
+        // warp 0 also has the dense rows; when there are any it takes no CSR rows: the outlier sums are what the owners of ALL strips
+        // wait for, they must not queue behind the dense-row work
+        const int tot = cb - ca, w0 = p.full_rows ? 0 : tot / NSPW, rest = tot - w0;
         r = spw == 0 ? ca : ca + w0 + (int)((long long)rest * (spw - 1) / (NSPW - 1));
         rb = spw == 0 ? ca + w0 : ca + w0 + (int)((long long)rest * spw / (NSPW - 1));
     }
     const int nr = rb - r;
-    const bool rows_in_smem = cb - ca <= SP_ROWS;                       // the CTA's row pointers live in shared memory
-    const bool local_sums = FUSED && SQLLM_CSR_LOCAL && rows_in_smem;  // ... and so do the row sums (same rule in the builders)
-    // (BOX: row sums are published as mailbox words when the warp is through)
-    const bool smem_sums = local_sums || (BOX && rows_in_smem);
+    const bool rows_in_smem = cb - ca <= SP_ROWS;      // the CTA's row pointers live in shared memory
+    const bool smem_sums = FUSED && rows_in_smem;      // ... and so do the row sums, published as mailbox words when the warp is through
     auto emit = [&](int row, float v) {
         if (smem_sums) srowacc[row - ca] += v;  // plain read-modify-write: a row belongs to this warp alone and its pieces arrive one after the other
-        else if (BOX) atomicAdd(reinterpret_cast<float *>(p.ws_cbox + row), v);  // (more rows per CTA than the shared accumulator holds: value half of the word)
+        else if (FUSED) atomicAdd(reinterpret_cast<float *>(p.ws_cbox + row), v);  // (more rows per CTA than the shared accumulator holds: value half of the word)
         else atomicAdd(acc_out + row, v);
     };
     int e_lo = 0, e_hi = 0;
@@ -507,7 +481,7 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
                     if (rs == 0) a += v;
                 }
                 if (rs != 0) j = p.topX;  // only slot 0 publishes
-                if constexpr (BOX) {
+                if constexpr (FUSED) {
                     // dense rows that feed the SAME channel travel as one word (the first of them carries the sum): the owner of that channel's
                     // strip then reads hc words, not hc per row - a checkpoint without dense rows loads as topX rows on channel 0 (llama.py:182)
                     const int cme = (rs == 0 && hj < p.topX) ? __ldg(p.fri + hj) : -1 - lane;
@@ -529,7 +503,7 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
                     for (int k = kb; k < ke; ++k, fr += p.topX) a += __ldg(fr) * xs_load<XH>(xs_u32, k);
                 }
             }
-            if constexpr (BOX) {
+            if constexpr (FUSED) {
                 // this CTA's part of dense row j: one self-validating word, no RED + fence + flag (the owner of the channel's strip sums the hc words of
                 // row j, lutgemv2_kernel's finishers); before: atomics into the accumulator, a MEMBAR.GPU and an announcement per strip - the fence
                 // alone held this warp, and with it every owner that waited for the announcement
@@ -537,23 +511,6 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
             } else if (j < p.topX) {
                 const int c = __ldg(p.fri + j);
                 if (c >= 0 && c < N) atomicAdd(acc_out + c, a);
-            }
-        }
-        if constexpr (FUSED && SQLLM_CSR_LOCAL) {
-            // announce this CTA's dense-row contributions now, early in the kernel: one fence, then a relaxed increment per distinct
-            // strip that holds a dense-row channel (every one of the hc contributing CTAs does this; the owners expect hc arrivals)
-            __threadfence();
-            __syncwarp();
-            int *flags = p.ws_cnt + 64;
-            for (int j = lane; j < p.topX; j += 32) {
-                const int c = __ldg(p.fri + j);
-                if (c < 0 || c >= N) continue;
-                bool seen = false;
-                for (int j2 = 0; j2 < j; ++j2) {
-                    const int c2 = __ldg(p.fri + j2);
-                    seen |= (c2 >= 0 && c2 < N && c2 / STRIP == c / STRIP);
-                }
-                if (!seen) asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(flags + c / STRIP) : "memory");
             }
         }
     }
@@ -627,10 +584,7 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
         __syncwarp();
         stage_chunk(ci + 2);  // this buffer is free again
     }
-    if constexpr (FUSED && SQLLM_CSR_LOCAL) {
-        if (!local_sums && cb > ca) __threadfence();  // (more owned rows than the row accumulator holds: sums went to global memory)
-        named_bar_sync(4, (NSPW + NBW) * 32);         // hand-over to the builders: row sums complete
-    } else if constexpr (BOX) {
+    if constexpr (FUSED) {
         // every row of this warp's share gets its word, outlier-free rows included (the owner of the strip waits for all 64 of them)
         __syncwarp();
         if (smem_sums) {
@@ -638,30 +592,6 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
         } else if (nr > 0) {
             __threadfence();  // the red.adds on the value halves come first
             for (int i = lane; i < nr; i += 32) asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(reinterpret_cast<uint32_t *>(p.ws_cbox + r + i) + 1), "r"(1u) : "memory");
-        }
-    } else if constexpr (FUSED) {
-        // Balanced mode: this CTA's outlier sums went to the global accumulator with red.add.  Announce them: all sparse warps meet,
-        // then ONE fence (by warp 0) and a relaxed increment per strip the CTA's rows touch (whatever their nnz) and per distinct
-        // strip that holds a dense-row channel - the owners of those strips expect exactly these arrivals.
-        named_bar_sync(5, NSPW * 32);
-        if (spw == 0) {
-            __threadfence();
-            __syncwarp();
-            int *flags = p.ws_cnt + 64;
-            if (cb > ca)
-                for (int s = ca / STRIP + lane; s <= (cb - 1) / STRIP; s += 32)
-                    asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(flags + s) : "memory");
-            if (p.full_rows && (int)blockIdx.x < p.hc)
-                for (int j = lane; j < p.topX; j += 32) {
-                    const int c = __ldg(p.fri + j);
-                    if (c < 0 || c >= N) continue;
-                    bool seen = false;
-                    for (int j2 = 0; j2 < j; ++j2) {
-                        const int c2 = __ldg(p.fri + j2);
-                        seen |= (c2 >= 0 && c2 < N && c2 / STRIP == c / STRIP);
-                    }
-                    if (!seen) asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(flags + c / STRIP) : "memory");
-                }
         }
     }
 }
@@ -715,17 +645,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_big)) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_small)) : "memory");
-        }
-        if (p.l2pf) {
-            // the CTA's whole chunk of weights -> L2, one box per lane and instruction, before the dependency wait: the ring then only has
-            // to cover L2 latency, and under PDL these requests overlap the previous kernel's tail
-            for (int seg = 0; seg < nseg; ++seg) {
-                const int sstart = seg == 0 ? 0 : seg * R - r0, send = min(len, (seg + 1) * R - r0);
-                const int u0 = r0 + sstart - seg * R, col0 = (s0 + seg) * STRIP;
-                for (int u = lane * SU2; u < send - sstart; u += 32 * SU2)
-                    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(&tm_big)),
-                                 "r"(col0), "r"((u0 + u) * C::ROWS) : "memory");
-            }
         }
         const int G = (int)gridDim.x;
         const size_t lut_lines = ((size_t)N * C::L * 4 + 127) / 128, per = (lut_lines + G - 1) / G;
@@ -785,7 +704,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         const uint32_t lutbuf = base + OFF_LUT, sacc = base + OFF_SACC;
         sts_u32(sacc + 4 * bt, 0u);
         sts_u32(sacc + 4 * (STRIP + bt), 0u);
-        int *const flags = p.ws_cnt + 64;
         bool dep_ok = false;
         auto dep_wait = [&]() { if (!dep_ok) { pdl_wait(); dep_ok = true; } };  // builders never read x: they only need this before writing
         const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
@@ -795,7 +713,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             const float v = lds_f32(a);
             sts_u32(a, 0u);
             const int strip = s0 + s, col = strip * STRIP + bt;
-            if constexpr (FUSED && SQLLM_BOX && !SQLLM_CSR_LOCAL) {
+            if constexpr (FUSED) {
                 // A strip is finished (converted to y) by the CTA in whose range it STARTS; a CTA that only holds a later part of it
                 // (that can only be its first segment) hands its sums to that owner through its mailbox row.
                 // ... or to ourselves: then they never leave the SM (sown[u][column] for the u-th owned strip; a strip inside one CTA is exactly
@@ -806,13 +724,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                 else if (col < N) atomicAdd(acc_out + col, v);
             } else {
                 if (col < N) atomicAdd(acc_out + col, v);
-                if constexpr (FUSED) {
-                    // (flag protocol) ... announces its contribution on the strip's flag
-                    if (s == 0 && r0 != 0) {
-                        named_bar_sync(3, NBT);
-                        if (bt == 0) asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(flags + strip) : "memory");
-                    }
-                }
             }
         };
         // The raw LUT rows of the first two strips are requested at once (one cold round trip, not two); later strips two ahead.
@@ -841,14 +752,12 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             }
         } else {
             // ---- finish the strips this CTA owns (those that start in its range).  Every table is built, so the builders have time: while
-            //      the consumers are still in the last segment they wait for the other contributors' announcements - dense CTAs holding a
-            //      later part, the hc dense-row CTAs if a dense-row channel lies in it (the strips' CSR outliers are summed by this CTA's
-            //      own sparse warp, in shared memory) - and fetch the accumulator.  What is left for the very end is y = accumulator + own last strip (+ bias): no round trip to
-            //      L2 after the last weight, no grid-wide step; a CTA leaves as soon as its own strips are complete.
-            //      Waits are bounded (2 s, then the workspace error word is set).
-#if SQLLM_BOX && !SQLLM_CSR_LOCAL
-            // ---- mailbox variant (shared with the sequence kernel, lutgemv_seq.cuh): own strip sums from shared memory, outlier sums and the later
-            //      CTAs' first-segment sums from their mailbox words, dense rows from one tagged word per (contributing CTA, row).
+            //      the consumers are still in the last segment they collect the other contributors' mailbox words - the outlier row sums of
+            //      the strips' columns, the first-segment sums of the later CTAs that hold a part of the last owned strip, one tagged word
+            //      per (contributing CTA, dense row) if a dense-row channel lies in an owned strip - and add them to this CTA's own strip
+            //      sums, which never leave shared memory.  What is left for the very end is y = collected sums + own last segment (+ bias):
+            //      no round trip to L2 after the last weight, no grid-wide step; a CTA leaves as soon as its own strips are complete.
+            //      Waits are bounded (2 s, then the workspace error word is set).  The sequence kernel (lutgemv_seq.cuh) finishes the same way.
             TRACE(12, bt == 0);
             const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
             const int so0 = (int)((cb0 + R - 1) / R), so1 = (int)((cb1 + R - 1) / R), nown = so1 - so0;
@@ -1024,109 +933,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                     }
                 }
             }
-            
-#else
-            if (nseg >= 2) {
-                mbar_wait(bar_u32 + 272 + 8 * ((nseg - 2) & 1), (uint32_t)(((nseg - 2) >> 1) & 1));
-                flush(nseg - 2);
-            }
-            const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
-            const int so0 = (int)((cb0 + R - 1) / R), so1 = (int)((cb1 + R - 1) / R), nown = so1 - so0;
-            const bool last_owned = nseg >= 2 || r0 == 0;  // the last segment's strip starts in this CTA's range (it is strip so1 - 1)
-            for (int i = bt; i < nown; i += NBT) {
-                const int strip = so0 + i;
-                int expect = (int)((((long long)strip + 1) * R - 1) / p.chunk) - (int)blockIdx.x;  // dense CTAs after this one
-                if (!SQLLM_CSR_LOCAL && p.rows) {  // every CTA whose share of the CSR rows touches the strip
-                    const int c0 = strip * STRIP, c1 = min(N, c0 + STRIP) - 1;
-                    expect += c1 / p.csr_rpc - c0 / p.csr_rpc + 1;
-                }
-                if (p.full_rows) {
-                    bool h = false;
-                    for (int j = 0; j < p.topX; ++j) {
-                        const int c = __ldg(p.fri + j);
-                        h |= (c >= 0 && c < N && c / STRIP == strip);
-                    }
-                    if (h) expect += p.hc;
-                }
-                if (expect > 0) {
-                    int seen;
-                    unsigned long long t0 = 0ull, t1;
-                    do {
-                        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(flags + strip) : "memory");
-                        if (seen >= expect) break;
-                        __nanosleep(40);
-                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                        if (t0 == 0ull) t0 = t1;
-                        if (t1 - t0 > 2000000000ull) { *reinterpret_cast<volatile int *>(p.ws_cnt + 16) = 1; break; }
-                    } while (true);
-                    flags[strip] = 0;
-                }
-            }
-            named_bar_sync(3, NBT);  // the polls above are through: the others' contributions to every owned strip are complete
-            const float *srowacc = reinterpret_cast<const float *>(sm + OFF_SROW + (SP_ROWS + 1) * 4);
-            const bool local_sums = SQLLM_CSR_LOCAL && p.rows && min(N, so1 * STRIP) - min(N, so0 * STRIP) <= SP_ROWS;  // same rule as the sparse warps'
-            const int w = p.xw_world ? N / p.xw_members : 0;
-            auto store_y = [&](int col, float yv) {
-                if (local_sums) yv += srowacc[col - so0 * STRIP];
-                if (p.bias) yv += __ldg(p.bias + col);
-                if (p.xw_world == 0) {
-                    if (p.y_is_half) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(yv);
-                    else reinterpret_cast<float *>(p.out)[col] = yv;
-                } else {
-                    // local column col of the stacked shard = column j of member m; it lands at [m][rank*w + j] of the
-                    // [members][n_full] vector in EVERY rank's arena
-                    const int mm = col / w, j = col - mm * w;
-                    const unsigned long long e = (unsigned long long)mm * p.xw_nfull + (unsigned long long)p.xw_rank * w + j;
-                    for (int pr = 0; pr < p.xw_world; ++pr) {
-                        unsigned char *dst = reinterpret_cast<unsigned char *>(__ldg(p.xw_base + pr) + p.xw_out_off);
-                        if (p.y_is_half) *reinterpret_cast<__half *>(dst + 2 * e) = __float2half_rn(yv);
-                        else *reinterpret_cast<float *>(dst + 4 * e) = yv;
-                    }
-                }
-            };
-            // accumulator values first (strips whose own part is already in it: all owned ones but, if owned, the last segment's; and what
-            // the others added to that last one - our own part of it never goes through memory), then wait for this CTA's sparse warps
-            // (their row sums are needed from here on), then the stores
-            const int nearly = last_owned ? nown - 1 : nown;
-            float vv[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int col = (so0 + u) * STRIP + bt;
-                vv[u] = (u < nearly && col < N) ? __ldcg(p.ws_acc + col) : 0.f;
-            }
-            float pre = 0.f;
-            const int lcol = (s0 + nseg - 1) * STRIP + bt;
-            if (last_owned && nseg > 0 && lcol < N) pre = __ldcg(p.ws_acc + lcol);
-            if (SQLLM_CSR_LOCAL) named_bar_sync(4, (NSPW + NBW) * 32);  // this CTA's own outlier row sums (sparse warps) are complete
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int col = (so0 + u) * STRIP + bt;
-                if (u < nearly && col < N) {
-                    p.ws_acc[col] = 0.f;
-                    store_y(col, vv[u]);
-                }
-            }
-            for (int i = 8; i < nearly; ++i) {  // (more than 8 owned strips: out_features > 75,000 - one at a time)
-                const int col = (so0 + i) * STRIP + bt;
-                if (col < N) {
-                    const float a = __ldcg(p.ws_acc + col);
-                    p.ws_acc[col] = 0.f;
-                    store_y(col, a);
-                }
-            }
-            if (last_owned && nseg > 0 && lcol < N) p.ws_acc[lcol] = 0.f;
-            TRACE(8, bt == 0);
-            if (nseg > 0) {
-                const int s = nseg - 1;
-                mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1));
-                if (last_owned) {
-                    const float own = lds_f32(sacc + 4 * ((s & 1) * STRIP + bt));
-                    if (lcol < N) store_y(lcol, pre + own);
-                } else {
-                    flush(s);  // a CTA that lies wholly inside a strip started by another one: contribute and announce
-                }
-            }
-#endif
             if (p.xw_world) {
                 // exchange: every owning CTA publishes its stores on every rank (system-scope release); CTA 0 (it always owns strip 0)
                 // then holds the grid open until every owning CTA of every rank has published on ours: when this grid completes, the
@@ -1213,43 +1019,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             mbar_wait(bar_u32 + 256 + 8 * b, (uint32_t)((seg >> 1) & 1));  // table b holds this strip
             TRACE(16 + (seg < 7 ? seg : 7), tid == 0);
             // Every consumer warp walks every stage of the segment (the empty barriers count NWC arrivals); a warp whose pair lies past
-            // the end of a ragged last stage just releases it.  Two stages per trip, ping-pong: while the gathers of one position run,
-            // the words (and x) of the next are already on their way from shared memory into the other register set.
-#if SQLLM_V2_PIPE
-            Fetch<BITS, XH> F0, F1;
-            int k = 0, sl0, sl1;
-            mbar_wait(bar_u32 + 8 * slot, par);
-            if (0 < mine) fetch2<BITS, XH>(F0, stage_of(slot), xaddr);
-            sl0 = slot;
-            advance();
-            while (true) {
-                sl1 = slot;
-                if (k + 1 < nstg) {
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (k + 1 < mine) fetch2<BITS, XH>(F1, stage_of(slot), xaddr + XBS);
-                    advance();
-                }
-                if (k < mine) math2<BITS, MODE, XH>(F0, jsel, l, segc, xaddr, A);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * sl0);  // stage k: its words went to registers a step ago
-                if (k + 1 >= nstg) break;
-                sl0 = slot;
-                if (k + 2 < nstg) {
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (k + 2 < mine) fetch2<BITS, XH>(F0, stage_of(slot), xaddr + 2 * XBS);
-                    advance();
-                }
-                if (k + 1 < mine) math2<BITS, MODE, XH>(F1, jsel, l, segc, xaddr + XBS, A);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * sl1);
-                if (k + 2 >= nstg) break;
-                k += 2;
-                xaddr += 2 * XBS;
-            }
-#else
-            // one stage per trip, no look-ahead: the smallest loop body.  (The two-stage ping-pong variant above hides the word fetch
-            // behind the previous position's gathers but doubles the body to ~290 instructions; with 23 warps in five roles on the SM
-            // the instruction cache misses ate the gain - ncu showed many stall samples on "no instruction".)
+            // the end of a ragged last stage just releases it.  One stage per trip, no look-ahead: the smallest loop body.  (A two-stage
+            // ping-pong variant that hides the word fetch behind the previous position's gathers doubles the body to ~290 instructions;
+            // with 23 warps in five roles on the SM the instruction cache misses ate the gain - ncu showed many stall samples on
+            // "no instruction".)
             for (int k = 0; k < nstg; ++k) {
                 mbar_wait(bar_u32 + 8 * slot, par);
                 if (k < mine) {
@@ -1262,7 +1035,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                 advance();
                 xaddr += XBS;
             }
-#endif
             {   // this strip's sums: lane (i, j=1) holds column t^1 in slot t - hand it to lane (i, j=0), which adds both into the CTA's
                 // shared accumulator of the strip (16 warps x 64 red.shared.add; the builders move it on to global memory)
                 float s[4];

@@ -38,6 +38,9 @@ SHAPES = [  # (bits, K, N, sparsity, topX, nonzero_full_rows, skew)
     (4, 4096, 12288, 0.0045, 10, True, True),   # 7B q+k+v stacked, skewed outliers
     (4, 256, 44032, 0.01, 4, True, False),      # more CSR rows per CTA than the shared row accumulator holds (mailbox fallback path)
     (3, 11008, 64, 0.01, 4, True, False),       # one strip, every CTA inside it: 147 mailbox rows for one owner
+    # narrower than one strip (out < 64): the round-1 kernel runs these in every mode, not only the deterministic one
+    (4, 256, 32, 0.02, 4, True, False),
+    (3, 128, 60, 0.0, 0, False, False),
 ]
 IDS = [f"w{b}-{k}x{n}-s{int(s*1e4)}-t{t}{'-nz' if z else ''}{'-skew' if sk else ''}" for b, k, n, s, t, z, sk in SHAPES]
 BATCHED_SHAPES = [s for s in SHAPES if s[1] <= 512] + [(4, 4096, 4096, 0.0045, 10, True, False), (3, 11008, 4096, 0.0045, 10, True, True)]
