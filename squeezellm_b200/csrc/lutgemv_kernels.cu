@@ -59,12 +59,12 @@ constexpr int STRIP = 64;                 // output columns per strip (16 lanes 
 constexpr int SU = 2 * NW;                // units per pipeline stage (one pair per consumer warp)
 constexpr int CSR_CH = 1024;              // CSR elements staged per chunk
 constexpr int SROWS_LD = 68;              // padded row-pointer slice per segment (65 used)
-constexpr int MAX_TOPX_FUSED = 128;
+constexpr int MAX_TOPX_FUSED = SQLLM_FUSED_MAX_TOPX;
 constexpr int NFIN_COLS = 1024;           // fast fused mode: about this many columns per finishing CTA ...
 constexpr int NFIN_MAX = 16;              // ... and at most this many finishers
 constexpr int HYB_R = 11;                 // dense rows: k-rows per lane slot requested before the dependency wait
 constexpr int MAX_STRIPS = 16320;         // per-strip tickets in the workspace header (out_features <= 1,044,480)
-constexpr int MAX_N_FUSED = 262144;        // fused path: the scratch accumulator lives at a fixed place in the workspace
+constexpr int MAX_N_FUSED = SQLLM_FUSED_MAX_OUT;  // fused path: the scratch accumulator lives at a fixed place in the workspace
 constexpr size_t WS_ACC_OFF = 65536;       // [64 KB, 64 KB + 4*MAX_N_FUSED): fp32 accumulator (zero between launches)
 constexpr int MAX_GRID_V2 = 256;           // v2 runs one CTA per SM
 constexpr size_t WS_HBOX_OFF = WS_ACC_OFF + (size_t)MAX_N_FUSED * 4;       // v2 mailboxes: [MAX_GRID_V2][64] x 8 bytes (partial strip sums)

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `unpack_indices`, `abi_version`.
+// Extra, not in the reference: `lutgemv_fused`, `unpack_indices`, `abi_version`, `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -415,4 +415,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           },
           "True if a bounded in-kernel wait of the fused path ever timed out on this stream's workspace (results are then incomplete)");
     m.def("sm_count", []() { return sqllm_device_sm_count(); });
+    m.def("fused_limits", []() {
+              py::dict d;
+              d["max_topx"] = SQLLM_FUSED_MAX_TOPX;
+              d["max_out_features"] = SQLLM_FUSED_MAX_OUT;
+              return d;
+          },
+          "largest layer the fused, exchange and sequence entry points accept: {'max_topx', 'max_out_features'} (the 12 symbols have no such limit)");
 }

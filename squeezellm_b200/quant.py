@@ -8,7 +8,8 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
   * `forward` (batch-1 branch, reference quant.py:212-312) uses ONE fused launch
     (`quant_cuda.lutgemv_fused`: fp16/fp32 x in, y out in x's dtype, bias + CSR + dense rows fused;
     `quant_cuda.set_deterministic(True)` selects the bit-reproducible summation) instead of
-    zeros + x.float() + 1-3 launches + y.to(dtype).  Set
+    zeros + x.float() + 1-3 launches + y.to(dtype).  Layers wider or with more dense rows than the fused launch
+    takes (`FUSED_LIMITS`, from the extension) run the reference's 12 symbols instead.  Set
     `QuantLinearLUT.use_fused = False` to go through the reference's 12 symbols exactly as quant.py does.
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
@@ -56,6 +57,8 @@ def _load_extension():
 
 
 quant_cuda = _load_extension()
+# largest layer the fused launch takes (include/sqllm_b200.h: SQLLM_FUSED_MAX_TOPX / SQLLM_FUSED_MAX_OUT); larger layers run the 12 symbols
+FUSED_LIMITS = quant_cuda.fused_limits()
 
 
 def round_to_nearest_pole_sim(w, poles):
@@ -164,6 +167,12 @@ class QuantLinearLUT(nn.Module):
             fr, fri = self.full_rows, self.full_row_indices
         return self.rows, self.cols, self.vals, fr, fri
 
+    def _fused_fits(self, full_rows):
+        """The fused launch keeps its cross-CTA sums in a fixed-size workspace: more output channels or dense rows than it holds
+        (a stacked q/k/v group adds up its members' dense rows) go through the 12 symbols, which have no such limit."""
+        topx = int(full_rows.shape[1]) if full_rows is not None else 0
+        return self.outfeatures <= FUSED_LIMITS["max_out_features"] and topx <= FUSED_LIMITS["max_topx"]
+
     def forward(self, x):
         if self._sibling_group is not None:
             group, index = self._sibling_group
@@ -172,8 +181,8 @@ class QuantLinearLUT(nn.Module):
         if x.shape[-1] == x.numel():
             outshape = list(x.shape)
             outshape[-1] = self.outfeatures
-            if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32):
-                rows, cols, vals, fr, fri = self._sparse_args()
+            rows, cols, vals, fr, fri = self._sparse_args()
+            if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32) and self._fused_fits(fr):
                 y = quant_cuda.lutgemv_fused(x.contiguous(), self.qweight, self.lookup_table, self.bits,
                                              self.bias, rows, cols, vals, fr, fri)
                 return y.reshape(outshape)

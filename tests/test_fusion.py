@@ -106,7 +106,12 @@ def test_fuse_siblings_walks_llama_like_modules():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("bits,K,widths,sp,topx", [(4, 4096, [4096, 4096, 4096], 0.0045, 10), (3, 4096, [11008, 11008], 0.0045, 10),
-                                                   (4, 512, [128, 256], 0.0, 0)], ids=["w4-qkv", "w3-gateup", "w4-small-dense"])
+                                                   (4, 512, [128, 256], 0.0, 0),
+                                                   # the middle member has no dense rows: 2 x topX stacked
+                                                   (4, 1024, [1024, 1024, 1024], 0.01, 16),   # 32: the topX <= 32 branch at its edge
+                                                   (3, 1024, [1024, 1024, 1024], 0.01, 17),   # 34: the general branch
+                                                   (4, 1024, [1024, 1024, 1024], 0.01, 70)],  # 140: more than the fused launch takes
+                         ids=["w4-qkv", "w3-gateup", "w4-small-dense", "w4-qkv-t16", "w3-qkv-t17", "w4-qkv-t70"])
 def test_stacked_launch_matches_members(bits, K, widths, sp, topx):
     Ls = _layers(bits, K, widths, sp, topx)
     ms = [_member(L).cuda() for L in Ls]

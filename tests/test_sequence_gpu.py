@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import REL_TOL, orc, rel_err
+from util import REL_TOL, late_owned_strips, orc, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -13,19 +13,34 @@ pytestmark = pytest.mark.gpu
 def _module(L, bits, K, N, topX):
     from squeezellm_b200.quant import QuantLinearLUT
     has_csr = L.get("rows") is not None
-    m = QuantLinearLUT(bits, K, N, False, include_sparse=has_csr, numvals=len(L["vals"]) if has_csr else 0, topX=topX if has_csr else 0)
+    dense_only = not has_csr and L.get("full_rows") is not None
+
+    class DenseRowsOnly(QuantLinearLUT):  # dense rows without CSR outliers (the C ABI takes them; a checkpoint never has them)
+        def _sparse_args(self):
+            return None, None, None, self.full_rows, self.full_row_indices
+
+    m = (DenseRowsOnly if dense_only else QuantLinearLUT)(bits, K, N, False, include_sparse=has_csr or dense_only,
+                                                           numvals=len(L["vals"]) if has_csr else 0, topX=topX if has_csr or dense_only else 0)
     sd = m.state_dict()
     m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in sd}, strict=False)
     return m.cuda()
 
 
 def _chain(bits, dims, sparsity, topX, seed):
-    """dims: [(K, N, x_offset into the previous output)]; returns oracle layers + modules."""
+    """dims: [(K, N, x_offset into the previous output)]; returns oracle layers + modules.  topX > 0 with sparsity 0: dense rows
+    without CSR outliers (the sequence kernel keeps at most 255 outlier rows per CTA, which rules CSR out on very wide items)."""
+    from squeezellm_b200.quant import quant_cuda as qc
     layers, mods = [], []
     for i, (K, N, _) in enumerate(dims):
         L = orc.make_layer(bits, K, N, sparsity=sparsity, topX=topX, seed=seed + 17 * i, nonzero_full_rows=True)
-        if topX and sparsity == 0:
-            L["full_rows"] = L["full_row_indices"] = None
+        rng = np.random.default_rng(seed + 17 * i + 1)
+        late = late_owned_strips(bits, K, N, qc.sm_count()) if topX > 32 else []
+        if topX > 32 and len(late):  # CTAs that own more than 8 strips: rows in their 9th and later strips, duplicates, channel 0
+            f = rng.choice(late, size=topX) * 64 + rng.integers(0, 64, size=topX)
+            f[1], f[2], f[3] = f[0], 0, N - 1
+            L["full_row_indices"] = f.astype(np.int32)
+        elif topX > 32 and i % 2 == 1:  # every row in one strip, with duplicates
+            L["full_row_indices"] = (N // 128 * 64 + rng.integers(0, 64, size=topX)).astype(np.int32)
         elif topX >= 3 and i % 2 == 0:  # dense rows that feed the same output channel (their parts travel combined), one of them channel 0
             L["full_row_indices"][1] = L["full_row_indices"][0]
             L["full_row_indices"][2] = 0
@@ -56,6 +71,11 @@ CASES = [  # (bits, dims, sparsity, topX)
     (4, [(512, 132, 0), (128, 200, 4), (192, 64, 8), (64, 512, 0), (512, 132, 0)], 0.01, 3),   # ragged strips, one-strip items
     (4, [(4096, 12288, 0), (4096, 4096, 8192), (4096, 22016, 0), (11008, 4096, 0)], 0.0045, 10, 3),  # LLaMA-7B decoder layer, three times over
     (3, [(4096, 12288, 0), (4096, 4096, 8192), (4096, 22016, 0), (11008, 4096, 0)], 0.0045, 10, 2),
+    # more than 32 dense rows: the general dense-row branch (duplicates, channel 0, all rows in one strip)
+    (4, [(256, 768, 0), (256, 256, 512), (256, 704, 0), (704, 256, 0)], 0.02, 33),
+    (3, [(256, 768, 0), (256, 256, 512), (256, 704, 0), (704, 256, 0)], 0.02, 128),
+    # a 131072-column item (CTAs own ~16 strips; dense rows in their 9th and later), then an item that reads its last 4096 outputs
+    (4, [(128, 131072, 0), (4096, 768, 126976), (768, 256, 0)], 0.0, 128),
 ]
 IDS = [f"w{c[0]}-{len(c[1])}items-K{c[1][0][0]}-s{int(c[2] * 1e4)}-t{c[3]}" for c in CASES]
 
@@ -87,16 +107,28 @@ def test_sequence_matches_layer_by_layer_and_oracle(case, mode):
             ys.append(cur)
     finally:
         quant_cuda.set_lut_mode("exact")
+    x_half = (x.astype(np.float32) * 0.5).astype(np.float16)
     for rep in range(3):  # replays: the tags of the previous token must not be taken for this one's
         if rep == 2:
-            seq.x.copy_(torch.from_numpy((x.astype(np.float32) * 0.5).astype(np.float16)).cuda())
+            seq.x.copy_(torch.from_numpy(x_half).cuda())
         outs = [o.clone() for o in seq.replay()]
         torch.cuda.synchronize()
         assert not seq.error(), "a bounded in-kernel wait of the sequence gave up"
         if rep == 2:
-            want = _oracle_chain(layers, dims, (x.astype(np.float32) * 0.5).astype(np.float16).astype(np.float64), lut_fp16=(mode == "fp16"))
+            want = _oracle_chain(layers, dims, x_half.astype(np.float64), lut_fp16=(mode == "fp16"))
+        got_all = [o.float().cpu().numpy().astype(np.float64) for o in outs]
+        for i, (L, (K, N, off)) in enumerate(zip(layers, dims)):
+            # per item, per element: the oracle applied to the fp16 vector this item actually consumed (seq.x, or the exported slice of
+            # its predecessor), so that no hand-over rounding blurs the check
+            xin = (x if rep < 2 else x_half).astype(np.float64) if i == 0 else got_all[i - 1][off:off + K]
+            LL = dict(L)
+            if mode == "fp16":
+                LL["lookup_table"] = L["lookup_table"].astype(np.float16).astype(np.float32)
+            wi = orc.forward_f64(LL, xin.astype(np.float32).reshape(1, K)).reshape(N)
+            err_i = rel_err(got_all[i], wi)
+            assert err_i < REL_TOL, f"rep {rep} item {i}: {err_i:.3e} against the oracle on the item's own input"
         for i, (o, w) in enumerate(zip(outs, want)):
-            got = o.float().cpu().numpy().astype(np.float64)
+            got = got_all[i]
             # fp16 hand-overs: one fp16 ulp of an input moves later outputs; compare in the max norm at the north_star tolerance,
             # plus the strict per-element metric for the first item (no hand-over before it)
             err = np.abs(got - w).max() / max(np.abs(w).max(), 1e-30)

@@ -67,6 +67,22 @@ class Args(ctypes.Structure):  # mirrors sqllm_lutgemv_args
                 ("full_row_indices", ctypes.c_void_p), ("topX", ctypes.c_int)]
 
 
+def late_owned_strips(bits, K, N, sm, first=8):
+    """Strips that are the (first+1)-th or later strip owned by some CTA of the one-CTA-per-SM kernels (lutgemv_v2.cuh, lutgemv_seq.cuh):
+    the [strip][unit] space (R units per 64-column strip) is cut into chunks of 2*ceil(T / (2*sm)) units, and a strip is owned by the CTA
+    in whose chunk it starts.  Their finishers keep `first` = 8 owned strips in shared memory; the sums of later ones go through the
+    global accumulator."""
+    R = K // 8 if bits == 4 else K // 32
+    strips = (N + 63) // 64
+    T = strips * R
+    chunk = max(2, 2 * ((T + 2 * sm - 1) // (2 * sm)))
+    out = []
+    for b in range((T + chunk - 1) // chunk):
+        so0, so1 = (b * chunk + R - 1) // R, (min(T, (b + 1) * chunk) + R - 1) // R
+        out.extend(range(so0 + first, so1))
+    return np.asarray(out, dtype=np.int64)
+
+
 def to_torch(layer, device="cuda"):
     """numpy layer dict (oracle.make_layer) -> dict of torch tensors on `device`."""
     import torch
