@@ -47,7 +47,8 @@ extern "C" {
 #define SQLLM_ECUDA (-2)    /* a CUDA runtime call or launch failed */
 #define SQLLM_EWORKSPACE (-3) /* workspace missing or too small */
 
-#define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_* */
+#define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
+                                 later + sqllm_lutgemm_fused (backward compatible, same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -124,6 +125,18 @@ int sqllm_workspace_error(const void *workspace, void *stream);
 int sqllm_lutgemv_fused(const sqllm_lutgemv_args *args,
                         const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
                         void *workspace, size_t workspace_bytes, void *stream);
+
+/* Fused module path for M >= 1 rows (prefill, evaluation) on the tensor cores (wgmma):
+ *   y[m][c] = bias[c] + LUT-GEMM + CSR + dense rows, written (not accumulated), from fp16 x [M][in_features] (row-major),
+ * in ONE launch.  args->batch = M; args->vec / args->mul are ignored.  y is fp16 (y_is_half) or fp32 [M][out_features].
+ * The outliers and dense rows are folded into the dequantized weight tiles, so there is no limit on topX or on the outliers per
+ * row; CSR column indices need not be ascending (ascending rows are cheaper).  Every weight is split into two fp16 parts of a
+ * per-column power-of-two scale and both are multiplied in (exact products, fp32 accumulation): the codebook is always used as
+ * stored, sqllm_set_lut_mode does not apply.  Every output is written once by one CTA in a fixed order: bit-reproducible.
+ * Requirements (checked, SQLLM_EINVAL otherwise): in_features % 32 == 0, batch >= 1, x and y 16-byte aligned, qweight,
+ * lookup_table and bias 4-byte aligned.  No workspace, no allocation, no host synchronisation: CUDA-graph capturable. */
+int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
+                        void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

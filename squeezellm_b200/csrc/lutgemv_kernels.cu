@@ -4,7 +4,8 @@
 //   VecQuant{3,4}MatMulKernelNUQPerChannel[Batched]  (:741-1038)   LUT GEMV
 //   SPMV_ATOMIC[_BATCHED]                            (:1040-1089)  CSR outliers
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
-// and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.
+// and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
+// LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused).
 //
 // Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every layer of 64 or more output columns in the
 // accumulate and the default (fast) fused mode.  lutgemv_kernel below ("v1") runs the deterministic fused mode
@@ -1056,6 +1057,7 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemv_v2.cuh"
 #include "lutgemv_seq.cuh"
 #include "lutgemm_batched.cuh"
+#include "lutgemm_tc.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
 // tables to their own size - up to 64 KB - so the host needs the real address, not a worst case; the kernel re-checks it)
@@ -1813,6 +1815,9 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     return SQLLM_OK;
 }
 
+// ---- tensor-core LUT-GEMM (lutgemm_tc.cuh) ------------------------------------------------------------------------------
+bool g_tc_attr[64] = {};
+
 }  // namespace
 
 // =================================================================================================
@@ -1981,6 +1986,48 @@ int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int
     p.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
     p.xw_out_off = xc->out_offset; p.xw_flag_off = xc->flag_offset; p.xw_state_off = xc->state_offset; p.xw_err_off = xc->error_offset;
     return launch<true>(a, pl, p, static_cast<cudaStream_t>(stream));
+}
+
+int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
+    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
+    if (a->out_features <= 0) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
+    if ((a->out_features + tc::BN - 1) / tc::BN > 65535) return fail(SQLLM_EINVAL, "out_features=%d exceeds %d", a->out_features, 65535 * tc::BN);
+    if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x) must be >= 1 (got %d)", a->batch);
+    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
+    if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
+    if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3) || (reinterpret_cast<uintptr_t>(bias) & 3))
+        return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
+    if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
+    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
+    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
+    {
+        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        if (!g_tc_attr[dev]) {
+            if (cudaFuncSetAttribute(tc::lutgemm_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM) != cudaSuccess ||
+                cudaFuncSetAttribute(tc::lutgemm_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM) != cudaSuccess)
+                return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
+            g_tc_attr[dev] = true;
+        }
+    }
+    tc::PT p;
+    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    p.x = static_cast<const __half *>(x); p.y = y; p.y_is_half = y_is_half ? 1 : 0; p.bias = bias;
+    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
+    const bool hyb = a->full_rows && a->topX > 0;
+    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
+    p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
+    const dim3 grid((a->batch + tc::BM - 1) / tc::BM, (a->out_features + tc::BN - 1) / tc::BN);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (a->bits == 4) tc::lutgemm_tc_kernel<4><<<grid, tc::THREADS, tc::SMEM, st>>>(p);
+    else tc::lutgemm_tc_kernel<3><<<grid, tc::THREADS, tc::SMEM, st>>>(p);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_fused launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
 }
 
 int sqllm_unpack_indices(int bits, const int32_t *qweight, int in_features, int out_features, uint8_t *idx, void *stream) {

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `unpack_indices`, `abi_version`, `fused_limits`.
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `unpack_indices`, `abi_version`, `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -168,8 +168,8 @@ torch::Tensor workspace_for(const torch::Tensor &like, size_t bytes) {
     return it->second;
 }
 
-// shared argument checking / descriptor filling of the two fused entry points
-void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
+// shared argument checking / descriptor filling of the fused entry points: everything but the shape of x
+void fill_layer_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
                      const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
                      const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
                      const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
@@ -185,7 +185,6 @@ void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
     a.in_features = (int)(qweight.size(0) / bits * 32);
     a.out_features = (int)qweight.size(1);
     a.batch = 1;
-    TORCH_CHECK(x.numel() == a.in_features, "x has ", x.numel(), " elements, expected in_features=", a.in_features);
     TORCH_CHECK(lookup_table.numel() == (int64_t)a.out_features * (1 << bits), "lookup_table must be [out, 2^bits]");
     a.qweight = qweight.data_ptr<int32_t>();
     a.lookup_table = lookup_table.data_ptr<float>();
@@ -209,6 +208,35 @@ void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
         a.full_row_indices = full_row_indices->data_ptr<int32_t>();
         a.topX = (int)full_rows->size(1);
     }
+}
+
+// ... of the matvec entry points: x holds one input vector
+void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
+                     const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
+                     const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
+                     const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
+                     const c10::optional<torch::Tensor> &full_row_indices) {
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    TORCH_CHECK(x.numel() == a.in_features, "x has ", x.numel(), " elements, expected in_features=", a.in_features);
+}
+
+// y [M, out] fp16 = bias + LUT-GEMM(x) [+ CSR] [+ dense rows] from fp16 x [M, in], on the tensor cores (sqllm_lutgemm_fused):
+// QuantLinearLUT.forward's batched branch (squeezellm/quant.py:314-379) in one launch.
+torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                            c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                            c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                            c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16, "lutgemm_fused: x must be fp16");
+    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemm_fused: x must be [M, in_features=", a.in_features, "]");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemm_fused: x must have 1 to 2^31-1 rows");
+    a.batch = (int)x.size(0);
+    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
+    check_status(sqllm_lutgemm_fused(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemm_fused");
+    return y;
 }
 
 // y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16/fp32 with numel == in; returns [out] in x's dtype
@@ -360,6 +388,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("vecquant4matmul_spmv_hybrid_nuq_perchannel_batched", &hybrid<4, true>, "4-bit LUT matmul + CSR + dense rows, batched");
     // additions
     m.def("lutgemv_fused", &lutgemv_fused, "fused QuantLinearLUT matvec: fp16/fp32 x -> y (bias, CSR, dense rows), one launch",
+          py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
+          py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
+          py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
+    m.def("lutgemm_fused", &lutgemm_fused, "fused QuantLinearLUT matmul on the tensor cores: fp16 x [M, in] -> fp16 y [M, out] (bias, CSR, dense rows), one launch",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());

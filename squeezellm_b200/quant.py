@@ -11,6 +11,9 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
     zeros + x.float() + 1-3 launches + y.to(dtype).  Layers wider or with more dense rows than the fused launch
     takes (`FUSED_LIMITS`, from the extension) run the reference's 12 symbols instead.  Set
     `QuantLinearLUT.use_fused = False` to go through the reference's 12 symbols exactly as quant.py does.
+  * `forward` with fp16 x of at least `TC_MIN_ROWS` rows (prefill, evaluation; reference quant.py:314-379) uses ONE
+    tensor-core launch (`quant_cuda.lutgemm_fused`, outliers and dense rows folded into the weight tiles) instead of
+    zeros + x.float() + 1-3 batched launches + out.to(dtype).
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
     (quant.py:238,282 vs quant_cuda.cpp:257-270), i.e. an AttributeError at the first forward.
@@ -93,6 +96,10 @@ class QuantLinearLUT(nn.Module):
     """Drop-in layer replacement (reference quant.py:28)."""
 
     use_fused = True  # class-wide switch: fused single-launch forward vs the reference's 12-symbol sequence
+    # fp16 inputs of at least this many rows run the tensor-core LUT-GEMM (quant_cuda.lutgemm_fused); fewer rows, fp32 / bf16
+    # inputs and use_fused = False run the batched symbols.  64: where a whole 7B decoder layer gets faster on an H100 (DESIGN.md
+    # section 3.6: 32 rows 1.08 vs 0.78 ms, 64 rows 1.09 vs 1.48 ms).
+    TC_MIN_ROWS = 64
     # codebook precision of the fused path is process-wide: quant_cuda.set_lut_mode("exact" | "fp16")  (include/sqllm_b200.h)
 
     def __init__(self, bits, infeatures, outfeatures, bias, include_sparse=False, numvals=0, topX=0,
@@ -194,6 +201,11 @@ class QuantLinearLUT(nn.Module):
             return y.to(dtype).reshape(outshape)
         out_shape = x.shape[:-1] + (self.outfeatures,)
         x = x.reshape(-1, x.shape[-1])
+        if QuantLinearLUT.use_fused and x.dtype == torch.float16 and x.shape[0] >= QuantLinearLUT.TC_MIN_ROWS:
+            rows, cols, vals, fr, fri = self._sparse_args()
+            out = quant_cuda.lutgemm_fused(x.contiguous(), self.qweight, self.lookup_table, self.bits,
+                                           None, rows, cols, vals, fr, fri).reshape(out_shape)
+            return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
         out = torch.zeros((x.shape[0], self.outfeatures), device=dev, dtype=torch.float32)
         dtype = x.dtype
         x = x.float().contiguous()
