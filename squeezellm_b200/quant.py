@@ -92,6 +92,13 @@ def pack_indices(idx_kn, bits):
     return q.view(np.int32)
 
 
+def _aligned(x):
+    """x as one contiguous block that starts on a 16-byte boundary: the kernels read x with 16-byte loads.  A contiguous view
+    whose storage offset is not a multiple of 8 fp16 / 4 fp32 elements (a slice of a larger buffer) is copied to fresh storage."""
+    x = x.contiguous()
+    return x.clone() if x.data_ptr() % 16 else x
+
+
 class QuantLinearLUT(nn.Module):
     """Drop-in layer replacement (reference quant.py:28)."""
 
@@ -190,25 +197,25 @@ class QuantLinearLUT(nn.Module):
             outshape[-1] = self.outfeatures
             rows, cols, vals, fr, fri = self._sparse_args()
             if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32) and self._fused_fits(fr):
-                y = quant_cuda.lutgemv_fused(x.contiguous(), self.qweight, self.lookup_table, self.bits,
+                y = quant_cuda.lutgemv_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                              self.bias, rows, cols, vals, fr, fri)
                 return y.reshape(outshape)
             # reference sequence (quant.py:213-312)
             y = self.bias.clone() if self.bias is not None else torch.zeros((self.outfeatures), device=dev, dtype=torch.float32)
             dtype = x.dtype
-            x = x.float().contiguous()
+            x = _aligned(x.float())
             self._dispatch(x, y, batched=False)
             return y.to(dtype).reshape(outshape)
         out_shape = x.shape[:-1] + (self.outfeatures,)
         x = x.reshape(-1, x.shape[-1])
         if QuantLinearLUT.use_fused and x.dtype == torch.float16 and x.shape[0] >= QuantLinearLUT.TC_MIN_ROWS:
             rows, cols, vals, fr, fri = self._sparse_args()
-            out = quant_cuda.lutgemm_fused(x.contiguous(), self.qweight, self.lookup_table, self.bits,
+            out = quant_cuda.lutgemm_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                            None, rows, cols, vals, fr, fri).reshape(out_shape)
             return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
         out = torch.zeros((x.shape[0], self.outfeatures), device=dev, dtype=torch.float32)
         dtype = x.dtype
-        x = x.float().contiguous()
+        x = _aligned(x.float())
         self._dispatch(x, out, batched=True)
         out = out.to(dtype).reshape(out_shape)
         return out + self.bias if self.bias is not None else out

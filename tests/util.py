@@ -33,6 +33,82 @@ def rel_err(a, b, b_absmax=None):
     return float((np.abs(a - b) / den).max())
 
 
+"""Per-element, condition-aware error bound.  rel_err's floor is 1 % of the largest output of the whole array, so an output far
+below the largest (a token whose activations are 1e-3 of another's) can be off by percents and still pass.  This bound scales with
+each element's own condition instead:
+
+    |got_i - want_i| <= r * |rounded_i| + eta + (1 + r) * e * S_i,      S_i = sum_k |x_k| |w_kc| + |bias_c|
+
+  * S: the oracle on abs_layer(L) and |x| (|lut + csr + dense| <= |lut| + |csr| + |dense|), with |bias| as one more term.
+  * r, eta: the final rounding to the output dtype (OUT_ROUNDING: relative unit roundoff and half the smallest subnormal);
+    `rounded` is the value that was rounded: the whole output when the bias is inside the sum, the sum without the bias where the
+    module rounds first and adds the bias afterwards.  The (1 + r) factor covers rounding a value that already carries e * S.
+  * e = E_ACC = 2^-20 = 16 u (u = 2^-24, fp32): every route forms each output from fp32 products that are exact (tensor cores) or
+    rounded once (CUDA cores: <= u * S together) and fp32 sums (DESIGN.md 3.1-3.6).  The tensor-core path also rounds the outlier
+    fold (lut + csr + dense, <= 2 u of each |w| with distinct dense rows) and keeps 22 bits of each folded weight in its hi/lo
+    split (<= 4 u of each |w|).  Additions: sums of terms of either sign keep their partial sums near sqrt(j) terms, so their
+    rounding errors total about u * S, not the worst case of (number of additions) * u * S (Higham & Mary, SIAM J. Sci. Comput.
+    41(5), 2019).  That is at most about 7 u; 16 u leaves a factor of two.
+"""
+U32 = 2.0 ** -24
+E_ACC = 2.0 ** -20
+OUT_ROUNDING = {"float32": (0.0, 0.0), "float16": (2.0 ** -11, 2.0 ** -25), "bfloat16": (2.0 ** -8, 2.0 ** -134)}
+
+
+def abs_layer(L):
+    """Copy of the layer dict with lookup_table, vals and full_rows replaced by their absolute values."""
+    A = dict(L)
+    for k in ("lookup_table", "vals", "full_rows"):
+        if A.get(k) is not None:
+            A[k] = np.abs(A[k])
+    return A
+
+
+def abs_sum(L, x, bias=None):
+    """S [rows, N] = sum_k |x_k| |w_kc| (+ |bias_c|) in fp64: the condition of every output."""
+    return orc.forward_f64(abs_layer(L), np.abs(x), mul_init=None if bias is None else np.abs(bias)[None, :])
+
+
+def bound_ratio(got, want, S, rounded=None, r=0.0, e=E_ACC, eta=0.0):
+    """max_i |got_i - want_i| / (r |rounded_i| + eta + (1 + r) e S_i); <= 1 passes.  rounded defaults to want.  An element whose
+    allowance is 0 (an all-zero row without bias) must be exact: any difference there gives inf, a NaN gives NaN."""
+    got = np.asarray(got, dtype=np.float64)
+    want = np.asarray(want, dtype=np.float64)
+    assert got.shape == want.shape == np.shape(S), (got.shape, want.shape, np.shape(S))
+    rounded = want if rounded is None else np.asarray(rounded, dtype=np.float64)
+    err = np.abs(got - want)
+    den = r * np.abs(rounded) + eta + (1.0 + r) * e * np.asarray(S, dtype=np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        q = np.where(err == 0, 0.0, err / den)
+    return float(q.max()) if q.size else 0.0
+
+
+MASSIVE_SCALE = 100.0
+
+
+def massive_channels(K):
+    """The three fixed input channels that carry "massive activations" in make_activations."""
+    return np.array([5, K // 2 + 3, K - 7])
+
+
+def make_activations(K, M, seed=0):
+    """Prefill-like fp16-exact activations [M, K] (fp32 array): rows of N(0, 1), each scaled by 10^U(-3, 2), with row 0 scaled by
+    exactly 1e-3 and row 1 by 1e2; the massive_channels x100 in every row; row 2 all zero and row 3 a single non-zero entry.  A
+    1e-3 row holds fp16 subnormals (|x| < 2^-14) in about 5 % of its entries."""
+    rng = np.random.default_rng(seed + 4242)
+    scale = 10.0 ** rng.uniform(-3.0, 2.0, size=M)
+    scale[:2] = (1e-3, 1e2)[:M]
+    x = rng.standard_normal((M, K)) * scale[:, None]
+    x[:, massive_channels(K)] *= MASSIVE_SCALE
+    x = np.clip(x, -60000.0, 60000.0).astype(np.float16).astype(np.float32)
+    if M > 2:
+        x[2] = 0.0
+    if M > 3:
+        x[3] = 0.0
+        x[3, K // 3] = 1.5
+    return x
+
+
 def sample_idx(n, cap=2048):
     """The output positions kept in golden data of large outputs: all of them up to `cap`, else `cap` positions spread over
     the vector by a prime stride (7919 divides none of the sizes used)."""
