@@ -53,7 +53,7 @@ extern "C" {
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
 
-/* Number of SMs x resident CTAs the persistent kernels will use on the current device
+/* Number of SMs of the current device, the grid of the one-GEMV and sequence kernels
  * (informational; also used by bench.py to report the grid). */
 int sqllm_device_sm_count(void);
 

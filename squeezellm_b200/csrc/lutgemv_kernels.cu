@@ -1079,16 +1079,84 @@ int fail(int code, const char *fmt, ...) {
     return code;
 }
 
-struct DevInfo {
-    int sm = 0;
-    bool attr_set = false;
-};
-// Process-wide state (mode switches, lazily read environment knobs, per-device attributes) is guarded by g_state_mu: the entry
+// Process-wide state (mode switches, lazily read environment knobs, per-device state) is guarded by g_state_mu: the entry
 // points may be called from several host threads.  Switching a mode (sqllm_set_deterministic / sqllm_set_lut_mode) while other
 // threads are launching is allowed but takes effect per call; do not switch while a CUDA graph that should keep the old mode is
 // being captured.
 std::recursive_mutex g_state_mu;
+
+struct DevInfo {
+    int sm = 0;
+    unsigned smem_raw = 0;               // shared-window address of dynamic shared memory; 0 until smem_window probes it
+    std::vector<const void *> smem_set;  // kernels whose dynamic shared-memory limit set_max_smem has raised
+};
 DevInfo g_dev[64];
+
+// The current device and its SM count, read once.  Caller holds g_state_mu.
+int cur_dev(int &dev) {
+    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
+    if (dev < 0 || dev >= 64) return fail(SQLLM_EINVAL, "device ordinal %d out of range", dev);
+    DevInfo &d = g_dev[dev];
+    if (d.sm == 0 && (cudaDeviceGetAttribute(&d.sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm <= 0)) {
+        d.sm = 0;
+        return fail(SQLLM_ECUDA, "cannot query SM count");
+    }
+    return SQLLM_OK;
+}
+
+// Raises the dynamic shared-memory limit of kernel `fn` to `bytes`, once per device.  Caller holds g_state_mu.
+template <typename F>
+int set_max_smem(DevInfo &d, F *fn, int bytes) {
+    const void *f = (const void *)fn;
+    if (std::find(d.smem_set.begin(), d.smem_set.end(), f) != d.smem_set.end()) return SQLLM_OK;
+    if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
+        return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
+    d.smem_set.push_back(f);
+    return SQLLM_OK;
+}
+
+// d.smem_raw from smem_base_probe, once per device.  The probe is synchronous and refused during stream capture: only v2 and sequence
+// plans ask for it, and the first of them on a device must come before any capture - any warm-up does.  Caller holds g_state_mu.
+int smem_window(DevInfo &d) {
+    if (d.smem_raw) return SQLLM_OK;
+    unsigned *d_out = nullptr, h_out = 0;
+    cudaError_t pe = cudaMalloc(&d_out, sizeof(unsigned));
+    if (pe == cudaSuccess) {
+        smem_base_probe<<<1, 1, 1024>>>(d_out);
+        pe = cudaMemcpy(&h_out, d_out, sizeof(unsigned), cudaMemcpyDeviceToHost);
+        cudaFree(d_out);
+    }
+    if (pe != cudaSuccess || h_out == 0) {
+        cudaGetLastError();
+        return fail(SQLLM_ECUDA, "shared-memory probe failed (first call inside a stream capture? run one call before capturing): %s", cudaGetErrorString(pe));
+    }
+    d.smem_raw = h_out;
+    return SQLLM_OK;
+}
+
+// cudaLaunchKernelEx with one attribute: programmatic stream serialisation for the GEMV kernels (their prologue and weight stream
+// overlap the previous kernel), cooperative for the sequence kernel (every CTA waits on every other one: they must all be resident).
+template <typename... P, typename... A>
+cudaError_t launch_ex(void (*fn)(P...), int grid, int block, int smem, cudaStream_t st, bool cooperative, const A &...args) {
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr;
+    if (cooperative) {
+        attr.id = cudaLaunchAttributeCooperative;
+        attr.val.cooperative = 1;
+    } else {
+        attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr.val.programmaticStreamSerializationAllowed = 1;
+    }
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, fn, args...);
+}
+
 int g_det = -1;
 int det_mode() {
     std::lock_guard<std::recursive_mutex> lk(g_state_mu);
@@ -1156,22 +1224,11 @@ int make_plan(int bits, int K, int N, int topX, bool has_csr_in, bool fused, Pla
     // staging: CSR cols/vals chunks (8 KB); the deterministic fused mode also stages the dense-row partials there (8 KB more)
     pl.has_stage = has_csr ? CSR_CH * 8 + ((fused && det_mode() == 1) ? CSR_CH * 8 : 0) : 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
-    if (dev < 0 || dev >= 64) return fail(SQLLM_EINVAL, "device ordinal %d out of range", dev);
+    int rc = cur_dev(dev);
+    if (rc) return rc;
     DevInfo &d = g_dev[dev];
-    if (d.sm == 0) {
-        if (cudaDeviceGetAttribute(&d.sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm <= 0)
-            return fail(SQLLM_ECUDA, "cannot query SM count");
-    }
-    if (!d.attr_set) {
-        const int mx = 227 * 1024;
-        cudaFuncSetAttribute(lutgemv_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-        cudaFuncSetAttribute(lutgemv_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-        cudaFuncSetAttribute(lutgemv_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-        cudaFuncSetAttribute(lutgemv_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-        if (cudaGetLastError() != cudaSuccess) return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed");
-        d.attr_set = true;
-    }
+    for (auto fn : {lutgemv_kernel<4, false>, lutgemv_kernel<4, true>, lutgemv_kernel<3, false>, lutgemv_kernel<3, true>})
+        if ((rc = set_max_smem(d, fn, 227 * 1024))) return rc;
     const int XU = bits == 4 ? 8 : 32;
     pl.R = bits == 4 ? K / 8 : K / 32;
     pl.strips = (N + STRIP - 1) / STRIP;
@@ -1274,24 +1331,6 @@ int check_common(const sqllm_lutgemv_args *a) {
     return SQLLM_OK;
 }
 
-template <int BITS, bool FUSED>
-cudaError_t launch_kernel(const Plan &pl, const Params &p, cudaStream_t st) {
-    std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    g_last_grid = pl.G;
-    cfg.gridDim = dim3(pl.G);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, lutgemv_kernel<BITS, FUSED>, p);
-}
-
 template <bool FUSED>
 int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t st) {
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
@@ -1316,7 +1355,8 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
     p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
     p.trace = g_trace;
     if (g_trace) g_trace += g_trace_stride;
-    const cudaError_t e = a->bits == 4 ? launch_kernel<4, FUSED>(pl, p, st) : launch_kernel<3, FUSED>(pl, p, st);
+    g_last_grid = pl.G;
+    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4, FUSED> : lutgemv_kernel<3, FUSED>, pl.G, THREADS, pl.smem, st, false, p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1325,7 +1365,6 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
 // =================================================================================================
 // v2 (lutgemv_v2.cuh): plan + launch.  One CTA per SM; all process-wide state behind one mutex / atomics.
 // =================================================================================================
-bool g_v2_attr[64] = {};
 int g_lut_mode = -1;     // 0: exact fp32 table, 1: fp16 pair table when x is fp16 (SQLLM_LUT_MODE=fp16 / sqllm_set_lut_mode)
 
 int lut_mode() {
@@ -1353,136 +1392,89 @@ K2Info k2_lookup(int bits, int variant, bool fused) {
 #undef K2E
 }
 
-struct Plan2 {
-    int R, strips, T, chunk, G, nstage, smem, hc, hrows, csr_rpc;
-    unsigned smem_raw;
-};
-unsigned g_smem_raw[64] = {};
-
-int make_plan2(int bits, int K, int N, int topX, int variant, bool fused, Plan2 &pl, K2Info &ki) {
-    int dev = 0, sm = 0;
-    unsigned smem_raw = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
-    if (dev < 0 || dev >= 64) return fail(SQLLM_EINVAL, "device ordinal %d out of range", dev);
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        DevInfo &d = g_dev[dev];
-        if (d.sm == 0 && (cudaDeviceGetAttribute(&d.sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm <= 0)) {
-            d.sm = 0;
-            return fail(SQLLM_ECUDA, "cannot query SM count");
-        }
-        sm = d.sm;
-        if (!g_v2_attr[dev]) {
-            for (int b = 3; b <= 4; ++b)
-                for (int v = 0; v < 3; ++v)
-                    for (int f = 0; f < 2; ++f)
-                        if (cudaFuncSetAttribute(k2_lookup(b, v, f != 0).fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-                            return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
-            // one-time probe (synchronous; refused during stream capture, so the first call must come before capture - any warm-up does)
-            unsigned *d_out = nullptr, h_out = 0;
-            cudaError_t pe = cudaMalloc(&d_out, sizeof(unsigned));
-            if (pe == cudaSuccess) {
-                smem_base_probe<<<1, 1, 1024>>>(d_out);
-                pe = cudaMemcpy(&h_out, d_out, sizeof(unsigned), cudaMemcpyDeviceToHost);
-                cudaFree(d_out);
-            }
-            if (pe != cudaSuccess || h_out == 0) {
-                cudaGetLastError();
-                return fail(SQLLM_ECUDA, "shared-memory probe failed (first call inside a stream capture? run one call before capturing): %s", cudaGetErrorString(pe));
-            }
-            g_smem_raw[dev] = h_out;
-            g_v2_attr[dev] = true;
-        }
-        smem_raw = g_smem_raw[dev];
-    }
-    ki = k2_lookup(bits, variant, fused);
-    pl.R = bits == 4 ? K / 8 : K / 32;
-    pl.strips = (N + STRIP - 1) / STRIP;
-    const long long T = (long long)pl.strips * pl.R;
+// Stream-K plan of one layer for the v2 and sequence kernels, on a grid of at most `sm` CTAs, and the layer's buffers: fills the
+// shape and buffer fields of p and returns the grid in G.
+int plan_layer(const sqllm_lutgemv_args &a, int sm, v2::P2 &p, int &G) {
+    const bool hyb = a.full_rows && a.topX > 0;
+    const int K = a.in_features, N = a.out_features;
+    p.qw = reinterpret_cast<const uint32_t *>(a.qweight);
+    p.lut = a.lookup_table;
+    p.rows = a.rows; p.cols = a.cols; p.vals = a.vals;
+    p.full_rows = hyb ? a.full_rows : nullptr;
+    p.fri = hyb ? a.full_row_indices : nullptr;
+    p.topX = hyb ? a.topX : 0;
+    p.csr_al16 = (a.rows && ((reinterpret_cast<uintptr_t>(a.cols) | reinterpret_cast<uintptr_t>(a.vals)) & 15) == 0) ? 1 : 0;
+    p.K = K; p.N = N;
+    p.R = a.bits == 4 ? K / 8 : K / 32;
+    p.strips = (N + STRIP - 1) / STRIP;
+    const long long T = (long long)p.strips * p.R;
     if (T > 0x3fffffff) return fail(SQLLM_EINVAL, "problem too large");
-    if (fused && N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the fused accumulator (max %d)", N, MAX_N_FUSED);
-    pl.T = (int)T;
-    int chunk = (int)(2 * ((T + 2LL * sm - 1) / (2LL * sm)));
-    if (chunk < 2) chunk = 2;
-    pl.chunk = chunk;
-    pl.G = (int)((T + chunk - 1) / chunk);
-    if (fused && pl.G > MAX_GRID_V2) return fail(SQLLM_EINVAL, "grid of %d CTAs exceeds the mailbox area (%d)", pl.G, MAX_GRID_V2);
-    // shared memory, exactly as lutgemv2_kernel carves it: [fixed][x][ring stages ...][table 0][table 1][... ring stages]
-    const unsigned raw = smem_raw;
-    const unsigned base = (raw + 127u) & ~127u;
-    const unsigned lo_base = base + v2::OFF_X + (unsigned)((K * (variant == 0 ? 4 : 2) + 127) & ~127);
-    const unsigned tab0 = (lo_base + (unsigned)ki.tab - 1u) & ~((unsigned)ki.tab - 1u);
-    const long long limit = (long long)raw + 227 * 1024;
-    const long long hi_room = limit - ((long long)tab0 + 2LL * ki.tab);
-    if (hi_room < 0) return fail(SQLLM_EINVAL, "in_features=%d does not fit the shared-memory carve-up of this table mode", K);
-    const int lo_cap = (int)((tab0 - lo_base) / (unsigned)ki.stage), hi_cap = (int)(hi_room / ki.stage);
-    int n = (chunk + v2::SU2 - 1) / v2::SU2 + 1;
-    if (n > v2::MAXD) n = v2::MAXD;
-    if (n > lo_cap + hi_cap) n = lo_cap + hi_cap;
-    if (n < 2) return fail(SQLLM_EINVAL, "in_features=%d leaves no room for a weight ring in shared memory", K);
-    const int n_lo = n < lo_cap ? n : lo_cap;
-    pl.nstage = n;
-    pl.smem = (int)((long long)tab0 + 2LL * ki.tab + (long long)(n - n_lo) * ki.stage - raw);
-    pl.smem_raw = raw;
-    pl.csr_rpc = (N + pl.G - 1) / pl.G;
-    pl.hc = pl.hrows = 0;
-    if (topX > 0) {
-        pl.hrows = (K + pl.G - 1) / pl.G;
-        pl.hc = (K + pl.hrows - 1) / pl.hrows;
+    p.T = (int)T;
+    p.chunk = std::max(2, (int)(2 * ((T + 2LL * sm - 1) / (2LL * sm))));
+    G = (int)((T + p.chunk - 1) / p.chunk);
+    p.csr_rpc = (N + G - 1) / G;
+    p.hc = p.hrows = 0;
+    if (hyb) {
+        p.hrows = (K + G - 1) / G;
+        p.hc = (K + p.hrows - 1) / p.hrows;
     }
     return SQLLM_OK;
 }
 
+// The two tensor maps over the packed matrix: 64 columns x (32 units | 2 units) boxes.
+int tensor_maps(const sqllm_lutgemv_args &a, CUtensorMap &big, CUtensorMap &small) {
+    const int rows_per_unit = a.bits == 4 ? 1 : 3, qrows = a.in_features / 32 * a.bits;
+    // (a matrix shorter than one full stage never issues the big box; its map is clamped so that the encoder accepts it)
+    const int rc = get_tensor_map(a.qweight, qrows, a.out_features, qrows < v2::SU2 * rows_per_unit ? 2 * rows_per_unit : v2::SU2 * rows_per_unit, big);
+    return rc ? rc : get_tensor_map(a.qweight, qrows, a.out_features, 2 * rows_per_unit, small);
+}
+
 int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cudaStream_t st) {
-    const bool hyb = a->full_rows && a->topX > 0;
-    Plan2 pl;
-    K2Info ki;
-    const int rc = make_plan2(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, variant, fused, pl, ki);
+    const K2Info ki = k2_lookup(a->bits, variant, fused);
+    int dev = 0, sm = 0;
+    unsigned raw = 0;
+    {
+        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        int rc = cur_dev(dev);
+        if (rc) return rc;
+        DevInfo &d = g_dev[dev];
+        for (int b = 3; b <= 4; ++b)
+            for (int v = 0; v < 3; ++v)
+                for (int f = 0; f < 2; ++f)
+                    if ((rc = set_max_smem(d, k2_lookup(b, v, f != 0).fn, 227 * 1024))) return rc;
+        if ((rc = smem_window(d))) return rc;
+        sm = d.sm;
+        raw = d.smem_raw;
+    }
+    int G = 0;
+    int rc = plan_layer(*a, sm, p, G);
     if (rc) return rc;
-    p.qw = reinterpret_cast<const uint32_t *>(a->qweight);
-    p.lut = a->lookup_table;
-    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-    p.full_rows = hyb ? a->full_rows : nullptr;
-    p.fri = hyb ? a->full_row_indices : nullptr;
-    p.topX = hyb ? a->topX : 0;
-    p.K = a->in_features; p.N = a->out_features;
-    p.R = pl.R; p.T = pl.T; p.chunk = pl.chunk; p.nstage = pl.nstage; p.smem_raw = pl.smem_raw;
-    p.hc = hyb ? pl.hc : 0; p.hrows = pl.hrows;
-    p.csr_rpc = pl.csr_rpc;
-    p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
-    p.strips = pl.strips;
+    if (fused && p.N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the fused accumulator (max %d)", p.N, MAX_N_FUSED);
+    if (fused && G > MAX_GRID_V2) return fail(SQLLM_EINVAL, "grid of %d CTAs exceeds the mailbox area (%d)", G, MAX_GRID_V2);
+    const unsigned base = (raw + 127u) & ~127u;
+    const unsigned xbytes = (unsigned)((p.K * (variant == 0 ? 4 : 2) + 127) & ~127);  // this layer's x, in its own dtype
+    // one GEMV: the ring needs no more stages than the CTA's chunk fills
+    const int n = v2::Carve(base, xbytes, 0u, ki.tab, 2, ki.stage, 0).depth(raw, 227 * 1024, ki.stage, (p.chunk + v2::SU2 - 1) / v2::SU2 + 1);
+    if (n < 0) return fail(SQLLM_EINVAL, "in_features=%d does not fit the shared-memory carve-up of this table mode", p.K);
+    if (n < 2) return fail(SQLLM_EINVAL, "in_features=%d leaves no room for a weight ring in shared memory", p.K);
+    const int smem = (int)(v2::Carve(base, xbytes, 0u, ki.tab, 2, ki.stage, n).end - raw);
+    p.nstage = n;
+    p.smem_raw = raw;
     p.nown_ctas = 0;
     if (p.xw_world)
-        for (int b = 0; b < pl.G; ++b) {  // CTAs in whose range at least one strip starts
-            const long long c0 = (long long)b * pl.chunk, c1 = std::min<long long>(pl.T, c0 + pl.chunk);
-            if ((c0 + pl.R - 1) / pl.R < (c1 + pl.R - 1) / pl.R) ++p.nown_ctas;
+        for (int b = 0; b < G; ++b) {  // CTAs in whose range at least one strip starts
+            const long long c0 = (long long)b * p.chunk, c1 = std::min<long long>(p.T, c0 + p.chunk);
+            if ((c0 + p.R - 1) / p.R < (c1 + p.R - 1) / p.R) ++p.nown_ctas;
         }
     {
         std::lock_guard<std::recursive_mutex> lk(g_state_mu);
         p.trace = g_trace;
         if (g_trace) g_trace += g_trace_stride;
-        g_last_grid = pl.G;
+        g_last_grid = G;
     }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(pl.G);
-    cfg.blockDim = dim3(v2::THREADS2);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    // two tensor maps over the packed matrix: 64 columns x (32 units | 2 units) boxes
-    const int rows_per_unit = a->bits == 4 ? 1 : 3, qrows = a->in_features / 32 * a->bits;
     CUtensorMap tm_big, tm_small;
-    // (a matrix shorter than one full stage never issues the big box; its map is clamped so that the encoder accepts it)
-    int trc = get_tensor_map(a->qweight, qrows, a->out_features, qrows < v2::SU2 * rows_per_unit ? 2 * rows_per_unit : v2::SU2 * rows_per_unit, tm_big);
-    if (trc) return trc;
-    trc = get_tensor_map(a->qweight, qrows, a->out_features, 2 * rows_per_unit, tm_small);
-    if (trc) return trc;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, ki.fn, p, tm_big, tm_small);
+    if ((rc = tensor_maps(*a, tm_big, tm_small))) return rc;
+    const cudaError_t e = launch_ex(ki.fn, G, v2::THREADS2, smem, st, false, p, tm_big, tm_small);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1492,7 +1484,7 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
 typedef void (*KSeq)(const seq::SeqCfg);
 struct KSeqInfo { KSeq fn; int tab, stage, ntb; };
 KSeqInfo kseq_lookup(int bits, int mode, bool multi) {
-#define KSE(B, M, X) KSeqInfo{seq::lutgemv_seq_kernel<B, M, X>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE, v2::C2<B, M>::TAB <= 16384 ? 4 : 2}
+#define KSE(B, M, X) KSeqInfo{seq::lutgemv_seq_kernel<B, M, X>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE, v2::C2<B, M>::NTB}
     if (bits == 4) {
         if (mode == 0) return multi ? KSE(4, 0, true) : KSE(4, 0, false);
         return multi ? KSE(4, 1, true) : KSE(4, 1, false);
@@ -1574,33 +1566,25 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         if (it < 0 || it >= n_items || !opt->export_dst[e] || (reinterpret_cast<uintptr_t>(opt->export_dst[e]) & 7))
             return fail(SQLLM_EINVAL, "sequence: export %d: bad item %d or destination (8-byte aligned fp16 vector)", e, it);
     }
-    // device attributes, shared-memory window, kernel attribute (make_plan2 does the one-time probe)
-    Plan2 probe;
-    K2Info ki2;
-    int rc = make_plan2(bits, items[0].a.in_features, items[0].a.out_features, 0, mode ? 2 : 1, true, probe, ki2);
-    if (rc) return rc;
     const KSeqInfo ki = kseq_lookup(bits, mode, world > 1);
     int dev = 0, sm = 0;
-    cudaGetDevice(&dev);
+    unsigned raw = 0;
     {
         std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        int rc = cur_dev(dev);
+        if (!rc) rc = set_max_smem(g_dev[dev], ki.fn, 227 * 1024);
+        if (!rc) rc = smem_window(g_dev[dev]);
+        if (rc) return rc;
         sm = g_dev[dev].sm;
+        raw = g_dev[dev].smem_raw;
     }
-    if (cudaFuncSetAttribute(ki.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-        return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
-    // shared memory, exactly as lutgemv_seq_kernel carves it: [fixed][x][strip sums][ring stages ...][tables][... ring stages]
-    const unsigned raw = probe.smem_raw, base = (raw + 127u) & ~127u;
-    const int xbytes = (kmax * 2 + 127) & ~127;
-    const unsigned lo_base = base + v2::OFF_X + (unsigned)xbytes + (unsigned)ki.ntb * STRIP * 4;
-    const unsigned tab0 = (lo_base + (unsigned)ki.tab - 1u) & ~((unsigned)ki.tab - 1u);
-    const long long limit = (long long)raw + 227 * 1024;
-    const long long hi_room = limit - ((long long)tab0 + (long long)ki.ntb * ki.tab);
-    if (hi_room < 0) return fail(SQLLM_EINVAL, "sequence: in_features=%d does not fit the shared-memory carve-up of this table mode", kmax);
-    const int lo_cap = (int)((tab0 - lo_base) / (unsigned)ki.stage), hi_cap = (int)(hi_room / ki.stage);
-    int nst = std::min(v2::MAXD, lo_cap + hi_cap);
+    const unsigned base = (raw + 127u) & ~127u;
+    const int xbytes = (kmax * 2 + 127) & ~127;  // every item's x is staged as fp16 in one buffer, and ntb strip-sum rows follow it
+    // no cap from the chunk: the weight stream runs on across items
+    const int nst = v2::Carve(base, xbytes, ki.ntb * STRIP * 4, ki.tab, ki.ntb, ki.stage, 0).depth(raw, 227 * 1024, ki.stage, v2::MAXD);
+    if (nst < 0) return fail(SQLLM_EINVAL, "sequence: in_features=%d does not fit the shared-memory carve-up of this table mode", kmax);
     if (nst < 2) return fail(SQLLM_EINVAL, "sequence: in_features=%d leaves no room for a weight ring in shared memory", kmax);
-    const int n_lo = std::min(nst, lo_cap);
-    const int smem = (int)((long long)tab0 + (long long)ki.ntb * ki.tab + (long long)(nst - n_lo) * ki.stage - raw);
+    const int smem = (int)(v2::Carve(base, xbytes, ki.ntb * STRIP * 4, ki.tab, ki.ntb, ki.stage, nst).end - raw);
 
     sqllm_sequence *s = new sqllm_sequence();
     s->dev = dev; s->n = n_items; s->bits = bits; s->mode = mode; s->world = world; s->rank = rank; s->grid = sm; s->smem = smem; s->fn = ki.fn;
@@ -1644,34 +1628,12 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         seq::SeqDesc &d = descs[i];
         memset(&d, 0, sizeof(d));
         v2::P2 &p = d.p;
-        const bool hyb = a.full_rows && a.topX > 0;
-        const int K = a.in_features, N = a.out_features;
-        p.qw = reinterpret_cast<const uint32_t *>(a.qweight);
-        p.lut = a.lookup_table;
-        p.rows = a.rows; p.cols = a.cols; p.vals = a.vals;
-        p.full_rows = hyb ? a.full_rows : nullptr;
-        p.fri = hyb ? a.full_row_indices : nullptr;
-        p.topX = hyb ? a.topX : 0;
-        p.K = K; p.N = N;
-        p.R = bits == 4 ? K / 8 : K / 32;
-        p.strips = (N + STRIP - 1) / STRIP;
-        const long long T = (long long)p.strips * p.R;
-        if (T > 0x3fffffff) return seq_fail_free(s, fail(SQLLM_EINVAL, "sequence: item %d too large", i));
-        p.T = (int)T;
-        int chunk = (int)(2 * ((T + 2LL * sm - 1) / (2LL * sm)));
-        if (chunk < 2) chunk = 2;
-        p.chunk = chunk;
-        const int G = (int)((T + chunk - 1) / chunk);
+        int G = 0;
+        int rc = plan_layer(a, sm, p, G);
+        if (rc) return seq_fail_free(s, rc);
         if (G > MAX_GRID_V2) return seq_fail_free(s, fail(SQLLM_EINVAL, "sequence: grid of %d CTAs exceeds the mailbox area", G));
-        p.nstage = nst; p.smem_raw = raw;
-        p.csr_rpc = (N + G - 1) / G;
         if (a.rows && p.csr_rpc > v2::SP_ROWS) return seq_fail_free(s, fail(SQLLM_EINVAL, "sequence: item %d: %d outlier rows per CTA exceed %d", i, p.csr_rpc, v2::SP_ROWS));
-        p.hc = p.hrows = 0;
-        if (hyb) {
-            p.hrows = (K + G - 1) / G;
-            p.hc = (K + p.hrows - 1) / p.hrows;
-        }
-        p.csr_al16 = (a.rows && ((reinterpret_cast<uintptr_t>(a.cols) | reinterpret_cast<uintptr_t>(a.vals)) & 15) == 0) ? 1 : 0;
+        p.nstage = nst; p.smem_raw = raw;
         p.y_is_half = 1;
         p.bias = it.bias;
         p.out = it.y;
@@ -1684,14 +1646,11 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         p.ws_dbox = reinterpret_cast<unsigned long long *>(ws + dbox_off[i]);
         p.xw_world = world > 1 ? world : 0; p.xw_rank = rank;
         p.xw_members = it.members > 0 ? it.members : 1;
-        p.xw_nfull = it.out_features_full > 0 ? it.out_features_full : N / p.xw_members;
+        p.xw_nfull = it.out_features_full > 0 ? it.out_features_full : p.N / p.xw_members;
         p.trace = opt->trace ? reinterpret_cast<unsigned long long *>(opt->trace) + (size_t)i * 1024 * 32 : nullptr;
         d.x_tag = it.x_from < 0 ? nullptr : reinterpret_cast<const uint32_t *>(static_cast<unsigned char *>(s->d_arena) + yoff[it.x_from]) + it.x_offset;
         d.y_off = yoff[i];
-        const int rows_per_unit = bits == 4 ? 1 : 3, qrows = K / 32 * bits;
-        rc = get_tensor_map(a.qweight, qrows, N, qrows < v2::SU2 * rows_per_unit ? 2 * rows_per_unit : v2::SU2 * rows_per_unit, d.tm_big);
-        if (!rc) rc = get_tensor_map(a.qweight, qrows, N, 2 * rows_per_unit, d.tm_small);
-        if (rc) return seq_fail_free(s, rc);
+        if ((rc = tensor_maps(a, d.tm_big, d.tm_small))) return seq_fail_free(s, rc);
     }
     std::vector<seq::SeqExport> ex(std::max(1, opt->n_export));
     for (int e = 0; e < opt->n_export; ++e) {
@@ -1725,18 +1684,7 @@ extern "C" int sqllm_sequence_run(sqllm_sequence *s, void *stream) {
     if (!s) return fail(SQLLM_EINVAL, "sequence: null handle");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     seq::seq_bump_epoch<<<1, 1, 0, st>>>(reinterpret_cast<unsigned *>(s->d_ws));
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(s->grid);
-    cfg.blockDim = dim3(v2::THREADS2);
-    cfg.dynamicSmemBytes = s->smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;  // every CTA waits on every other one: they must all be resident
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, s->fn, s->cfg);
+    const cudaError_t e = launch_ex(s->fn, s->grid, v2::THREADS2, s->smem, st, true, s->cfg);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "sequence launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1769,19 +1717,15 @@ extern "C" void sqllm_sequence_destroy(sqllm_sequence *s) {
 namespace {
 
 // ---- batched symbols: tile kernel + outlier kernels (lutgemm_batched.cuh) ----------------------------------------------
-bool g_batched_attr[64] = {};
 int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     using namespace batched;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
     {
         std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        if (!g_batched_attr[dev]) {
-            if (cudaFuncSetAttribute(lutgemm_batched_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-                cudaFuncSetAttribute(lutgemm_batched_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-                return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
-            g_batched_attr[dev] = true;
-        }
+        int dev = 0;
+        int rc = cur_dev(dev);
+        if (!rc) rc = set_max_smem(g_dev[dev], lutgemm_batched_kernel<4>, 227 * 1024);
+        if (!rc) rc = set_max_smem(g_dev[dev], lutgemm_batched_kernel<3>, 227 * 1024);
+        if (rc) return rc;
     }
     const int K = a->in_features, N = a->out_features, B = a->batch;
     const int XU = a->bits == 4 ? 8 : 32, tab = a->bits == 4 ? CB<4>::TAB : CB<3>::TAB;
@@ -1815,8 +1759,68 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     return SQLLM_OK;
 }
 
-// ---- tensor-core LUT-GEMM (lutgemm_tc.cuh) ------------------------------------------------------------------------------
-bool g_tc_attr[64] = {};
+// ---- fused GEMV: v2, or v1 for the deterministic mode and layers narrower than one strip; with an exchange descriptor the
+// result goes to every rank's arena instead of y ---------------------------------------------------------------------------------
+int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
+                  void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, cudaStream_t st) {
+    int rc = check_common(a);
+    if (rc) return rc;
+    if (!x || (!xc && !y)) return fail(SQLLM_EINVAL, xc ? "x / exchange descriptor must not be null" : "x / y must not be null");
+    if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(bias) & 15))
+        return fail(SQLLM_EINVAL, xc ? "bias must be 16-byte aligned" : "y and bias must be 16-byte aligned");
+    const int det = det_mode();
+    if (xc) {
+        if (det == 1) return fail(SQLLM_EINVAL, "the exchange path needs the default (non-deterministic) fused mode");
+        if (xc->world < 1 || xc->world > 64 || xc->rank < 0 || xc->rank >= xc->world) return fail(SQLLM_EINVAL, "bad world / rank (%d / %d)", xc->world, xc->rank);
+        if (xc->members < 1 || a->out_features % xc->members) return fail(SQLLM_EINVAL, "out_features=%d is not %d equal members", a->out_features, xc->members);
+        const int w = a->out_features / xc->members;
+        if (w % 4) return fail(SQLLM_EINVAL, "shard width %d must be a multiple of 4", w);
+        if (xc->out_features_full < xc->world * w) return fail(SQLLM_EINVAL, "out_features_full=%d < world * shard width = %d", xc->out_features_full, xc->world * w);
+        if (!xc->peer_base) return fail(SQLLM_EINVAL, "peer_base must not be null");
+        if ((xc->out_offset & 15) || (xc->flag_offset & 7) || (xc->state_offset & 7) || (xc->error_offset & 3)) return fail(SQLLM_EINVAL, "misaligned arena offsets");
+        if ((xc->out_features_full * (y_is_half ? 2 : 4)) % 16 || (w * (y_is_half ? 2 : 4)) % 8) return fail(SQLLM_EINVAL, "vector sizes must keep 8/16-byte store alignment");
+    }
+    const bool hyb = a->full_rows && a->topX > 0;
+    if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
+    unsigned char *ws = static_cast<unsigned char *>(workspace);
+    auto set_exchange = [xc](auto &p) {  // the two kernels' parameter blocks name the exchange fields alike
+        if (!xc) return;
+        p.xw_world = xc->world; p.xw_rank = xc->rank; p.xw_members = xc->members; p.xw_nfull = xc->out_features_full;
+        p.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
+        p.xw_out_off = xc->out_offset; p.xw_flag_off = xc->flag_offset; p.xw_state_off = xc->state_offset; p.xw_err_off = xc->error_offset;
+    };
+    if (det == 0 && a->out_features >= STRIP) {
+        if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
+        v2::P2 q;
+        memset(&q, 0, sizeof(q));
+        q.ws_cnt = reinterpret_cast<int *>(ws);
+        q.ws_acc = reinterpret_cast<float *>(ws + WS_ACC_OFF);
+        q.ws_hbox = reinterpret_cast<unsigned long long *>(ws + WS_HBOX_OFF);
+        q.ws_cbox = reinterpret_cast<unsigned long long *>(ws + WS_CBOX_OFF);
+        q.ws_dbox = reinterpret_cast<unsigned long long *>(ws + WS_DBOX_OFF);
+        q.x = x; q.out = y; q.y_is_half = y_is_half; q.bias = bias;
+        set_exchange(q);
+        return launch2(a, x_is_half ? (lut_mode() == 1 ? 2 : 1) : 0, true, q, st);
+    }
+    Plan pl;
+    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, true, pl);
+    if (rc) return rc;
+    if (!workspace || workspace_bytes < pl.ws_bytes)
+        return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", pl.ws_bytes, workspace_bytes);
+    Params p;
+    memset(&p, 0, sizeof(p));
+    p.ws_cnt = reinterpret_cast<int *>(ws + pl.ws_cnt_off);
+    p.ws_hyb_cnt = reinterpret_cast<int *>(ws + pl.ws_hybcnt_off);
+    p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
+    p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
+    p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
+    p.ws_acc = reinterpret_cast<float *>(ws + pl.ws_acc_off);
+    p.det = det;
+    p.x = x; p.x_is_half = x_is_half; p.out = y; p.y_is_half = y_is_half; p.bias = bias;
+    set_exchange(p);
+    return launch<true>(a, pl, p, st);
+}
 
 }  // namespace
 
@@ -1850,10 +1854,9 @@ int sqllm_debug_last_grid(void) { return g_last_grid; }
 const char *sqllm_last_error(void) { return g_err; }
 
 int sqllm_device_sm_count(void) {
-    int dev = 0, sm = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-    if (cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
-    return sm;
+    std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+    int dev = 0;
+    return cur_dev(dev) ? 0 : g_dev[dev].sm;
 }
 
 size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int topX) {
@@ -1895,97 +1898,16 @@ int sqllm_lutgemv(const sqllm_lutgemv_args *a, void *stream) {
 
 int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half,
                         const float *bias, void *workspace, size_t workspace_bytes, void *stream) {
-    int rc = check_common(a);
-    if (rc) return rc;
-    if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
-    if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
-    if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(bias) & 15)) return fail(SQLLM_EINVAL, "y and bias must be 16-byte aligned");
-    const bool hyb = a->full_rows && a->topX > 0;
-    if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
-    unsigned char *ws = static_cast<unsigned char *>(workspace);
-    if (det_mode() == 0 && a->out_features >= STRIP) {
-        if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
-        v2::P2 q;
-        memset(&q, 0, sizeof(q));
-        q.ws_cnt = reinterpret_cast<int *>(ws);
-        q.ws_acc = reinterpret_cast<float *>(ws + WS_ACC_OFF);
-        q.ws_hbox = reinterpret_cast<unsigned long long *>(ws + WS_HBOX_OFF);
-        q.ws_cbox = reinterpret_cast<unsigned long long *>(ws + WS_CBOX_OFF);
-        q.ws_dbox = reinterpret_cast<unsigned long long *>(ws + WS_DBOX_OFF);
-        q.x = x; q.out = y; q.y_is_half = y_is_half; q.bias = bias;
-        return launch2(a, x_is_half ? (lut_mode() == 1 ? 2 : 1) : 0, true, q, static_cast<cudaStream_t>(stream));
-    }
-    Plan pl;
-    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, true, pl);
-    if (rc) return rc;
-    if (!workspace || workspace_bytes < pl.ws_bytes)
-        return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", pl.ws_bytes, workspace_bytes);
-    Params p;
-    memset(&p, 0, sizeof(p));
-    p.ws_cnt = reinterpret_cast<int *>(ws + pl.ws_cnt_off);
-    p.ws_hyb_cnt = reinterpret_cast<int *>(ws + pl.ws_hybcnt_off);
-    p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
-    p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
-    p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
-    p.ws_acc = reinterpret_cast<float *>(ws + pl.ws_acc_off);
-    p.det = det_mode();
-    p.x = x; p.x_is_half = x_is_half; p.out = y; p.y_is_half = y_is_half; p.bias = bias;
-    return launch<true>(a, pl, p, static_cast<cudaStream_t>(stream));
+    return lutgemv_fused(a, x, x_is_half, y, y_is_half, bias, workspace, workspace_bytes, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int x_is_half, int y_is_half, const float *bias,
                                  void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, void *stream) {
-    int rc = check_common(a);
-    if (rc) return rc;
-    if (!x || !xc) return fail(SQLLM_EINVAL, "x / exchange descriptor must not be null");
-    if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
-    if (reinterpret_cast<uintptr_t>(bias) & 15) return fail(SQLLM_EINVAL, "bias must be 16-byte aligned");
-    if (det_mode() == 1) return fail(SQLLM_EINVAL, "the exchange path needs the default (non-deterministic) fused mode");
-    if (xc->world < 1 || xc->world > 64 || xc->rank < 0 || xc->rank >= xc->world) return fail(SQLLM_EINVAL, "bad world / rank (%d / %d)", xc->world, xc->rank);
-    if (xc->members < 1 || a->out_features % xc->members) return fail(SQLLM_EINVAL, "out_features=%d is not %d equal members", a->out_features, xc->members);
-    const int w = a->out_features / xc->members;
-    if (w % 4) return fail(SQLLM_EINVAL, "shard width %d must be a multiple of 4", w);
-    if (xc->out_features_full < xc->world * w) return fail(SQLLM_EINVAL, "out_features_full=%d < world * shard width = %d", xc->out_features_full, xc->world * w);
-    if (!xc->peer_base) return fail(SQLLM_EINVAL, "peer_base must not be null");
-    if ((xc->out_offset & 15) || (xc->flag_offset & 7) || (xc->state_offset & 7) || (xc->error_offset & 3)) return fail(SQLLM_EINVAL, "misaligned arena offsets");
-    if ((xc->out_features_full * (y_is_half ? 2 : 4)) % 16 || (w * (y_is_half ? 2 : 4)) % 8) return fail(SQLLM_EINVAL, "vector sizes must keep 8/16-byte store alignment");
-    const bool hyb = a->full_rows && a->topX > 0;
-    if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
-    unsigned char *ws = static_cast<unsigned char *>(workspace);
-    if (a->out_features >= STRIP) {
-        if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
-        v2::P2 q;
-        memset(&q, 0, sizeof(q));
-        q.ws_cnt = reinterpret_cast<int *>(ws);
-        q.ws_acc = reinterpret_cast<float *>(ws + WS_ACC_OFF);
-        q.ws_hbox = reinterpret_cast<unsigned long long *>(ws + WS_HBOX_OFF);
-        q.ws_cbox = reinterpret_cast<unsigned long long *>(ws + WS_CBOX_OFF);
-        q.ws_dbox = reinterpret_cast<unsigned long long *>(ws + WS_DBOX_OFF);
-        q.x = x; q.out = nullptr; q.y_is_half = y_is_half; q.bias = bias;
-        q.xw_world = xc->world; q.xw_rank = xc->rank; q.xw_members = xc->members; q.xw_nfull = xc->out_features_full;
-        q.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
-        q.xw_out_off = xc->out_offset; q.xw_flag_off = xc->flag_offset; q.xw_state_off = xc->state_offset; q.xw_err_off = xc->error_offset;
-        return launch2(a, x_is_half ? (lut_mode() == 1 ? 2 : 1) : 0, true, q, static_cast<cudaStream_t>(stream));
+    if (!xc) {
+        const int rc = check_common(a);
+        return rc ? rc : fail(SQLLM_EINVAL, "x / exchange descriptor must not be null");
     }
-    Plan pl;
-    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, true, pl);
-    if (rc) return rc;
-    if (!workspace || workspace_bytes < pl.ws_bytes)
-        return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", pl.ws_bytes, workspace_bytes);
-    Params p;
-    memset(&p, 0, sizeof(p));
-    p.ws_cnt = reinterpret_cast<int *>(ws + pl.ws_cnt_off);
-    p.ws_hyb_cnt = reinterpret_cast<int *>(ws + pl.ws_hybcnt_off);
-    p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
-    p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
-    p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
-    p.ws_acc = reinterpret_cast<float *>(ws + pl.ws_acc_off);
-    p.det = 0;
-    p.x = x; p.x_is_half = x_is_half; p.out = nullptr; p.y_is_half = y_is_half; p.bias = bias;
-    p.xw_world = xc->world; p.xw_rank = xc->rank; p.xw_members = xc->members; p.xw_nfull = xc->out_features_full;
-    p.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
-    p.xw_out_off = xc->out_offset; p.xw_flag_off = xc->flag_offset; p.xw_state_off = xc->state_offset; p.xw_err_off = xc->error_offset;
-    return launch<true>(a, pl, p, static_cast<cudaStream_t>(stream));
+    return lutgemv_fused(a, x, x_is_half, nullptr, y_is_half, bias, workspace, workspace_bytes, xc, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
@@ -2003,16 +1925,13 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int
     if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
     if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
     if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
     {
         std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        if (!g_tc_attr[dev]) {
-            if (cudaFuncSetAttribute(tc::lutgemm_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM) != cudaSuccess ||
-                cudaFuncSetAttribute(tc::lutgemm_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM) != cudaSuccess)
-                return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
-            g_tc_attr[dev] = true;
-        }
+        int dev = 0;
+        int rc = cur_dev(dev);
+        if (!rc) rc = set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4>, tc::SMEM);
+        if (!rc) rc = set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3>, tc::SMEM);
+        if (rc) return rc;
     }
     tc::PT p;
     p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;

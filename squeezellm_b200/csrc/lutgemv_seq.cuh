@@ -250,7 +250,7 @@ template <int BITS, int MODE, bool MULTI>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c) {
     using C = C2<BITS, MODE>;
     constexpr bool XH = true;
-    constexpr int NTB = C::TAB <= 16384 ? 4 : 2;  // table buffers (and strip accumulators): 4 x 4 KB exact, 2 x 64 KB for the 4-bit pair table
+    constexpr int NTB = C::NTB;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     if (raw != c.smem_raw) __trap();
@@ -260,11 +260,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
     const uint32_t bar_u32 = base + OFF_BAR;   // full[s] +8s, empty[s] +128+8s, tfull[b] +256+8b, tfree[b] +288+8b
     const uint32_t xs_u32 = base + OFF_X;
     const uint32_t sacc0 = xs_u32 + (uint32_t)c.xbytes;                 // float [NTB][64]
-    const uint32_t lo_base = sacc0 + NTB * STRIP * 4;
-    const uint32_t tab0 = (lo_base + (uint32_t)C::TAB - 1u) & ~((uint32_t)C::TAB - 1u);
     const int nstage = c.nstage;
-    const int n_lo = min(nstage, (int)((tab0 - lo_base) / C::STAGE));
-    const uint32_t hi_base = tab0 + NTB * C::TAB - (uint32_t)n_lo * C::STAGE;
+    const Carve cv(base, (uint32_t)c.xbytes, NTB * STRIP * 4, C::TAB, NTB, C::STAGE, nstage);
+    const uint32_t lo_base = cv.lo_base, tab0 = cv.tab0, hi_base = cv.hi_base;
+    const int n_lo = cv.n_lo;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid == 0) {

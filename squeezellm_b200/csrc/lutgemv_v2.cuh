@@ -86,6 +86,35 @@ struct C2 {
     static constexpr int XU = BITS == 4 ? 8 : 32;            // inputs per unit
     static constexpr int UNIT = ROWS * STRIP * 4;            // bytes of one unit in a stage
     static constexpr int STAGE = SU2 * UNIT;                 // 8 KB / 24 KB
+    static constexpr int NTB = TAB <= 16384 ? 4 : 2;         // sequence kernel: table buffers (and strip accumulators), 4 x 4 KB exact, 2 x 64 KB for the 4-bit pair table
+};
+
+// Shared-memory carve-up of lutgemv2_kernel and lutgemv_seq_kernel, from the 128-byte aligned base:
+//   [fixed OFF_X][x: xbytes][front][ring stages 0 .. n_lo)[ntab tables, each aligned to its own size][ring stages n_lo .. nstage)
+// The kernels place their buffers by it and the host sizes the launch and the ring by it: both must see the same addresses.
+struct Carve {
+    uint32_t lo_base;  // ring stage s < n_lo lives at lo_base + s * stage
+    uint32_t tab0;     // table b lives at tab0 + b * tab
+    uint32_t tab_end;
+    int lo_cap;        // ring stages that fit below the tables
+    int n_lo;
+    uint32_t hi_base;  // ring stage s >= n_lo lives at hi_base + s * stage
+    uint32_t end;      // end of the used window
+    __host__ __device__ __forceinline__ Carve(uint32_t base, uint32_t xbytes, uint32_t front, uint32_t tab, int ntab, uint32_t stage, int nstage)
+        : lo_base(base + OFF_X + xbytes + front),
+          tab0((lo_base + tab - 1u) & ~(tab - 1u)),
+          tab_end(tab0 + (uint32_t)ntab * tab),
+          lo_cap((int)((tab0 - lo_base) / stage)),
+          n_lo(nstage < lo_cap ? nstage : lo_cap),
+          hi_base(tab_end - (uint32_t)n_lo * stage),
+          end(hi_base + (uint32_t)nstage * stage) {}
+    // host: the ring depth for a window of `bytes` from `raw` - the stages that fit below and above the tables, at most `cap` and
+    // MAXD; -1: the tables themselves do not fit
+    int depth(uint32_t raw, int bytes, uint32_t stage, int cap) const {
+        const long long hi_room = (long long)raw + bytes - (long long)tab_end;
+        if (hi_room < 0) return -1;
+        return (int)std::min<long long>(std::min(cap, MAXD), lo_cap + hi_room / stage);
+    }
 };
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
@@ -612,11 +641,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     unsigned char *sm = smem_raw + (base - raw);
     const uint32_t bar_u32 = base + OFF_BAR;
     const uint32_t xs_u32 = base + OFF_X;
-    const uint32_t lo_base = xs_u32 + (uint32_t)((p.K * (XH ? 2 : 4) + 127) & ~127);
-    const uint32_t tab0 = (lo_base + (uint32_t)C::TAB - 1u) & ~((uint32_t)C::TAB - 1u);  // two tables, each aligned to its own size
     const int nstage = p.nstage;
-    const int n_lo = min(nstage, (int)((tab0 - lo_base) / C::STAGE));       // ring stages that fit below the aligned tables
-    const uint32_t hi_base = tab0 + 2 * C::TAB - (uint32_t)n_lo * C::STAGE; // stage s >= n_lo lives at hi_base + s * STAGE
+    const Carve cv(base, (uint32_t)((p.K * (XH ? 2 : 4) + 127) & ~127), 0u, C::TAB, 2, C::STAGE, nstage);
+    const uint32_t lo_base = cv.lo_base, tab0 = cv.tab0, hi_base = cv.hi_base;
+    const int n_lo = cv.n_lo;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int N = p.N, R = p.R;
