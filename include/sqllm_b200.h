@@ -60,8 +60,8 @@ int sqllm_device_sm_count(void);
 /* ---------------------------------------------------------------------------------------------
  * Workspace.  Used only by the *_fused entry point (cross-CTA accumulator, counters, deterministic-mode partials).
  * Must be zero-filled once after allocation (cudaMemset); the library keeps it consistent afterwards.  One
- * workspace serves layers of any shape, but must not be used by two streams concurrently.  The size returned
- * does not depend on the summation mode.
+ * workspace serves layers of any shape, but must not be used by two streams concurrently.  A size returned in either
+ * summation mode serves both.
  * ------------------------------------------------------------------------------------------- */
 size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int topX);
 
@@ -90,8 +90,8 @@ typedef struct sqllm_lutgemv_args {
 int sqllm_lutgemv(const sqllm_lutgemv_args *args, void *stream);
 
 /* Fused-path summation mode (process-wide).
- *   0 (default; env SQLLM_DETERMINISTIC unset): contributions are added with red.add.f32 into a workspace accumulator, like the
- *     reference's atomicAdd - results can differ in the last bits from run to run; the last CTAs of the grid convert it to y.
+ *   0 (default; env SQLLM_DETERMINISTIC unset): contributions are added in the order they arrive (red.add.f32), like the
+ *     reference's atomicAdd - results can differ in the last bits from run to run.
  *   1: per-strip partials reduced in a fixed order by the last-arriving contributor - bit-reproducible, 1.3-2x slower on
  *     layers with outliers. */
 void sqllm_set_deterministic(int on);

@@ -7,9 +7,9 @@
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
 // LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused).
 //
-// Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every layer of 64 or more output columns in the
-// accumulate and the default (fast) fused mode.  lutgemv_kernel below ("v1") runs the deterministic fused mode
-// (sqllm_set_deterministic / SQLLM_DETERMINISTIC=1) and layers narrower than one strip (out_features < 64) in every mode.
+// Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default
+// (fast) fused mode, whatever its width: a layer narrower than one strip is a layer whose only strip is ragged.
+// lutgemv_kernel below ("v1") is the kernel of the deterministic fused mode (sqllm_set_deterministic / SQLLM_DETERMINISTIC=1).
 // v1 (DESIGN.md has the full story and the measurements):
 //   * ONE launch per GEMV.  The [units x strips] iteration space (unit = one packed row for 4-bit,
 //     one 3-row / 32-input group for 3-bit; strip = 64 output columns) is flattened strip-major and
@@ -25,10 +25,8 @@
 //       - sparse warp: CSR rows spread evenly over all CTAs, staged with 16-byte cp.async, x gathered in batches,
 //         per-row sums in storage order; plus a k-slice of the topX dense rows.
 //   * Only the slice of x a CTA needs is staged (fp32, converted from fp16 on the way in).
-//   * Flush: accumulate mode (the reference's 12 symbols; `mul` pre-filled by the caller) issues one red.add.f32 per
-//     (CTA, column).  Fused mode (QuantLinearLUT.forward): fast (default) = red.add into a workspace accumulator, a
-//     release counter, and the last CTAs of the grid convert / store y (optionally into every rank's peer-mapped arena:
-//     the multi-GPU exchange); deterministic = per-strip partials + tickets, fixed summation order.
+//   * Flush: per-strip partials in the workspace and one ticket per contributor; the last contributor of a strip sums them in a
+//     fixed order, adds the bias and stores y.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -59,10 +57,8 @@ constexpr int MAXSEG = 4;                 // strips a CTA may touch
 constexpr int STRIP = 64;                 // output columns per strip (16 lanes x 4 columns)
 constexpr int SU = 2 * NW;                // units per pipeline stage (one pair per consumer warp)
 constexpr int CSR_CH = 1024;              // CSR elements staged per chunk
-constexpr int SROWS_LD = 68;              // padded row-pointer slice per segment (65 used)
+constexpr int STAGE = CSR_CH * 16;        // staging buffer: a chunk of CSR cols + vals (8 KB), then the dense-row partials (8 KB)
 constexpr int MAX_TOPX_FUSED = SQLLM_FUSED_MAX_TOPX;
-constexpr int NFIN_COLS = 1024;           // fast fused mode: about this many columns per finishing CTA ...
-constexpr int NFIN_MAX = 16;              // ... and at most this many finishers
 constexpr int HYB_R = 11;                 // dense rows: k-rows per lane slot requested before the dependency wait
 constexpr int MAX_STRIPS = 16320;         // per-strip tickets in the workspace header (out_features <= 1,044,480)
 constexpr int MAX_N_FUSED = SQLLM_FUSED_MAX_OUT;  // fused path: the scratch accumulator lives at a fixed place in the workspace
@@ -77,8 +73,8 @@ struct Params {
     const uint32_t *qw;
     const float *lut;
     const void *x;      // fp32 or fp16 [K]
-    void *out;          // accumulate mode: float* mul ; fused: fp32/fp16 y
-    const float *bias;  // fused only, may be null
+    void *out;          // fp32/fp16 y
+    const float *bias;  // may be null
     const int *rows, *cols;
     const float *vals;
     const float *full_rows;
@@ -95,23 +91,14 @@ struct Params {
     int hc;       // CTAs that take a slice of the dense rows
     int hrows;    // k-rows per such CTA
     int x_is_half, y_is_half;
-    int maxc;     // max dense contributors per strip (fused)
+    int maxc;     // max dense contributors per strip
     float *ws_part;   // [strips][maxc+1][64]
     int *ws_cnt;      // [strips]
     float *ws_hyb;    // [hc][topX]
-    int *ws_hyb_cnt;  // [1]
-    int has_csr;
-    int has_stage;   // bytes of the shared-memory staging buffer: 0, CSR_CH*8 (CSR cols+vals) or CSR_CH*16 (+ dense-row partials, deterministic mode)
+    int has_stage;   // bytes of the shared-memory staging buffer: 0 or STAGE
     int csr_al16;    // cols / vals are 16-byte aligned: stage them with 16-byte cp.async
     int csr_rpc;     // CSR rows (output channels) handled per CTA: rows are spread evenly over all CTAs
-    float *ws_csr;   // [N] CSR row sums (deterministic fused mode)
-    float *ws_acc;   // [N] fp32 accumulator, zero between launches (fast fused mode)
-    // optional exchange (column-sharded layers): finishers store their slice into every rank's arena over NVLink
-    int xw_world, xw_rank, xw_members, xw_nfull;   // xw_world == 0: no exchange
-    const unsigned long long *xw_base;             // device array [world]: base address of every rank's symmetric arena
-    unsigned long long xw_out_off, xw_flag_off, xw_state_off, xw_err_off;
-    int nfin;        // fast fused mode: CTAs (the last ones of the grid) that share the final conversion
-    int det;         // fused mode: 1 = deterministic per-strip tickets, 0 = red.add into ws_acc + one global ticket per CTA
+    float *ws_csr;   // [N] CSR row sums
     unsigned long long *trace;  // debug timeline (only written when built with -DSQLLM_TRACE and non-null)
 };
 
@@ -360,7 +347,7 @@ __device__ __forceinline__ void consume(const Words<3> &g, const int jsel, const
     for (int t = 0; t < 4; ++t) consume3_col(a[t], b[t], c[t], lsv[t], xp, acc[t]);
 }
 
-// ---- fused mode: who contributes to a strip, and the per-column final reduction ----------------------
+// ---- who contributes to a strip, and the per-column final reduction ----------------------
 __device__ __forceinline__ bool strip_has_hybrid(const Params &p, int strip) {
     if (!p.full_rows) return false;
     bool h = false;
@@ -370,7 +357,7 @@ __device__ __forceinline__ bool strip_has_hybrid(const Params &p, int strip) {
     }
     return h;
 }
-// Contributors that take a ticket on strip `strip` (deterministic fused mode): nd dense CTAs (stream-K), ncsr CTAs whose CSR row
+// Contributors that take a ticket on strip `strip`: nd dense CTAs (stream-K), ncsr CTAs whose CSR row
 // range touches the strip and - if a dense row lands in it - all hc dense-row contributors.
 __device__ __forceinline__ int strip_contributors(const Params &p, int strip, int &nd, bool &hyb) {
     const int first = (int)(((long long)strip * p.R) / p.chunk);
@@ -452,9 +439,9 @@ __device__ __forceinline__ float load_x(const Params &p, int k) {  // read-only 
 // step is lane-parallel: row pointers live one-per-lane (shuffles / ballots instead of serial scans), cols/vals are staged
 // with cp.async, x is gathered in batches of independent loads, per-row sums are taken in storage order (deterministic).
 // Everything static (row pointers, cols/vals, dense-row values) is requested BEFORE griddepcontrol.wait.
-// Results: accumulate mode -> red.add on mul; fused mode -> ws_csr[row] / dense-row partials + a ticket on the strips touched.
+// Results: ws_csr[row] / dense-row partials + a ticket on the strips touched.
 // =================================================================================================
-template <int BITS, bool FUSED>
+template <int BITS>
 __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, const uint32_t sm_u32, const int lane, float *hyb_tot,
                                             const int nseg, const int s0) {
     using C = Cfg<BITS>;
@@ -516,7 +503,7 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
     __syncwarp();
     TRACE(14, lane == 0);
 
-    // ---------------- phase B: needs x (and, in fused mode, the workspace) ----------------
+    // ---------------- phase B: needs x and the workspace ----------------
     // (1) topX dense rows: CTA b < hc takes k-rows [kb, ke)
     if (hyb_on) {
         for (int jb = 0; jb < (hyb_multi ? 1 : p.topX); jb += 32) {
@@ -548,31 +535,19 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
                     for (int k = kb; k < ke; ++k, fr += p.topX) a += __ldg(fr) * load_x(p, k);
                 }
             }
-            if (j < p.topX) {
-                if (FUSED && p.det) {
-                    p.ws_hyb[(size_t)blockIdx.x * p.topX + j] = a;
-                } else {
-                    const int c = __ldg(p.fri + j);
-                    if (c >= 0 && c < N) atomicAdd((FUSED ? p.ws_acc : reinterpret_cast<float *>(p.out)) + c, a);
-                }
-            }
+            if (j < p.topX) p.ws_hyb[(size_t)blockIdx.x * p.topX + j] = a;
         }
     }
     TRACE(15, lane == 0);
 
     // (2) CSR outliers
-    float *const acc_out = FUSED ? p.ws_acc : reinterpret_cast<float *>(p.out);  // where red.add contributions go (non-deterministic modes)
-    auto emit = [&](int row, float v) {
-        if (FUSED && p.det) p.ws_csr[row] = v;
-        else atomicAdd(acc_out + row, v);
-    };
     while (r < rb) {
         if (m == 0) {  // a single row longer than the staging buffer: straight from global memory, whole warp
             const int e1 = __shfl_sync(0xffffffffu, rp, 1);
             float a = 0.f;
             for (int e = base + lane; e < e1; e += 32) a += __ldg(p.vals + e) * load_x(p, __ldg(p.cols + e));
             a = warp_sum(a);
-            if (lane == 0) emit(r, a);
+            if (lane == 0) p.ws_csr[r] = a;
             r += 1;
         } else {
             cp_async_wait_all();
@@ -600,7 +575,7 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
                 int e = a0;
                 for (; e + 1 < a1; e += 2) { ea += svals[e]; eb += svals[e + 1]; }
                 if (e < a1) ea += svals[e];
-                emit(r + lane, ea + eb);
+                p.ws_csr[r + lane] = ea + eb;
             }
             unsigned longm = __ballot_sync(0xffffffffu, n > 64);  // long rows: the whole warp on each, fixed xor tree
             while (longm) {
@@ -610,32 +585,30 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
                 float a = 0.f;
                 for (int e = b0 + lane; e < b1; e += 32) a += svals[e];
                 a = warp_sum(a);
-                if (lane == 0) emit(r + i, a);
+                if (lane == 0) p.ws_csr[r + i] = a;
             }
             __syncwarp();
             r += m;
         }
         if (r < rb) group_begin();
     }
-    if (FUSED && p.det) {
-        // publish: one fence for everything this warp wrote (CSR row sums, dense-row partials), then one ticket per strip touched
-        const uint32_t hstage_u32 = svals_u32 + CSR_CH * 4;
-        const float *hstage = svals + CSR_CH;
-        __syncwarp();
-        if (p.rows && ra < rb)
-            for (int strip = ra / STRIP; strip <= (rb - 1) / STRIP; ++strip) warp_ticket(p, strip, lane, hstage_u32, hstage, hyb_tot);
-        if (hyb_on) {  // every distinct strip that owns a dense-row output channel
-            for (int j0 = 0; j0 < p.topX; ++j0) {
-                const int cj0 = __ldg(p.fri + j0);
-                if (cj0 < 0 || cj0 >= N) continue;
-                const int strip = cj0 / STRIP;
-                bool seen = false;
-                for (int j = 0; j < j0; ++j) {
-                    const int cj = __ldg(p.fri + j);
-                    seen |= (cj >= 0 && cj < N && cj / STRIP == strip);
-                }
-                if (!seen) warp_ticket(p, strip, lane, hstage_u32, hstage, hyb_tot);
+    // publish: one fence for everything this warp wrote (CSR row sums, dense-row partials), then one ticket per strip touched
+    const uint32_t hstage_u32 = svals_u32 + CSR_CH * 4;
+    const float *hstage = svals + CSR_CH;
+    __syncwarp();
+    if (p.rows && ra < rb)
+        for (int strip = ra / STRIP; strip <= (rb - 1) / STRIP; ++strip) warp_ticket(p, strip, lane, hstage_u32, hstage, hyb_tot);
+    if (hyb_on) {  // every distinct strip that owns a dense-row output channel
+        for (int j0 = 0; j0 < p.topX; ++j0) {
+            const int cj0 = __ldg(p.fri + j0);
+            if (cj0 < 0 || cj0 >= N) continue;
+            const int strip = cj0 / STRIP;
+            bool seen = false;
+            for (int j = 0; j < j0; ++j) {
+                const int cj = __ldg(p.fri + j);
+                seen |= (cj >= 0 && cj < N && cj / STRIP == strip);
             }
+            if (!seen) warp_ticket(p, strip, lane, hstage_u32, hstage, hyb_tot);
         }
     }
 }
@@ -643,7 +616,7 @@ __device__ __forceinline__ void sparse_warp(const Params &p, unsigned char *sm, 
 // =================================================================================================
 // The kernel
 // =================================================================================================
-template <int BITS, bool FUSED>
+template <int BITS>
 __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Params p) {
     using C = Cfg<BITS>;
     extern __shared__ unsigned char smem_raw[];
@@ -721,7 +694,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
         }
     };
     if (warp == WARP_SPARSE) {
-        sparse_warp<BITS, FUSED>(p, sm, sm_u32, lane, hyb_tot + maxseg * MAX_TOPX_FUSED, nseg, s0);
+        sparse_warp<BITS>(p, sm, sm_u32, lane, hyb_tot + maxseg * MAX_TOPX_FUSED, nseg, s0);
         TRACE(10, lane == 0);
     } else {
         // ---- the first PF weight fetches of every lane go out before anything else.  They do not depend on the previous
@@ -757,7 +730,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
         }
 
         TRACE(2, tid == 0);
-        // Everything below reads data the previous kernel may have produced (x, mul, workspace).  One thread waits on the
+        // Everything below reads data the previous kernel may have produced (x, workspace).  One thread waits on the
         // programmatic dependency; the other consumers sleep on a hardware barrier instead of each polling it.
         if (tid == 0) pdl_wait();
         named_bar_sync(6, NW * 32);
@@ -865,28 +838,14 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
     if (tid < MAXSEG * STRIP) {
         const int seg = tid >> 6, c = tid & 63;
         const bool active = seg < nseg;
-        float tot = 0.f;
-        int strip = 0, nd = 1, slot = 0;
+        int strip = 0, nd = 1, expected = 1;
         bool hyb = false;
         if (active) {
             strip = s0 + seg;
+            float tot = 0.f;
 #pragma unroll
             for (int w = 0; w < NW; ++w) tot += part[(seg * NW + w) * STRIP + c];
-        }
-        if (!FUSED) {
-            const int col = strip * STRIP + c;
-            if (active && col < N) atomicAdd(reinterpret_cast<float *>(p.out) + col, tot);
-            TRACE(11, tid == 0);
-            return;
-        }
-        if (!p.det) {  // fast fused mode: same red.add, into the zeroed scratch accumulator; conversion happens below
-            const int col = strip * STRIP + c;
-            if (active && col < N) atomicAdd(p.ws_acc + col, tot);
-        } else {
-        int expected = 1;
-        if (active) {
             expected = strip_contributors(p, strip, nd, hyb);
-            slot = (int)blockIdx.x - (int)(((long long)strip * R) / p.chunk);
             if (expected == 1) {  // this CTA is the strip's only contributor: store directly
                 const int col = strip * STRIP + c;
                 if (col < N) {
@@ -895,6 +854,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
                     else reinterpret_cast<float *>(p.out)[col] = tot;
                 }
             } else {
+                const int slot = (int)blockIdx.x - (int)(((long long)strip * R) / p.chunk);
                 p.ws_part[((size_t)strip * p.maxc + slot) * STRIP + c] = tot;
             }
         }
@@ -919,111 +879,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
             }
             final_store(p, strip, c, nd, hyb ? ht : nullptr);
         }
-        }  // det
         TRACE(11, tid == 0);
-    }
-    if (FUSED && !p.det) {
-        // Fast fused mode.  Every CTA announces "my red.adds are out" with one fire-and-forget red.release on a gpu-scope counter
-        // and leaves.  The last `nfin` CTAs of the grid (by index - they are dispatched last) stay, wait until the counter reaches
-        // the grid size, and each turns its 1/nfin slice of the accumulator into y (+ bias, converted) and re-zeroes it.  One CTA
-        // alone is too slow for a wide layer; 16 of them need one L2 round trip.
-        // All CTAs of a launch are co-resident by construction (make_plan sizes the grid to the occupancy), so the wait cannot
-        // deadlock; the counter is reset by the last finisher for the next launch (kernel boundary orders it).
-        __syncthreads();  // all red.adds of this CTA issued
-        const int G = (int)gridDim.x, nfin = p.nfin;
-        const int fidx = (int)blockIdx.x - (G - nfin);
-        if (tid == 0) {
-            asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(p.ws_hyb_cnt) : "memory");
-            if (fidx >= 0) {
-                int seen;
-                do {
-                    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.ws_hyb_cnt) : "memory");
-                    if (seen < G) __nanosleep(40);
-                } while (seen < G);
-            }
-        }
-        TRACE(8, tid == 0);  // announced (finishers: all arrived)
-        if (fidx < 0) return;
-        __syncthreads();
-        {
-            const float4 *acc4 = reinterpret_cast<const float4 *>(p.ws_acc);
-            const int n4 = N >> 2;
-            const int per = (n4 + nfin - 1) / nfin;
-            const int lo = min(n4, fidx * per), hi = min(n4, lo + per);
-            for (int c0 = lo + tid; c0 < hi; c0 += 4 * THREADS) {
-                float4 v[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int c4 = c0 + u * THREADS;
-                    v[u] = c4 < hi ? __ldcg(acc4 + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int c4 = c0 + u * THREADS;
-                    if (c4 < hi) {
-                        reinterpret_cast<float4 *>(p.ws_acc)[c4] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (p.bias) {
-                            const float4 bv = __ldg(reinterpret_cast<const float4 *>(p.bias) + c4);
-                            v[u].x += bv.x; v[u].y += bv.y; v[u].z += bv.z; v[u].w += bv.w;
-                        }
-                        uint2 pk = make_uint2(0u, 0u);
-                        if (p.y_is_half) {
-                            __half2 lo2 = __floats2half2_rn(v[u].x, v[u].y), hi2 = __floats2half2_rn(v[u].z, v[u].w);
-                            pk.x = *reinterpret_cast<uint32_t *>(&lo2);
-                            pk.y = *reinterpret_cast<uint32_t *>(&hi2);
-                        }
-                        if (p.xw_world == 0) {
-                            if (p.y_is_half) reinterpret_cast<uint2 *>(p.out)[c4] = pk;
-                            else reinterpret_cast<float4 *>(p.out)[c4] = v[u];
-                        } else {
-                            // local column 4*c4 of the stacked shard = column j of member m; it lands at [m][rank*w + j] of the
-                            // [members][n_full] vector in EVERY rank's arena (w % 4 == 0: a quad never straddles members)
-                            const int w = N / p.xw_members, col = 4 * c4, m = col / w, j = col - m * w;
-                            const unsigned long long e = (unsigned long long)m * p.xw_nfull + (unsigned long long)p.xw_rank * w + j;
-                            for (int pr = 0; pr < p.xw_world; ++pr) {
-                                unsigned char *dst = reinterpret_cast<unsigned char *>(__ldg(p.xw_base + pr) + p.xw_out_off);
-                                if (p.y_is_half) *reinterpret_cast<uint2 *>(dst + 2 * e) = pk;
-                                else *reinterpret_cast<float4 *>(dst + 4 * e) = v[u];
-                            }
-                        }
-                    }
-                }
-            }
-        }
-        TRACE(9, tid == 0);
-        __syncthreads();
-        if (tid == 0) {
-            unsigned long long target = 0ull;
-            if (p.xw_world) {
-                // publish this finisher's stores on every rank (system-scope release), then wait until every finisher of every
-                // rank has published on ours: when this grid completes, the local vector is whole.  Counters only grow
-                // (expected arrivals so far live next to the flag), so nothing is ever reset across ranks.  The wait is bounded:
-                // a rank that never shows up sets the error word instead of hanging the GPU.
-                const unsigned long long self = __ldg(p.xw_base + p.xw_rank);
-                target = *reinterpret_cast<volatile unsigned long long *>(self + p.xw_state_off) + (unsigned long long)p.xw_world * nfin;
-                __threadfence_system();
-                for (int pr = 0; pr < p.xw_world; ++pr)
-                    atomicAdd_system(reinterpret_cast<unsigned long long *>(__ldg(p.xw_base + pr) + p.xw_flag_off), 1ull);
-                unsigned long long seen, t0, t1;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-                const bool broken = *reinterpret_cast<volatile unsigned int *>(self + p.xw_err_off) != 0u;  // an earlier wait gave up: do not wait again
-                if (!broken) do {
-                    asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(seen) : "l"(self + p.xw_flag_off) : "memory");
-                    if (seen >= target) break;
-                    __nanosleep(100);
-                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                    if (t1 - t0 > 2000000000ull) { *reinterpret_cast<volatile unsigned int *>(self + p.xw_err_off) = 1u; break; }
-                } while (true);
-            }
-            // the finisher that completes the set puts both counters back to zero (and advances the expected arrivals)
-            int done;
-            asm volatile("atom.relaxed.gpu.global.add.s32 %0, [%1], 1;" : "=r"(done) : "l"(p.ws_hyb_cnt + 32) : "memory");
-            if (done == nfin - 1) {
-                p.ws_hyb_cnt[0] = 0;
-                p.ws_hyb_cnt[32] = 0;
-                if (p.xw_world) *reinterpret_cast<volatile unsigned long long *>(__ldg(p.xw_base + p.xw_rank) + p.xw_state_off) = target;
-            }
-        }
     }
 }
 
@@ -1163,7 +1019,7 @@ int det_mode() {
     if (g_det < 0) { const char *e = getenv("SQLLM_DETERMINISTIC"); g_det = (e && e[0] == '1') ? 1 : 0; }
     return g_det;
 }
-// g_det - fused mode: 1 = deterministic per-strip tickets, 0 = red.add + one global ticket (default; SQLLM_DETERMINISTIC=1 or sqllm_set_deterministic)
+// g_det - fused mode: 1 = v1, deterministic per-strip tickets (SQLLM_DETERMINISTIC=1 or sqllm_set_deterministic), 0 = v2 (default)
 int g_last_grid = 0;
 unsigned long long *g_trace = nullptr;
 size_t g_trace_stride = 0;
@@ -1214,20 +1070,21 @@ int get_tensor_map(const void *qweight, int rows, int cols, int box_rows, CUtens
 
 struct Plan {
     int R, strips, T, chunk, G, maxc, hc, hrows, smem, maxseg, x_direct, xfloats;
-    size_t ws_cnt_off, ws_hybcnt_off, ws_hyb_off, ws_part_off, ws_csr_off, ws_acc_off, ws_bytes;
+    size_t ws_cnt_off, ws_hyb_off, ws_part_off, ws_csr_off, ws_bytes;
     int csr_rpc, has_stage;
 };
 
-int make_plan(int bits, int K, int N, int topX, bool has_csr_in, bool fused, Plan &pl) {
+// stage: bytes of the shared-memory staging buffer when the layer has CSR outliers or dense rows: STAGE for a launch (smaller only
+// in sqllm_workspace_bytes)
+int make_plan(int bits, int K, int N, int topX, bool has_csr_in, int stage, Plan &pl) {
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);  // lazily initialised statics below
     const bool has_csr = has_csr_in || topX > 0;  // from here on: "a staging buffer is needed"
-    // staging: CSR cols/vals chunks (8 KB); the deterministic fused mode also stages the dense-row partials there (8 KB more)
-    pl.has_stage = has_csr ? CSR_CH * 8 + ((fused && det_mode() == 1) ? CSR_CH * 8 : 0) : 0;
+    pl.has_stage = has_csr ? stage : 0;
     int dev = 0;
     int rc = cur_dev(dev);
     if (rc) return rc;
     DevInfo &d = g_dev[dev];
-    for (auto fn : {lutgemv_kernel<4, false>, lutgemv_kernel<4, true>, lutgemv_kernel<3, false>, lutgemv_kernel<3, true>})
+    for (auto fn : {lutgemv_kernel<4>, lutgemv_kernel<3>})
         if ((rc = set_max_smem(d, fn, 227 * 1024))) return rc;
     const int XU = bits == 4 ? 8 : 32;
     pl.R = bits == 4 ? K / 8 : K / 32;
@@ -1235,11 +1092,10 @@ int make_plan(int bits, int K, int N, int topX, bool has_csr_in, bool fused, Pla
     const long long T = (long long)pl.strips * pl.R;
     if (T > 0x3fffffff) return fail(SQLLM_EINVAL, "problem too large");
     pl.T = (int)T;
-    if (pl.strips > MAX_STRIPS || (fused && N > MAX_N_FUSED)) return fail(SQLLM_EINVAL, "out_features=%d exceeds the workspace header (max %d)", N, MAX_N_FUSED);
+    if (pl.strips > MAX_STRIPS || N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the workspace header (max %d)", N, MAX_N_FUSED);
 
-    // The grid must be co-resident (the fast fused mode's finishers wait for every CTA): a plan whose shared memory lets fewer
-    // than CTAS_PER_SM CTAs onto an SM would run a second wave.  Plan for CTAS_PER_SM, ask the occupancy calculator, and fall
-    // back to fewer CTAs per SM if it disagrees.
+    // One wave: a plan whose shared memory lets fewer than CTAS_PER_SM CTAs onto an SM would run a second one.  Plan for
+    // CTAS_PER_SM, ask the occupancy calculator, and fall back to fewer CTAs per SM if it disagrees.
     int use_cps = CTAS_PER_SM;
 replan:
     const int G0 = d.sm * use_cps;
@@ -1256,7 +1112,7 @@ replan:
     {
         static std::mutex occ_mu;
         static std::unordered_map<unsigned long long, int> occ_cache;
-        const unsigned long long key = ((unsigned long long)smem << 8) | (unsigned long long)((bits == 4 ? 2 : 0) | (fused ? 1 : 0));
+        const unsigned long long key = ((unsigned long long)smem << 8) | (unsigned long long)bits;
         int occ = -1;
         {
             std::lock_guard<std::mutex> lk(occ_mu);
@@ -1264,12 +1120,7 @@ replan:
             if (it != occ_cache.end()) occ = it->second;
         }
         if (occ < 0) {
-            const int threads = THREADS;
-            cudaError_t e;
-            if (bits == 4) e = fused ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lutgemv_kernel<4, true>, threads, smem)
-                                     : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lutgemv_kernel<4, false>, threads, smem);
-            else e = fused ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lutgemv_kernel<3, true>, threads, smem)
-                           : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lutgemv_kernel<3, false>, threads, smem);
+            const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, THREADS, smem);
             if (e != cudaSuccess) return fail(SQLLM_ECUDA, "occupancy query failed: %s", cudaGetErrorString(e));
             std::lock_guard<std::mutex> lk(occ_mu);
             occ_cache[key] = occ;
@@ -1285,35 +1136,28 @@ replan:
     pl.maxc = (pl.R - 1) / chunk + 2;
     pl.hc = 0;
     pl.hrows = 0;
-    int hc_det = 0;  // workspace is sized for the deterministic mode whatever the current mode
+    int hc = 0;
     if (topX > 0) {
         // dense-row contributors: as few k-rows per CTA as the grid allows, down to what one warp requests before the dependency
-        // wait (HYB_R steps of 32/topX rows).  Deterministic mode also needs the partials (hc*topX floats) to fit the
-        // 2*CSR_CH-float staging buffer of the finisher.
+        // wait (HYB_R steps of 32/topX rows), and no more partials (hc*topX floats) than the 2*CSR_CH-float staging buffer of the
+        // finisher holds
         const int rows_pre = HYB_R * (topX <= 32 ? 32 / topX : 1);
-        int hc = pl.G;
-        if (hc > (K + rows_pre - 1) / rows_pre) hc = (K + rows_pre - 1) / rows_pre;
-        hc_det = hc;
-        if (hc_det > 2 * CSR_CH / topX) hc_det = 2 * CSR_CH / topX;
-        if (hc_det < 1) hc_det = 1;
-        if (fused && det_mode() == 1) hc = hc_det;
+        hc = std::min({pl.G, (K + rows_pre - 1) / rows_pre, 2 * CSR_CH / topX});
         if (hc < 1) hc = 1;
         pl.hrows = (K + hc - 1) / hc;
         pl.hc = (K + pl.hrows - 1) / pl.hrows;
     }
     pl.csr_rpc = (N + pl.G - 1) / pl.G;
     if (pl.csr_rpc < 1) pl.csr_rpc = 1;
-    // Fixed header: [0,4) dense-row ticket, [256, 256+4*MAX_STRIPS) per-strip tickets.  Tickets must never
-    // share bytes with data regions of ANY shape (the workspace is reused across layers of different sizes).
+    // Fixed header: [256, 256+4*MAX_STRIPS) per-strip tickets.  Tickets must never share bytes with data regions of ANY shape
+    // (the workspace is reused across layers of different sizes).
     size_t off = WS_HEADER;
-    pl.ws_hybcnt_off = 0;
     pl.ws_cnt_off = 256;
-    pl.ws_hyb_off = off; off += (size_t)hc_det * (topX > 0 ? topX : 0) * 4;
+    pl.ws_hyb_off = off; off += (size_t)hc * topX * 4;
     off = (off + 255) & ~(size_t)255;
     pl.ws_part_off = off; off += (size_t)pl.strips * pl.maxc * STRIP * 4;
     off = (off + 255) & ~(size_t)255;
     pl.ws_csr_off = off; off += (size_t)N * 4;
-    pl.ws_acc_off = WS_ACC_OFF;
     pl.ws_bytes = off;
     return SQLLM_OK;
 }
@@ -1331,7 +1175,6 @@ int check_common(const sqllm_lutgemv_args *a) {
     return SQLLM_OK;
 }
 
-template <bool FUSED>
 int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t st) {
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
     p.qw = reinterpret_cast<const uint32_t *>(a->qweight);
@@ -1345,18 +1188,13 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
     p.R = pl.R; p.strips = pl.strips; p.T = pl.T; p.chunk = pl.chunk;
     p.maxseg = pl.maxseg; p.x_direct = pl.x_direct; p.xfloats = pl.xfloats;
     p.hc = hyb ? pl.hc : 0; p.hrows = pl.hrows; p.maxc = pl.maxc;
-    p.has_csr = a->rows ? 1 : 0;
     p.has_stage = pl.has_stage;
     p.csr_rpc = pl.csr_rpc;
-    p.nfin = (a->out_features + NFIN_COLS - 1) / NFIN_COLS;
-    if (p.nfin > NFIN_MAX) p.nfin = NFIN_MAX;
-    if (p.nfin > pl.G) p.nfin = pl.G;
-    if (p.nfin < 1) p.nfin = 1;
     p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
     p.trace = g_trace;
     if (g_trace) g_trace += g_trace_stride;
     g_last_grid = pl.G;
-    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4, FUSED> : lutgemv_kernel<3, FUSED>, pl.G, THREADS, pl.smem, st, false, p);
+    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, pl.G, THREADS, pl.smem, st, false, p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1378,17 +1216,19 @@ int lut_mode() {
 
 typedef void (*K2)(const v2::P2, const CUtensorMap, const CUtensorMap);
 struct K2Info { K2 fn; int tab, stage; };
-// [bits==4][variant][fused] ; variant 0: exact, fp32 x ; 1: exact, fp16 x ; 2: fp16 pair table, fp16 x
+// fused: variant 0: exact, fp32 x ; 1: exact, fp16 x ; 2: fp16 pair table, fp16 x.  Accumulate mode (the 12 symbols): variant 0 only.
 K2Info k2_lookup(int bits, int variant, bool fused) {
 #define K2E(B, M, XH, F) K2Info{v2::lutgemv2_kernel<B, M, XH, F>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE}
     if (bits == 4) {
-        if (variant == 0) return fused ? K2E(4, 0, false, true) : K2E(4, 0, false, false);
-        if (variant == 1) return fused ? K2E(4, 0, true, true) : K2E(4, 0, true, false);
-        return fused ? K2E(4, 1, true, true) : K2E(4, 1, true, false);
+        if (!fused) return K2E(4, 0, false, false);
+        if (variant == 0) return K2E(4, 0, false, true);
+        if (variant == 1) return K2E(4, 0, true, true);
+        return K2E(4, 1, true, true);
     }
-    if (variant == 0) return fused ? K2E(3, 0, false, true) : K2E(3, 0, false, false);
-    if (variant == 1) return fused ? K2E(3, 0, true, true) : K2E(3, 0, true, false);
-    return fused ? K2E(3, 1, true, true) : K2E(3, 1, true, false);
+    if (!fused) return K2E(3, 0, false, false);
+    if (variant == 0) return K2E(3, 0, false, true);
+    if (variant == 1) return K2E(3, 0, true, true);
+    return K2E(3, 1, true, true);
 #undef K2E
 }
 
@@ -1438,10 +1278,11 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
         int rc = cur_dev(dev);
         if (rc) return rc;
         DevInfo &d = g_dev[dev];
-        for (int b = 3; b <= 4; ++b)
+        for (int b = 3; b <= 4; ++b) {
+            if ((rc = set_max_smem(d, k2_lookup(b, 0, false).fn, 227 * 1024))) return rc;
             for (int v = 0; v < 3; ++v)
-                for (int f = 0; f < 2; ++f)
-                    if ((rc = set_max_smem(d, k2_lookup(b, v, f != 0).fn, 227 * 1024))) return rc;
+                if ((rc = set_max_smem(d, k2_lookup(b, v, true).fn, 227 * 1024))) return rc;
+        }
         if ((rc = smem_window(d))) return rc;
         sm = d.sm;
         raw = d.smem_raw;
@@ -1759,8 +1600,8 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     return SQLLM_OK;
 }
 
-// ---- fused GEMV: v2, or v1 for the deterministic mode and layers narrower than one strip; with an exchange descriptor the
-// result goes to every rank's arena instead of y ---------------------------------------------------------------------------------
+// ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
+// arena instead of y ---------------------------------------------------------------------------------------------------------------
 int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
                   void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, cudaStream_t st) {
     int rc = check_common(a);
@@ -1784,13 +1625,7 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, voi
     const bool hyb = a->full_rows && a->topX > 0;
     if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
     unsigned char *ws = static_cast<unsigned char *>(workspace);
-    auto set_exchange = [xc](auto &p) {  // the two kernels' parameter blocks name the exchange fields alike
-        if (!xc) return;
-        p.xw_world = xc->world; p.xw_rank = xc->rank; p.xw_members = xc->members; p.xw_nfull = xc->out_features_full;
-        p.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
-        p.xw_out_off = xc->out_offset; p.xw_flag_off = xc->flag_offset; p.xw_state_off = xc->state_offset; p.xw_err_off = xc->error_offset;
-    };
-    if (det == 0 && a->out_features >= STRIP) {
+    if (det == 0) {
         if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
         v2::P2 q;
         memset(&q, 0, sizeof(q));
@@ -1800,26 +1635,27 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, voi
         q.ws_cbox = reinterpret_cast<unsigned long long *>(ws + WS_CBOX_OFF);
         q.ws_dbox = reinterpret_cast<unsigned long long *>(ws + WS_DBOX_OFF);
         q.x = x; q.out = y; q.y_is_half = y_is_half; q.bias = bias;
-        set_exchange(q);
-        return launch2(a, x_is_half ? (lut_mode() == 1 ? 2 : 1) : 0, true, q, st);
+        if (xc) {
+            q.xw_world = xc->world; q.xw_rank = xc->rank; q.xw_members = xc->members; q.xw_nfull = xc->out_features_full;
+            q.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
+            q.xw_out_off = xc->out_offset; q.xw_flag_off = xc->flag_offset; q.xw_state_off = xc->state_offset; q.xw_err_off = xc->error_offset;
+        }
+        // layers narrower than one strip keep the exact codebook in the fp16 table mode: their results do not depend on the mode
+        return launch2(a, x_is_half ? (lut_mode() == 1 && a->out_features >= STRIP ? 2 : 1) : 0, true, q, st);
     }
     Plan pl;
-    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, true, pl);
+    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, STAGE, pl);
     if (rc) return rc;
     if (!workspace || workspace_bytes < pl.ws_bytes)
         return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", pl.ws_bytes, workspace_bytes);
     Params p;
     memset(&p, 0, sizeof(p));
     p.ws_cnt = reinterpret_cast<int *>(ws + pl.ws_cnt_off);
-    p.ws_hyb_cnt = reinterpret_cast<int *>(ws + pl.ws_hybcnt_off);
     p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
     p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
     p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
-    p.ws_acc = reinterpret_cast<float *>(ws + pl.ws_acc_off);
-    p.det = det;
     p.x = x; p.x_is_half = x_is_half; p.out = y; p.y_is_half = y_is_half; p.bias = bias;
-    set_exchange(p);
-    return launch<true>(a, pl, p, st);
+    return launch(a, pl, p, st);
 }
 
 }  // namespace
@@ -1863,10 +1699,13 @@ size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int to
     Plan pl;
     if (bits != 3 && bits != 4) return 0;
     if (in_features <= 0 || in_features % 64 || out_features <= 0) return 0;
-    // CSR staging changes the shared-memory footprint, hence occupancy, grid and chunk: take the max of both plans.
+    // CSR staging changes the shared-memory footprint, hence occupancy, grid and chunk: take the max of both plans.  The
+    // deterministic mode gets exactly what its kernel needs.  The default mode plans with the CSR cols / vals alone in the staging
+    // buffer: less shared memory, at least as many CTAs and strip partials, so a workspace sized in either mode serves both.
+    const int stage = det_mode() == 1 ? STAGE : CSR_CH * 8;
     size_t b = 0;
     for (int csr = 0; csr < 2; ++csr)
-        if (make_plan(bits, in_features, out_features, topX, csr != 0, true, pl) == SQLLM_OK && pl.ws_bytes > b) b = pl.ws_bytes;
+        if (make_plan(bits, in_features, out_features, topX, csr != 0, stage, pl) == SQLLM_OK && pl.ws_bytes > b) b = pl.ws_bytes;
     return b;
 }
 
@@ -1876,24 +1715,12 @@ int sqllm_lutgemv(const sqllm_lutgemv_args *a, void *stream) {
     if (!a->vec || !a->mul) return fail(SQLLM_EINVAL, "vec / mul must not be null");
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch must be >= 1");
     if (reinterpret_cast<uintptr_t>(a->vec) & 15) return fail(SQLLM_EINVAL, "vec must be 16-byte aligned");
-    const bool hyb = a->full_rows && a->topX > 0;
     if (a->batch >= 2) return launch_batched(a, static_cast<cudaStream_t>(stream));
-    if (a->out_features >= STRIP) {
-        v2::P2 q;
-        memset(&q, 0, sizeof(q));
-        q.x = a->vec;
-        q.out = a->mul;
-        return launch2(a, 0, false, q, static_cast<cudaStream_t>(stream));
-    }
-    Plan pl;
-    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, false, pl);
-    if (rc) return rc;
-    Params p;
-    memset(&p, 0, sizeof(p));
-    p.x = a->vec;
-    p.out = a->mul;
-    p.x_is_half = 0;
-    return launch<false>(a, pl, p, static_cast<cudaStream_t>(stream));
+    v2::P2 q;
+    memset(&q, 0, sizeof(q));
+    q.x = a->vec;
+    q.out = a->mul;
+    return launch2(a, 0, false, q, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half,

@@ -134,7 +134,7 @@ def _every_mode(lib, L, pair_table=True, accumulate=True):
     yh = _fused(qc, T, xf.half())
     assert yh.dtype == torch.float16 and rel_err(yh.float().cpu().numpy(), want) < REL_TOL, "fused, fp16 x"
     if pair_table:
-        # layers narrower than one strip run the round-1 kernel, which has no pair table: they keep the exact codebook
+        # layers narrower than one strip keep the exact codebook in the fp16 table mode
         want16 = orc.forward_f64(_lut16(L), x, mul_init=L["bias"][None, :]) if L["outfeatures"] >= 64 else want
         assert rel_err(_pair_abi(lib, T, xf.half()), want16) < TIGHT_TOL, "fused, fp16 pair table"
     qc.set_deterministic(True)
@@ -162,13 +162,13 @@ def test_dense_rows_every_mode(lib, topx, pattern):
 @pytest.mark.parametrize("pattern", ["chan0", "one-strip", "edges", "mixed"])
 @pytest.mark.parametrize("topx", [1, 17, 33, 128])
 def test_dense_rows_narrow_layer_every_mode(lib, topx, pattern):
-    """N = 60 < 64: the round-1 kernel, its hybrid_totals (tp <= 16 split) in the deterministic mode."""
+    """N = 60 < 64: one ragged strip in every mode; in the deterministic mode the round-1 kernel's hybrid_totals (tp <= 16 split)."""
     _every_mode(lib, _layer(4, 512, 60, topx, pattern, sparsity=0.02, seed=topx + 500))
 
 
 @pytest.mark.parametrize("topx", [129, 256])
 def test_dense_rows_accumulate_symbols_beyond_the_fused_limit(topx):
-    """The 12 symbols have no topX limit of their own (v2 and, for N < 64, round 1)."""
+    """The 12 symbols have no topX limit of their own (v2, N < 64 included)."""
     from squeezellm_b200.quant import quant_cuda as qc
     for bits, K, N, pattern in ((4, 1024, 1000, "mixed"), (3, 512, 1000, "one-strip"), (4, 512, 60, "mixed")):
         L = _layer(bits, K, N, topx, pattern, seed=topx + N)
@@ -291,7 +291,7 @@ def _shifted(t, off):
     return v
 
 
-@pytest.mark.parametrize("N", [1000, 60], ids=["v2", "round1-narrow"])
+@pytest.mark.parametrize("N", [1000, 60], ids=["v2", "narrow"])
 def test_unaligned_outlier_arrays(lib, N):
     from squeezellm_b200.quant import quant_cuda as qc
     bits, K, topx = 4, 2048, 10

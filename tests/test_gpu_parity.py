@@ -38,7 +38,7 @@ SHAPES = [  # (bits, K, N, sparsity, topX, nonzero_full_rows, skew)
     (4, 4096, 12288, 0.0045, 10, True, True),   # 7B q+k+v stacked, skewed outliers
     (4, 256, 44032, 0.01, 4, True, False),      # more CSR rows per CTA than the shared row accumulator holds (mailbox fallback path)
     (3, 11008, 64, 0.01, 4, True, False),       # one strip, every CTA inside it: 147 mailbox rows for one owner
-    # narrower than one strip (out < 64): the round-1 kernel runs these in every mode, not only the deterministic one
+    # narrower than one strip (out < 64): a layer whose only strip is ragged
     (4, 256, 32, 0.02, 4, True, False),
     (3, 128, 60, 0.0, 0, False, False),
 ]

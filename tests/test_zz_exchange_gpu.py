@@ -13,7 +13,7 @@ FLAG, STATE, ERROR, DATA = 0, 64, 128, 4096
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("bits,K,w,members,sp,topx", [(4, 1024, 1024, 2, 0.01, 4), (3, 512, 256, 1, 0.0, 0), (4, 4096, 4096, 3, 0.0045, 10),
-                                                      (4, 256, 32, 1, 0.02, 4),  # narrower than one strip: the round-1 kernel's exchange
+                                                      (4, 256, 32, 1, 0.02, 4),  # narrower than one strip: one ragged strip
                                                       (3, 1024, 512, 3, 0.01, 40)],  # more than 32 dense rows: the general dense-row branch
                          ids=["w4-2x1024", "w3-1x256", "w4-qkv", "w4-1x32", "w3-3x512-t40"])
 def test_exchange_world1_matches_oracle_and_counts_arrivals(bits, K, w, members, sp, topx):
