@@ -1243,7 +1243,6 @@ int plan_layer(const sqllm_lutgemv_args &a, int sm, v2::P2 &p, int &G) {
     p.full_rows = hyb ? a.full_rows : nullptr;
     p.fri = hyb ? a.full_row_indices : nullptr;
     p.topX = hyb ? a.topX : 0;
-    p.csr_al16 = (a.rows && ((reinterpret_cast<uintptr_t>(a.cols) | reinterpret_cast<uintptr_t>(a.vals)) & 15) == 0) ? 1 : 0;
     p.K = K; p.N = N;
     p.R = a.bits == 4 ? K / 8 : K / 32;
     p.strips = (N + STRIP - 1) / STRIP;
@@ -1473,7 +1472,6 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         int rc = plan_layer(a, sm, p, G);
         if (rc) return seq_fail_free(s, rc);
         if (G > MAX_GRID_V2) return seq_fail_free(s, fail(SQLLM_EINVAL, "sequence: grid of %d CTAs exceeds the mailbox area", G));
-        if (a.rows && p.csr_rpc > v2::SP_ROWS) return seq_fail_free(s, fail(SQLLM_EINVAL, "sequence: item %d: %d outlier rows per CTA exceed %d", i, p.csr_rpc, v2::SP_ROWS));
         p.nstage = nst; p.smem_raw = raw;
         p.y_is_half = 1;
         p.bias = it.bias;

@@ -1,6 +1,6 @@
 // lutgemv_seq.cuh - the SEQUENCE kernel: one persistent launch runs a whole list of dependent LUT-GEMVs (a decode token's QuantLinear
 // matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Included by lutgemv_kernels.cu after lutgemv_v2.cuh;
-// the per-position math, table builders, outlier warps and mailboxes are v2's (namespace v2), what is new is everything BETWEEN two GEMVs.
+// the per-position math, table builders, outlier warps (sparse3) and mailboxes are v2's (namespace v2), what is new is everything BETWEEN two GEMVs.
 //
 // Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
 // carries a fixed cost (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
@@ -83,168 +83,6 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
     }
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// Outlier warps of the sequence kernel.  v2::sparse2 stages the (col, val) chunks in shared memory, forms the products in place and sums
-// rows from there: four or more DEPENDENT shared-memory round trips per chunk, each queueing for hundreds of cycles behind the consumers'
-// gathers (the LSU is what bounds the kernel) - the timeline of a 4096x4096 layer showed the outlier warps finishing well after x arrived
-// and after the last consumer warp: they, not the weights, set the layer's critical path
-// (tests/perf/seq_trace.cu).  Here nothing but x goes through shared memory:
-//   * LPR lanes share a row (LPR from the average row length), 32 / LPR rows per pass; a lane keeps its <= 8 (col, val) pairs of the
-//     pass in REGISTERS, loaded straight from global memory (L2: prefetched at entry) - everything static, so the first pass is in
-//     registers before x arrives and the loads of pass k+1 are issued before pass k is summed;
-//   * after x: one round of x gathers (the only shared-memory accesses), FMAs, a shuffle tree over the LPR lanes, and ONE 64-bit tagged
-//     store of the row sum into the row's mailbox word (rows without outliers store 0: the strip's owner waits for all its rows);
-//   * the part of a row beyond 8 x LPR elements is summed by the whole warp (skewed rows).
-// Dense rows (topX): as in v2 (the CTA's k-slice, requested before x arrives, red.add + one announcement per strip).
-// ---------------------------------------------------------------------------------------------------------------------------
-template <bool XH>
-__device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const int spw, const int lane, const uint32_t boxtag) {
-    const int N = p.N;
-    const uint32_t xs_u32 = base + OFF_X;
-    // ---------------- static: dense-row slice ----------------
-    float hfr[HYB_R2];
-    const bool hyb_on = p.full_rows && spw == 0 && (int)blockIdx.x < p.hc;
-    const bool hyb_multi = hyb_on && p.topX <= 32;
-    int kb = 0, ke = 0, nsl = 1, rs = 0, hj = lane;
-    if (hyb_on) { kb = blockIdx.x * p.hrows; ke = min(p.K, kb + p.hrows); }
-    if (hyb_multi) {
-        nsl = 32 / p.topX;
-        rs = lane / p.topX;
-        hj = lane - rs * p.topX;
-#pragma unroll
-        for (int i = 0; i < HYB_R2; ++i) {
-            const int k = kb + rs + nsl * i;
-            hfr[i] = (rs < nsl && k < ke) ? __ldg(p.full_rows + (size_t)k * p.topX + hj) : 0.f;
-        }
-    }
-    // ---------------- static: this warp's CSR rows [r, rb) of the CTA's [ca, cb) ----------------
-    int r = 0, rb = 0;
-    if (p.rows) {
-        const int ca = min(N, (int)blockIdx.x * p.csr_rpc), cb = min(N, ca + p.csr_rpc);
-        // warp 0 has the dense rows (atomics + a fence before its announcement) and then takes no CSR rows: outlier sums are what
-        // the owners of ALL strips wait for, they must not queue behind that fence
-        const int tot = cb - ca, w0 = p.full_rows ? 0 : tot / NSPW, rest = tot - w0;
-        r = spw == 0 ? ca : ca + w0 + (int)((long long)rest * (spw - 1) / (NSPW - 1));
-        rb = spw == 0 ? ca + w0 : ca + w0 + (int)((long long)rest * spw / (NSPW - 1));
-    }
-    const int nr = rb - r;
-    int LPR = 4;
-    if (nr > 0) {
-        const int e_lo = __ldg(p.rows + r), e_hi = __ldg(p.rows + rb);
-        const int avg = (e_hi - e_lo) / nr;
-        LPR = avg > 128 ? 32 : avg > 64 ? 16 : avg > 32 ? 8 : avg > 8 ? 4 : 2;
-    }
-    const int RPP = 32 / LPR, part = lane & (LPR - 1), rslot = lane / LPR;
-    const int npass = (nr + RPP - 1) / RPP;
-    constexpr int T = 8;  // (col, val) pairs per lane and pass
-    auto load_ptrs = [&](int pass, int &a0, int &a1) {
-        const int row = r + pass * RPP + rslot;
-        a0 = a1 = 0;
-        if (pass < npass && row < rb) { a0 = __ldg(p.rows + row); a1 = __ldg(p.rows + row + 1); }
-    };
-    auto load_elems = [&](int a0, int a1, int (&cc)[T], float (&vv)[T]) {
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-            const int e = a0 + part + t * LPR;
-            const bool ok = e < a1;
-            cc[t] = ok ? __ldg(p.cols + e) : 0;
-            vv[t] = ok ? __ldg(p.vals + e) : 0.f;
-        }
-    };
-    int a0c, a1c, a0n, a1n, a0nn, a1nn;
-    int cc[T], cn[T];
-    float vv[T], vn[T];
-    load_ptrs(0, a0c, a1c);
-    load_ptrs(1, a0n, a1n);
-    load_elems(a0c, a1c, cc, vv);
-
-    named_bar_sync(2, NCT + NSPW * 32);  // x is in shared memory
-
-    // ---------------- dense rows (v2's phase B) ----------------
-    if (hyb_on) {
-        for (int jb = 0; jb < (hyb_multi ? 1 : p.topX); jb += 32) {
-            float a = 0.f;
-            int j;
-            if (hyb_multi) {
-                j = hj;
-#pragma unroll
-                for (int i = 0; i < HYB_R2; ++i) {
-                    const int k = kb + rs + nsl * i;
-                    if (rs < nsl && k < ke) a += hfr[i] * xs_load<XH>(xs_u32, k);
-                }
-                for (int k = kb + rs + nsl * HYB_R2; rs < nsl && k < ke; k += nsl)
-                    a += __ldg(p.full_rows + (size_t)k * p.topX + hj) * xs_load<XH>(xs_u32, k);
-                for (int sl = 1; sl < nsl; ++sl) {
-                    const float v = __shfl_sync(0xffffffffu, a, (hj + sl * p.topX) & 31);
-                    if (rs == 0) a += v;
-                }
-                if (rs != 0) j = p.topX;
-                // dense rows that feed the SAME channel travel as one word (the first of them carries the sum): the owner of that channel's
-                // strip then reads hc words, not hc per row - a checkpoint without dense rows loads as topX rows on channel 0 (llama.py:182)
-                {
-                    const int cme = (rs == 0 && hj < p.topX) ? __ldg(p.fri + hj) : -1 - lane;
-                    bool first = true;
-                    float tot = a;
-                    for (int j2 = 0; j2 < p.topX; ++j2) {
-                        const int c2 = __shfl_sync(0xffffffffu, cme, j2);
-                        const float a2 = __shfl_sync(0xffffffffu, a, j2);
-                        if (c2 == cme && j2 < hj) first = false;
-                        if (c2 == cme && j2 > hj) tot += a2;
-                    }
-                    a = tot;
-                    if (!first) j = p.topX;
-                }
-            } else {
-                j = jb + lane;
-                if (j < p.topX) {
-                    const float *fr = p.full_rows + (size_t)kb * p.topX + j;
-                    for (int k = kb; k < ke; ++k, fr += p.topX) a += __ldg(fr) * xs_load<XH>(xs_u32, k);
-                }
-            }
-            // this CTA's part of dense row j: one tagged word, no fence, no flag (the owner of the channel's strip sums the hc words of row j)
-            if (j < p.topX) st_relaxed_u64(p.ws_dbox + (size_t)j * MAX_GRID_V2 + blockIdx.x, box_word(a, boxtag));
-        }
-    }
-    // ---------------- CSR passes ----------------
-    for (int pass = 0; pass < npass; ++pass) {
-        load_ptrs(pass + 2, a0nn, a1nn);
-        load_elems(a0n, a1n, cn, vn);
-        float s0 = 0.f, s1 = 0.f;
-        {
-            float xv[T];
-#pragma unroll
-            for (int t = 0; t < T; ++t) xv[t] = xs_load<XH>(xs_u32, cc[t]);   // (padding slots read x[0] with val 0)
-#pragma unroll
-            for (int t = 0; t < T; t += 2) { s0 = fmaf(vv[t], xv[t], s0); s1 = fmaf(vv[t + 1], xv[t + 1], s1); }
-        }
-        float tot = s0 + s1;
-        for (int d = 1; d < LPR; d <<= 1) tot += __shfl_xor_sync(0xffffffffu, tot, d);
-        // rows longer than T * LPR: the whole warp sums the remainder, row after row
-        unsigned longm = __ballot_sync(0xffffffffu, part == 0 && a1c - a0c > T * LPR);
-        while (longm) {
-            const int i = __ffs(longm) - 1;
-            longm &= longm - 1;
-            const int b0 = __shfl_sync(0xffffffffu, a0c, i) + T * LPR, b1 = __shfl_sync(0xffffffffu, a1c, i);
-            float a = 0.f, b = 0.f;
-            for (int e = b0 + lane; e < b1; e += 128) {
-                const int c0 = __ldg(p.cols + e), c1 = e + 32 < b1 ? __ldg(p.cols + e + 32) : 0, c2 = e + 64 < b1 ? __ldg(p.cols + e + 64) : 0,
-                          c3 = e + 96 < b1 ? __ldg(p.cols + e + 96) : 0;
-                const float v0 = __ldg(p.vals + e), v1 = e + 32 < b1 ? __ldg(p.vals + e + 32) : 0.f, v2 = e + 64 < b1 ? __ldg(p.vals + e + 64) : 0.f,
-                            v3 = e + 96 < b1 ? __ldg(p.vals + e + 96) : 0.f;
-                a = fmaf(v0, xs_load<XH>(xs_u32, c0), a); b = fmaf(v1, xs_load<XH>(xs_u32, c1), b);
-                a = fmaf(v2, xs_load<XH>(xs_u32, c2), a); b = fmaf(v3, xs_load<XH>(xs_u32, c3), b);
-            }
-            a = warp_sum(a + b);
-            if (lane == i) tot += a;
-        }
-        const int row = r + pass * RPP + rslot;
-        if (part == 0 && row < rb) st_relaxed_u64(p.ws_cbox + row, box_word(tot, boxtag));
-        a0c = a0n; a1c = a1n; a0n = a0nn; a1n = a1nn;
-#pragma unroll
-        for (int t = 0; t < T; ++t) { cc[t] = cn[t]; vv[t] = vn[t]; }
-    }
-}
 
 template <int BITS, int MODE, bool MULTI>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c) {
@@ -348,10 +186,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             }
         }
     } else if (warp >= WARP_SP) {
-        // =========================== outlier warps (v2::sparse2, once per GEMV) ===========================
+        // =========================== outlier warps (v2::sparse3, once per GEMV) ===========================
         for (int g = 0; g < ngemv; ++g) {
             const P2 &p = c.descs[g].p;
-            sparse3<XH>(p, base, warp - WARP_SP, lane, (epoch << 10) | (uint32_t)(g + 1));
+            sparse3<XH, true>(p, base, warp - WARP_SP, lane, nullptr, (epoch << 10) | (uint32_t)(g + 1));
             TRACE(10, lane == 0);
             if (g + 1 < ngemv) bar_arrive(6, NCT + NSPW * 32);  // done reading this GEMV's x from shared memory
         }
@@ -382,8 +220,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             // and then they never leave the SM: sown[u][column] for the u-th owned strip (a strip inside one CTA is exactly one segment).
             // (v2 and the first sequence build sent them through the global accumulator - a RED and, in the finishing pass, a load that has to
             // wait for it: L2 round trips on the critical path between the last weight and y.)
-            const uint32_t sown = base + OFF_SROW;  // float [SOWN][64] (the row arrays of v2's outlier warps are not used by the sequence kernel)
-            constexpr int SOWN = (2 * (SP_ROWS + 1) * 4) / (STRIP * 4);
+            const uint32_t sown = base + OFF_FIN;   // float [SOWN][64], as in lutgemv2_kernel
+            constexpr int SOWN = 8;
             const int ofs = r0 != 0 ? 1 : 0;        // segment s is owned strip s - ofs
             auto flush = [&](int s) {
                 const uint32_t a = sacc_of(s);
@@ -424,8 +262,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             const int lidx = last_owned && nseg > 0 ? nown - 1 : -1;
             const int nh = lidx >= 0 ? (int)((((long long)(so1 - 1) + 1) * R - 1) / p.chunk) - (int)blockIdx.x : 0;
             // Dense rows whose channel lies in a strip we own: listed now (static), summed below.  sdj[i] = dense row, sden[i] = its sum.
-            int *const sdj = reinterpret_cast<int *>(sm + OFF_CSR);
-            const uint32_t sden = base + OFF_CSR + 4 * 128, sdn_a = base + OFF_CSR + 8 * 128;
+            int *const sdj = reinterpret_cast<int *>(sm + OFF_FIN + 2048);
+            const uint32_t sden = base + OFF_FIN + 2048 + 4 * 128, sdn_a = base + OFF_FIN + 2048 + 8 * 128;
             if (p.full_rows) {
                 // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads for the 30
                 //  dense rows of a stacked q/k/v layer - on every CTA, before its first mailbox row went out)

@@ -17,7 +17,8 @@
 //   * fp16 PAIR table (MODE 1): entry [a | b<<BITS] = half2(LUT[a], LUT[b]) - one PRMT-built (4-bit: the byte of the packed word IS
 //     the entry number) shared-memory lookup serves TWO weights, and the products are fp16 x fp16 -> fp32 accumulate with
 //     exact products (fhfma2; tests/perf/microbench2.cu measures the loop).  The only rounding is LUT -> fp16 (2^-11 relative per centroid); it needs fp16 x.
-//   * x is staged whole (as fp16 when it is given as fp16), the sparse warps gather it from shared memory.
+//   * x is staged whole (as fp16 when it is given as fp16), the sparse warps gather it from shared memory (sparse3: nothing else of
+//     theirs goes through shared memory).
 #pragma once
 
 namespace v2 {
@@ -34,17 +35,12 @@ constexpr int NCT = NWC * 32;                   // consumer threads
 constexpr int NBT = NBW * 32;                   // builder threads: one per column slot of a strip
 constexpr int SU2 = 2 * NWC;                    // units per stage (one pair per consumer warp)
 constexpr int MAXD = 16;                        // ring depth limit (mbarrier slots)
-constexpr int SP_CH = 256;                      // sparse warp: non-zeros per staged chunk (two chunk buffers per warp)
-constexpr int SP_ROWS = 255;                    // owned rows whose pointers / sums are kept in shared memory (CTA-wide)
-constexpr int SP_BYTES = 2 * SP_CH * 8;         // per sparse warp: 2 x (cols + vals) = 4 KB
 constexpr int HYB_R2 = 11;
 static_assert(NBT == STRIP, "one builder thread per column of a strip");
 // shared-memory carve-up, offsets from a 128-byte aligned base
 constexpr int OFF_BAR = 0;                      // full[s] at +8s, empty[s] at +128+8s, tfull[b] at +256+8b, tfree[b] at +272+8b
 constexpr int OFF_SACC = 512;                   // float [2][64]: per-strip sums of the consumer warps (red.shared.add), ping-pong by strip parity
-constexpr int OFF_CSR = OFF_SACC + 2 * STRIP * 4;            // per sparse warp: 2 x {int cols[SP_CH], float vals[SP_CH]}
-constexpr int OFF_SROW = OFF_CSR + NSPW * SP_BYTES;          // CTA-wide: int srow[SP_ROWS + 1], float srowacc[SP_ROWS + 1]
-constexpr int OFF_LUT = OFF_SROW + 2 * (SP_ROWS + 1) * 4;        // 2 x raw fp32 LUT rows of a strip (64 columns x 16 values), staged ahead by the builders
+constexpr int OFF_LUT = OFF_SACC + 2 * STRIP * 4;            // 2 x raw fp32 LUT rows of a strip (64 columns x 16 values), staged ahead by the builders
 constexpr int LUTBUF = STRIP * (16 * 4 + 16);                // a strip's raw LUT rows, one per column SLOT, row stride L*4 + 16 bytes (see lut_prefetch)
 constexpr int OFF_FIN = OFF_LUT + 2 * LUTBUF;                // finishers: float sown[8][64] (own strip sums), int sdj[128], float sden[128], int sdn (dense rows)
 constexpr int OFF_X = OFF_FIN + 4096;                        // x (fp16 or fp32), then [ring stages][table 0][table 1][ring stages]
@@ -63,7 +59,7 @@ struct P2 {
     int topX, K, N, R, T, chunk, nstage;
     unsigned smem_raw;   // shared-window address of the dynamic shared memory the host planned the carve-up for (checked by the kernel)
     int y_is_half;
-    int hc, hrows, csr_rpc, csr_al16;
+    int hc, hrows, csr_rpc;
     float *ws_acc;       // fused: [N] fp32 accumulator, zero between launches
     unsigned long long *ws_hbox;  // fused: [grid][64] partial strip sums of a CTA's first segment when the strip starts in an earlier CTA
     unsigned long long *ws_cbox;  // fused: [N] outlier (CSR) row sums; both {float value, u32 valid}, all zero between launches
@@ -380,10 +376,24 @@ __device__ __forceinline__ void math2(const Fetch<BITS, XH> &F, const int jsel, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// Sparse warp(s) (NSPW per CTA).  CSR rows (= output channels) are spread evenly over the CTAs (csr_rpc consecutive rows each, split
-// between the CTA's sparse warps); warp 0 also takes the CTA's k-slice of the topX dense rows.  Everything static (row pointers, the
-// first cols/vals group, dense-row values) is requested before the x barrier; x comes from shared memory.  Per-row sums are taken in
-// storage order; results go out as one red.add per row (accumulate mode) or as mailbox words (fused mode).
+// Outlier warps (NSPW per CTA), shared by lutgemv2_kernel and the sequence kernel.  CSR rows (= output channels) are spread evenly over
+// the CTAs (csr_rpc consecutive rows each, split between the CTA's sparse warps); warp 0 also takes the CTA's k-slice of the topX dense
+// rows.  Nothing but x goes through shared memory: the LSU pipe is what bounds the kernel, so every dependent shared-memory access of
+// these warps queues for hundreds of cycles behind the consumers' gathers.  (Before: the (col, val) pairs were staged in 256-element
+// chunks with cp.async, the products formed in place and the rows summed from there - four or more dependent shared-memory round trips
+// per chunk; on a 4096x4096 layer the outlier warps finished after the last consumer warp and set the layer's critical path,
+// tests/perf/seq_trace.cu.)  Here:
+//   * LPR lanes share a row (LPR from the average row length), 32 / LPR rows per pass; a lane keeps its <= T (col, val) pairs of the
+//     pass in REGISTERS, loaded straight from global memory (the warp's whole non-zero range is prefetched into L2 at entry) -
+//     everything static, so the first pass is in registers before x arrives and the loads of pass k+1 are issued before pass k is summed;
+//   * after x: one round of x gathers (the only shared-memory accesses), FMAs, a shuffle tree over the LPR lanes, and one result per
+//     row: a 64-bit mailbox word {sum, boxtag} (fused mode; rows without outliers store 0: the strip's owner waits for all its rows) or
+//     one red.add into `acc_out` (accumulate mode: the 12 symbols);
+//   * the part of a row beyond T x LPR elements is summed by the whole warp (skewed rows).
+// `boxtag` is 1 for the one-GEMV kernel (the owner resets the words) and the (token, GEMV) tag for the sequence kernel (box_word).
+// Dense rows: this CTA's k-slice of full_rows, prefetched into L2 at entry, the first HYB_R2 per row slot in registers before x arrives
+// (the rest is read after x: from L2, not from HBM - every owner of a dense-row channel waits for the slowest CTA's warp 0); one mailbox word per
+// (CTA, dense row), rows on the same channel combined (fused), or one red.add per dense row into its channel (accumulate).
 // ---------------------------------------------------------------------------------------------------------------------------
 template <bool XH>
 __device__ __forceinline__ float xs_load(const uint32_t xs_u32, const int k) {
@@ -397,19 +407,20 @@ __device__ __forceinline__ float xs_load(const uint32_t xs_u32, const int k) {
 }
 
 template <bool XH, bool FUSED>
-__device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const uint32_t base, const int spw, const int lane, float *acc_out, const uint32_t boxtag = 1u) {
+__device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const int spw, const int lane, float *acc_out, const uint32_t boxtag) {
     const int N = p.N;
     const uint32_t xs_u32 = base + OFF_X;
-    const uint32_t stage_u32 = base + OFF_CSR + spw * SP_BYTES;       // this warp's chunk buffer b: cols at +b*SP_CH*8, vals SP_CH*4 further
-    int *srow = reinterpret_cast<int *>(sm + OFF_SROW);               // [SP_ROWS + 1] row pointers of the CTA's rows (FUSED, when they fit)
-    float *srowacc = reinterpret_cast<float *>(srow + SP_ROWS + 1);   // [SP_ROWS + 1] their outlier sums, picked up by the builders
-
-    // ---------------- phase A: static data ----------------
+    // ---------------- static: dense-row slice ----------------
     float hfr[HYB_R2];
     const bool hyb_on = p.full_rows && spw == 0 && (int)blockIdx.x < p.hc;
     const bool hyb_multi = hyb_on && p.topX <= 32;  // 32/topX k-rows per warp step: lane = (row slot, column j)
     int kb = 0, ke = 0, nsl = 1, rs = 0, hj = lane;
-    if (hyb_on) { kb = blockIdx.x * p.hrows; ke = min(p.K, kb + p.hrows); }
+    if (hyb_on) {
+        kb = blockIdx.x * p.hrows; ke = min(p.K, kb + p.hrows);
+        // the slice is contiguous ([kb, ke) x topX floats): into L2 now, so that the rows read after x arrives are L2 hits
+        const char *f0 = reinterpret_cast<const char *>(p.full_rows + (size_t)kb * p.topX);
+        for (int i = lane; i < (int)(((size_t)(ke - kb) * p.topX * 4 + 127) / 128); i += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(f0 + 128 * i));
+    }
     if (hyb_multi) {
         nsl = 32 / p.topX;
         rs = lane / p.topX;
@@ -420,78 +431,54 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
             hfr[i] = (rs < nsl && k < ke) ? __ldg(p.full_rows + (size_t)k * p.topX + hj) : 0.f;
         }
     }
-    // This CTA's CSR rows [ca, cb): csr_rpc consecutive rows, the same share for every CTA, whichever strips they fall in.  Accumulate mode
-    // (the 12 symbols) adds each row sum into `mul` with one red.add; fused mode publishes it as a mailbox word that the owner of the row's
-    // strip (the CTA in whose range the strip starts) collects when it writes y.  The rows are split over the NSPW sparse warps.
-    int ca = 0, cb = 0;
+    // ---------------- static: this warp's CSR rows [r, rb) of the CTA's [ca, cb) ----------------
+    int r = 0, rb = 0;
     if (p.rows) {
-        ca = min(N, (int)blockIdx.x * p.csr_rpc);
-        cb = min(N, ca + p.csr_rpc);
-    }
-    int r, rb;
-    {
-        // warp 0 also has the dense rows; when there are any it takes no CSR rows: the outlier sums are what the owners of ALL strips
-        // wait for, they must not queue behind the dense-row work
+        const int ca = min(N, (int)blockIdx.x * p.csr_rpc), cb = min(N, ca + p.csr_rpc);
+        // warp 0 has the dense rows and then takes no CSR rows: the outlier sums are what the owners of ALL strips wait for, they must
+        // not queue behind the dense-row work
         const int tot = cb - ca, w0 = p.full_rows ? 0 : tot / NSPW, rest = tot - w0;
         r = spw == 0 ? ca : ca + w0 + (int)((long long)rest * (spw - 1) / (NSPW - 1));
         rb = spw == 0 ? ca + w0 : ca + w0 + (int)((long long)rest * spw / (NSPW - 1));
     }
     const int nr = rb - r;
-    const bool rows_in_smem = cb - ca <= SP_ROWS;      // the CTA's row pointers live in shared memory
-    const bool smem_sums = FUSED && rows_in_smem;      // ... and so do the row sums, published as mailbox words when the warp is through
-    auto emit = [&](int row, float v) {
-        if (smem_sums) srowacc[row - ca] += v;  // plain read-modify-write: a row belongs to this warp alone and its pieces arrive one after the other
-        else if (FUSED) atomicAdd(reinterpret_cast<float *>(p.ws_cbox + row), v);  // (more rows per CTA than the shared accumulator holds: value half of the word)
-        else atomicAdd(acc_out + row, v);
-    };
-    int e_lo = 0, e_hi = 0;
+    int LPR = 4;
     if (nr > 0) {
-        if (rows_in_smem)
-            for (int i = lane; i <= nr; i += 32) {
-                srow[r - ca + i] = __ldg(p.rows + r + i);   // (the boundary entry is written by both neighbours, with the same value)
-                if (i < nr) srowacc[r - ca + i] = 0.f;
-            }
-        e_lo = __ldg(p.rows + r);
-        e_hi = __ldg(p.rows + rb);
-    }
-    // This warp's non-zeros [e_lo, e_hi) go to L2 right away (a CTA has ~5-25 KB of outliers and only two small chunks per warp fit the
-    // staging buffers: under a saturated HBM every further chunk would otherwise cost a DRAM round trip), and are then walked
-    // in chunks of SP_CH staged with 16-byte cp.async into two buffers.  Shared-memory accesses of these warps queue behind the
-    // consumers' (the LSU pipe is what bounds the kernel), i.e. each dependent access costs hundreds of cycles: that is why there are
-    // NSPW warps with independent chains (one warp alone sets the critical path) and why every step below batches independent loads.
-    for (int e = (e_lo & ~31) + 32 * lane; e < e_hi; e += 32 * 32) {
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.cols + e));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.vals + e));
-    }
-    const bool al16 = p.csr_al16 != 0;
-    const int c_lo = al16 ? (e_lo & ~3) : e_lo;  // chunk grid: 16-byte aligned element index when the arrays are
-    auto stage_chunk = [&](int ci) {              // chunk ci covers elements [c_lo + ci*SP_CH, +SP_CH) -> buffer ci & 1
-        const int t0 = c_lo + ci * SP_CH;
-        const uint32_t dc = stage_u32 + (ci & 1) * (SP_CH * 8), dv = dc + SP_CH * 4;
-        if (t0 < e_hi) {
-            if (al16) {
-                for (int e = 4 * lane; e < SP_CH; e += 128) {
-                    const int nb = min(16, 4 * (e_hi - (t0 + e)));  // the last quad is clipped with the src-size operand: nothing past e_hi is read
-                    if (nb > 0) {
-                        cp_async16_clip(dc + 4 * e, p.cols + t0 + e, nb);
-                        cp_async16_clip(dv + 4 * e, p.vals + t0 + e, nb);
-                    }
-                }
-            } else {
-                for (int e = lane; e < SP_CH && t0 + e < e_hi; e += 32) {
-                    cp_async4(dc + 4 * e, p.cols + t0 + e);
-                    cp_async4(dv + 4 * e, p.vals + t0 + e);
-                }
-            }
+        const int e_lo = __ldg(p.rows + r), e_hi = __ldg(p.rows + rb);
+        for (int e = (e_lo & ~31) + 32 * lane; e < e_hi; e += 32 * 32) {
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(p.cols + e));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(p.vals + e));
         }
-        cp_async_commit();  // exactly one group per chunk, empty or not
+        const int avg = (e_hi - e_lo) / nr;
+        LPR = avg > 128 ? 32 : avg > 64 ? 16 : avg > 32 ? 8 : avg > 8 ? 4 : 2;
+    }
+    const int RPP = 32 / LPR, part = lane & (LPR - 1), rslot = lane / LPR;
+    const int npass = (nr + RPP - 1) / RPP;
+    constexpr int T = 8;  // (col, val) pairs per lane and pass
+    auto load_ptrs = [&](int pass, int &a0, int &a1) {
+        const int row = r + pass * RPP + rslot;
+        a0 = a1 = 0;
+        if (pass < npass && row < rb) { a0 = __ldg(p.rows + row); a1 = __ldg(p.rows + row + 1); }
     };
-    stage_chunk(0);
-    stage_chunk(1);
+    auto load_elems = [&](int a0, int a1, int (&cc)[T], float (&vv)[T]) {
+#pragma unroll
+        for (int t = 0; t < T; ++t) {
+            const int e = a0 + part + t * LPR;
+            const bool ok = e < a1;
+            cc[t] = ok ? __ldg(p.cols + e) : 0;
+            vv[t] = ok ? __ldg(p.vals + e) : 0.f;
+        }
+    };
+    int a0c, a1c, a0n, a1n, a0nn, a1nn;
+    int cc[T], cn[T];
+    float vv[T], vn[T];
+    load_ptrs(0, a0c, a1c);
+    load_ptrs(1, a0n, a1n);
+    load_elems(a0c, a1c, cc, vv);
 
     named_bar_sync(2, NCT + NSPW * 32);  // x is in shared memory (and the previous kernel has completed: the consumers waited on it)
 
-    // ---------------- phase B ----------------
+    // ---------------- dense rows ----------------
     if (hyb_on) {
         for (int jb = 0; jb < (hyb_multi ? 1 : p.topX); jb += 32) {
             float a = 0.f;
@@ -533,95 +520,58 @@ __device__ __forceinline__ void sparse2(const P2 &p, unsigned char *sm, const ui
                 }
             }
             if constexpr (FUSED) {
-                // this CTA's part of dense row j: one self-validating word, no RED + fence + flag (the owner of the channel's strip sums the hc words of
-                // row j, lutgemv2_kernel's finishers); before: atomics into the accumulator, a MEMBAR.GPU and an announcement per strip - the fence
-                // alone held this warp, and with it every owner that waited for the announcement
-                if (j < p.topX) st_relaxed_u64(p.ws_dbox + (size_t)j * MAX_GRID_V2 + blockIdx.x, box_word(a));
+                // this CTA's part of dense row j: one self-validating word, no RED + fence + flag (the owner of the channel's strip sums the
+                // hc words of row j, the finishers of lutgemv2_kernel / lutgemv_seq_kernel)
+                if (j < p.topX) st_relaxed_u64(p.ws_dbox + (size_t)j * MAX_GRID_V2 + blockIdx.x, box_word(a, boxtag));
             } else if (j < p.topX) {
                 const int c = __ldg(p.fri + j);
                 if (c >= 0 && c < N) atomicAdd(acc_out + c, a);
             }
         }
     }
-    int rcur = r;  // first row that still has non-zeros at or after the current chunk
-    const int avg = nr > 0 ? (e_hi - e_lo) / nr : 0;
-    const int LPR = avg > 32 ? 8 : avg > 12 ? 4 : avg > 5 ? 2 : 1;  // lanes per row (power of two)
-    for (int ci = 0; c_lo + ci * SP_CH < e_hi; ++ci) {
-        const int t0 = c_lo + ci * SP_CH, t1 = min(t0 + SP_CH, e_hi), f0 = max(t0, e_lo);
-        const int *scols = reinterpret_cast<const int *>(sm + OFF_CSR + spw * SP_BYTES + (ci & 1) * (SP_CH * 8));
-        float *svals = reinterpret_cast<float *>(sm + OFF_CSR + spw * SP_BYTES + (ci & 1) * (SP_CH * 8) + SP_CH * 4);
-        cp_async_wait_pending<1>();  // all but the newest group have landed: this chunk is there
-        __syncwarp();
-        // products in place: all (col, val) loads of a trip first, then the x gathers, then the stores
-        for (int e0 = f0 - t0 + lane; e0 < t1 - t0; e0 += 256) {
-            int cc[8];
-            float xv[8], vv[8];
+    // ---------------- CSR passes ----------------
+    for (int pass = 0; pass < npass; ++pass) {
+        load_ptrs(pass + 2, a0nn, a1nn);
+        load_elems(a0n, a1n, cn, vn);
+        float s0 = 0.f, s1 = 0.f;
+        {
+            float xv[T];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const bool ok = e0 + 32 * j < t1 - t0;
-                cc[j] = ok ? scols[e0 + 32 * j] : 0;
-                vv[j] = ok ? svals[e0 + 32 * j] : 0.f;
-            }
+            for (int t = 0; t < T; ++t) xv[t] = a0c + part + t * LPR < a1c ? xs_load<XH>(xs_u32, cc[t]) : 0.f;  // (padding: no gather)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) xv[j] = xs_load<XH>(xs_u32, cc[j]);
+            for (int t = 0; t < T; t += 2) { s0 = fmaf(vv[t], xv[t], s0); s1 = fmaf(vv[t + 1], xv[t + 1], s1); }
+        }
+        float tot = s0 + s1;
+        for (int d = 1; d < LPR; d <<= 1) tot += __shfl_xor_sync(0xffffffffu, tot, d);
+        // rows longer than T * LPR: the whole warp sums the remainder, row after row
+        unsigned longm = __ballot_sync(0xffffffffu, part == 0 && a1c - a0c > T * LPR);
+        while (longm) {
+            const int i = __ffs(longm) - 1;
+            longm &= longm - 1;
+            const int b0 = __shfl_sync(0xffffffffu, a0c, i) + T * LPR, b1 = __shfl_sync(0xffffffffu, a1c, i);
+            float a = 0.f, b = 0.f;
+            for (int e = b0 + lane; e < b1; e += 128) {
+                const int c0 = __ldg(p.cols + e), c1 = e + 32 < b1 ? __ldg(p.cols + e + 32) : 0, c2 = e + 64 < b1 ? __ldg(p.cols + e + 64) : 0,
+                          c3 = e + 96 < b1 ? __ldg(p.cols + e + 96) : 0;
+                const float v0 = __ldg(p.vals + e), v1 = e + 32 < b1 ? __ldg(p.vals + e + 32) : 0.f, v2 = e + 64 < b1 ? __ldg(p.vals + e + 64) : 0.f,
+                            v3 = e + 96 < b1 ? __ldg(p.vals + e + 96) : 0.f;
+                a = fmaf(v0, xs_load<XH>(xs_u32, c0), a);
+                if (e + 32 < b1) b = fmaf(v1, xs_load<XH>(xs_u32, c1), b);
+                if (e + 64 < b1) a = fmaf(v2, xs_load<XH>(xs_u32, c2), a);
+                if (e + 96 < b1) b = fmaf(v3, xs_load<XH>(xs_u32, c3), b);
+            }
+            a = warp_sum(a + b);
+            if (lane == i) tot += a;
+        }
+        const int row = r + pass * RPP + rslot;
+        if constexpr (FUSED) {
+            if (part == 0 && row < rb) st_relaxed_u64(p.ws_cbox + row, box_word(tot, boxtag));
+        } else {
+            if (part == 0 && row < rb && a1c > a0c) atomicAdd(acc_out + row, tot);
+        }
+        a0c = a0n; a1c = a1n; a0n = a0nn; a1n = a1nn;
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (e0 + 32 * j < t1 - t0) svals[e0 + 32 * j] = vv[j] * xv[j];
-        }
-        __syncwarp();
-        // rows that intersect [f0, t1), 32 / LPR at a time from rcur: LPR lanes share a row (lane part p takes elements p, p + LPR, ...
-        // of the row's piece, four independent loads per trip), their partial sums are folded with shuffles and the row's piece is
-        // added to its sum (a row that straddles chunks arrives in pieces).  LPR grows with the average row length: a dependent
-        // shared-memory trip costs this warp hundreds of cycles, a 50-element row summed by one lane would be 13 of them.
-        while (true) {
-            const int row = rcur + lane / LPR, part = lane & (LPR - 1);
-            int a0 = e_hi, a1 = e_hi;
-            if (row < rb) {
-                a0 = rows_in_smem ? srow[row - ca] : __ldg(p.rows + row);
-                a1 = rows_in_smem ? srow[row - ca + 1] : __ldg(p.rows + row + 1);
-            }
-            const bool inter = row < rb && a0 < t1;
-            const int s0 = max(a0, f0) - t0, s1 = min(a1, t1) - t0;
-            const int n = inter ? s1 - s0 : 0;
-            float ea = 0.f, eb = 0.f, ec = 0.f, ed = 0.f;
-            if (n > 0 && n <= 64 * LPR) {
-                for (int e = s0 + part; e < s1; e += 4 * LPR) {  // four independent (predicated) loads per trip
-                    const float q0 = svals[e];
-                    const float q1 = e + LPR < s1 ? svals[e + LPR] : 0.f;
-                    const float q2 = e + 2 * LPR < s1 ? svals[e + 2 * LPR] : 0.f;
-                    const float q3 = e + 3 * LPR < s1 ? svals[e + 3 * LPR] : 0.f;
-                    ea += q0; eb += q1; ec += q2; ed += q3;
-                }
-            }
-            float tot = (ea + eb) + (ec + ed);
-            for (int d = 1; d < LPR; d <<= 1) tot += __shfl_xor_sync(0xffffffffu, tot, d);
-            if (part == 0 && n > 0 && n <= 64 * LPR) emit(row, tot);
-            unsigned longm = __ballot_sync(0xffffffffu, part == 0 && n > 64 * LPR);  // very long pieces: the whole warp on each
-            while (longm) {
-                const int i = __ffs(longm) - 1;
-                longm &= longm - 1;
-                const int b0 = __shfl_sync(0xffffffffu, s0, i), b1 = __shfl_sync(0xffffffffu, s1, i);
-                float a = 0.f;
-                for (int e = b0 + lane; e < b1; e += 32) a += svals[e];
-                a = warp_sum(a);
-                if (lane == 0) emit(rcur + i / LPR, a);
-            }
-            const int ndone = __popc(__ballot_sync(0xffffffffu, part == 0 && row < rb && a1 <= t1));  // rows are sorted: a prefix
-            rcur += ndone;
-            if (ndone < 32 / LPR || rcur >= rb) break;  // the last row of the pass still has non-zeros beyond this chunk (or no rows are left)
-        }
-        __syncwarp();
-        stage_chunk(ci + 2);  // this buffer is free again
-    }
-    if constexpr (FUSED) {
-        // every row of this warp's share gets its word, outlier-free rows included (the owner of the strip waits for all 64 of them)
-        __syncwarp();
-        if (smem_sums) {
-            for (int i = lane; i < nr; i += 32) st_relaxed_u64(p.ws_cbox + r + i, box_word(srowacc[r - ca + i], boxtag));
-        } else if (nr > 0) {
-            __threadfence();  // the red.adds on the value halves come first
-            for (int i = lane; i < nr; i += 32) asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(reinterpret_cast<uint32_t *>(p.ws_cbox + r + i) + 1), "r"(1u) : "memory");
-        }
+        for (int t = 0; t < T; ++t) { cc[t] = cn[t]; vv[t] = vn[t]; }
     }
 }
 
@@ -722,7 +672,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             }
         }
     } else if (warp >= WARP_SP) {
-        sparse2<XH, FUSED>(p, sm, base, warp - WARP_SP, lane, acc_out);
+        sparse3<XH, FUSED>(p, base, warp - WARP_SP, lane, acc_out, 1u);
         TRACE(10, lane == 0);
     } else if (warp >= WARP_BLD) {
         // =========================== table builders (2 warps, thread = column slot) ===========================
