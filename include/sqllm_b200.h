@@ -48,7 +48,7 @@ extern "C" {
 #define SQLLM_EWORKSPACE (-3) /* workspace missing or too small */
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
-                                 later + sqllm_lutgemm_fused (backward compatible, same version) */
+                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows (backward compatible, same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -137,6 +137,23 @@ int sqllm_lutgemv_fused(const sqllm_lutgemv_args *args,
  * lookup_table and bias 4-byte aligned.  No workspace, no allocation, no host synchronisation: CUDA-graph capturable. */
 int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
                         void *stream);
+
+/* Fused module path for a few fp16 rows (decode of several sequences, speculative-decoding verification, short prompts) on the
+ * CUDA cores: y[m][c] = bias[c] + LUT-GEMV + CSR + dense rows, written (not accumulated), from fp16 x [M][in_features]
+ * (row-major), in ONE launch.  args->batch = M >= 1 (any M is correct; QuantLinearLUT sends 2 to 63 rows here); args->vec /
+ * args->mul are ignored.  y is fp16 (y_is_half) or fp32 [M][out_features].  The exact fp32 codebook and fp32 sums are always
+ * used: sqllm_set_lut_mode does not apply.  Every output is written once by one CTA in a fixed order (thread-block clusters
+ * split K; the leader adds the peers' partial sums over distributed shared memory), so results are bit-reproducible and a
+ * row's result does not depend on M or on the other rows: sqllm_set_deterministic does not apply either.  No limit on topX or on
+ * the outliers per row; duplicate dense-row channels add up; dense-row channels outside [0, out_features) and CSR columns
+ * outside [0, in_features) are ignored.  in_features <= SQLLM_ROWS_MAX_IN (the slab of x each CTA stages must fit its shared
+ * memory); out_features <= 65535 * 64.  Requirements (checked, SQLLM_EINVAL otherwise): in_features % 32 == 0,
+ * out_features % 4 == 0, batch >= 1, non-null qweight / lookup_table / x / y, x and y 16-byte aligned, qweight, lookup_table
+ * and bias 4-byte aligned, topX >= 0, full_row_indices present with full_rows.  No workspace, no allocation, no host
+ * synchronisation: CUDA-graph capturable and safe on several streams at once. */
+#define SQLLM_ROWS_MAX_IN 49152
+int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
+                       void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

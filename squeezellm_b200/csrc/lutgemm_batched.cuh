@@ -57,10 +57,11 @@ struct Dec3 {
     }
 };
 
-// acc[b][t] += sum_k wv[t][k] * x_b[k] for the BT batch rows; x rows are BT consecutive rows of `xs` (row pitch xpitch bytes)
-__device__ __forceinline__ void fma_rows(float (&acc)[BT][4], const float (&wv)[4][8], const uint32_t xaddr, const uint32_t xpitch) {
+// acc[b][t] += sum_k wv[t][k] * x_b[k] for NB batch rows; x rows are NB consecutive rows of `xs` (row pitch xpitch bytes)
+template <int NB>
+__device__ __forceinline__ void fma_rows(float (&acc)[NB][4], const float (&wv)[4][8], const uint32_t xaddr, const uint32_t xpitch) {
 #pragma unroll
-    for (int b = 0; b < BT; ++b) {
+    for (int b = 0; b < NB; ++b) {
         const float4 xa = lds_v4(xaddr + b * xpitch), xb = lds_v4(xaddr + b * xpitch + 16);
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
@@ -71,6 +72,45 @@ __device__ __forceinline__ void fma_rows(float (&acc)[BT][4], const float (&wv)[
             d = fmaf(wv[t][4], xb.x, d); d = fmaf(wv[t][5], xb.y, d); d = fmaf(wv[t][6], xb.z, d); d = fmaf(wv[t][7], xb.w, d);
             acc[b][t] += d;
         }
+    }
+}
+
+// One position of one lane: its 4 columns x one unit (the words in cur) decoded once from the table, through the PRMT / LOP3
+// addresses l[] and segc, and applied to NB rows of x at xaddr.  Half-warp 1 (jsel) walks its columns in the order 1,0,3,2.
+template <int BITS, int NB>
+__device__ __forceinline__ void unit_fma(float (&acc)[NB][4], const uint4 (&cur)[CB<BITS>::ROWS], const int jsel, const uint32_t (&l)[4],
+                                         const uint32_t segc, const uint32_t xaddr, const uint32_t xpitch) {
+    if constexpr (BITS == 4) {
+        const uint4 q = cur[0];
+        const uint32_t w[4] = {jsel ? q.y : q.x, jsel ? q.x : q.y, jsel ? q.w : q.z, jsel ? q.z : q.w};
+        float wv[4][8];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const uint32_t E = (w[t] & 0x0F0F0F0Fu) | segc;
+            const uint32_t O = ((w[t] >> 4) & 0x0F0F0F0Fu) | segc;
+            wv[t][0] = lds_f32(__byte_perm(E, l[t], 0x7604)); wv[t][1] = lds_f32(__byte_perm(O, l[t], 0x7604));
+            wv[t][2] = lds_f32(__byte_perm(E, l[t], 0x7614)); wv[t][3] = lds_f32(__byte_perm(O, l[t], 0x7614));
+            wv[t][4] = lds_f32(__byte_perm(E, l[t], 0x7624)); wv[t][5] = lds_f32(__byte_perm(O, l[t], 0x7624));
+            wv[t][6] = lds_f32(__byte_perm(E, l[t], 0x7634)); wv[t][7] = lds_f32(__byte_perm(O, l[t], 0x7634));
+        }
+        fma_rows<NB>(acc, wv, xaddr, xpitch);
+    } else {
+        const uint32_t a[4] = {jsel ? cur[0].y : cur[0].x, jsel ? cur[0].x : cur[0].y, jsel ? cur[0].w : cur[0].z, jsel ? cur[0].z : cur[0].w};
+        const uint32_t b[4] = {jsel ? cur[1].y : cur[1].x, jsel ? cur[1].x : cur[1].y, jsel ? cur[1].w : cur[1].z, jsel ? cur[1].z : cur[1].w};
+        const uint32_t c[4] = {jsel ? cur[2].y : cur[2].x, jsel ? cur[2].x : cur[2].y, jsel ? cur[2].w : cur[2].z, jsel ? cur[2].z : cur[2].w};
+        float wv[4][8];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) Dec3<0, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
+        fma_rows<NB>(acc, wv, xaddr, xpitch);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) Dec3<8, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
+        fma_rows<NB>(acc, wv, xaddr + 32, xpitch);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) Dec3<16, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
+        fma_rows<NB>(acc, wv, xaddr + 64, xpitch);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) Dec3<24, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
+        fma_rows<NB>(acc, wv, xaddr + 96, xpitch);
     }
 }
 
@@ -136,39 +176,7 @@ __global__ void __launch_bounds__(BTHREADS) lutgemm_batched_kernel(const PB p) {
     load_unit(u, cur);
     for (; u - jsel < nu; u += 2 * BW) {   // warp-uniform bound (nu is even: a pair never straddles the end)
         load_unit(u + 2 * BW, nxt);
-        const uint32_t xaddr = xs + (uint32_t)(u * C::XU * 4);
-        if constexpr (BITS == 4) {
-            const uint4 q = cur[0];
-            const uint32_t w[4] = {jsel ? q.y : q.x, jsel ? q.x : q.y, jsel ? q.w : q.z, jsel ? q.z : q.w};
-            float wv[4][8];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-                const uint32_t E = (w[t] & 0x0F0F0F0Fu) | segc;
-                const uint32_t O = ((w[t] >> 4) & 0x0F0F0F0Fu) | segc;
-                wv[t][0] = lds_f32(__byte_perm(E, l[t], 0x7604)); wv[t][1] = lds_f32(__byte_perm(O, l[t], 0x7604));
-                wv[t][2] = lds_f32(__byte_perm(E, l[t], 0x7614)); wv[t][3] = lds_f32(__byte_perm(O, l[t], 0x7614));
-                wv[t][4] = lds_f32(__byte_perm(E, l[t], 0x7624)); wv[t][5] = lds_f32(__byte_perm(O, l[t], 0x7624));
-                wv[t][6] = lds_f32(__byte_perm(E, l[t], 0x7634)); wv[t][7] = lds_f32(__byte_perm(O, l[t], 0x7634));
-            }
-            fma_rows(acc, wv, xaddr, xpitch);
-        } else {
-            const uint32_t a[4] = {jsel ? cur[0].y : cur[0].x, jsel ? cur[0].x : cur[0].y, jsel ? cur[0].w : cur[0].z, jsel ? cur[0].z : cur[0].w};
-            const uint32_t b[4] = {jsel ? cur[1].y : cur[1].x, jsel ? cur[1].x : cur[1].y, jsel ? cur[1].w : cur[1].z, jsel ? cur[1].z : cur[1].w};
-            const uint32_t c[4] = {jsel ? cur[2].y : cur[2].x, jsel ? cur[2].x : cur[2].y, jsel ? cur[2].w : cur[2].z, jsel ? cur[2].z : cur[2].w};
-            float wv[4][8];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) Dec3<0, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
-            fma_rows(acc, wv, xaddr, xpitch);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) Dec3<8, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
-            fma_rows(acc, wv, xaddr + 32, xpitch);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) Dec3<16, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
-            fma_rows(acc, wv, xaddr + 64, xpitch);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) Dec3<24, 0>::run(wv[t], a[t], b[t], c[t], l[t]);
-            fma_rows(acc, wv, xaddr + 96, xpitch);
-        }
+        unit_fma<BITS, BT>(acc, cur, jsel, l, segc, xs + (uint32_t)(u * C::XU * 4), xpitch);
 #pragma unroll
         for (int r = 0; r < C::ROWS; ++r) cur[r] = nxt[r];
     }

@@ -5,7 +5,8 @@
 //   SPMV_ATOMIC[_BATCHED]                            (:1040-1089)  CSR outliers
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
-// LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused).
+// LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused), a few fp16 rows a multi-row GEMV with a cluster split-K
+// (lutgemv_rows.cuh, sqllm_lutgemv_rows).
 //
 // Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default
 // (fast) fused mode, whatever its width: a layer narrower than one strip is a layer whose only strip is ragged.
@@ -913,6 +914,7 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemv_v2.cuh"
 #include "lutgemv_seq.cuh"
 #include "lutgemm_batched.cuh"
+#include "lutgemv_rows.cuh"
 #include "lutgemm_tc.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
@@ -1598,6 +1600,33 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     return SQLLM_OK;
 }
 
+// ---- a few fp16 rows (lutgemv_rows.cuh): plan + launch ------------------------------------------------------------------
+// Slabs per strip S (the cluster size) from K, N and the SM count only - never from M, so that a row's result does not depend on
+// M: the smallest S in {1, 2, 4, 8} that gives at least two CTAs per SM and a slab of at most SLAB_GOAL inputs, with no more
+// slabs than units.  Rows per CTA RB from M: 2, 4 or 8 (a row computes the same bits whatever RB is).
+struct RowsPlan { int S, ks, kpad, RB, smem; };
+int rows_plan(int bits, int K, int N, int M, int sm, RowsPlan &pl) {
+    using namespace rows;
+    const int XU = bits == 4 ? 8 : 32, R = K / XU, strips = (N + STRIP - 1) / STRIP;
+    int S = 1;
+    while (S < MAX_SLABS && 2 * S <= R && ((long long)strips * S < 2LL * sm || (long long)(R + S - 1) / S * XU > SLAB_GOAL)) S *= 2;
+    pl.S = S;
+    pl.ks = (R + S - 1) / S;
+    pl.kpad = (pl.ks + (pl.ks & 1)) * XU;
+    pl.RB = M <= 2 ? 2 : M <= 4 ? 4 : 8;
+#define RS(B, RBV) SR<B, RBV>::total(pl.kpad)
+    pl.smem = bits == 4 ? (pl.RB == 2 ? RS(4, 2) : pl.RB == 4 ? RS(4, 4) : RS(4, 8)) : (pl.RB == 2 ? RS(3, 2) : pl.RB == 4 ? RS(3, 4) : RS(3, 8));
+#undef RS
+    if (pl.smem > 227 * 1024) return fail(SQLLM_EINVAL, "in_features=%d needs %d B of shared memory per CTA (> 227 KB)", K, pl.smem);
+    return SQLLM_OK;
+}
+
+typedef void (*KRows)(const rows::PR);
+KRows krows_lookup(int bits, int RB) {
+    if (bits == 4) return RB == 2 ? rows::lutgemv_rows_kernel<4, 2> : RB == 4 ? rows::lutgemv_rows_kernel<4, 4> : rows::lutgemv_rows_kernel<4, 8>;
+    return RB == 2 ? rows::lutgemv_rows_kernel<3, 2> : RB == 4 ? rows::lutgemv_rows_kernel<3, 4> : rows::lutgemv_rows_kernel<3, 8>;
+}
+
 // ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
 // arena instead of y ---------------------------------------------------------------------------------------------------------------
 int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
@@ -1771,6 +1800,62 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int
     else tc::lutgemm_tc_kernel<3><<<grid, tc::THREADS, tc::SMEM, st>>>(p);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_fused launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
+    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
+    if (a->in_features > SQLLM_ROWS_MAX_IN) return fail(SQLLM_EINVAL, "in_features=%d exceeds %d: the slab of x a CTA stages would not fit its shared memory", a->in_features, SQLLM_ROWS_MAX_IN);
+    if (a->out_features <= 0 || a->out_features % 4) return fail(SQLLM_EINVAL, "out_features=%d must be a positive multiple of 4", a->out_features);
+    if ((a->out_features + STRIP - 1) / STRIP > 65535) return fail(SQLLM_EINVAL, "out_features=%d exceeds %d", a->out_features, 65535 * STRIP);
+    if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x) must be >= 1 (got %d)", a->batch);
+    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
+    if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
+    if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3) || (reinterpret_cast<uintptr_t>(bias) & 3))
+        return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
+    if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
+    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
+    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
+    int sm = 0;
+    RowsPlan pl;
+    {
+        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        int dev = 0;
+        int rc = cur_dev(dev);
+        if (rc) return rc;
+        sm = g_dev[dev].sm;
+        if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
+        if ((rc = set_max_smem(g_dev[dev], krows_lookup(a->bits, pl.RB), 227 * 1024))) return rc;
+    }
+    const int groups = (a->batch + pl.RB - 1) / pl.RB;
+    if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
+    rows::PR p;
+    memset(&p, 0, sizeof(p));
+    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    p.x = static_cast<const __half *>(x); p.y = y; p.y_is_half = y_is_half ? 1 : 0; p.bias = bias;
+    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
+    const bool hyb = a->full_rows && a->topX > 0;
+    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
+    p.K = a->in_features; p.N = a->out_features; p.M = a->batch; p.R = a->bits == 4 ? p.K / 8 : p.K / 32;
+    p.ks = pl.ks; p.kpad = pl.kpad;
+    p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0;
+    // the one launch with a cluster dimension: the S CTAs of a strip's cluster split its K
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(pl.S, (a->out_features + STRIP - 1) / STRIP, groups);
+    cfg.blockDim = dim3(rows::RTHREADS);
+    cfg.dynamicSmemBytes = pl.smem;
+    cfg.stream = static_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = pl.S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, krows_lookup(a->bits, pl.RB), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

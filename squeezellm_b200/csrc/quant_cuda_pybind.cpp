@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `unpack_indices`, `abi_version`, `fused_limits`.
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `unpack_indices`, `abi_version`, `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -239,6 +239,25 @@ torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     return y;
 }
 
+// y [M, out] fp16 = bias + LUT-GEMV(x) [+ CSR] [+ dense rows] from fp16 x [M, in], a few rows on the CUDA cores (sqllm_lutgemv_rows):
+// QuantLinearLUT.forward's batched branch for 2 to QuantLinearLUT.ROWS_MAX rows in one launch.
+torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                           c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                           c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                           c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16, "lutgemv_rows: x must be fp16");
+    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemv_rows: x must be [M, in_features=", a.in_features, "]");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemv_rows: x must have 1 to 2^31-1 rows");
+    a.batch = (int)x.size(0);
+    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
+    check_status(sqllm_lutgemv_rows(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemv_rows");
+    return y;
+}
+
 // y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16/fp32 with numel == in; returns [out] in x's dtype
 // (QuantLinearLUT.forward's matvec branch, squeezellm/quant.py:212-312, in one launch).
 torch::Tensor lutgemv_fused(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
@@ -395,6 +414,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
+    m.def("lutgemv_rows", &lutgemv_rows, "fused QuantLinearLUT matmul for a few rows on the CUDA cores: fp16 x [M, in] -> fp16 y [M, out] (bias, CSR, dense rows), one launch",
+          py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
+          py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
+          py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
     m.def("lutgemv_fused_exchange", &lutgemv_fused_exchange,
           "fused matvec of a column shard that stores its result into every rank's symmetric arena (NVLink peer memory) and waits for the peers'",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias"), py::arg("rows"), py::arg("cols"),
@@ -451,7 +474,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               py::dict d;
               d["max_topx"] = SQLLM_FUSED_MAX_TOPX;
               d["max_out_features"] = SQLLM_FUSED_MAX_OUT;
+              d["rows_max_in_features"] = SQLLM_ROWS_MAX_IN;
               return d;
           },
-          "largest layer the fused, exchange and sequence entry points accept: {'max_topx', 'max_out_features'} (the 12 symbols have no such limit)");
+          "largest layer the fused, exchange and sequence entry points accept: {'max_topx', 'max_out_features'} (the 12 symbols have no such "
+          "limit), and the largest in_features of lutgemv_rows: 'rows_max_in_features'");
 }

@@ -14,6 +14,10 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
   * `forward` with fp16 x of at least `TC_MIN_ROWS` rows (prefill, evaluation; reference quant.py:314-379) uses ONE
     tensor-core launch (`quant_cuda.lutgemm_fused`, outliers and dense rows folded into the weight tiles) instead of
     zeros + x.float() + 1-3 batched launches + out.to(dtype).
+  * `forward` with fp16 x of 2 to `ROWS_MAX` rows (and fewer than `TC_MIN_ROWS`; several sequences decoding at once, speculative-
+    decoding verification, short prompts) uses ONE CUDA-core launch (`quant_cuda.lutgemv_rows`: a multi-row LUT-GEMV whose
+    thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence.  fp32 / bf16 x and
+    `use_fused = False` keep the reference's batched symbols.
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
     (quant.py:238,282 vs quant_cuda.cpp:257-270), i.e. an AttributeError at the first forward.
@@ -107,6 +111,9 @@ class QuantLinearLUT(nn.Module):
     # inputs and use_fused = False run the batched symbols.  64: where a whole 7B decoder layer gets faster on an H100 (DESIGN.md
     # section 3.6: 32 rows 1.08 vs 0.78 ms, 64 rows 1.09 vs 1.48 ms).
     TC_MIN_ROWS = 64
+    # fp16 inputs of 2 to ROWS_MAX rows (below TC_MIN_ROWS) run the multi-row GEMV (quant_cuda.lutgemv_rows).  63: it is faster than
+    # the batched symbols on a whole 7B decoder layer at every measured row count up to 63 on an H100 (DESIGN.md section 3.9).
+    ROWS_MAX = 63
     # codebook precision of the fused path is process-wide: quant_cuda.set_lut_mode("exact" | "fp16")  (include/sqllm_b200.h)
 
     def __init__(self, bits, infeatures, outfeatures, bias, include_sparse=False, numvals=0, topX=0,
@@ -187,6 +194,10 @@ class QuantLinearLUT(nn.Module):
         topx = int(full_rows.shape[1]) if full_rows is not None else 0
         return self.outfeatures <= FUSED_LIMITS["max_out_features"] and topx <= FUSED_LIMITS["max_topx"]
 
+    def _rows_fits(self):
+        """The layers quant_cuda.lutgemv_rows takes: out_features a multiple of 4, in_features up to the slab its CTAs stage."""
+        return self.outfeatures % 4 == 0 and self.infeatures <= FUSED_LIMITS["rows_max_in_features"]
+
     def forward(self, x):
         if self._sibling_group is not None:
             group, index = self._sibling_group
@@ -213,6 +224,12 @@ class QuantLinearLUT(nn.Module):
             out = quant_cuda.lutgemm_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                            None, rows, cols, vals, fr, fri).reshape(out_shape)
             return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
+        if (QuantLinearLUT.use_fused and x.dtype == torch.float16 and 2 <= x.shape[0] <= QuantLinearLUT.ROWS_MAX
+                and self._rows_fits()):
+            rows, cols, vals, fr, fri = self._sparse_args()
+            out = quant_cuda.lutgemv_rows(_aligned(x), self.qweight, self.lookup_table, self.bits,
+                                          None, rows, cols, vals, fr, fri).reshape(out_shape)
+            return out + self.bias if self.bias is not None else out
         out = torch.zeros((x.shape[0], self.outfeatures), device=dev, dtype=torch.float32)
         dtype = x.dtype
         x = _aligned(x.float())
