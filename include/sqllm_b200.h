@@ -48,7 +48,7 @@ extern "C" {
 #define SQLLM_EWORKSPACE (-3) /* workspace missing or too small */
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
-                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows (backward compatible, same version) */
+                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t (backward compatible, same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -154,6 +154,34 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void
 #define SQLLM_ROWS_MAX_IN 49152
 int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
                        void *stream);
+
+/* Element types of sqllm_lutgemm_t's dy and dx. */
+#define SQLLM_DT_F32 0
+#define SQLLM_DT_F16 1
+#define SQLLM_DT_BF16 2
+
+/* Input gradient of the layer (backpropagation through QuantLinearLUT): the transposed LUT-GEMM
+ *   dx[m][k] = sum_c dy[m][c] W[k][c],   W[k][c] = LUT[c][idx(k,c)] + CSR(c,k) + sum_j full_rows[k][j] [full_row_indices[j] == c]
+ * from dy [M][out_features] (row-major; fp32, fp16 or bf16: dy_dtype) into dx [M][in_features] (written, not accumulated; fp32
+ * or dy's dtype: dx_dtype).  args->batch = M; args->vec / args->mul are ignored; there is no bias term.  The outlier rules are
+ * those of the forward entry points: duplicate dense-row channels add up, CSR columns outside [0, in_features) and dense-row
+ * channels outside [0, out_features) are ignored, no limit on topX or on the entries per CSR row, CSR columns need not be
+ * ascending.  Every output is written once by one CTA in a fixed order: bit-reproducible.
+ *   path 1 = tensor cores (fp16 / bf16 dy only): 128 x 128 dx tiles on wgmma, the reduction axis in chunks of 64 columns; every
+ *     folded weight is split exactly (fp16 dy: hi + lo fp16 parts of a per-chunk power-of-two scale; bf16 dy: three bf16 parts),
+ *     products are exact and sums fp32.  A weight more than about 2^20 below the largest weight of its 64-column chunk is kept
+ *     to about 2^-40 of that largest weight (fp16 dy).
+ *   path 2 = CUDA cores (any dy dtype): exact fp32 codebook and fp32 sums; thread-block clusters split out_features and the
+ *     leader adds the peers' partial sums over distributed shared memory; a row's result does not depend on M or on the other
+ *     rows.
+ *   path 0 = path 1 for fp16 / bf16 dy of at least SQLLM_BWD_TC_MIN_ROWS rows, else path 2.
+ * Requirements (checked, SQLLM_EINVAL otherwise): in_features % 32 == 0, out_features >= 1, batch >= 1, non-null qweight /
+ * lookup_table / dy / dx, qweight and lookup_table 4-byte aligned, dy aligned to its element size, dx 16-byte aligned,
+ * topX >= 0, full_row_indices present with full_rows.  No workspace, no allocation, no host synchronisation: CUDA-graph
+ * capturable and safe on several streams at once. */
+#define SQLLM_BWD_TC_MIN_ROWS 96
+int sqllm_lutgemm_t(const sqllm_lutgemv_args *args, const void *dy, int dy_dtype, void *dx, int dx_dtype, int path,
+                    void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

@@ -6,7 +6,8 @@
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
 // LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused), a few fp16 rows a multi-row GEMV with a cluster split-K
-// (lutgemv_rows.cuh, sqllm_lutgemv_rows).
+// (lutgemv_rows.cuh, sqllm_lutgemv_rows).  The input gradient dx = dy . W^T has a transposed LUT-GEMM on the tensor cores
+// (lutgemm_tc_t.cuh) and one on the CUDA cores (lutgemm_t.cuh), both behind sqllm_lutgemm_t.
 //
 // Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default
 // (fast) fused mode, whatever its width: a layer narrower than one strip is a layer whose only strip is ragged.
@@ -29,6 +30,7 @@
 //   * Flush: per-strip partials in the workspace and one ticket per contributor; the last contributor of a strip sums them in a
 //     fixed order, adds the bias and stores y.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -916,6 +918,8 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemm_batched.cuh"
 #include "lutgemv_rows.cuh"
 #include "lutgemm_tc.cuh"
+#include "lutgemm_t.cuh"
+#include "lutgemm_tc_t.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
 // tables to their own size - up to 64 KB - so the host needs the real address, not a worst case; the kernel re-checks it)
@@ -1627,6 +1631,28 @@ KRows krows_lookup(int bits, int RB) {
     return RB == 2 ? rows::lutgemv_rows_kernel<3, 2> : RB == 4 ? rows::lutgemv_rows_kernel<3, 4> : rows::lutgemv_rows_kernel<3, 8>;
 }
 
+// ---- input gradient (lutgemm_t.cuh): plan + launch --------------------------------------------------------------------------
+// Strip splits S (the cluster size) from K, N and the SM count only - never from M, so that a row's result does not depend on M:
+// the smallest S in {1, 2, 4, 8} that gives at least two CTAs per SM, with at least two strips per CTA.  Rows per CTA RB from M:
+// 1, 2, 4 or 8 (a row computes the same bits whatever RB is).
+struct TPlan { int S, RB, smem; };
+void t_plan(int K, int N, int M, int sm, TPlan &pl) {
+    using namespace bwd;
+    const int slabs = (K + KS - 1) / KS, strips = (N + STRIP - 1) / STRIP;
+    int S = 1;
+    while (S < MAX_SPLIT && 4 * S <= strips && (long long)slabs * S < 2LL * sm) S *= 2;
+    pl.S = S;
+    pl.RB = M <= 1 ? 1 : M <= 2 ? 2 : M <= 4 ? 4 : 8;
+    pl.smem = pl.RB == 1 ? ST<1>::TOTAL : pl.RB == 2 ? ST<2>::TOTAL : pl.RB == 4 ? ST<4>::TOTAL : ST<8>::TOTAL;
+}
+
+typedef void (*KT)(const bwd::PT);
+KT kt_lookup(int bits, int RB) {
+    using namespace bwd;
+    if (bits == 4) return RB == 1 ? lutgemm_t_kernel<4, 1> : RB == 2 ? lutgemm_t_kernel<4, 2> : RB == 4 ? lutgemm_t_kernel<4, 4> : lutgemm_t_kernel<4, 8>;
+    return RB == 1 ? lutgemm_t_kernel<3, 1> : RB == 2 ? lutgemm_t_kernel<3, 2> : RB == 4 ? lutgemm_t_kernel<3, 4> : lutgemm_t_kernel<3, 8>;
+}
+
 // ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
 // arena instead of y ---------------------------------------------------------------------------------------------------------------
 int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
@@ -1856,6 +1882,99 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int 
     cfg.numAttrs = 1;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, krows_lookup(a->bits, pl.RB), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+int sqllm_lutgemm_t(const sqllm_lutgemv_args *a, const void *dy, int dy_dtype, void *dx, int dx_dtype, int path, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
+    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
+    if ((a->in_features + bwd::KS - 1) / bwd::KS > 65535) return fail(SQLLM_EINVAL, "in_features=%d exceeds %d", a->in_features, 65535 * bwd::KS);
+    if (a->out_features <= 0) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
+    if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of dy) must be >= 1 (got %d)", a->batch);
+    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
+    if (!dy || !dx) return fail(SQLLM_EINVAL, "dy / dx must not be null");
+    if (dy_dtype != SQLLM_DT_F32 && dy_dtype != SQLLM_DT_F16 && dy_dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
+    if (dx_dtype != SQLLM_DT_F32 && dx_dtype != dy_dtype) return fail(SQLLM_EINVAL, "dx_dtype=%d must be SQLLM_DT_F32 or dy's dtype (%d)", dx_dtype, dy_dtype);
+    if (path < 0 || path > 2) return fail(SQLLM_EINVAL, "path=%d must be 0 (auto), 1 (tensor cores) or 2 (CUDA cores)", path);
+    if (path == 1 && dy_dtype == SQLLM_DT_F32) return fail(SQLLM_EINVAL, "path=1 (tensor cores) takes fp16 or bf16 dy, not fp32");
+    if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3))
+        return fail(SQLLM_EINVAL, "qweight and lookup_table must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(dy) & (dy_dtype == SQLLM_DT_F32 ? 3 : 1)) return fail(SQLLM_EINVAL, "dy must be aligned to its element size");
+    if (reinterpret_cast<uintptr_t>(dx) & 15) return fail(SQLLM_EINVAL, "dx must be 16-byte aligned");
+    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
+    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
+    if (path == 0) path = dy_dtype != SQLLM_DT_F32 && a->batch >= SQLLM_BWD_TC_MIN_ROWS ? 1 : 2;
+    if (path == 1) {
+        const bool bf = dy_dtype == SQLLM_DT_BF16;
+        {
+            std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+            int dev = 0;
+            int rc = cur_dev(dev);
+            if (!rc) rc = bf ? set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<4, true>, tct::L<3>::SMEM)
+                             : set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<4, false>, tct::L<2>::SMEM);
+            if (!rc) rc = bf ? set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<3, true>, tct::L<3>::SMEM)
+                             : set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<3, false>, tct::L<2>::SMEM);
+            if (rc) return rc;
+        }
+        tct::PT p;
+        memset(&p, 0, sizeof(p));
+        p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+        p.dy = dy; p.dx = dx; p.dx_dt = dx_dtype;
+        p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
+        const bool hyb = a->full_rows && a->topX > 0;
+        p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
+        p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
+        p.dy_al16 = (reinterpret_cast<uintptr_t>(dy) & 15) == 0 && a->out_features % 8 == 0;
+        const dim3 grid((a->batch + tc::BM - 1) / tc::BM, (a->in_features + tct::BK - 1) / tct::BK);
+        cudaStream_t st = static_cast<cudaStream_t>(stream);
+        if (bf) {
+            if (a->bits == 4) tct::lutgemm_tc_t_kernel<4, true><<<grid, tct::THREADS, tct::L<3>::SMEM, st>>>(p);
+            else tct::lutgemm_tc_t_kernel<3, true><<<grid, tct::THREADS, tct::L<3>::SMEM, st>>>(p);
+        } else {
+            if (a->bits == 4) tct::lutgemm_tc_t_kernel<4, false><<<grid, tct::THREADS, tct::L<2>::SMEM, st>>>(p);
+            else tct::lutgemm_tc_t_kernel<3, false><<<grid, tct::THREADS, tct::L<2>::SMEM, st>>>(p);
+        }
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_t (tensor cores) launch failed: %s", cudaGetErrorString(e));
+        return SQLLM_OK;
+    }
+    int sm = 0;
+    TPlan pl;
+    {
+        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        int dev = 0;
+        int rc = cur_dev(dev);
+        if (rc) return rc;
+        sm = g_dev[dev].sm;
+        t_plan(a->in_features, a->out_features, a->batch, sm, pl);
+        if ((rc = set_max_smem(g_dev[dev], kt_lookup(a->bits, pl.RB), pl.smem))) return rc;
+    }
+    const int groups = (a->batch + pl.RB - 1) / pl.RB;
+    if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
+    bwd::PT p;
+    memset(&p, 0, sizeof(p));
+    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    p.dy = dy; p.dx = dx; p.dy_dt = dy_dtype; p.dx_dt = dx_dtype;
+    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
+    const bool hyb = a->full_rows && a->topX > 0;
+    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
+    p.K = a->in_features; p.N = a->out_features; p.M = a->batch;
+    p.strips = (a->out_features + STRIP - 1) / STRIP;
+    p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0 && a->out_features % 4 == 0;
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(pl.S, (a->in_features + bwd::KS - 1) / bwd::KS, groups);
+    cfg.blockDim = dim3(bwd::TTHREADS);
+    cfg.dynamicSmemBytes = pl.smem;
+    cfg.stream = static_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = pl.S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kt_lookup(a->bits, pl.RB), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_t launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

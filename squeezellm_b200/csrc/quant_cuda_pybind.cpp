@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `unpack_indices`, `abi_version`, `fused_limits`.
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemm_t`, `unpack_indices`, `abi_version`, `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -173,9 +173,9 @@ void fill_layer_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
                      const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
                      const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
                      const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
-                     const c10::optional<torch::Tensor> &full_row_indices) {
+                     const c10::optional<torch::Tensor> &full_row_indices, bool check_x_dtype = true) {
     TORCH_CHECK(x.is_cuda() && x.is_contiguous(), "x must be a contiguous CUDA tensor");
-    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
+    if (check_x_dtype) TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
     TORCH_CHECK(bits == 3 || bits == 4, "bits must be 3 or 4");
     need(qweight, "qweight", torch::kInt32, x);
     need(lookup_table, "lookup_table", torch::kFloat32, x);
@@ -256,6 +256,33 @@ torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor
     torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
     check_status(sqllm_lutgemv_rows(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemv_rows");
     return y;
+}
+
+// dx [M, in] = dy [M, out] . W^T (LUT + CSR + dense rows), in dy's dtype (fp16, bf16 or fp32): the input gradient of
+// QuantLinearLUT (sqllm_lutgemm_t).  path: "auto" (the library picks), "tc" (tensor cores) or "cuda" (CUDA cores).
+torch::Tensor lutgemm_t(torch::Tensor dy, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                        c10::optional<torch::Tensor> rows, c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                        c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices,
+                        const std::string &path) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(dy));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, dy, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices, false);
+    int dt;
+    switch (dy.scalar_type()) {
+        case torch::kFloat32: dt = SQLLM_DT_F32; break;
+        case torch::kFloat16: dt = SQLLM_DT_F16; break;
+        case torch::kBFloat16: dt = SQLLM_DT_BF16; break;
+        default: TORCH_CHECK(false, "lutgemm_t: dy must be fp16, bf16 or fp32 (got ", dy.scalar_type(), ")");
+    }
+    TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", "lutgemm_t: path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
+    TORCH_CHECK(dy.dim() == 2 && dy.size(1) == a.out_features, "lutgemm_t: dy must be [M, out_features=", a.out_features, "]");
+    TORCH_CHECK(dy.size(0) >= 1 && dy.size(0) <= INT32_MAX, "lutgemm_t: dy must have 1 to 2^31-1 rows");
+    a.batch = (int)dy.size(0);
+    torch::Tensor dx = torch::empty({dy.size(0), (int64_t)a.in_features}, dy.options());
+    check_status(sqllm_lutgemm_t(&a, dy.data_ptr(), dt, dx.data_ptr(), dt, path == "auto" ? 0 : path == "tc" ? 1 : 2, cur_stream()),
+                 "quant_cuda.lutgemm_t");
+    return dx;
 }
 
 // y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16/fp32 with numel == in; returns [out] in x's dtype
@@ -418,6 +445,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
+    m.def("lutgemm_t", &lutgemm_t, "input gradient of QuantLinearLUT: dy [M, out] -> dx [M, in] = dy . W^T (CSR, dense rows), in dy's dtype, one launch",
+          py::arg("dy"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("rows") = py::none(),
+          py::arg("cols") = py::none(), py::arg("vals") = py::none(), py::arg("full_rows") = py::none(),
+          py::arg("full_row_indices") = py::none(), py::arg("path") = "auto");
     m.def("lutgemv_fused_exchange", &lutgemv_fused_exchange,
           "fused matvec of a column shard that stores its result into every rank's symmetric arena (NVLink peer memory) and waits for the peers'",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias"), py::arg("rows"), py::arg("cols"),

@@ -18,6 +18,11 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
     decoding verification, short prompts) uses ONE CUDA-core launch (`quant_cuda.lutgemv_rows`: a multi-row LUT-GEMV whose
     thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence.  fp32 / bf16 x and
     `use_fused = False` keep the reference's batched symbols.
+  * `loss.backward()` works through the layer when x requires grad (the reference has no backward: its outputs carry no
+    graph).  x gets dx = dy . W^T from ONE launch (`quant_cuda.lutgemm_t`: a transposed LUT-GEMM, on the tensor cores for fp16 /
+    bf16 gradients of at least `BWD_TC_MIN_ROWS` rows, else on the CUDA cores; outliers and dense rows included); the buffers are constants and get no gradient.  The forward of such a call takes the same route
+    and gives the same bits as without grad; every other call goes exactly as before.  `use_fused` does not affect the
+    backward.  The sharded, exchange and sequence paths (sharding.py, runtime.py) give no gradient.
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
     (quant.py:238,282 vs quant_cuda.cpp:257-270), i.e. an AttributeError at the first forward.
@@ -37,6 +42,7 @@ import sys
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 
@@ -114,6 +120,10 @@ class QuantLinearLUT(nn.Module):
     # fp16 inputs of 2 to ROWS_MAX rows (below TC_MIN_ROWS) run the multi-row GEMV (quant_cuda.lutgemv_rows).  63: it is faster than
     # the batched symbols on a whole 7B decoder layer at every measured row count up to 63 on an H100 (DESIGN.md section 3.9).
     ROWS_MAX = 63
+    # fp16 / bf16 gradients of at least this many rows run the input gradient on the tensor cores (quant_cuda.lutgemm_t path
+    # "tc"); fewer rows and fp32 gradients on the CUDA cores.  96: where the two cross on a whole 7B decoder layer on an H100
+    # (DESIGN.md section 3.10: 64 rows 5.96 vs 5.12 ms, 512 rows 8.05 vs 40.8 ms; the CUDA-core time grows 80 us per row).
+    BWD_TC_MIN_ROWS = 96
     # codebook precision of the fused path is process-wide: quant_cuda.set_lut_mode("exact" | "fp16")  (include/sqllm_b200.h)
 
     def __init__(self, bits, infeatures, outfeatures, bias, include_sparse=False, numvals=0, topX=0,
@@ -199,6 +209,24 @@ class QuantLinearLUT(nn.Module):
         return self.outfeatures % 4 == 0 and self.infeatures <= FUSED_LIMITS["rows_max_in_features"]
 
     def forward(self, x):
+        # a sibling member asks its group, whose stacked layer comes back here: the gradient flows through the stacked layer's
+        # node and autograd's slice backward adds the members' shares
+        if self._sibling_group is None and torch.is_grad_enabled() and x.requires_grad:
+            return _QuantLinearLUTFunction.apply(x, self)
+        return self._forward_impl(x)
+
+    def _grad_buffers(self):
+        """The tensors the input gradient reads (the layer's weights as the backward sees them)."""
+        return (self.qweight, self.lookup_table) + tuple(t for t in self._sparse_args() if t is not None)
+
+    def _input_grad(self, dy):
+        """dx [M, in] = dy [M, out] . W^T in dy's dtype (quant_cuda.lutgemm_t): the backward of every forward route.  fp16 / bf16
+        gradients of at least BWD_TC_MIN_ROWS rows run on the tensor cores, everything else on the CUDA cores."""
+        rows, cols, vals, fr, fri = self._sparse_args()
+        path = "tc" if dy.dtype in (torch.float16, torch.bfloat16) and dy.shape[0] >= QuantLinearLUT.BWD_TC_MIN_ROWS else "cuda"
+        return quant_cuda.lutgemm_t(_aligned(dy), self.qweight, self.lookup_table, self.bits, rows, cols, vals, fr, fri, path=path)
+
+    def _forward_impl(self, x):
         if self._sibling_group is not None:
             group, index = self._sibling_group
             return group.member_forward(index, x)
@@ -251,6 +279,34 @@ class QuantLinearLUT(nn.Module):
         else:
             fn = getattr(quant_cuda, f"vecquant{b}matmul_nuq_perchannel{sfx}")
             fn(x, self.qweight, y, self.lookup_table)
+
+
+class _QuantLinearLUTFunction(torch.autograd.Function):
+    """y = QuantLinearLUT._forward_impl(x) with dx = dy . W^T.  The layer's buffers are constants: only x gets a gradient (no
+    gradient for the codebook, the outliers or the bias), and nothing is saved for backward but the layer itself."""
+
+    @staticmethod
+    def forward(ctx, x, layer):
+        ctx.layer = layer
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        # the buffers are read again at backward time: remember their versions, so that an in-place change in between (a weight
+        # reload) raises instead of silently giving the gradient of the new weights
+        ctx.versions = [(t, t._version) for t in layer._grad_buffers()]
+        return layer._forward_impl(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        layer = ctx.layer
+        now = layer._grad_buffers()
+        if len(now) != len(ctx.versions) or any(t is not u or t._version != v for (t, v), u in zip(ctx.versions, now)):
+            raise RuntimeError("QuantLinearLUT: the layer's buffers were modified or replaced between forward and backward; "
+                               "the input gradient would use the new weights")
+        dy = dy.reshape(-1, layer.outfeatures)
+        if dy.shape[0] == 0:
+            return torch.zeros(ctx.x_shape, dtype=ctx.x_dtype, device=dy.device), None
+        dx = layer._input_grad(dy)
+        return dx.to(ctx.x_dtype).reshape(ctx.x_shape), None
 
 
 def make_quant_lut(module, names, bits, name="", include_sparse=False, numvals=None, topX=0, balanced=False,

@@ -14,6 +14,8 @@ import torch
 
 
 class GraphedDecodeStep:
+    """A decode step captured once as a CUDA graph and replayed; an inference path: its outputs carry no gradient."""
+
     def __init__(self, step_fn, example_x, warmup=3, static_input=False):
         """static_input=True: `example_x` itself is the static input buffer (a DecodeSequence's `x`), not a clone of it."""
         assert example_x.is_cuda, "example_x must be a CUDA tensor (static input buffer is cloned from it)"
@@ -67,7 +69,8 @@ class SeqVec:
 class DecodeSequence:
     """A token step recorded as a list of dependent QuantLinearLUT matvecs and run as ONE persistent kernel launch
     (csrc/lutgemv_seq.cuh): the weight stream never stops between two matvecs and results travel from one matvec to the
-    next as self-validating tagged words - no launch, no grid barrier in between.
+    next as self-validating tagged words - no launch, no grid barrier in between.  An inference path: its results carry no
+    gradient.
 
         seq = DecodeSequence(hidden, device)                  # seq.x: static fp16 input buffer [hidden]
         qkv = seq.matvec(stacked_qkv_layer, seq.input)        # -> SeqVec over the full output

@@ -58,7 +58,8 @@ def shard_state(state, c0, c1):
 
 
 class ShardedQuantLinearLUT(nn.Module):
-    """One rank's column shard of a QuantLinearLUT + the all-reduce that rebuilds the full output vector."""
+    """One rank's column shard of a QuantLinearLUT + the all-reduce that rebuilds the full output vector.  Gives no gradient:
+    its output is built in place by the all-reduce, outside autograd."""
 
     def __init__(self, local, outfeatures, c0, c1, group=None, matvec_fn=None):
         super().__init__()
@@ -78,7 +79,8 @@ class ShardedQuantLinearLUT(nn.Module):
 
     def forward(self, x):
         import torch.distributed as dist
-        y_local = self.matvec_fn(x) if self.matvec_fn is not None else self.local(x)
+        # _forward_impl: no autograd node here - the in-place all-reduce below carries no gradient
+        y_local = self.matvec_fn(x) if self.matvec_fn is not None else self.local._forward_impl(x)
         lead = y_local.shape[:-1]
         full = torch.zeros(lead + (self.outfeatures,), dtype=y_local.dtype, device=y_local.device)
         full[..., self.c0:self.c1] = y_local
@@ -109,7 +111,8 @@ def exchange_stacked(y_local, members, rank, world, out=None, group=None):
 class PeerExchange:
     """Arena in torch symmetric memory (peer-mapped over NVLink) + the bookkeeping `quant_cuda.lutgemv_fused_exchange`
     needs: the kernel's finishing CTAs store their slice of y into every rank's arena and wait for the peers', so a
-    column-sharded layer needs no separate collective (include/sqllm_b200.h, sqllm_lutgemv_fused_exchange).
+    column-sharded layer needs no separate collective (include/sqllm_b200.h, sqllm_lutgemv_fused_exchange).  Its results
+    carry no gradient.
 
     One arena per rank, identical layout everywhere: [0,8) arrival counter, [64,72) expected arrivals (local), [128,132)
     error word, destination vectors from 4096 on (one per `name`, [members][out_features_full] in the activation dtype).
@@ -211,7 +214,8 @@ class PeerArena:
 
 
 class ShardedSiblingGroup:
-    """Column shards of a set of sibling layers (same input) run as ONE stacked launch per rank + ONE exchange.
+    """Column shards of a set of sibling layers (same input) run as ONE stacked launch per rank + ONE exchange.  Gives no
+    gradient: the exchange runs outside autograd.
 
     Built from the full (unsharded) QuantLinearLUT members: every rank keeps columns [rank*w, (rank+1)*w) of each member
     (`shard_state`), stacks those shards along N (`fusion.stack_buffers`) and answers the members' `forward(x)` through the
@@ -276,7 +280,7 @@ class ShardedSiblingGroup:
         elif self.peer is not None and x.shape[-1] == x.numel():
             return self.peer.forward(self.layer, x, self.name, nm, self.n_full)       # [members, n_full], exchange done in-kernel
         else:
-            y = self.layer(x)
+            y = self.layer._forward_impl(x)  # no autograd node: the exchange carries no gradient
         return exchange_stacked(y, nm, self.rank, self.world, group=self.pg)            # [..., members, n_full]
 
     def member_forward(self, i, x):
