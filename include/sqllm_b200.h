@@ -48,7 +48,8 @@ extern "C" {
 #define SQLLM_EWORKSPACE (-3) /* workspace missing or too small */
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
-                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t (backward compatible, same version) */
+                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad (backward compatible,
+                                 same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -182,6 +183,28 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void 
 #define SQLLM_BWD_TC_MIN_ROWS 96
 int sqllm_lutgemm_t(const sqllm_lutgemv_args *args, const void *dy, int dy_dtype, void *dx, int dx_dtype, int path,
                     void *stream);
+
+/* Gradients of the layer's continuous parameters (fine-tuning the codebook with the indices fixed), from G = x^T . dy:
+ *   G[k][c]          = sum_m x[m][k] dy[m][c]
+ *   dlut[c][v]       = sum_{k : idx(k,c) = v} G[k][c]                              [out_features][2^bits]
+ *   dvals[e]         = G[cols[e]][c] for e in CSR row c and 0 <= cols[e] < K, else 0    [nnz]
+ *   dfull_rows[k][j] = G[k][full_row_indices[j]] if 0 <= full_row_indices[j] < N, else 0 [in_features][topX]
+ * x [M][in_features] and dy [M][out_features] are row-major (x_dtype, dy_dtype: SQLLM_DT_*, any pair); args->batch = M.  The outputs
+ * are fp32, written (not accumulated); a NULL output is not computed.  dvals needs args->rows / cols (the entries of CSR rows
+ * [rows[0], rows[out_features]) are written; args->vals is not read), dfull_rows needs args->full_row_indices and topX >= 1
+ * (args->full_rows is not read); the lookup table is not read either.  Duplicate CSR entries and duplicate dense-row channels each
+ * get the full G of their position.  The gradient is that of the exact codebook whatever sqllm_set_lut_mode says.
+ *   path 1 = tensor cores (x and dy both fp16 or both bf16): wgmma m64n128k16 on the operands as given, exact products, fp32 sums.
+ *   path 2 = CUDA cores (any dtype pair): fp32 products and sums of the values as given.
+ *   path 0 = path 1 when x and dy are both fp16 or both bf16 and M >= SQLLM_LUT_GRAD_TC_MIN_ROWS, else path 2.
+ * Both reduce each 128 x 128 tile of G over M in fixed chunks, bucket it in ascending k, and add the bins of the CTAs of a
+ * thread-block cluster (which split in_features) in rank order: every output is written once in a fixed order, bit-reproducible.
+ * Requirements (checked, SQLLM_EINVAL otherwise): in_features % 32 == 0, out_features >= 1, batch >= 1, non-null qweight / x / dy,
+ * at least one output, qweight and the outputs 4-byte aligned, x and dy aligned to their element size, topX >= 0.  No workspace,
+ * no allocation, no host synchronisation: CUDA-graph capturable and safe on several streams at once. */
+#define SQLLM_LUT_GRAD_TC_MIN_ROWS 8
+int sqllm_lut_grad(const sqllm_lutgemv_args *args, const void *x, int x_dtype, const void *dy, int dy_dtype, float *dlut, float *dvals,
+                   float *dfull_rows, int path, void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

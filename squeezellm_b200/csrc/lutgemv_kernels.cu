@@ -7,7 +7,9 @@
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
 // LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused), a few fp16 rows a multi-row GEMV with a cluster split-K
 // (lutgemv_rows.cuh, sqllm_lutgemv_rows).  The input gradient dx = dy . W^T has a transposed LUT-GEMM on the tensor cores
-// (lutgemm_tc_t.cuh) and one on the CUDA cores (lutgemm_t.cuh), both behind sqllm_lutgemm_t.
+// (lutgemm_tc_t.cuh) and one on the CUDA cores (lutgemm_t.cuh), both behind sqllm_lutgemm_t.  The gradients of the codebook,
+// the CSR values and the dense rows come from G = x^T . dy, bucketed by the packed indices: on the tensor cores
+// (lut_grad_tc.cuh) or the CUDA cores (lut_grad.cuh), both behind sqllm_lut_grad.
 //
 // Two GEMV kernels live here.  lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default
 // (fast) fused mode, whatever its width: a layer narrower than one strip is a layer whose only strip is ragged.
@@ -920,6 +922,8 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemm_tc.cuh"
 #include "lutgemm_t.cuh"
 #include "lutgemm_tc_t.cuh"
+#include "lut_grad.cuh"
+#include "lut_grad_tc.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
 // tables to their own size - up to 64 KB - so the host needs the real address, not a worst case; the kernel re-checks it)
@@ -1653,6 +1657,17 @@ KT kt_lookup(int bits, int RB) {
     return RB == 1 ? lutgemm_t_kernel<3, 1> : RB == 2 ? lutgemm_t_kernel<3, 2> : RB == 4 ? lutgemm_t_kernel<3, 4> : lutgemm_t_kernel<3, 8>;
 }
 
+// ---- codebook gradient (lut_grad.cuh, lut_grad_tc.cuh): plan -------------------------------------------------------------
+// K splits S (the cluster size) from K, N and the SM count only: the smallest S in {1, 2, 4, 8} that gives at least one CTA per
+// SM, with at least two k-tiles per CTA.
+int lg_split(int K, int N, int sm) {
+    using namespace lg;
+    const int ktiles = (K + TK - 1) / TK, ctiles = (N + TC - 1) / TC;
+    int S = 1;
+    while (S < MAX_SPLIT && 4 * S <= ktiles && (long long)ctiles * S < sm) S *= 2;
+    return S;
+}
+
 // ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
 // arena instead of y ---------------------------------------------------------------------------------------------------------------
 int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
@@ -1975,6 +1990,81 @@ int sqllm_lutgemm_t(const sqllm_lutgemv_args *a, const void *dy, int dy_dtype, v
     cfg.numAttrs = 1;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, kt_lookup(a->bits, pl.RB), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_t launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+int sqllm_lut_grad(const sqllm_lutgemv_args *a, const void *x, int x_dtype, const void *dy, int dy_dtype, float *dlut, float *dvals,
+                   float *dfull_rows, int path, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
+    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
+    if (a->out_features <= 0) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
+    if ((a->out_features + lg::TC - 1) / lg::TC > 65535) return fail(SQLLM_EINVAL, "out_features=%d exceeds %d", a->out_features, 65535 * lg::TC);
+    if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x and dy) must be >= 1 (got %d)", a->batch);
+    if (!a->qweight) return fail(SQLLM_EINVAL, "qweight must not be null");
+    if (!x || !dy) return fail(SQLLM_EINVAL, "x / dy must not be null");
+    const auto dt_ok = [](int d) { return d == SQLLM_DT_F32 || d == SQLLM_DT_F16 || d == SQLLM_DT_BF16; };
+    if (!dt_ok(x_dtype)) return fail(SQLLM_EINVAL, "x_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", x_dtype);
+    if (!dt_ok(dy_dtype)) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
+    if (path < 0 || path > 2) return fail(SQLLM_EINVAL, "path=%d must be 0 (auto), 1 (tensor cores) or 2 (CUDA cores)", path);
+    const bool tc_dtypes = x_dtype == dy_dtype && x_dtype != SQLLM_DT_F32;
+    if (path == 1 && !tc_dtypes)
+        return fail(SQLLM_EINVAL, "path=1 (tensor cores) takes x and dy both fp16 or both bf16 (got x_dtype=%d, dy_dtype=%d)", x_dtype, dy_dtype);
+    if (!dlut && !dvals && !dfull_rows) return fail(SQLLM_EINVAL, "no output requested: dlut, dvals and dfull_rows are all null");
+    if (dvals && (!a->rows || !a->cols)) return fail(SQLLM_EINVAL, "dvals needs the CSR arrays (rows, cols)");
+    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
+    if (dfull_rows && (!a->full_row_indices || a->topX < 1)) return fail(SQLLM_EINVAL, "dfull_rows needs the dense rows (full_row_indices, topX >= 1)");
+    if (reinterpret_cast<uintptr_t>(a->qweight) & 3) return fail(SQLLM_EINVAL, "qweight must be 4-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(x) & (x_dtype == SQLLM_DT_F32 ? 3 : 1)) || (reinterpret_cast<uintptr_t>(dy) & (dy_dtype == SQLLM_DT_F32 ? 3 : 1)))
+        return fail(SQLLM_EINVAL, "x and dy must be aligned to their element size");
+    if ((reinterpret_cast<uintptr_t>(dlut) & 3) || (reinterpret_cast<uintptr_t>(dvals) & 3) || (reinterpret_cast<uintptr_t>(dfull_rows) & 3))
+        return fail(SQLLM_EINVAL, "dlut, dvals and dfull_rows must be 4-byte aligned");
+    if (path == 0) path = tc_dtypes && a->batch >= SQLLM_LUT_GRAD_TC_MIN_ROWS ? 1 : 2;
+
+    lg::PG p;
+    memset(&p, 0, sizeof(p));
+    p.qw = reinterpret_cast<const uint32_t *>(a->qweight);
+    p.x = x; p.dy = dy; p.x_dt = x_dtype; p.dy_dt = dy_dtype;
+    p.rows = dvals ? a->rows : nullptr; p.cols = dvals ? a->cols : nullptr;
+    p.fri = dfull_rows ? a->full_row_indices : nullptr; p.topX = dfull_rows ? a->topX : 0;
+    p.dlut = dlut; p.dvals = dvals; p.dfull = dfull_rows;
+    p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
+    p.ktiles = (a->in_features + lg::TK - 1) / lg::TK;
+    p.x_al16 = (reinterpret_cast<uintptr_t>(x) & 15) == 0;  // in_features % 32 == 0: every row is then 16-byte aligned
+    p.dy_al16 = (reinterpret_cast<uintptr_t>(dy) & 15) == 0 && a->out_features % 8 == 0;
+    const bool bf = dy_dtype == SQLLM_DT_BF16;
+    void (*kern)(const lg::PG);
+    int smem;
+    if (path == 1) {
+        kern = bf ? (a->bits == 4 ? lgt::lut_grad_tc_kernel<4, true> : lgt::lut_grad_tc_kernel<3, true>)
+                  : (a->bits == 4 ? lgt::lut_grad_tc_kernel<4, false> : lgt::lut_grad_tc_kernel<3, false>);
+        smem = lgt::SMEM;
+    } else {
+        kern = a->bits == 4 ? lg::lut_grad_kernel<4> : lg::lut_grad_kernel<3>;
+        smem = lg::SMEM;
+    }
+    int S = 1;
+    {
+        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+        int dev = 0;
+        int rc = cur_dev(dev);
+        if (rc) return rc;
+        S = lg_split(a->in_features, a->out_features, g_dev[dev].sm);
+        if ((rc = set_max_smem(g_dev[dev], kern, smem))) return rc;
+    }
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(S, (a->out_features + lg::TC - 1) / lg::TC);
+    cfg.blockDim = dim3(lg::THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = static_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lut_grad launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

@@ -10,7 +10,8 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemm_t`, `unpack_indices`, `abi_version`, `fused_limits`.
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemm_t`, `lut_grad`, `unpack_indices`, `abi_version`,
+// `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -258,6 +259,17 @@ torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor
     return y;
 }
 
+// SQLLM_DT_* of an fp32 / fp16 / bf16 tensor
+int dtype_code(const torch::Tensor &t, const char *what) {
+    switch (t.scalar_type()) {
+        case torch::kFloat32: return SQLLM_DT_F32;
+        case torch::kFloat16: return SQLLM_DT_F16;
+        case torch::kBFloat16: return SQLLM_DT_BF16;
+        default: TORCH_CHECK(false, what, " must be fp16, bf16 or fp32 (got ", t.scalar_type(), ")");
+    }
+    return -1;
+}
+
 // dx [M, in] = dy [M, out] . W^T (LUT + CSR + dense rows), in dy's dtype (fp16, bf16 or fp32): the input gradient of
 // QuantLinearLUT (sqllm_lutgemm_t).  path: "auto" (the library picks), "tc" (tensor cores) or "cuda" (CUDA cores).
 torch::Tensor lutgemm_t(torch::Tensor dy, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
@@ -268,13 +280,7 @@ torch::Tensor lutgemm_t(torch::Tensor dy, torch::Tensor qweight, torch::Tensor l
     sqllm_lutgemv_args a;
     const float *bias_p;
     fill_layer_args(a, bias_p, dy, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices, false);
-    int dt;
-    switch (dy.scalar_type()) {
-        case torch::kFloat32: dt = SQLLM_DT_F32; break;
-        case torch::kFloat16: dt = SQLLM_DT_F16; break;
-        case torch::kBFloat16: dt = SQLLM_DT_BF16; break;
-        default: TORCH_CHECK(false, "lutgemm_t: dy must be fp16, bf16 or fp32 (got ", dy.scalar_type(), ")");
-    }
+    const int dt = dtype_code(dy, "lutgemm_t: dy");
     TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", "lutgemm_t: path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
     TORCH_CHECK(dy.dim() == 2 && dy.size(1) == a.out_features, "lutgemm_t: dy must be [M, out_features=", a.out_features, "]");
     TORCH_CHECK(dy.size(0) >= 1 && dy.size(0) <= INT32_MAX, "lutgemm_t: dy must have 1 to 2^31-1 rows");
@@ -283,6 +289,42 @@ torch::Tensor lutgemm_t(torch::Tensor dy, torch::Tensor qweight, torch::Tensor l
     check_status(sqllm_lutgemm_t(&a, dy.data_ptr(), dt, dx.data_ptr(), dt, path == "auto" ? 0 : path == "tc" ? 1 : 2, cur_stream()),
                  "quant_cuda.lutgemm_t");
     return dx;
+}
+
+// (dlut [out, 2^bits], dvals [nnz], dfull_rows [in, topX]) fp32 from x [M, in] and dy [M, out] (sqllm_lut_grad): the gradients of
+// QuantLinearLUT's codebook, CSR values and dense rows, one launch; None for an output not asked for.  path: "auto", "tc" or "cuda".
+py::tuple lut_grad(torch::Tensor x, torch::Tensor dy, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                   c10::optional<torch::Tensor> rows, c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                   c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices, bool want_lut, bool want_vals,
+                   bool want_full_rows, const std::string &path) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices, false);
+    const int xdt = dtype_code(x, "lut_grad: x"), dydt = dtype_code(dy, "lut_grad: dy");
+    TORCH_CHECK(dy.is_cuda() && dy.is_contiguous() && dy.device() == x.device(), "lut_grad: dy must be a contiguous CUDA tensor on x's device");
+    TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", "lut_grad: path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
+    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lut_grad: x must be [M, in_features=", a.in_features, "]");
+    TORCH_CHECK(dy.dim() == 2 && dy.size(1) == a.out_features && dy.size(0) == x.size(0),
+                "lut_grad: dy must be [M=", x.size(0), ", out_features=", a.out_features, "]");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lut_grad: x must have 1 to 2^31-1 rows");
+    TORCH_CHECK(want_lut || want_vals || want_full_rows, "lut_grad: nothing requested (want_lut, want_vals and want_full_rows are all False)");
+    TORCH_CHECK(!want_vals || a.rows, "lut_grad: want_vals needs the CSR arrays rows / cols / vals");
+    TORCH_CHECK(!want_full_rows || a.topX > 0, "lut_grad: want_full_rows needs full_rows / full_row_indices");
+    a.batch = (int)x.size(0);
+    const auto f32 = x.options().dtype(torch::kFloat32);
+    torch::Tensor dlut, dvals, dfull;
+    if (want_lut) dlut = torch::empty({(int64_t)a.out_features, (int64_t)1 << bits}, f32);
+    if (want_vals) dvals = torch::zeros({vals->numel()}, f32);  // entries outside the CSR rows' range [rows[0], rows[out]) stay 0
+    if (want_full_rows) dfull = torch::empty({(int64_t)a.in_features, (int64_t)a.topX}, f32);
+    float *pl = want_lut ? dlut.data_ptr<float>() : nullptr, *pv = want_vals && dvals.numel() ? dvals.data_ptr<float>() : nullptr;
+    float *pf = want_full_rows ? dfull.data_ptr<float>() : nullptr;
+    if (pl || pv || pf)  // else only an empty dvals was asked for
+        check_status(sqllm_lut_grad(&a, x.data_ptr(), xdt, dy.data_ptr(), dydt, pl, pv, pf, path == "auto" ? 0 : path == "tc" ? 1 : 2,
+                                    cur_stream()),
+                     "quant_cuda.lut_grad");
+    auto opt = [](const torch::Tensor &t) -> py::object { return t.defined() ? py::cast(t) : py::none(); };
+    return py::make_tuple(opt(dlut), opt(dvals), opt(dfull));
 }
 
 // y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16/fp32 with numel == in; returns [out] in x's dtype
@@ -449,6 +491,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("dy"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("rows") = py::none(),
           py::arg("cols") = py::none(), py::arg("vals") = py::none(), py::arg("full_rows") = py::none(),
           py::arg("full_row_indices") = py::none(), py::arg("path") = "auto");
+    m.def("lut_grad", &lut_grad, "gradients of QuantLinearLUT's codebook, CSR values and dense rows from x [M, in] and dy [M, out]: "
+          "(dlut, dvals, dfull_rows) fp32, None where not requested, one launch",
+          py::arg("x"), py::arg("dy"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("rows") = py::none(),
+          py::arg("cols") = py::none(), py::arg("vals") = py::none(), py::arg("full_rows") = py::none(),
+          py::arg("full_row_indices") = py::none(), py::arg("want_lut") = true, py::arg("want_vals") = false,
+          py::arg("want_full_rows") = false, py::arg("path") = "auto");
     m.def("lutgemv_fused_exchange", &lutgemv_fused_exchange,
           "fused matvec of a column shard that stores its result into every rank's symmetric arena (NVLink peer memory) and waits for the peers'",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias"), py::arg("rows"), py::arg("cols"),

@@ -130,7 +130,8 @@ class SiblingGroup:
 
 def fuse_siblings(model, groups=LLAMA_SIBLINGS, share_storage=True):
     """Group sibling QuantLinearLUT attributes of every sub-module of `model` (default: LLaMA's q/k/v and gate/up).
-    Call it after the checkpoint is loaded and the model is on its device.  Returns the SiblingGroup list."""
+    Call it after the checkpoint is loaded and the model is on its device.  Groups with a member whose codebook is being trained
+    (QuantLinearLUT.train_codebook) are left unfused.  Returns the SiblingGroup list."""
     made = []
     for mod in model.modules():
         for names in groups:
@@ -140,6 +141,8 @@ def fuse_siblings(model, groups=LLAMA_SIBLINGS, share_storage=True):
             if any(getattr(m, "_sibling_group", None) is not None for m in ms):
                 continue
             if len({(m.infeatures, m.bits, m.qweight.device) for m in ms}) != 1:
+                continue
+            if any(m._trained for m in ms):  # codebook training (QuantLinearLUT.train_codebook) runs on unstacked layers only
                 continue
             made.append(SiblingGroup(ms, share_storage=share_storage))
     return made

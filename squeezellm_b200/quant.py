@@ -23,6 +23,9 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
     bf16 gradients of at least `BWD_TC_MIN_ROWS` rows, else on the CUDA cores; outliers and dense rows included); the buffers are constants and get no gradient.  The forward of such a call takes the same route
     and gives the same bits as without grad; every other call goes exactly as before.  `use_fused` does not affect the
     backward.  The sharded, exchange and sequence paths (sharding.py, runtime.py) give no gradient.
+  * `train_codebook()` makes the codebook (and optionally the CSR values, dense rows and bias) nn.Parameters on the same storage:
+    their gradients come from ONE more launch (`quant_cuda.lut_grad`: G = x^T . dy bucketed by the packed indices); the indices
+    stay fixed and the checkpoint format does not change.
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
     (quant.py:238,282 vs quant_cuda.cpp:257-270), i.e. an AttributeError at the first forward.
@@ -163,6 +166,9 @@ class QuantLinearLUT(nn.Module):
     def pack2(self, linear, lookup_table, include_sparse, num_nonzero_per_thread=-1):
         """Fill the buffers from per-channel (centroids, indices) and an outlier matrix
         (reference quant.py:97-208).  lookup_table = (lut, outliers); lut[c][0] = (centroids, indices)."""
+        if self._trained:  # it replaces the tensors, which would leave the trained parameters (and an optimizer's references) behind
+            raise RuntimeError(f"QuantLinearLUT.pack2: the layer's {', '.join(self._trained)} are trained parameters "
+                               "(train_codebook); pack2 fills the buffers of a layer before training, not after")
         if self.include_bias:
             self.bias = linear.bias.clone()
         lut, outliers = lookup_table
@@ -211,13 +217,55 @@ class QuantLinearLUT(nn.Module):
     def forward(self, x):
         # a sibling member asks its group, whose stacked layer comes back here: the gradient flows through the stacked layer's
         # node and autograd's slice backward adds the members' shares
+        if self._trained:
+            params = tuple(getattr(self, n) for n in self._trained)
+            if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+                return _QuantLinearLUTCodebookFunction.apply(x, self, self._trained, *params)
+            return self._forward_impl(x)
         if self._sibling_group is None and torch.is_grad_enabled() and x.requires_grad:
             return _QuantLinearLUTFunction.apply(x, self)
         return self._forward_impl(x)
 
+    TRAINABLE = ("lookup_table", "vals", "full_rows", "bias")
+    _trained = ()  # names of the tensors train_codebook made parameters, in TRAINABLE order
+
+    def train_codebook(self, lookup_table=True, vals=False, full_rows=False, bias=False):
+        """Make the selected tensors trainable: the per-channel codebook `lookup_table` [out, 2^bits], the CSR outlier values
+        `vals`, the dense rows `full_rows` [in, topX] and the `bias`.  Each becomes an nn.Parameter under the same name and on the
+        same storage, so state_dict keys (the checkpoint format) do not change; the packed indices stay fixed.  Returns the list of
+        the selected parameters (e.g. for an optimizer).  The backward then computes their gradients in one extra launch
+        (quant_cuda.lut_grad) besides the input gradient.  Calling it again adds to the set; nothing is made untrainable."""
+        if self._sibling_group is not None:
+            raise RuntimeError("QuantLinearLUT.train_codebook: this layer is a member of a sibling group (fusion.fuse_siblings); "
+                               "codebook training needs the layers unfused: call train_codebook before fuse_siblings")
+        want = [n for n, on in zip(self.TRAINABLE, (lookup_table, vals, full_rows, bias)) if on]
+        rows, cols, vals_t, fr, fri = self._sparse_args()
+        have = {"lookup_table": self.lookup_table, "vals": vals_t, "full_rows": fr, "bias": self.bias}
+        for n in want:
+            if have[n] is None:
+                what = {"vals": "CSR outliers (include_sparse with rows / cols / vals)", "full_rows": "dense rows (topX > 0)",
+                        "bias": "bias"}.get(n, n)
+                raise ValueError(f"QuantLinearLUT.train_codebook: the layer has no {what}, so `{n}` cannot be trained")
+            if n != "bias" and have[n].dtype != torch.float32:  # checked for every tensor before any is converted
+                raise ValueError(f"QuantLinearLUT.train_codebook: `{n}` must be fp32 (got {have[n].dtype})")
+        for n in want:
+            t = getattr(self, n)
+            if not isinstance(t, nn.Parameter):
+                del self._buffers[n]
+                self.register_parameter(n, nn.Parameter(t))  # same storage, same state_dict key
+        self._trained = tuple(n for n in self.TRAINABLE if n in want or n in self._trained)
+        return [getattr(self, n) for n in want]
+
     def _grad_buffers(self):
         """The tensors the input gradient reads (the layer's weights as the backward sees them)."""
         return (self.qweight, self.lookup_table) + tuple(t for t in self._sparse_args() if t is not None)
+
+    def _codebook_grad(self, x, dy, names):
+        """(dlut, dvals, dfull_rows) for x [M, in] and dy [M, out] (quant_cuda.lut_grad, one launch), None where not in names."""
+        rows, cols, vals, fr, fri = self._sparse_args()
+        return quant_cuda.lut_grad(_aligned(x), _aligned(dy), self.qweight, self.lookup_table, self.bits, rows, cols, vals, fr, fri,
+                                   want_lut="lookup_table" in names, want_vals="vals" in names,
+                                   want_full_rows="full_rows" in names, path="auto")
 
     def _input_grad(self, dy):
         """dx [M, in] = dy [M, out] . W^T in dy's dtype (quant_cuda.lutgemm_t): the backward of every forward route.  fp16 / bf16
@@ -307,6 +355,47 @@ class _QuantLinearLUTFunction(torch.autograd.Function):
             return torch.zeros(ctx.x_shape, dtype=ctx.x_dtype, device=dy.device), None
         dx = layer._input_grad(dy)
         return dx.to(ctx.x_dtype).reshape(ctx.x_shape), None
+
+
+class _QuantLinearLUTCodebookFunction(torch.autograd.Function):
+    """y = QuantLinearLUT._forward_impl(x) for a layer with trained tensors (QuantLinearLUT.train_codebook): dx = dy . W^T as in
+    _QuantLinearLUTFunction, the codebook / CSR-value / dense-row gradients from G = x^T . dy in one quant_cuda.lut_grad launch,
+    dbias = sum of dy over the rows.  x is saved only when one of the first three is wanted."""
+
+    @staticmethod
+    def forward(ctx, x, layer, names, *params):
+        ctx.layer, ctx.names = layer, names
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.versions = [(t, t._version) for t in layer._grad_buffers() + ((layer.bias,) if "bias" in names else ())]
+        ctx.grid_names = tuple(n for i, n in enumerate(names) if n != "bias" and ctx.needs_input_grad[3 + i])
+        if ctx.grid_names:
+            ctx.save_for_backward(x)
+        return layer._forward_impl(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        layer, names = ctx.layer, ctx.names
+        now = layer._grad_buffers() + ((layer.bias,) if "bias" in names else ())
+        if len(now) != len(ctx.versions) or any(t is not u or t._version != v for (t, v), u in zip(ctx.versions, now)):
+            raise RuntimeError("QuantLinearLUT: the layer's buffers were modified or replaced between forward and backward; "
+                               "the gradients would use the new weights")
+        dy = dy.reshape(-1, layer.outfeatures)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = (layer._input_grad(dy).to(ctx.x_dtype) if dy.shape[0] else
+                  torch.zeros(ctx.x_shape, dtype=ctx.x_dtype, device=dy.device)).reshape(ctx.x_shape)
+        grads = dict.fromkeys(names)
+        if ctx.grid_names:
+            (x,) = ctx.saved_tensors
+            if dy.shape[0]:
+                dlut, dvals, dfull = layer._codebook_grad(x.reshape(-1, layer.infeatures), dy, ctx.grid_names)
+                grads.update(lookup_table=dlut, vals=dvals, full_rows=dfull)
+            else:
+                grads.update({n: torch.zeros_like(getattr(layer, n)) for n in ctx.grid_names})
+        if "bias" in names and ctx.needs_input_grad[3 + names.index("bias")]:
+            grads["bias"] = dy.sum(0, dtype=torch.float32).to(layer.bias.dtype)
+        return (dx, None, None) + tuple(grads[n] if ctx.needs_input_grad[3 + i] else None for i, n in enumerate(names))
 
 
 def make_quant_lut(module, names, bits, name="", include_sparse=False, numvals=None, topX=0, balanced=False,
