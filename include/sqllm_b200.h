@@ -48,8 +48,8 @@ extern "C" {
 #define SQLLM_EWORKSPACE (-3) /* workspace missing or too small */
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
-                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad (backward compatible,
-                                 same version) */
+                                 later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
+                                 sqllm_lutgemm_fused_dt (backward compatible, same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -156,10 +156,23 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void
 int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
                        void *stream);
 
-/* Element types of sqllm_lutgemm_t's dy and dx. */
+/* Element types of the tensors of sqllm_lutgemm_fused_dt, sqllm_lutgemm_t and sqllm_lut_grad. */
 #define SQLLM_DT_F32 0
 #define SQLLM_DT_F16 1
 #define SQLLM_DT_BF16 2
+
+/* sqllm_lutgemm_fused for fp16 or bf16 x: the same tensor-core LUT-GEMM, y[m][c] = bias[c] + LUT-GEMM + CSR + dense rows, written
+ * (not accumulated), from x [M][in_features] (row-major) of x_dtype = SQLLM_DT_F16 or SQLLM_DT_BF16 into y [M][out_features] of
+ * y_dtype = SQLLM_DT_F32 or x's dtype.  fp16 x is computed exactly as by sqllm_lutgemm_fused (which calls this).  bf16 x: every
+ * folded weight (codebook + CSR + dense rows, over the column's power-of-two scale) is split exactly into three bf16 parts,
+ * hi = bf16(w), mid = bf16(w - hi), lo = bf16(w - hi - mid), which carry the fp32 value down to bf16's subnormal range; x is
+ * exact in bf16, so every product on the tensor cores is exact and the sums are fp32.  The codebook is always used as stored:
+ * sqllm_set_lut_mode does not apply.  Every output is written once by one CTA in a fixed order: results are bit-reproducible,
+ * and a row's bits do not depend on M or on the other rows.  Requirements (checked, SQLLM_EINVAL otherwise): those of
+ * sqllm_lutgemm_fused, and the two dtype codes above.  No workspace, no allocation, no host synchronisation: CUDA-graph
+ * capturable and safe on several streams at once. */
+int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
+                           void *stream);
 
 /* Input gradient of the layer (backpropagation through QuantLinearLUT): the transposed LUT-GEMM
  *   dx[m][k] = sum_c dy[m][c] W[k][c],   W[k][c] = LUT[c][idx(k,c)] + CSR(c,k) + sum_j full_rows[k][j] [full_row_indices[j] == c]

@@ -19,7 +19,8 @@
 //     sum = fma(acc, S_i, sum) (S_i is a power of two: exact).  hi + lo carry about 22 significant bits of w / S_i.  Known limit:
 //     a weight more than about 2^20 below the largest weight of its chunk falls into fp16's subnormal range in lo and is kept to
 //     about 2^-40 of that largest weight (absolute, not relative).
-//   * bf16 dy: w is split into three bf16 parts (about 24 significant bits); bf16 has fp32's exponent range, so no scale.
+//   * bf16 dy: w is split into three bf16 parts (tc::split3_bf16x2, all 24 significant bits); bf16 has fp32's exponent range, so
+//     no scale.
 // CSR columns outside [0, K) and dense-row channels outside [0, N) are ignored; duplicate entries add up.  No limit on topX or on the
 // entries per CSR row (each thread scans its column's CSR row in full: rows need not be ascending).
 #pragma once
@@ -226,19 +227,10 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_t_kernel(const PT p) {
                 uint32_t pv[3][4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    uint32_t h[3][2];
+                    uint32_t h[3];
+                    tc::split3_bf16x2(w[8 * t + 2 * u], w[8 * t + 2 * u + 1], h);
 #pragma unroll
-                    for (int s = 0; s < 2; ++s) {
-                        float r = w[8 * t + 2 * u + s];
-#pragma unroll
-                        for (int pp = 0; pp < 3; ++pp) {
-                            const __nv_bfloat16 x = __float2bfloat16_rn(r);
-                            h[pp][s] = (uint32_t)__bfloat16_as_ushort(x);
-                            r -= __bfloat162float(x);  // exact
-                        }
-                    }
-#pragma unroll
-                    for (int pp = 0; pp < 3; ++pp) pv[pp][u] = h[pp][0] | (h[pp][1] << 16);
+                    for (int pp = 0; pp < 3; ++pp) pv[pp][u] = h[pp];
                 }
                 const uint32_t off = rowoff + ((((uint32_t)(4 * (q & 1) + t)) ^ (uint32_t)(c & 7)) << 4);
 #pragma unroll

@@ -4,8 +4,8 @@
 //   VecQuant{3,4}MatMulKernelNUQPerChannel[Batched]  (:741-1038)   LUT GEMV
 //   SPMV_ATOMIC[_BATCHED]                            (:1040-1089)  CSR outliers
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
-// and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 inputs have a tensor-core
-// LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused), a few fp16 rows a multi-row GEMV with a cluster split-K
+// and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 / bf16 inputs have a
+// tensor-core LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused_dt), a few fp16 rows a multi-row GEMV with a cluster split-K
 // (lutgemv_rows.cuh, sqllm_lutgemv_rows).  The input gradient dx = dy . W^T has a transposed LUT-GEMM on the tensor cores
 // (lutgemm_tc_t.cuh) and one on the CUDA cores (lutgemm_t.cuh), both behind sqllm_lutgemm_t.  The gradients of the codebook,
 // the CSR values and the dense rows come from G = x^T . dy, bucketed by the packed indices: on the tensor cores
@@ -1806,6 +1806,11 @@ int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int
 }
 
 int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
+    return sqllm_lutgemm_fused_dt(a, x, SQLLM_DT_F16, y, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias, stream);
+}
+
+int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
+                           void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
     if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
     if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
@@ -1814,31 +1819,41 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x) must be >= 1 (got %d)", a->batch);
     if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
     if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
+    if (x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "x_dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", x_dtype);
+    if (y_dtype != SQLLM_DT_F32 && y_dtype != x_dtype) return fail(SQLLM_EINVAL, "y_dtype=%d must be SQLLM_DT_F32 or x's dtype (%d)", y_dtype, x_dtype);
     if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3) || (reinterpret_cast<uintptr_t>(bias) & 3))
         return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
     if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
     if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
     if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
     if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
+    const bool bf = x_dtype == SQLLM_DT_BF16;
     {
         std::lock_guard<std::recursive_mutex> lk(g_state_mu);
         int dev = 0;
         int rc = cur_dev(dev);
-        if (!rc) rc = set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4>, tc::SMEM);
-        if (!rc) rc = set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3>, tc::SMEM);
+        if (!rc) rc = bf ? set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4, true>, tc::L<3>::SMEM)
+                         : set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4, false>, tc::L<2>::SMEM);
+        if (!rc) rc = bf ? set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3, true>, tc::L<3>::SMEM)
+                         : set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3, false>, tc::L<2>::SMEM);
         if (rc) return rc;
     }
     tc::PT p;
     p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
-    p.x = static_cast<const __half *>(x); p.y = y; p.y_is_half = y_is_half ? 1 : 0; p.bias = bias;
+    p.x = static_cast<const unsigned short *>(x); p.y = y; p.y_16 = y_dtype != SQLLM_DT_F32; p.bias = bias;
     p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
     const bool hyb = a->full_rows && a->topX > 0;
     p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
     p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
     const dim3 grid((a->batch + tc::BM - 1) / tc::BM, (a->out_features + tc::BN - 1) / tc::BN);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (a->bits == 4) tc::lutgemm_tc_kernel<4><<<grid, tc::THREADS, tc::SMEM, st>>>(p);
-    else tc::lutgemm_tc_kernel<3><<<grid, tc::THREADS, tc::SMEM, st>>>(p);
+    if (bf) {
+        if (a->bits == 4) tc::lutgemm_tc_kernel<4, true><<<grid, tc::THREADS, tc::L<3>::SMEM, st>>>(p);
+        else tc::lutgemm_tc_kernel<3, true><<<grid, tc::THREADS, tc::L<3>::SMEM, st>>>(p);
+    } else {
+        if (a->bits == 4) tc::lutgemm_tc_kernel<4, false><<<grid, tc::THREADS, tc::L<2>::SMEM, st>>>(p);
+        else tc::lutgemm_tc_kernel<3, false><<<grid, tc::THREADS, tc::L<2>::SMEM, st>>>(p);
+    }
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_fused launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;

@@ -221,8 +221,19 @@ void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
     TORCH_CHECK(x.numel() == a.in_features, "x has ", x.numel(), " elements, expected in_features=", a.in_features);
 }
 
-// y [M, out] fp16 = bias + LUT-GEMM(x) [+ CSR] [+ dense rows] from fp16 x [M, in], on the tensor cores (sqllm_lutgemm_fused):
-// QuantLinearLUT.forward's batched branch (squeezellm/quant.py:314-379) in one launch.
+// SQLLM_DT_* of an fp32 / fp16 / bf16 tensor
+int dtype_code(const torch::Tensor &t, const char *what) {
+    switch (t.scalar_type()) {
+        case torch::kFloat32: return SQLLM_DT_F32;
+        case torch::kFloat16: return SQLLM_DT_F16;
+        case torch::kBFloat16: return SQLLM_DT_BF16;
+        default: TORCH_CHECK(false, what, " must be fp16, bf16 or fp32 (got ", t.scalar_type(), ")");
+    }
+    return -1;
+}
+
+// y [M, out] = bias + LUT-GEMM(x) [+ CSR] [+ dense rows] from fp16 or bf16 x [M, in], in x's dtype, on the tensor cores
+// (sqllm_lutgemm_fused_dt): QuantLinearLUT.forward's batched branch (squeezellm/quant.py:314-379) in one launch.
 torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
                             c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
                             c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
@@ -230,13 +241,15 @@ torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
     sqllm_lutgemv_args a;
     const float *bias_p;
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
-    TORCH_CHECK(x.scalar_type() == torch::kFloat16, "lutgemm_fused: x must be fp16");
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, false);
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kBFloat16,
+                "lutgemm_fused: x must be fp16 or bf16 (got ", x.scalar_type(), ")");
+    const int dt = dtype_code(x, "lutgemm_fused: x");
     TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemm_fused: x must be [M, in_features=", a.in_features, "]");
     TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemm_fused: x must have 1 to 2^31-1 rows");
     a.batch = (int)x.size(0);
     torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
-    check_status(sqllm_lutgemm_fused(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemm_fused");
+    check_status(sqllm_lutgemm_fused_dt(&a, x.data_ptr(), dt, y.data_ptr(), dt, bias_p, cur_stream()), "quant_cuda.lutgemm_fused");
     return y;
 }
 
@@ -257,17 +270,6 @@ torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor
     torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
     check_status(sqllm_lutgemv_rows(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemv_rows");
     return y;
-}
-
-// SQLLM_DT_* of an fp32 / fp16 / bf16 tensor
-int dtype_code(const torch::Tensor &t, const char *what) {
-    switch (t.scalar_type()) {
-        case torch::kFloat32: return SQLLM_DT_F32;
-        case torch::kFloat16: return SQLLM_DT_F16;
-        case torch::kBFloat16: return SQLLM_DT_BF16;
-        default: TORCH_CHECK(false, what, " must be fp16, bf16 or fp32 (got ", t.scalar_type(), ")");
-    }
-    return -1;
 }
 
 // dx [M, in] = dy [M, out] . W^T (LUT + CSR + dense rows), in dy's dtype (fp16, bf16 or fp32): the input gradient of
@@ -479,7 +481,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
-    m.def("lutgemm_fused", &lutgemm_fused, "fused QuantLinearLUT matmul on the tensor cores: fp16 x [M, in] -> fp16 y [M, out] (bias, CSR, dense rows), one launch",
+    m.def("lutgemm_fused", &lutgemm_fused, "fused QuantLinearLUT matmul on the tensor cores: fp16 or bf16 x [M, in] -> y [M, out] in x's dtype (bias, CSR, dense rows), one launch",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());

@@ -11,13 +11,14 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
     zeros + x.float() + 1-3 launches + y.to(dtype).  Layers wider or with more dense rows than the fused launch
     takes (`FUSED_LIMITS`, from the extension) run the reference's 12 symbols instead.  Set
     `QuantLinearLUT.use_fused = False` to go through the reference's 12 symbols exactly as quant.py does.
-  * `forward` with fp16 x of at least `TC_MIN_ROWS` rows (prefill, evaluation; reference quant.py:314-379) uses ONE
-    tensor-core launch (`quant_cuda.lutgemm_fused`, outliers and dense rows folded into the weight tiles) instead of
-    zeros + x.float() + 1-3 batched launches + out.to(dtype).
+  * `forward` with fp16 x of at least `TC_MIN_ROWS` rows, or bf16 x of at least `BF16_TC_MIN_ROWS` rows (prefill, evaluation,
+    bf16 training; reference quant.py:314-379) uses ONE tensor-core launch (`quant_cuda.lutgemm_fused`, outliers and dense rows
+    folded into the weight tiles, output in x's dtype, bit-reproducible) instead of zeros + x.float() + 1-3 batched launches +
+    out.to(dtype).
   * `forward` with fp16 x of 2 to `ROWS_MAX` rows (and fewer than `TC_MIN_ROWS`; several sequences decoding at once, speculative-
     decoding verification, short prompts) uses ONE CUDA-core launch (`quant_cuda.lutgemv_rows`: a multi-row LUT-GEMV whose
-    thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence.  fp32 / bf16 x and
-    `use_fused = False` keep the reference's batched symbols.
+    thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence.  fp32 x, bf16 x of
+    2 to `BF16_TC_MIN_ROWS - 1` rows and `use_fused = False` keep the reference's batched symbols.
   * `loss.backward()` works through the layer when x requires grad (the reference has no backward: its outputs carry no
     graph).  x gets dx = dy . W^T from ONE launch (`quant_cuda.lutgemm_t`: a transposed LUT-GEMM, on the tensor cores for fp16 /
     bf16 gradients of at least `BWD_TC_MIN_ROWS` rows, else on the CUDA cores; outliers and dense rows included); the buffers are constants and get no gradient.  The forward of such a call takes the same route
@@ -116,10 +117,14 @@ class QuantLinearLUT(nn.Module):
     """Drop-in layer replacement (reference quant.py:28)."""
 
     use_fused = True  # class-wide switch: fused single-launch forward vs the reference's 12-symbol sequence
-    # fp16 inputs of at least this many rows run the tensor-core LUT-GEMM (quant_cuda.lutgemm_fused); fewer rows, fp32 / bf16
-    # inputs and use_fused = False run the batched symbols.  64: where a whole 7B decoder layer gets faster on an H100 (DESIGN.md
+    # fp16 inputs of at least this many rows run the tensor-core LUT-GEMM (quant_cuda.lutgemm_fused); fewer rows, fp32 inputs
+    # and use_fused = False run the batched symbols (bf16 inputs: BF16_TC_MIN_ROWS).  64: where a whole 7B decoder layer gets faster on an H100 (DESIGN.md
     # section 3.6: 32 rows 1.08 vs 0.78 ms, 64 rows 1.09 vs 1.48 ms).
     TC_MIN_ROWS = 64
+    # bf16 inputs of at least this many rows run the same tensor-core LUT-GEMM with three bf16 weight parts; fewer rows run the
+    # batched symbols.  80: the smallest measured row count above TC_MIN_ROWS at which a whole 7B decoder layer is faster on an
+    # H100 (DESIGN.md section 3.6: 80 rows 1.48 vs 1.90 ms; the tensor cores already win at 64 rows, 1.46 vs 1.56 ms).
+    BF16_TC_MIN_ROWS = 80
     # fp16 inputs of 2 to ROWS_MAX rows (below TC_MIN_ROWS) run the multi-row GEMV (quant_cuda.lutgemv_rows).  63: it is faster than
     # the batched symbols on a whole 7B decoder layer at every measured row count up to 63 on an H100 (DESIGN.md section 3.9).
     ROWS_MAX = 63
@@ -295,7 +300,8 @@ class QuantLinearLUT(nn.Module):
             return y.to(dtype).reshape(outshape)
         out_shape = x.shape[:-1] + (self.outfeatures,)
         x = x.reshape(-1, x.shape[-1])
-        if QuantLinearLUT.use_fused and x.dtype == torch.float16 and x.shape[0] >= QuantLinearLUT.TC_MIN_ROWS:
+        tc_min = {torch.float16: QuantLinearLUT.TC_MIN_ROWS, torch.bfloat16: QuantLinearLUT.BF16_TC_MIN_ROWS}.get(x.dtype)
+        if QuantLinearLUT.use_fused and tc_min is not None and x.shape[0] >= tc_min:
             rows, cols, vals, fr, fri = self._sparse_args()
             out = quant_cuda.lutgemm_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                            None, rows, cols, vals, fr, fri).reshape(out_shape)
