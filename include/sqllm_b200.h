@@ -49,7 +49,8 @@ extern "C" {
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
-                                 sqllm_lutgemm_fused_dt (backward compatible, same version) */
+                                 sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt (backward compatible,
+                                 same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -156,7 +157,8 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void
 int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
                        void *stream);
 
-/* Element types of the tensors of sqllm_lutgemm_fused_dt, sqllm_lutgemm_t and sqllm_lut_grad. */
+/* Element types of the tensors of sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_lutgemm_t and
+ * sqllm_lut_grad. */
 #define SQLLM_DT_F32 0
 #define SQLLM_DT_F16 1
 #define SQLLM_DT_BF16 2
@@ -173,6 +175,27 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void 
  * capturable and safe on several streams at once. */
 int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
                            void *stream);
+
+/* sqllm_lutgemv_fused with the element types as codes, and bf16 x besides fp32 and fp16: the same one-vector LUT-GEMV,
+ * y[c] = bias[c] + LUT-GEMV + CSR + dense rows, written (not accumulated).  Pairs (x_dtype, y_dtype):
+ *   SQLLM_DT_F32  x: y SQLLM_DT_F32 or SQLLM_DT_F16;   SQLLM_DT_F16 x: y SQLLM_DT_F32 or SQLLM_DT_F16;
+ *   SQLLM_DT_BF16 x: y SQLLM_DT_F32 or SQLLM_DT_BF16;  any other pair: SQLLM_EINVAL (the message names both codes).
+ * fp32 and fp16 x are computed exactly as by sqllm_lutgemv_fused (which calls this).  bf16 x is staged in its own type and every
+ * value is widened to fp32 exactly before its product: the exact fp32 codebook and fp32 sums, in both summation modes
+ * (sqllm_set_deterministic).  SQLLM_LUT_FP16_PAIR applies to fp16 x only: bf16 x keeps the exact table, as fp32 x does.  Every
+ * other requirement (alignment, SQLLM_FUSED_MAX_*, the workspace) is that of sqllm_lutgemv_fused; CUDA-graph capturable, one
+ * workspace per stream. */
+int sqllm_lutgemv_fused_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
+                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* sqllm_lutgemv_rows for fp16 or bf16 x: the same multi-row LUT-GEMV from x [M][in_features] of x_dtype = SQLLM_DT_F16 or
+ * SQLLM_DT_BF16 into y [M][out_features] of y_dtype = SQLLM_DT_F32 or x's dtype; any other pair: SQLLM_EINVAL (the message names
+ * both codes).  fp16 x is computed exactly as by sqllm_lutgemv_rows (which calls this).  bf16 x is widened to fp32 exactly as the
+ * CTA stages it; from there on both types run the same code: exact fp32 codebook, fp32 sums, bit-reproducible, a row's result
+ * independent of M and of the other rows.  Every other requirement is that of sqllm_lutgemv_rows (in_features <=
+ * SQLLM_ROWS_MAX_IN, out_features % 4 == 0, alignment); no workspace, CUDA-graph capturable, safe on several streams at once. */
+int sqllm_lutgemv_rows_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
+                          void *stream);
 
 /* Input gradient of the layer (backpropagation through QuantLinearLUT): the transposed LUT-GEMM
  *   dx[m][k] = sum_c dy[m][c] W[k][c],   W[k][c] = LUT[c][idx(k,c)] + CSR(c,k) + sum_j full_rows[k][j] [full_row_indices[j] == c]

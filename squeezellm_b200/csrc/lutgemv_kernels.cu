@@ -5,8 +5,8 @@
 //   SPMV_ATOMIC[_BATCHED]                            (:1040-1089)  CSR outliers
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.  Prefill-sized fp16 / bf16 inputs have a
-// tensor-core LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused_dt), a few fp16 rows a multi-row GEMV with a cluster split-K
-// (lutgemv_rows.cuh, sqllm_lutgemv_rows).  The input gradient dx = dy . W^T has a transposed LUT-GEMM on the tensor cores
+// tensor-core LUT-GEMM of their own (lutgemm_tc.cuh, sqllm_lutgemm_fused_dt), a few fp16 / bf16 rows a multi-row GEMV with a cluster
+// split-K (lutgemv_rows.cuh, sqllm_lutgemv_rows_dt).  The input gradient dx = dy . W^T has a transposed LUT-GEMM on the tensor cores
 // (lutgemm_tc_t.cuh) and one on the CUDA cores (lutgemm_t.cuh), both behind sqllm_lutgemm_t.  The gradients of the codebook,
 // the CSR values and the dense rows come from G = x^T . dy, bucketed by the packed indices: on the tensor cores
 // (lut_grad_tc.cuh) or the CUDA cores (lut_grad.cuh), both behind sqllm_lut_grad.
@@ -28,7 +28,7 @@
 //         gathers); products go into pairs of fp32 accumulators (two fma.rn.f32 per pair).  No tensor cores: this is a gather-bound GEMV.
 //       - sparse warp: CSR rows spread evenly over all CTAs, staged with 16-byte cp.async, x gathered in batches,
 //         per-row sums in storage order; plus a k-slice of the topX dense rows.
-//   * Only the slice of x a CTA needs is staged (fp32, converted from fp16 on the way in).
+//   * Only the slice of x a CTA needs is staged (fp32, converted from fp16 or bf16 on the way in).
 //   * Flush: per-strip partials in the workspace and one ticket per contributor; the last contributor of a strip sums them in a
 //     fixed order, adds the bias and stores y.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
@@ -43,6 +43,7 @@
 
 #include <algorithm>
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -77,8 +78,8 @@ constexpr size_t WS_HEADER = WS_DBOX_OFF + (size_t)MAX_TOPX_FUSED * MAX_GRID_V2 
 struct Params {
     const uint32_t *qw;
     const float *lut;
-    const void *x;      // fp32 or fp16 [K]
-    void *out;          // fp32/fp16 y
+    const void *x;      // [K], x_dt
+    void *out;          // y, y_dt
     const float *bias;  // may be null
     const int *rows, *cols;
     const float *vals;
@@ -95,7 +96,7 @@ struct Params {
     int xfloats;  // floats in the x staging buffer
     int hc;       // CTAs that take a slice of the dense rows
     int hrows;    // k-rows per such CTA
-    int x_is_half, y_is_half;
+    int x_dt, y_dt;     // SQLLM_DT_* of x (fp32, fp16 or bf16) and of y (fp32 or 16-bit)
     int maxc;     // max dense contributors per strip
     float *ws_part;   // [strips][maxc+1][64]
     int *ws_cnt;      // [strips]
@@ -184,6 +185,20 @@ __device__ __forceinline__ float sum2(uint64_t v) {
     float lo, hi;
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
     return lo + hi;
+}
+// Element types of x in the GEMV kernels: float, __half or __nv_bfloat16.  A 16-bit y has x's 16-bit type (fp16 for fp32 x).
+template <typename XT> constexpr bool x_is16 = !std::is_same<XT, float>::value;
+template <typename XT> using y16_t = typename std::conditional<std::is_same<XT, __nv_bfloat16>::value, __nv_bfloat16, __half>::type;
+template <typename T> __device__ __forceinline__ T f32_to(float v);
+template <> __device__ __forceinline__ __half f32_to<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 f32_to<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+// the two bf16 values of a word (lo, hi) as fp32, exactly: a bf16 is the upper half of its fp32 (one shift, one mask)
+__device__ __forceinline__ float2 bf16x2_to_f32x2(uint32_t h) { return make_float2(__uint_as_float(h << 16), __uint_as_float(h & 0xFFFF0000u)); }
+// ... and of either 16-bit type
+template <typename XT>
+__device__ __forceinline__ float2 x16x2_to_f32x2(uint32_t h) {
+    if constexpr (std::is_same<XT, __nv_bfloat16>::value) return bf16x2_to_f32x2(h);
+    else return __half22float2(*reinterpret_cast<const __half2 *>(&h));
 }
 __device__ __forceinline__ float warp_sum(float v) {  // fixed xor tree -> deterministic
 #pragma unroll
@@ -401,6 +416,11 @@ __device__ __forceinline__ void hybrid_totals(const Params &p, uint32_t stage_u3
     }
     __syncwarp();
 }
+__device__ __forceinline__ void store_y(const Params &p, int col, float v) {
+    if (p.y_dt == SQLLM_DT_F16) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(v);
+    else if (p.y_dt == SQLLM_DT_BF16) reinterpret_cast<__nv_bfloat16 *>(p.out)[col] = __float2bfloat16_rn(v);
+    else reinterpret_cast<float *>(p.out)[col] = v;
+}
 __device__ __forceinline__ void final_store(const Params &p, int strip, int c, int nd, const float *hyb_tot) {
     const int col = strip * STRIP + c;
     if (col >= p.N) return;
@@ -412,8 +432,7 @@ __device__ __forceinline__ void final_store(const Params &p, int strip, int c, i
         for (int j = 0; j < p.topX; ++j)
             if (__ldg(p.fri + j) == col) tot += hyb_tot[j];
     if (p.bias) tot += p.bias[col];
-    if (p.y_is_half) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(tot);
-    else reinterpret_cast<float *>(p.out)[col] = tot;
+    store_y(p, col, tot);
 }
 // one warp takes a ticket on `strip` and, if it is the last contributor, reduces and stores the strip's 64 columns
 __device__ __forceinline__ void warp_ticket(const Params &p, int strip, int lane, uint32_t hstage_u32, const float *hstage, float *hyb_tot) {
@@ -435,7 +454,9 @@ __device__ __forceinline__ void warp_ticket(const Params &p, int strip, int lane
 }
 
 __device__ __forceinline__ float load_x(const Params &p, int k) {  // read-only path: x stays in L1 across the gathers
-    return p.x_is_half ? __half2float(__ldg(reinterpret_cast<const __half *>(p.x) + k)) : __ldg(reinterpret_cast<const float *>(p.x) + k);
+    if (p.x_dt == SQLLM_DT_F16) return __half2float(__ldg(reinterpret_cast<const __half *>(p.x) + k));
+    if (p.x_dt == SQLLM_DT_BF16) return __uint_as_float((uint32_t)__ldg(reinterpret_cast<const unsigned short *>(p.x) + k) << 16);
+    return __ldg(reinterpret_cast<const float *>(p.x) + k);
 }
 
 // =================================================================================================
@@ -748,12 +769,19 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
             const int dst_unit = p.x_direct ? ua : (seg * R + ua - r0);     // compact: indexed by unit offset
             const int nfl = (ub - ua) * C::XU;
             const int src_f = ua * C::XU, dst_f = dst_unit * C::XU;
-            if (p.x_is_half) {
+            if (p.x_dt == SQLLM_DT_F16) {
                 const __half *xh = reinterpret_cast<const __half *>(p.x) + src_f;
                 for (int e = tid; e < nfl / 4; e += NW * 32) {  // 4 halves in, one float4 out per thread: conflict-free stores
                     const uint2 u = __ldg(reinterpret_cast<const uint2 *>(xh) + e);
                     const __half2 *h = reinterpret_cast<const __half2 *>(&u);
                     const float2 f0 = __half22float2(h[0]), f1 = __half22float2(h[1]);
+                    reinterpret_cast<float4 *>(xs + dst_f)[e] = make_float4(f0.x, f0.y, f1.x, f1.y);
+                }
+            } else if (p.x_dt == SQLLM_DT_BF16) {
+                const __nv_bfloat16 *xb = reinterpret_cast<const __nv_bfloat16 *>(p.x) + src_f;
+                for (int e = tid; e < nfl / 4; e += NW * 32) {  // the same, 4 bf16 in
+                    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(xb) + e);
+                    const float2 f0 = bf16x2_to_f32x2(u.x), f1 = bf16x2_to_f32x2(u.y);
                     reinterpret_cast<float4 *>(xs + dst_f)[e] = make_float4(f0.x, f0.y, f1.x, f1.y);
                 }
             } else {
@@ -855,8 +883,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) lutgemv_kernel(const Par
                 const int col = strip * STRIP + c;
                 if (col < N) {
                     if (p.bias) tot += p.bias[col];
-                    if (p.y_is_half) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(tot);
-                    else reinterpret_cast<float *>(p.out)[col] = tot;
+                    store_y(p, col, tot);
                 }
             } else {
                 const int slot = (int)blockIdx.x - (int)(((long long)strip * R) / p.chunk);
@@ -1226,19 +1253,23 @@ int lut_mode() {
 
 typedef void (*K2)(const v2::P2, const CUtensorMap, const CUtensorMap);
 struct K2Info { K2 fn; int tab, stage; };
-// fused: variant 0: exact, fp32 x ; 1: exact, fp16 x ; 2: fp16 pair table, fp16 x.  Accumulate mode (the 12 symbols): variant 0 only.
+// fused: variant 0: exact, fp32 x ; 1: exact, fp16 x ; 2: fp16 pair table, fp16 x ; 3: exact, bf16 x.  Accumulate mode (the 12
+// symbols): variant 0 only.
+constexpr int K2_VARIANTS = 4;
 K2Info k2_lookup(int bits, int variant, bool fused) {
-#define K2E(B, M, XH, F) K2Info{v2::lutgemv2_kernel<B, M, XH, F>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE}
+#define K2E(B, M, XT, F) K2Info{v2::lutgemv2_kernel<B, M, XT, F>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE}
     if (bits == 4) {
-        if (!fused) return K2E(4, 0, false, false);
-        if (variant == 0) return K2E(4, 0, false, true);
-        if (variant == 1) return K2E(4, 0, true, true);
-        return K2E(4, 1, true, true);
+        if (!fused) return K2E(4, 0, float, false);
+        if (variant == 0) return K2E(4, 0, float, true);
+        if (variant == 1) return K2E(4, 0, __half, true);
+        if (variant == 3) return K2E(4, 0, __nv_bfloat16, true);
+        return K2E(4, 1, __half, true);
     }
-    if (!fused) return K2E(3, 0, false, false);
-    if (variant == 0) return K2E(3, 0, false, true);
-    if (variant == 1) return K2E(3, 0, true, true);
-    return K2E(3, 1, true, true);
+    if (!fused) return K2E(3, 0, float, false);
+    if (variant == 0) return K2E(3, 0, float, true);
+    if (variant == 1) return K2E(3, 0, __half, true);
+    if (variant == 3) return K2E(3, 0, __nv_bfloat16, true);
+    return K2E(3, 1, __half, true);
 #undef K2E
 }
 
@@ -1289,7 +1320,7 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
         DevInfo &d = g_dev[dev];
         for (int b = 3; b <= 4; ++b) {
             if ((rc = set_max_smem(d, k2_lookup(b, 0, false).fn, 227 * 1024))) return rc;
-            for (int v = 0; v < 3; ++v)
+            for (int v = 0; v < K2_VARIANTS; ++v)
                 if ((rc = set_max_smem(d, k2_lookup(b, v, true).fn, 227 * 1024))) return rc;
         }
         if ((rc = smem_window(d))) return rc;
@@ -1608,7 +1639,7 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     return SQLLM_OK;
 }
 
-// ---- a few fp16 rows (lutgemv_rows.cuh): plan + launch ------------------------------------------------------------------
+// ---- a few fp16 / bf16 rows (lutgemv_rows.cuh): plan + launch ------------------------------------------------------------------
 // Slabs per strip S (the cluster size) from K, N and the SM count only - never from M, so that a row's result does not depend on
 // M: the smallest S in {1, 2, 4, 8} that gives at least two CTAs per SM and a slab of at most SLAB_GOAL inputs, with no more
 // slabs than units.  Rows per CTA RB from M: 2, 4 or 8 (a row computes the same bits whatever RB is).
@@ -1630,10 +1661,13 @@ int rows_plan(int bits, int K, int N, int M, int sm, RowsPlan &pl) {
 }
 
 typedef void (*KRows)(const rows::PR);
-KRows krows_lookup(int bits, int RB) {
-    if (bits == 4) return RB == 2 ? rows::lutgemv_rows_kernel<4, 2> : RB == 4 ? rows::lutgemv_rows_kernel<4, 4> : rows::lutgemv_rows_kernel<4, 8>;
-    return RB == 2 ? rows::lutgemv_rows_kernel<3, 2> : RB == 4 ? rows::lutgemv_rows_kernel<3, 4> : rows::lutgemv_rows_kernel<3, 8>;
+template <typename XT>
+KRows krows_lookup_t(int bits, int RB) {
+    using namespace rows;
+    if (bits == 4) return RB == 2 ? lutgemv_rows_kernel<4, 2, XT> : RB == 4 ? lutgemv_rows_kernel<4, 4, XT> : lutgemv_rows_kernel<4, 8, XT>;
+    return RB == 2 ? lutgemv_rows_kernel<3, 2, XT> : RB == 4 ? lutgemv_rows_kernel<3, 4, XT> : lutgemv_rows_kernel<3, 8, XT>;
 }
+KRows krows_lookup(int bits, int RB, bool bf16) { return bf16 ? krows_lookup_t<__nv_bfloat16>(bits, RB) : krows_lookup_t<__half>(bits, RB); }
 
 // ---- input gradient (lutgemm_t.cuh): plan + launch --------------------------------------------------------------------------
 // Strip splits S (the cluster size) from K, N and the SM count only - never from M, so that a row's result does not depend on M:
@@ -1670,7 +1704,8 @@ int lg_split(int K, int N, int sm) {
 
 // ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
 // arena instead of y ---------------------------------------------------------------------------------------------------------------
-int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half, const float *bias,
+// x_dt / y_dt: SQLLM_DT_* codes, a pair sqllm_lutgemv_fused_dt accepts
+int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y, int y_dt, const float *bias,
                   void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, cudaStream_t st) {
     int rc = check_common(a);
     if (rc) return rc;
@@ -1688,7 +1723,8 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, voi
         if (xc->out_features_full < xc->world * w) return fail(SQLLM_EINVAL, "out_features_full=%d < world * shard width = %d", xc->out_features_full, xc->world * w);
         if (!xc->peer_base) return fail(SQLLM_EINVAL, "peer_base must not be null");
         if ((xc->out_offset & 15) || (xc->flag_offset & 7) || (xc->state_offset & 7) || (xc->error_offset & 3)) return fail(SQLLM_EINVAL, "misaligned arena offsets");
-        if ((xc->out_features_full * (y_is_half ? 2 : 4)) % 16 || (w * (y_is_half ? 2 : 4)) % 8) return fail(SQLLM_EINVAL, "vector sizes must keep 8/16-byte store alignment");
+        const int yb = y_dt == SQLLM_DT_F32 ? 4 : 2;
+        if ((xc->out_features_full * yb) % 16 || (w * yb) % 8) return fail(SQLLM_EINVAL, "vector sizes must keep 8/16-byte store alignment");
     }
     const bool hyb = a->full_rows && a->topX > 0;
     if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
@@ -1702,14 +1738,16 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, voi
         q.ws_hbox = reinterpret_cast<unsigned long long *>(ws + WS_HBOX_OFF);
         q.ws_cbox = reinterpret_cast<unsigned long long *>(ws + WS_CBOX_OFF);
         q.ws_dbox = reinterpret_cast<unsigned long long *>(ws + WS_DBOX_OFF);
-        q.x = x; q.out = y; q.y_is_half = y_is_half; q.bias = bias;
+        q.x = x; q.out = y; q.y_is_half = y_dt != SQLLM_DT_F32; q.bias = bias;
         if (xc) {
             q.xw_world = xc->world; q.xw_rank = xc->rank; q.xw_members = xc->members; q.xw_nfull = xc->out_features_full;
             q.xw_base = reinterpret_cast<const unsigned long long *>(xc->peer_base);
             q.xw_out_off = xc->out_offset; q.xw_flag_off = xc->flag_offset; q.xw_state_off = xc->state_offset; q.xw_err_off = xc->error_offset;
         }
-        // layers narrower than one strip keep the exact codebook in the fp16 table mode: their results do not depend on the mode
-        return launch2(a, x_is_half ? (lut_mode() == 1 && a->out_features >= STRIP ? 2 : 1) : 0, true, q, st);
+        // layers narrower than one strip keep the exact codebook in the fp16 table mode: their results do not depend on the mode;
+        // bf16 x always does (the pair table multiplies fp16 by fp16)
+        const int variant = x_dt == SQLLM_DT_F16 ? (lut_mode() == 1 && a->out_features >= STRIP ? 2 : 1) : x_dt == SQLLM_DT_BF16 ? 3 : 0;
+        return launch2(a, variant, true, q, st);
     }
     Plan pl;
     rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, STAGE, pl);
@@ -1722,7 +1760,7 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, voi
     p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
     p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
     p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
-    p.x = x; p.x_is_half = x_is_half; p.out = y; p.y_is_half = y_is_half; p.bias = bias;
+    p.x = x; p.x_dt = x_dt; p.out = y; p.y_dt = y_dt; p.bias = bias;
     return launch(a, pl, p, st);
 }
 
@@ -1793,7 +1831,17 @@ int sqllm_lutgemv(const sqllm_lutgemv_args *a, void *stream) {
 
 int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_half, void *y, int y_is_half,
                         const float *bias, void *workspace, size_t workspace_bytes, void *stream) {
-    return lutgemv_fused(a, x, x_is_half, y, y_is_half, bias, workspace, workspace_bytes, nullptr, static_cast<cudaStream_t>(stream));
+    return sqllm_lutgemv_fused_dt(a, x, x_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, y, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias,
+                                  workspace, workspace_bytes, stream);
+}
+
+int sqllm_lutgemv_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
+                           void *workspace, size_t workspace_bytes, void *stream) {
+    const int y16 = x_dtype == SQLLM_DT_BF16 ? SQLLM_DT_BF16 : SQLLM_DT_F16;  // the 16-bit y of this x: fp16 for fp32 x
+    if ((x_dtype != SQLLM_DT_F32 && x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) || (y_dtype != SQLLM_DT_F32 && y_dtype != y16))
+        return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or the "
+                                  "16-bit type of x (SQLLM_DT_F16 for fp32 x)", x_dtype, y_dtype);
+    return lutgemv_fused(a, x, x_dtype, y, y_dtype, bias, workspace, workspace_bytes, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int x_is_half, int y_is_half, const float *bias,
@@ -1802,7 +1850,8 @@ int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int
         const int rc = check_common(a);
         return rc ? rc : fail(SQLLM_EINVAL, "x / exchange descriptor must not be null");
     }
-    return lutgemv_fused(a, x, x_is_half, nullptr, y_is_half, bias, workspace, workspace_bytes, xc, static_cast<cudaStream_t>(stream));
+    return lutgemv_fused(a, x, x_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, nullptr, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias, workspace,
+                         workspace_bytes, xc, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
@@ -1860,6 +1909,13 @@ int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dty
 }
 
 int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {
+    return sqllm_lutgemv_rows_dt(a, x, SQLLM_DT_F16, y, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias, stream);
+}
+
+int sqllm_lutgemv_rows_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias, void *stream) {
+    if ((x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) || (y_dtype != SQLLM_DT_F32 && y_dtype != x_dtype))
+        return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or x's dtype", x_dtype, y_dtype);
+    const bool bf = x_dtype == SQLLM_DT_BF16;
     if (!a) return fail(SQLLM_EINVAL, "null args");
     if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
     if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
@@ -1884,14 +1940,14 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int 
         if (rc) return rc;
         sm = g_dev[dev].sm;
         if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
-        if ((rc = set_max_smem(g_dev[dev], krows_lookup(a->bits, pl.RB), 227 * 1024))) return rc;
+        if ((rc = set_max_smem(g_dev[dev], krows_lookup(a->bits, pl.RB, bf), 227 * 1024))) return rc;
     }
     const int groups = (a->batch + pl.RB - 1) / pl.RB;
     if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
     rows::PR p;
     memset(&p, 0, sizeof(p));
     p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
-    p.x = static_cast<const __half *>(x); p.y = y; p.y_is_half = y_is_half ? 1 : 0; p.bias = bias;
+    p.x = x; p.y = y; p.y_16 = y_dtype != SQLLM_DT_F32; p.bias = bias;
     p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
     const bool hyb = a->full_rows && a->topX > 0;
     p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
@@ -1910,7 +1966,7 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int 
     attr.val.clusterDim.x = pl.S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, krows_lookup(a->bits, pl.RB), p);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, krows_lookup(a->bits, pl.RB, bf), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }

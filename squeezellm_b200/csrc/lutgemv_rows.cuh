@@ -1,13 +1,15 @@
-// lutgemv_rows.cuh - the multi-row LUT-GEMV behind sqllm_lutgemv_rows: 2 to 63 fp16 rows (decode of several sequences,
+// lutgemv_rows.cuh - the multi-row LUT-GEMV behind sqllm_lutgemv_rows_dt: a few fp16 or bf16 rows (decode of several sequences,
 // speculative-decoding verification, short prompts) in ONE launch.  Included by lutgemv_kernels.cu inside its anonymous namespace,
 // after lutgemm_batched.cuh, whose table layout, decode and row FMAs (batched::unit_fma) it shares.
 //
-//   y[m][c] = sum_k W[k][c] x[m][k] + CSR + dense rows (+ bias),  fp16 x [M][K], y fp16 or fp32, exact fp32 codebook, fp32 sums.
+//   y[m][c] = sum_k W[k][c] x[m][k] + CSR + dense rows (+ bias),  fp16 or bf16 x [M][K] (XT), y fp32 or x's type, exact fp32
+//   codebook, fp32 sums.
 //
 // Tiling: a CTA owns one 64-column strip, one K-slab and one group of RB rows; grid (S, strips, ceil(M / RB)), launched as clusters of
 // (S, 1, 1): the S CTAs of a cluster split the strip's K.  S comes from K, N and the SM count only (rows_plan), never from M, and
 // every row runs the same instructions whatever RB is, so a row's result does not depend on M or on the other rows.
-//   * x: the CTA stages its slab of its rows, converted to fp32, rows padded to an even number of units with zeros.
+//   * x: the CTA stages its slab of its rows, converted to fp32 (exact for both types), rows padded to an even number of units with
+//     zeros.  Nothing after the staging depends on x's type.
 //   * weights: each lane reads its 16 bytes per unit row straight from global memory, one position ahead (as lutgemm_batched_kernel),
 //     decodes its 4 columns x one unit once and runs them against all RB rows.
 //   * outliers, folded per slab: the CSR entries of the strip's 64 channels whose column lies in the slab (gathered from the staged
@@ -30,8 +32,8 @@ constexpr int MAX_SLABS = 8;          // S <= 8: portable cluster size
 struct PR {
     const uint32_t *qw;
     const float *lut;
-    const __half *x;    // [M][K]
-    void *y;            // [M][N], fp16 or fp32
+    const void *x;      // [M][K], fp16 or bf16 (the kernel's XT)
+    void *y;            // [M][N], fp32 or XT
     const float *bias;  // may be null
     const int *rows, *cols;
     const float *vals;
@@ -41,7 +43,7 @@ struct PR {
     int K, N, M, R;     // R = units per strip
     int ks;             // units per slab
     int kpad;           // floats per staged x row: ks rounded up to an even number of units
-    int y_is_half;
+    int y_16;           // y is XT, not fp32
     int qw_al16;        // qweight is 16-byte aligned: 16-byte weight loads
 };
 
@@ -71,7 +73,7 @@ __device__ __forceinline__ float4 ld_cluster_v4(uint32_t local, uint32_t rank) {
     return v;
 }
 
-template <int BITS, int RB>
+template <int BITS, int RB, typename XT>
 __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
     using C = batched::CB<BITS>;
     using L = SR<BITS, RB>;
@@ -105,9 +107,9 @@ __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
             const int b = e / n8, q = e - b * n8;
             float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
             if (b0 + b < p.M && 8 * q < kn) {
-                const uint4 h = __ldg(reinterpret_cast<const uint4 *>(p.x + (size_t)(b0 + b) * p.K + k_lo + 8 * q));
-                const float2 f0 = __half22float2(*reinterpret_cast<const __half2 *>(&h.x)), f1 = __half22float2(*reinterpret_cast<const __half2 *>(&h.y));
-                const float2 f2 = __half22float2(*reinterpret_cast<const __half2 *>(&h.z)), f3 = __half22float2(*reinterpret_cast<const __half2 *>(&h.w));
+                const uint4 h = __ldg(reinterpret_cast<const uint4 *>(static_cast<const XT *>(p.x) + (size_t)(b0 + b) * p.K + k_lo + 8 * q));
+                const float2 f0 = x16x2_to_f32x2<XT>(h.x), f1 = x16x2_to_f32x2<XT>(h.y);
+                const float2 f2 = x16x2_to_f32x2<XT>(h.z), f3 = x16x2_to_f32x2<XT>(h.w);
                 lo = make_float4(f0.x, f0.y, f1.x, f1.y);
                 hi = make_float4(f2.x, f2.y, f3.x, f3.y);
             }
@@ -245,12 +247,18 @@ __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
                 s.x += __ldg(p.bias + col); s.y += __ldg(p.bias + col + 1); s.z += __ldg(p.bias + col + 2); s.w += __ldg(p.bias + col + 3);
             }
             const size_t o = (size_t)row * p.N + col;
-            if (p.y_is_half) {
-                const __half2 h01 = __floats2half2_rn(s.x, s.y), h23 = __floats2half2_rn(s.z, s.w);
+            if (p.y_16) {
                 uint2 v;
-                v.x = *reinterpret_cast<const uint32_t *>(&h01);
-                v.y = *reinterpret_cast<const uint32_t *>(&h23);
-                *reinterpret_cast<uint2 *>(static_cast<__half *>(p.y) + o) = v;
+                if constexpr (std::is_same<XT, __nv_bfloat16>::value) {
+                    const __nv_bfloat162 h01 = __floats2bfloat162_rn(s.x, s.y), h23 = __floats2bfloat162_rn(s.z, s.w);
+                    v.x = *reinterpret_cast<const uint32_t *>(&h01);
+                    v.y = *reinterpret_cast<const uint32_t *>(&h23);
+                } else {
+                    const __half2 h01 = __floats2half2_rn(s.x, s.y), h23 = __floats2half2_rn(s.z, s.w);
+                    v.x = *reinterpret_cast<const uint32_t *>(&h01);
+                    v.y = *reinterpret_cast<const uint32_t *>(&h23);
+                }
+                *reinterpret_cast<uint2 *>(static_cast<XT *>(p.y) + o) = v;
             } else {
                 *reinterpret_cast<float4 *>(static_cast<float *>(p.y) + o) = s;
             }

@@ -87,7 +87,7 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
 template <int BITS, int MODE, bool MULTI>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c) {
     using C = C2<BITS, MODE>;
-    constexpr bool XH = true;
+    using XT = __half;
     constexpr int NTB = C::NTB;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -189,7 +189,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         // =========================== outlier warps (v2::sparse3, once per GEMV) ===========================
         for (int g = 0; g < ngemv; ++g) {
             const P2 &p = c.descs[g].p;
-            sparse3<XH, true>(p, base, warp - WARP_SP, lane, nullptr, (epoch << 10) | (uint32_t)(g + 1));
+            sparse3<XT, true>(p, base, warp - WARP_SP, lane, nullptr, (epoch << 10) | (uint32_t)(g + 1));
             TRACE(10, lane == 0);
             if (g + 1 < ngemv) bar_arrive(6, NCT + NSPW * 32);  // done reading this GEMV's x from shared memory
         }
@@ -485,9 +485,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 for (int k = 0; k < nstg; ++k) {
                     mbar_wait(bar_u32 + 8 * slot, par);
                     if (k < mine) {
-                        Fetch<BITS, XH> F;
-                        fetch2<BITS, XH>(F, stage_of(slot), xaddr);
-                        math2<BITS, MODE, XH>(F, jsel, l, segc, xaddr, A);
+                        Fetch<BITS, XT> F;
+                        fetch2<BITS, XT>(F, stage_of(slot), xaddr);
+                        math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);

@@ -17,8 +17,8 @@
 //   * fp16 PAIR table (MODE 1): entry [a | b<<BITS] = half2(LUT[a], LUT[b]) - one PRMT-built (4-bit: the byte of the packed word IS
 //     the entry number) shared-memory lookup serves TWO weights, and the products are fp16 x fp16 -> fp32 accumulate with
 //     exact products (fhfma2; tests/perf/microbench2.cu measures the loop).  The only rounding is LUT -> fp16 (2^-11 relative per centroid); it needs fp16 x.
-//   * x is staged whole (as fp16 when it is given as fp16), the sparse warps gather it from shared memory (sparse3: nothing else of
-//     theirs goes through shared memory).
+//   * x is staged whole in its own type (fp32, fp16 or bf16: the XT template parameter; 16-bit pairs are widened to fp32 in registers),
+//     the sparse warps gather it from shared memory (sparse3: nothing else of theirs goes through shared memory).
 #pragma once
 
 namespace v2 {
@@ -50,7 +50,7 @@ struct P2 {
     const uint32_t *qw;
     const float *lut;
     const void *x;
-    void *out;           // accumulate mode: float* mul ; fused: fp32/fp16 y
+    void *out;           // accumulate mode: float* mul ; fused: fp32 or 16-bit y (y16_t of x's type)
     const float *bias;
     const int *rows, *cols;
     const float *vals;
@@ -127,8 +127,10 @@ __device__ __forceinline__ void fhfma2(float &acc_lo, float &acc_hi, uint32_t w,
         "fma.rn.f32 %0, fwl, fxl, %0;\nfma.rn.f32 %1, fwh, fxh, %1;\n}"
         : "+f"(acc_lo), "+f"(acc_hi) : "r"(w), "r"(x));
 }
-__device__ __forceinline__ uint64_t half2_to_f32x2(uint32_t h) {
-    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&h));
+// the two 16-bit x values of a word (fp16 or bf16: XT) as a packed fp32 pair, exactly
+template <typename XT>
+__device__ __forceinline__ uint64_t x2_to_f32x2(uint32_t h) {
+    const float2 f = x16x2_to_f32x2<XT>(h);
     return pack2(f.x, f.y);
 }
 __device__ __forceinline__ uint32_t f32x2_to_half2(float lo, float hi) {
@@ -244,17 +246,19 @@ struct Acc {
     float f[8];
 };
 
-// What a lane pulls out of a stage for one position: its 16 bytes (x 3 rows for 3-bit) and - 4-bit only, 8 inputs - its slice of x.
-template <int BITS, bool XH> struct Fetch;
-template <> struct Fetch<4, true> { uint4 q, xh; };
-template <> struct Fetch<4, false> { uint4 q; float4 xa, xb; };
-template <bool XH> struct Fetch<3, XH> { uint4 a, b, c; };
+// What a lane pulls out of a stage for one position: its 16 bytes (x 3 rows for 3-bit) and - 4-bit only, 8 inputs - its slice of x
+// (X16: x is staged in a 16-bit type, fp16 or bf16).
+template <int BITS, bool X16> struct FetchX;
+template <> struct FetchX<4, true> { uint4 q, xh; };
+template <> struct FetchX<4, false> { uint4 q; float4 xa, xb; };
+template <bool X16> struct FetchX<3, X16> { uint4 a, b, c; };
+template <int BITS, typename XT> using Fetch = FetchX<BITS, x_is16<XT>>;
 
-template <int BITS, bool XH>
-__device__ __forceinline__ void fetch2(Fetch<BITS, XH> &F, const uint32_t unit_addr, const uint32_t xaddr) {
+template <int BITS, typename XT>
+__device__ __forceinline__ void fetch2(Fetch<BITS, XT> &F, const uint32_t unit_addr, const uint32_t xaddr) {
     if constexpr (BITS == 4) {
         F.q = lds_u4(unit_addr);
-        if constexpr (XH) F.xh = lds_u4(xaddr);
+        if constexpr (x_is16<XT>) F.xh = lds_u4(xaddr);
         else { F.xa = lds_v4(xaddr); F.xb = lds_v4(xaddr + 16); }
     } else {
         F.a = lds_u4(unit_addr);
@@ -264,11 +268,11 @@ __device__ __forceinline__ void fetch2(Fetch<BITS, XH> &F, const uint32_t unit_a
 }
 
 // 4-bit, exact fp32 table (v1's loop): E/O = even/odd nibbles in separate bytes, OR-ed with bits 12..15 of the table address.
-template <bool XH>
-__device__ __forceinline__ void consume4_exact(const Fetch<4, XH> &F, const int jsel, const uint32_t (&l)[4], const uint32_t segc, Acc &A) {
+template <typename XT>
+__device__ __forceinline__ void consume4_exact(const Fetch<4, XT> &F, const int jsel, const uint32_t (&l)[4], const uint32_t segc, Acc &A) {
     uint64_t x01, x23, x45, x67;
-    if constexpr (XH) {
-        x01 = half2_to_f32x2(F.xh.x); x23 = half2_to_f32x2(F.xh.y); x45 = half2_to_f32x2(F.xh.z); x67 = half2_to_f32x2(F.xh.w);
+    if constexpr (x_is16<XT>) {
+        x01 = x2_to_f32x2<XT>(F.xh.x); x23 = x2_to_f32x2<XT>(F.xh.y); x45 = x2_to_f32x2<XT>(F.xh.z); x67 = x2_to_f32x2<XT>(F.xh.w);
     } else {
         x01 = pack2(F.xa.x, F.xa.y); x23 = pack2(F.xa.z, F.xa.w); x45 = pack2(F.xb.x, F.xb.y); x67 = pack2(F.xb.z, F.xb.w);
     }
@@ -289,7 +293,7 @@ __device__ __forceinline__ void consume4_exact(const Fetch<4, XH> &F, const int 
     }
 }
 // 4-bit, fp16 pair table (64 KB aligned): byte j of a packed word = (index of input 2j) | (index of input 2j+1) << 4 = the entry number.
-__device__ __forceinline__ void consume4_pair(const Fetch<4, true> &F, const int jsel, const uint32_t (&l)[4], Acc &A) {
+__device__ __forceinline__ void consume4_pair(const Fetch<4, __half> &F, const int jsel, const uint32_t (&l)[4], Acc &A) {
     const uint4 q = F.q, xh = F.xh;  // halves (x0,x1) (x2,x3) (x4,x5) (x6,x7)
     const uint32_t w[4] = {jsel ? q.y : q.x, jsel ? q.x : q.y, jsel ? q.w : q.z, jsel ? q.z : q.w};
 #pragma unroll
@@ -333,10 +337,10 @@ __device__ __forceinline__ void consume3_pair_col(const uint32_t w0, const uint3
 }
 #undef LKP
 
-template <int BITS, int MODE, bool XH>
-__device__ __forceinline__ void math2(const Fetch<BITS, XH> &F, const int jsel, const uint32_t (&l)[4], const uint32_t segc, const uint32_t xaddr, Acc &A) {
+template <int BITS, int MODE, typename XT>
+__device__ __forceinline__ void math2(const Fetch<BITS, XT> &F, const int jsel, const uint32_t (&l)[4], const uint32_t segc, const uint32_t xaddr, Acc &A) {
     if constexpr (BITS == 4) {
-        if constexpr (MODE == 0) consume4_exact<XH>(F, jsel, l, segc, A);
+        if constexpr (MODE == 0) consume4_exact<XT>(F, jsel, l, segc, A);
         else consume4_pair(F, jsel, l, A);
     } else {
         const uint4 ga = F.a, gb = F.b, gc = F.c;
@@ -345,12 +349,12 @@ __device__ __forceinline__ void math2(const Fetch<BITS, XH> &F, const int jsel, 
         const uint32_t c[4] = {jsel ? gc.y : gc.x, jsel ? gc.x : gc.y, jsel ? gc.w : gc.z, jsel ? gc.z : gc.w};
         if constexpr (MODE == 0) {
             uint64_t xp[16];
-            if constexpr (XH) {
+            if constexpr (x_is16<XT>) {
 #pragma unroll
                 for (int v = 0; v < 4; ++v) {
                     const uint4 h = lds_u4(xaddr + 16 * v);
-                    xp[4 * v] = half2_to_f32x2(h.x); xp[4 * v + 1] = half2_to_f32x2(h.y);
-                    xp[4 * v + 2] = half2_to_f32x2(h.z); xp[4 * v + 3] = half2_to_f32x2(h.w);
+                    xp[4 * v] = x2_to_f32x2<XT>(h.x); xp[4 * v + 1] = x2_to_f32x2<XT>(h.y);
+                    xp[4 * v + 2] = x2_to_f32x2<XT>(h.z); xp[4 * v + 3] = x2_to_f32x2<XT>(h.w);
                 }
             } else {
 #pragma unroll
@@ -395,18 +399,19 @@ __device__ __forceinline__ void math2(const Fetch<BITS, XH> &F, const int jsel, 
 // (the rest is read after x: from L2, not from HBM - every owner of a dense-row channel waits for the slowest CTA's warp 0); one mailbox word per
 // (CTA, dense row), rows on the same channel combined (fused), or one red.add per dense row into its channel (accumulate).
 // ---------------------------------------------------------------------------------------------------------------------------
-template <bool XH>
+template <typename XT>
 __device__ __forceinline__ float xs_load(const uint32_t xs_u32, const int k) {
-    if constexpr (XH) {
+    if constexpr (x_is16<XT>) {
         unsigned short h;
         asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(xs_u32 + 2 * k));
-        return __half2float(__ushort_as_half(h));
+        if constexpr (std::is_same<XT, __nv_bfloat16>::value) return __uint_as_float((uint32_t)h << 16);
+        else return __half2float(__ushort_as_half(h));
     } else {
         return lds_f32(xs_u32 + 4 * k);
     }
 }
 
-template <bool XH, bool FUSED>
+template <typename XT, bool FUSED>
 __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const int spw, const int lane, float *acc_out, const uint32_t boxtag) {
     const int N = p.N;
     const uint32_t xs_u32 = base + OFF_X;
@@ -488,10 +493,10 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
 #pragma unroll
                 for (int i = 0; i < HYB_R2; ++i) {
                     const int k = kb + rs + nsl * i;
-                    if (rs < nsl && k < ke) a += hfr[i] * xs_load<XH>(xs_u32, k);
+                    if (rs < nsl && k < ke) a += hfr[i] * xs_load<XT>(xs_u32, k);
                 }
                 for (int k = kb + rs + nsl * HYB_R2; rs < nsl && k < ke; k += nsl)
-                    a += __ldg(p.full_rows + (size_t)k * p.topX + hj) * xs_load<XH>(xs_u32, k);
+                    a += __ldg(p.full_rows + (size_t)k * p.topX + hj) * xs_load<XT>(xs_u32, k);
                 for (int sl = 1; sl < nsl; ++sl) {  // fold the row slots onto slot 0 in fixed order
                     const float v = __shfl_sync(0xffffffffu, a, (hj + sl * p.topX) & 31);
                     if (rs == 0) a += v;
@@ -516,7 +521,7 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
                 j = jb + lane;
                 if (j < p.topX) {
                     const float *fr = p.full_rows + (size_t)kb * p.topX + j;
-                    for (int k = kb; k < ke; ++k, fr += p.topX) a += __ldg(fr) * xs_load<XH>(xs_u32, k);
+                    for (int k = kb; k < ke; ++k, fr += p.topX) a += __ldg(fr) * xs_load<XT>(xs_u32, k);
                 }
             }
             if constexpr (FUSED) {
@@ -537,7 +542,7 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
         {
             float xv[T];
 #pragma unroll
-            for (int t = 0; t < T; ++t) xv[t] = a0c + part + t * LPR < a1c ? xs_load<XH>(xs_u32, cc[t]) : 0.f;  // (padding: no gather)
+            for (int t = 0; t < T; ++t) xv[t] = a0c + part + t * LPR < a1c ? xs_load<XT>(xs_u32, cc[t]) : 0.f;  // (padding: no gather)
 #pragma unroll
             for (int t = 0; t < T; t += 2) { s0 = fmaf(vv[t], xv[t], s0); s1 = fmaf(vv[t + 1], xv[t + 1], s1); }
         }
@@ -555,10 +560,10 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
                           c3 = e + 96 < b1 ? __ldg(p.cols + e + 96) : 0;
                 const float v0 = __ldg(p.vals + e), v1 = e + 32 < b1 ? __ldg(p.vals + e + 32) : 0.f, v2 = e + 64 < b1 ? __ldg(p.vals + e + 64) : 0.f,
                             v3 = e + 96 < b1 ? __ldg(p.vals + e + 96) : 0.f;
-                a = fmaf(v0, xs_load<XH>(xs_u32, c0), a);
-                if (e + 32 < b1) b = fmaf(v1, xs_load<XH>(xs_u32, c1), b);
-                if (e + 64 < b1) a = fmaf(v2, xs_load<XH>(xs_u32, c2), a);
-                if (e + 96 < b1) b = fmaf(v3, xs_load<XH>(xs_u32, c3), b);
+                a = fmaf(v0, xs_load<XT>(xs_u32, c0), a);
+                if (e + 32 < b1) b = fmaf(v1, xs_load<XT>(xs_u32, c1), b);
+                if (e + 64 < b1) a = fmaf(v2, xs_load<XT>(xs_u32, c2), a);
+                if (e + 96 < b1) b = fmaf(v3, xs_load<XT>(xs_u32, c3), b);
             }
             a = warp_sum(a + b);
             if (lane == i) tot += a;
@@ -576,13 +581,15 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// The kernel.  MODE 0: exact fp32 table ; MODE 1: fp16 pair table (needs XH).  XH: x is given (and staged) as fp16.
+// The kernel.  MODE 0: exact fp32 table ; MODE 1: fp16 pair table (needs fp16 x).  XT: x's element type (float, __half or
+// __nv_bfloat16), in which it is given and staged; a 16-bit y (p.y_is_half) is y16_t<XT>.
 // ---------------------------------------------------------------------------------------------------------------------------
-template <int BITS, int MODE, bool XH, bool FUSED>
+template <int BITS, int MODE, typename XT, bool FUSED>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const __grid_constant__ CUtensorMap tm_big,
                                                                const __grid_constant__ CUtensorMap tm_small) {
     using C = C2<BITS, MODE>;
-    static_assert(MODE == 0 || XH, "the pair table multiplies fp16 by fp16: it needs fp16 x");
+    using Y16 = y16_t<XT>;
+    static_assert(MODE == 0 || std::is_same<XT, __half>::value, "the pair table multiplies fp16 by fp16: it needs fp16 x");
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     if (raw != p.smem_raw) __trap();  // the host planned the carve-up (table alignment) for another window address
@@ -592,7 +599,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     const uint32_t bar_u32 = base + OFF_BAR;
     const uint32_t xs_u32 = base + OFF_X;
     const int nstage = p.nstage;
-    const Carve cv(base, (uint32_t)((p.K * (XH ? 2 : 4) + 127) & ~127), 0u, C::TAB, 2, C::STAGE, nstage);
+    const Carve cv(base, (uint32_t)((p.K * (int)sizeof(XT) + 127) & ~127), 0u, C::TAB, 2, C::STAGE, nstage);
     const uint32_t lo_base = cv.lo_base, tab0 = cv.tab0, hi_base = cv.hi_base;
     const int n_lo = cv.n_lo;
 
@@ -672,7 +679,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             }
         }
     } else if (warp >= WARP_SP) {
-        sparse3<XH, FUSED>(p, base, warp - WARP_SP, lane, acc_out, 1u);
+        sparse3<XT, FUSED>(p, base, warp - WARP_SP, lane, acc_out, 1u);
         TRACE(10, lane == 0);
     } else if (warp >= WARP_BLD) {
         // =========================== table builders (2 warps, thread = column slot) ===========================
@@ -842,7 +849,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                 auto store_y = [&](int col, float yv) {
                     if (p.bias) yv += __ldg(p.bias + col);
                     if (p.xw_world == 0) {
-                        if (p.y_is_half) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(yv);
+                        if (p.y_is_half) reinterpret_cast<Y16 *>(p.out)[col] = f32_to<Y16>(yv);
                         else reinterpret_cast<float *>(p.out)[col] = yv;
                     } else {
                         // local column col of the stacked shard = column j of member m; it lands at [m][rank*w + j] of the
@@ -851,7 +858,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                         const unsigned long long e = (unsigned long long)mm * p.xw_nfull + (unsigned long long)p.xw_rank * w + j;
                         for (int pr = 0; pr < p.xw_world; ++pr) {
                             unsigned char *dst = reinterpret_cast<unsigned char *>(__ldg(p.xw_base + pr) + p.xw_out_off);
-                            if (p.y_is_half) *reinterpret_cast<__half *>(dst + 2 * e) = __float2half_rn(yv);
+                            if (p.y_is_half) *reinterpret_cast<Y16 *>(dst + 2 * e) = f32_to<Y16>(yv);
                             else *reinterpret_cast<float *>(dst + 4 * e) = yv;
                         }
                     }
@@ -950,7 +957,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         named_bar_sync(1, NCT);
         TRACE(3, tid == 0);
         {   // stage x whole, in its own type
-            const int n16 = p.K * (XH ? 2 : 4) / 16;
+            const int n16 = p.K * (int)sizeof(XT) / 16;
             for (int e = tid; e < n16; e += NCT) cp_async16(xs_u32 + 16 * e, reinterpret_cast<const unsigned char *>(p.x) + 16 * (size_t)e);
             cp_async_commit();
             cp_async_wait_all();
@@ -967,7 +974,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                                    (uint32_t)((((2 ^ jsel) << 4) | i16) << 2), (uint32_t)((((3 ^ jsel) << 4) | i16) << 2)};
         const uint32_t sacc_lane = base + OFF_SACC + (4 * i16) * 4;
         const uint32_t lane_in_stage = (uint32_t)((2 * warp + jsel) * C::UNIT + i16 * 16);
-        constexpr int XB = C::XU * (XH ? 2 : 4);  // bytes of x per unit
+        constexpr int XB = C::XU * (int)sizeof(XT);  // bytes of x per unit
         constexpr int XBS = SU2 * XB;             // ... per stage
 
         int slot = 0;
@@ -1004,9 +1011,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             for (int k = 0; k < nstg; ++k) {
                 mbar_wait(bar_u32 + 8 * slot, par);
                 if (k < mine) {
-                    Fetch<BITS, XH> F;
-                    fetch2<BITS, XH>(F, stage_of(slot), xaddr);
-                    math2<BITS, MODE, XH>(F, jsel, l, segc, xaddr, A);
+                    Fetch<BITS, XT> F;
+                    fetch2<BITS, XT>(F, stage_of(slot), xaddr);
+                    math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemm_t`, `lut_grad`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -211,13 +211,17 @@ void fill_layer_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
     }
 }
 
-// ... of the matvec entry points: x holds one input vector
+// ... of the matvec entry points: x holds one input vector, fp16 or fp32 (and bf16 where bf16_ok: lutgemv_fused; the exchange and
+// sequence paths are fp16 / fp32 only)
 void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
                      const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
                      const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
                      const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
-                     const c10::optional<torch::Tensor> &full_row_indices) {
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+                     const c10::optional<torch::Tensor> &full_row_indices, bool bf16_ok = false) {
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, !bf16_ok);
+    if (bf16_ok)
+        TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32 || x.scalar_type() == torch::kBFloat16,
+                    "x must be fp16, bf16 or fp32");
     TORCH_CHECK(x.numel() == a.in_features, "x has ", x.numel(), " elements, expected in_features=", a.in_features);
 }
 
@@ -254,7 +258,7 @@ torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
 }
 
 // y [M, out] fp16 = bias + LUT-GEMV(x) [+ CSR] [+ dense rows] from fp16 x [M, in], a few rows on the CUDA cores (sqllm_lutgemv_rows):
-// QuantLinearLUT.forward's batched branch for 2 to QuantLinearLUT.ROWS_MAX rows in one launch.
+// QuantLinearLUT.forward's batched branch for 2 to QuantLinearLUT.ROWS_MAX rows in one launch.  bf16 x: lutgemv_rows_bf16.
 torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
                            c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
                            c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
@@ -269,6 +273,26 @@ torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor
     a.batch = (int)x.size(0);
     torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
     check_status(sqllm_lutgemv_rows(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemv_rows");
+    return y;
+}
+
+// The same for bf16 x [M, in] -> bf16 y [M, out] (sqllm_lutgemv_rows_dt): QuantLinearLUT.forward's batched branch for 2 to
+// QuantLinearLUT.BF16_ROWS_MAX bf16 rows.  A symbol of its own, so that lutgemv_rows keeps meaning "the fp16 rows route".
+torch::Tensor lutgemv_rows_bf16(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                                c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                                c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                                c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, false);
+    TORCH_CHECK(x.scalar_type() == torch::kBFloat16, "lutgemv_rows_bf16: x must be bf16 (got ", x.scalar_type(), ")");
+    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemv_rows_bf16: x must be [M, in_features=", a.in_features, "]");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemv_rows_bf16: x must have 1 to 2^31-1 rows");
+    a.batch = (int)x.size(0);
+    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
+    check_status(sqllm_lutgemv_rows_dt(&a, x.data_ptr(), SQLLM_DT_BF16, y.data_ptr(), SQLLM_DT_BF16, bias_p, cur_stream()),
+                 "quant_cuda.lutgemv_rows_bf16");
     return y;
 }
 
@@ -329,7 +353,7 @@ py::tuple lut_grad(torch::Tensor x, torch::Tensor dy, torch::Tensor qweight, tor
     return py::make_tuple(opt(dlut), opt(dvals), opt(dfull));
 }
 
-// y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16/fp32 with numel == in; returns [out] in x's dtype
+// y = bias + LUT-GEMV(x) [+ CSR] [+ dense rows]; x fp16 / bf16 / fp32 with numel == in; returns [out] in x's dtype
 // (QuantLinearLUT.forward's matvec branch, squeezellm/quant.py:212-312, in one launch).
 torch::Tensor lutgemv_fused(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
                             c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
@@ -338,13 +362,13 @@ torch::Tensor lutgemv_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
     sqllm_lutgemv_args a;
     const float *bias_p;
-    fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, true);
     const size_t need_ws = sqllm_workspace_bytes(bits, a.in_features, a.out_features, a.topX);
     TORCH_CHECK(need_ws > 0, "sqllm_workspace_bytes failed: ", sqllm_last_error());
     torch::Tensor ws = workspace_for(x, need_ws);
     torch::Tensor y = torch::empty({(int64_t)a.out_features}, x.options());
-    const int half = x.scalar_type() == torch::kFloat16;
-    const int rc = sqllm_lutgemv_fused(&a, x.data_ptr(), half, y.data_ptr(), half, bias_p, ws.data_ptr(), (size_t)ws.numel(), cur_stream());
+    const int dt = dtype_code(x, "lutgemv_fused: x");
+    const int rc = sqllm_lutgemv_fused_dt(&a, x.data_ptr(), dt, y.data_ptr(), dt, bias_p, ws.data_ptr(), (size_t)ws.numel(), cur_stream());
     check_status(rc, "quant_cuda.lutgemv_fused");
     return y;
 }
@@ -477,7 +501,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("vecquant3matmul_spmv_hybrid_nuq_perchannel_batched", &hybrid<3, true>, "3-bit LUT matmul + CSR + dense rows, batched");
     m.def("vecquant4matmul_spmv_hybrid_nuq_perchannel_batched", &hybrid<4, true>, "4-bit LUT matmul + CSR + dense rows, batched");
     // additions
-    m.def("lutgemv_fused", &lutgemv_fused, "fused QuantLinearLUT matvec: fp16/fp32 x -> y (bias, CSR, dense rows), one launch",
+    m.def("lutgemv_fused", &lutgemv_fused, "fused QuantLinearLUT matvec: fp16 / bf16 / fp32 x -> y in x's dtype (bias, CSR, dense rows), one launch",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
@@ -486,6 +510,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
     m.def("lutgemv_rows", &lutgemv_rows, "fused QuantLinearLUT matmul for a few rows on the CUDA cores: fp16 x [M, in] -> fp16 y [M, out] (bias, CSR, dense rows), one launch",
+          py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
+          py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
+          py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
+    m.def("lutgemv_rows_bf16", &lutgemv_rows_bf16, "lutgemv_rows for bf16 x [M, in] -> bf16 y [M, out] (bias, CSR, dense rows), one launch",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());

@@ -6,7 +6,7 @@ rows, cols, vals, full_rows, full_row_indices, startrows), `pack2`, `forward` an
 as the reference, so `llama.py`-style loaders work unchanged.  Differences, all behind the same API:
 
   * `forward` (batch-1 branch, reference quant.py:212-312) uses ONE fused launch
-    (`quant_cuda.lutgemv_fused`: fp16/fp32 x in, y out in x's dtype, bias + CSR + dense rows fused;
+    (`quant_cuda.lutgemv_fused`: fp16 / bf16 / fp32 x in, y out in x's dtype, bias + CSR + dense rows fused;
     `quant_cuda.set_deterministic(True)` selects the bit-reproducible summation) instead of
     zeros + x.float() + 1-3 launches + y.to(dtype).  Layers wider or with more dense rows than the fused launch
     takes (`FUSED_LIMITS`, from the extension) run the reference's 12 symbols instead.  Set
@@ -17,8 +17,9 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
     out.to(dtype).
   * `forward` with fp16 x of 2 to `ROWS_MAX` rows (and fewer than `TC_MIN_ROWS`; several sequences decoding at once, speculative-
     decoding verification, short prompts) uses ONE CUDA-core launch (`quant_cuda.lutgemv_rows`: a multi-row LUT-GEMV whose
-    thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence.  fp32 x, bf16 x of
-    2 to `BF16_TC_MIN_ROWS - 1` rows and `use_fused = False` keep the reference's batched symbols.
+    thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence; bf16 x of 2 to
+    `BF16_ROWS_MAX` rows the same kernel with bf16 in and out (`quant_cuda.lutgemv_rows_bf16`).  fp32 x and `use_fused = False`
+    keep the reference's batched symbols.
   * `loss.backward()` works through the layer when x requires grad (the reference has no backward: its outputs carry no
     graph).  x gets dx = dy . W^T from ONE launch (`quant_cuda.lutgemm_t`: a transposed LUT-GEMM, on the tensor cores for fp16 /
     bf16 gradients of at least `BWD_TC_MIN_ROWS` rows, else on the CUDA cores; outliers and dense rows included); the buffers are constants and get no gradient.  The forward of such a call takes the same route
@@ -122,12 +123,16 @@ class QuantLinearLUT(nn.Module):
     # section 3.6: 32 rows 1.08 vs 0.78 ms, 64 rows 1.09 vs 1.48 ms).
     TC_MIN_ROWS = 64
     # bf16 inputs of at least this many rows run the same tensor-core LUT-GEMM with three bf16 weight parts; fewer rows run the
-    # batched symbols.  80: the smallest measured row count above TC_MIN_ROWS at which a whole 7B decoder layer is faster on an
+    # multi-row GEMV (BF16_ROWS_MAX).  80: the smallest measured row count above TC_MIN_ROWS at which a whole 7B decoder layer is faster on an
     # H100 (DESIGN.md section 3.6: 80 rows 1.48 vs 1.90 ms; the tensor cores already win at 64 rows, 1.46 vs 1.56 ms).
     BF16_TC_MIN_ROWS = 80
     # fp16 inputs of 2 to ROWS_MAX rows (below TC_MIN_ROWS) run the multi-row GEMV (quant_cuda.lutgemv_rows).  63: it is faster than
     # the batched symbols on a whole 7B decoder layer at every measured row count up to 63 on an H100 (DESIGN.md section 3.9).
     ROWS_MAX = 63
+    # bf16 inputs of 2 to BF16_ROWS_MAX rows (below BF16_TC_MIN_ROWS) run the same multi-row GEMV (quant_cuda.lutgemv_rows_bf16).
+    # 79: it is faster than the batched symbols on a whole 7B decoder layer at every measured row count up to 79 on an H100
+    # (DESIGN.md section 3.12).
+    BF16_ROWS_MAX = 79
     # fp16 / bf16 gradients of at least this many rows run the input gradient on the tensor cores (quant_cuda.lutgemm_t path
     # "tc"); fewer rows and fp32 gradients on the CUDA cores.  96: where the two cross on a whole 7B decoder layer on an H100
     # (DESIGN.md section 3.10: 64 rows 5.96 vs 5.12 ms, 512 rows 8.05 vs 40.8 ms; the CUDA-core time grows 80 us per row).
@@ -288,7 +293,7 @@ class QuantLinearLUT(nn.Module):
             outshape = list(x.shape)
             outshape[-1] = self.outfeatures
             rows, cols, vals, fr, fri = self._sparse_args()
-            if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32) and self._fused_fits(fr):
+            if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32, torch.bfloat16) and self._fused_fits(fr):
                 y = quant_cuda.lutgemv_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                              self.bias, rows, cols, vals, fr, fri)
                 return y.reshape(outshape)
@@ -306,11 +311,11 @@ class QuantLinearLUT(nn.Module):
             out = quant_cuda.lutgemm_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
                                            None, rows, cols, vals, fr, fri).reshape(out_shape)
             return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
-        if (QuantLinearLUT.use_fused and x.dtype == torch.float16 and 2 <= x.shape[0] <= QuantLinearLUT.ROWS_MAX
-                and self._rows_fits()):
+        rows_max = {torch.float16: QuantLinearLUT.ROWS_MAX, torch.bfloat16: QuantLinearLUT.BF16_ROWS_MAX}.get(x.dtype)
+        if QuantLinearLUT.use_fused and rows_max is not None and 2 <= x.shape[0] <= rows_max and self._rows_fits():
             rows, cols, vals, fr, fri = self._sparse_args()
-            out = quant_cuda.lutgemv_rows(_aligned(x), self.qweight, self.lookup_table, self.bits,
-                                          None, rows, cols, vals, fr, fri).reshape(out_shape)
+            rows_fn = quant_cuda.lutgemv_rows if x.dtype == torch.float16 else quant_cuda.lutgemv_rows_bf16
+            out = rows_fn(_aligned(x), self.qweight, self.lookup_table, self.bits, None, rows, cols, vals, fr, fri).reshape(out_shape)
             return out + self.bias if self.bias is not None else out
         out = torch.zeros((x.shape[0], self.outfeatures), device=dev, dtype=torch.float32)
         dtype = x.dtype
