@@ -396,6 +396,28 @@ void sqllm_sequence_destroy(sqllm_sequence *s);
 int sqllm_unpack_indices(int bits, const int32_t *qweight, int in_features, int out_features,
                          uint8_t *idx, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Quantizer: exact weighted 1-D k-means per row (the codebook fit of reference quantization/nuq.py:50-58,
+ * solved exactly by dynamic programming instead of sklearn's seeded Lloyd; DESIGN.md section 3.13).
+ *   w, s        fp32 [rows, n]   values and sample weights (s >= 0 and finite, w finite: not checked on the device);
+ *                                a row whose weights are all zero is weighted uniformly (nuq.py:174-175)
+ *   centroids   fp32 [rows, k]   the optimal centroids, non-decreasing; a cluster with no weight repeats its neighbour's
+ *   labels      uint8 [rows, n]  nearest centroid of every element, ties to the lower index:
+ *                                label(w) = #{j in 1..k-1 : w > fl32(0.5f * (c[j-1] + c[j]))}
+ *   requirements (SQLLM_EINVAL otherwise, checked before any device access): rows >= 1, 2 <= k <= 16, k <= n <= 65535,
+ *   non-null 4-byte aligned w / s / centroids, non-null labels, a 256-byte aligned workspace.
+ * The workspace (no initialisation needed) holds one chunk of rows; sqllm_kmeans1d_workspace_bytes gives its size for
+ * (rows, n, k) (it queries the sort's temporary storage, so it needs a current device).  Results are bit-reproducible and a
+ * row's result depends on that row alone; no atomics; capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------- */
+int sqllm_kmeans1d_workspace_bytes(int rows, int n, int k, size_t *bytes);
+int sqllm_kmeans1d(const float *w, const float *s, int rows, int n, int k, float *centroids, uint8_t *labels,
+                   void *workspace, size_t workspace_bytes, void *stream);
+
+/* labels uint8 [out, in] (one row per output channel, as sqllm_kmeans1d gives them) -> qweight int32 [in/32*bits, out],
+ * bit-identical to the reference's pack2 (quant.py:171-208).  in % 32 == 0; each label is taken modulo 2^bits. */
+int sqllm_pack_indices(int bits, const uint8_t *labels, int in_features, int out_features, int32_t *qweight, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

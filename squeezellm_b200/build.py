@@ -47,7 +47,7 @@ def build_lib(verbose=False):
                     os.path.join(CSRC, "lutgemm_batched.cuh"), os.path.join(CSRC, "lutgemv_rows.cuh"),
                     os.path.join(CSRC, "lutgemm_tc.cuh"), os.path.join(CSRC, "lutgemm_t.cuh"),
                     os.path.join(CSRC, "lutgemm_tc_t.cuh"), os.path.join(CSRC, "lut_grad.cuh"),
-                    os.path.join(CSRC, "lut_grad_tc.cuh")]):
+                    os.path.join(CSRC, "lut_grad_tc.cuh"), os.path.join(CSRC, "kmeans1d.cuh")]):
         nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
         cmd = [nvcc] + NVCC_FLAGS + ["-ccbin", _cxx(), "-I", INCLUDE, "-shared", "-o", out, src]
         if verbose:

@@ -35,6 +35,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <cub/device/device_segmented_radix_sort.cuh>
 #include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -951,6 +952,7 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemm_tc_t.cuh"
 #include "lut_grad.cuh"
 #include "lut_grad_tc.cuh"
+#include "kmeans1d.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
 // tables to their own size - up to 64 KB - so the host needs the real address, not a worst case; the kernel re-checks it)
@@ -2146,6 +2148,111 @@ int sqllm_unpack_indices(int bits, const int32_t *qweight, int in_features, int 
                                                                        in_features, out_features, idx);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "unpack launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+// ---- weighted 1-D k-means and the GPU pack (kmeans1d.cuh) ----------------------------------------------------------------
+namespace {
+constexpr size_t KM_BUDGET = (size_t)512 << 20;  // workspace rows are chunked to about this many bytes
+
+size_t km_align(size_t b) { return (b + 255) & ~(size_t)255; }
+
+size_t km_row_bytes(int n, int k) {
+    const size_t n1 = (size_t)n + 1;
+    return 2 * sizeof(float) * n + (3 + 2) * sizeof(double) * n1 + (size_t)(k - 1) * sizeof(uint16_t) * n1;
+}
+
+int km_chunk(int rows, int n, int k) { return (int)std::max<size_t>(1, std::min<size_t>(rows, KM_BUDGET / km_row_bytes(n, k))); }
+
+struct KmLayout {
+    size_t offs, keys, vals, pref, d, opt, temp, temp_bytes, total;
+};
+
+int km_check(int rows, int n, int k) {
+    if (rows < 1) return fail(SQLLM_EINVAL, "kmeans1d: rows=%d must be >= 1", rows);
+    if (k < 2 || k > km::MAX_K) return fail(SQLLM_EINVAL, "kmeans1d: k=%d must be in [2, %d]", k, km::MAX_K);
+    if (n < k || n > km::MAX_N) return fail(SQLLM_EINVAL, "kmeans1d: n=%d must be in [k=%d, %d]", n, k, km::MAX_N);
+    return SQLLM_OK;
+}
+
+int km_layout(int rows, int n, int k, KmLayout &L) {
+    const int C = km_chunk(rows, n, k);
+    const size_t n1 = (size_t)n + 1, items = (size_t)C * n;
+    size_t temp = 0;
+    const cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairs(nullptr, temp, (const float *)nullptr, (float *)nullptr,
+                                                                   (const float *)nullptr, (float *)nullptr, (int)items, C,
+                                                                   (const int *)nullptr, (const int *)nullptr);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kmeans1d: sort workspace query failed: %s", cudaGetErrorString(e));
+    size_t o = 0;
+    L.offs = o; o += km_align(sizeof(int) * (C + 1));
+    L.keys = o; o += km_align(sizeof(float) * items);
+    L.vals = o; o += km_align(sizeof(float) * items);
+    L.pref = o; o += km_align(3 * sizeof(double) * n1 * C);
+    L.d = o; o += km_align(2 * sizeof(double) * n1 * C);
+    L.opt = o; o += km_align((size_t)(k - 1) * sizeof(uint16_t) * n1 * C);
+    L.temp = o; L.temp_bytes = temp; o += km_align(temp);
+    L.total = o;
+    return SQLLM_OK;
+}
+}  // namespace
+
+int sqllm_kmeans1d_workspace_bytes(int rows, int n, int k, size_t *bytes) {
+    if (!bytes) return fail(SQLLM_EINVAL, "kmeans1d_workspace_bytes: bytes must not be null");
+    int rc = km_check(rows, n, k);
+    if (rc) return rc;
+    KmLayout L;
+    if ((rc = km_layout(rows, n, k, L))) return rc;
+    *bytes = L.total;
+    return SQLLM_OK;
+}
+
+int sqllm_kmeans1d(const float *w, const float *s, int rows, int n, int k, float *centroids, uint8_t *labels, void *workspace,
+                   size_t workspace_bytes, void *stream) {
+    int rc = km_check(rows, n, k);
+    if (rc) return rc;
+    if (!w || !s || !centroids || !labels) return fail(SQLLM_EINVAL, "kmeans1d: w / s / centroids / labels must not be null");
+    if (((uintptr_t)w | (uintptr_t)s | (uintptr_t)centroids) & 3) return fail(SQLLM_EINVAL, "kmeans1d: w / s / centroids must be 4-byte aligned");
+    if (!workspace) return fail(SQLLM_EWORKSPACE, "kmeans1d: workspace must not be null");
+    if ((uintptr_t)workspace & 255) return fail(SQLLM_EINVAL, "kmeans1d: workspace must be 256-byte aligned");
+    KmLayout L;
+    if ((rc = km_layout(rows, n, k, L))) return rc;
+    if (workspace_bytes < L.total)
+        return fail(SQLLM_EWORKSPACE, "kmeans1d: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char *ws = static_cast<char *>(workspace);
+    int *offs = reinterpret_cast<int *>(ws + L.offs);
+    float *keys = reinterpret_cast<float *>(ws + L.keys), *vals = reinterpret_cast<float *>(ws + L.vals);
+    const int C = km_chunk(rows, n, k);
+    km::segment_offsets_kernel<<<(C + 256) / 256, 256, 0, st>>>(offs, C, n);
+    for (int r0 = 0; r0 < rows; r0 += C) {
+        const int c = std::min(C, rows - r0);
+        const size_t at = (size_t)r0 * n;
+        size_t temp = L.temp_bytes;
+        cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairs(ws + L.temp, temp, w + at, keys, s + at, vals, c * n, c, offs,
+                                                                 offs + 1, 0, 32, st);
+        if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kmeans1d: segmented sort failed: %s", cudaGetErrorString(e));
+        km::kmeans1d_kernel<<<c, km::THREADS, 0, st>>>(keys, vals, w + at, n, k, reinterpret_cast<double *>(ws + L.pref),
+                                                       reinterpret_cast<double *>(ws + L.d), reinterpret_cast<uint16_t *>(ws + L.opt),
+                                                       centroids + (size_t)r0 * k, labels + at);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kmeans1d launch failed: %s", cudaGetErrorString(e));
+    }
+    return SQLLM_OK;
+}
+
+int sqllm_pack_indices(int bits, const uint8_t *labels, int in_features, int out_features, int32_t *qweight, void *stream) {
+    if (bits != 3 && bits != 4) return fail(SQLLM_EINVAL, "pack_indices: bits=%d must be 3 or 4", bits);
+    if (in_features <= 0 || in_features % 32)
+        return fail(SQLLM_EINVAL, "pack_indices: in_features=%d must be a positive multiple of 32", in_features);
+    if (out_features <= 0) return fail(SQLLM_EINVAL, "pack_indices: out_features=%d must be >= 1", out_features);
+    if (!labels || !qweight) return fail(SQLLM_EINVAL, "pack_indices: labels / qweight must not be null");
+    if ((uintptr_t)qweight & 3) return fail(SQLLM_EINVAL, "pack_indices: qweight must be 4-byte aligned");
+    const size_t work = (size_t)in_features / 32 * out_features;
+    const int grid = (int)std::min<size_t>(4096, (work + 255) / 256);
+    km::pack_indices_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(bits, labels, in_features, out_features,
+                                                                                 reinterpret_cast<uint32_t *>(qweight));
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "pack_indices launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

@@ -483,6 +483,35 @@ torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     return idx;
 }
 
+std::tuple<torch::Tensor, torch::Tensor> kmeans1d(torch::Tensor w, torch::Tensor s, int k) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(w));
+    need(w, "w", torch::kFloat32, w);
+    need(s, "sample_weight", torch::kFloat32, w);
+    TORCH_CHECK(w.dim() == 2 && s.sizes() == w.sizes(), "w and sample_weight must both be [rows, n]");
+    const int R = (int)w.size(0), n = (int)w.size(1);
+    size_t bytes = 0;
+    check_status(sqllm_kmeans1d_workspace_bytes(R, n, k, &bytes), "quant_cuda.kmeans1d");
+    auto opt = torch::TensorOptions().device(w.device());
+    torch::Tensor ws = torch::empty({(int64_t)bytes}, opt.dtype(torch::kUInt8));
+    torch::Tensor cent = torch::empty({R, k}, opt.dtype(torch::kFloat32));
+    torch::Tensor labels = torch::empty({R, n}, opt.dtype(torch::kUInt8));
+    check_status(sqllm_kmeans1d(w.data_ptr<float>(), s.data_ptr<float>(), R, n, k, cent.data_ptr<float>(), labels.data_ptr<uint8_t>(),
+                                ws.data_ptr(), bytes, cur_stream()),
+                 "quant_cuda.kmeans1d");
+    return {cent, labels};
+}
+
+torch::Tensor pack_indices(torch::Tensor labels, int bits) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(labels));
+    need(labels, "labels", torch::kUInt8, labels);
+    TORCH_CHECK(bits == 3 || bits == 4, "bits must be 3 or 4");
+    TORCH_CHECK(labels.dim() == 2 && labels.size(1) % 32 == 0, "labels must be [out, in] with in a multiple of 32");
+    const int N = (int)labels.size(0), K = (int)labels.size(1);
+    torch::Tensor q = torch::empty({K / 32 * bits, N}, torch::TensorOptions().dtype(torch::kInt32).device(labels.device()));
+    check_status(sqllm_pack_indices(bits, labels.data_ptr<uint8_t>(), K, N, q.data_ptr<int32_t>(), cur_stream()), "quant_cuda.pack_indices");
+    return q;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -551,6 +580,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("sequence_reset_error", [](int64_t h) { check_status(sqllm_sequence_reset_error(reinterpret_cast<sqllm_sequence *>(h), cur_stream()), "quant_cuda.sequence_reset_error"); },
           "clear the sequence's error word on the current stream");
     m.def("sequence_destroy", [](int64_t h) { sqllm_sequence_destroy(reinterpret_cast<sqllm_sequence *>(h)); });
+    m.def("kmeans1d", &kmeans1d, "exact weighted 1-D k-means per row: w, sample_weight fp32 [rows, n], k -> (centroids fp32 [rows, k], "
+          "labels uint8 [rows, n]); deterministic", py::arg("w"), py::arg("sample_weight"), py::arg("k"));
+    m.def("pack_indices", &pack_indices, "labels uint8 [out, in] -> qweight int32 [in/32*bits, out] in the reference's packed layout",
+          py::arg("labels"), py::arg("bits"));
     m.def("unpack_indices", &unpack_indices, "GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },

@@ -1,0 +1,156 @@
+"""Quantize a model on the GPU into QuantLinearLUT layers: the reference's offline pipeline (quantization/nuq.py,
+squeezellm/outliers.py, quantization/generate_outlier_config.py, squeezellm/quant.py pack2) restated on top of the
+`quant_cuda` extension.
+
+  * `kmeans_codebook`: the per-output-channel weighted k-means of nuq.py:50-58,164-176, solved EXACTLY by a dynamic program
+    on the sorted row (quant_cuda.kmeans1d; DESIGN.md section 3.13) instead of one seeded sklearn KMeans per row on the CPU.
+    Its objective is never above sklearn's, and the result is deterministic.
+  * `outlier_threshold`: the IQR rule of generate_outlier_config.py:47-53.
+  * `split_outliers`: the sensitivity and threshold masks of outliers.py:14-23,52-60.
+  * `quantize_linear` / `quantize_model`: the codebook fit, then the pack of quant.py:97-208 on the device (quant_cuda.pack_indices
+    and a CSR of outlier minus zero centroid); buffers bit-identical to QuantLinearLUT.pack2 on the same inputs.
+    `checkpoint.save_checkpoint` writes the result in the reference's format.
+
+The Fisher information (the squared gradients) is the caller's: a state dict keyed like the model's (`<layer>.weight`).
+"""
+import torch
+
+from .checkpoint import find_linear_layers
+from .quant import QuantLinearLUT, quant_cuda
+
+__all__ = ["kmeans_codebook", "outlier_threshold", "split_outliers", "quantize_linear", "quantize_model"]
+
+
+def kmeans_codebook(weight, sample_weight, bits):
+    """Per-row exact weighted k-means with 2^bits clusters: weight, sample_weight [N, K] CUDA tensors ->
+    (lookup_table fp32 [N, 2^bits] non-decreasing, labels uint8 [N, K] = nearest centroid, ties to the lower index).
+    A row whose sample weights are all zero is weighted uniformly (nuq.py:174-175)."""
+    if bits not in (3, 4):
+        raise ValueError(f"kmeans_codebook: bits={bits} must be 3 or 4")
+    if not (torch.is_tensor(weight) and torch.is_tensor(sample_weight)):
+        raise ValueError("kmeans_codebook: weight and sample_weight must be tensors")
+    if weight.dim() != 2 or weight.shape != sample_weight.shape:
+        raise ValueError(f"kmeans_codebook: weight {tuple(weight.shape)} and sample_weight {tuple(sample_weight.shape)} "
+                         "must be the same [out, in] shape")
+    if not (weight.is_cuda and sample_weight.is_cuda) or weight.device != sample_weight.device:
+        raise ValueError("kmeans_codebook: weight and sample_weight must be CUDA tensors on one device")
+    if weight.shape[1] % 32:
+        raise ValueError(f"kmeans_codebook: in_features={weight.shape[1]} must be a multiple of 32")
+    w = weight.detach().float().contiguous()
+    s = sample_weight.detach().float().contiguous()
+    if not bool(torch.isfinite(w).all()):
+        raise ValueError("kmeans_codebook: weight has non-finite values")
+    if not bool((torch.isfinite(s) & (s >= 0)).all()):
+        raise ValueError("kmeans_codebook: sample weights must be finite and >= 0")
+    return quant_cuda.kmeans1d(w, s, 2 ** bits)
+
+
+def _numpy_linear_quantile(sorted_flat, q):
+    """numpy.quantile(..., method="linear") of a sorted 1-D fp32 tensor, as numpy evaluates it: the fraction and numpy's lerp
+    (exact at both ends) in fp32.  -> 0-d fp32 tensor on the CPU."""
+    n = sorted_flat.numel()
+    h = (n - 1) * q
+    lo = int(h // 1)
+    t = torch.tensor(h - lo, dtype=torch.float32)
+    a, b = sorted_flat[lo].cpu(), sorted_flat[min(lo + 1, n - 1)].cpu()
+    diff = b - a
+    return b - diff * (1 - t) if t >= 0.5 else a + diff * t
+
+
+def outlier_threshold(weight, range):
+    """The outlier threshold of generate_outlier_config.py:47-53: max(|q1 - r IQR|, |q3 + r IQR|) with numpy's
+    linear-interpolation quartiles of all the layer's weights, r = `range`, evaluated in fp32 as numpy does for an fp32 array.
+    Sorted on the tensor's device (torch.quantile rejects inputs of more than 2^24 elements)."""
+    flat = torch.sort(weight.detach().float().reshape(-1)).values
+    q1, q3 = _numpy_linear_quantile(flat, 0.25), _numpy_linear_quantile(flat, 0.75)
+    lo, hi = q1 - range * (q3 - q1), q3 + range * (q3 - q1)
+    return float(torch.maximum(lo.abs(), hi.abs()))
+
+
+def split_outliers(weight, fisher, threshold=None, sensitivity=0.0):
+    """-> (dense, outliers), both fp32 [out, in]: the masks of outliers.py.  Sensitivity first (outliers.py:14-23): the
+    numel * sensitivity / 100 largest Fisher values by topk, then every weight whose Fisher value is STRICTLY above the last of
+    them (ties with it stay dense; a count of 0 takes none).  Then the threshold on what remains (outliers.py:52-60):
+    w >= threshold or w <= -threshold, in fp32."""
+    w = weight.detach().float()
+    mask = torch.zeros_like(w, dtype=torch.bool)
+    if sensitivity:
+        g = fisher.detach().to(w.device).float()
+        if g.shape != w.shape:
+            raise ValueError(f"split_outliers: fisher {tuple(g.shape)} must have the weight's shape {tuple(w.shape)}")
+        num = int(g.numel() * sensitivity / 100)
+        if num > 0:
+            mask = g > g.reshape(-1).topk(k=num).values[-1]
+    outliers = w * mask
+    dense = w * ~mask
+    if threshold is not None:
+        t = torch.logical_or(dense >= threshold, dense <= -threshold)
+        outliers = outliers + dense * t
+        dense = dense * ~t
+    return dense, outliers
+
+
+def quantize_linear(linear, fisher, bits, threshold=None, sensitivity=0.0):
+    """nn.Linear -> QuantLinearLUT on the linear's (CUDA) device, dense-and-sparse when a threshold or a sensitivity is given.
+
+    Sample weight of each weight = fisher * (dense weight != 0); a row whose sum is 0 gets all ones (nuq.py:172-175).  The
+    buffers are those QuantLinearLUT.pack2 makes from the same centroids, labels and outlier matrix: qweight packed on the device,
+    the bias copied, CSR of (outlier - the row's centroid nearest to zero) (quant.py:117-123), topX = 0."""
+    if bits not in (3, 4):
+        raise ValueError(f"quantize_linear: bits={bits} must be 3 or 4")
+    weight = linear.weight
+    if not weight.is_cuda:
+        raise ValueError("quantize_linear: the linear's weight must be on a CUDA device")
+    out_f, in_f = weight.shape
+    fisher = fisher.detach().to(weight.device).float()
+    if fisher.shape != weight.shape:
+        raise ValueError(f"quantize_linear: fisher {tuple(fisher.shape)} must have the weight's shape {tuple(weight.shape)}")
+    sparse = threshold is not None or bool(sensitivity)
+    if sparse:
+        dense, outliers = split_outliers(weight, fisher, threshold, sensitivity)
+    else:
+        dense, outliers = weight.detach().float(), None
+    lut, labels = kmeans_codebook(dense, fisher * (dense != 0), bits)
+
+    q = QuantLinearLUT(bits, in_f, out_f, linear.bias is not None, include_sparse=sparse, topX=0).to(weight.device)
+    q.lookup_table = lut
+    q.qweight = quant_cuda.pack_indices(labels, bits)
+    if linear.bias is not None:
+        q.bias = linear.bias.detach().clone()
+    if sparse:
+        zero = lut.gather(1, lut.abs().argmin(dim=1, keepdim=True))
+        outliers = torch.where(outliers != 0, outliers - zero, outliers)
+        csr = outliers.to_sparse(layout=torch.sparse_csr)
+        q.register_buffer("rows", csr.crow_indices().to(torch.int32))
+        q.register_buffer("cols", csr.col_indices().to(torch.int32))
+        q.register_buffer("vals", csr.values().to(torch.float32))
+        q.numvals = int(q.vals.shape[0])
+    return q
+
+
+def _set_module(model, name, module):
+    parent, _, attr = name.rpartition(".")
+    setattr(model.get_submodule(parent) if parent else model, attr, module)
+
+
+def quantize_model(model, fisher_state, bits, outlier_range=None, sensitivity=0.0, skip=("lm_head",)):
+    """Replace every nn.Linear of `model` (checkpoint.find_linear_layers, except `skip`) by its quantize_linear result, in
+    place and one layer at a time.  fisher_state[f"{name}.weight"] holds the layer's squared gradients (the reference's
+    gradient checkpoints).  outlier_range: the IQR range of generate_outlier_config.py, giving each layer's threshold
+    (outlier_threshold); sensitivity: the percentage of outliers.py.  Returns {layer name: CSR nnz} of the sparse layers;
+    checkpoint.save_checkpoint(model, path, bits) then writes the reference's packed format."""
+    layers = find_linear_layers(model)
+    for name in skip:
+        layers.pop(name, None)
+    missing = [n for n in layers if f"{n}.weight" not in fisher_state]
+    if missing:
+        raise KeyError(f"quantize_model: fisher_state has no entry for {missing[:4]}{' ...' if len(missing) > 4 else ''}")
+    numvals = {}
+    for name, linear in layers.items():
+        thr = outlier_threshold(linear.weight, outlier_range) if outlier_range is not None else None
+        q = quantize_linear(linear, fisher_state[f"{name}.weight"], bits, threshold=thr, sensitivity=sensitivity)
+        _set_module(model, name, q)
+        if q.include_sparse:
+            numvals[name] = q.numvals
+        del linear
+    return numvals
