@@ -5,6 +5,7 @@
 
 `python -m squeezellm_b200.build` or `__graft_entry__.build()`.
 """
+import glob
 import os
 import shutil
 import subprocess
@@ -43,11 +44,7 @@ def build_lib(verbose=False):
     src = os.path.join(CSRC, "lutgemv_kernels.cu")
     hdr = os.path.join(INCLUDE, "sqllm_b200.h")
     out = lib_path()
-    if _newer(out, [src, hdr, os.path.join(CSRC, "lutgemv_v2.cuh"), os.path.join(CSRC, "lutgemv_seq.cuh"),
-                    os.path.join(CSRC, "lutgemm_batched.cuh"), os.path.join(CSRC, "lutgemv_rows.cuh"),
-                    os.path.join(CSRC, "lutgemm_tc.cuh"), os.path.join(CSRC, "lutgemm_t.cuh"),
-                    os.path.join(CSRC, "lutgemm_tc_t.cuh"), os.path.join(CSRC, "lut_grad.cuh"),
-                    os.path.join(CSRC, "lut_grad_tc.cuh"), os.path.join(CSRC, "kmeans1d.cuh")]):
+    if _newer(out, [src, hdr] + glob.glob(os.path.join(CSRC, "*.cuh"))):
         nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
         cmd = [nvcc] + NVCC_FLAGS + ["-ccbin", _cxx(), "-I", INCLUDE, "-shared", "-o", out, src]
         if verbose:

@@ -43,6 +43,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <initializer_list>
 #include <mutex>
 #include <type_traits>
 #include <unordered_map>
@@ -983,32 +984,9 @@ std::recursive_mutex g_state_mu;
 struct DevInfo {
     int sm = 0;
     unsigned smem_raw = 0;               // shared-window address of dynamic shared memory; 0 until smem_window probes it
-    std::vector<const void *> smem_set;  // kernels whose dynamic shared-memory limit set_max_smem has raised
+    std::vector<const void *> smem_set;  // kernels whose dynamic shared-memory limit dev_setup has raised
 };
 DevInfo g_dev[64];
-
-// The current device and its SM count, read once.  Caller holds g_state_mu.
-int cur_dev(int &dev) {
-    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
-    if (dev < 0 || dev >= 64) return fail(SQLLM_EINVAL, "device ordinal %d out of range", dev);
-    DevInfo &d = g_dev[dev];
-    if (d.sm == 0 && (cudaDeviceGetAttribute(&d.sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm <= 0)) {
-        d.sm = 0;
-        return fail(SQLLM_ECUDA, "cannot query SM count");
-    }
-    return SQLLM_OK;
-}
-
-// Raises the dynamic shared-memory limit of kernel `fn` to `bytes`, once per device.  Caller holds g_state_mu.
-template <typename F>
-int set_max_smem(DevInfo &d, F *fn, int bytes) {
-    const void *f = (const void *)fn;
-    if (std::find(d.smem_set.begin(), d.smem_set.end(), f) != d.smem_set.end()) return SQLLM_OK;
-    if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
-        return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
-    d.smem_set.push_back(f);
-    return SQLLM_OK;
-}
 
 // d.smem_raw from smem_base_probe, once per device.  The probe is synchronous and refused during stream capture: only v2 and sequence
 // plans ask for it, and the first of them on a device must come before any capture - any warm-up does.  Caller holds g_state_mu.
@@ -1029,18 +1007,68 @@ int smem_window(DevInfo &d) {
     return SQLLM_OK;
 }
 
-// cudaLaunchKernelEx with one attribute: programmatic stream serialisation for the GEMV kernels (their prologue and weight stream
-// overlap the previous kernel), cooperative for the sequence kernel (every CTA waits on every other one: they must all be resident).
+// A kernel and the dynamic shared memory it is launched with.
+struct KernelSmem {
+    const void *fn = nullptr;
+    int bytes = 0;
+    KernelSmem() = default;
+    template <typename... P>
+    KernelSmem(void (*f)(P...), int b) : fn((const void *)f), bytes(b) {}
+};
+
+// The device set-up of every launch, under g_state_mu: resolves the current device (its SM count is read once), raises the dynamic
+// shared-memory limit of each kernel in `ks` (once per device), and returns the SM count in *sm and the shared-memory window in
+// *smem_raw where asked (the window is probed on the first request, see smem_window).  `ks` is a braced list of KernelSmem, or an array.
+template <typename List = std::initializer_list<KernelSmem>>
+int dev_setup(const List &ks, int *sm = nullptr, unsigned *smem_raw = nullptr) {
+    std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
+    if (dev < 0 || dev >= 64) return fail(SQLLM_EINVAL, "device ordinal %d out of range", dev);
+    DevInfo &d = g_dev[dev];
+    if (d.sm == 0 && (cudaDeviceGetAttribute(&d.sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm <= 0)) {
+        d.sm = 0;
+        return fail(SQLLM_ECUDA, "cannot query SM count");
+    }
+    for (const KernelSmem &k : ks) {
+        if (std::find(d.smem_set.begin(), d.smem_set.end(), k.fn) != d.smem_set.end()) continue;
+        if (cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.bytes) != cudaSuccess)
+            return fail(SQLLM_ECUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
+        d.smem_set.push_back(k.fn);
+    }
+    if (smem_raw) {
+        const int rc = smem_window(d);
+        if (rc) return rc;
+        *smem_raw = d.smem_raw;
+    }
+    if (sm) *sm = d.sm;
+    return SQLLM_OK;
+}
+
+// The one attribute of a cudaLaunchKernelEx launch: programmatic stream serialisation for the GEMV kernels that wait on the grid
+// dependency (their prologue and weight stream overlap the previous kernel), cooperative for the sequence kernel (every CTA waits on
+// every other one: they must all be resident), or a cluster of `cluster` CTAs along x for the kernels whose CTAs reduce through each
+// other's shared memory.
+struct LaunchAttr {
+    int cluster;
+    bool cooperative;
+};
+constexpr LaunchAttr PDL{0, false}, COOPERATIVE{0, true};
+constexpr LaunchAttr cluster_of(int n) { return {n, false}; }
+
 template <typename... P, typename... A>
-cudaError_t launch_ex(void (*fn)(P...), int grid, int block, int smem, cudaStream_t st, bool cooperative, const A &...args) {
+cudaError_t launch_ex(void (*fn)(P...), dim3 grid, int block, int smem, cudaStream_t st, LaunchAttr la, const A &...args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
+    cfg.gridDim = grid;
     cfg.blockDim = dim3(block);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr;
-    if (cooperative) {
+    if (la.cluster > 0) {
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = la.cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    } else if (la.cooperative) {
         attr.id = cudaLaunchAttributeCooperative;
         attr.val.cooperative = 1;
     } else {
@@ -1050,6 +1078,40 @@ cudaError_t launch_ex(void (*fn)(P...), int grid, int block, int smem, cudaStrea
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, fn, args...);
+}
+
+// The layer's buffers in a kernel's parameter struct (every one names them qw, lut, rows, cols, vals, full_rows, fri, topX): the
+// dense rows only when both full_rows and topX > 0 are given, so that p.topX > 0 means "the layer has dense rows".
+template <typename P>
+void set_layer(P &p, const sqllm_lutgemv_args &a) {
+    const bool hyb = a.full_rows && a.topX > 0;
+    p.qw = reinterpret_cast<const uint32_t *>(a.qweight);
+    p.lut = a.lookup_table;
+    p.rows = a.rows; p.cols = a.cols; p.vals = a.vals;
+    p.full_rows = hyb ? a.full_rows : nullptr;
+    p.fri = hyb ? a.full_row_indices : nullptr;
+    p.topX = hyb ? a.topX : 0;
+}
+
+// SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16
+bool dt_valid(int dt) { return dt == SQLLM_DT_F32 || dt == SQLLM_DT_F16 || dt == SQLLM_DT_BF16; }
+
+// The descriptor checks every GEMV / GEMM entry point shares, in this order: in_features a positive multiple of k_mult (64 or 32),
+// out_features a positive multiple of n_mult (4, or 1 for "positive"), the packed matrix and codebook given, and dense rows only with
+// their indices.  Each entry point makes its own checks after these.
+int check_layer(const sqllm_lutgemv_args *a, int k_mult, int n_mult) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
+    if (a->in_features <= 0 || a->in_features % k_mult)
+        return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of %d", a->in_features, k_mult);
+    if (a->out_features <= 0 || a->out_features % n_mult) {
+        if (n_mult == 1) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
+        return fail(SQLLM_EINVAL, "out_features=%d must be a positive multiple of %d", a->out_features, n_mult);
+    }
+    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
+    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
+    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
+    return SQLLM_OK;
 }
 
 int g_det = -1;
@@ -1119,12 +1181,9 @@ int make_plan(int bits, int K, int N, int topX, bool has_csr_in, int stage, Plan
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);  // lazily initialised statics below
     const bool has_csr = has_csr_in || topX > 0;  // from here on: "a staging buffer is needed"
     pl.has_stage = has_csr ? stage : 0;
-    int dev = 0;
-    int rc = cur_dev(dev);
+    int sm = 0;
+    const int rc = dev_setup({{lutgemv_kernel<4>, 227 * 1024}, {lutgemv_kernel<3>, 227 * 1024}}, &sm);
     if (rc) return rc;
-    DevInfo &d = g_dev[dev];
-    for (auto fn : {lutgemv_kernel<4>, lutgemv_kernel<3>})
-        if ((rc = set_max_smem(d, fn, 227 * 1024))) return rc;
     const int XU = bits == 4 ? 8 : 32;
     pl.R = bits == 4 ? K / 8 : K / 32;
     pl.strips = (N + STRIP - 1) / STRIP;
@@ -1137,7 +1196,7 @@ int make_plan(int bits, int K, int N, int topX, bool has_csr_in, int stage, Plan
     // CTAS_PER_SM, ask the occupancy calculator, and fall back to fewer CTAs per SM if it disagrees.
     int use_cps = CTAS_PER_SM;
 replan:
-    const int G0 = d.sm * use_cps;
+    const int G0 = sm * use_cps;
     int chunk = (int)(2 * ((T + 2LL * G0 - 1) / (2LL * G0)));  // an even number of units: a consumer warp's pair never straddles the end
     if (chunk > 3 * pl.R) chunk = 3 * pl.R;  // a CTA may touch at most MAXSEG strips
     if (chunk < 2) chunk = 2;
@@ -1149,19 +1208,14 @@ replan:
     const int smem = bits == 4 ? Cfg<4>::total(maxseg, xfl, pl.has_stage) : Cfg<3>::total(maxseg, xfl, pl.has_stage);
     if (smem > 227 * 1024) return fail(SQLLM_EINVAL, "in_features=%d needs %d B of shared memory (> 227 KB)", K, smem);
     {
-        static std::mutex occ_mu;
         static std::unordered_map<unsigned long long, int> occ_cache;
         const unsigned long long key = ((unsigned long long)smem << 8) | (unsigned long long)bits;
         int occ = -1;
-        {
-            std::lock_guard<std::mutex> lk(occ_mu);
-            auto it = occ_cache.find(key);
-            if (it != occ_cache.end()) occ = it->second;
-        }
+        auto it = occ_cache.find(key);
+        if (it != occ_cache.end()) occ = it->second;
         if (occ < 0) {
             const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, THREADS, smem);
             if (e != cudaSuccess) return fail(SQLLM_ECUDA, "occupancy query failed: %s", cudaGetErrorString(e));
-            std::lock_guard<std::mutex> lk(occ_mu);
             occ_cache[key] = occ;
         }
         if (occ < 1) return fail(SQLLM_EINVAL, "kernel does not fit an SM (shared memory %d B)", smem);
@@ -1201,39 +1255,30 @@ replan:
     return SQLLM_OK;
 }
 
+// the descriptor checks of sqllm_lutgemv, the fused one-GEMV entry points and the sequence: the shared ones with in_features a
+// multiple of 64 and out_features a multiple of 4, then a 16-byte aligned matrix and codebook
 int check_common(const sqllm_lutgemv_args *a) {
-    if (!a) return fail(SQLLM_EINVAL, "null args");
-    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
-    if (a->in_features <= 0 || a->in_features % 64) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 64", a->in_features);
-    if (a->out_features <= 0 || a->out_features % 4) return fail(SQLLM_EINVAL, "out_features=%d must be a positive multiple of 4", a->out_features);
-    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
+    const int rc = check_layer(a, 64, 4);
+    if (rc) return rc;
     if (reinterpret_cast<uintptr_t>(a->qweight) & 15) return fail(SQLLM_EINVAL, "qweight must be 16-byte aligned");
     if (reinterpret_cast<uintptr_t>(a->lookup_table) & 15) return fail(SQLLM_EINVAL, "lookup_table must be 16-byte aligned");
-    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
-    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
     return SQLLM_OK;
 }
 
 int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t st) {
     std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
-    p.qw = reinterpret_cast<const uint32_t *>(a->qweight);
-    p.lut = a->lookup_table;
-    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-    const bool hyb = a->full_rows && a->topX > 0;
-    p.full_rows = hyb ? a->full_rows : nullptr;
-    p.fri = hyb ? a->full_row_indices : nullptr;
-    p.topX = hyb ? a->topX : 0;
+    set_layer(p, *a);
     p.K = a->in_features; p.N = a->out_features;
     p.R = pl.R; p.strips = pl.strips; p.T = pl.T; p.chunk = pl.chunk;
     p.maxseg = pl.maxseg; p.x_direct = pl.x_direct; p.xfloats = pl.xfloats;
-    p.hc = hyb ? pl.hc : 0; p.hrows = pl.hrows; p.maxc = pl.maxc;
+    p.hc = p.topX > 0 ? pl.hc : 0; p.hrows = pl.hrows; p.maxc = pl.maxc;
     p.has_stage = pl.has_stage;
     p.csr_rpc = pl.csr_rpc;
     p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
     p.trace = g_trace;
     if (g_trace) g_trace += g_trace_stride;
     g_last_grid = pl.G;
-    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, pl.G, THREADS, pl.smem, st, false, p);
+    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, pl.G, THREADS, pl.smem, st, PDL, p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1278,14 +1323,8 @@ K2Info k2_lookup(int bits, int variant, bool fused) {
 // Stream-K plan of one layer for the v2 and sequence kernels, on a grid of at most `sm` CTAs, and the layer's buffers: fills the
 // shape and buffer fields of p and returns the grid in G.
 int plan_layer(const sqllm_lutgemv_args &a, int sm, v2::P2 &p, int &G) {
-    const bool hyb = a.full_rows && a.topX > 0;
     const int K = a.in_features, N = a.out_features;
-    p.qw = reinterpret_cast<const uint32_t *>(a.qweight);
-    p.lut = a.lookup_table;
-    p.rows = a.rows; p.cols = a.cols; p.vals = a.vals;
-    p.full_rows = hyb ? a.full_rows : nullptr;
-    p.fri = hyb ? a.full_row_indices : nullptr;
-    p.topX = hyb ? a.topX : 0;
+    set_layer(p, a);
     p.K = K; p.N = N;
     p.R = a.bits == 4 ? K / 8 : K / 32;
     p.strips = (N + STRIP - 1) / STRIP;
@@ -1296,7 +1335,7 @@ int plan_layer(const sqllm_lutgemv_args &a, int sm, v2::P2 &p, int &G) {
     G = (int)((T + p.chunk - 1) / p.chunk);
     p.csr_rpc = (N + G - 1) / G;
     p.hc = p.hrows = 0;
-    if (hyb) {
+    if (p.topX > 0) {
         p.hrows = (K + G - 1) / G;
         p.hc = (K + p.hrows - 1) / p.hrows;
     }
@@ -1313,25 +1352,18 @@ int tensor_maps(const sqllm_lutgemv_args &a, CUtensorMap &big, CUtensorMap &smal
 
 int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cudaStream_t st) {
     const K2Info ki = k2_lookup(a->bits, variant, fused);
-    int dev = 0, sm = 0;
-    unsigned raw = 0;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int rc = cur_dev(dev);
-        if (rc) return rc;
-        DevInfo &d = g_dev[dev];
-        for (int b = 3; b <= 4; ++b) {
-            if ((rc = set_max_smem(d, k2_lookup(b, 0, false).fn, 227 * 1024))) return rc;
-            for (int v = 0; v < K2_VARIANTS; ++v)
-                if ((rc = set_max_smem(d, k2_lookup(b, v, true).fn, 227 * 1024))) return rc;
-        }
-        if ((rc = smem_window(d))) return rc;
-        sm = d.sm;
-        raw = d.smem_raw;
+    KernelSmem all[2 * (1 + K2_VARIANTS)];  // every v2 kernel: accumulate mode and each fused variant, both widths
+    int nk = 0;
+    for (int b = 3; b <= 4; ++b) {
+        all[nk++] = {k2_lookup(b, 0, false).fn, 227 * 1024};
+        for (int v = 0; v < K2_VARIANTS; ++v) all[nk++] = {k2_lookup(b, v, true).fn, 227 * 1024};
     }
-    int G = 0;
-    int rc = plan_layer(*a, sm, p, G);
+    int sm = 0;
+    unsigned raw = 0;
+    int rc = dev_setup(all, &sm, &raw);
     if (rc) return rc;
+    int G = 0;
+    if ((rc = plan_layer(*a, sm, p, G))) return rc;
     if (fused && p.N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the fused accumulator (max %d)", p.N, MAX_N_FUSED);
     if (fused && G > MAX_GRID_V2) return fail(SQLLM_EINVAL, "grid of %d CTAs exceeds the mailbox area (%d)", G, MAX_GRID_V2);
     const unsigned base = (raw + 127u) & ~127u;
@@ -1357,7 +1389,7 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
     }
     CUtensorMap tm_big, tm_small;
     if ((rc = tensor_maps(*a, tm_big, tm_small))) return rc;
-    const cudaError_t e = launch_ex(ki.fn, G, v2::THREADS2, smem, st, false, p, tm_big, tm_small);
+    const cudaError_t e = launch_ex(ki.fn, G, v2::THREADS2, smem, st, PDL, p, tm_big, tm_small);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1386,7 +1418,7 @@ size_t seq_item_len(const sqllm_seq_item &it) {  // elements of the item's full-
 }  // namespace
 
 struct sqllm_sequence {
-    int dev = 0, n = 0, bits = 0, mode = 0, world = 1, rank = 0, grid = 0, smem = 0;
+    int n = 0, bits = 0, mode = 0, world = 1, rank = 0, grid = 0, smem = 0;
     seq::SeqCfg cfg;
     KSeq fn = nullptr;
     void *d_descs = nullptr, *d_exports = nullptr, *d_ws = nullptr, *d_arena = nullptr;
@@ -1417,10 +1449,7 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
     int kmax = 0;
     for (int i = 0; i < n_items; ++i) {
         const sqllm_seq_item &it = items[i];
-        sqllm_lutgemv_args a = it.a;
-        a.batch = 1;
-        a.vec = reinterpret_cast<const float *>(16);  // (vec / mul are not used by a sequence; check_common wants them non-null)
-        a.mul = reinterpret_cast<float *>(16);
+        const sqllm_lutgemv_args &a = it.a;
         const int rc = check_common(&a);
         if (rc) return rc;
         if (a.bits != bits) return fail(SQLLM_EINVAL, "sequence: item %d has bits=%d, item 0 has %d (one sequence, one width)", i, a.bits, bits);
@@ -1450,17 +1479,10 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
             return fail(SQLLM_EINVAL, "sequence: export %d: bad item %d or destination (8-byte aligned fp16 vector)", e, it);
     }
     const KSeqInfo ki = kseq_lookup(bits, mode, world > 1);
-    int dev = 0, sm = 0;
+    int sm = 0;
     unsigned raw = 0;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int rc = cur_dev(dev);
-        if (!rc) rc = set_max_smem(g_dev[dev], ki.fn, 227 * 1024);
-        if (!rc) rc = smem_window(g_dev[dev]);
-        if (rc) return rc;
-        sm = g_dev[dev].sm;
-        raw = g_dev[dev].smem_raw;
-    }
+    const int rc = dev_setup({{ki.fn, 227 * 1024}}, &sm, &raw);
+    if (rc) return rc;
     const unsigned base = (raw + 127u) & ~127u;
     const int xbytes = (kmax * 2 + 127) & ~127;  // every item's x is staged as fp16 in one buffer, and ntb strip-sum rows follow it
     // no cap from the chunk: the weight stream runs on across items
@@ -1470,7 +1492,7 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
     const int smem = (int)(v2::Carve(base, xbytes, ki.ntb * STRIP * 4, ki.tab, ki.ntb, ki.stage, nst).end - raw);
 
     sqllm_sequence *s = new sqllm_sequence();
-    s->dev = dev; s->n = n_items; s->bits = bits; s->mode = mode; s->world = world; s->rank = rank; s->grid = sm; s->smem = smem; s->fn = ki.fn;
+    s->n = n_items; s->bits = bits; s->mode = mode; s->world = world; s->rank = rank; s->grid = sm; s->smem = smem; s->fn = ki.fn;
     // workspace: [0,4) token counter, [64,68) error word, per parity {flags [64 + MAX_STRIPS] ints, accumulator [MAX_N_FUSED] floats} (only
     // used by CTAs that own more than 8 strips), then EVERY item's own mailboxes: outlier row sums [N], partial strip sums [grid][64],
     // dense-row parts [topX][MAX_GRID_V2].  Mailboxes are not shared between items: an item may read only a slice of its predecessor's
@@ -1566,7 +1588,7 @@ extern "C" int sqllm_sequence_run(sqllm_sequence *s, void *stream) {
     if (!s) return fail(SQLLM_EINVAL, "sequence: null handle");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     seq::seq_bump_epoch<<<1, 1, 0, st>>>(reinterpret_cast<unsigned *>(s->d_ws));
-    const cudaError_t e = launch_ex(s->fn, s->grid, v2::THREADS2, s->smem, st, true, s->cfg);
+    const cudaError_t e = launch_ex(s->fn, s->grid, v2::THREADS2, s->smem, st, COOPERATIVE, s->cfg);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "sequence launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -1601,14 +1623,9 @@ namespace {
 // ---- batched symbols: tile kernel + outlier kernels (lutgemm_batched.cuh) ----------------------------------------------
 int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     using namespace batched;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int dev = 0;
-        int rc = cur_dev(dev);
-        if (!rc) rc = set_max_smem(g_dev[dev], lutgemm_batched_kernel<4>, 227 * 1024);
-        if (!rc) rc = set_max_smem(g_dev[dev], lutgemm_batched_kernel<3>, 227 * 1024);
-        if (rc) return rc;
-    }
+    const auto kern = a->bits == 4 ? lutgemm_batched_kernel<4> : lutgemm_batched_kernel<3>;
+    const int rc = dev_setup({{kern, 227 * 1024}});
+    if (rc) return rc;
     const int K = a->in_features, N = a->out_features, B = a->batch;
     const int XU = a->bits == 4 ? 8 : 32, tab = a->bits == 4 ? CB<4>::TAB : CB<3>::TAB;
     PB p;
@@ -1625,8 +1642,7 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
     const int strips = (N + STRIP - 1) / STRIP, btiles = (B + BT - 1) / BT;
     if (btiles > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", B, 65535 * BT);
     const dim3 grid(strips, slabs, btiles);
-    if (a->bits == 4) lutgemm_batched_kernel<4><<<grid, BTHREADS, smem, st>>>(p);
-    else lutgemm_batched_kernel<3><<<grid, BTHREADS, smem, st>>>(p);
+    kern<<<grid, BTHREADS, smem, st>>>(p);
     if (a->rows) {
         const dim3 blk(32, 8), g((N + 7) / 8, std::min((B + 31) / 32, 64));
         csr_batched_kernel<<<g, blk, 0, st>>>(a->rows, a->cols, a->vals, a->vec, a->mul, K, N, B);
@@ -1798,9 +1814,8 @@ int sqllm_debug_last_grid(void) { return g_last_grid; }
 const char *sqllm_last_error(void) { return g_err; }
 
 int sqllm_device_sm_count(void) {
-    std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-    int dev = 0;
-    return cur_dev(dev) ? 0 : g_dev[dev].sm;
+    int sm = 0;
+    return dev_setup({}, &sm) ? 0 : sm;
 }
 
 size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int topX) {
@@ -1840,7 +1855,7 @@ int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_hal
 int sqllm_lutgemv_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
                            void *workspace, size_t workspace_bytes, void *stream) {
     const int y16 = x_dtype == SQLLM_DT_BF16 ? SQLLM_DT_BF16 : SQLLM_DT_F16;  // the 16-bit y of this x: fp16 for fp32 x
-    if ((x_dtype != SQLLM_DT_F32 && x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) || (y_dtype != SQLLM_DT_F32 && y_dtype != y16))
+    if (!dt_valid(x_dtype) || (y_dtype != SQLLM_DT_F32 && y_dtype != y16))
         return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or the "
                                   "16-bit type of x (SQLLM_DT_F16 for fp32 x)", x_dtype, y_dtype);
     return lutgemv_fused(a, x, x_dtype, y, y_dtype, bias, workspace, workspace_bytes, nullptr, static_cast<cudaStream_t>(stream));
@@ -1862,13 +1877,10 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int
 
 int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
                            void *stream) {
-    if (!a) return fail(SQLLM_EINVAL, "null args");
-    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
-    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
-    if (a->out_features <= 0) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
+    int rc = check_layer(a, 32, 1);
+    if (rc) return rc;
     if ((a->out_features + tc::BN - 1) / tc::BN > 65535) return fail(SQLLM_EINVAL, "out_features=%d exceeds %d", a->out_features, 65535 * tc::BN);
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x) must be >= 1 (got %d)", a->batch);
-    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
     if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
     if (x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "x_dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", x_dtype);
     if (y_dtype != SQLLM_DT_F32 && y_dtype != x_dtype) return fail(SQLLM_EINVAL, "y_dtype=%d must be SQLLM_DT_F32 or x's dtype (%d)", y_dtype, x_dtype);
@@ -1876,35 +1888,17 @@ int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dty
         return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
     if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
     if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
-    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
-    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
     const bool bf = x_dtype == SQLLM_DT_BF16;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int dev = 0;
-        int rc = cur_dev(dev);
-        if (!rc) rc = bf ? set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4, true>, tc::L<3>::SMEM)
-                         : set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<4, false>, tc::L<2>::SMEM);
-        if (!rc) rc = bf ? set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3, true>, tc::L<3>::SMEM)
-                         : set_max_smem(g_dev[dev], tc::lutgemm_tc_kernel<3, false>, tc::L<2>::SMEM);
-        if (rc) return rc;
-    }
+    const auto kern = a->bits == 4 ? (bf ? tc::lutgemm_tc_kernel<4, true> : tc::lutgemm_tc_kernel<4, false>)
+                                   : (bf ? tc::lutgemm_tc_kernel<3, true> : tc::lutgemm_tc_kernel<3, false>);
+    const int smem = bf ? tc::L<3>::SMEM : tc::L<2>::SMEM;
+    if ((rc = dev_setup({{kern, smem}}))) return rc;
     tc::PT p;
-    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    set_layer(p, *a);
     p.x = static_cast<const unsigned short *>(x); p.y = y; p.y_16 = y_dtype != SQLLM_DT_F32; p.bias = bias;
-    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-    const bool hyb = a->full_rows && a->topX > 0;
-    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
     p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
     const dim3 grid((a->batch + tc::BM - 1) / tc::BM, (a->out_features + tc::BN - 1) / tc::BN);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (bf) {
-        if (a->bits == 4) tc::lutgemm_tc_kernel<4, true><<<grid, tc::THREADS, tc::L<3>::SMEM, st>>>(p);
-        else tc::lutgemm_tc_kernel<3, true><<<grid, tc::THREADS, tc::L<3>::SMEM, st>>>(p);
-    } else {
-        if (a->bits == 4) tc::lutgemm_tc_kernel<4, false><<<grid, tc::THREADS, tc::L<2>::SMEM, st>>>(p);
-        else tc::lutgemm_tc_kernel<3, false><<<grid, tc::THREADS, tc::L<2>::SMEM, st>>>(p);
-    }
+    kern<<<grid, tc::THREADS, smem, static_cast<cudaStream_t>(stream)>>>(p);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_fused launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
@@ -1915,74 +1909,47 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *a, const void *x, void *y, int 
 }
 
 int sqllm_lutgemv_rows_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias, void *stream) {
+    int rc = check_layer(a, 32, 4);
+    if (rc) return rc;
     if ((x_dtype != SQLLM_DT_F16 && x_dtype != SQLLM_DT_BF16) || (y_dtype != SQLLM_DT_F32 && y_dtype != x_dtype))
         return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or x's dtype", x_dtype, y_dtype);
-    const bool bf = x_dtype == SQLLM_DT_BF16;
-    if (!a) return fail(SQLLM_EINVAL, "null args");
-    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
-    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
     if (a->in_features > SQLLM_ROWS_MAX_IN) return fail(SQLLM_EINVAL, "in_features=%d exceeds %d: the slab of x a CTA stages would not fit its shared memory", a->in_features, SQLLM_ROWS_MAX_IN);
-    if (a->out_features <= 0 || a->out_features % 4) return fail(SQLLM_EINVAL, "out_features=%d must be a positive multiple of 4", a->out_features);
     if ((a->out_features + STRIP - 1) / STRIP > 65535) return fail(SQLLM_EINVAL, "out_features=%d exceeds %d", a->out_features, 65535 * STRIP);
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x) must be >= 1 (got %d)", a->batch);
-    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
     if (!x || !y) return fail(SQLLM_EINVAL, "x / y must not be null");
     if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3) || (reinterpret_cast<uintptr_t>(bias) & 3))
         return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
     if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
     if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
-    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
-    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
     int sm = 0;
+    if ((rc = dev_setup({}, &sm))) return rc;
     RowsPlan pl;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int dev = 0;
-        int rc = cur_dev(dev);
-        if (rc) return rc;
-        sm = g_dev[dev].sm;
-        if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
-        if ((rc = set_max_smem(g_dev[dev], krows_lookup(a->bits, pl.RB, bf), 227 * 1024))) return rc;
-    }
+    if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
+    const KRows kern = krows_lookup(a->bits, pl.RB, x_dtype == SQLLM_DT_BF16);
+    if ((rc = dev_setup({{kern, 227 * 1024}}))) return rc;
     const int groups = (a->batch + pl.RB - 1) / pl.RB;
     if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
     rows::PR p;
     memset(&p, 0, sizeof(p));
-    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    set_layer(p, *a);
     p.x = x; p.y = y; p.y_16 = y_dtype != SQLLM_DT_F32; p.bias = bias;
-    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-    const bool hyb = a->full_rows && a->topX > 0;
-    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
     p.K = a->in_features; p.N = a->out_features; p.M = a->batch; p.R = a->bits == 4 ? p.K / 8 : p.K / 32;
     p.ks = pl.ks; p.kpad = pl.kpad;
     p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0;
-    // the one launch with a cluster dimension: the S CTAs of a strip's cluster split its K
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(pl.S, (a->out_features + STRIP - 1) / STRIP, groups);
-    cfg.blockDim = dim3(rows::RTHREADS);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = pl.S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, krows_lookup(a->bits, pl.RB, bf), p);
+    // the S CTAs of a strip's cluster split its K
+    const cudaError_t e = launch_ex(kern, dim3(pl.S, (a->out_features + STRIP - 1) / STRIP, groups), rows::RTHREADS, pl.smem,
+                                    static_cast<cudaStream_t>(stream), cluster_of(pl.S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 
 int sqllm_lutgemm_t(const sqllm_lutgemv_args *a, const void *dy, int dy_dtype, void *dx, int dx_dtype, int path, void *stream) {
-    if (!a) return fail(SQLLM_EINVAL, "null args");
-    if (a->bits != 3 && a->bits != 4) return fail(SQLLM_EINVAL, "bits must be 3 or 4 (got %d)", a->bits);
-    if (a->in_features <= 0 || a->in_features % 32) return fail(SQLLM_EINVAL, "in_features=%d must be a positive multiple of 32", a->in_features);
+    int rc = check_layer(a, 32, 1);
+    if (rc) return rc;
     if ((a->in_features + bwd::KS - 1) / bwd::KS > 65535) return fail(SQLLM_EINVAL, "in_features=%d exceeds %d", a->in_features, 65535 * bwd::KS);
-    if (a->out_features <= 0) return fail(SQLLM_EINVAL, "out_features=%d must be positive", a->out_features);
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of dy) must be >= 1 (got %d)", a->batch);
-    if (!a->qweight || !a->lookup_table) return fail(SQLLM_EINVAL, "qweight / lookup_table must not be null");
     if (!dy || !dx) return fail(SQLLM_EINVAL, "dy / dx must not be null");
-    if (dy_dtype != SQLLM_DT_F32 && dy_dtype != SQLLM_DT_F16 && dy_dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
+    if (!dt_valid(dy_dtype)) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
     if (dx_dtype != SQLLM_DT_F32 && dx_dtype != dy_dtype) return fail(SQLLM_EINVAL, "dx_dtype=%d must be SQLLM_DT_F32 or dy's dtype (%d)", dx_dtype, dy_dtype);
     if (path < 0 || path > 2) return fail(SQLLM_EINVAL, "path=%d must be 0 (auto), 1 (tensor cores) or 2 (CUDA cores)", path);
     if (path == 1 && dy_dtype == SQLLM_DT_F32) return fail(SQLLM_EINVAL, "path=1 (tensor cores) takes fp16 or bf16 dy, not fp32");
@@ -1990,78 +1957,42 @@ int sqllm_lutgemm_t(const sqllm_lutgemv_args *a, const void *dy, int dy_dtype, v
         return fail(SQLLM_EINVAL, "qweight and lookup_table must be 4-byte aligned");
     if (reinterpret_cast<uintptr_t>(dy) & (dy_dtype == SQLLM_DT_F32 ? 3 : 1)) return fail(SQLLM_EINVAL, "dy must be aligned to its element size");
     if (reinterpret_cast<uintptr_t>(dx) & 15) return fail(SQLLM_EINVAL, "dx must be 16-byte aligned");
-    if (a->topX < 0) return fail(SQLLM_EINVAL, "topX < 0");
-    if (a->full_rows && a->topX > 0 && !a->full_row_indices) return fail(SQLLM_EINVAL, "full_rows given without full_row_indices");
     if (path == 0) path = dy_dtype != SQLLM_DT_F32 && a->batch >= SQLLM_BWD_TC_MIN_ROWS ? 1 : 2;
     if (path == 1) {
         const bool bf = dy_dtype == SQLLM_DT_BF16;
-        {
-            std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-            int dev = 0;
-            int rc = cur_dev(dev);
-            if (!rc) rc = bf ? set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<4, true>, tct::L<3>::SMEM)
-                             : set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<4, false>, tct::L<2>::SMEM);
-            if (!rc) rc = bf ? set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<3, true>, tct::L<3>::SMEM)
-                             : set_max_smem(g_dev[dev], tct::lutgemm_tc_t_kernel<3, false>, tct::L<2>::SMEM);
-            if (rc) return rc;
-        }
+        const auto kern = a->bits == 4 ? (bf ? tct::lutgemm_tc_t_kernel<4, true> : tct::lutgemm_tc_t_kernel<4, false>)
+                                       : (bf ? tct::lutgemm_tc_t_kernel<3, true> : tct::lutgemm_tc_t_kernel<3, false>);
+        const int smem = bf ? tct::L<3>::SMEM : tct::L<2>::SMEM;
+        if ((rc = dev_setup({{kern, smem}}))) return rc;
         tct::PT p;
         memset(&p, 0, sizeof(p));
-        p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+        set_layer(p, *a);
         p.dy = dy; p.dx = dx; p.dx_dt = dx_dtype;
-        p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-        const bool hyb = a->full_rows && a->topX > 0;
-        p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
         p.M = a->batch; p.K = a->in_features; p.N = a->out_features;
         p.dy_al16 = (reinterpret_cast<uintptr_t>(dy) & 15) == 0 && a->out_features % 8 == 0;
         const dim3 grid((a->batch + tc::BM - 1) / tc::BM, (a->in_features + tct::BK - 1) / tct::BK);
-        cudaStream_t st = static_cast<cudaStream_t>(stream);
-        if (bf) {
-            if (a->bits == 4) tct::lutgemm_tc_t_kernel<4, true><<<grid, tct::THREADS, tct::L<3>::SMEM, st>>>(p);
-            else tct::lutgemm_tc_t_kernel<3, true><<<grid, tct::THREADS, tct::L<3>::SMEM, st>>>(p);
-        } else {
-            if (a->bits == 4) tct::lutgemm_tc_t_kernel<4, false><<<grid, tct::THREADS, tct::L<2>::SMEM, st>>>(p);
-            else tct::lutgemm_tc_t_kernel<3, false><<<grid, tct::THREADS, tct::L<2>::SMEM, st>>>(p);
-        }
+        kern<<<grid, tct::THREADS, smem, static_cast<cudaStream_t>(stream)>>>(p);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_t (tensor cores) launch failed: %s", cudaGetErrorString(e));
         return SQLLM_OK;
     }
     int sm = 0;
+    if ((rc = dev_setup({}, &sm))) return rc;
     TPlan pl;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int dev = 0;
-        int rc = cur_dev(dev);
-        if (rc) return rc;
-        sm = g_dev[dev].sm;
-        t_plan(a->in_features, a->out_features, a->batch, sm, pl);
-        if ((rc = set_max_smem(g_dev[dev], kt_lookup(a->bits, pl.RB), pl.smem))) return rc;
-    }
+    t_plan(a->in_features, a->out_features, a->batch, sm, pl);
+    const KT kern = kt_lookup(a->bits, pl.RB);
+    if ((rc = dev_setup({{kern, pl.smem}}))) return rc;
     const int groups = (a->batch + pl.RB - 1) / pl.RB;
     if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
     bwd::PT p;
     memset(&p, 0, sizeof(p));
-    p.qw = reinterpret_cast<const uint32_t *>(a->qweight); p.lut = a->lookup_table;
+    set_layer(p, *a);
     p.dy = dy; p.dx = dx; p.dy_dt = dy_dtype; p.dx_dt = dx_dtype;
-    p.rows = a->rows; p.cols = a->cols; p.vals = a->vals;
-    const bool hyb = a->full_rows && a->topX > 0;
-    p.full_rows = hyb ? a->full_rows : nullptr; p.fri = hyb ? a->full_row_indices : nullptr; p.topX = hyb ? a->topX : 0;
     p.K = a->in_features; p.N = a->out_features; p.M = a->batch;
     p.strips = (a->out_features + STRIP - 1) / STRIP;
     p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0 && a->out_features % 4 == 0;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(pl.S, (a->in_features + bwd::KS - 1) / bwd::KS, groups);
-    cfg.blockDim = dim3(bwd::TTHREADS);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = pl.S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kt_lookup(a->bits, pl.RB), p);
+    const cudaError_t e = launch_ex(kern, dim3(pl.S, (a->in_features + bwd::KS - 1) / bwd::KS, groups), bwd::TTHREADS, pl.smem,
+                                    static_cast<cudaStream_t>(stream), cluster_of(pl.S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemm_t launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -2076,9 +2007,8 @@ int sqllm_lut_grad(const sqllm_lutgemv_args *a, const void *x, int x_dtype, cons
     if (a->batch < 1) return fail(SQLLM_EINVAL, "batch (rows of x and dy) must be >= 1 (got %d)", a->batch);
     if (!a->qweight) return fail(SQLLM_EINVAL, "qweight must not be null");
     if (!x || !dy) return fail(SQLLM_EINVAL, "x / dy must not be null");
-    const auto dt_ok = [](int d) { return d == SQLLM_DT_F32 || d == SQLLM_DT_F16 || d == SQLLM_DT_BF16; };
-    if (!dt_ok(x_dtype)) return fail(SQLLM_EINVAL, "x_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", x_dtype);
-    if (!dt_ok(dy_dtype)) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
+    if (!dt_valid(x_dtype)) return fail(SQLLM_EINVAL, "x_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", x_dtype);
+    if (!dt_valid(dy_dtype)) return fail(SQLLM_EINVAL, "dy_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", dy_dtype);
     if (path < 0 || path > 2) return fail(SQLLM_EINVAL, "path=%d must be 0 (auto), 1 (tensor cores) or 2 (CUDA cores)", path);
     const bool tc_dtypes = x_dtype == dy_dtype && x_dtype != SQLLM_DT_F32;
     if (path == 1 && !tc_dtypes)
@@ -2116,27 +2046,12 @@ int sqllm_lut_grad(const sqllm_lutgemv_args *a, const void *x, int x_dtype, cons
         kern = a->bits == 4 ? lg::lut_grad_kernel<4> : lg::lut_grad_kernel<3>;
         smem = lg::SMEM;
     }
-    int S = 1;
-    {
-        std::lock_guard<std::recursive_mutex> lk(g_state_mu);
-        int dev = 0;
-        int rc = cur_dev(dev);
-        if (rc) return rc;
-        S = lg_split(a->in_features, a->out_features, g_dev[dev].sm);
-        if ((rc = set_max_smem(g_dev[dev], kern, smem))) return rc;
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(S, (a->out_features + lg::TC - 1) / lg::TC);
-    cfg.blockDim = dim3(lg::THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
+    int sm = 0;
+    const int rc = dev_setup({{kern, smem}}, &sm);
+    if (rc) return rc;
+    const int S = lg_split(a->in_features, a->out_features, sm);
+    const cudaError_t e = launch_ex(kern, dim3(S, (a->out_features + lg::TC - 1) / lg::TC), lg::THREADS, smem,
+                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lut_grad launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }

@@ -154,7 +154,10 @@ std::mutex g_ws_mutex;
 std::map<std::pair<int, void *>, torch::Tensor> g_ws;  // (device, stream) -> zero-initialised workspace
 std::vector<torch::Tensor> g_ws_retired;               // outgrown workspaces: never freed, a captured CUDA graph may still point at them
 
-torch::Tensor workspace_for(const torch::Tensor &like, size_t bytes) {
+// the workspace of the current (device, stream) for the fused call of layer a, on like's device
+torch::Tensor workspace_for(const torch::Tensor &like, const sqllm_lutgemv_args &a) {
+    const size_t bytes = sqllm_workspace_bytes(a.bits, a.in_features, a.out_features, a.topX);
+    TORCH_CHECK(bytes > 0, "sqllm_workspace_bytes failed: ", sqllm_last_error());
     std::lock_guard<std::mutex> lock(g_ws_mutex);
     const auto key = std::make_pair((int)like.get_device(), cur_stream());
     auto it = g_ws.find(key);
@@ -169,14 +172,14 @@ torch::Tensor workspace_for(const torch::Tensor &like, size_t bytes) {
     return it->second;
 }
 
-// shared argument checking / descriptor filling of the fused entry points: everything but the shape of x
+// shared argument checking / descriptor filling of the fused entry points: everything but the dtype and the shape of x (each
+// binding checks those)
 void fill_layer_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
                      const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
                      const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
                      const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
-                     const c10::optional<torch::Tensor> &full_row_indices, bool check_x_dtype = true) {
+                     const c10::optional<torch::Tensor> &full_row_indices) {
     TORCH_CHECK(x.is_cuda() && x.is_contiguous(), "x must be a contiguous CUDA tensor");
-    if (check_x_dtype) TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
     TORCH_CHECK(bits == 3 || bits == 4, "bits must be 3 or 4");
     need(qweight, "qweight", torch::kInt32, x);
     need(lookup_table, "lookup_table", torch::kFloat32, x);
@@ -211,17 +214,13 @@ void fill_layer_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::T
     }
 }
 
-// ... of the matvec entry points: x holds one input vector, fp16 or fp32 (and bf16 where bf16_ok: lutgemv_fused; the exchange and
-// sequence paths are fp16 / fp32 only)
+// ... of the matvec entry points: x holds one input vector
 void fill_fused_args(sqllm_lutgemv_args &a, const float *&bias_p, const torch::Tensor &x, const torch::Tensor &qweight,
                      const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
                      const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
                      const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
-                     const c10::optional<torch::Tensor> &full_row_indices, bool bf16_ok = false) {
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, !bf16_ok);
-    if (bf16_ok)
-        TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32 || x.scalar_type() == torch::kBFloat16,
-                    "x must be fp16, bf16 or fp32");
+                     const c10::optional<torch::Tensor> &full_row_indices) {
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
     TORCH_CHECK(x.numel() == a.in_features, "x has ", x.numel(), " elements, expected in_features=", a.in_features);
 }
 
@@ -236,44 +235,57 @@ int dtype_code(const torch::Tensor &t, const char *what) {
     return -1;
 }
 
+// "path" of lutgemm_t and lut_grad -> the path code of sqllm_lutgemm_t / sqllm_lut_grad
+int path_code(const std::string &path, const char *name) {
+    TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", name, ": path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
+    return path == "auto" ? 0 : path == "tc" ? 1 : 2;
+}
+
+// The bindings x [M, in] -> y [M, out] in x's dtype: the shape checks, y and the call of `entry` (sqllm_lutgemm_fused_dt or
+// sqllm_lutgemv_rows_dt).  The binding `name` has checked x's dtype.
+typedef int (*RowsEntry)(const sqllm_lutgemv_args *, const void *, int, void *, int, const float *, void *);
+torch::Tensor layer_rows(const char *name, RowsEntry entry, const torch::Tensor &x, const torch::Tensor &qweight,
+                         const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
+                         const c10::optional<torch::Tensor> &rows, const c10::optional<torch::Tensor> &cols,
+                         const c10::optional<torch::Tensor> &vals, const c10::optional<torch::Tensor> &full_rows,
+                         const c10::optional<torch::Tensor> &full_row_indices) {
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, name, ": x must be [M, in_features=", a.in_features, "]");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, name, ": x must have 1 to 2^31-1 rows");
+    a.batch = (int)x.size(0);
+    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
+    const int dt = dtype_code(x, "x");
+    const int rc = entry(&a, x.data_ptr(), dt, y.data_ptr(), dt, bias_p, cur_stream());
+    TORCH_CHECK(rc == SQLLM_OK, "quant_cuda.", name, ": ", sqllm_last_error());
+    return y;
+}
+
 // y [M, out] = bias + LUT-GEMM(x) [+ CSR] [+ dense rows] from fp16 or bf16 x [M, in], in x's dtype, on the tensor cores
 // (sqllm_lutgemm_fused_dt): QuantLinearLUT.forward's batched branch (squeezellm/quant.py:314-379) in one launch.
 torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
                             c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
                             c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
                             c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
-    const at::cuda::OptionalCUDAGuard guard(device_of(x));
-    sqllm_lutgemv_args a;
-    const float *bias_p;
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, false);
     TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kBFloat16,
                 "lutgemm_fused: x must be fp16 or bf16 (got ", x.scalar_type(), ")");
-    const int dt = dtype_code(x, "lutgemm_fused: x");
-    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemm_fused: x must be [M, in_features=", a.in_features, "]");
-    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemm_fused: x must have 1 to 2^31-1 rows");
-    a.batch = (int)x.size(0);
-    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
-    check_status(sqllm_lutgemm_fused_dt(&a, x.data_ptr(), dt, y.data_ptr(), dt, bias_p, cur_stream()), "quant_cuda.lutgemm_fused");
-    return y;
+    return layer_rows("lutgemm_fused", sqllm_lutgemm_fused_dt, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows,
+                      full_row_indices);
 }
 
-// y [M, out] fp16 = bias + LUT-GEMV(x) [+ CSR] [+ dense rows] from fp16 x [M, in], a few rows on the CUDA cores (sqllm_lutgemv_rows):
+// y [M, out] fp16 = bias + LUT-GEMV(x) [+ CSR] [+ dense rows] from fp16 x [M, in], a few rows on the CUDA cores (sqllm_lutgemv_rows_dt):
 // QuantLinearLUT.forward's batched branch for 2 to QuantLinearLUT.ROWS_MAX rows in one launch.  bf16 x: lutgemv_rows_bf16.
 torch::Tensor lutgemv_rows(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
                            c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
                            c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
                            c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
-    const at::cuda::OptionalCUDAGuard guard(device_of(x));
-    sqllm_lutgemv_args a;
-    const float *bias_p;
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    // bf16 x is refused with the message of the fp16 / fp32 decode bindings (it has lutgemv_rows_bf16), fp32 x with its own
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
     TORCH_CHECK(x.scalar_type() == torch::kFloat16, "lutgemv_rows: x must be fp16");
-    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemv_rows: x must be [M, in_features=", a.in_features, "]");
-    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemv_rows: x must have 1 to 2^31-1 rows");
-    a.batch = (int)x.size(0);
-    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
-    check_status(sqllm_lutgemv_rows(&a, x.data_ptr(), y.data_ptr(), 1, bias_p, cur_stream()), "quant_cuda.lutgemv_rows");
-    return y;
+    return layer_rows("lutgemv_rows", sqllm_lutgemv_rows_dt, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows,
+                      full_row_indices);
 }
 
 // The same for bf16 x [M, in] -> bf16 y [M, out] (sqllm_lutgemv_rows_dt): QuantLinearLUT.forward's batched branch for 2 to
@@ -282,18 +294,9 @@ torch::Tensor lutgemv_rows_bf16(torch::Tensor x, torch::Tensor qweight, torch::T
                                 c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
                                 c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
                                 c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
-    const at::cuda::OptionalCUDAGuard guard(device_of(x));
-    sqllm_lutgemv_args a;
-    const float *bias_p;
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, false);
     TORCH_CHECK(x.scalar_type() == torch::kBFloat16, "lutgemv_rows_bf16: x must be bf16 (got ", x.scalar_type(), ")");
-    TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lutgemv_rows_bf16: x must be [M, in_features=", a.in_features, "]");
-    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "lutgemv_rows_bf16: x must have 1 to 2^31-1 rows");
-    a.batch = (int)x.size(0);
-    torch::Tensor y = torch::empty({x.size(0), (int64_t)a.out_features}, x.options());
-    check_status(sqllm_lutgemv_rows_dt(&a, x.data_ptr(), SQLLM_DT_BF16, y.data_ptr(), SQLLM_DT_BF16, bias_p, cur_stream()),
-                 "quant_cuda.lutgemv_rows_bf16");
-    return y;
+    return layer_rows("lutgemv_rows_bf16", sqllm_lutgemv_rows_dt, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows,
+                      full_row_indices);
 }
 
 // dx [M, in] = dy [M, out] . W^T (LUT + CSR + dense rows), in dy's dtype (fp16, bf16 or fp32): the input gradient of
@@ -305,15 +308,14 @@ torch::Tensor lutgemm_t(torch::Tensor dy, torch::Tensor qweight, torch::Tensor l
     const at::cuda::OptionalCUDAGuard guard(device_of(dy));
     sqllm_lutgemv_args a;
     const float *bias_p;
-    fill_layer_args(a, bias_p, dy, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices, false);
+    fill_layer_args(a, bias_p, dy, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices);
     const int dt = dtype_code(dy, "lutgemm_t: dy");
-    TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", "lutgemm_t: path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
+    const int pc = path_code(path, "lutgemm_t");
     TORCH_CHECK(dy.dim() == 2 && dy.size(1) == a.out_features, "lutgemm_t: dy must be [M, out_features=", a.out_features, "]");
     TORCH_CHECK(dy.size(0) >= 1 && dy.size(0) <= INT32_MAX, "lutgemm_t: dy must have 1 to 2^31-1 rows");
     a.batch = (int)dy.size(0);
     torch::Tensor dx = torch::empty({dy.size(0), (int64_t)a.in_features}, dy.options());
-    check_status(sqllm_lutgemm_t(&a, dy.data_ptr(), dt, dx.data_ptr(), dt, path == "auto" ? 0 : path == "tc" ? 1 : 2, cur_stream()),
-                 "quant_cuda.lutgemm_t");
+    check_status(sqllm_lutgemm_t(&a, dy.data_ptr(), dt, dx.data_ptr(), dt, pc, cur_stream()), "quant_cuda.lutgemm_t");
     return dx;
 }
 
@@ -326,10 +328,10 @@ py::tuple lut_grad(torch::Tensor x, torch::Tensor dy, torch::Tensor qweight, tor
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
     sqllm_lutgemv_args a;
     const float *bias_p;
-    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices, false);
+    fill_layer_args(a, bias_p, x, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices);
     const int xdt = dtype_code(x, "lut_grad: x"), dydt = dtype_code(dy, "lut_grad: dy");
     TORCH_CHECK(dy.is_cuda() && dy.is_contiguous() && dy.device() == x.device(), "lut_grad: dy must be a contiguous CUDA tensor on x's device");
-    TORCH_CHECK(path == "auto" || path == "tc" || path == "cuda", "lut_grad: path must be 'auto', 'tc' or 'cuda' (got '", path, "')");
+    const int pc = path_code(path, "lut_grad");
     TORCH_CHECK(x.dim() == 2 && x.size(1) == a.in_features, "lut_grad: x must be [M, in_features=", a.in_features, "]");
     TORCH_CHECK(dy.dim() == 2 && dy.size(1) == a.out_features && dy.size(0) == x.size(0),
                 "lut_grad: dy must be [M=", x.size(0), ", out_features=", a.out_features, "]");
@@ -346,9 +348,7 @@ py::tuple lut_grad(torch::Tensor x, torch::Tensor dy, torch::Tensor qweight, tor
     float *pl = want_lut ? dlut.data_ptr<float>() : nullptr, *pv = want_vals && dvals.numel() ? dvals.data_ptr<float>() : nullptr;
     float *pf = want_full_rows ? dfull.data_ptr<float>() : nullptr;
     if (pl || pv || pf)  // else only an empty dvals was asked for
-        check_status(sqllm_lut_grad(&a, x.data_ptr(), xdt, dy.data_ptr(), dydt, pl, pv, pf, path == "auto" ? 0 : path == "tc" ? 1 : 2,
-                                    cur_stream()),
-                     "quant_cuda.lut_grad");
+        check_status(sqllm_lut_grad(&a, x.data_ptr(), xdt, dy.data_ptr(), dydt, pl, pv, pf, pc, cur_stream()), "quant_cuda.lut_grad");
     auto opt = [](const torch::Tensor &t) -> py::object { return t.defined() ? py::cast(t) : py::none(); };
     return py::make_tuple(opt(dlut), opt(dvals), opt(dfull));
 }
@@ -360,12 +360,12 @@ torch::Tensor lutgemv_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
                             c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
                             c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32 || x.scalar_type() == torch::kBFloat16,
+                "x must be fp16, bf16 or fp32");
     sqllm_lutgemv_args a;
     const float *bias_p;
-    fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices, true);
-    const size_t need_ws = sqllm_workspace_bytes(bits, a.in_features, a.out_features, a.topX);
-    TORCH_CHECK(need_ws > 0, "sqllm_workspace_bytes failed: ", sqllm_last_error());
-    torch::Tensor ws = workspace_for(x, need_ws);
+    fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
+    torch::Tensor ws = workspace_for(x, a);
     torch::Tensor y = torch::empty({(int64_t)a.out_features}, x.options());
     const int dt = dtype_code(x, "lutgemv_fused: x");
     const int rc = sqllm_lutgemv_fused_dt(&a, x.data_ptr(), dt, y.data_ptr(), dt, bias_p, ws.data_ptr(), (size_t)ws.numel(), cur_stream());
@@ -382,12 +382,11 @@ void lutgemv_fused_exchange(torch::Tensor x, torch::Tensor qweight, torch::Tenso
                             int64_t peer_base, int64_t out_offset, int64_t flag_offset, int64_t state_offset, int64_t error_offset,
                             int world, int rank, int members, int out_features_full) {
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
     sqllm_lutgemv_args a;
     const float *bias_p;
     fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
-    const size_t need_ws = sqllm_workspace_bytes(bits, a.in_features, a.out_features, a.topX);
-    TORCH_CHECK(need_ws > 0, "sqllm_workspace_bytes failed: ", sqllm_last_error());
-    torch::Tensor ws = workspace_for(x, need_ws);
+    torch::Tensor ws = workspace_for(x, a);
     sqllm_exchange xc;
     memset(&xc, 0, sizeof(xc));
     xc.world = world; xc.rank = rank; xc.members = members; xc.out_features_full = out_features_full;
@@ -428,7 +427,7 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
         it.out_features_full = t[13].cast<int>();
         TORCH_CHECK(qweight.is_cuda() && qweight.dim() == 2 && (bits == 3 || bits == 4), "sequence item ", i, ": qweight must be a packed CUDA matrix");
         const int K = (int)(qweight.size(0) / bits * 32);
-        torch::Tensor xs;  // what the shared checks look at (device, dtype, numel): the external input, or a stand-in of the right length
+        torch::Tensor xs;  // what the shared checks look at (device, numel): the external input, or a stand-in of the right length
         if (it.x_from < 0) {
             TORCH_CHECK(!t[11].is_none(), "sequence item ", i, ": x_from = -1 needs x_ext");
             xs = t[11].cast<torch::Tensor>();
