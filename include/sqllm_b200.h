@@ -49,8 +49,8 @@ extern "C" {
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
-                                 sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt (backward compatible,
-                                 same version) */
+                                 sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize
+                                 (backward compatible, same version) */
 
 int sqllm_abi_version(void);
 const char *sqllm_last_error(void);
@@ -157,8 +157,8 @@ int sqllm_lutgemm_fused(const sqllm_lutgemv_args *args, const void *x_half, void
 int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void *y, int y_is_half, const float *bias,
                        void *stream);
 
-/* Element types of the tensors of sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_lutgemm_t and
- * sqllm_lut_grad. */
+/* Element types of the tensors of sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_lutgemm_t,
+ * sqllm_lut_grad and sqllm_dequantize. */
 #define SQLLM_DT_F32 0
 #define SQLLM_DT_F16 1
 #define SQLLM_DT_BF16 2
@@ -241,6 +241,22 @@ int sqllm_lutgemm_t(const sqllm_lutgemv_args *args, const void *dy, int dy_dtype
 #define SQLLM_LUT_GRAD_TC_MIN_ROWS 8
 int sqllm_lut_grad(const sqllm_lutgemv_args *args, const void *x, int x_dtype, const void *dy, int dy_dtype, float *dlut, float *dvals,
                    float *dfull_rows, int path, void *stream);
+
+/* The dense weight of the layer's output channels [col0, col0 + ncols): W [ncols][in_features] (row-major: nn.Linear.weight's
+ * [out, in] layout) of w_dtype = SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, written (not accumulated).  Every element is
+ *   w  = lookup_table[c][idx(k, c)]                                        (fp32)
+ *   w += vals[e]          for each CSR entry e of row c with cols[e] == k, in storage order          (fp32 adds)
+ *   w += full_rows[k][j]  for each j with full_row_indices[j] == c, in ascending j                  (fp32 adds)
+ *   W[c - col0][k] = w rounded once, to nearest even, to w_dtype
+ * CSR columns outside [0, in_features) and dense-row channels outside [0, out_features) are ignored; duplicates add up; no limit
+ * on topX or on the entries per CSR row.  The codebook is the stored fp32 table: sqllm_set_lut_mode does not apply.  The column
+ * range lets a caller dequantize one member of stacked sibling layers without copying the packed weights.  args->vec, mul and
+ * batch are ignored.  Every output is written once by one thread: bit-reproducible.  Requirements (checked, SQLLM_EINVAL
+ * otherwise): in_features % 32 == 0, out_features >= 1, 0 <= col0, ncols >= 1, col0 + ncols <= out_features, non-null qweight /
+ * lookup_table / w, full_row_indices present with full_rows, topX >= 0, qweight and
+ * lookup_table 4-byte aligned, w 16-byte aligned.  No workspace, no allocation, no host synchronisation: CUDA-graph capturable
+ * and safe on several streams at once. */
+int sqllm_dequantize(const sqllm_lutgemv_args *args, int col0, int ncols, void *w, int w_dtype, void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

@@ -11,6 +11,7 @@ import shutil
 import subprocess
 import sys
 import sysconfig
+import tempfile
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
@@ -58,33 +59,51 @@ def build_ext(verbose=False):
     import torch
     from torch.utils import cpp_extension
 
-    build_lib(verbose)
     src = os.path.join(CSRC, "quant_cuda_pybind.cpp")
     hdr = os.path.join(INCLUDE, "sqllm_b200.h")
     out = ext_path()
-    if _newer(out, [src, hdr]):
-        tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
-        inc = []
-        for p in cpp_extension.include_paths("cuda") + [sysconfig.get_paths()["include"], INCLUDE]:
-            inc += ["-isystem" if "torch" in p or "cuda" in p else "-I", p]
-        abi = int(torch._C._GLIBCXX_USE_CXX11_ABI)
-        cmd = [_cxx(), "-std=c++17", "-O2", "-fPIC", "-shared", "-fvisibility=hidden",
-               f"-D_GLIBCXX_USE_CXX11_ABI={abi}", "-DTORCH_EXTENSION_NAME=quant_cuda", "-DTORCH_API_INCLUDE_EXTENSION_H",
-               *inc, src, "-o", out,
-               "-L", PKG, "-lsqllm_b200", "-Wl,-rpath,$ORIGIN",
-               "-L", tlib, "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch", "-ltorch_python",
-               f"-Wl,-rpath,{tlib}"]
-        cuda_lib = "/usr/local/cuda/lib64"
-        if os.path.isdir(cuda_lib):
-            cmd += ["-L", cuda_lib, "-lcudart"]
+    if not _newer(out, [src, hdr]):
+        build_lib(verbose)
+        return out
+    tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
+    inc = []
+    for p in cpp_extension.include_paths("cuda") + [sysconfig.get_paths()["include"], INCLUDE]:
+        inc += ["-isystem" if "torch" in p or "cuda" in p else "-I", p]
+    abi = int(torch._C._GLIBCXX_USE_CXX11_ABI)
+    tmp = tempfile.mkdtemp(prefix="sqllm_ext_")
+    obj = os.path.join(tmp, "quant_cuda_pybind.o")
+    compile_cmd = [_cxx(), "-std=c++17", "-O2", "-fPIC", "-fvisibility=hidden",
+                   f"-D_GLIBCXX_USE_CXX11_ABI={abi}", "-DTORCH_EXTENSION_NAME=quant_cuda", "-DTORCH_API_INCLUDE_EXTENSION_H",
+                   *inc, "-c", src, "-o", obj]
+    link_cmd = [_cxx(), "-shared", obj, "-o", out,
+                "-L", PKG, "-lsqllm_b200", "-Wl,-rpath,$ORIGIN",
+                "-L", tlib, "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch", "-ltorch_python",
+                f"-Wl,-rpath,{tlib}"]
+    cuda_lib = "/usr/local/cuda/lib64"
+    if os.path.isdir(cuda_lib):
+        link_cmd += ["-L", cuda_lib, "-lcudart"]
+    if verbose:
+        print(" ".join(compile_cmd))
+    try:
+        # the adapter compiles against the header alone: its compile runs while nvcc builds the library, only the link waits
+        proc = subprocess.Popen(compile_cmd)
+        try:
+            build_lib(verbose)
+        finally:
+            rc = proc.wait()
+        if rc:
+            raise subprocess.CalledProcessError(rc, compile_cmd)
         if verbose:
-            print(" ".join(cmd))
-        subprocess.check_call(cmd)
+            print(" ".join(link_cmd))
+        subprocess.check_call(link_cmd)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
     return out
 
 
 def build_all(verbose=False):
-    return build_lib(verbose), build_ext(verbose)
+    ext = build_ext(verbose)  # builds the library too, overlapped with the adapter's compile
+    return lib_path(), ext
 
 
 if __name__ == "__main__":

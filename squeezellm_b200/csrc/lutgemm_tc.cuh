@@ -125,6 +125,13 @@ __device__ __forceinline__ void dec3(float (&w)[32], const uint32_t w0, const ui
     w[J] = lds_f32(lb + (idx3<J>(w0, w1, w2) << 9));
     if constexpr (J + 1 < 32) dec3<J + 1>(w, w0, w1, w2, lb);
 }
+// the 32 weights of a 4-bit group from its four words (8 nibbles each, lowest first)
+__device__ __forceinline__ void dec4(float (&w)[32], const uint32_t (&q)[4], const uint32_t lb) {
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int n = 0; n < 8; ++n) w[8 * r + n] = lds_f32(lb + (((q[r] >> (4 * n)) & 15u) << 9));
+}
 
 __device__ __forceinline__ void add_at(float (&w)[32], const int kk, const float v) {  // w[kk] += v, kk in [0, 32), registers only
 #pragma unroll
@@ -243,10 +250,7 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
             const uint32_t q0 = wq[0], q1 = wq[1], q2 = wq[2], q3 = wq[3];
             load_words(i + 1);
             const uint32_t q[4] = {q0, q1, q2, q3};
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int n = 0; n < 8; ++n) w[8 * r + n] = lds_f32(lb + (((q[r] >> (4 * n)) & 15u) << 9));
+            dec4(w, q, lb);
         } else {
             const uint32_t q0 = wq[0], q1 = wq[1], q2 = wq[2];
             load_words(i + 1);

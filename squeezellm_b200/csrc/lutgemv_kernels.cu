@@ -954,6 +954,7 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lut_grad.cuh"
 #include "lut_grad_tc.cuh"
 #include "kmeans1d.cuh"
+#include "dequant.cuh"
 
 // shared-window address at which a kernel without static shared memory sees its dynamic shared memory (the v2 carve-up aligns
 // tables to their own size - up to 64 KB - so the host needs the real address, not a worst case; the kernel re-checks it)
@@ -2053,6 +2054,33 @@ int sqllm_lut_grad(const sqllm_lutgemv_args *a, const void *x, int x_dtype, cons
     const cudaError_t e = launch_ex(kern, dim3(S, (a->out_features + lg::TC - 1) / lg::TC), lg::THREADS, smem,
                                     static_cast<cudaStream_t>(stream), cluster_of(S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lut_grad launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+int sqllm_dequantize(const sqllm_lutgemv_args *a, int col0, int ncols, void *w, int w_dtype, void *stream) {
+    int rc = check_layer(a, 32, 1);
+    if (rc) return rc;
+    if ((a->in_features + dq::BK - 1) / dq::BK > 65535) return fail(SQLLM_EINVAL, "in_features=%d exceeds %d", a->in_features, 65535 * dq::BK);
+    if (col0 < 0 || ncols < 1 || col0 > a->out_features - ncols)
+        return fail(SQLLM_EINVAL, "column range col0=%d, ncols=%d must be non-empty and lie in [0, out_features=%d)", col0, ncols, a->out_features);
+    if (!w) return fail(SQLLM_EINVAL, "w must not be null");
+    if (!dt_valid(w_dtype)) return fail(SQLLM_EINVAL, "w_dtype=%d is not SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16", w_dtype);
+    if ((reinterpret_cast<uintptr_t>(a->qweight) & 3) || (reinterpret_cast<uintptr_t>(a->lookup_table) & 3))
+        return fail(SQLLM_EINVAL, "qweight and lookup_table must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(w) & 15) return fail(SQLLM_EINVAL, "w must be 16-byte aligned");
+    void (*kern)(const dq::PD);
+    if (w_dtype == SQLLM_DT_F32) kern = a->bits == 4 ? dq::dequant_kernel<4, float> : dq::dequant_kernel<3, float>;
+    else if (w_dtype == SQLLM_DT_F16) kern = a->bits == 4 ? dq::dequant_kernel<4, __half> : dq::dequant_kernel<3, __half>;
+    else kern = a->bits == 4 ? dq::dequant_kernel<4, __nv_bfloat16> : dq::dequant_kernel<3, __nv_bfloat16>;
+    if ((rc = dev_setup({{kern, dq::SMEM}}))) return rc;
+    dq::PD p;
+    memset(&p, 0, sizeof(p));
+    set_layer(p, *a);
+    p.K = a->in_features; p.N = a->out_features; p.c0 = col0; p.n = ncols; p.w = w;
+    const dim3 grid((ncols + dq::BN - 1) / dq::BN, (a->in_features + dq::BK - 1) / dq::BK);
+    kern<<<grid, dq::THREADS, dq::SMEM, static_cast<cudaStream_t>(stream)>>>(p);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "dequantize launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -471,6 +471,27 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
     return reinterpret_cast<int64_t>(h);
 }
 
+// W [ncols, in] in `dtype` (fp32, fp16 or bf16) = the dense weight of output channels [col0, col0 + ncols) (codebook + CSR + dense
+// rows, sqllm_dequantize): QuantLinearLUT.dequantize.  ncols = -1: to the last channel.  A new tensor on qweight's device.
+torch::Tensor dequantize(torch::Tensor qweight, torch::Tensor lookup_table, int bits, c10::optional<torch::Tensor> rows,
+                         c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals, c10::optional<torch::Tensor> full_rows,
+                         c10::optional<torch::Tensor> full_row_indices, at::ScalarType dtype, int64_t col0, int64_t ncols) {
+    TORCH_CHECK(qweight.defined() && qweight.is_cuda() && qweight.is_contiguous(), "dequantize: qweight must be a contiguous CUDA tensor");
+    const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
+    sqllm_lutgemv_args a;
+    const float *bias_p;
+    fill_layer_args(a, bias_p, qweight, qweight, lookup_table, bits, c10::nullopt, rows, cols, vals, full_rows, full_row_indices);
+    TORCH_CHECK(dtype == torch::kFloat32 || dtype == torch::kFloat16 || dtype == torch::kBFloat16,
+                "dequantize: dtype must be torch.float32, torch.float16 or torch.bfloat16 (got ", dtype, ")");
+    if (ncols == -1) ncols = a.out_features - col0;
+    TORCH_CHECK(col0 >= 0 && ncols >= 1 && col0 + ncols <= a.out_features, "dequantize: columns [col0=", col0, ", col0 + ncols=",
+                col0 + ncols, ") must be non-empty and lie in [0, out_features=", a.out_features, ")");
+    torch::Tensor w = torch::empty({ncols, (int64_t)a.in_features}, qweight.options().dtype(dtype));
+    const int dt = dtype == torch::kFloat32 ? SQLLM_DT_F32 : dtype == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
+    check_status(sqllm_dequantize(&a, (int)col0, (int)ncols, w.data_ptr(), dt, cur_stream()), "quant_cuda.dequantize");
+    return w;
+}
+
 torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
     need(qweight, "qweight", torch::kInt32, qweight);
@@ -583,6 +604,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "labels uint8 [rows, n]); deterministic", py::arg("w"), py::arg("sample_weight"), py::arg("k"));
     m.def("pack_indices", &pack_indices, "labels uint8 [out, in] -> qweight int32 [in/32*bits, out] in the reference's packed layout",
           py::arg("labels"), py::arg("bits"));
+    m.def("dequantize", &dequantize, "dense weight of QuantLinearLUT: W [ncols, in] in dtype (codebook + CSR + dense rows) for output channels "
+          "[col0, col0 + ncols); ncols = -1: to the last channel; one launch",
+          py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("rows") = py::none(), py::arg("cols") = py::none(),
+          py::arg("vals") = py::none(), py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none(),
+          py::arg("dtype") = torch::kFloat16, py::arg("col0") = 0, py::arg("ncols") = -1);
     m.def("unpack_indices", &unpack_indices, "GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },

@@ -127,6 +127,18 @@ class SiblingGroup:
             self._x = self._y = None
         return y
 
+    def dissolve(self):
+        """Make every member a stand-alone layer again: buffers that are views of the stacked layer become the member's own
+        contiguous copies, and the member forgets the group (its forward then runs its own buffers)."""
+        for m in self.members:
+            for name in ("qweight", "lookup_table"):
+                t = getattr(m, name)
+                if t._base is not None:  # a view of the stacked buffer (share_storage)
+                    setattr(m, name, t.clone(memory_format=torch.contiguous_format))
+            object.__setattr__(m, "_sibling_group", None)
+        self._x = self._y = None
+        self._pending = set()
+
 
 def fuse_siblings(model, groups=LLAMA_SIBLINGS, share_storage=True):
     """Group sibling QuantLinearLUT attributes of every sub-module of `model` (default: LLaMA's q/k/v and gate/up).

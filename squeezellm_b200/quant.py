@@ -28,6 +28,8 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
   * `train_codebook()` makes the codebook (and optionally the CSR values, dense rows and bias) nn.Parameters on the same storage:
     their gradients come from ONE more launch (`quant_cuda.lut_grad`: G = x^T . dy bucketed by the packed indices); the indices
     stay fixed and the checkpoint format does not change.
+  * `dequantize(dtype)` gives the dense [out, in] weight the layer stands for (codebook + CSR outliers + dense rows, one launch:
+    `quant_cuda.dequantize`) and `to_linear(dtype)` an nn.Linear holding it; the reference has neither.
   * `balanced=True` raises NotImplementedError up front: the reference dispatches it to
     `vecquant{3,4}matmul_spmv_balanced_nuq_perchannel`, which its extension never defines
     (quant.py:238,282 vs quant_cuda.cpp:257-270), i.e. an AttributeError at the first forward.
@@ -283,6 +285,29 @@ class QuantLinearLUT(nn.Module):
         rows, cols, vals, fr, fri = self._sparse_args()
         path = "tc" if dy.dtype in (torch.float16, torch.bfloat16) and dy.shape[0] >= QuantLinearLUT.BWD_TC_MIN_ROWS else "cuda"
         return quant_cuda.lutgemm_t(_aligned(dy), self.qweight, self.lookup_table, self.bits, rows, cols, vals, fr, fri, path=path)
+
+    def dequantize(self, dtype=torch.float16):
+        """The dense weight this layer stands for, [out, in] (nn.Linear.weight's layout) in `dtype` (fp16, bf16 or fp32) on the
+        layer's device, without gradient: codebook + CSR outliers + dense rows summed in fp32 and rounded once
+        (quant_cuda.dequantize, one launch; include/sqllm_b200.h: sqllm_dequantize gives the exact order).  A sibling member
+        (fusion.fuse_siblings) dequantizes its rows of the stacked layer; a layer whose codebook is being trained
+        (train_codebook) uses the parameters' current values.  The bias is not part of it (see to_linear)."""
+        col0, layer = 0, self
+        if self._sibling_group is not None:
+            group, index = self._sibling_group
+            col0, layer = group.offsets[index], group.layer
+        rows, cols, vals, fr, fri = (t.detach() if t is not None else None for t in layer._sparse_args())
+        return quant_cuda.dequantize(layer.qweight, layer.lookup_table.detach(), layer.bits, rows, cols, vals, fr, fri,
+                                     dtype=dtype, col0=col0, ncols=self.outfeatures)
+
+    def to_linear(self, dtype=torch.float16):
+        """An nn.Linear on the layer's device with weight = dequantize(dtype) and the bias cast to `dtype`."""
+        weight = self.dequantize(dtype)
+        linear = nn.Linear(self.infeatures, self.outfeatures, bias=self.bias is not None, device="meta")
+        linear.weight = nn.Parameter(weight)
+        if self.bias is not None:
+            linear.bias = nn.Parameter(self.bias.detach().to(dtype=dtype, copy=True))
+        return linear
 
     def _forward_impl(self, x):
         if self._sibling_group is not None:

@@ -10,6 +10,8 @@ squeezellm/outliers.py, quantization/generate_outlier_config.py, squeezellm/quan
   * `quantize_linear` / `quantize_model`: the codebook fit, then the pack of quant.py:97-208 on the device (quant_cuda.pack_indices
     and a CSR of outlier minus zero centroid); buffers bit-identical to QuantLinearLUT.pack2 on the same inputs.
     `checkpoint.save_checkpoint` writes the result in the reference's format.
+  * `dequantize_model`: the way back, every QuantLinearLUT replaced by an nn.Linear holding its dense weight
+    (QuantLinearLUT.to_linear, quant_cuda.dequantize), e.g. to export a fine-tuned model as a plain dense checkpoint.
 
 The Fisher information (the squared gradients) is the caller's: a state dict keyed like the model's (`<layer>.weight`).
 """
@@ -18,7 +20,7 @@ import torch
 from .checkpoint import find_linear_layers
 from .quant import QuantLinearLUT, quant_cuda
 
-__all__ = ["kmeans_codebook", "outlier_threshold", "split_outliers", "quantize_linear", "quantize_model"]
+__all__ = ["kmeans_codebook", "outlier_threshold", "split_outliers", "quantize_linear", "quantize_model", "dequantize_model"]
 
 
 def kmeans_codebook(weight, sample_weight, bits):
@@ -154,3 +156,18 @@ def quantize_model(model, fisher_state, bits, outlier_range=None, sensitivity=0.
             numvals[name] = q.numvals
         del linear
     return numvals
+
+
+def dequantize_model(model, dtype=torch.float16):
+    """The inverse of quantize_model: replace every QuantLinearLUT below `model` by its QuantLinearLUT.to_linear(dtype), in place
+    and one layer at a time, after dissolving the sibling groups (fusion.fuse_siblings) of its layers.  model.state_dict() then
+    has the keys of the dense model (`<layer>.weight`, `<layer>.bias`), so e.g. a Hugging Face model's save_pretrained writes a
+    plain dense checkpoint.  Returns the names of the replaced layers."""
+    layers = find_linear_layers(model, kinds=(QuantLinearLUT,))
+    for q in layers.values():
+        if q._sibling_group is not None:
+            q._sibling_group[0].dissolve()
+    names = list(layers)
+    for name in names:
+        _set_module(model, name, layers.pop(name).to_linear(dtype))
+    return names
