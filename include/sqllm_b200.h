@@ -49,7 +49,8 @@ extern "C" {
 
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
-                                 sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize
+                                 sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
+                                 sqllm_fisher_accumulate
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -257,6 +258,22 @@ int sqllm_lut_grad(const sqllm_lutgemv_args *args, const void *x, int x_dtype, c
  * lookup_table 4-byte aligned, w 16-byte aligned.  No workspace, no allocation, no host synchronisation: CUDA-graph capturable
  * and safe on several streams at once. */
 int sqllm_dequantize(const sqllm_lutgemv_args *args, int col0, int ncols, void *w, int w_dtype, void *stream);
+
+/* The diagonal of the empirical Fisher information of a linear layer, accumulated into fisher [out_features][in_features] (fp32,
+ * row-major: nn.Linear.weight's [out, in] layout).  x [rows][in_features] and dy [rows][out_features] (the layer's input and the
+ * gradient of its output) are row-major, both of dtype = SQLLM_DT_F16 or SQLLM_DT_BF16; sample s is rows [s seq_len, (s + 1)
+ * seq_len).  Every element is
+ *   g_s   = sum_{t in sample s} dy[t][n] x[t][k]    per 64-row chunk of the sample, in ascending order: the chunk's exact products
+ *                                                   summed in the tensor core's fp32 accumulator, the chunk sums added in fp32
+ *   f     = fmaf(g_s, g_s, f)                       for s = 0, 1, ... in ascending order, from f = 0 (fp32)
+ *   fisher[n][k] = fisher[n][k] + f                 (one fp32 add)
+ * so fisher gains sum_s g_s^2: the squares of the per-sample weight gradients, not the square of their sum.  Every element is read
+ * once and written once by one thread: bit-reproducible.  Requirements (checked, SQLLM_EINVAL otherwise): rows, seq_len >= 1,
+ * rows % seq_len == 0, in_features and out_features positive multiples of 8, out_features <= 8388480, non-null x / dy / fisher,
+ * all three 16-byte aligned.
+ * No workspace, no atomics, no host synchronisation: CUDA-graph capturable and safe on several streams at once. */
+int sqllm_fisher_accumulate(const void *x, const void *dy, int dtype, int rows, int seq_len, int in_features, int out_features,
+                            float *fisher, void *stream);
 
 /* Fused forward of a COLUMN SHARD with the exchange built in (multi-GPU; the reference has none - north_star's
  * "column-shard each QuantLinear + all-reduce on the output vector", done by the kernel instead of a separate collective).

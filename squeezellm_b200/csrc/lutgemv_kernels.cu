@@ -953,6 +953,7 @@ __global__ void unpack_kernel(int bits, const uint32_t *__restrict__ q, int K, i
 #include "lutgemm_tc_t.cuh"
 #include "lut_grad.cuh"
 #include "lut_grad_tc.cuh"
+#include "fisher.cuh"
 #include "kmeans1d.cuh"
 #include "dequant.cuh"
 
@@ -2081,6 +2082,36 @@ int sqllm_dequantize(const sqllm_lutgemv_args *a, int col0, int ncols, void *w, 
     kern<<<grid, dq::THREADS, dq::SMEM, static_cast<cudaStream_t>(stream)>>>(p);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "dequantize launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+int sqllm_fisher_accumulate(const void *x, const void *dy, int dtype, int rows, int seq_len, int in_features, int out_features,
+                            float *fisher, void *stream) {
+    if (dtype != SQLLM_DT_F16 && dtype != SQLLM_DT_BF16)
+        return fail(SQLLM_EINVAL, "fisher_accumulate: dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", dtype);
+    if (rows < 1) return fail(SQLLM_EINVAL, "fisher_accumulate: rows=%d must be >= 1", rows);
+    if (seq_len < 1) return fail(SQLLM_EINVAL, "fisher_accumulate: seq_len=%d must be >= 1", seq_len);
+    if (rows % seq_len) return fail(SQLLM_EINVAL, "fisher_accumulate: rows=%d must be a multiple of seq_len=%d", rows, seq_len);
+    if (in_features < 1 || in_features % 8)
+        return fail(SQLLM_EINVAL, "fisher_accumulate: in_features=%d must be a positive multiple of 8", in_features);
+    if (out_features < 1 || out_features % 8)
+        return fail(SQLLM_EINVAL, "fisher_accumulate: out_features=%d must be a positive multiple of 8", out_features);
+    if ((out_features + fis::TN - 1) / fis::TN > 65535)
+        return fail(SQLLM_EINVAL, "fisher_accumulate: out_features=%d exceeds %d", out_features, 65535 * fis::TN);
+    if (!x || !dy || !fisher) return fail(SQLLM_EINVAL, "fisher_accumulate: x / dy / fisher must not be null");
+    if (((uintptr_t)x | (uintptr_t)dy | (uintptr_t)fisher) & 15)
+        return fail(SQLLM_EINVAL, "fisher_accumulate: x / dy / fisher must be 16-byte aligned");
+    void (*kern)(const fis::PF) = dtype == SQLLM_DT_BF16 ? fis::fisher_kernel<true> : fis::fisher_kernel<false>;
+    const int rc = dev_setup({{kern, fis::SMEM}});
+    if (rc) return rc;
+    fis::PF p;
+    memset(&p, 0, sizeof(p));
+    p.x = x; p.dy = dy; p.f = fisher;
+    p.rows = rows; p.T = seq_len; p.K = in_features; p.N = out_features;
+    const dim3 grid((in_features + fis::TK - 1) / fis::TK, (out_features + fis::TN - 1) / fis::TN);
+    // a cluster of one, not PDL: the kernel does not wait on the grid dependency, it reads x, dy and F as the previous kernel left them
+    const cudaError_t e = launch_ex(kern, grid, fis::THREADS, fis::SMEM, static_cast<cudaStream_t>(stream), cluster_of(1), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "fisher_accumulate launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
 

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -492,6 +492,33 @@ torch::Tensor dequantize(torch::Tensor qweight, torch::Tensor lookup_table, int 
     return w;
 }
 
+// fisher [out, in] fp32 += sum_s (dy_s^T x_s)^2 over the samples of seq_len rows of x [rows, in] and dy [rows, out], both fp16 or
+// both bf16 (sqllm_fisher_accumulate), in place.
+void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, int64_t seq_len) {
+    TORCH_CHECK(x.defined() && x.is_cuda() && x.is_contiguous(), "fisher_accumulate: x must be a contiguous CUDA tensor");
+    TORCH_CHECK(dy.defined() && dy.is_cuda() && dy.is_contiguous(), "fisher_accumulate: dy must be a contiguous CUDA tensor");
+    TORCH_CHECK(fisher.defined() && fisher.is_cuda() && fisher.is_contiguous(), "fisher_accumulate: fisher must be a contiguous CUDA tensor");
+    TORCH_CHECK(dy.device() == x.device(), "fisher_accumulate: dy is on ", dy.device(), " but x is on ", x.device());
+    TORCH_CHECK(fisher.device() == x.device(), "fisher_accumulate: fisher is on ", fisher.device(), " but x is on ", x.device());
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kBFloat16,
+                "fisher_accumulate: x must be fp16 or bf16 (got ", x.scalar_type(), ")");
+    TORCH_CHECK(dy.scalar_type() == x.scalar_type(), "fisher_accumulate: dy must have x's dtype ", x.scalar_type(), " (got ", dy.scalar_type(), ")");
+    TORCH_CHECK(fisher.scalar_type() == torch::kFloat32, "fisher_accumulate: fisher must be fp32 (got ", fisher.scalar_type(), ")");
+    TORCH_CHECK(x.dim() == 2 && dy.dim() == 2, "fisher_accumulate: x must be [rows, in] and dy [rows, out]");
+    TORCH_CHECK(dy.size(0) == x.size(0), "fisher_accumulate: dy has ", dy.size(0), " rows but x has ", x.size(0));
+    TORCH_CHECK(fisher.dim() == 2 && fisher.size(0) == dy.size(1) && fisher.size(1) == x.size(1), "fisher_accumulate: fisher must be [out=",
+                dy.size(1), ", in=", x.size(1), "] (got ", fisher.sizes(), ")");
+    TORCH_CHECK(x.size(0) >= 1 && x.size(0) <= INT32_MAX, "fisher_accumulate: x must have 1 to 2^31-1 rows (got ", x.size(0), ")");
+    TORCH_CHECK(x.size(1) <= INT32_MAX && dy.size(1) <= INT32_MAX, "fisher_accumulate: in and out must be below 2^31");
+    TORCH_CHECK(seq_len >= 1 && x.size(0) % seq_len == 0, "fisher_accumulate: seq_len=", seq_len, " must be >= 1 and divide the ",
+                x.size(0), " rows of x");
+    const at::cuda::OptionalCUDAGuard guard(device_of(x));
+    const int dt = x.scalar_type() == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
+    check_status(sqllm_fisher_accumulate(x.data_ptr(), dy.data_ptr(), dt, (int)x.size(0), (int)seq_len, (int)x.size(1), (int)dy.size(1),
+                                         fisher.data_ptr<float>(), cur_stream()),
+                 "quant_cuda.fisher_accumulate");
+}
+
 torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
     need(qweight, "qweight", torch::kInt32, qweight);
@@ -609,6 +636,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("rows") = py::none(), py::arg("cols") = py::none(),
           py::arg("vals") = py::none(), py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none(),
           py::arg("dtype") = torch::kFloat16, py::arg("col0") = 0, py::arg("ncols") = -1);
+    m.def("fisher_accumulate", &fisher_accumulate, "Fisher information of a linear layer, in place: fisher fp32 [out, in] += sum over "
+          "the samples of seq_len rows of (dy_s^T x_s)^2, x [rows, in] and dy [rows, out] both fp16 or both bf16; one launch",
+          py::arg("x"), py::arg("dy"), py::arg("fisher"), py::arg("seq_len"));
     m.def("unpack_indices", &unpack_indices, "GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },

@@ -12,15 +12,20 @@ squeezellm/outliers.py, quantization/generate_outlier_config.py, squeezellm/quan
     `checkpoint.save_checkpoint` writes the result in the reference's format.
   * `dequantize_model`: the way back, every QuantLinearLUT replaced by an nn.Linear holding its dense weight
     (QuantLinearLUT.to_linear, quant_cuda.dequantize), e.g. to export a fine-tuned model as a plain dense checkpoint.
-
-The Fisher information (the squared gradients) is the caller's: a state dict keyed like the model's (`<layer>.weight`).
+  * `fisher_information`: the first stage, the weights of the k-means: the diagonal of the empirical Fisher information, the sum
+    over calibration sequences of each sequence's squared weight gradient (quant_cuda.fisher_accumulate, DESIGN.md section 3.15).
+    Its result is the `fisher_state` quantize_model takes, so fisher_information -> quantize_model -> save_checkpoint turns a
+    dense model into a SqueezeLLM checkpoint.
 """
 import torch
 
 from .checkpoint import find_linear_layers
 from .quant import QuantLinearLUT, quant_cuda
 
-__all__ = ["kmeans_codebook", "outlier_threshold", "split_outliers", "quantize_linear", "quantize_model", "dequantize_model"]
+__all__ = ["kmeans_codebook", "outlier_threshold", "split_outliers", "quantize_linear", "quantize_model", "dequantize_model",
+           "fisher_information"]
+
+_FISHER_DTYPES = (torch.float16, torch.bfloat16)  # the operand types of quant_cuda.fisher_accumulate
 
 
 def kmeans_codebook(weight, sample_weight, bits):
@@ -171,3 +176,96 @@ def dequantize_model(model, dtype=torch.float16):
     for name in names:
         _set_module(model, name, layers.pop(name).to_linear(dtype))
     return names
+
+
+def fisher_information(model, batches, layers=None, skip=("lm_head",)):
+    """The diagonal of the empirical Fisher information of the model's linear layers: {f"{name}.weight": fp32 [out, in]} with
+    F = sum over every sequence s of every batch of g_s * g_s, g_s the layer's weight gradient of s's loss alone.  The result is
+    the `fisher_state` of quantize_model.
+
+    model: a Hugging Face causal LM in fp16 or bf16, called as model(ids).logits.  batches: an iterable of token tensors [B, T]
+    (T >= 2), one sequence per row.  layers: names from checkpoint.find_linear_layers (not in `skip`) to restrict the result to -
+    the fp32 result of a 7B model's decoder linears takes 25.9 GB, so a large model can be done in several passes; None: every
+    linear not in `skip`.
+
+    The loss of a sequence is the SUM of its next-token cross-entropies and a batch's loss is the sum over its sequences, so every
+    g_s is the gradient of a batch holding s alone, and the batching changes F by rounding only.  (The sum also keeps the logit
+    gradients O(1) rather than O(1/T), clear of fp16 underflow.)  F's scale does not matter to quantize_model: the weighted k-means
+    and the sensitivity top-k are invariant to a constant factor.
+
+    One backward per batch: forward hooks keep each selected layer's input x, a hook on its output receives dy, and
+    quant_cuda.fisher_accumulate adds sum_s (dy_s^T x_s)^2 into F on the tensor cores, from the 16-bit x and dy, without forming
+    any weight gradient.  No parameter requires grad during the run (the embedding's output does), so no .grad is created; the
+    hooks, requires_grad and the training mode are restored afterwards, also on error.  Raises ValueError for a layer that runs
+    more than once in one forward (tied or reused weights: its per-call squares would be wrong), is not fp16 / bf16, or has in or
+    out features not a multiple of 8, and for a result that is not finite."""
+    found = find_linear_layers(model)
+    for name in skip:
+        found.pop(name, None)
+    if layers is not None:
+        unknown = [n for n in layers if n not in found]
+        if unknown:
+            raise ValueError(f"fisher_information: layers {unknown[:4]} are not linear layers of the model outside skip={tuple(skip)}")
+        found = {n: found[n] for n in layers}
+    if not found:
+        raise ValueError("fisher_information: no layer selected")
+    for name, lin in found.items():
+        if lin.weight.dtype not in _FISHER_DTYPES:
+            raise ValueError(f"fisher_information: layer {name} is {lin.weight.dtype}; fp16 or bf16 is needed")
+        if lin.in_features % 8 or lin.out_features % 8:
+            raise ValueError(f"fisher_information: layer {name} is {lin.in_features} -> {lin.out_features}; in and out features must be "
+                             "multiples of 8")
+    fisher = {name: torch.zeros(lin.out_features, lin.in_features, device=lin.weight.device,
+                                dtype=torch.promote_types(torch.float32, lin.weight.dtype)) for name, lin in found.items()}
+    calls = dict.fromkeys(found, 0)
+    seq_len = [0]
+
+    def layer_hook(name):
+        def hook(module, inputs, out):
+            calls[name] += 1
+            if calls[name] > 1:
+                raise ValueError(f"fisher_information: layer {name} ran more than once in one forward (tied or reused weights)")
+            x = inputs[0].detach()
+            rows = x.numel() // module.in_features
+            if rows % seq_len[0] or not out.requires_grad:
+                raise ValueError(f"fisher_information: layer {name} did not see [B, T={seq_len[0]}, in] rows on the path to the loss")
+            x = x.reshape(rows, module.in_features).contiguous()
+            out.register_hook(lambda dy: quant_cuda.fisher_accumulate(
+                x, dy.reshape(rows, module.out_features).contiguous(), fisher[name], seq_len[0]))
+        return hook
+
+    def embed_hook(module, inputs, out):
+        return out.requires_grad_()
+
+    saved = [(p, p.requires_grad) for p in model.parameters()]
+    was_training = model.training
+    handles = []
+    try:
+        for p, _ in saved:
+            p.requires_grad_(False)
+        model.eval()
+        handles.append(model.get_input_embeddings().register_forward_hook(embed_hook))
+        handles += [lin.register_forward_hook(layer_hook(name)) for name, lin in found.items()]
+        for ids in batches:
+            if ids.dim() != 2 or ids.shape[1] < 2:
+                raise ValueError(f"fisher_information: a batch must be token ids [B, T] with T >= 2 (got {tuple(ids.shape)})")
+            seq_len[0] = ids.shape[1]
+            for name in calls:
+                calls[name] = 0
+            with torch.enable_grad():
+                logits = model(ids).logits
+                logits = logits[:, :-1].reshape(-1, logits.shape[-1])
+                logits = logits.to(torch.promote_types(logits.dtype, torch.float32))  # fp32 softmax of 16-bit logits
+                loss = torch.nn.functional.cross_entropy(logits, ids[:, 1:].reshape(-1), reduction="sum")
+                del logits
+                loss.backward()
+    finally:
+        for h in handles:
+            h.remove()
+        for p, rg in saved:
+            p.requires_grad_(rg)
+        model.train(was_training)
+    for name, f in fisher.items():
+        if not bool(torch.isfinite(f).all()):
+            raise ValueError(f"fisher_information: the Fisher information of layer {name} is not finite")
+    return {f"{name}.weight": f for name, f in fisher.items()}
