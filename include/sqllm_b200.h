@@ -50,7 +50,7 @@ extern "C" {
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
-                                 sqllm_fisher_accumulate
+                                 sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -300,6 +300,12 @@ int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *args,
                                  const void *x, int x_is_half, int y_is_half, const float *bias,
                                  void *workspace, size_t workspace_bytes, const sqllm_exchange *xchg, void *stream);
 
+/* sqllm_lutgemv_fused_exchange with dtype codes: x of x_dtype, the destination vectors of y_dtype, exactly the pairs of
+ * sqllm_lutgemv_fused_dt (SQLLM_DT_BF16 x: SQLLM_DT_F32 or SQLLM_DT_BF16 vectors, each element rounded once with the bias inside
+ * the fp32 sum); any other pair: SQLLM_EINVAL with sqllm_lutgemv_fused_dt's message.  sqllm_lutgemv_fused_exchange calls this. */
+int sqllm_lutgemv_fused_exchange_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, int y_dtype, const float *bias,
+                                    void *workspace, size_t workspace_bytes, const sqllm_exchange *xchg, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * The reference's 12 launchers, one C entry point each.
  * ------------------------------------------------------------------------------------------- */
@@ -377,7 +383,8 @@ int sqllm_vecquant4matmul_spmv_hybrid_nuq_perchannel_batched(const int32_t *rows
  * Replaces the reference's per-layer launch loop during decode (squeezellm/llama.py:226-234 calls
  * QuantLinearLUT.forward once per layer; each forward is quant.py:212-312, i.e. 1-3 launches of
  * quant_cuda_kernel.cu:132-738).  Every item is one fused matvec (as sqllm_lutgemv_fused, fp16 in
- * and out); its input is either an external fp16 vector or a slice of an earlier item's output.
+ * and out, or bf16 in and out with sqllm_sequence_create_dt); its input is either an external
+ * vector or a slice of an earlier item's output.
  * The kernel keeps the weight stream running across item boundaries and hands results from one
  * item to the next as self-validating tagged words in an arena (csrc/lutgemv_seq.cuh) - no
  * launch, no grid-wide barrier, no fence between two matvecs.  All items share `bits`.
@@ -395,8 +402,8 @@ typedef struct sqllm_seq_item {
     const float *bias;       /* optional, [out_features] */
     int x_from;              /* -1: x_ext ; i >= 0: the (full-length) output vector of item i < this item's index */
     int x_offset;            /* first element of that vector this item reads (multiple of 4); it reads in_features elements */
-    const void *x_ext;       /* fp16 [in_features], read by every run (x_from == -1) */
-    void *y;                 /* optional plain fp16 [out_features] copy of this item's own output columns */
+    const void *x_ext;       /* [in_features] of the sequence's dtype (fp16 unless sqllm_sequence_create_dt says bf16), read by every run (x_from == -1) */
+    void *y;                 /* optional plain [out_features] copy of this item's own output columns, of the sequence's dtype */
     int members;             /* several GPUs: the item stacks `members` column shards of equal width (else 1) */
     int out_features_full;   /* several GPUs: full length of one member's output vector (else out_features) */
 } sqllm_seq_item;
@@ -407,7 +414,7 @@ typedef struct sqllm_seq_options {
     void *arena;             /* world > 1: this rank's peer-visible arena (zero-filled once); NULL on one GPU: allocated here */
     size_t arena_bytes;
     const uint64_t *peer_base; /* world > 1: DEVICE array of `world` arena base addresses as seen from this rank */
-    int n_export;            /* results wanted as plain fp16 vectors: item indices and destinations (full length) */
+    int n_export;            /* results wanted as plain vectors of the sequence's dtype: item indices and destinations (full length) */
     const int *export_items;
     void *const *export_dst;
     uint64_t *trace;         /* debug builds (-DSQLLM_TRACE): [n_items][1024][32] time stamps, else NULL */
@@ -416,6 +423,12 @@ typedef struct sqllm_seq_options {
 /* bytes of arena a sequence over these items needs (0 on error) */
 size_t sqllm_sequence_arena_bytes(const sqllm_seq_item *items, int n_items);
 int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, sqllm_sequence **out);
+/* The same for the activation type `dtype`: SQLLM_DT_F16 (what sqllm_sequence_create makes) or SQLLM_DT_BF16.  It is the type of
+ * every x_ext, of the values the items hand over (the low half of each tagged word), of the items' y copies and of the export
+ * destinations; every item's output is rounded to it once, with the bias inside the fp32 sum.  A bf16 sequence uses the exact
+ * table whatever opt->lut_mode says (the pair table multiplies fp16 by fp16).  Any other code: SQLLM_EINVAL (the message names
+ * it), checked before any device access like the other arguments. */
+int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, int dtype, sqllm_sequence **out);
 /* two launches on `stream` (token counter, then the persistent kernel); CUDA-graph capturable */
 int sqllm_sequence_run(sqllm_sequence *s, void *stream);
 /* synchronises `stream`; 1 if a bounded in-kernel wait ever gave up (results incomplete), 0 if not, < 0 on error */

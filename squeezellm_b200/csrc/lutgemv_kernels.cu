@@ -1097,6 +1097,16 @@ void set_layer(P &p, const sqllm_lutgemv_args &a) {
 
 // SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16
 bool dt_valid(int dt) { return dt == SQLLM_DT_F32 || dt == SQLLM_DT_F16 || dt == SQLLM_DT_BF16; }
+// the (x, y) dtype pairs of the one-GEMV entry points (sqllm_lutgemv_fused_dt, sqllm_lutgemv_fused_exchange_dt): y is fp32 or the
+// 16-bit type of x, and that is fp16 for fp32 x
+bool fused_dt_pair(int x_dt, int y_dt) {
+    const int y16 = x_dt == SQLLM_DT_BF16 ? SQLLM_DT_BF16 : SQLLM_DT_F16;
+    return dt_valid(x_dt) && (y_dt == SQLLM_DT_F32 || y_dt == y16);
+}
+int fused_dt_fail(int x_dt, int y_dt) {
+    return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or the "
+                              "16-bit type of x (SQLLM_DT_F16 for fp32 x)", x_dt, y_dt);
+}
 
 // The descriptor checks every GEMV / GEMM entry point shares, in this order: in_features a positive multiple of k_mult (64 or 32),
 // out_features a positive multiple of n_mult (4, or 1 for "positive"), the packed matrix and codebook given, and dense rows only with
@@ -1400,14 +1410,21 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
 // ---- sequences (lutgemv_seq.cuh): plan + descriptors at create time, two launches per run -----------------------------
 typedef void (*KSeq)(const seq::SeqCfg);
 struct KSeqInfo { KSeq fn; int tab, stage, ntb; };
-KSeqInfo kseq_lookup(int bits, int mode, bool multi) {
+// bf16 x always takes the exact table (the pair table multiplies fp16 by fp16), whatever `mode` says
+KSeqInfo kseq_lookup(int bits, int mode, bool multi, bool bf16) {
 #define KSE(B, M, X) KSeqInfo{seq::lutgemv_seq_kernel<B, M, X>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE, v2::C2<B, M>::NTB}
+#define KSB(B, X) KSeqInfo{seq::lutgemv_seq_kernel<B, 0, X, __nv_bfloat16>, v2::C2<B, 0>::TAB, v2::C2<B, 0>::STAGE, v2::C2<B, 0>::NTB}
+    if (bf16) {
+        if (bits == 4) return multi ? KSB(4, true) : KSB(4, false);
+        return multi ? KSB(3, true) : KSB(3, false);
+    }
     if (bits == 4) {
         if (mode == 0) return multi ? KSE(4, 0, true) : KSE(4, 0, false);
         return multi ? KSE(4, 1, true) : KSE(4, 1, false);
     }
     if (mode == 0) return multi ? KSE(3, 0, true) : KSE(3, 0, false);
     return multi ? KSE(3, 1, true) : KSE(3, 1, false);
+#undef KSB
 #undef KSE
 }
 constexpr int SEQ_MAX_ITEMS = 1023;  // the mailbox tag keeps 10 bits for the item
@@ -1442,12 +1459,20 @@ extern "C" size_t sqllm_sequence_arena_bytes(const sqllm_seq_item *items, int n_
 }
 
 extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, sqllm_sequence **out) {
+    return sqllm_sequence_create_dt(items, n_items, opt, SQLLM_DT_F16, out);
+}
+
+extern "C" int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, int dtype, sqllm_sequence **out) {
+    if (dtype != SQLLM_DT_F16 && dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "sequence: dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", dtype);
+    const bool bf = dtype == SQLLM_DT_BF16;
+    const char *const tn = bf ? "bf16" : "fp16";
     if (!items || !opt || !out || n_items <= 0) return fail(SQLLM_EINVAL, "sequence: null / empty arguments");
     if (n_items > SEQ_MAX_ITEMS) return fail(SQLLM_EINVAL, "sequence: at most %d items (got %d)", SEQ_MAX_ITEMS, n_items);
     const int world = opt->world > 0 ? opt->world : 1, rank = opt->rank;
     if (world > 64 || rank < 0 || rank >= world) return fail(SQLLM_EINVAL, "sequence: bad world / rank (%d / %d)", world, rank);
     if (world > 1 && (!opt->arena || !opt->peer_base)) return fail(SQLLM_EINVAL, "sequence: several GPUs need a peer-visible arena and peer_base");
-    const int bits = items[0].a.bits, mode = opt->lut_mode == SQLLM_LUT_FP16_PAIR ? 1 : 0;
+    // bf16 x keeps the exact table in the fp16 table mode, as sqllm_lutgemv_fused_dt does
+    const int bits = items[0].a.bits, mode = opt->lut_mode == SQLLM_LUT_FP16_PAIR && !bf ? 1 : 0;
     int kmax = 0;
     for (int i = 0; i < n_items; ++i) {
         const sqllm_seq_item &it = items[i];
@@ -1466,7 +1491,7 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         if (seq_item_len(it) % 4) return fail(SQLLM_EINVAL, "sequence: item %d: output length must be a multiple of 4", i);
         if (it.x_from >= i || it.x_from < -1) return fail(SQLLM_EINVAL, "sequence: item %d: x_from=%d must name an earlier item (or -1)", i, it.x_from);
         if (it.x_from < 0) {
-            if (!it.x_ext || (reinterpret_cast<uintptr_t>(it.x_ext) & 15)) return fail(SQLLM_EINVAL, "sequence: item %d: x_ext must be a 16-byte aligned fp16 vector", i);
+            if (!it.x_ext || (reinterpret_cast<uintptr_t>(it.x_ext) & 15)) return fail(SQLLM_EINVAL, "sequence: item %d: x_ext must be a 16-byte aligned %s vector", i, tn);
         } else {
             if (it.x_offset < 0 || it.x_offset % 4 || (size_t)it.x_offset + a.in_features > seq_item_len(items[it.x_from]))
                 return fail(SQLLM_EINVAL, "sequence: item %d reads [%d, %d) of item %d's %zu outputs", i, it.x_offset, it.x_offset + a.in_features, it.x_from, seq_item_len(items[it.x_from]));
@@ -1478,15 +1503,15 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
         if (!opt->export_items || !opt->export_dst) return fail(SQLLM_EINVAL, "sequence: export arrays missing");
         const int it = opt->export_items[e];
         if (it < 0 || it >= n_items || !opt->export_dst[e] || (reinterpret_cast<uintptr_t>(opt->export_dst[e]) & 7))
-            return fail(SQLLM_EINVAL, "sequence: export %d: bad item %d or destination (8-byte aligned fp16 vector)", e, it);
+            return fail(SQLLM_EINVAL, "sequence: export %d: bad item %d or destination (8-byte aligned %s vector)", e, it, tn);
     }
-    const KSeqInfo ki = kseq_lookup(bits, mode, world > 1);
+    const KSeqInfo ki = kseq_lookup(bits, mode, world > 1, bf);
     int sm = 0;
     unsigned raw = 0;
     const int rc = dev_setup({{ki.fn, 227 * 1024}}, &sm, &raw);
     if (rc) return rc;
     const unsigned base = (raw + 127u) & ~127u;
-    const int xbytes = (kmax * 2 + 127) & ~127;  // every item's x is staged as fp16 in one buffer, and ntb strip-sum rows follow it
+    const int xbytes = (kmax * 2 + 127) & ~127;  // every item's x is staged in the 16-bit dtype in one buffer, and ntb strip-sum rows follow it
     // no cap from the chunk: the weight stream runs on across items
     const int nst = v2::Carve(base, xbytes, ki.ntb * STRIP * 4, ki.tab, ki.ntb, ki.stage, 0).depth(raw, 227 * 1024, ki.stage, v2::MAXD);
     if (nst < 0) return fail(SQLLM_EINVAL, "sequence: in_features=%d does not fit the shared-memory carve-up of this table mode", kmax);
@@ -1856,21 +1881,24 @@ int sqllm_lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_is_hal
 
 int sqllm_lutgemv_fused_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
                            void *workspace, size_t workspace_bytes, void *stream) {
-    const int y16 = x_dtype == SQLLM_DT_BF16 ? SQLLM_DT_BF16 : SQLLM_DT_F16;  // the 16-bit y of this x: fp16 for fp32 x
-    if (!dt_valid(x_dtype) || (y_dtype != SQLLM_DT_F32 && y_dtype != y16))
-        return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or the "
-                                  "16-bit type of x (SQLLM_DT_F16 for fp32 x)", x_dtype, y_dtype);
+    if (!fused_dt_pair(x_dtype, y_dtype)) return fused_dt_fail(x_dtype, y_dtype);
     return lutgemv_fused(a, x, x_dtype, y, y_dtype, bias, workspace, workspace_bytes, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemv_fused_exchange(const sqllm_lutgemv_args *a, const void *x, int x_is_half, int y_is_half, const float *bias,
                                  void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, void *stream) {
+    return sqllm_lutgemv_fused_exchange_dt(a, x, x_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias,
+                                           workspace, workspace_bytes, xc, stream);
+}
+
+int sqllm_lutgemv_fused_exchange_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtype, int y_dtype, const float *bias,
+                                    void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, void *stream) {
+    if (!fused_dt_pair(x_dtype, y_dtype)) return fused_dt_fail(x_dtype, y_dtype);
     if (!xc) {
         const int rc = check_common(a);
         return rc ? rc : fail(SQLLM_EINVAL, "x / exchange descriptor must not be null");
     }
-    return lutgemv_fused(a, x, x_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, nullptr, y_is_half ? SQLLM_DT_F16 : SQLLM_DT_F32, bias, workspace,
-                         workspace_bytes, xc, static_cast<cudaStream_t>(stream));
+    return lutgemv_fused(a, x, x_dtype, nullptr, y_dtype, bias, workspace, workspace_bytes, xc, static_cast<cudaStream_t>(stream));
 }
 
 int sqllm_lutgemm_fused(const sqllm_lutgemv_args *a, const void *x, void *y, int y_is_half, const float *bias, void *stream) {

@@ -8,10 +8,11 @@
 //   * grid = #SMs, launched ONCE per token; every CTA walks the same list of GEMV descriptors (global memory, written at create time);
 //   * the TMA producer warp never stops at a GEMV boundary: while the consumers finish GEMV g and wait for its result, the ring already
 //     holds the first 128 KB per SM of GEMV g+1 - weights do not depend on activations;
-//   * the dependency itself is data flow, not a grid-wide event: y is written as SELF-VALIDATING 32-bit words {fp16 value, 16-bit tag of
-//     the token} (single-copy atomic: no fence, no flag, no second round trip), the consumers of the next GEMV poll the words of their x
-//     straight out of L2 and repack them into fp16 in shared memory.  A stale word carries the previous token's tag, so nothing is ever
-//     reset.  The cross-CTA mailboxes of v2 carry a (token, GEMV) tag the same way.
+//   * the dependency itself is data flow, not a grid-wide event: y is written as SELF-VALIDATING 32-bit words {16-bit value, 16-bit tag
+//     of the token} (single-copy atomic: no fence, no flag, no second round trip), the consumers of the next GEMV poll the words of their
+//     x straight out of L2 and repack the values in shared memory.  The value is the sequence's activation type (fp16 or bf16: the XT
+//     template parameter); only the word's maker converts, everything else moves bits.  A stale word carries the previous token's tag,
+//     so nothing is ever reset.  The cross-CTA mailboxes of v2 carry a (token, GEMV) tag the same way.
 //   * on several GPUs (column shards) the owner of a strip stores its tagged words into EVERY rank's arena over NVLink; the poll of the
 //     next GEMV is the whole exchange - no collective, no flag round trip (v2's exchange waits on a system-scope flag per launch).
 #pragma once
@@ -22,12 +23,12 @@ using namespace v2;
 struct alignas(128) SeqDesc {
     CUtensorMap tm_big, tm_small;   // 64 columns x (32 units | 2 units) boxes over the packed matrix
     P2 p;                           // the GEMV: buffers, stream-K plan, workspace pointers (accumulator / flags alternate by GEMV parity)
-    const uint32_t *x_tag;          // first tagged word of x in the local arena; null: p.x is a plain fp16 vector (the token's input)
+    const uint32_t *x_tag;          // first tagged word of x in the local arena; null: p.x is a plain 16-bit vector (the token's input)
     unsigned long long y_off;       // byte offset of this GEMV's tagged output vector in every rank's arena
 };
 struct SeqExport {
     const uint32_t *src;            // tagged words in the local arena
-    void *dst;                      // plain fp16
+    void *dst;                      // plain 16-bit vector (the sequence's activation type)
     int n;
 };
 struct SeqCfg {
@@ -54,11 +55,13 @@ __device__ __forceinline__ uint4 ld_relaxed_v4(const uint32_t *p) {
     else asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
     return v;
 }
+__device__ __forceinline__ unsigned short bits16(const __half v) { return __half_as_ushort(v); }
+__device__ __forceinline__ unsigned short bits16(const __nv_bfloat16 v) { return __bfloat16_as_ushort(v); }
 __device__ __forceinline__ bool tags_ok(const uint4 w, const uint32_t want) {
     return (((w.x ^ want) | (w.y ^ want) | (w.z ^ want) | (w.w ^ want)) >> 16) == 0u;
 }
 // Four tagged words (16 bytes) at a time, up to four pieces per thread in flight; a piece that is not there yet is simply read again
-// (bounded: 2 s, then the error word).  Returns through `sink(piece index, lo, hi)`: two packed half2.
+// (bounded: 2 s, then the error word).  Returns through `sink(piece index, lo, hi)`: two packed pairs of 16-bit values.
 template <bool SYS, typename F>
 __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, const int tid, const int nthr, const uint32_t want, int *err, F sink) {
     for (int i0 = tid; i0 < n4; i0 += 4 * nthr) {
@@ -84,10 +87,13 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
 }
 
 
-template <int BITS, int MODE, bool MULTI>
+// XT: the sequence's 16-bit activation type (__half or __nv_bfloat16): the type of x_ext, of the value half of every tagged word, of
+// the items' plain y copies and of the exports.  The poll, the staging and the exports only move bits; a word is made in store_y.
+template <int BITS, int MODE, bool MULTI, typename XT = __half>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c) {
     using C = C2<BITS, MODE>;
-    using XT = __half;
+    static_assert(std::is_same<XT, __half>::value || std::is_same<XT, __nv_bfloat16>::value, "x is fp16 or bf16");
+    static_assert(MODE == 0 || std::is_same<XT, __half>::value, "the pair table multiplies fp16 by fp16: it needs fp16 x");
     constexpr int NTB = C::NTB;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -358,7 +364,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 const int w = MULTI ? N / p.xw_members : 0;
                 auto store_y = [&](int col, float yv) {
                     if (p.bias) yv += __ldg(p.bias + col);
-                    const uint32_t word = (xtag << 16) | (uint32_t)__half_as_ushort(__float2half_rn(yv));
+                    const XT yh = f32_to<XT>(yv);   // the one rounding: the bias is inside the fp32 sum
+                    const uint32_t word = (xtag << 16) | (uint32_t)bits16(yh);
                     if constexpr (!MULTI) {
                         asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(c.arena_base + d.y_off + 4ull * (unsigned)col), "r"(word) : "memory");
                     } else {
@@ -368,7 +375,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                         for (int pr = 0; pr < c.world; ++pr)
                             asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(__ldg(c.peer_base + pr) + d.y_off + 4ull * e), "r"(word) : "memory");
                     }
-                    if (p.out) reinterpret_cast<__half *>(p.out)[col] = __float2half_rn(yv);
+                    // (the same value as yh, converted again as before bf16 existed: reusing yh reschedules the fp16 MULTI instantiations)
+                    if (p.out) reinterpret_cast<XT *>(p.out)[col] = f32_to<XT>(yv);
                 };
                 // per owned strip but the last segment's: [our own sums (+ dense rows), from shared memory] + [the column's outlier sum]
                 TRACE(14, bt == 0);
@@ -522,7 +530,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             TRACE(6, tid == 0);
             q0 += nseg;
         }
-        // exports: plain fp16 copies of the vectors the caller asked for (on several GPUs this is also where the last exchange completes)
+        // exports: plain 16-bit copies of the vectors the caller asked for (on several GPUs this is also where the last exchange completes)
         for (int e = (int)blockIdx.x; e < c.nexport; e += (int)gridDim.x) {
             const SeqExport ex = c.exports[e];
             poll_tagged<MULTI>(ex.src, ex.n / 4, tid, NCT, xwant, c.err, [&](int i, uint32_t lo, uint32_t hi) {

@@ -373,16 +373,14 @@ torch::Tensor lutgemv_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     return y;
 }
 
-// Column shard with the exchange built in (include/sqllm_b200.h, sqllm_lutgemv_fused_exchange): the result is written into every
-// rank's symmetric arena; nothing is returned.  peer_base: address of the device array of arena base addresses.
-void lutgemv_fused_exchange(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
-                            c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
-                            c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
-                            c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices,
-                            int64_t peer_base, int64_t out_offset, int64_t flag_offset, int64_t state_offset, int64_t error_offset,
-                            int world, int rank, int members, int out_features_full) {
+// Column shard with the exchange built in (include/sqllm_b200.h, sqllm_lutgemv_fused_exchange_dt): the result is written into every
+// rank's symmetric arena in x's dtype; nothing is returned.  The binding `name` has checked x's dtype.  peer_base: address of the device array of arena base addresses.
+void exchange_call(const char *name, torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                   c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows, c10::optional<torch::Tensor> cols,
+                   c10::optional<torch::Tensor> vals, c10::optional<torch::Tensor> full_rows,
+                   c10::optional<torch::Tensor> full_row_indices, int64_t peer_base, int64_t out_offset, int64_t flag_offset,
+                   int64_t state_offset, int64_t error_offset, int world, int rank, int members, int out_features_full) {
     const at::cuda::OptionalCUDAGuard guard(device_of(x));
-    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
     sqllm_lutgemv_args a;
     const float *bias_p;
     fill_fused_args(a, bias_p, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices);
@@ -392,20 +390,49 @@ void lutgemv_fused_exchange(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     xc.world = world; xc.rank = rank; xc.members = members; xc.out_features_full = out_features_full;
     xc.peer_base = reinterpret_cast<const uint64_t *>(peer_base);
     xc.out_offset = (size_t)out_offset; xc.flag_offset = (size_t)flag_offset; xc.state_offset = (size_t)state_offset; xc.error_offset = (size_t)error_offset;
-    const int half = x.scalar_type() == torch::kFloat16;
-    const int rc = sqllm_lutgemv_fused_exchange(&a, x.data_ptr(), half, half, bias_p, ws.data_ptr(), (size_t)ws.numel(), &xc, cur_stream());
-    check_status(rc, "quant_cuda.lutgemv_fused_exchange");
+    const int dt = dtype_code(x, name);  // the arena vectors are in x's dtype
+    const int rc = sqllm_lutgemv_fused_exchange_dt(&a, x.data_ptr(), dt, dt, bias_p, ws.data_ptr(), (size_t)ws.numel(), &xc, cur_stream());
+    check_status(rc, (std::string("quant_cuda.") + name).c_str());
+}
+
+// fp16 or fp32 x; the vectors in x's dtype.  bf16 x: lutgemv_fused_exchange_bf16.
+void lutgemv_fused_exchange(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                            c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                            c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                            c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices,
+                            int64_t peer_base, int64_t out_offset, int64_t flag_offset, int64_t state_offset, int64_t error_offset,
+                            int world, int rank, int members, int out_features_full) {
+    TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kFloat32, "x must be fp16 or fp32");
+    exchange_call("lutgemv_fused_exchange", x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices,
+                  peer_base, out_offset, flag_offset, state_offset, error_offset, world, rank, members, out_features_full);
+}
+
+// The same for bf16 x, bf16 vectors in the arenas.  A symbol of its own, so that lutgemv_fused_exchange keeps its fp16 / fp32 contract
+// (as lutgemv_rows / lutgemv_rows_bf16).
+void lutgemv_fused_exchange_bf16(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                                 c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                                 c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                                 c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices,
+                                 int64_t peer_base, int64_t out_offset, int64_t flag_offset, int64_t state_offset, int64_t error_offset,
+                                 int world, int rank, int members, int out_features_full) {
+    TORCH_CHECK(x.scalar_type() == torch::kBFloat16, "lutgemv_fused_exchange_bf16: x must be bf16 (got ", x.scalar_type(), ")");
+    exchange_call("lutgemv_fused_exchange_bf16", x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows, full_row_indices,
+                  peer_base, out_offset, flag_offset, state_offset, error_offset, world, rank, members, out_features_full);
 }
 
 
 // ---- sequences (include/sqllm_b200.h, sqllm_sequence_*): one persistent launch for a list of dependent fused matvecs -----------
 // items: list of tuples (qweight, lookup_table, bits, bias|None, rows|None, cols|None, vals|None, full_rows|None, full_row_indices|None,
 //                        x_from, x_offset, x_ext|None, members, out_features_full)
-// exports: list of (item index, fp16 destination tensor of the item's full output length).  The caller keeps every tensor alive for the
-// life of the handle (squeezellm_b200.runtime.DecodeSequence does).  peer_base / arena: several GPUs only (0 / None otherwise).
+// exports: list of (item index, destination tensor of the item's full output length).  dtype: the activation type, torch.float16 or
+// torch.bfloat16 (sqllm_sequence_create_dt): every x_ext and every export destination has it.  The caller keeps every tensor alive for
+// the life of the handle (squeezellm_b200.runtime.DecodeSequence does).  peer_base / arena: several GPUs only (0 / None otherwise).
 int64_t sequence_create(py::list items, py::list exports, const std::string &lut_mode, int world, int rank,
-                        c10::optional<torch::Tensor> arena, int64_t peer_base) {
+                        c10::optional<torch::Tensor> arena, int64_t peer_base, at::ScalarType dtype) {
     TORCH_CHECK(lut_mode == "exact" || lut_mode == "fp16", "lut mode must be 'exact' or 'fp16'");
+    TORCH_CHECK(dtype == torch::kFloat16 || dtype == torch::kBFloat16, "sequence_create: dtype must be torch.float16 or torch.bfloat16 (got ", dtype, ")");
+    const bool bf = dtype == torch::kBFloat16;
+    const char *const tn = bf ? "bf16" : "fp16";
     const int n = (int)items.size();
     TORCH_CHECK(n > 0, "sequence_create: no items");
     std::vector<sqllm_seq_item> its(n);
@@ -431,9 +458,9 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
         if (it.x_from < 0) {
             TORCH_CHECK(!t[11].is_none(), "sequence item ", i, ": x_from = -1 needs x_ext");
             xs = t[11].cast<torch::Tensor>();
-            TORCH_CHECK(xs.scalar_type() == torch::kFloat16, "sequence item ", i, ": x_ext must be fp16");
+            TORCH_CHECK(xs.scalar_type() == dtype, "sequence item ", i, ": x_ext must be ", tn, " (the sequence's dtype; got ", xs.scalar_type(), ")");
         } else {
-            xs = torch::empty({(int64_t)K}, torch::TensorOptions().dtype(torch::kFloat16).device(qweight.device()));
+            xs = torch::empty({(int64_t)K}, torch::TensorOptions().dtype(dtype).device(qweight.device()));
         }
         const float *bias_p = nullptr;
         fill_fused_args(it.a, bias_p, xs, qweight, lut, bits, opt(3), opt(4), opt(5), opt(6), opt(7), opt(8));
@@ -449,7 +476,8 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
         py::tuple t = exports[e].cast<py::tuple>();
         ex_items[e] = t[0].cast<int>();
         torch::Tensor d = t[1].cast<torch::Tensor>();
-        TORCH_CHECK(d.is_cuda() && d.is_contiguous() && d.scalar_type() == torch::kFloat16, "export ", e, ": destination must be a contiguous fp16 CUDA tensor");
+        TORCH_CHECK(d.is_cuda() && d.is_contiguous() && d.scalar_type() == dtype, "export ", e, ": destination must be a contiguous ", tn,
+                    " CUDA tensor (the sequence's dtype; got ", d.scalar_type(), ")");
         TORCH_CHECK(ex_items[e] >= 0 && ex_items[e] < n, "export ", e, ": bad item index");
         const sqllm_seq_item &it = its[ex_items[e]];
         const int64_t len = (int64_t)(it.members > 0 ? it.members : 1) * (it.out_features_full > 0 ? it.out_features_full : it.a.out_features / std::max(1, it.members));
@@ -467,7 +495,7 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
     o.peer_base = reinterpret_cast<const uint64_t *>(peer_base);
     o.n_export = ne; o.export_items = ex_items.data(); o.export_dst = ex_dst.data();
     sqllm_sequence *h = nullptr;
-    check_status(sqllm_sequence_create(its.data(), n, &o, &h), "quant_cuda.sequence_create");
+    check_status(sqllm_sequence_create_dt(its.data(), n, &o, bf ? SQLLM_DT_BF16 : SQLLM_DT_F16, &h), "quant_cuda.sequence_create");
     return reinterpret_cast<int64_t>(h);
 }
 
@@ -609,9 +637,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("vals"), py::arg("full_rows"), py::arg("full_row_indices"), py::arg("peer_base"), py::arg("out_offset"),
           py::arg("flag_offset"), py::arg("state_offset"), py::arg("error_offset"), py::arg("world"), py::arg("rank"), py::arg("members"),
           py::arg("out_features_full"));
+    m.def("lutgemv_fused_exchange_bf16", &lutgemv_fused_exchange_bf16,
+          "lutgemv_fused_exchange for bf16 x: bf16 vectors in every rank's arena",
+          py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias"), py::arg("rows"), py::arg("cols"),
+          py::arg("vals"), py::arg("full_rows"), py::arg("full_row_indices"), py::arg("peer_base"), py::arg("out_offset"),
+          py::arg("flag_offset"), py::arg("state_offset"), py::arg("error_offset"), py::arg("world"), py::arg("rank"), py::arg("members"),
+          py::arg("out_features_full"));
     m.def("sequence_create", &sequence_create, "one persistent launch for a list of dependent fused matvecs (see squeezellm_b200.runtime.DecodeSequence)",
           py::arg("items"), py::arg("exports"), py::arg("lut_mode") = "exact", py::arg("world") = 1, py::arg("rank") = 0,
-          py::arg("arena") = py::none(), py::arg("peer_base") = 0);
+          py::arg("arena") = py::none(), py::arg("peer_base") = 0, py::arg("dtype") = torch::kFloat16);
     m.def("sequence_arena_bytes", [](py::list lens) {
               size_t off = 0;
               for (auto l : lens) off += ((size_t)l.cast<int64_t>() * 4 + 127) / 128 * 128;

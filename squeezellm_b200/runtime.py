@@ -72,21 +72,27 @@ class DecodeSequence:
     next as self-validating tagged words - no launch, no grid barrier in between.  An inference path: its results carry no
     gradient.
 
-        seq = DecodeSequence(hidden, device)                  # seq.x: static fp16 input buffer [hidden]
+        seq = DecodeSequence(hidden, device)                  # seq.x: static input buffer [hidden] (fp16, or dtype=torch.bfloat16)
         qkv = seq.matvec(stacked_qkv_layer, seq.input)        # -> SeqVec over the full output
         o   = seq.matvec(o_proj, qkv[2 * hidden:3 * hidden])
         ...
-        seq.compile(outputs=[d])                              # d: the SeqVec whose plain fp16 copy is wanted
+        seq.compile(outputs=[d])                              # d: the SeqVec whose plain copy is wanted
         y = seq.replay()[0]                                   # run on the current stream (CUDA-graph capturable)
 
     It replaces the per-layer launch loop of the reference's decode (llama.py:226-234) for the QuantLinear layers; whatever
     sits between them in a real model (attention, norms) has to run as its own launches, i.e. a model is cut into sequences
-    at those points.  Layers must be QuantLinearLUT modules of one bit width, on one device, used with fp16 activations.
+    at those points.  Layers must be QuantLinearLUT modules of one bit width, on one device.
+    `dtype` is the activation type, torch.float16 or torch.bfloat16: that of `x`, of the values handed from one matvec to the next
+    and of the outputs; every output is rounded to it once, with the bias inside the fp32 sum.  A bf16 sequence uses the exact
+    codebook whatever `lut_mode` says (the fp16 pair table multiplies fp16 by fp16), as QuantLinearLUT does for one bf16 row.
     On several GPUs pass `peer` (sharding.PeerArena): every layer is this rank's column shard."""
 
-    def __init__(self, in_features, device, lut_mode=None, peer=None):
+    def __init__(self, in_features, device, lut_mode=None, peer=None, dtype=torch.float16):
+        if dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError(f"DecodeSequence: dtype must be torch.float16 or torch.bfloat16 (got {dtype})")
         self.device = torch.device(device)
-        self.x = torch.zeros(in_features, dtype=torch.float16, device=self.device)
+        self.dtype = dtype
+        self.x = torch.zeros(in_features, dtype=dtype, device=self.device)
         self.input = SeqVec(-1, 0, in_features)
         self._items, self._lens, self._keep = [], [], []
         self._handle, self.outputs, self._out_vecs = None, [], []
@@ -116,16 +122,17 @@ class DecodeSequence:
         for v in outputs:
             assert v.item >= 0, "the input is not an output"
             if v.item not in bufs:
-                bufs[v.item] = torch.zeros(self._lens[v.item], dtype=torch.float16, device=self.device)
+                bufs[v.item] = torch.zeros(self._lens[v.item], dtype=self.dtype, device=self.device)
                 exports.append((v.item, bufs[v.item]))
         self.outputs = [bufs[v.item][v.offset:v.offset + v.length] for v in outputs]
         with torch.cuda.device(self.device):
             if self.peer is not None:
                 arena, peer_base = self.peer.arena_for(quant_cuda.sequence_arena_bytes(self._lens))
-                self._handle = quant_cuda.sequence_create(self._items, exports, mode, self.peer.world, self.peer.rank, arena, peer_base)
+                self._handle = quant_cuda.sequence_create(self._items, exports, mode, self.peer.world, self.peer.rank, arena, peer_base,
+                                                          dtype=self.dtype)
                 self._arena = arena
             else:
-                self._handle = quant_cuda.sequence_create(self._items, exports, mode)
+                self._handle = quant_cuda.sequence_create(self._items, exports, mode, dtype=self.dtype)
         self._exports = exports
         self._quant_cuda = quant_cuda
         return self

@@ -158,9 +158,10 @@ class PeerExchange:
         if self.check_every and self.calls % self.check_every == 0 and not torch.cuda.is_current_stream_capturing():
             self.check()  # surfaces a timed-out wait in the product path (costs a device synchronisation: every check_every calls only)
         rows, cols, vals, fr, fri = layer._sparse_args()
-        quant_cuda.lutgemv_fused_exchange(x.contiguous().reshape(-1), layer.qweight, layer.lookup_table, layer.bits, layer.bias,
-                                          rows, cols, vals, fr, fri, self.peer_base, off, self.FLAG, self.STATE, self.ERROR,
-                                          self.world, self.rank, members, n_full)
+        # bf16 x has a binding of its own (bf16 vectors in the arenas); fp16 / fp32 x keep theirs
+        call = quant_cuda.lutgemv_fused_exchange_bf16 if x.dtype == torch.bfloat16 else quant_cuda.lutgemv_fused_exchange
+        call(x.contiguous().reshape(-1), layer.qweight, layer.lookup_table, layer.bits, layer.bias, rows, cols, vals, fr, fri,
+             self.peer_base, off, self.FLAG, self.STATE, self.ERROR, self.world, self.rank, members, n_full)
         return view
 
     def error(self):
