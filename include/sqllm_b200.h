@@ -50,7 +50,8 @@ extern "C" {
 #define SQLLM_ABI_VERSION 4   /* 2: + sqllm_lutgemv_fused_exchange, sqllm_set_deterministic ; 3: + sqllm_set_lut_mode, sqllm_workspace_error ; 4: + sqllm_sequence_*,
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
-                                 sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt
+                                 sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
+                                 sqllm_lutgemm_fused_f32
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -176,6 +177,23 @@ int sqllm_lutgemv_rows(const sqllm_lutgemv_args *args, const void *x_half, void 
  * capturable and safe on several streams at once. */
 int sqllm_lutgemm_fused_dt(const sqllm_lutgemv_args *args, const void *x, int x_dtype, void *y, int y_dtype, const float *bias,
                            void *stream);
+
+/* sqllm_lutgemm_fused for fp32 x: the same tensor-core LUT-GEMM, y[m][c] = bias[c] + LUT-GEMM + CSR + dense rows, written (not
+ * accumulated), from fp32 x [M][in_features] (row-major) into fp32 y [M][out_features].  fp32 x is not exact in a 16-bit operand, so
+ * both sides are split exactly into three bf16 parts with the same rule: x = x_h + x_m + x_l with x_h = bf16(x),
+ * x_m = bf16(x - x_h), x_l = bf16(x - x_h - x_m), and each folded weight w (codebook + CSR + dense rows, over the column's
+ * power-of-two scale) = w_h + w_m + w_l as for bf16 x.  Per 64-k chunk the tensor cores multiply the six part pairs whose orders
+ * sum to at most 2, smallest first: x_l.w_h, x_m.w_m, x_h.w_l, then x_m.w_h, x_h.w_m, then x_h.w_h (each over the chunk's four
+ * k16 steps), into one fp32 accumulator that starts from zero and is added into the fp32 running sum once per chunk.  Every
+ * product is exact; the dropped terms x_m.w_l + x_l.w_m + x_l.w_l are below 2^-23 |x||w| per product (about 2 u, u = 2^-24), so
+ * each output is within a few u of sum_k |x_k||w_kc| of the exact result, as for fp16 and bf16 x.  Below |x| of about 2^-110
+ * (1e-33) the lower parts of x fall into bf16's subnormal range and the split keeps x only to within 2^-133 absolute.  The codebook
+ * is always used as stored: sqllm_set_lut_mode does not apply.  Every output is written once by one CTA in a fixed order: results
+ * are bit-reproducible, and a row's bits do not depend on M or on the other rows.  Any topX and any number of outliers.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_lutgemm_fused (in_features % 32 == 0,
+ * batch >= 1, non-null x and y, x and y 16-byte aligned, qweight, lookup_table and bias 4-byte aligned).  No workspace, no
+ * allocation, no host synchronisation: CUDA-graph capturable and safe on several streams at once. */
+int sqllm_lutgemm_fused_f32(const sqllm_lutgemv_args *args, const float *x, float *y, const float *bias, void *stream);
 
 /* sqllm_lutgemv_fused with the element types as codes, and bf16 x besides fp32 and fp16: the same one-vector LUT-GEMV,
  * y[c] = bias[c] + LUT-GEMV + CSR + dense rows, written (not accumulated).  Pairs (x_dtype, y_dtype):

@@ -1,5 +1,11 @@
-// lutgemm_tc.cuh - tensor-core (wgmma) LUT-GEMM for M >= 1 rows of fp16 or bf16 activations: sqllm_lutgemm_fused_dt.  Included
-// by lutgemv_kernels.cu inside its anonymous namespace.
+// lutgemm_tc.cuh - tensor-core (wgmma) LUT-GEMM for M >= 1 rows of fp16 or bf16 activations (sqllm_lutgemm_fused_dt) or fp32 ones
+// (sqllm_lutgemm_fused_f32).  Included by lutgemv_kernels.cu inside its anonymous namespace.
+//
+// fp32 x (F32X) is not exact in a 16-bit operand: it is split like the weights into three bf16 parts (split3_bf16x2), loaded into
+// registers at the start of each chunk's build (the loads fly while the weights are decoded) and stored as three x tiles of the
+// same swizzled layout; the MMAs take the six part products whose orders sum to at most 2 (x_l.w_h, x_m.w_m, x_h.w_l, x_m.w_h,
+// x_h.w_m, x_h.w_h: smallest first, 24 k16 steps per chunk, 384 products per accumulator before the promotion).  The dropped
+// x_m.w_l + x_l.w_m + x_l.w_l are below 2^-23 |x w| per product.  fp32 x always writes fp32 y.
 //
 //   y[M, N] = bias + x . W_lut + x . S_csr + x . W_dense            (one launch, every output written once, no atomics)
 //
@@ -36,10 +42,11 @@ namespace tc {
 
 constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int THREADS = 256;  // two warpgroups
-constexpr int XS = 0, XS_BYTES = BM * BK * 2;
-constexpr int B0 = XS + 2 * XS_BYTES, B_BYTES = BN * BK * 2;  // part pp of buffer b at B0 + (2 pp + b) B_BYTES
-template <int NPART>                                          // weight parts: 2 (fp16 x: hi, lo) or 3 (bf16 x: hi, mid, lo)
+constexpr int XS = 0, XS_BYTES = BM * BK * 2;  // x part q of buffer b at XS + (XPART b + q) XS_BYTES
+constexpr int B_BYTES = BN * BK * 2;
+template <int NPART, int XPART = 1>  // weight parts: 2 (fp16 x: hi, lo) or 3 (bf16 / fp32 x: hi, mid, lo); x parts: 3 for fp32 x
 struct L {
+    static constexpr int B0 = XS + 2 * XPART * XS_BYTES;    // weight part pp of buffer b at B0 + (2 pp + b) B_BYTES
     static constexpr int LUT = B0 + 2 * NPART * B_BYTES;    // fp32 [16][BN]
     static constexpr int SCALE = LUT + 16 * BN * 4;         // fp32 [BN] s_c
     static constexpr int DSUM = SCALE + BN * 4;             // fp32 [BN] sum of the column's dense-row maxima
@@ -139,12 +146,15 @@ __device__ __forceinline__ void add_at(float (&w)[32], const int kk, const float
         if (j == kk) w[j] += v;
 }
 
-template <int BITS, bool BF>  // BF: bf16 x (three weight parts), else fp16 x (two)
+// BF: bf16 x (three weight parts), else fp16 x (two).  F32X (with BF): fp32 x, split into three bf16 parts like the weights.
+template <int BITS, bool BF, bool F32X = false>
 __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
+    static_assert(BF || !F32X, "fp32 x takes the bf16 operands");
     constexpr int LV = 1 << BITS;
     constexpr int WROWS = BITS == 4 ? 4 : 3;  // packed words per (column, 32 k)
     constexpr int NPART = BF ? 3 : 2;
-    using G = L<NPART>;
+    constexpr int XPART = F32X ? 3 : 1;
+    using G = L<NPART, XPART>;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t sb = (raw + 1023u) & ~1023u;
@@ -154,7 +164,8 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
     int *dcnt_s = reinterpret_cast<int *>(sm + G::DCNT);
     int *dfirst_s = reinterpret_cast<int *>(sm + G::DFIRST);
     float *red_s = reinterpret_cast<float *>(sm + G::RED);
-    const auto bpart = [&](int pp, int b) { return sb + (uint32_t)(B0 + (2 * pp + b) * B_BYTES); };  // part pp of buffer b
+    const auto bpart = [&](int pp, int b) { return sb + (uint32_t)(G::B0 + (2 * pp + b) * B_BYTES); };  // part pp of buffer b
+    const auto xpart = [&](int q, int b) { return sb + (uint32_t)(XS + (XPART * b + q) * XS_BYTES); };  // x part q of buffer b
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int c = tid & (BN - 1), h = tid >> 7;  // decode role: tile column, k-half of the chunk
@@ -231,18 +242,31 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
         for (int r = 0; r < WROWS; ++r) wq[r] = (i < nch && kb < K && cvalid) ? __ldg(p.qw + (size_t)(r0 + r) * N + col) : 0u;
     };
 
-    // operands of chunk i into buffer b: x by cp.async, this thread's 32 weights of column c decoded, folded, split and stored
+    // operands of chunk i into buffer b: x by cp.async (fp32 x: loaded into registers here, split and stored after the weights),
+    // this thread's 32 weights of column c decoded, folded, split and stored
+    constexpr int XV = BM * BK / 4 / THREADS;  // fp32 x: float4 loads per thread and chunk
     auto stage = [&](int i, int b) {
         const int k0 = i * BK;
-        const uint32_t xs = sb + XS + b * XS_BYTES;
+        float4 xv[F32X ? XV : 1];
+        if constexpr (F32X) {  // the loads are in flight while the weights are decoded
+            const float *xf = reinterpret_cast<const float *>(p.x);
 #pragma unroll
-        for (int q = 0; q < BM * BK / 8 / THREADS; ++q) {
-            const int idx = tid + q * THREADS, r = idx >> 3, ch = idx & 7;
-            const int gr = m0 + r, gk = k0 + ch * 8;
-            const bool ok = gr < p.M && gk < K;
-            cp_async16_clip(xs + r * 128 + ((ch ^ (r & 7)) << 4), ok ? p.x + (size_t)gr * K + gk : p.x, ok ? 16 : 0);
+            for (int q = 0; q < XV; ++q) {
+                const int idx = tid + q * THREADS, r = idx >> 4, c4 = idx & 15;
+                const int gr = m0 + r, gk = k0 + 4 * c4;
+                xv[q] = gr < p.M && gk < K ? __ldg(reinterpret_cast<const float4 *>(xf + (size_t)gr * K + gk)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+        } else {
+            const uint32_t xs = sb + XS + b * XS_BYTES;
+#pragma unroll
+            for (int q = 0; q < BM * BK / 8 / THREADS; ++q) {
+                const int idx = tid + q * THREADS, r = idx >> 3, ch = idx & 7;
+                const int gr = m0 + r, gk = k0 + ch * 8;
+                const bool ok = gr < p.M && gk < K;
+                cp_async16_clip(xs + r * 128 + ((ch ^ (r & 7)) << 4), ok ? p.x + (size_t)gr * K + gk : p.x, ok ? 16 : 0);
+            }
+            cp_async_commit();
         }
-        cp_async_commit();
 
         const int kb = k0 + 32 * h;
         float w[32];  // the next chunk's words are requested before this chunk's are decoded
@@ -308,6 +332,19 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
                 asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(bpart(1, b) + off), "r"(lv[0]), "r"(lv[1]), "r"(lv[2]), "r"(lv[3]) : "memory");
             }
         }
+        if constexpr (F32X) {  // x = hi + mid + lo exactly (split3_bf16x2), part q into its own tile: k 4 c4 .. 4 c4 + 3 of row r
+#pragma unroll
+            for (int q = 0; q < XV; ++q) {
+                const int idx = tid + q * THREADS, r = idx >> 4, c4 = idx & 15;
+                uint32_t t01[3], t23[3];
+                split3_bf16x2(xv[q].x, xv[q].y, t01);
+                split3_bf16x2(xv[q].z, xv[q].w, t23);
+                const uint32_t off = r * 128 + ((((uint32_t)(c4 >> 1)) ^ (uint32_t)(r & 7)) << 4) + (c4 & 1) * 8;
+#pragma unroll
+                for (int pp = 0; pp < 3; ++pp)
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(xpart(pp, b) + off), "r"(t01[pp]), "r"(t23[pp]) : "memory");
+            }
+        }
     };
 
     load_words(0);
@@ -324,7 +361,15 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
         const int b = i & 1;
         const uint32_t xa = sb + XS + b * XS_BYTES + g * 64 * 128;
         wgmma_fence();
-        if constexpr (BF) {  // lo, mid, hi: smallest part first
+        if constexpr (F32X) {  // the six x part . w part products of part orders summing to <= 2, smallest first
+            constexpr int PX[6] = {2, 1, 0, 1, 0, 0}, PW[6] = {0, 1, 2, 0, 1, 0};  // 0 hi, 1 mid, 2 lo
+#pragma unroll
+            for (int t = 0; t < 6; ++t)
+#pragma unroll
+                for (int s = 0; s < BK / 16; ++s)
+                    wgmma_m64n128k16<true>(acc, sw128_desc(xpart(PX[t], b) + g * 64 * 128 + 32 * s), sw128_desc(bpart(PW[t], b) + 32 * s),
+                                           t > 0 || s > 0);
+        } else if constexpr (BF) {  // lo, mid, hi: smallest part first
 #pragma unroll
             for (int pp = NPART - 1; pp >= 0; --pp)
 #pragma unroll
@@ -363,7 +408,7 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
             float v0 = sum[4 * n + 2 * i] * scale_s[cl], v1 = sum[4 * n + 2 * i + 1] * scale_s[cl + 1];
             if (p.bias) { v0 += __ldg(p.bias + gc); if (gc + 1 < N) v1 += __ldg(p.bias + gc + 1); }
             const size_t o = (size_t)row * N + gc;
-            if (p.y_16) {
+            if (!F32X && p.y_16) {
                 if constexpr (BF) {
                     __nv_bfloat16 *y = reinterpret_cast<__nv_bfloat16 *>(p.y);
                     if (gc + 1 < N && !(N & 1)) *reinterpret_cast<__nv_bfloat162 *>(y + o) = __floats2bfloat162_rn(v0, v1);

@@ -242,7 +242,7 @@ int path_code(const std::string &path, const char *name) {
 }
 
 // The bindings x [M, in] -> y [M, out] in x's dtype: the shape checks, y and the call of `entry` (sqllm_lutgemm_fused_dt or
-// sqllm_lutgemv_rows_dt).  The binding `name` has checked x's dtype.
+// sqllm_lutgemv_rows_dt, or sqllm_lutgemm_fused_f32 through lutgemm_f32_entry).  The binding `name` has checked x's dtype.
 typedef int (*RowsEntry)(const sqllm_lutgemv_args *, const void *, int, void *, int, const float *, void *);
 torch::Tensor layer_rows(const char *name, RowsEntry entry, const torch::Tensor &x, const torch::Tensor &qweight,
                          const torch::Tensor &lookup_table, int bits, const c10::optional<torch::Tensor> &bias,
@@ -272,6 +272,23 @@ torch::Tensor lutgemm_fused(torch::Tensor x, torch::Tensor qweight, torch::Tenso
     TORCH_CHECK(x.scalar_type() == torch::kFloat16 || x.scalar_type() == torch::kBFloat16,
                 "lutgemm_fused: x must be fp16 or bf16 (got ", x.scalar_type(), ")");
     return layer_rows("lutgemm_fused", sqllm_lutgemm_fused_dt, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows,
+                      full_row_indices);
+}
+
+// sqllm_lutgemm_fused_f32 behind layer_rows' entry signature (the dtype codes are SQLLM_DT_F32: lutgemm_fused_f32 checked x)
+int lutgemm_f32_entry(const sqllm_lutgemv_args *a, const void *x, int, void *y, int, const float *bias, void *stream) {
+    return sqllm_lutgemm_fused_f32(a, static_cast<const float *>(x), static_cast<float *>(y), bias, stream);
+}
+
+// The same for fp32 x [M, in] -> fp32 y [M, out] (sqllm_lutgemm_fused_f32: x split exactly into three bf16 parts, six part
+// products per k-step): QuantLinearLUT.forward's batched branch for QuantLinearLUT.FP32_TC_MIN_ROWS or more fp32 rows.  A symbol
+// of its own, so that lutgemm_fused keeps meaning "16-bit x".
+torch::Tensor lutgemm_fused_f32(torch::Tensor x, torch::Tensor qweight, torch::Tensor lookup_table, int bits,
+                                c10::optional<torch::Tensor> bias, c10::optional<torch::Tensor> rows,
+                                c10::optional<torch::Tensor> cols, c10::optional<torch::Tensor> vals,
+                                c10::optional<torch::Tensor> full_rows, c10::optional<torch::Tensor> full_row_indices) {
+    TORCH_CHECK(x.scalar_type() == torch::kFloat32, "lutgemm_fused_f32: x must be fp32 (got ", x.scalar_type(), ")");
+    return layer_rows("lutgemm_fused_f32", lutgemm_f32_entry, x, qweight, lookup_table, bits, bias, rows, cols, vals, full_rows,
                       full_row_indices);
 }
 
@@ -610,6 +627,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
     m.def("lutgemm_fused", &lutgemm_fused, "fused QuantLinearLUT matmul on the tensor cores: fp16 or bf16 x [M, in] -> y [M, out] in x's dtype (bias, CSR, dense rows), one launch",
+          py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
+          py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
+          py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());
+    m.def("lutgemm_fused_f32", &lutgemm_fused_f32, "lutgemm_fused for fp32 x [M, in] -> fp32 y [M, out] (x split into three bf16 parts; bias, CSR, dense rows), one launch",
           py::arg("x"), py::arg("qweight"), py::arg("lookup_table"), py::arg("bits"), py::arg("bias") = py::none(),
           py::arg("rows") = py::none(), py::arg("cols") = py::none(), py::arg("vals") = py::none(),
           py::arg("full_rows") = py::none(), py::arg("full_row_indices") = py::none());

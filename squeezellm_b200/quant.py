@@ -14,12 +14,13 @@ as the reference, so `llama.py`-style loaders work unchanged.  Differences, all 
   * `forward` with fp16 x of at least `TC_MIN_ROWS` rows, or bf16 x of at least `BF16_TC_MIN_ROWS` rows (prefill, evaluation,
     bf16 training; reference quant.py:314-379) uses ONE tensor-core launch (`quant_cuda.lutgemm_fused`, outliers and dense rows
     folded into the weight tiles, output in x's dtype, bit-reproducible) instead of zeros + x.float() + 1-3 batched launches +
-    out.to(dtype).
+    out.to(dtype).  fp32 x of at least `FP32_TC_MIN_ROWS` rows runs the same kernel with x split exactly into three bf16 parts
+    (`quant_cuda.lutgemm_fused_f32`, fp32 output).
   * `forward` with fp16 x of 2 to `ROWS_MAX` rows (and fewer than `TC_MIN_ROWS`; several sequences decoding at once, speculative-
     decoding verification, short prompts) uses ONE CUDA-core launch (`quant_cuda.lutgemv_rows`: a multi-row LUT-GEMV whose
     thread-block clusters split K, outliers and dense rows folded per K-slab) instead of the same sequence; bf16 x of 2 to
-    `BF16_ROWS_MAX` rows the same kernel with bf16 in and out (`quant_cuda.lutgemv_rows_bf16`).  fp32 x and `use_fused = False`
-    keep the reference's batched symbols.
+    `BF16_ROWS_MAX` rows the same kernel with bf16 in and out (`quant_cuda.lutgemv_rows_bf16`).  fp32 x of fewer than
+    `FP32_TC_MIN_ROWS` rows and `use_fused = False` keep the reference's batched symbols.
   * `loss.backward()` works through the layer when x requires grad (the reference has no backward: its outputs carry no
     graph).  x gets dx = dy . W^T from ONE launch (`quant_cuda.lutgemm_t`: a transposed LUT-GEMM, on the tensor cores for fp16 /
     bf16 gradients of at least `BWD_TC_MIN_ROWS` rows, else on the CUDA cores; outliers and dense rows included); the buffers are constants and get no gradient.  The forward of such a call takes the same route
@@ -128,6 +129,11 @@ class QuantLinearLUT(nn.Module):
     # multi-row GEMV (BF16_ROWS_MAX).  80: the smallest measured row count above TC_MIN_ROWS at which a whole 7B decoder layer is faster on an
     # H100 (DESIGN.md section 3.6: 80 rows 1.48 vs 1.90 ms; the tensor cores already win at 64 rows, 1.46 vs 1.56 ms).
     BF16_TC_MIN_ROWS = 80
+    # fp32 inputs of at least this many rows run the same tensor-core LUT-GEMM with x split into three bf16 parts as well
+    # (quant_cuda.lutgemm_fused_f32, six part products per k-step); fewer rows and use_fused = False run the batched symbols.
+    # 128: the smallest measured row count from which a whole 7B decoder layer is faster on an H100 (DESIGN.md section 3.6: 96 rows
+    # 2.35 vs 2.20 ms, 128 rows 2.35 vs 2.91 ms); the kernel costs about the same up to 128 rows, the batched symbols grow per row.
+    FP32_TC_MIN_ROWS = 128
     # fp16 inputs of 2 to ROWS_MAX rows (below TC_MIN_ROWS) run the multi-row GEMV (quant_cuda.lutgemv_rows).  63: it is faster than
     # the batched symbols on a whole 7B decoder layer at every measured row count up to 63 on an H100 (DESIGN.md section 3.9).
     ROWS_MAX = 63
@@ -330,11 +336,12 @@ class QuantLinearLUT(nn.Module):
             return y.to(dtype).reshape(outshape)
         out_shape = x.shape[:-1] + (self.outfeatures,)
         x = x.reshape(-1, x.shape[-1])
-        tc_min = {torch.float16: QuantLinearLUT.TC_MIN_ROWS, torch.bfloat16: QuantLinearLUT.BF16_TC_MIN_ROWS}.get(x.dtype)
+        tc_min = {torch.float16: QuantLinearLUT.TC_MIN_ROWS, torch.bfloat16: QuantLinearLUT.BF16_TC_MIN_ROWS,
+                  torch.float32: QuantLinearLUT.FP32_TC_MIN_ROWS}.get(x.dtype)
         if QuantLinearLUT.use_fused and tc_min is not None and x.shape[0] >= tc_min:
             rows, cols, vals, fr, fri = self._sparse_args()
-            out = quant_cuda.lutgemm_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
-                                           None, rows, cols, vals, fr, fri).reshape(out_shape)
+            tc_fn = quant_cuda.lutgemm_fused_f32 if x.dtype == torch.float32 else quant_cuda.lutgemm_fused
+            out = tc_fn(_aligned(x), self.qweight, self.lookup_table, self.bits, None, rows, cols, vals, fr, fri).reshape(out_shape)
             return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
         rows_max = {torch.float16: QuantLinearLUT.ROWS_MAX, torch.bfloat16: QuantLinearLUT.BF16_ROWS_MAX}.get(x.dtype)
         if QuantLinearLUT.use_fused and rows_max is not None and 2 <= x.shape[0] <= rows_max and self._rows_fits():
