@@ -210,7 +210,10 @@ __global__ void csr_batched_kernel(const int *__restrict__ rows, const int *__re
     for (int b = blockIdx.y * blockDim.x + threadIdx.x; b < B; b += gridDim.y * blockDim.x) {
         const float *xb = x + (size_t)b * K;
         float a = 0.f;
-        for (int e = e0; e < e1; ++e) a += __ldg(vals + e) * __ldg(xb + __ldg(cols + e));  // storage order, like the oracle
+        for (int e = e0; e < e1; ++e) {  // storage order, like the oracle
+            const int k = __ldg(cols + e);
+            if ((unsigned)k < (unsigned)K) a += __ldg(vals + e) * __ldg(xb + k);  // columns outside [0, K) are ignored, as on the fused routes
+        }
         if (e1 > e0) atomicAdd(mul + (size_t)b * N + row, a);
     }
 }

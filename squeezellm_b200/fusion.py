@@ -123,6 +123,10 @@ class SiblingGroup:
             self.launches += 1
         self._pending.discard(i)
         y = self._y[..., self.offsets[i]:self.offsets[i + 1]]
+        if y.dtype != x.dtype and self.members[i].bias is None:
+            # another member's bias promoted the stacked batch result to fp32 (out.to(dtype) + fp32 bias); this member has none, so
+            # its slice is its x-dtype output + 0.0: casting back is exact and gives the dtype and bits it returns alone
+            y = y.to(x.dtype)
         if not self._pending:
             self._x = self._y = None
         return y

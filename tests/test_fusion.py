@@ -7,7 +7,7 @@ import torch
 
 from squeezellm_b200.quant import QuantLinearLUT
 from squeezellm_b200 import fusion
-from util import orc, rel_err, REL_TOL
+from util import OUT_ROUNDING, abs_sum, bound_ratio, make_activations, orc
 
 
 def _member(L, bias=False):
@@ -104,17 +104,40 @@ def test_fuse_siblings_walks_llama_like_modules():
     assert fusion.fuse_siblings(model) == [], "idempotent"
 
 
+def _truth(L, x, bias_inside):
+    """want, S and the rounded quantity of layer L on x [M, K] (numpy, the exact values the layer saw), with L's bias if it has one:
+    inside the rounded sum for a one-row call, added after the rounding otherwise (tests/util.py, bound_ratio)."""
+    b = L.get("bias")
+    want, S = orc.forward_f64(L, x), abs_sum(L, x)
+    if b is None:
+        return want, S, want
+    b = b.astype(np.float64)[None, :]
+    return want + b, S + np.abs(b), (want + b if bias_inside else want)
+
+
+def _bound(y, L, x, y_dtype):
+    M = x.shape[0]
+    want, S, rounded = _truth(L, x, bias_inside=M == 1)
+    r, eta = OUT_ROUNDING[str(y_dtype).split(".")[1]]
+    return bound_ratio(y.float().cpu().numpy().reshape(M, -1), want, S, rounded, r, eta=eta)
+
+
+GPU_GROUPS = [(4, 4096, [4096, 4096, 4096], 0.0045, 10), (3, 4096, [11008, 11008], 0.0045, 10), (4, 512, [128, 256], 0.0, 0),
+              # the middle member has no dense rows: 2 x topX stacked
+              (4, 1024, [1024, 1024, 1024], 0.01, 16),   # 32: the topX <= 32 branch at its edge
+              (3, 1024, [1024, 1024, 1024], 0.01, 17),   # 34: the general branch
+              (4, 1024, [1024, 1024, 1024], 0.01, 70)]   # 140: more than the fused launch takes
+GPU_IDS = ["w4-qkv", "w3-gateup", "w4-small-dense", "w4-qkv-t16", "w3-qkv-t17", "w4-qkv-t70"]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("bits,K,widths,sp,topx", [(4, 4096, [4096, 4096, 4096], 0.0045, 10), (3, 4096, [11008, 11008], 0.0045, 10),
-                                                   (4, 512, [128, 256], 0.0, 0),
-                                                   # the middle member has no dense rows: 2 x topX stacked
-                                                   (4, 1024, [1024, 1024, 1024], 0.01, 16),   # 32: the topX <= 32 branch at its edge
-                                                   (3, 1024, [1024, 1024, 1024], 0.01, 17),   # 34: the general branch
-                                                   (4, 1024, [1024, 1024, 1024], 0.01, 70)],  # 140: more than the fused launch takes
-                         ids=["w4-qkv", "w3-gateup", "w4-small-dense", "w4-qkv-t16", "w3-qkv-t17", "w4-qkv-t70"])
-def test_stacked_launch_matches_members(bits, K, widths, sp, topx):
-    Ls = _layers(bits, K, widths, sp, topx)
-    ms = [_member(L).cuda() for L in Ls]
+@pytest.mark.parametrize("bits,K,widths,sp,topx,bias", [g + (False,) for g in GPU_GROUPS] + [g + (True,) for g in GPU_GROUPS],
+                         ids=GPU_IDS + [i + "-bias" for i in GPU_IDS])
+def test_stacked_launch_matches_members(bits, K, widths, sp, topx, bias):
+    """One row (the fused decode launch, bias inside the sum) and two rows (the multi-row launch, bias added after the rounding):
+    every member's slice of the stacked launch against the fp64 oracle per element (bound_ratio), and next to its own launch."""
+    Ls = _layers(bits, K, widths, sp, topx, bias=bias)
+    ms = [_member(L, bias=bias).cuda() for L in Ls]
     x = torch.from_numpy(orc.make_vec(K, seed=12)).cuda().half().reshape(1, 1, K)
     alone = [m(x) for m in ms]
     g = fusion.SiblingGroup(ms)
@@ -123,13 +146,52 @@ def test_stacked_launch_matches_members(bits, K, widths, sp, topx):
     assert g.launches == 1
     for L, m, a, t in zip(Ls, ms, alone, together):
         assert t.shape == (1, 1, L["outfeatures"]) and t.dtype == torch.float16
-        want = orc.forward_f64(L, x.float().cpu().numpy().reshape(1, K))
-        assert rel_err(t.float().cpu().numpy(), want) < REL_TOL
-        assert rel_err(t.float().cpu().numpy(), a.float().cpu().numpy()) < REL_TOL
+        x_np = x.float().cpu().numpy().reshape(1, K)
+        assert _bound(t, L, x_np, t.dtype) <= 1.0
+        assert _bound(a, L, x_np, a.dtype) <= 1.0
         assert not m.qweight.is_contiguous() or len(widths) == 1  # a view of the stacked matrix, not a copy
-    # prefill-shaped input goes through the stacked layer's batched symbols
     xb = torch.from_numpy(orc.make_vec(K, batch=2, seed=13)).cuda().half().reshape(1, 2, K)
     yb = [m(xb) for m in ms]
+    assert g.launches == 2
     for L, y in zip(Ls, yb):
-        want = orc.forward_f64(L, xb.float().cpu().numpy().reshape(2, K))
-        assert rel_err(y.float().cpu().numpy().reshape(2, -1), want) < REL_TOL
+        assert y.shape == (1, 2, L["outfeatures"]) and y.dtype == (torch.float32 if bias else torch.float16)
+        assert _bound(y, L, xb.float().cpu().numpy().reshape(2, K), torch.float16) <= 1.0
+
+
+MIXED_BIAS_CASES = [(torch.float16, M) for M in (1, 5, 64)] + [(torch.bfloat16, M) for M in (1, 5, 80)] + \
+                   [(torch.float32, M) for M in (1, 128)]
+
+
+@pytest.fixture(scope="module")
+def mixed_bias_layers():
+    """q / k / v at GQA widths (1024 / 256 / 256 over 1024 inputs) with outliers and dense rows; q and v have a bias, k has none
+    (Whisper's attention)."""
+    return [orc.make_layer(4, 1024, n, sparsity=0.0045, topX=10, seed=71 + i, nonzero_full_rows=True, bias=i != 1)
+            for i, n in enumerate((1024, 256, 256))]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("dtype,M", MIXED_BIAS_CASES, ids=[f"{str(d).split('.')[1]}-M{m}" for d, m in MIXED_BIAS_CASES])
+def test_member_without_bias_keeps_its_dtype_in_a_group_with_biases(mixed_bias_layers, dtype, M):
+    """A batch through a stacked layer that has a bias comes back as out.to(dtype) + fp32 bias, i.e. fp32.  The member without a
+    bias returns what it returns alone: x's dtype (HF's attention rejects q / k / v of mixed dtypes), the same shape, and values
+    within the bound; on the launches whose bits do not depend on the call (the multi-row and the tensor-core LUT-GEMM) the same
+    bits as alone."""
+    Ls = mixed_bias_layers
+    alone = [_member(L, bias=L["bias"] is not None).cuda() for L in Ls]
+    ms = [_member(L, bias=L["bias"] is not None).cuda() for L in Ls]
+    g = fusion.SiblingGroup(ms)
+    x = torch.from_numpy(make_activations(1024, M, seed=M)).cuda().to(dtype).reshape(1, M, 1024)
+    x_np = x.float().cpu().numpy().reshape(M, 1024)
+    want_alone = [a(x) for a in alone]
+    got = [m(x) for m in ms]
+    torch.cuda.synchronize()
+    assert g.launches == 1
+    reproducible = M > 1 and (dtype != torch.float32 or M >= QuantLinearLUT.FP32_TC_MIN_ROWS)
+    for L, a, y in zip(Ls, want_alone, got):
+        assert y.dtype == a.dtype and y.shape == a.shape == (1, M, L["outfeatures"]), (y.dtype, a.dtype, y.shape)
+        assert _bound(y, L, x_np, dtype) <= 1.0
+        if reproducible:
+            assert torch.equal(y, a)
+    assert got[1].dtype == dtype
+    assert got[0].dtype == (dtype if M == 1 else torch.float32)

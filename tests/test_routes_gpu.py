@@ -2,9 +2,15 @@
 (bound_ratio) next to the old rel_err, on prefill-like activations (util.make_activations: rows from 1e-3 to 1e2, massive channels,
 an all-zero row, a one-entry row).
 
-Routes (QuantLinearLUT.forward):  1 row, fp16 / fp32 x -> "gemv_fused" (lutgemv_fused, bias inside the sum);  1 row bf16 x or
-use_fused = False -> "symbols_1row" (the reference's 12 symbols onto a copy of the bias);  fp16 x of TC_MIN_ROWS rows or more ->
-"tc" (lutgemm_fused, fp16 out, bias added afterwards);  everything else -> "batched" (the _batched symbols, out.to(dtype) + bias).
+Routes (QuantLinearLUT.forward; the quant_cuda binding each call reaches, as a spy on the extension records it):
+  * 1 row, fp16 / bf16 / fp32 x -> "lutgemv_fused" (bias inside the sum);  1 row with use_fused = False -> "symbols" (the
+    reference's 1-row symbols onto a copy of the bias).
+  * fp16 x of 2 to ROWS_MAX (63) rows -> "lutgemv_rows";  TC_MIN_ROWS (64) rows or more -> "lutgemm_fused".
+  * bf16 x of 2 to BF16_ROWS_MAX (79) rows -> "lutgemv_rows_bf16";  BF16_TC_MIN_ROWS (80) rows or more -> "lutgemm_fused".
+  * fp32 x of 2 to FP32_TC_MIN_ROWS - 1 (127) rows -> "symbols_batched" (the _batched symbols);  128 rows or more ->
+    "lutgemm_fused_f32".
+  * 2 rows or more with use_fused = False -> "symbols_batched".
+Every route but the 1-row ones rounds the sum to x's dtype and adds the bias afterwards (out.to(dtype) + bias).
 Also: the output dtype and shape the reference's quant.py gives, the input left unchanged, the same rows through every route,
 bitwise row independence of the tensor-core kernel, three streams and a graph replay at once, and inputs that are not 16-byte
 aligned."""
@@ -14,7 +20,7 @@ import torch
 
 from test_error_bound_host import SHAPES
 from test_prefill_tc_gpu import abi_call
-from util import OUT_ROUNDING, REL_TOL, TIGHT_TOL, abs_sum, bound_ratio, load_lib, make_activations, orc, rel_err, to_torch
+from util import OUT_ROUNDING, REL_TOL, abs_layer, TIGHT_TOL, abs_sum, bound_ratio, load_lib, make_activations, orc, rel_err, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -36,9 +42,49 @@ def record(request):
 
 
 def route(M, dtype, fused):
+    """The route the table above names for M rows of x in `dtype` (every layer here fits the fused launches).  The row counts are
+    the table's, not QuantLinearLUT's thresholds: a changed threshold fails here until the table, and the cases it picks, follow."""
     if M == 1:
-        return "gemv_fused" if fused and dtype != "bf16" else "symbols_1row"
-    return "tc" if fused and dtype == "fp16" and M >= 64 else "batched"
+        return "lutgemv_fused" if fused else "symbols"
+    if not fused:
+        return "symbols_batched"
+    if M >= {"fp16": 64, "bf16": 80, "fp32": 128}[dtype]:
+        return "lutgemm_fused_f32" if dtype == "fp32" else "lutgemm_fused"
+    if M <= {"fp16": 63, "bf16": 79}.get(dtype, 0):
+        return "lutgemv_rows" if dtype == "fp16" else "lutgemv_rows_bf16"
+    return "symbols_batched"
+
+
+# routes whose results are the same bits on every call, whatever the alignment of x: no atomics
+REPRODUCIBLE = {"lutgemv_rows", "lutgemv_rows_bf16", "lutgemm_fused", "lutgemm_fused_f32"}
+
+
+def binding_route(name):
+    """The route a quant_cuda binding name belongs to."""
+    if name.startswith("vecquant"):
+        return "symbols_batched" if name.endswith("_batched") else "symbols"
+    return name
+
+
+@pytest.fixture
+def spy(monkeypatch):
+    """The quant_cuda forward bindings QuantLinearLUT.forward calls, in order (a list of names; clear it between calls)."""
+    from squeezellm_b200 import quant
+    calls = []
+    for n in dir(quant.quant_cuda):
+        if n.startswith(("lutgemv", "lutgemm", "vecquant")):
+            real = getattr(quant.quant_cuda, n)
+            monkeypatch.setattr(quant.quant_cuda, n, (lambda real, n: lambda *a, **kw: (calls.append(n), real(*a, **kw))[1])(real, n))
+    return calls
+
+
+def taken(spy, M, dtype, fused):
+    """The one route the last call reached; it must be the one the table names."""
+    assert len(spy) == 1, spy
+    rt = binding_route(spy[0])
+    assert rt == route(M, dtype, fused), (spy[0], M, dtype, fused)
+    del spy[:]
+    return rt
 
 
 def _cases():
@@ -48,7 +94,7 @@ def _cases():
             ms = SMALL_M + (LARGE_M if (K, N, bits) in LARGE_SHAPES and dtype != "bf16" else [])
             for M in ms:
                 for fused in (True, False):
-                    if not fused and route(M, dtype, False) == route(M, dtype, True):
+                    if not fused and route(M, dtype, True) == "symbols_batched":  # the unfused branch takes the same route
                         continue
                     for bias in (True, False):
                         out.append(pytest.param((K, N, bits), M, dtype, bias, fused,
@@ -122,7 +168,7 @@ def run_module(m, x, fused):
 
 def check(got, D, dtype, rows, bias, rt, record=None):
     """The bound and the old metric on got [len(rows), N] (numpy) computed by route rt from x of dtype."""
-    want, S, rounded = expected(D, dtype, rows, bias, bias_inside=rt in ("gemv_fused", "symbols_1row"))
+    want, S, rounded = expected(D, dtype, rows, bias, bias_inside=rt in ("lutgemv_fused", "symbols"))
     r, eta = OUT_ROUNDING[str(DTYPES[dtype]).split(".")[1]]
     ratio = bound_ratio(got, want, S, rounded, r, eta=eta)
     if record is not None:
@@ -135,13 +181,13 @@ def check(got, D, dtype, rows, bias, rt, record=None):
 
 
 @pytest.mark.parametrize("shape,M,dtype,bias,fused", _cases())
-def test_route_vs_oracle(record, shape, M, dtype, bias, fused):
+def test_route_vs_oracle(record, spy, shape, M, dtype, bias, fused):
     D = layer_data(shape)
     K, N, _ = shape
-    rt = route(M, dtype, fused)
     xt = torch.from_numpy(D.x[:M]).cuda().to(DTYPES[dtype]).reshape(1, M, K)
     x_before = xt.clone()
     y = run_module(D.modules[bias], xt, fused)
+    rt = taken(spy, M, dtype, fused)
     assert torch.equal(xt, x_before), "forward modified its input"
     # quant.py: a 1-row input comes back in its own dtype (y.to(dtype)); a batch as out.to(dtype) + bias
     want_dtype = xt.dtype if M == 1 or not bias else torch.result_type(torch.empty(0, dtype=xt.dtype), D.bias)
@@ -156,20 +202,24 @@ def test_route_vs_oracle(record, shape, M, dtype, bias, fused):
 
 # ---- the same rows through every route ----------------------------------------------------------------------------------------
 @pytest.mark.parametrize("shape", [SHAPES[1], SHAPES[9]], ids=["w3_4096x4096", "w4_512x132"])
-def test_same_rows_through_every_route(record, shape):
+def test_same_rows_through_every_route(record, spy, shape):
     D = layer_data(shape)
     K, N, _ = shape
     M, one = 64, list(range(8))  # 64 rows as a batch; the first 8 (1e-3, 1e2, zero, one-entry rows among them) one at a time
     m = D.modules[True]
     x16 = torch.from_numpy(D.x[:M]).cuda().half()
     ratios = {}
-    for rt, fused, xin in (("tc", True, x16), ("batched", False, x16), ("batched", True, x16.float())):
+    for fused, xin in ((True, x16), (False, x16), (True, x16.float())):
         dtype = "fp16" if xin.dtype == torch.float16 else "fp32"
         got = run_module(m, xin, fused).float().cpu().numpy()
+        rt = taken(spy, M, dtype, fused)
         ratios[f"{rt}-{dtype}"] = check(got, D, dtype, list(range(M)), True, rt)
-    for rt, fused in (("gemv_fused", True), ("symbols_1row", False)):
-        got = np.stack([run_module(m, x16[i], fused).float().cpu().numpy() for i in one])
-        ratios[rt] = check(got, D, "fp16", one, True, rt)
+    for fused in (True, False):
+        got = []
+        for i in one:
+            got.append(run_module(m, x16[i], fused).float().cpu().numpy())
+            rt = taken(spy, 1, "fp16", fused)
+        ratios[rt] = check(np.stack(got), D, "fp16", one, True, rt)
     record("bound_ratios", ratios)
 
 
@@ -281,13 +331,14 @@ def test_three_streams_and_a_graph_replay_at_once(record):
 
 
 # ---- x that is not 16-byte aligned -----------------------------------------------------------------------------------------------
-MISALIGNED = [("fp16", M, off) for M in (1, 5, 64) for off in range(1, 8)] + [("fp32", M, off) for M in (1, 5, 64) for off in range(1, 4)]
+MISALIGNED = [("fp16", M, off) for M in (1, 5, 64) for off in range(1, 8)] + [("fp32", M, off) for M in (1, 5, 64) for off in range(1, 4)] + \
+             [("bf16", M, off) for M in (1, 5, 80) for off in range(1, 8)] + [("fp32", 128, off) for off in range(1, 4)]
 
 
 @pytest.mark.parametrize("dtype,M,offset", MISALIGNED, ids=[f"{d}-M{m}-off{o}" for d, m, o in MISALIGNED])
-def test_misaligned_x(record, dtype, M, offset):
+def test_misaligned_x(record, spy, dtype, M, offset):
     """A contiguous view that starts `offset` elements into its storage computes what the aligned input computes: bit-identical
-    on the tensor cores (fixed order), within the bound elsewhere (their cross-CTA sums use atomics)."""
+    on the routes without atomics (REPRODUCIBLE), within the bound elsewhere (their cross-CTA sums use atomics)."""
     shape = SHAPES[1]
     D = layer_data(shape)
     K, N, _ = shape
@@ -299,8 +350,39 @@ def test_misaligned_x(record, dtype, M, offset):
     assert xv.is_contiguous() and xv.data_ptr() % 16
     y = run_module(m, xv, True)
     assert torch.equal(xv, xa.reshape(1, M, K))
-    rt = route(M, dtype, True)
-    if rt == "tc":
+    rt = taken(spy, M, dtype, True)
+    if rt in REPRODUCIBLE:
         assert torch.equal(y, run_module(m, xa.reshape(1, M, K), True))
     got = y.reshape(M, N).float().cpu().numpy()
     check(got, D, dtype, list(range(M)), True, rt, record)
+
+
+# ---- CSR columns outside [0, in_features) ------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("dtype,fused", [("fp32", True), ("fp16", False)], ids=["fp32-fused", "fp16-unfused"])
+def test_out_of_range_csr_columns_are_ignored_on_the_batched_route(spy, dtype, fused):
+    """The _batched symbols skip CSR entries whose column lies outside [0, in_features), as every fused route does: x sits at the
+    start of a NaN-filled buffer, so a gather past its end would turn the output NaN (or fault at the end of an allocation)."""
+    from backward_ref import dense_w_f64
+    from squeezellm_b200.quant import QuantLinearLUT
+    K, N, M = 1024, 512, 5
+    L = orc.make_layer(4, K, N, sparsity=0.01, topX=10, seed=77, nonzero_full_rows=True)
+    L["cols"] = L["cols"].copy()
+    L["cols"][0], L["cols"][-1] = K + 9, -3
+    T = to_torch(L)
+    m = QuantLinearLUT(4, K, N, False, include_sparse=True, numvals=len(L["vals"]), topX=10)
+    for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices"):
+        setattr(m, k, T[k])
+    x = torch.from_numpy(make_activations(K, M, seed=78)).cuda()
+    buf = torch.full((M * K + 4 * K,), float("nan"), device="cuda")
+    xt = buf[:M * K].view(M, K)
+    xt.copy_(x)
+    if dtype == "fp16":
+        buf = buf.half()
+        xt = buf[:M * K].view(M, K)
+    y = run_module(m, xt, fused)
+    taken(spy, M, dtype, fused)
+    W = dense_w_f64(L)  # ignores the out-of-range entries
+    x64 = xt.double().cpu().numpy()
+    r, eta = OUT_ROUNDING[str(DTYPES[dtype]).split(".")[1]]
+    ratio = bound_ratio(y.float().cpu().numpy(), x64 @ W, np.abs(x64) @ np.abs(dense_w_f64(abs_layer(L))), None, r, eta=eta)
+    assert ratio <= 1.0, ratio
