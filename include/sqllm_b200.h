@@ -51,7 +51,7 @@ extern "C" {
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
-                                 sqllm_lutgemm_fused_f32
+                                 sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -447,6 +447,36 @@ int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, const sqllm_
  * table whatever opt->lut_mode says (the pair table multiplies fp16 by fp16).  Any other code: SQLLM_EINVAL (the message names
  * it), checked before any device access like the other arguments. */
 int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, int dtype, sqllm_sequence **out);
+
+/* What a decoder layer puts between two matvecs, inside the same launch: per item, a transform of its input and a residual added to
+ * its output.  Every op rounds to the sequence's dtype once:
+ *   SQLLM_SEQ_X_RMSNORM   x'_k = round(w_k (x_k r)), r = 1 / sqrt(S / K + eps), S = sum x_k^2 in fp32 in one fixed order (every CTA
+ *                         computes the same bits); w = norm_weight [in_features] of the sequence's dtype.  (HF's RMSNorm rounds x r to
+ *                         the dtype before multiplying by w: one rounding more.)
+ *   SQLLM_SEQ_X_SILU_MUL  x'_k = round(silu(g_k) u_k), silu(g) = g / (1 + exp(-g)) in fp32; g = the item's input (x_from, x_offset),
+ *                         u = in_features elements of item x2_from's output from x2_offset (an earlier item, possibly the same as x_from)
+ *   residual              y = round(sum + bias + r): r = element res_offset + e of item res_from's full-length output (res_from earlier
+ *                         than the item; e = the element of the item's own full-length output), or element e of res_ext, a plain vector
+ *                         of the item's full length; res_from = -1 and res_ext = NULL: none.
+ * On several GPUs every vector involved is full length, as the items' outputs are. */
+#define SQLLM_SEQ_X_PLAIN 0
+#define SQLLM_SEQ_X_RMSNORM 1
+#define SQLLM_SEQ_X_SILU_MUL 2
+typedef struct sqllm_seq_op {
+    int x_op;                /* SQLLM_SEQ_X_* */
+    const void *norm_weight; /* RMSNorm: [in_features] of the sequence's dtype, 16-byte aligned */
+    float eps;               /* RMSNorm: finite, >= 0 */
+    int x2_from, x2_offset;  /* SiLU gating: the up slice (earlier item, offset a multiple of 4) */
+    int res_from, res_offset; /* residual: earlier item and first element (a multiple of 4), or -1 */
+    const void *res_ext;     /* residual: external vector (16-byte aligned), or NULL */
+} sqllm_seq_op;
+
+/* sqllm_sequence_create_dt with one op per item (ops[i] for items[i]); ops == NULL: exactly sqllm_sequence_create_dt, and so is a
+ * list of ops that do nothing (x_op plain, res_from -1, res_ext NULL).  Bad ops (unknown x_op; null or misaligned norm_weight; eps not
+ * finite or < 0; an x2 slice out of range; a residual source not earlier or too short; misaligned res_ext) give SQLLM_EINVAL with a
+ * message naming the item, before any device access. */
+int sqllm_sequence_create_ops(const sqllm_seq_item *items, const sqllm_seq_op *ops, int n_items, const sqllm_seq_options *opt, int dtype,
+                              sqllm_sequence **out);
 /* two launches on `stream` (token counter, then the persistent kernel); CUDA-graph capturable */
 int sqllm_sequence_run(sqllm_sequence *s, void *stream);
 /* synchronises `stream`; 1 if a bounded in-kernel wait ever gave up (results incomplete), 0 if not, < 0 on error */

@@ -43,6 +43,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <initializer_list>
 #include <mutex>
 #include <type_traits>
@@ -1411,6 +1412,21 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
 typedef void (*KSeq)(const seq::SeqCfg);
 struct KSeqInfo { KSeq fn; int tab, stage, ntb; };
 // bf16 x always takes the exact table (the pair table multiplies fp16 by fp16), whatever `mode` says
+// ops: the instance that also runs the items' RMSNorm / SiLU gating / residual (sqllm_sequence_create_ops with at least one op)
+KSeqInfo kseq_lookup_ops(int bits, int mode, bool multi, bool bf16) {
+#define KSO(B, M, X, T) KSeqInfo{seq::lutgemv_seq_kernel<B, M, X, T, true>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE, v2::C2<B, M>::NTB}
+    if (bf16) {
+        if (bits == 4) return multi ? KSO(4, 0, true, __nv_bfloat16) : KSO(4, 0, false, __nv_bfloat16);
+        return multi ? KSO(3, 0, true, __nv_bfloat16) : KSO(3, 0, false, __nv_bfloat16);
+    }
+    if (bits == 4) {
+        if (mode == 0) return multi ? KSO(4, 0, true, __half) : KSO(4, 0, false, __half);
+        return multi ? KSO(4, 1, true, __half) : KSO(4, 1, false, __half);
+    }
+    if (mode == 0) return multi ? KSO(3, 0, true, __half) : KSO(3, 0, false, __half);
+    return multi ? KSO(3, 1, true, __half) : KSO(3, 1, false, __half);
+#undef KSO
+}
 KSeqInfo kseq_lookup(int bits, int mode, bool multi, bool bf16) {
 #define KSE(B, M, X) KSeqInfo{seq::lutgemv_seq_kernel<B, M, X>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE, v2::C2<B, M>::NTB}
 #define KSB(B, X) KSeqInfo{seq::lutgemv_seq_kernel<B, 0, X, __nv_bfloat16>, v2::C2<B, 0>::TAB, v2::C2<B, 0>::STAGE, v2::C2<B, 0>::NTB}
@@ -1440,7 +1456,7 @@ struct sqllm_sequence {
     int n = 0, bits = 0, mode = 0, world = 1, rank = 0, grid = 0, smem = 0;
     seq::SeqCfg cfg;
     KSeq fn = nullptr;
-    void *d_descs = nullptr, *d_exports = nullptr, *d_ws = nullptr, *d_arena = nullptr;
+    void *d_descs = nullptr, *d_exports = nullptr, *d_ws = nullptr, *d_arena = nullptr, *d_ops = nullptr;
     bool own_arena = false;
 };
 
@@ -1463,6 +1479,43 @@ extern "C" int sqllm_sequence_create(const sqllm_seq_item *items, int n_items, c
 }
 
 extern "C" int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items, const sqllm_seq_options *opt, int dtype, sqllm_sequence **out) {
+    return sqllm_sequence_create_ops(items, nullptr, n_items, opt, dtype, out);
+}
+
+namespace {
+bool seq_op_active(const sqllm_seq_op &o) { return o.x_op != SQLLM_SEQ_X_PLAIN || o.res_from >= 0 || o.res_ext; }
+
+// the checks of one item's op (items[i], ops[i]); the item's own checks have passed
+int check_seq_op(const sqllm_seq_item *items, const sqllm_seq_op &o, int i, const char *tn) {
+    const sqllm_lutgemv_args &a = items[i].a;
+    const uintptr_t ga = reinterpret_cast<uintptr_t>(o.norm_weight), ra = reinterpret_cast<uintptr_t>(o.res_ext);
+    if (o.x_op != SQLLM_SEQ_X_PLAIN && o.x_op != SQLLM_SEQ_X_RMSNORM && o.x_op != SQLLM_SEQ_X_SILU_MUL)
+        return fail(SQLLM_EINVAL, "sequence: item %d: unknown x_op=%d", i, o.x_op);
+    if (o.x_op == SQLLM_SEQ_X_RMSNORM) {
+        if (!o.norm_weight || (ga & 15)) return fail(SQLLM_EINVAL, "sequence: item %d: norm_weight must be a 16-byte aligned %s vector", i, tn);
+        if (!std::isfinite(o.eps) || o.eps < 0.f) return fail(SQLLM_EINVAL, "sequence: item %d: eps=%g must be finite and >= 0", i, (double)o.eps);
+    }
+    if (o.x_op == SQLLM_SEQ_X_SILU_MUL) {
+        if (o.x2_from < 0 || o.x2_from >= i) return fail(SQLLM_EINVAL, "sequence: item %d: x2_from=%d must name an earlier item", i, o.x2_from);
+        if (o.x2_offset < 0 || o.x2_offset % 4 || (size_t)o.x2_offset + a.in_features > seq_item_len(items[o.x2_from]))
+            return fail(SQLLM_EINVAL, "sequence: item %d: x2 reads [%d, %d) of item %d's %zu outputs", i, o.x2_offset, o.x2_offset + a.in_features,
+                        o.x2_from, seq_item_len(items[o.x2_from]));
+    }
+    if (o.res_from >= 0 && o.res_ext) return fail(SQLLM_EINVAL, "sequence: item %d: one residual source: res_from=%d or res_ext, not both", i, o.res_from);
+    if (o.res_from >= i || o.res_from < -1) return fail(SQLLM_EINVAL, "sequence: item %d: residual source res_from=%d must name an earlier item (or -1)", i, o.res_from);
+    if (o.res_from >= 0) {
+        const size_t n = seq_item_len(items[i]), m = seq_item_len(items[o.res_from]);
+        if (o.res_offset < 0 || o.res_offset % 4 || (size_t)o.res_offset + n > m)
+            return fail(SQLLM_EINVAL, "sequence: item %d: residual reads [%d, %zu) of item %d's %zu outputs (the item's full length is %zu)",
+                        i, o.res_offset, (size_t)std::max(0, o.res_offset) + n, o.res_from, m, n);
+    }
+    if (ra & 15) return fail(SQLLM_EINVAL, "sequence: item %d: res_ext must be a 16-byte aligned %s vector", i, tn);
+    return SQLLM_OK;
+}
+}  // namespace
+
+extern "C" int sqllm_sequence_create_ops(const sqllm_seq_item *items, const sqllm_seq_op *ops, int n_items, const sqllm_seq_options *opt, int dtype,
+                                         sqllm_sequence **out) {
     if (dtype != SQLLM_DT_F16 && dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "sequence: dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", dtype);
     const bool bf = dtype == SQLLM_DT_BF16;
     const char *const tn = bf ? "bf16" : "fp16";
@@ -1505,7 +1558,13 @@ extern "C" int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items
         if (it < 0 || it >= n_items || !opt->export_dst[e] || (reinterpret_cast<uintptr_t>(opt->export_dst[e]) & 7))
             return fail(SQLLM_EINVAL, "sequence: export %d: bad item %d or destination (8-byte aligned %s vector)", e, it, tn);
     }
-    const KSeqInfo ki = kseq_lookup(bits, mode, world > 1, bf);
+    bool any_op = false;
+    for (int i = 0; ops && i < n_items; ++i) {
+        const int rc = check_seq_op(items, ops[i], i, tn);
+        if (rc) return rc;
+        any_op = any_op || seq_op_active(ops[i]);
+    }
+    const KSeqInfo ki = any_op ? kseq_lookup_ops(bits, mode, world > 1, bf) : kseq_lookup(bits, mode, world > 1, bf);
     int sm = 0;
     unsigned raw = 0;
     const int rc = dev_setup({{ki.fn, 227 * 1024}}, &sm, &raw);
@@ -1595,6 +1654,24 @@ extern "C" int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items
         cudaMalloc(&s->d_exports, ex.size() * sizeof(seq::SeqExport)) != cudaSuccess ||
         cudaMemcpy(s->d_exports, ex.data(), ex.size() * sizeof(seq::SeqExport), cudaMemcpyHostToDevice) != cudaSuccess)
         return seq_fail_free(s, fail(SQLLM_ECUDA, "sequence: descriptor upload failed: %s", cudaGetErrorString(cudaGetLastError())));
+    if (any_op) {
+        std::vector<seq::SeqOp> so(n_items);
+        for (int i = 0; i < n_items; ++i) {
+            const sqllm_seq_op &o = ops[i];
+            seq::SeqOp &q = so[i];
+            memset(&q, 0, sizeof(q));
+            q.x_op = o.x_op;
+            q.eps = o.eps;
+            q.gamma = o.x_op == SQLLM_SEQ_X_RMSNORM ? o.norm_weight : nullptr;
+            if (o.x_op == SQLLM_SEQ_X_SILU_MUL)
+                q.x2_tag = reinterpret_cast<const uint32_t *>(static_cast<unsigned char *>(s->d_arena) + yoff[o.x2_from]) + o.x2_offset;
+            if (o.res_from >= 0) q.res_tag = reinterpret_cast<const uint32_t *>(static_cast<unsigned char *>(s->d_arena) + yoff[o.res_from]) + o.res_offset;
+            q.res_ext = o.res_ext;
+        }
+        if (cudaMalloc(&s->d_ops, so.size() * sizeof(seq::SeqOp)) != cudaSuccess ||
+            cudaMemcpy(s->d_ops, so.data(), so.size() * sizeof(seq::SeqOp), cudaMemcpyHostToDevice) != cudaSuccess)
+            return seq_fail_free(s, fail(SQLLM_ECUDA, "sequence: op upload failed: %s", cudaGetErrorString(cudaGetLastError())));
+    }
     seq::SeqCfg &c = s->cfg;
     memset(&c, 0, sizeof(c));
     c.descs = static_cast<const seq::SeqDesc *>(s->d_descs);
@@ -1607,6 +1684,7 @@ extern "C" int sqllm_sequence_create_dt(const sqllm_seq_item *items, int n_items
     c.arena_base = reinterpret_cast<unsigned long long>(s->d_arena);
     c.exports = static_cast<const seq::SeqExport *>(s->d_exports);
     c.nexport = opt->n_export;
+    c.ops = static_cast<const seq::SeqOp *>(s->d_ops);
     *out = s;
     return SQLLM_OK;
 }
@@ -1640,6 +1718,7 @@ extern "C" void sqllm_sequence_destroy(sqllm_sequence *s) {
     if (!s) return;
     cudaFree(s->d_descs);
     cudaFree(s->d_exports);
+    cudaFree(s->d_ops);
     cudaFree(s->d_ws);
     if (s->own_arena) cudaFree(s->d_arena);
     delete s;

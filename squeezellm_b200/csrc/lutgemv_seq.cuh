@@ -31,6 +31,17 @@ struct SeqExport {
     void *dst;                      // plain 16-bit vector (the sequence's activation type)
     int n;
 };
+// What an item of an OPS instance does besides its matvec (sqllm_sequence_create_ops), one per item in a parallel array: a transform
+// of the staged x (RMSNorm, or SiLU gating with a second polled slice) and a residual added to the output inside its one rounding.
+enum : int { SEQ_X_PLAIN = 0, SEQ_X_RMSNORM = 1, SEQ_X_SILU_MUL = 2 };
+struct SeqOp {
+    const void *gamma;              // RMSNorm: weight [K] of XT
+    const uint32_t *x2_tag;         // SiLU gating: first tagged word of the up slice in the local arena (x is the gate)
+    const uint32_t *res_tag;        // residual: first tagged word of an earlier item's full-length vector in the local arena, or null
+    const void *res_ext;            // ... or a plain XT vector of the item's full output length, or null
+    float eps;
+    int x_op;                       // SEQ_X_*
+};
 struct SeqCfg {
     const SeqDesc *descs;
     int ngemv;
@@ -43,6 +54,7 @@ struct SeqCfg {
     unsigned long long arena_base;        // ... and our own
     const SeqExport *exports;
     int nexport;
+    const SeqOp *ops;               // [ngemv]: read by the OPS instances only
 };
 
 __global__ void seq_bump_epoch(unsigned *epoch) { *epoch = *epoch + 1u; }
@@ -86,10 +98,70 @@ __device__ __forceinline__ void poll_tagged(const uint32_t *src, const int n4, c
     }
 }
 
+// ---- the OPS instances' extras ----
+template <bool SYS>
+__device__ __forceinline__ uint32_t ld_relaxed_u32(const uint32_t *p) {
+    uint32_t v;
+    if constexpr (SYS) asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    else asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+template <typename XT>
+__device__ __forceinline__ uint32_t f32x2_to_xt2(float lo, float hi) {
+    return (uint32_t)bits16(f32_to<XT>(lo)) | ((uint32_t)bits16(f32_to<XT>(hi)) << 16);
+}
+// silu(g) u on two packed pairs, in fp32 (silu(g) = g / (1 + e^-g): -0 for g -> -inf, g for g -> +inf), one rounding to XT per value
+template <typename XT>
+__device__ __forceinline__ uint32_t silu_mul2(uint32_t g2, uint32_t u2) {
+    const float2 g = x16x2_to_f32x2<XT>(g2), u = x16x2_to_f32x2<XT>(u2);
+    return f32x2_to_xt2<XT>(g.x / (1.f + expf(-g.x)) * u.x, g.y / (1.f + expf(-g.y)) * u.y);
+}
+// RMSNorm of the staged x in place, by the NCT consumer threads (x complete in shared memory, and again at the end for the caller's
+// barrier): S = sum x_k^2 in fp32 in an order fixed by the thread layout alone - thread t takes the 8-element pieces t, t + NCT, ...
+// one fma after the other, the warp adds its lanes by the fixed xor tree, every thread adds the 16 warp sums 0..15 from `scratch` - so
+// every CTA holds the same bits; r = 1 / sqrt(S / K + eps); x'_k = round_XT(gamma_k (x_k r)).  (HF's LlamaRMSNorm rounds twice:
+// (x r).to(dtype), then gamma times that; here x r stays in fp32 and only the product with gamma is rounded.)
+template <typename XT>
+__device__ __forceinline__ void rmsnorm_x(uint32_t xs, int K, const XT *gamma, float eps, uint32_t scratch, int tid) {
+    const int n8 = K / 8;
+    float s = 0.f;
+    for (int e = tid; e < n8; e += NCT) {
+        uint32_t w[4];
+        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "r"(xs + 16u * (uint32_t)e));
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 f = x16x2_to_f32x2<XT>(w[j]);
+            s = fmaf(f.x, f.x, s);
+            s = fmaf(f.y, f.y, s);
+        }
+    }
+    s = warp_sum(s);
+    if ((tid & 31) == 0) sts_u32(scratch + 4u * (uint32_t)(tid >> 5), __float_as_uint(s));
+    named_bar_sync(1, NCT);
+    float S = 0.f;
+#pragma unroll
+    for (int w = 0; w < NWC; ++w) S += lds_f32(scratch + 4u * w);
+    const float r = 1.f / sqrtf(S / (float)K + eps);
+    for (int e = tid; e < n8; e += NCT) {
+        uint32_t w[4];
+        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "r"(xs + 16u * (uint32_t)e));
+        const uint4 gw = __ldg(reinterpret_cast<const uint4 *>(gamma) + e);
+        const uint32_t gg[4] = {gw.x, gw.y, gw.z, gw.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 f = x16x2_to_f32x2<XT>(w[j]), g = x16x2_to_f32x2<XT>(gg[j]);
+            w[j] = f32x2_to_xt2<XT>(g.x * (f.x * r), g.y * (f.y * r));
+        }
+        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(xs + 16u * (uint32_t)e), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
+    }
+}
+
 
 // XT: the sequence's 16-bit activation type (__half or __nv_bfloat16): the type of x_ext, of the value half of every tagged word, of
 // the items' plain y copies and of the exports.  The poll, the staging and the exports only move bits; a word is made in store_y.
-template <int BITS, int MODE, bool MULTI, typename XT = __half>
+// OPS: the instance that also runs every item's SeqOp (c.ops): RMSNorm or SiLU gating of the staged x before barrier 2, a residual in
+// store_y.  The instances without it never read c.ops.
+template <int BITS, int MODE, bool MULTI, typename XT = __half, bool OPS = false>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c) {
     using C = C2<BITS, MODE>;
     static_assert(std::is_same<XT, __half>::value || std::is_same<XT, __nv_bfloat16>::value, "x is fp16 or bf16");
@@ -319,6 +391,37 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
 #pragma unroll
                 for (int h = 0; h < 3; ++h)
                     hw[h] = h < nh ? ld_relaxed_u64(p.ws_hbox + ((size_t)blockIdx.x + 1 + h) * STRIP + bt) : box_word(0.f, boxtag);
+                // OPS residual: one word per owned column, issued with the mailbox words.  An external vector's element is given the token's
+                // tag here; an earlier item's word is taken like x (read again until it carries the tag, bounded).  Column col reads the
+                // element of the full-length vector that store_y writes: col on one GPU, e below on several.
+                const uint32_t *res_tag = nullptr;
+                const XT *res_ext = nullptr;
+                if constexpr (OPS) {
+                    res_tag = c.ops[g].res_tag;
+                    res_ext = static_cast<const XT *>(c.ops[g].res_ext);
+                }
+                auto res_index = [&](int col) -> unsigned {
+                    if constexpr (!MULTI) return (unsigned)col;
+                    const int wm = N / p.xw_members, mm = col / wm;
+                    return (unsigned)(mm * p.xw_nfull + c.rank * wm + (col - mm * wm));
+                };
+                auto res_word = [&](int col) -> uint32_t {
+                    if (res_tag) return ld_relaxed_u32<MULTI>(res_tag + res_index(col));
+                    if (res_ext) return xwant | (uint32_t)bits16(res_ext[res_index(col)]);
+                    return 0u;
+                };
+                uint32_t rw[FAST], rlast = 0u;
+                if constexpr (OPS) {
+                    if (res_tag || res_ext) {
+#pragma unroll
+                        for (int u = 0; u < FAST; ++u) {
+                            const int col = (so0 + u) * STRIP + bt;
+                            rw[u] = u < nown && u != lidx && col < N ? res_word(col) : 0u;   // (the last owned strip's word: rlast)
+                        }
+                        const int lcol = (so0 + lidx) * STRIP + bt;
+                        if (lidx >= 0 && lcol < N) rlast = res_word(lcol);
+                    }
+                }
                 // dense rows: hc tagged words per listed row (one from every contributing CTA), four loads in flight per thread; row sums are
                 // collected in shared memory and added to the column they belong to by the thread that owns that column
                 float last_dense = 0.f;
@@ -362,8 +465,23 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                     named_bar_sync(3, NBT);  // (the list and the sums are reused by the next item; an idle CTA has no other barrier before that)
                 }
                 const int w = MULTI ? N / p.xw_members : 0;
-                auto store_y = [&](int col, float yv) {
+                auto store_y = [&](int col, float yv, uint32_t rword = 0u) {
                     if (p.bias) yv += __ldg(p.bias + col);
+                    if constexpr (OPS) {
+                        if (res_tag || res_ext) {  // y = round_XT(sum + bias + r): the residual too is inside the one rounding
+                            if ((rword ^ xwant) >> 16) {
+                                const uint32_t *const src = res_tag + res_index(col);
+                                unsigned long long t0, t1;
+                                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+                                do {
+                                    rword = ld_relaxed_u32<MULTI>(src);
+                                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+                                    if (t1 - t0 > 2000000000ull) { *reinterpret_cast<volatile int *>(err) = 1; break; }
+                                } while ((rword ^ xwant) >> 16);
+                            }
+                            yv += x16x2_to_f32x2<XT>(rword & 0xFFFFu).x;
+                        }
+                    }
                     const XT yh = f32_to<XT>(yv);   // the one rounding: the bias is inside the fp32 sum
                     const uint32_t word = (xtag << 16) | (uint32_t)bits16(yh);
                     if constexpr (!MULTI) {
@@ -389,7 +507,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                         if (u != lidx && u < SOWN) yv = lds_f32(sown + 4u * (uint32_t)(u * STRIP + bt));
                         if (p.rows) yv += box_take(cw[u], p.ws_cbox + col, err, boxtag, true);
                         if (u == lidx) last_others += yv;
-                        else store_y(col, yv);
+                        else store_y(col, yv, OPS ? rw[u] : 0u);
                     }
                 }
                 for (int i = FAST; i < nown; ++i) {  // (more owned strips than FAST; beyond SOWN the sums went through the global accumulator)
@@ -400,7 +518,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                         else if (i != lidx) yv = lds_f32(sown + 4u * (uint32_t)(i * STRIP + bt));
                         if (p.rows) yv += box_take(0ull, p.ws_cbox + col, err, boxtag, true);
                         if (i == lidx) last_others += yv;
-                        else store_y(col, yv);
+                        else store_y(col, yv, OPS ? res_word(col) : 0u);
                     }
                 }
                 TRACE(15, bt == 0);
@@ -427,7 +545,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                         const float own = lds_f32(a);
                         sts_u32(a, 0u);
                         const int lcol = (s0 + s) * STRIP + bt;
-                        if (lcol < N) store_y(lcol, last_others + own);
+                        if (lcol < N) store_y(lcol, last_others + own, rlast);
                     } else {
                         flush(s);
                     }
@@ -468,6 +586,24 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 poll_tagged<MULTI>(d.x_tag, p.K / 4, tid, NCT, xwant, c.err, [&](int i, uint32_t lo, uint32_t hi) {
                     asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(xs_u32 + 8u * (uint32_t)i), "r"(lo), "r"(hi) : "memory");
                 });
+            }
+            if constexpr (OPS) {
+                const SeqOp &o = c.ops[g];
+                const int xop = o.x_op;
+                if (xop != SEQ_X_PLAIN) {
+                    named_bar_sync(1, NCT);  // the whole x is staged (a copied or polled piece may come from another thread)
+                    if (xop == SEQ_X_RMSNORM) {
+                        // scratch: the 16 warp sums in the fixed area's strip-sum rows, which only the one-GEMV kernel uses
+                        rmsnorm_x<XT>(xs_u32, p.K, static_cast<const XT *>(o.gamma), o.eps, base + OFF_SACC, tid);
+                    } else {
+                        poll_tagged<MULTI>(o.x2_tag, p.K / 4, tid, NCT, xwant, c.err, [&](int i, uint32_t lo, uint32_t hi) {
+                            const uint32_t a = xs_u32 + 8u * (uint32_t)i;
+                            uint32_t g0, g1;
+                            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(g0), "=r"(g1) : "r"(a));
+                            asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(silu_mul2<XT>(g0, lo)), "r"(silu_mul2<XT>(g1, hi)) : "memory");
+                        });
+                    }
+                }
             }
             named_bar_sync(2, NCT + NSPW * 32);  // x visible to the consumers and the outlier warps
             TRACE(4, tid == 0);

@@ -18,6 +18,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <map>
 #include <mutex>
 #include <string>
@@ -444,14 +445,57 @@ void lutgemv_fused_exchange_bf16(torch::Tensor x, torch::Tensor qweight, torch::
 // exports: list of (item index, destination tensor of the item's full output length).  dtype: the activation type, torch.float16 or
 // torch.bfloat16 (sqllm_sequence_create_dt): every x_ext and every export destination has it.  The caller keeps every tensor alive for
 // the life of the handle (squeezellm_b200.runtime.DecodeSequence does).  peer_base / arena: several GPUs only (0 / None otherwise).
+// ops (keyword, sqllm_sequence_create_ops): None, or one entry per item: None (nothing) or a tuple
+//     (x_op, norm_weight|None, eps, x2_from, x2_offset, res_from, res_offset, res_ext|None)
+// with x_op 0 plain, 1 RMSNorm, 2 SiLU gating; norm_weight and res_ext contiguous CUDA tensors of the sequence's dtype.  The op checks
+// that need no item (x_op, eps, which items the sources name, the tensors) come first; the rest are the C entry point's.
+std::vector<sqllm_seq_op> sequence_ops(const py::object &ops, int n, at::ScalarType dtype, const char *tn) {
+    std::vector<sqllm_seq_op> v;
+    if (ops.is_none()) return v;
+    py::list l = ops.cast<py::list>();
+    TORCH_CHECK((int)l.size() == n, "sequence_create: ", l.size(), " ops for ", n, " items");
+    v.resize(n);
+    for (int i = 0; i < n; ++i) {
+        sqllm_seq_op &o = v[i];
+        memset(&o, 0, sizeof(o));
+        o.x2_from = o.res_from = -1;
+        if (l[i].is_none()) continue;
+        py::tuple t = l[i].cast<py::tuple>();
+        TORCH_CHECK(t.size() == 8, "sequence op ", i, ": expected None or an 8-tuple (x_op, norm_weight, eps, x2_from, x2_offset, res_from, res_offset, res_ext)");
+        o.x_op = t[0].cast<int>();
+        o.eps = t[2].cast<float>();
+        o.x2_from = t[3].cast<int>(); o.x2_offset = t[4].cast<int>();
+        o.res_from = t[5].cast<int>(); o.res_offset = t[6].cast<int>();
+        TORCH_CHECK(o.x_op == SQLLM_SEQ_X_PLAIN || o.x_op == SQLLM_SEQ_X_RMSNORM || o.x_op == SQLLM_SEQ_X_SILU_MUL, "sequence item ", i, ": unknown x_op=", o.x_op);
+        auto vec = [&](int k, const char *name) -> const void * {
+            if (t[k].is_none()) return nullptr;
+            torch::Tensor w = t[k].cast<torch::Tensor>();
+            TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.scalar_type() == dtype, "sequence item ", i, ": ", name, " must be a contiguous ", tn,
+                        " CUDA tensor (the sequence's dtype; got ", w.scalar_type(), w.is_cuda() ? "" : " on the CPU", ")");
+            return w.data_ptr();
+        };
+        o.norm_weight = vec(1, "norm_weight");
+        o.res_ext = vec(7, "res_ext");
+        if (o.x_op == SQLLM_SEQ_X_RMSNORM) {
+            TORCH_CHECK(o.norm_weight, "sequence item ", i, ": RMSNorm needs norm_weight");
+            TORCH_CHECK(std::isfinite(o.eps) && o.eps >= 0.f, "sequence item ", i, ": eps=", o.eps, " must be finite and >= 0");
+        }
+        if (o.x_op == SQLLM_SEQ_X_SILU_MUL)
+            TORCH_CHECK(o.x2_from >= 0 && o.x2_from < i, "sequence item ", i, ": x2_from=", o.x2_from, " must name an earlier item");
+        TORCH_CHECK(o.res_from >= -1 && o.res_from < i, "sequence item ", i, ": residual source res_from=", o.res_from, " must name an earlier item (or -1)");
+    }
+    return v;
+}
+
 int64_t sequence_create(py::list items, py::list exports, const std::string &lut_mode, int world, int rank,
-                        c10::optional<torch::Tensor> arena, int64_t peer_base, at::ScalarType dtype) {
+                        c10::optional<torch::Tensor> arena, int64_t peer_base, at::ScalarType dtype, py::object ops) {
     TORCH_CHECK(lut_mode == "exact" || lut_mode == "fp16", "lut mode must be 'exact' or 'fp16'");
     TORCH_CHECK(dtype == torch::kFloat16 || dtype == torch::kBFloat16, "sequence_create: dtype must be torch.float16 or torch.bfloat16 (got ", dtype, ")");
     const bool bf = dtype == torch::kBFloat16;
     const char *const tn = bf ? "bf16" : "fp16";
     const int n = (int)items.size();
     TORCH_CHECK(n > 0, "sequence_create: no items");
+    const std::vector<sqllm_seq_op> sops = sequence_ops(ops, n, dtype, tn);
     std::vector<sqllm_seq_item> its(n);
     c10::optional<torch::Tensor> first;
     for (int i = 0; i < n; ++i) {
@@ -512,7 +556,8 @@ int64_t sequence_create(py::list items, py::list exports, const std::string &lut
     o.peer_base = reinterpret_cast<const uint64_t *>(peer_base);
     o.n_export = ne; o.export_items = ex_items.data(); o.export_dst = ex_dst.data();
     sqllm_sequence *h = nullptr;
-    check_status(sqllm_sequence_create_dt(its.data(), n, &o, bf ? SQLLM_DT_BF16 : SQLLM_DT_F16, &h), "quant_cuda.sequence_create");
+    check_status(sqllm_sequence_create_ops(its.data(), sops.empty() ? nullptr : sops.data(), n, &o, bf ? SQLLM_DT_BF16 : SQLLM_DT_F16, &h),
+                 "quant_cuda.sequence_create");
     return reinterpret_cast<int64_t>(h);
 }
 
@@ -666,7 +711,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("out_features_full"));
     m.def("sequence_create", &sequence_create, "one persistent launch for a list of dependent fused matvecs (see squeezellm_b200.runtime.DecodeSequence)",
           py::arg("items"), py::arg("exports"), py::arg("lut_mode") = "exact", py::arg("world") = 1, py::arg("rank") = 0,
-          py::arg("arena") = py::none(), py::arg("peer_base") = 0, py::arg("dtype") = torch::kFloat16);
+          py::arg("arena") = py::none(), py::arg("peer_base") = 0, py::arg("dtype") = torch::kFloat16, py::kw_only(), py::arg("ops") = py::none());
     m.def("sequence_arena_bytes", [](py::list lens) {
               size_t off = 0;
               for (auto l : lens) off += ((size_t)l.cast<int64_t>() * 4 + 127) / 128 * 128;

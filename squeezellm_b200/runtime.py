@@ -52,7 +52,8 @@ class GraphedDecodeStep:
 
 
 class SeqVec:
-    """A vector inside a DecodeSequence: the token's input (item -1) or (a slice of) the output of one of its matvecs."""
+    """A vector inside a DecodeSequence: an external input (item -1: `seq.x`; -2, -3, ...: the vectors of `new_input`) or (a slice of)
+    the output of one of its matvecs."""
 
     def __init__(self, item, offset, length):
         self.item, self.offset, self.length = item, offset, length
@@ -85,7 +86,10 @@ class DecodeSequence:
     `dtype` is the activation type, torch.float16 or torch.bfloat16: that of `x`, of the values handed from one matvec to the next
     and of the outputs; every output is rounded to it once, with the bias inside the fp32 sum.  A bf16 sequence uses the exact
     codebook whatever `lut_mode` says (the fp16 pair table multiplies fp16 by fp16), as QuantLinearLUT does for one bf16 row.
-    On several GPUs pass `peer` (sharding.PeerArena): every layer is this rank's column shard."""
+    On several GPUs pass `peer` (sharding.PeerArena): every layer is this rank's column shard.
+
+    What a decoder layer puts between two matvecs runs inside the same launch (`matvec`'s keywords): an RMSNorm of the input, SiLU
+    gating of the input by a second vector, a residual added to the output - each rounded to `dtype` once (lutgemv_seq.cuh)."""
 
     def __init__(self, in_features, device, lut_mode=None, peer=None, dtype=torch.float16):
         if dtype not in (torch.float16, torch.bfloat16):
@@ -94,24 +98,61 @@ class DecodeSequence:
         self.dtype = dtype
         self.x = torch.zeros(in_features, dtype=dtype, device=self.device)
         self.input = SeqVec(-1, 0, in_features)
-        self._items, self._lens, self._keep = [], [], []
+        self._ext = [self.x]   # external vector of item -1 - j: self._ext[j]
+        self._items, self._lens, self._keep, self._ops = [], [], [], []
         self._handle, self.outputs, self._out_vecs = None, [], []
         self.lut_mode = lut_mode
         self.peer = peer
 
-    def matvec(self, layer, x, members=1):
-        """Record y = layer(x).  `members`: on several GPUs, how many equal column shards `layer` stacks (q/k/v: 3)."""
+    def new_input(self, n):
+        """Another external vector of n elements: (its SeqVec, its static tensor), read by every run like `x`."""
+        assert self._handle is None, "sequence already compiled"
+        t = torch.zeros(n, dtype=self.dtype, device=self.device)
+        self._ext.append(t)
+        return SeqVec(-len(self._ext), 0, n), t
+
+    def _ext_tensor(self, v):
+        t = self._ext[-v.item - 1]
+        return t if v.offset == 0 and v.length == t.numel() else t[v.offset:v.offset + v.length]
+
+    def matvec(self, layer, x, members=1, *, norm=None, up=None, residual=None):
+        """Record y = layer(x).  `members`: on several GPUs, how many equal column shards `layer` stacks (q/k/v: 3).
+        norm=(weight, eps): the layer reads RMSNorm(x) (weight [in_features] of the sequence's dtype); up=SeqVec: it reads
+        silu(x) * up (up: an earlier matvec's output); residual=SeqVec: y = layer(...) + residual, the residual of y's full length."""
         assert self._handle is None, "sequence already compiled"
         assert isinstance(x, SeqVec) and x.length == layer.infeatures, f"input has {len(x)} elements, layer wants {layer.infeatures}"
         assert x.item < len(self._items)
+        assert norm is None or up is None, "one input transform per matvec: norm or up"
         world = self.peer.world if self.peer is not None else 1
         assert layer.outfeatures % members == 0
         nfull = layer.outfeatures // members * world
         rows, cols, vals, fr, fri = layer._sparse_args()
         self._items.append((layer.qweight, layer.lookup_table, layer.bits, layer.bias, rows, cols, vals, fr, fri,
-                            x.item, x.offset, self.x if x.item < 0 else None, members, nfull))
+                            x.item, x.offset, self._ext_tensor(x) if x.item < 0 else None, members, nfull))
         self._keep.append(layer)
         self._lens.append(members * nfull)
+        op = None
+        if norm is not None or up is not None or residual is not None:
+            x_op, weight, eps, x2 = 0, None, 0.0, (-1, 0)
+            if norm is not None:
+                weight, eps = norm
+                assert weight.numel() == layer.infeatures, f"norm weight has {weight.numel()} elements, layer wants {layer.infeatures}"
+                x_op, weight = 1, weight.to(device=self.device, dtype=self.dtype).contiguous()
+                self._keep.append(weight)
+            if up is not None:
+                assert isinstance(up, SeqVec) and 0 <= up.item < len(self._items) - 1, "up must be an earlier matvec's output"
+                assert up.length == layer.infeatures, f"up has {len(up)} elements, layer wants {layer.infeatures}"
+                x_op, x2 = 2, (up.item, up.offset)
+            res, res_ext = (-1, 0), None
+            if residual is not None:
+                assert isinstance(residual, SeqVec) and residual.length == members * nfull, \
+                    f"residual has {len(residual)} elements, the output has {members * nfull}"
+                if residual.item >= 0:
+                    res = (residual.item, residual.offset)
+                else:
+                    res_ext = self._ext_tensor(residual)
+            op = (x_op, weight, float(eps), x2[0], x2[1], res[0], res[1], res_ext)
+        self._ops.append(op)
         return SeqVec(len(self._items) - 1, 0, members * nfull)
 
     def compile(self, outputs):
@@ -125,14 +166,15 @@ class DecodeSequence:
                 bufs[v.item] = torch.zeros(self._lens[v.item], dtype=self.dtype, device=self.device)
                 exports.append((v.item, bufs[v.item]))
         self.outputs = [bufs[v.item][v.offset:v.offset + v.length] for v in outputs]
+        ops = self._ops if any(o is not None for o in self._ops) else None
         with torch.cuda.device(self.device):
             if self.peer is not None:
                 arena, peer_base = self.peer.arena_for(quant_cuda.sequence_arena_bytes(self._lens))
                 self._handle = quant_cuda.sequence_create(self._items, exports, mode, self.peer.world, self.peer.rank, arena, peer_base,
-                                                          dtype=self.dtype)
+                                                          dtype=self.dtype, ops=ops)
                 self._arena = arena
             else:
-                self._handle = quant_cuda.sequence_create(self._items, exports, mode, dtype=self.dtype)
+                self._handle = quant_cuda.sequence_create(self._items, exports, mode, dtype=self.dtype, ops=ops)
         self._exports = exports
         self._quant_cuda = quant_cuda
         return self
