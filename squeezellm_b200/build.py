@@ -3,6 +3,9 @@
   squeezellm_b200/libsqllm_b200.so                 CUDA kernels + C ABI   (nvcc, sm_90a only)
   squeezellm_b200/quant_cuda.<abi>.so              pybind11 adapter        (g++, links the above)
 
+The library is one translation unit per kernel family (csrc/*.cu), compiled in parallel into squeezellm_b200/obj/ and linked
+with one `nvcc -shared`.  A unit is recompiled when it or any header is newer than its object.
+
 `python -m squeezellm_b200.build` or `__graft_entry__.build()`.
 """
 import glob
@@ -17,6 +20,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 INCLUDE = os.path.join(ROOT, "include")
+OBJ = os.path.join(PKG, "obj")
 
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC"]  # fast-math deliberately NOT used
@@ -42,14 +46,27 @@ def ext_path():
 
 
 def build_lib(verbose=False):
-    src = os.path.join(CSRC, "lutgemv_kernels.cu")
-    hdr = os.path.join(INCLUDE, "sqllm_b200.h")
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    hdrs = [os.path.join(INCLUDE, "sqllm_b200.h")] + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h"))
+    os.makedirs(OBJ, exist_ok=True)
+    objs, jobs = [], []
+    for src in sorted(glob.glob(os.path.join(CSRC, "*.cu"))):
+        obj = os.path.join(OBJ, os.path.basename(src)[:-3] + ".o")
+        objs.append(obj)
+        if _newer(obj, [src] + hdrs):
+            cmd = [nvcc] + NVCC_FLAGS + ["-ccbin", _cxx(), "-I", INCLUDE, "-c", "-o", obj, src]
+            if verbose:
+                cmd.insert(1, "-Xptxas=-v")
+                print(" ".join(cmd))
+            jobs.append((subprocess.Popen(cmd), cmd))
+    rcs = [(p.wait(), cmd) for p, cmd in jobs]  # every compile ends before a failure is raised
+    for rc, cmd in rcs:
+        if rc:
+            raise subprocess.CalledProcessError(rc, cmd)
     out = lib_path()
-    if _newer(out, [src, hdr] + glob.glob(os.path.join(CSRC, "*.cuh"))):
-        nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-        cmd = [nvcc] + NVCC_FLAGS + ["-ccbin", _cxx(), "-I", INCLUDE, "-shared", "-o", out, src]
+    if _newer(out, objs):
+        cmd = [nvcc] + NVCC_FLAGS + ["-ccbin", _cxx(), "-shared", "-o", out] + objs
         if verbose:
-            cmd.insert(1, "-Xptxas=-v")
             print(" ".join(cmd))
         subprocess.check_call(cmd)
     return out

@@ -1,6 +1,6 @@
 // dequant.cuh - the dense weight of a layer, W[c][k] = codebook + CSR outliers + dense rows, written as fp32, fp16 or bf16 [n][K]
-// (nn.Linear.weight's [out, in] layout) for the column range [c0, c0 + n): sqllm_dequantize.  Included by lutgemv_kernels.cu
-// inside its anonymous namespace, after lutgemm_tc.cuh (whose index decoders it shares).
+// (nn.Linear.weight's [out, in] layout) for the column range [c0, c0 + n): sqllm_dequantize.  It shares the index
+// decoders of lutgemm_tc.cuh.
 //
 // Every element is defined exactly:
 //   w  = lookup_table[c][idx(k, c)]                                        (fp32)
@@ -20,6 +20,10 @@
 //   * W: each thread rounds 4 (fp32) or 8 (fp16 / bf16) consecutive k of one row and writes them with one 16-byte store.
 // Every output element is written once by one thread: no atomics, no workspace, bit-reproducible.
 #pragma once
+#include "common.cuh"
+#include "lutgemm_tc.cuh"
+
+namespace {
 
 namespace dq {
 
@@ -167,3 +171,5 @@ __global__ void __launch_bounds__(THREADS) dequant_kernel(const PD p) {
 }
 
 }  // namespace dq
+
+}  // namespace

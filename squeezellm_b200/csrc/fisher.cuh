@@ -1,6 +1,6 @@
 // fisher.cuh - the diagonal of the empirical Fisher information of a linear layer on the tensor cores (wgmma), behind
-// sqllm_fisher_accumulate.  Included by lutgemv_kernels.cu inside its anonymous namespace, after lut_grad_tc.cuh, whose MN-major
-// staging (lgt::stage) and wgmma (lgt::wgmma_tt) it uses, and lutgemm_tc_t.cuh (tct::mn_desc).
+// sqllm_fisher_accumulate.  It uses the MN-major staging (lgt::stage) and wgmma (lgt::wgmma_tt) of lut_grad_tc.cuh
+// and the descriptor of lutgemm_tc_t.cuh (tct::mn_desc).
 //
 //   F[n][k] += sum_s g_s[n][k]^2,   g_s = dy_s^T x_s   (sample s: rows [s T, s T + T) of x [rows, K] and dy [rows, N])
 //
@@ -16,6 +16,12 @@
 // fixed order.  The tile is 128 x 128 because the promotion costs a second accumulator: acc, sum and the F tile are 3 x 64
 // registers per thread, which leaves room for addressing under the 255-register limit of one 256-thread CTA per SM.
 #pragma once
+#include "common.cuh"
+#include "lut_grad_tc.cuh"
+#include "lutgemm_tc.cuh"
+#include "lutgemm_tc_t.cuh"
+
+namespace {
 
 namespace fis {
 
@@ -106,3 +112,5 @@ __global__ void __launch_bounds__(THREADS, 1) fisher_kernel(const PF p) {
 }
 
 }  // namespace fis
+
+}  // namespace

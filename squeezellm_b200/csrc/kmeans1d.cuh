@@ -16,6 +16,9 @@
 // Every sum has a fixed order and every argmin is a lexicographic (value, index) minimum, so a row's result depends on that row
 // alone: not on the other rows, the chunking, the stream or the run.
 #pragma once
+#include <stdint.h>
+
+namespace {
 
 namespace km {
 
@@ -255,3 +258,5 @@ __global__ void segment_offsets_kernel(int *offs, int rows, int n) {
 }
 
 }  // namespace km
+
+}  // namespace

@@ -1,6 +1,5 @@
 // lut_grad.cuh - gradients of QuantLinearLUT's continuous parameters behind sqllm_lut_grad: the per-channel codebook, the CSR
-// outlier values and the dense rows, from G = x^T . dy.  Included by lutgemv_kernels.cu inside its anonymous namespace, after
-// lutgemm_tc.cuh (3-bit index helpers) and lutgemv_rows.cuh (cluster helpers).  This file holds the plan,
+// outlier values and the dense rows, from G = x^T . dy (3-bit index helpers: lutgemm_tc.cuh).  This file holds the plan,
 // the epilogue and the cluster reduction that both kernels share, and the CUDA-core kernel; lut_grad_tc.cuh the tensor-core one.
 //
 //   G[k][c] = sum_m x[m][k] dy[m][c]                                   (K x N, the reduction over the rows)
@@ -20,6 +19,10 @@
 // After the slab the bins ([2^bits][128] fp32) of the S CTAs are added by the leader over DSMEM in rank order and dLUT is written
 // once.  No workspace, no atomics, no spin-waits: bit-reproducible, CUDA-graph capturable and safe on several streams.
 #pragma once
+#include "common.cuh"
+#include "lutgemm_tc.cuh"
+
+namespace {
 
 namespace lg {
 
@@ -249,3 +252,5 @@ __global__ void __launch_bounds__(THREADS, 1) lut_grad_kernel(const PG p) {
 }
 
 }  // namespace lg
+
+}  // namespace

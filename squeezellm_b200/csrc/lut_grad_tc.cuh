@@ -1,6 +1,6 @@
 // lut_grad_tc.cuh - the tile of G = x^T . dy on the tensor cores (wgmma) for sqllm_lut_grad when x and dy are both fp16 or both
-// bf16.  Included by lutgemv_kernels.cu inside its anonymous namespace, after lut_grad.cuh (plan, epilogue, cluster reduction)
-// and lutgemm_tc_t.cuh (MN-major descriptor).
+// bf16.  It uses the plan, epilogue and cluster reduction of lut_grad.cuh and the MN-major descriptor of
+// lutgemm_tc_t.cuh.
 //
 // Per k-tile the CTA walks M in chunks of 64 rows, double-buffered with cp.async:
 //   * x [64 m x 128 k] is the A operand and dy [64 m x 128 c] the B operand, both stored as they lie in memory - contiguous along
@@ -12,6 +12,12 @@
 // from zero and the chunk's result is added into a running fp32 sum with FADD (the promotion of lutgemm_tc.cuh): the tensor core's
 // own accumulation never sees more than 64 products per output.
 #pragma once
+#include "common.cuh"
+#include "lut_grad.cuh"
+#include "lutgemm_tc.cuh"
+#include "lutgemm_tc_t.cuh"
+
+namespace {
 
 namespace lgt {
 
@@ -142,3 +148,5 @@ __global__ void __launch_bounds__(THREADS, 1) lut_grad_tc_kernel(const lg::PG p)
 }
 
 }  // namespace lgt
+
+}  // namespace

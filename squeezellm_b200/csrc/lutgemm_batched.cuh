@@ -1,5 +1,4 @@
-// lutgemm_batched.cuh - the six *_batched symbols done properly (SURVEY.md 8(f) row 3).  Included by lutgemv_kernels.cu inside its
-// anonymous namespace.
+// lutgemm_batched.cuh - the six *_batched symbols done properly (SURVEY.md 8(f) row 3).
 //
 // Reference: VecQuant{3,4}MatMulKernelNUQPerChannelBatched (squeezellm/quant_cuda_kernel.cu:884-1038) loops `for b` INSIDE every
 // thread, one look-up and one FMA per (weight, batch row) with the weight word re-read from memory each time; SPMV_ATOMIC_BATCHED
@@ -13,6 +12,9 @@
 //   * csr_batched_kernel / dense_rows_batched_kernel: the outlier terms, one thread per (batch row, output channel | dense row column).
 // Results accumulate into `mul` (the reference's contract: the caller pre-fills zeros or bias, quant.py:316-318).
 #pragma once
+#include "common.cuh"
+
+namespace {
 
 namespace batched {
 
@@ -249,3 +251,5 @@ __global__ void dense_rows_batched_kernel(const float *__restrict__ full_rows, c
 }
 
 }  // namespace batched
+
+}  // namespace

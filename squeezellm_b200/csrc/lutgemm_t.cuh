@@ -1,5 +1,4 @@
 // lutgemm_t.cuh - the transposed LUT-GEMM behind sqllm_lutgemm_t: the input gradient of QuantLinearLUT on the CUDA cores.
-// Included by lutgemv_kernels.cu inside its anonymous namespace, after lutgemv_rows.cuh (cluster helpers).
 //
 //   dx[m][k] = sum_c dy[m][c] W[k][c],   W[k][c] = LUT[c][idx(k,c)] + CSR(c,k) + sum_j full_rows[k][j] [fri[j] == c]
 //
@@ -28,6 +27,9 @@
 //     workspace, no atomics: bit-reproducible, safe on several streams, CUDA-graph capturable.
 // CSR columns outside [0, K) and dense-row channels outside [0, N) are ignored.
 #pragma once
+#include "common.cuh"
+
+namespace {
 
 namespace bwd {
 
@@ -298,3 +300,5 @@ __global__ void __launch_bounds__(TTHREADS, 2) lutgemm_t_kernel(const PT p) {
 }
 
 }  // namespace bwd
+
+}  // namespace

@@ -1,5 +1,5 @@
 // lutgemm_tc.cuh - tensor-core (wgmma) LUT-GEMM for M >= 1 rows of fp16 or bf16 activations (sqllm_lutgemm_fused_dt) or fp32 ones
-// (sqllm_lutgemm_fused_f32).  Included by lutgemv_kernels.cu inside its anonymous namespace.
+// (sqllm_lutgemm_fused_f32).
 //
 // fp32 x (F32X) is not exact in a 16-bit operand: it is split like the weights into three bf16 parts (split3_bf16x2), loaded into
 // registers at the start of each chunk's build (the loads fly while the weights are decoded) and stored as three x tiles of the
@@ -37,6 +37,9 @@
 // ascending is filtered in full at every chunk instead (slow, still exact).  Column indices outside [0, K) and dense-row indices
 // outside [0, N) are ignored.  No limit on topX or on the number of outliers.
 #pragma once
+#include "common.cuh"
+
+namespace {
 
 namespace tc {
 
@@ -428,3 +431,5 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_kernel(const PT p) {
 }
 
 }  // namespace tc
+
+}  // namespace

@@ -1,6 +1,6 @@
 // lutgemm_tc_t.cuh - the transposed LUT-GEMM on the tensor cores (wgmma), behind sqllm_lutgemm_t's tensor-core path: the input
-// gradient of QuantLinearLUT for fp16 or bf16 dy.  Included by lutgemv_kernels.cu inside its anonymous namespace, after
-// lutgemm_tc.cuh, whose operand layout, wgmma descriptors and 3-bit index helpers it shares.
+// gradient of QuantLinearLUT for fp16 or bf16 dy.  It shares the operand layout, wgmma descriptors and 3-bit index
+// helpers of lutgemm_tc.cuh.
 //
 //   dx[M, K] = dy[M, N] . W^T,   W = LUT + CSR + dense rows          (one launch, every output written once, no atomics)
 //
@@ -24,6 +24,10 @@
 // CSR columns outside [0, K) and dense-row channels outside [0, N) are ignored; duplicate entries add up.  No limit on topX or on the
 // entries per CSR row (each thread scans its column's CSR row in full: rows need not be ascending).
 #pragma once
+#include "common.cuh"
+#include "lutgemm_tc.cuh"
+
+namespace {
 
 namespace tct {
 
@@ -299,3 +303,5 @@ __global__ void __launch_bounds__(THREADS, 1) lutgemm_tc_t_kernel(const PT p) {
 }
 
 }  // namespace tct
+
+}  // namespace

@@ -1,6 +1,6 @@
 // lutgemv_rows.cuh - the multi-row LUT-GEMV behind sqllm_lutgemv_rows_dt: a few fp16 or bf16 rows (decode of several sequences,
-// speculative-decoding verification, short prompts) in ONE launch.  Included by lutgemv_kernels.cu inside its anonymous namespace,
-// after lutgemm_batched.cuh, whose table layout, decode and row FMAs (batched::unit_fma) it shares.
+// speculative-decoding verification, short prompts) in ONE launch.  It shares the table layout, decode and row FMAs
+// (batched::unit_fma) of lutgemm_batched.cuh.
 //
 //   y[m][c] = sum_k W[k][c] x[m][k] + CSR + dense rows (+ bias),  fp16 or bf16 x [M][K] (XT), y fp32 or x's type, exact fp32
 //   codebook, fp32 sums.
@@ -20,6 +20,10 @@
 //     peers' shared memory alive until then.  No workspace, no atomics, no spin-waits: bit-reproducible, safe on several streams,
 //     CUDA-graph capturable.
 #pragma once
+#include "common.cuh"
+#include "lutgemm_batched.cuh"
+
+namespace {
 
 namespace rows {
 
@@ -59,19 +63,6 @@ struct SR {
     // + C::TAB of slack: the table is aligned up from wherever dynamic shared memory starts
     __host__ __device__ static int total(int kpad) { return C::TAB + off_red(kpad) + RW * RB * 4; }
 };
-
-__device__ __forceinline__ uint32_t cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ float4 ld_cluster_v4(uint32_t local, uint32_t rank) {  // the same shared address in CTA `rank` of the cluster
-    uint32_t a;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(local), "r"(rank));
-    float4 v;
-    asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
 
 template <int BITS, int RB, typename XT>
 __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
@@ -268,3 +259,5 @@ __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
 }
 
 }  // namespace rows
+
+}  // namespace

@@ -1,5 +1,5 @@
 // lutgemv_seq.cuh - the SEQUENCE kernel: one persistent launch runs a whole list of dependent LUT-GEMVs (a decode token's QuantLinear
-// matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Included by lutgemv_kernels.cu after lutgemv_v2.cuh;
+// matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Built on lutgemv_v2.cuh:
 // the per-position math, table builders, outlier warps (sparse3) and mailboxes are v2's (namespace v2), what is new is everything BETWEEN two GEMVs.
 //
 // Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
@@ -16,6 +16,10 @@
 //   * on several GPUs (column shards) the owner of a strip stores its tagged words into EVERY rank's arena over NVLink; the poll of the
 //     next GEMV is the whole exchange - no collective, no flag round trip (v2's exchange waits on a system-scope flag per launch).
 #pragma once
+#include "common.cuh"
+#include "lutgemv_v2.cuh"
+
+namespace {
 
 namespace seq {
 using namespace v2;
@@ -678,3 +682,5 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
 }
 
 }  // namespace seq
+
+}  // namespace

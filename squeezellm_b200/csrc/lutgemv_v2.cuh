@@ -1,5 +1,4 @@
 // lutgemv_v2.cuh - round-2 kernel: ONE fat CTA per SM, TMA-fed weight ring, one strip table at a time, optional fp16 pair tables.
-// Included by lutgemv_kernels.cu inside its anonymous namespace (shares the PTX helpers defined there).
 //
 // Same job as lutgemv_kernel (v1): y[c] (+)= sum_k LUT[c][idx(k,c)] * x[k]  (+ CSR outliers + topX dense rows), replacing
 // squeezellm/quant_cuda_kernel.cu:741-880 (LUT GEMV), :1040-1059 (SPMV_ATOMIC), :1092-1123 (DenseMatVecKernel).
@@ -20,6 +19,9 @@
 //   * x is staged whole in its own type (fp32, fp16 or bf16: the XT template parameter; 16-bit pairs are widened to fp32 in registers),
 //     the sparse warps gather it from shared memory (sparse3: nothing else of theirs goes through shared memory).
 #pragma once
+#include "common.cuh"
+
+namespace {
 
 namespace v2 {
 
@@ -1053,3 +1055,5 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
 }
 
 }  // namespace v2
+
+}  // namespace

@@ -1,5 +1,5 @@
 // seq_trace.cu - timing and per-CTA timeline of the sequence kernel (C ABI) on LLaMA-shaped decoder layers with synthetic buffers.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a [-DSQLLM_TRACE] -I include -o tests/perf/seq_trace tests/perf/seq_trace.cu squeezellm_b200/csrc/lutgemv_kernels.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a [-DSQLLM_TRACE] -I include -o tests/perf/seq_trace tests/perf/seq_trace.cu squeezellm_b200/csrc/*.cu
 //   ./seq_trace bits hidden ffn layers lut_mode(0|1) sparse(0|1) [trace_layer]
 // Prints us per token and per decoder layer; with -DSQLLM_TRACE also, for the 4 GEMVs of `trace_layer`, min / median / max over CTAs of
 // every phase stamp relative to the first stamp of that layer.

@@ -1,7 +1,7 @@
 // trace_harness.cu - timeline of a chain of back-to-back GEMVs (C ABI, PDL, CUDA graph).  Links a -DSQLLM_TRACE build of
-// lutgemv_kernels.cu.  Prints, per launch, min/max over CTAs of each phase stamp relative to the chain start (ns).
+// the library (squeezellm_b200/csrc/*.cu).  Prints, per launch, min/max over CTAs of each phase stamp relative to the chain start (ns).
 //   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -DSQLLM_TRACE -I include -o trace_harness \
-//        tests/perf/trace_harness.cu squeezellm_b200/csrc/lutgemv_kernels.cu
+//        tests/perf/trace_harness.cu squeezellm_b200/csrc/*.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -215,7 +215,7 @@ def check_call(bk, name, width, x, y, lut_fp16=False, L=None):
     if L is not bk.L[name]:
         W, Wa = torch.from_numpy(dense_w_f64(L)).cuda(), torch.from_numpy(dense_w_f64(abs_layer(L))).cuda()
     elif lut_fp16 and M == 1 and x.dtype == torch.float16 and width >= 64:
-        W, Wa = bk.w_fp16_lut(name)  # lutgemv_kernels.cu: the fp16 table serves fp16 x on layers of at least one 64-column strip
+        W, Wa = bk.w_fp16_lut(name)  # lutgemv.cu (lutgemv_fused): the fp16 table serves fp16 x on layers of at least one 64-column strip
     else:
         W, Wa = bk.W[name], bk.Wa[name]
     x64 = x.reshape(M, K).double()
