@@ -52,30 +52,26 @@ def stack_buffers(members):
                                  for m in members]).contiguous()
     else:
         out["bias"] = None
-    has_csr = [bool(m.include_sparse and hasattr(m, "rows")) for m in members]
-    if any(has_csr):
+    # each member's outliers as its own forward reads them, so that its slice of the stacked result is what it gives alone
+    sparse = [m._sparse_args() for m in members]
+    if any(s[0] is not None for s in sparse):
         rows, cols, vals, base = [torch.zeros(1, dtype=torch.int32, device=dev)], [], [], 0
-        for m, h in zip(members, has_csr):
-            if h:
-                r = m.rows.to(torch.int64)
+        for m, (r, c, v, _, _) in zip(members, sparse):
+            if r is not None:
+                r = r.to(torch.int64)
                 rows.append((r[1:] + base).to(torch.int32))
-                cols.append(m.cols)
-                vals.append(m.vals)
+                cols.append(c)
+                vals.append(v)
                 base += int(r[-1])
             else:
                 rows.append(torch.full((m.outfeatures,), base, dtype=torch.int32, device=dev))
         out["rows"] = torch.cat(rows).contiguous()
         out["cols"] = torch.cat(cols).contiguous() if cols else torch.zeros(0, dtype=torch.int32, device=dev)
         out["vals"] = torch.cat(vals).contiguous() if vals else torch.zeros(0, dtype=torch.float32, device=dev)
-    dense = [m for m in members if m.include_sparse and m.topX > 0 and hasattr(m, "full_rows")]
+    dense = [(s[3], s[4] + o) for s, o in zip(sparse, offs) if s[3] is not None]
     if dense:
-        fr, fri = [], []
-        for m, o in zip(members, offs):
-            if m.include_sparse and m.topX > 0 and hasattr(m, "full_rows"):
-                fr.append(m.full_rows)
-                fri.append(m.full_row_indices + o)
-        out["full_rows"] = torch.cat(fr, dim=1).contiguous()
-        out["full_row_indices"] = torch.cat(fri).to(torch.int32).contiguous()
+        out["full_rows"] = torch.cat([fr for fr, _ in dense], dim=1).contiguous()
+        out["full_row_indices"] = torch.cat([fri for _, fri in dense]).to(torch.int32).contiguous()
     return out
 
 
@@ -84,52 +80,50 @@ class SiblingGroup:
 
     def __init__(self, members, share_storage=True):
         self.members = list(members)
-        b = stack_buffers(self.members)
-        self.offsets = b["offsets"]
-        topX = int(b["full_rows"].shape[1]) if "full_rows" in b else 0
-        numvals = int(b["vals"].shape[0]) if "vals" in b else 0
-        layer = QuantLinearLUT(b["bits"], b["infeatures"], b["outfeatures"], b["bias"] is not None,
-                               include_sparse="rows" in b, numvals=0, topX=0)
-        layer.qweight, layer.lookup_table = b["qweight"], b["lookup_table"]
-        if b["bias"] is not None:
-            layer.bias = b["bias"]
-        if "rows" in b:
-            layer.register_buffer("rows", b["rows"])
-            layer.register_buffer("cols", b["cols"])
-            layer.register_buffer("vals", b["vals"])
-            layer.numvals = numvals
-        if topX:
-            layer.register_buffer("full_rows", b["full_rows"])
-            layer.register_buffer("full_row_indices", b["full_row_indices"])
-            layer.topX = topX
-        self.layer = layer
+        self._join(stack_buffers(self.members))
         if share_storage:  # members keep their buffer names (state_dict stays loadable/savable) as views of the stacked storage
             for m, o in zip(self.members, self.offsets):
-                m.qweight = layer.qweight[:, o:o + m.outfeatures]
-                m.lookup_table = layer.lookup_table[o:o + m.outfeatures]
+                m.qweight = self.layer.qweight[:, o:o + m.outfeatures]
+                m.lookup_table = self.layer.lookup_table[o:o + m.outfeatures]
+
+    def _join(self, stacked):
+        """Make the stacked layer from stack_buffers' result and hand every member's forward to this group, with an empty cache."""
+        self.offsets = stacked["offsets"]
+        self.layer = QuantLinearLUT.from_buffers(stacked["bits"], stacked)
         for i, m in enumerate(self.members):
             object.__setattr__(m, "_sibling_group", (self, i))
-        self._x = None
-        self._ver = None
-        self._y = None
+        self._x = self._ver = self._y = None
         self._pending = set()
         self.launches = 0  # stacked launches issued (tests / bench count these)
 
     def member_forward(self, i, x):
         if not (self._x is x and self._ver == _version(x) and i in self._pending):
-            self._y = self.layer(x)
+            self._y = self._stacked(x)
             self._x, self._ver = x, _version(x)
             self._pending = set(range(len(self.members)))
             self.launches += 1
         self._pending.discard(i)
-        y = self._y[..., self.offsets[i]:self.offsets[i + 1]]
+        y = self._member_result(i, x, self._y)
+        if not self._pending:
+            self._x = self._y = None
+        return y
+
+    def _stacked(self, x):
+        """The stacked result for x, computed once per input and shared by the members."""
+        return self.layer(x)
+
+    def _member_result(self, i, x, y):
+        """Member i's output out of the stacked result y."""
+        y = y[..., self.offsets[i]:self.offsets[i + 1]]
         if y.dtype != x.dtype and self.members[i].bias is None:
             # another member's bias promoted the stacked batch result to fp32 (out.to(dtype) + fp32 bias); this member has none, so
             # its slice is its x-dtype output + 0.0: casting back is exact and gives the dtype and bits it returns alone
             y = y.to(x.dtype)
-        if not self._pending:
-            self._x = self._y = None
         return y
+
+    def member_columns(self, i):
+        """(stacked layer, first column) of member i's weights: what QuantLinearLUT.dequantize reads."""
+        return self.layer, self.offsets[i]
 
     def dissolve(self):
         """Make every member a stand-alone layer again: buffers that are views of the stacked layer become the member's own

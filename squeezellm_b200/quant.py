@@ -180,6 +180,29 @@ class QuantLinearLUT(nn.Module):
         self.balanced = balanced
         self._sibling_group = None  # (SiblingGroup, index) once fusion.fuse_siblings has stacked this layer with its siblings
 
+    BUFFERS = ("qweight", "bias", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices")
+
+    @classmethod
+    def from_buffers(cls, bits, buffers):
+        """The layer that holds `buffers` (checkpoint names -> tensors: qweight, lookup_table and optionally bias, rows / cols /
+        vals, full_rows / full_row_indices; None and other keys are skipped) as its own buffers: no copy and no cast, so a layer
+        can hold views of a larger storage (a sibling group's members) and keep a bias in the dtype it was given.  in_features
+        and out_features come from qweight, numvals from vals, topX from full_rows; the CSR arrays make the layer sparse."""
+        b = {k: buffers[k] for k in cls.BUFFERS if buffers.get(k) is not None}
+        if "qweight" not in b or "lookup_table" not in b:
+            raise ValueError("QuantLinearLUT.from_buffers: qweight and lookup_table are required")
+        for group in (("rows", "cols", "vals"), ("full_rows", "full_row_indices")):
+            if 0 < sum(k in b for k in group) < len(group):
+                raise ValueError(f"QuantLinearLUT.from_buffers: {' / '.join(group)} come together; got only "
+                                 f"{', '.join(k for k in group if k in b)}")
+        with torch.device("meta"):  # the constructor's zero buffers are all replaced below
+            m = cls(bits, b["qweight"].shape[0] // bits * 32, b["qweight"].shape[1], "bias" in b, include_sparse="rows" in b,
+                    numvals=int(b["vals"].numel()) if "vals" in b else 0,
+                    topX=int(b["full_rows"].shape[1]) if "full_rows" in b else 0)
+        for name, t in b.items():
+            m.register_buffer(name, t)
+        return m
+
     # ------------------------------------------------------------------------------------------
     def pack2(self, linear, lookup_table, include_sparse, num_nonzero_per_thread=-1):
         """Fill the buffers from per-channel (centroids, indices) and an outlier matrix
@@ -235,13 +258,10 @@ class QuantLinearLUT(nn.Module):
     def forward(self, x):
         # a sibling member asks its group, whose stacked layer comes back here: the gradient flows through the stacked layer's
         # node and autograd's slice backward adds the members' shares
-        if self._trained:
-            params = tuple(getattr(self, n) for n in self._trained)
-            if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
-                return _QuantLinearLUTCodebookFunction.apply(x, self, self._trained, *params)
-            return self._forward_impl(x)
-        if self._sibling_group is None and torch.is_grad_enabled() and x.requires_grad:
-            return _QuantLinearLUTFunction.apply(x, self)
+        params = tuple(getattr(self, n) for n in self._trained)
+        wants_dx = x.requires_grad and (bool(self._trained) or self._sibling_group is None)
+        if torch.is_grad_enabled() and (wants_dx or any(p.requires_grad for p in params)):
+            return _QuantLinearLUTFunction.apply(x, self, self._trained, *params)
         return self._forward_impl(x)
 
     TRAINABLE = ("lookup_table", "vals", "full_rows", "bias")
@@ -301,7 +321,7 @@ class QuantLinearLUT(nn.Module):
         col0, layer = 0, self
         if self._sibling_group is not None:
             group, index = self._sibling_group
-            col0, layer = group.offsets[index], group.layer
+            layer, col0 = group.member_columns(index)
         rows, cols, vals, fr, fri = (t.detach() if t is not None else None for t in layer._sparse_args())
         return quant_cuda.dequantize(layer.qweight, layer.lookup_table.detach(), layer.bits, rows, cols, vals, fr, fri,
                                      dtype=dtype, col0=col0, ncols=self.outfeatures)
@@ -319,42 +339,44 @@ class QuantLinearLUT(nn.Module):
         if self._sibling_group is not None:
             group, index = self._sibling_group
             return group.member_forward(index, x)
-        dev = self.qweight.device
-        if x.shape[-1] == x.numel():
-            outshape = list(x.shape)
-            outshape[-1] = self.outfeatures
-            rows, cols, vals, fr, fri = self._sparse_args()
-            if QuantLinearLUT.use_fused and x.dtype in (torch.float16, torch.float32, torch.bfloat16) and self._fused_fits(fr):
-                y = quant_cuda.lutgemv_fused(_aligned(x), self.qweight, self.lookup_table, self.bits,
-                                             self.bias, rows, cols, vals, fr, fri)
-                return y.reshape(outshape)
-            # reference sequence (quant.py:213-312)
-            y = self.bias.clone() if self.bias is not None else torch.zeros((self.outfeatures), device=dev, dtype=torch.float32)
-            dtype = x.dtype
-            x = _aligned(x.float())
-            self._dispatch(x, y, batched=False)
-            return y.to(dtype).reshape(outshape)
         out_shape = x.shape[:-1] + (self.outfeatures,)
-        x = x.reshape(-1, x.shape[-1])
-        tc_min = {torch.float16: QuantLinearLUT.TC_MIN_ROWS, torch.bfloat16: QuantLinearLUT.BF16_TC_MIN_ROWS,
-                  torch.float32: QuantLinearLUT.FP32_TC_MIN_ROWS}.get(x.dtype)
-        if QuantLinearLUT.use_fused and tc_min is not None and x.shape[0] >= tc_min:
-            rows, cols, vals, fr, fri = self._sparse_args()
-            tc_fn = quant_cuda.lutgemm_fused_f32 if x.dtype == torch.float32 else quant_cuda.lutgemm_fused
-            out = tc_fn(_aligned(x), self.qweight, self.lookup_table, self.bits, None, rows, cols, vals, fr, fri).reshape(out_shape)
-            return out + self.bias if self.bias is not None else out  # the bias is added as below: same dtype and rounding
-        rows_max = {torch.float16: QuantLinearLUT.ROWS_MAX, torch.bfloat16: QuantLinearLUT.BF16_ROWS_MAX}.get(x.dtype)
-        if QuantLinearLUT.use_fused and rows_max is not None and 2 <= x.shape[0] <= rows_max and self._rows_fits():
-            rows, cols, vals, fr, fri = self._sparse_args()
-            rows_fn = quant_cuda.lutgemv_rows if x.dtype == torch.float16 else quant_cuda.lutgemv_rows_bf16
-            out = rows_fn(_aligned(x), self.qweight, self.lookup_table, self.bits, None, rows, cols, vals, fr, fri).reshape(out_shape)
-            return out + self.bias if self.bias is not None else out
-        out = torch.zeros((x.shape[0], self.outfeatures), device=dev, dtype=torch.float32)
-        dtype = x.dtype
-        x = _aligned(x.float())
-        self._dispatch(x, out, batched=True)
-        out = out.to(dtype).reshape(out_shape)
-        return out + self.bias if self.bias is not None else out
+        batched = x.shape[-1] != x.numel()
+        if batched:
+            x = x.reshape(-1, x.shape[-1])
+        rows, cols, vals, fr, fri = self._sparse_args()
+        launch = self._fused_launch(x, batched, fr) if QuantLinearLUT.use_fused else None
+        if launch is None:
+            out = self._reference_forward(x, batched)
+        else:  # one row: the bias inside the launch's sum; batches: added below, in the same dtype and rounding as the reference's
+            out = launch(_aligned(x), self.qweight, self.lookup_table, self.bits, None if batched else self.bias,
+                         rows, cols, vals, fr, fri)
+        out = out.reshape(out_shape)
+        return out + self.bias if batched and self.bias is not None else out
+
+    def _fused_launch(self, x, batched, full_rows):
+        """The fused binding that runs x (one row, or [M, K]), or None where the reference's symbols run it."""
+        if not batched:
+            fits = x.dtype in (torch.float16, torch.float32, torch.bfloat16) and self._fused_fits(full_rows)
+            return quant_cuda.lutgemv_fused if fits else None
+        M, cls = x.shape[0], QuantLinearLUT
+        tc_min = {torch.float16: cls.TC_MIN_ROWS, torch.bfloat16: cls.BF16_TC_MIN_ROWS, torch.float32: cls.FP32_TC_MIN_ROWS}.get(x.dtype)
+        if tc_min is not None and M >= tc_min:
+            return quant_cuda.lutgemm_fused_f32 if x.dtype == torch.float32 else quant_cuda.lutgemm_fused
+        rows_max = {torch.float16: cls.ROWS_MAX, torch.bfloat16: cls.BF16_ROWS_MAX}.get(x.dtype)
+        if rows_max is not None and 2 <= M <= rows_max and self._rows_fits():
+            return quant_cuda.lutgemv_rows if x.dtype == torch.float16 else quant_cuda.lutgemv_rows_bf16
+        return None
+
+    def _reference_forward(self, x, batched):
+        """The reference's sequence (quant.py:213-379): x in fp32, one of the 12 symbols into an fp32 output that one row starts
+        from the bias and a batch from zero, then the output in x's dtype."""
+        if batched or self.bias is None:
+            shape = (x.shape[0], self.outfeatures) if batched else (self.outfeatures,)
+            y = torch.zeros(shape, device=self.qweight.device, dtype=torch.float32)
+        else:
+            y = self.bias.clone()
+        self._dispatch(_aligned(x.float()), y, batched)
+        return y.to(x.dtype)
 
     def _dispatch(self, x, y, batched):
         """Pick 1 of the 12 quant_cuda symbols by (bits, batched, dense|spmv|hybrid) - reference quant.py:222-309,320-379."""
@@ -373,42 +395,17 @@ class QuantLinearLUT(nn.Module):
 
 
 class _QuantLinearLUTFunction(torch.autograd.Function):
-    """y = QuantLinearLUT._forward_impl(x) with dx = dy . W^T.  The layer's buffers are constants: only x gets a gradient (no
-    gradient for the codebook, the outliers or the bias), and nothing is saved for backward but the layer itself."""
-
-    @staticmethod
-    def forward(ctx, x, layer):
-        ctx.layer = layer
-        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
-        # the buffers are read again at backward time: remember their versions, so that an in-place change in between (a weight
-        # reload) raises instead of silently giving the gradient of the new weights
-        ctx.versions = [(t, t._version) for t in layer._grad_buffers()]
-        return layer._forward_impl(x)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, dy):
-        layer = ctx.layer
-        now = layer._grad_buffers()
-        if len(now) != len(ctx.versions) or any(t is not u or t._version != v for (t, v), u in zip(ctx.versions, now)):
-            raise RuntimeError("QuantLinearLUT: the layer's buffers were modified or replaced between forward and backward; "
-                               "the input gradient would use the new weights")
-        dy = dy.reshape(-1, layer.outfeatures)
-        if dy.shape[0] == 0:
-            return torch.zeros(ctx.x_shape, dtype=ctx.x_dtype, device=dy.device), None
-        dx = layer._input_grad(dy)
-        return dx.to(ctx.x_dtype).reshape(ctx.x_shape), None
-
-
-class _QuantLinearLUTCodebookFunction(torch.autograd.Function):
-    """y = QuantLinearLUT._forward_impl(x) for a layer with trained tensors (QuantLinearLUT.train_codebook): dx = dy . W^T as in
-    _QuantLinearLUTFunction, the codebook / CSR-value / dense-row gradients from G = x^T . dy in one quant_cuda.lut_grad launch,
-    dbias = sum of dy over the rows.  x is saved only when one of the first three is wanted."""
+    """y = QuantLinearLUT._forward_impl(x) with dx = dy . W^T.  `names` are the layer's trained tensors
+    (QuantLinearLUT.train_codebook) and `params` their values: the codebook / CSR-value / dense-row gradients come from
+    G = x^T . dy in one quant_cuda.lut_grad launch, dbias = sum of dy over the rows.  Without trained tensors the buffers are
+    constants and only x gets a gradient.  x is saved only when one of the first three is wanted."""
 
     @staticmethod
     def forward(ctx, x, layer, names, *params):
         ctx.layer, ctx.names = layer, names
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        # the buffers are read again at backward time: remember their versions, so that an in-place change in between (a weight
+        # reload) raises instead of silently giving the gradient of the new weights
         ctx.versions = [(t, t._version) for t in layer._grad_buffers() + ((layer.bias,) if "bias" in names else ())]
         ctx.grid_names = tuple(n for i, n in enumerate(names) if n != "bias" and ctx.needs_input_grad[3 + i])
         if ctx.grid_names:

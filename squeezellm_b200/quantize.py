@@ -119,20 +119,15 @@ def quantize_linear(linear, fisher, bits, threshold=None, sensitivity=0.0):
         dense, outliers = weight.detach().float(), None
     lut, labels = kmeans_codebook(dense, fisher * (dense != 0), bits)
 
-    q = QuantLinearLUT(bits, in_f, out_f, linear.bias is not None, include_sparse=sparse, topX=0).to(weight.device)
-    q.lookup_table = lut
-    q.qweight = quant_cuda.pack_indices(labels, bits)
-    if linear.bias is not None:
-        q.bias = linear.bias.detach().clone()
+    buffers = {"qweight": quant_cuda.pack_indices(labels, bits), "lookup_table": lut,
+               "bias": linear.bias.detach().clone() if linear.bias is not None else None}
     if sparse:
         zero = lut.gather(1, lut.abs().argmin(dim=1, keepdim=True))
         outliers = torch.where(outliers != 0, outliers - zero, outliers)
         csr = outliers.to_sparse(layout=torch.sparse_csr)
-        q.register_buffer("rows", csr.crow_indices().to(torch.int32))
-        q.register_buffer("cols", csr.col_indices().to(torch.int32))
-        q.register_buffer("vals", csr.values().to(torch.float32))
-        q.numvals = int(q.vals.shape[0])
-    return q
+        buffers.update(rows=csr.crow_indices().to(torch.int32), cols=csr.col_indices().to(torch.int32),
+                       vals=csr.values().to(torch.float32))
+    return QuantLinearLUT.from_buffers(bits, buffers)
 
 
 def _set_module(model, name, module):

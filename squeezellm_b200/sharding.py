@@ -19,6 +19,9 @@ local compute - the product path always uses the CUDA module.
 import torch
 import torch.nn as nn
 
+from .fusion import SiblingGroup, stack_buffers
+from .quant import QuantLinearLUT
+
 
 def shard_bounds(outfeatures, world, align=4):
     """Contiguous, `align`-aligned, as-equal-as-possible output ranges: list of (c0, c1), len == world."""
@@ -35,16 +38,18 @@ def shard_bounds(outfeatures, world, align=4):
 
 
 def shard_state(state, c0, c1):
-    """Slice a QuantLinearLUT state dict (reference buffer names, squeezellm/quant.py:48-95) to channels [c0, c1)."""
-    out = {"qweight": state["qweight"][:, c0:c1].contiguous(), "lookup_table": state["lookup_table"][c0:c1].contiguous()}
+    """Slice a QuantLinearLUT state dict (reference buffer names, squeezellm/quant.py:48-95) to channels [c0, c1).  Every tensor
+    of the result is a contiguous copy of its own, in the dtype of the layer's buffer (int32 indices, fp32 values), as
+    load_state_dict into a fresh layer would give it: a shard keeps no view of the full layer's storage."""
+    out = {"qweight": state["qweight"][:, c0:c1], "lookup_table": state["lookup_table"][c0:c1]}
     if state.get("bias") is not None:
-        out["bias"] = state["bias"][c0:c1].contiguous()
+        out["bias"] = state["bias"][c0:c1]
     if state.get("rows") is not None:
         rows = state["rows"]
         a, b = int(rows[c0]), int(rows[c1])
-        out["rows"] = (rows[c0:c1 + 1] - rows[c0]).to(torch.int32).contiguous()
-        out["cols"] = state["cols"][a:b].contiguous()
-        out["vals"] = state["vals"][a:b].contiguous()
+        out["rows"] = rows[c0:c1 + 1] - rows[c0]
+        out["cols"] = state["cols"][a:b]
+        out["vals"] = state["vals"][a:b]
     if state.get("full_rows") is not None:
         idx = state["full_row_indices"]
         keep = torch.nonzero((idx >= c0) & (idx < c1)).flatten()
@@ -53,8 +58,9 @@ def shard_state(state, c0, c1):
         fi = torch.zeros_like(idx)
         fr[:, :len(keep)] = state["full_rows"][:, keep]
         fi[:len(keep)] = (idx[keep] - c0).to(idx.dtype)
-        out["full_rows"], out["full_row_indices"] = fr.contiguous(), fi.contiguous()
-    return out
+        out["full_rows"], out["full_row_indices"] = fr, fi
+    return {k: v.to(torch.float32 if v.is_floating_point() else torch.int32, memory_format=torch.contiguous_format, copy=True)
+            for k, v in out.items()}
 
 
 class ShardedQuantLinearLUT(nn.Module):
@@ -69,12 +75,14 @@ class ShardedQuantLinearLUT(nn.Module):
 
     @classmethod
     def from_full(cls, full_state, bits, infeatures, outfeatures, rank, world, include_sparse, topX, device, group=None):
-        from .quant import QuantLinearLUT
+        """Rank `rank`'s shard of the layer whose state dict is `full_state` (QuantLinearLUT.from_buffers on shard_state).
+        `infeatures`, `include_sparse` and `topX` must be those of full_state's buffers (CSR arrays: include_sparse)."""
         c0, c1 = shard_bounds(outfeatures, world)[rank]
-        st = shard_state(full_state, c0, c1)
-        m = QuantLinearLUT(bits, infeatures, c1 - c0, "bias" in st, include_sparse=include_sparse,
-                           numvals=int(st["vals"].numel()) if "vals" in st else 0, topX=topX)
-        m.load_state_dict(st, strict=False)
+        m = QuantLinearLUT.from_buffers(bits, shard_state(full_state, c0, c1))
+        if (m.infeatures, m.include_sparse, m.topX) != (infeatures, bool(include_sparse), topX):
+            raise ValueError(f"ShardedQuantLinearLUT.from_full: full_state holds a layer with in_features={m.infeatures}, "
+                             f"include_sparse={m.include_sparse}, topX={m.topX}; the arguments say {infeatures}, "
+                             f"{bool(include_sparse)}, {topX}")
         return cls(m.to(device), outfeatures, c0, c1, group)
 
     def forward(self, x):
@@ -214,21 +222,18 @@ class PeerArena:
         return arena, int(hdl.buffer_ptrs_dev)
 
 
-class ShardedSiblingGroup:
+class ShardedSiblingGroup(SiblingGroup):
     """Column shards of a set of sibling layers (same input) run as ONE stacked launch per rank + ONE exchange.  Gives no
     gradient: the exchange runs outside autograd.
 
     Built from the full (unsharded) QuantLinearLUT members: every rank keeps columns [rank*w, (rank+1)*w) of each member
-    (`shard_state`), stacks those shards along N (`fusion.stack_buffers`) and answers the members' `forward(x)` through the
-    same one-result cache protocol as `fusion.SiblingGroup` - so model code is unchanged: `q_proj(x)`, `k_proj(x)`,
-    `v_proj(x)` return FULL-width vectors on every rank.  The exchange is `PeerExchange` (in-kernel stores over NVLink, no
-    collective) when one is given, else one NCCL all-reduce per stacked launch (`exchange_stacked`).
+    (`shard_state`), stacks those shards along N (`fusion.stack_buffers`) and answers the members' `forward(x)` through
+    `fusion.SiblingGroup`'s one-result cache - so model code is unchanged: `q_proj(x)`, `k_proj(x)`, `v_proj(x)` return
+    FULL-width vectors on every rank.  The exchange is `PeerExchange` (in-kernel stores over NVLink, no collective) when one is
+    given, else one NCCL all-reduce per stacked launch (`exchange_stacked`).
     A single layer (o_proj, down_proj) is simply a group of one.  `compute` lets CPU tests stand in for the CUDA launch."""
 
     def __init__(self, members, rank, world, name, peer=None, group=None, compute=None):
-        from .fusion import stack_buffers, _version
-        from .quant import QuantLinearLUT
-        self._version = _version
         self.members, self.rank, self.world, self.name, self.peer, self.pg, self.compute = list(members), rank, world, name, peer, group, compute
         n_full = {m.outfeatures for m in self.members}
         if len(n_full) != 1:
@@ -238,28 +243,10 @@ class ShardedSiblingGroup:
         if (c1 - c0) * world != self.n_full:
             raise ValueError(f"out_features={self.n_full} does not split into {world} equal 4-aligned shards")
         self.w = c1 - c0
-        shards = []
-        for m in self.members:
-            st = shard_state({k: v for k, v in m.state_dict().items()}, c0, c1)
-            s = QuantLinearLUT(m.bits, m.infeatures, self.w, "bias" in st, include_sparse="rows" in st,
-                               numvals=int(st["vals"].numel()) if "vals" in st else 0, topX=int(st["full_rows"].shape[1]) if "full_rows" in st else 0)
-            s.load_state_dict(st, strict=False)
-            shards.append(s.to(m.qweight.device))
-        b = stack_buffers(shards)
-        layer = QuantLinearLUT(b["bits"], b["infeatures"], b["outfeatures"], b["bias"] is not None, include_sparse="rows" in b)
-        layer.qweight, layer.lookup_table = b["qweight"], b["lookup_table"]
-        if b["bias"] is not None:
-            layer.bias = b["bias"]
-        if "rows" in b:
-            for k in ("rows", "cols", "vals"):
-                layer.register_buffer(k, b[k])
-            layer.numvals = int(b["vals"].numel())
-        if "full_rows" in b:
-            layer.register_buffer("full_rows", b["full_rows"])
-            layer.register_buffer("full_row_indices", b["full_row_indices"])
-            layer.topX = int(b["full_rows"].shape[1])
-        self.layer = layer
-        for i, (m, o) in enumerate(zip(self.members, b["offsets"])):
+        shards = [QuantLinearLUT.from_buffers(m.bits, shard_state(m.state_dict(), c0, c1)) for m in self.members]
+        self._join(stack_buffers(shards))
+        layer = self.layer
+        for m, o in zip(self.members, self.offsets):
             # the member keeps its buffer names but now holds this rank's shard (views of the stacked storage)
             m.qweight = layer.qweight[:, o:o + self.w]
             m.lookup_table = layer.lookup_table[o:o + self.w]
@@ -269,12 +256,16 @@ class ShardedSiblingGroup:
             m.include_sparse, m.numvals, m.topX = False, 0, 0
             if m.bias is not None:
                 m.bias = layer.bias[o:o + self.w]
-            object.__setattr__(m, "_sibling_group", (self, i))
-        self._x = self._ver = self._y = None
-        self._pending = set()
-        self.launches = 0
 
-    def _run(self, x):
+    def member_columns(self, i):
+        raise NotImplementedError("QuantLinearLUT.dequantize: this layer is column-sharded (sharding.shard_model) and holds only "
+                                  "this rank's columns; dequantize the full layer before sharding it")
+
+    def dissolve(self):
+        raise NotImplementedError("ShardedSiblingGroup.dissolve: its members hold only this rank's columns and cannot stand "
+                                  "alone again; rebuild the full layers from the checkpoint instead")
+
+    def _stacked(self, x):
         nm = len(self.members)
         if self.compute is not None:
             y = self.compute(self.layer, x)
@@ -284,22 +275,14 @@ class ShardedSiblingGroup:
             y = self.layer._forward_impl(x)  # no autograd node: the exchange carries no gradient
         return exchange_stacked(y, nm, self.rank, self.world, group=self.pg)            # [..., members, n_full]
 
-    def member_forward(self, i, x):
-        if not (self._x is x and self._ver == self._version(x) and i in self._pending):
-            self._y = self._run(x)
-            self._x, self._ver = x, self._version(x)
-            self._pending = set(range(len(self.members)))
-            self.launches += 1
-        self._pending.discard(i)
-        y = self._y[..., i, :]
+    def _member_result(self, i, x, y):
+        y = y[..., i, :]
         if self.peer is not None and self.compute is None:
             # the peer path returns a view of a persistent arena slot that the next call of this layer overwrites (remotely, from
             # other ranks): hand out a private copy, like nn.Linear would (N elements - nothing next to the matvec)
             y = y.clone()
         if y.dim() < x.dim():                      # decode-shaped input [1, 1, K] -> [1, 1, N] like QuantLinearLUT.forward
             y = y.reshape(x.shape[:-1] + (self.n_full,))
-        if not self._pending:
-            self._x = self._y = None
         return y
 
 
@@ -308,7 +291,6 @@ def shard_model(model, rank, world, peer=None, group=None, siblings=(("q_proj", 
     ShardedSiblingGroup each, every other QuantLinearLUT a group of one.  Every rank must call it on the same model.
     Returns the groups (their `.launches` count stacked launches).  Exchange names alternate so that consecutive launches
     never share a destination (PeerExchange's requirement)."""
-    from .quant import QuantLinearLUT
     groups = []
     for mod_name, mod in model.named_modules():
         taken = set()

@@ -14,7 +14,7 @@ import torch
 
 from backward_ref import backward_and_abs_sum, backward_f64
 from test_error_bound_host import SHAPES
-from util import OUT_ROUNDING, Args, bound_ratio, load_lib, make_activations, orc, to_torch
+from util import OUT_ROUNDING, Args, bound_ratio, load_lib, make_activations, orc, quant_layer, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -308,16 +308,8 @@ def test_three_streams_at_once(lib):
 
 # ---- module level -------------------------------------------------------------------------------------------------------
 def _module(L, bias=False):
-    from squeezellm_b200.quant import QuantLinearLUT
-    K, N, bits = L["infeatures"], L["outfeatures"], L["bits"]
-    topX = 0 if L.get("full_rows") is None else L["full_rows"].shape[1]
-    m = QuantLinearLUT(bits, K, N, bias, include_sparse=L.get("rows") is not None,
-                       numvals=0 if L.get("vals") is None else len(L["vals"]), topX=topX)
-    st = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}
-    if bias:
-        st["bias"] = torch.from_numpy(np.random.default_rng(K).standard_normal(N).astype(np.float32))
-    m.load_state_dict(st, strict=False)
-    return m.cuda()
+    K, N = L["infeatures"], L["outfeatures"]
+    return quant_layer(L, bias=np.random.default_rng(K).standard_normal(N).astype(np.float32) if bias else None).cuda()
 
 
 @pytest.fixture

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import Args, REL_TOL, TIGHT_TOL, late_owned_strips, load_lib, orc, rel_err, to_torch
+from util import Args, REL_TOL, TIGHT_TOL, late_owned_strips, load_lib, orc, quant_layer, rel_err, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -224,14 +224,7 @@ def test_dense_rows_llama_qkv_shape(lib, topx):
 # ---------------------------------------------------------------------------------------------------------------------------------
 # B. QuantLinearLUT falls back to the 12 symbols for layers the fused launch does not take
 def _module(L):
-    from squeezellm_b200.quant import QuantLinearLUT
-    sparse = L.get("rows") is not None
-    topx = int(L["full_rows"].shape[1]) if L.get("full_rows") is not None else 0
-    m = QuantLinearLUT(L["bits"], L["infeatures"], L["outfeatures"], L.get("bias") is not None, include_sparse=sparse,
-                       numvals=len(L["vals"]) if sparse else 0, topX=topx)
-    sd = m.state_dict()
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in sd}, strict=False)
-    return m.cuda()
+    return quant_layer(L).cuda()
 
 
 @pytest.mark.parametrize("K,N,topx", [(64, 262208, 4), (512, 1000, 129)], ids=["out262208", "topx129"])

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from test_gpu_parity import IDS, SHAPES
-from util import abs_sum, bound_ratio, orc, to_torch
+from util import abs_sum, bound_ratio, orc, quant_layer, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -247,12 +247,9 @@ def test_against_the_forward_oracle(qc, shape):
 
 # ---- module ---------------------------------------------------------------------------------------------------------------------
 def _module(kind, bits=4, K=256, N=192, seed=0):
-    from squeezellm_b200.quant import QuantLinearLUT
     sp, topx = {"plain": (0.0, 0), "biased": (0.0, 0), "sparse": (0.02, 0), "hybrid": (0.02, 6)}[kind]
     L = orc.make_layer(bits, K, N, sparsity=sp, topX=topx, seed=seed, nonzero_full_rows=True, bias=kind == "biased")
-    m = QuantLinearLUT(bits, K, N, kind == "biased", include_sparse=sp > 0, numvals=len(L["vals"]) if sp else 0, topX=topx)
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()})
-    return L, m.cuda()
+    return L, quant_layer(L).cuda()
 
 
 @pytest.mark.parametrize("kind", ["plain", "biased", "sparse", "hybrid"])

@@ -7,17 +7,7 @@ import torch
 
 from squeezellm_b200.quant import QuantLinearLUT
 from squeezellm_b200 import fusion
-from util import OUT_ROUNDING, abs_sum, bound_ratio, make_activations, orc
-
-
-def _member(L, bias=False):
-    sparse = L.get("rows") is not None
-    topx = int(L["full_rows"].shape[1]) if L.get("full_rows") is not None else 0
-    m = QuantLinearLUT(L["bits"], L["infeatures"], L["outfeatures"], bias, include_sparse=sparse,
-                       numvals=len(L["vals"]) if sparse else 0, topX=topx)
-    sd = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}
-    m.load_state_dict(sd, strict=False)
-    return m
+from util import OUT_ROUNDING, abs_sum, bound_ratio, layer_as_read, make_activations, orc, quant_layer
 
 
 def _layers(bits, K, widths, sparsity, topx, bias=False):
@@ -25,29 +15,45 @@ def _layers(bits, K, widths, sparsity, topx, bias=False):
                            nonzero_full_rows=True, bias=bias) for i, n in enumerate(widths)]
 
 
-@pytest.mark.parametrize("bits", [3, 4])
-def test_stacked_buffers_equal_members_side_by_side(bits):
-    """oracle(stacked layer) == concat(oracle(member_i)) exactly: same packed words, LUT rows, CSR entries, dense rows.
-    Member 1 has no outliers at all (mixed groups must still stack)."""
-    K, widths = 256, [64, 128, 192]
-    Ls = _layers(bits, K, widths, 0.02, 3, bias=True)
-    ms = [_member(L, bias=True) for L in Ls]
+def _rowless_dense_member(bits, K, N, seed):
+    """include_sparse and dense rows but no CSR arrays (make_quant_lut with numvals 0): its forward reads no outliers at all."""
+    L = orc.make_layer(bits, K, N, topX=3, seed=seed, nonzero_full_rows=True, bias=True)
+    m = QuantLinearLUT(bits, K, N, True, include_sparse=True, numvals=0, topX=3)
+    m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray)})
+    return m
+
+
+STACK_CASES = [(3, "mixed"), (4, "mixed"), (3, "csr-next-to-rowless-dense"), (4, "csr-next-to-rowless-dense")]
+
+
+@pytest.mark.parametrize("bits,group", STACK_CASES, ids=["3", "4", "3-csr-next-to-rowless-dense", "4-csr-next-to-rowless-dense"])
+def test_stacked_buffers_equal_members_side_by_side(bits, group):
+    """oracle(stacked layer) == concat(oracle(member_i as its own forward reads it)) exactly: same packed words, LUT rows, CSR
+    entries, dense rows.  mixed: member 1 has no outliers at all (mixed groups must still stack).  csr-next-to-rowless-dense: a
+    member with CSR and dense rows next to one whose dense rows its forward ignores (no CSR arrays)."""
+    K = 256
+    if group == "mixed":
+        ms = [quant_layer(L) for L in _layers(bits, K, [64, 128, 192], 0.02, 3, bias=True)]
+    else:
+        ms = [quant_layer(orc.make_layer(bits, K, 64, sparsity=0.02, topX=3, seed=31, nonzero_full_rows=True, bias=True)),
+              _rowless_dense_member(bits, K, 128, seed=32)]
+    n = sum(m.outfeatures for m in ms)
     b = fusion.stack_buffers(ms)
-    assert b["offsets"] == [0, 64, 192, 384] and b["qweight"].shape == (K // 32 * bits, 384)
-    stacked = dict(bits=bits, infeatures=K, outfeatures=384, bias=None,
+    assert b["offsets"] == list(np.cumsum([0] + [m.outfeatures for m in ms])) and b["qweight"].shape == (K // 32 * bits, n)
+    stacked = dict(bits=bits, infeatures=K, outfeatures=n, bias=None,
                    **{k: b[k].numpy() for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices")})
     x = orc.make_vec(K, seed=3)
     got = orc.forward_f64(stacked, x)
-    want = np.concatenate([orc.forward_f64(L, x) for L in Ls], axis=1)
+    want = np.concatenate([orc.forward_f64(layer_as_read(m), x) for m in ms], axis=1)
     assert np.array_equal(got, want)
-    assert torch.equal(b["bias"], torch.cat([torch.from_numpy(L["bias"]) for L in Ls]))
-    assert b["rows"][-1].item() == len(b["cols"]) == sum(len(L["vals"]) for L in Ls if L.get("vals") is not None)
+    assert torch.equal(b["bias"], torch.cat([m.bias for m in ms]))
+    assert b["rows"][-1].item() == len(b["cols"]) == sum(len(m._sparse_args()[2]) for m in ms if m._sparse_args()[2] is not None)
 
 
 def test_result_cache_protocol():
     """One stacked call per distinct input; each member consumes once; a new / modified x recomputes."""
     K = 64
-    ms = [_member(orc.make_layer(4, K, n, seed=n)) for n in (32, 64)]
+    ms = [quant_layer(orc.make_layer(4, K, n, seed=n)) for n in (32, 64)]
     g = fusion.SiblingGroup(ms)
     # members expose their buffers as views of the stacked storage (state_dict keys unchanged)
     assert ms[1].qweight.data_ptr() == g.layer.qweight.data_ptr() + 32 * 4 and not ms[1].qweight.is_contiguous()
@@ -84,14 +90,14 @@ def test_fuse_siblings_walks_llama_like_modules():
         def __init__(self):
             super().__init__()
             for n in ("q_proj", "k_proj", "v_proj", "o_proj"):
-                setattr(self, n, _member(orc.make_layer(4, 64, 64, seed=5)))
+                setattr(self, n, quant_layer(orc.make_layer(4, 64, 64, seed=5)))
 
     class Mlp(torch.nn.Module):
         def __init__(self):
             super().__init__()
-            self.gate_proj = _member(orc.make_layer(4, 64, 128, seed=6))
-            self.up_proj = _member(orc.make_layer(4, 64, 128, seed=7))
-            self.down_proj = _member(orc.make_layer(4, 128, 64, seed=8))
+            self.gate_proj = quant_layer(orc.make_layer(4, 64, 128, seed=6))
+            self.up_proj = quant_layer(orc.make_layer(4, 64, 128, seed=7))
+            self.down_proj = quant_layer(orc.make_layer(4, 128, 64, seed=8))
 
     class Block(torch.nn.Module):
         def __init__(self):
@@ -137,7 +143,7 @@ def test_stacked_launch_matches_members(bits, K, widths, sp, topx, bias):
     """One row (the fused decode launch, bias inside the sum) and two rows (the multi-row launch, bias added after the rounding):
     every member's slice of the stacked launch against the fp64 oracle per element (bound_ratio), and next to its own launch."""
     Ls = _layers(bits, K, widths, sp, topx, bias=bias)
-    ms = [_member(L, bias=bias).cuda() for L in Ls]
+    ms = [quant_layer(L).cuda() for L in Ls]
     x = torch.from_numpy(orc.make_vec(K, seed=12)).cuda().half().reshape(1, 1, K)
     alone = [m(x) for m in ms]
     g = fusion.SiblingGroup(ms)
@@ -178,8 +184,8 @@ def test_member_without_bias_keeps_its_dtype_in_a_group_with_biases(mixed_bias_l
     within the bound; on the launches whose bits do not depend on the call (the multi-row and the tensor-core LUT-GEMM) the same
     bits as alone."""
     Ls = mixed_bias_layers
-    alone = [_member(L, bias=L["bias"] is not None).cuda() for L in Ls]
-    ms = [_member(L, bias=L["bias"] is not None).cuda() for L in Ls]
+    alone = [quant_layer(L).cuda() for L in Ls]
+    ms = [quant_layer(L).cuda() for L in Ls]
     g = fusion.SiblingGroup(ms)
     x = torch.from_numpy(make_activations(1024, M, seed=M)).cuda().to(dtype).reshape(1, M, 1024)
     x_np = x.float().cpu().numpy().reshape(M, 1024)

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN, Args, REL_TOL, TIGHT_TOL, load_lib, orc, rel_err, sample_idx, to_torch
+from util import GOLDEN, Args, REL_TOL, TIGHT_TOL, load_lib, orc, quant_layer, rel_err, sample_idx, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -214,10 +214,7 @@ def test_module_forward_matches_reference_sequence(qc):
     for bits, sparse, topx in [(4, False, 0), (3, True, 0), (4, True, 10)]:
         K, N = 4096, 4096
         L = orc.make_layer(bits, K, N, sparsity=0.0045 if sparse else 0.0, topX=topx, seed=9, nonzero_full_rows=True)
-        m = QuantLinearLUT(bits, K, N, False, include_sparse=sparse, numvals=len(L["vals"]) if sparse else 0, topX=topx)
-        sd = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}
-        m.load_state_dict(sd, strict=False)
-        m = m.cuda()
+        m = quant_layer(L).cuda()
         x = torch.from_numpy(orc.make_vec(K, seed=8)).cuda().half().reshape(1, 1, K)
         QuantLinearLUT.use_fused = True
         y_f = m(x)

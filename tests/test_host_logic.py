@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn as nn
 
-from util import orc, rel_err, TIGHT_TOL
+from util import layer_as_read, orc, quant_layer, rel_err, TIGHT_TOL
 
 
 def test_quantlinearlut_buffers_match_reference_format():
@@ -25,6 +25,29 @@ def test_quantlinearlut_buffers_match_reference_format():
         QuantLinearLUT(2, 256, 128, False)
     with pytest.raises(NotImplementedError, match="balanced"):
         QuantLinearLUT(4, 256, 128, False, include_sparse=True, numvals=5, balanced=True)
+
+
+@pytest.mark.parametrize("kind", ["dense", "csr", "csr+dense-rows", "biased"])
+def test_from_buffers_equals_constructor_and_load_state_dict(kind):
+    """QuantLinearLUT.from_buffers: the state_dict (keys, dtypes, values) and attributes of the constructor + load_state_dict,
+    holding the given tensors themselves (no copy)."""
+    from squeezellm_b200.quant import QuantLinearLUT
+    sp, topx = {"dense": (0.0, 0), "csr": (0.02, 0), "csr+dense-rows": (0.02, 5), "biased": (0.02, 5)}[kind]
+    L = orc.make_layer(3, 256, 128, sparsity=sp, topX=topx, seed=6, nonzero_full_rows=True, bias=kind == "biased")
+    buffers = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray)}
+    want = QuantLinearLUT(3, 256, 128, L["bias"] is not None, include_sparse=sp > 0, numvals=len(L["vals"]) if sp else 0, topX=topx)
+    want.load_state_dict(buffers)
+    got = QuantLinearLUT.from_buffers(3, buffers)
+    sd, sd_want = got.state_dict(), want.state_dict()
+    assert list(sd) == list(sd_want)
+    assert all(sd[k].dtype == sd_want[k].dtype and torch.equal(sd[k], sd_want[k]) for k in sd)
+    attrs = ("infeatures", "outfeatures", "bits", "include_sparse", "include_bias", "numvals", "topX")
+    assert [getattr(got, a) for a in attrs] == [getattr(want, a) for a in attrs]
+    assert all(getattr(got, k) is t for k, t in buffers.items())
+    for missing in ("qweight", "lookup_table", "rows", "vals", "full_row_indices"):  # incomplete sets fail here, not at a launch
+        if missing in buffers:
+            with pytest.raises((ValueError, KeyError)):
+                QuantLinearLUT.from_buffers(3, {k: t for k, t in buffers.items() if k != missing})
 
 
 def test_make_quant_lut_replaces_named_linears_like_the_reference():
@@ -79,6 +102,56 @@ def test_shard_bounds_and_state_reassemble():
         Ls = dict(bits=4, infeatures=256, outfeatures=c1 - c0, **{k: v.numpy() for k, v in s.items()})
         got[:, c0:c1] = orc.forward_f64(Ls, x, mul_init=Ls["bias"][None])
     assert np.allclose(got, want, rtol=1e-12, atol=1e-12)
+
+
+def _csr_in_first_half():
+    """w4 128 -> 64 with CSR outliers in channels [0, 32) only and dense rows for channels 5, 40 and 50: the second half of a
+    two-way split gets an empty CSR next to its dense rows."""
+    L = orc.make_layer(4, 128, 64, sparsity=0.05, topX=3, seed=11, nonzero_full_rows=True)
+    n = int(L["rows"][32])
+    L["rows"] = np.concatenate([L["rows"][:33], np.full(32, n)]).astype(np.int32)
+    L["cols"], L["vals"] = L["cols"][:n], L["vals"][:n]
+    L["full_row_indices"] = np.array([5, 40, 50], dtype=np.int32)
+    return L
+
+
+def test_shard_without_csr_entries_keeps_its_dense_rows():
+    """A shard whose channels have no CSR entry holds an empty CSR, so its forward still reads its dense rows: the shards of
+    from_full and of a ShardedSiblingGroup reassemble the full layer.  from_full rejects arguments that contradict the state."""
+    from squeezellm_b200.sharding import ShardedQuantLinearLUT, ShardedSiblingGroup
+    L = _csr_in_first_half()
+    st = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray)}
+    x = orc.make_vec(128, seed=1)
+    want = orc.forward_f64(L, x)
+    for rank, (c0, c1) in enumerate([(0, 32), (32, 64)]):
+        shard = ShardedQuantLinearLUT.from_full(st, 4, 128, 64, rank, 2, True, 3, "cpu").local
+        group = ShardedSiblingGroup([quant_layer(L)], rank, 2, "o_proj").layer
+        for m in (shard, group):
+            assert m._sparse_args()[3] is not None
+            assert np.allclose(orc.forward_f64(layer_as_read(m), x), want[:, c0:c1], rtol=1e-12, atol=1e-12)
+    for args in ((4, 96, 64, 0, 2, True, 3), (4, 128, 64, 0, 2, False, 3), (4, 128, 64, 0, 2, True, 0)):
+        with pytest.raises(ValueError, match="from_full"):
+            ShardedQuantLinearLUT.from_full(st, *args, "cpu")
+
+
+def test_sharded_members_refuse_dequantize_and_dissolve():
+    """A sharded member holds only its rank's columns: dequantize / to_linear and its group's dissolve raise and change nothing."""
+    from squeezellm_b200.sharding import ShardedSiblingGroup
+    ms = [quant_layer(orc.make_layer(4, 128, 64, sparsity=0.02, topX=3, seed=20 + i, nonzero_full_rows=True)) for i in range(3)]
+    g = ShardedSiblingGroup(ms, 0, 2, "qkv")
+
+    def snapshot():
+        return [(m._sibling_group, m.outfeatures, {k: (v.data_ptr(), tuple(v.shape)) for k, v in m.state_dict().items()})
+                for m in ms]
+    before = snapshot()
+    for m in ms:
+        with pytest.raises(NotImplementedError, match="sharded"):
+            m.dequantize()
+        with pytest.raises(NotImplementedError, match="sharded"):
+            m.to_linear()
+    with pytest.raises(NotImplementedError, match="dissolve"):
+        g.dissolve()
+    assert snapshot() == before and all(m._sibling_group[0] is g for m in ms)
 
 
 def _free_port():
@@ -172,17 +245,10 @@ def _layer_dict(m):
 
 def _worker_shard_model(rank, world, port, q):
     import torch.distributed as dist
-    from squeezellm_b200.quant import QuantLinearLUT
     from squeezellm_b200.sharding import shard_model
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        def member(L, sparse, topx):
-            m = QuantLinearLUT(L["bits"], L["infeatures"], L["outfeatures"], False, include_sparse=sparse,
-                               numvals=len(L["vals"]) if sparse else 0, topX=topx)
-            m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}, strict=False)
-            return m
-
         class Attn(nn.Module):
             def __init__(self):
                 super().__init__()
@@ -190,7 +256,7 @@ def _worker_shard_model(rank, world, port, q):
                 for i, n in enumerate(("q_proj", "k_proj", "v_proj", "o_proj")):
                     L = orc.make_layer(4, 128, 64, sparsity=0.05, topX=3, seed=40 + i, nonzero_full_rows=True)
                     self.full[n] = L
-                    setattr(self, n, member(L, True, 3))
+                    setattr(self, n, quant_layer(L))
 
         attn = Attn()
         groups = shard_model(attn, rank, world)

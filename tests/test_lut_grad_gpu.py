@@ -18,7 +18,7 @@ import torch
 
 from lut_grad_ref import dense_w_torch, lut_grad_f64
 from test_error_bound_host import SHAPES
-from util import bound_ratio, make_activations, orc, to_torch
+from util import bound_ratio, make_activations, orc, quant_layer, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -256,16 +256,8 @@ def test_three_streams_at_once():
 
 # ---- module level ------------------------------------------------------------------------------------------------------------
 def _module(L, bias=False):
-    from squeezellm_b200.quant import QuantLinearLUT
-    K, N, bits = L["infeatures"], L["outfeatures"], L["bits"]
-    topX = 0 if L.get("full_rows") is None else L["full_rows"].shape[1]
-    m = QuantLinearLUT(bits, K, N, bias, include_sparse=L.get("rows") is not None,
-                       numvals=0 if L.get("vals") is None else len(L["vals"]), topX=topX)
-    st = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}
-    if bias:
-        st["bias"] = torch.from_numpy(np.random.default_rng(K).standard_normal(N).astype(np.float32))
-    m.load_state_dict(st, strict=False)
-    return m.cuda()
+    K, N = L["infeatures"], L["outfeatures"]
+    return quant_layer(L, bias=np.random.default_rng(K).standard_normal(N).astype(np.float32) if bias else None).cuda()
 
 
 @pytest.mark.parametrize("bias", [False, True])

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from lut_grad_ref import dense_w_torch, lut_grad_f64
-from util import HEADER, Args, header_symbols, load_lib, orc
+from util import HEADER, Args, header_symbols, load_lib, orc, quant_layer
 
 F32, F16, BF16 = 0, 1, 2
 
@@ -157,13 +157,7 @@ def test_declared_in_the_header_and_the_version_unchanged():
 
 # ---- the module: train_codebook ---------------------------------------------------------------------------------------------
 def _module(L, bias=False):
-    from squeezellm_b200.quant import QuantLinearLUT
-    topX = 0 if L.get("full_rows") is None else L["full_rows"].shape[1]
-    m = QuantLinearLUT(L["bits"], L["infeatures"], L["outfeatures"], bias, include_sparse=L.get("rows") is not None,
-                       numvals=0 if L.get("vals") is None else len(L["vals"]), topX=topX)
-    st = {k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}
-    m.load_state_dict(st, strict=False)
-    return m
+    return quant_layer(L, bias=np.zeros(L["outfeatures"], dtype=np.float32) if bias else None)
 
 
 def test_train_codebook_makes_parameters_on_the_same_storage():

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from test_gpu_parity import BATCHED_SHAPES, IDS, SHAPES, batched_id, batched_inputs, ref_comparable
-from util import GOLDEN, Args, REL_TOL, TIGHT_TOL, load_lib, orc, rel_err, sample_idx, to_torch
+from util import GOLDEN, Args, REL_TOL, TIGHT_TOL, load_lib, orc, quant_layer, rel_err, sample_idx, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -244,11 +244,8 @@ def test_graph_capture_and_replay_with_new_inputs(qc):
 
 
 # ---- QuantLinearLUT routing ---------------------------------------------------------------------------------------------------
-def _module(L, bits, K, N, topx):
-    from squeezellm_b200.quant import QuantLinearLUT
-    m = QuantLinearLUT(bits, K, N, False, include_sparse=True, numvals=len(L["vals"]), topX=topx)
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}, strict=False)
-    return m.cuda()
+def _module(L):
+    return quant_layer(L, bias=None).cuda()
 
 
 @pytest.fixture
@@ -267,7 +264,7 @@ def test_module_routing(spy):
     from squeezellm_b200.quant import QuantLinearLUT
     K = N = 4096
     L = orc.make_layer(4, K, N, sparsity=0.0045, topX=10, seed=12, nonzero_full_rows=True)
-    m = _module(L, 4, K, N, 10)
+    m = _module(L)
     x = orc.make_vec(K, batch=2048, seed=12)
     y = m(torch.from_numpy(x).cuda().half().reshape(1, 2048, K))
     assert spy == [(2048, K)]
@@ -293,7 +290,7 @@ def test_sibling_group_members_get_their_slices(spy):
     Ls = [orc.make_layer(4, K, n, sparsity=0.01, topX=3, seed=20 + n, nonzero_full_rows=True) for n in (256, 128, 192)]
     block = torch.nn.Module()
     for name, L, n in zip(("q_proj", "k_proj", "v_proj"), Ls, (256, 128, 192)):
-        setattr(block, name, _module(L, 4, K, n, 3))
+        setattr(block, name, _module(L))
     assert len(fuse_siblings(block)) == 1
     x = orc.make_vec(K, batch=M, seed=21)
     xt = torch.from_numpy(x).cuda().half().reshape(1, M, K)

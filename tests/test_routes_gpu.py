@@ -125,10 +125,7 @@ class LayerData:
         self.bias = T["bias"]
         self.modules = {}
         for has_bias in (True, False):
-            m = QuantLinearLUT(bits, K, N, has_bias, include_sparse=True, numvals=len(self.L["vals"]), topX=10)
-            for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices") + (("bias",) if has_bias else ()):
-                setattr(m, k, T[k])
-            self.modules[has_bias] = m
+            self.modules[has_bias] = QuantLinearLUT.from_buffers(bits, T if has_bias else dict(T, bias=None))
 
     def check_rows(self, M):
         return [r for r in self.rows if r < M]
@@ -369,9 +366,7 @@ def test_out_of_range_csr_columns_are_ignored_on_the_batched_route(spy, dtype, f
     L["cols"] = L["cols"].copy()
     L["cols"][0], L["cols"][-1] = K + 9, -3
     T = to_torch(L)
-    m = QuantLinearLUT(4, K, N, False, include_sparse=True, numvals=len(L["vals"]), topX=10)
-    for k in ("qweight", "lookup_table", "rows", "cols", "vals", "full_rows", "full_row_indices"):
-        setattr(m, k, T[k])
+    m = QuantLinearLUT.from_buffers(4, T)
     x = torch.from_numpy(make_activations(K, M, seed=78)).cuda()
     buf = torch.full((M * K + 4 * K,), float("nan"), device="cuda")
     xt = buf[:M * K].view(M, K)

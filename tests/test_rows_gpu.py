@@ -12,8 +12,8 @@ import torch
 
 from test_error_bound_host import SHAPES
 from test_gpu_parity import BATCHED_SHAPES, batched_id, batched_inputs, ref_comparable
-from util import (GOLDEN, OUT_ROUNDING, REL_TOL, TIGHT_TOL, Args, abs_sum, bound_ratio, load_lib, make_activations, orc, rel_err,
-                  sample_idx, to_torch)
+from util import (GOLDEN, OUT_ROUNDING, REL_TOL, TIGHT_TOL, Args, abs_sum, bound_ratio, load_lib, make_activations, orc, quant_layer,
+                  rel_err, sample_idx, to_torch)
 
 pytestmark = pytest.mark.gpu
 
@@ -325,11 +325,8 @@ def test_three_streams_at_once(qc, record):
 
 
 # ---- QuantLinearLUT routing ---------------------------------------------------------------------------------------------------------
-def _module(L, bits, K, N, topx, bias=False):
-    from squeezellm_b200.quant import QuantLinearLUT
-    m = QuantLinearLUT(bits, K, N, bias, include_sparse=True, numvals=len(L["vals"]), topX=topx)
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}, strict=False)
-    return m.cuda()
+def _module(L, bias=False):
+    return quant_layer(L, bias=L["bias"] if bias else None).cuda()
 
 
 @pytest.fixture
@@ -348,7 +345,7 @@ def test_module_routing(spy):
     from squeezellm_b200.quant import QuantLinearLUT
     K = N = 4096
     L = orc.make_layer(4, K, N, sparsity=0.0045, topX=10, seed=12, nonzero_full_rows=True)
-    m = _module(L, 4, K, N, 10)
+    m = _module(L)
     x = make_activations(K, QuantLinearLUT.TC_MIN_ROWS, seed=12)
     top = min(QuantLinearLUT.ROWS_MAX, QuantLinearLUT.TC_MIN_ROWS - 1)
     for M in (2, top):
@@ -378,7 +375,7 @@ def test_module_output_dtype_and_shape_match_the_batched_branch(bias):
     from squeezellm_b200.quant import QuantLinearLUT
     K, N, M = 1024, 260, 6
     L = orc.make_layer(3, K, N, sparsity=0.01, topX=4, seed=13, nonzero_full_rows=True, bias=True)
-    m = _module(L, 3, K, N, 4, bias=bias)
+    m = _module(L, bias=bias)
     if bias:
         m.bias = torch.from_numpy(L["bias"]).cuda()
     x = torch.from_numpy(make_activations(K, M, seed=13)).cuda().half().reshape(2, 3, K)
@@ -398,7 +395,7 @@ def test_sibling_group_members_get_their_slices(spy):
     Ls = [orc.make_layer(4, K, n, sparsity=0.01, topX=3, seed=20 + n, nonzero_full_rows=True) for n in (256, 128, 192)]
     block = torch.nn.Module()
     for name, L, n in zip(("q_proj", "k_proj", "v_proj"), Ls, (256, 128, 192)):
-        setattr(block, name, _module(L, 4, K, n, 3))
+        setattr(block, name, _module(L))
     assert len(fuse_siblings(block)) == 1
     x = make_activations(K, M, seed=21)
     xt = torch.from_numpy(x).cuda().half().reshape(1, M, K)
@@ -415,7 +412,7 @@ def test_module_misaligned_x(spy, offset):
     """A contiguous fp16 view that starts `offset` elements into its storage gives the aligned input's result, bit for bit."""
     K, N, M = 4096, 4096, 5
     L = orc.make_layer(4, K, N, sparsity=0.0045, topX=10, seed=14, nonzero_full_rows=True)
-    m = _module(L, 4, K, N, 10)
+    m = _module(L)
     xa = torch.from_numpy(make_activations(K, M, seed=14)).cuda().half()
     buf = torch.zeros(M * K + 8, device="cuda", dtype=torch.float16)
     xv = buf[offset:offset + M * K].view(1, M, K)

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from util import OUT_ROUNDING, abs_sum, bound_ratio, orc, to_torch
+from util import OUT_ROUNDING, abs_sum, bound_ratio, orc, quant_layer, to_torch
 
 pytestmark = pytest.mark.gpu
 
@@ -95,7 +95,6 @@ def _local_peer(device):
 
 def _block(seed):
     """A tiny Llama-shaped decoder block of QuantLinearLUT layers (hidden 256, intermediate 704), q/k/v with a bias."""
-    from squeezellm_b200.quant import QuantLinearLUT
     H, I = 256, 704
     shapes = {"q_proj": (H, H, True), "k_proj": (H, H, True), "v_proj": (H, H, True), "o_proj": (H, H, False),
               "gate_proj": (H, I, False), "up_proj": (H, I, False), "down_proj": (I, H, False)}
@@ -103,9 +102,7 @@ def _block(seed):
     for i, (name, (K, N, bias)) in enumerate(shapes.items()):
         L = orc.make_layer(4, K, N, sparsity=0.01, topX=3, seed=seed + i, nonzero_full_rows=True, bias=bias)
         L["lookup_table"] = (L["lookup_table"] * (50.0 / np.sqrt(K))).astype(np.float32)
-        m = QuantLinearLUT(4, K, N, bias, include_sparse=True, numvals=len(L["vals"]), topX=3)
-        m.load_state_dict({k: torch.from_numpy(v) for k, v in L.items() if isinstance(v, np.ndarray) and k in m.state_dict()}, strict=False)
-        setattr(block, name, m.cuda())
+        setattr(block, name, quant_layer(L).cuda())
         layers[name] = L
     return block, layers
 

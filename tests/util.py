@@ -159,6 +159,24 @@ def late_owned_strips(bits, K, N, sm, first=8):
     return np.asarray(out, dtype=np.int64)
 
 
+def quant_layer(layer, **override):
+    """The QuantLinearLUT (CPU buffers) of an oracle layer dict (oracle.make_layer), through QuantLinearLUT.from_buffers on copies
+    of its arrays; `override` replaces entries first (bias=None: a layer without a bias)."""
+    import torch
+    from squeezellm_b200.quant import QuantLinearLUT
+    d = dict(layer, **override)
+    return QuantLinearLUT.from_buffers(d["bits"], {k: torch.tensor(v) for k, v in d.items() if isinstance(v, np.ndarray)})
+
+
+def layer_as_read(m):
+    """The oracle layer dict of what QuantLinearLUT m's own forward reads (CPU buffers): its packed words and LUT rows, and the
+    outliers that m._sparse_args() gives it; no bias."""
+    rows, cols, vals, fr, fri = (t.numpy() if t is not None else None for t in m._sparse_args())
+    return dict(bits=m.bits, infeatures=m.infeatures, outfeatures=m.outfeatures, qweight=m.qweight.contiguous().numpy(),
+                lookup_table=m.lookup_table.contiguous().numpy(), bias=None, rows=rows, cols=cols, vals=vals, full_rows=fr,
+                full_row_indices=fri)
+
+
 def to_torch(layer, device="cuda"):
     """numpy layer dict (oracle.make_layer) -> dict of torch tensors on `device`."""
     import torch
