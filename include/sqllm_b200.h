@@ -51,7 +51,8 @@ extern "C" {
                                  later + sqllm_lutgemm_fused, sqllm_lutgemv_rows, sqllm_lutgemm_t, sqllm_lut_grad,
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
-                                 sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops
+                                 sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
+                                 sqllm_attn_decode_splits
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -484,6 +485,45 @@ int sqllm_sequence_error(sqllm_sequence *s, void *stream);
 /* clears the error word on `stream` (after a start-up skew between ranks has been dealt with: barrier, then reset on every rank) */
 int sqllm_sequence_reset_error(sqllm_sequence *s, void *stream);
 void sqllm_sequence_destroy(sqllm_sequence *s);
+
+/* ---------------------------------------------------------------------------------------------
+ * Decode attention: one layer of a batch-1 decoder for one token, in ONE launch - rotary on q and the new k, the append of the new
+ * k / v to a static KV cache, and attention over the cache up to the token's own position, with grouped KV heads.
+ *   qkv       [n_heads*d | n_kv*d | n_kv*d] of dtype: the stacked q | k | v projection of the token
+ *   pos       DEVICE int32: the token's position (on the device so that a captured CUDA graph can advance it)
+ *   rope_cos, rope_sin  fp32 [capacity][d/2]: the rotary tables at positions 0 .. capacity-1 (any rope type; the tables carry it)
+ *   k_cache, v_cache    [n_kv][capacity][d] of dtype
+ *   out       [n_heads*d] of dtype
+ * Numerics (c = rope_cos[pos], s = rope_sin[pos], i < d/2, rotate-half convention):
+ *   q'_i = q_i c_i - q_{i+d/2} s_i,  q'_{i+d/2} = q_{i+d/2} c_i + q_i s_i           in fp32, then times scale * log2(e), not rounded
+ *   k'   the same rotary of the new k in fp32, rounded to dtype once; it is stored at k_cache[kv][pos] and v unchanged at
+ *        v_cache[kv][pos], the only cache elements the call writes
+ *   out[h] = round( sum_t 2^(z_t - M) V[t] / sum_t 2^(z_t - M) ),  z_t = q'_h . K[t] (fp32 FMAs), t = 0 .. pos, kv = h / (n_heads / n_kv),
+ *        where K[pos], V[pos] are k', v: an online softmax in fp32 whose partial states (max, sum, weighted sum) are combined in a fixed
+ *        order, rounded to dtype once.  No cache slot past pos is read.  Bit-reproducible: no atomics, no workspace.
+ * pos outside [0, capacity): the call writes nothing at all (a guard, not a mode).
+ * Launch shape: per KV head (and per 8 query heads of a larger group) one thread-block cluster of
+ * sqllm_attn_decode_splits(n_heads, n_kv, SM count) CTAs, which take the positions in blocks of 64: with B = pos/64 + 1 blocks, CTA r
+ * takes positions [r C, (r+1) C) with C = 64 ceil(B / splits).
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): dtype SQLLM_DT_F16 or SQLLM_DT_BF16, n_heads a
+ * positive multiple of n_kv >= 1, head_dim 64 or 128, capacity >= 1, scale finite and > 0, every pointer non-null and 16-byte
+ * aligned.  No allocation, no host synchronisation: CUDA-graph capturable and safe on several streams at once (on different caches). */
+typedef struct sqllm_attn_decode_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions of the cache */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;
+    const int32_t *pos;
+    const float *rope_cos, *rope_sin;
+    void *k_cache, *v_cache;
+    void *out;
+} sqllm_attn_decode_args;
+
+int sqllm_attn_decode(const sqllm_attn_decode_args *args, void *stream);
+/* CTAs per cluster of sqllm_attn_decode on a device of sm_count SMs: min(8, max(1, sm_count / (n_kv ceil(n_heads / n_kv / 8)))),
+ * 0 for invalid arguments.  Independent of pos. */
+int sqllm_attn_decode_splits(int n_heads, int n_kv, int sm_count);
 
 /* Test hook: unpack the packed indices on the GPU exactly as the GEMV kernels do
  * (idx uint8 [in, out]); lets tests prove the integer path bit-exact on its own. */

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -609,6 +609,47 @@ void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, 
                  "quant_cuda.fisher_accumulate");
 }
 
+// One layer's decode attention (sqllm_attn_decode): rotary, the append of k / v at slot *pos of the caches, attention over slots
+// 0..*pos into out, on the current stream.  The checks that need no device run first, on tensors of any device, so that a CPU caller
+// sees the same rejections; then every tensor must be a CUDA tensor on qkv's device.
+void attn_decode(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
+                 torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {&pos, "pos"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
+                                                                  {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
+    for (const auto &t : all) {
+        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), "attn_decode: ", t.second, " must be a contiguous tensor");
+        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), "attn_decode: ", t.second, " must be 16-byte aligned");
+    }
+    const auto dt = qkv.scalar_type();
+    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, "attn_decode: dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
+    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, "attn_decode: n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
+    TORCH_CHECK(k_cache.dim() == 3 && k_cache.size(0) == n_kv, "attn_decode: k_cache must be [n_kv=", n_kv, ", capacity, head_dim] (got ",
+                k_cache.sizes(), ")");
+    const int64_t cap = k_cache.size(1), d = k_cache.size(2);
+    TORCH_CHECK(d == 64 || d == 128, "attn_decode: head_dim=", d, " is not 64 or 128");
+    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, "attn_decode: capacity=", cap, " must be >= 1");
+    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), "attn_decode: scale=", scale, " must be finite and > 0");
+    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt,
+                "attn_decode: k_cache, v_cache and out must have qkv's dtype ", dt);
+    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), "attn_decode: v_cache must have k_cache's shape ", k_cache.sizes(), " (got ", v_cache.sizes(), ")");
+    TORCH_CHECK(qkv.numel() == (n_heads + 2 * n_kv) * d, "attn_decode: qkv has ", qkv.numel(), " elements, want (n_heads + 2 n_kv) head_dim = ",
+                (n_heads + 2 * n_kv) * d);
+    TORCH_CHECK(out.numel() == n_heads * d, "attn_decode: out has ", out.numel(), " elements, want n_heads head_dim = ", n_heads * d);
+    TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.numel() == 1, "attn_decode: pos must be one int32 element");
+    for (const torch::Tensor *t : {&rope_cos, &rope_sin})
+        TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->dim() == 2 && t->size(0) == cap && t->size(1) == d / 2,
+                    "attn_decode: rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
+    for (const auto &t : all)
+        TORCH_CHECK(t.first->is_cuda() && t.first->device() == qkv.device(), "attn_decode: ", t.second, " must be a CUDA tensor, on the device of qkv");
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    sqllm_attn_decode_args a;
+    a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
+    a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
+    a.qkv = qkv.data_ptr(); a.pos = pos.data_ptr<int32_t>(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
+    a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    check_status(sqllm_attn_decode(&a, cur_stream()), "quant_cuda.attn_decode");
+}
+
 torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
     need(qweight, "qweight", torch::kInt32, qweight);
@@ -739,7 +780,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("fisher_accumulate", &fisher_accumulate, "Fisher information of a linear layer, in place: fisher fp32 [out, in] += sum over "
           "the samples of seq_len rows of (dy_s^T x_s)^2, x [rows, in] and dy [rows, out] both fp16 or both bf16; one launch",
           py::arg("x"), py::arg("dy"), py::arg("fisher"), py::arg("seq_len"));
-    m.def("unpack_indices", &unpack_indices, "GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
+    m.def("attn_decode", &attn_decode, "one layer's batch-1 decode attention: rotary on q and k, k / v appended at slot pos of the caches, "
+          "softmax(scale q K^T[0..pos]) V[0..pos] per head (GQA) into out, one launch on the current stream",
+          py::arg("qkv"), py::arg("pos"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_cache"), py::arg("v_cache"), py::arg("out"),
+          py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_decode_splits", [](int n_heads, int n_kv) {
+              const int sm = sqllm_device_sm_count();
+              TORCH_CHECK(sm > 0, "attn_decode_splits: ", sqllm_last_error());
+              return sqllm_attn_decode_splits(n_heads, n_kv, sm);
+          }, "CTAs per cluster of attn_decode on the current device (independent of pos)");
+    m.def("unpack_indices", &unpack_indices,"GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },
           "fused path: True = bit-reproducible fixed-order reduction, False (default) = red.add accumulation");

@@ -10,6 +10,8 @@ It exists because the reference drives the path from Python one launch at a time
 (llama.py:226-234, quant_cuda_kernel.cu:147), which costs more host time per call than the kernels take on an
 H100; our kernels launch on the current stream precisely so that they can be captured.
 """
+from typing import NamedTuple
+
 import torch
 
 
@@ -91,12 +93,13 @@ class DecodeSequence:
     What a decoder layer puts between two matvecs runs inside the same launch (`matvec`'s keywords): an RMSNorm of the input, SiLU
     gating of the input by a second vector, a residual added to the output - each rounded to `dtype` once (lutgemv_seq.cuh)."""
 
-    def __init__(self, in_features, device, lut_mode=None, peer=None, dtype=torch.float16):
+    def __init__(self, in_features, device, lut_mode=None, peer=None, dtype=torch.float16, x=None):
+        """x: a tensor the sequence reads as its input instead of a buffer of its own (another kernel's output, say), not copied."""
         if dtype not in (torch.float16, torch.bfloat16):
             raise ValueError(f"DecodeSequence: dtype must be torch.float16 or torch.bfloat16 (got {dtype})")
         self.device = torch.device(device)
         self.dtype = dtype
-        self.x = torch.zeros(in_features, dtype=dtype, device=self.device)
+        self.x = self._bind(x, in_features, "x")
         self.input = SeqVec(-1, 0, in_features)
         self._ext = [self.x]   # external vector of item -1 - j: self._ext[j]
         self._items, self._lens, self._keep, self._ops = [], [], [], []
@@ -104,10 +107,30 @@ class DecodeSequence:
         self.lut_mode = lut_mode
         self.peer = peer
 
-    def new_input(self, n):
-        """Another external vector of n elements: (its SeqVec, its static tensor), read by every run like `x`."""
+    def _bind(self, t, n, name):
+        """A new zero vector of n elements, or the checked tensor t that the sequence reads in its place."""
+        if t is None:
+            return torch.zeros(n, dtype=self.dtype, device=self.device)
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"DecodeSequence: {name} must be a tensor (got {type(t).__name__})")
+        if t.dtype != self.dtype:
+            raise ValueError(f"DecodeSequence: {name} has dtype {t.dtype}, the sequence's is {self.dtype}")
+        dev = self.device
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        if t.device != dev:
+            raise ValueError(f"DecodeSequence: {name} is on {t.device}, the sequence on {self.device}")
+        if t.dim() != 1 or t.numel() != n or not t.is_contiguous():
+            raise ValueError(f"DecodeSequence: {name} must be a contiguous vector of {n} elements (got shape {tuple(t.shape)})")
+        if t.data_ptr() % 16:
+            raise ValueError(f"DecodeSequence: {name} must be 16-byte aligned")
+        return t
+
+    def new_input(self, n, tensor=None):
+        """Another external vector of n elements: (its SeqVec, its static tensor), read by every run like `x`.  tensor: read this one
+        (another sequence's output, say) instead of a new buffer, not copied."""
         assert self._handle is None, "sequence already compiled"
-        t = torch.zeros(n, dtype=self.dtype, device=self.device)
+        t = self._bind(tensor, n, "tensor")
         self._ext.append(t)
         return SeqVec(-len(self._ext), 0, n), t
 
@@ -203,3 +226,314 @@ class DecodeSequence:
                 self._handle = None
         except Exception:
             pass
+
+
+# ---- whole-model greedy decode -----------------------------------------------------------------------------------------------------
+DECODER_CLASSES = ("LlamaForCausalLM", "MistralForCausalLM", "Qwen2ForCausalLM")
+_PROJ = (("self_attn", ("q_proj", "k_proj", "v_proj", "o_proj")), ("mlp", ("gate_proj", "up_proj", "down_proj")))
+
+
+class PlanItem(NamedTuple):
+    """One matvec of a decoder sequence.  x / up / residual are (source, offset, length): source "x" is the sequence's input, "h" its
+    residual input, anything else the output of an earlier item of the same sequence.  norm is the RMSNorm module whose weight and eps
+    the item applies to its input."""
+    name: str
+    layer: object
+    x: tuple
+    norm: object = None
+    up: tuple = None
+    residual: tuple = None
+
+
+class SeqPlan(NamedTuple):
+    """One DecodeSequence: its input ("embed": the token's embedding, "attn": the attention output), its residual input h (None, "embed"
+    or (sequence name, item name): an exported output of an earlier sequence), its items and the item outputs it exports."""
+    name: str
+    x: str
+    h: object
+    items: list
+    outputs: list
+
+
+class AttnPlan(NamedTuple):
+    """The attention launch of decoder layer `layer`, reading the stacked q|k|v output (sequence name, item name)."""
+    layer: int
+    qkv: tuple
+
+
+def _decoder_layout(model, max_len):
+    """The checks of SequenceDecoder that need no device, in the order they are made; raises ValueError naming the reason.  Returns
+    the model's decoder layers."""
+    import transformers
+    name = type(model).__name__
+    if name not in DECODER_CLASSES or type(model) is not getattr(transformers, name):
+        raise ValueError(f"SequenceDecoder: {name} is not supported (only {', '.join(DECODER_CLASSES)})")
+    if not isinstance(max_len, int) or max_len < 1:
+        raise ValueError(f"SequenceDecoder: max_len must be a positive int (got {max_len!r})")
+    cfg = model.config
+    if "sliding_attention" in (getattr(cfg, "layer_types", None) or ()):
+        raise ValueError("SequenceDecoder: sliding-window attention is not supported (config.layer_types has sliding_attention layers)")
+    if name == "MistralForCausalLM" and cfg.sliding_window is not None and cfg.sliding_window < max_len:
+        raise ValueError(f"SequenceDecoder: sliding-window attention is not supported (sliding_window={cfg.sliding_window} < "
+                         f"max_len={max_len})")
+    if getattr(cfg, "hidden_act", "silu") != "silu":
+        raise ValueError(f"SequenceDecoder: hidden_act={cfg.hidden_act!r} is not silu")
+    layers = model.model.layers
+    head_dim = layers[0].self_attn.head_dim
+    if head_dim not in (64, 128):
+        raise ValueError(f"SequenceDecoder: head_dim={head_dim} is not 64 or 128")
+    from .quant import QuantLinearLUT
+    quant = []
+    for i, layer in enumerate(layers):
+        for block, names in _PROJ:
+            for n in names:
+                m = getattr(getattr(layer, block), n)
+                if not isinstance(m, QuantLinearLUT):
+                    raise ValueError(f"SequenceDecoder: layers.{i}.{block}.{n} is a {type(m).__name__}, not a QuantLinearLUT")
+                quant.append((f"layers.{i}.{block}.{n}", m))
+    if isinstance(model.lm_head, QuantLinearLUT):
+        quant.append(("lm_head", model.lm_head))
+    bits = sorted({m.bits for _, m in quant})
+    if len(bits) > 1:
+        raise ValueError(f"SequenceDecoder: mixed bit widths {bits}: the layers must share one")
+    for n, m in quant:
+        if m._trained:
+            raise ValueError(f"SequenceDecoder: {n} is being trained (train_codebook: {', '.join(m._trained)})")
+    dtype = model.model.embed_tokens.weight.dtype
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"SequenceDecoder: the model is {dtype}; only float16 and bfloat16 models are supported")
+    return layers
+
+
+def _stacked(module, names):
+    """The stacked layer of the sibling group that holds exactly module.<names>, in that order."""
+    ms = [getattr(module, n) for n in names]
+    g = ms[0]._sibling_group
+    if g is None or g[0].members != ms:
+        raise ValueError(f"SequenceDecoder: {', '.join(names)} are not one sibling group (fusion.fuse_siblings could not stack them)")
+    return g[0].layer
+
+
+def decoder_plan(model, max_len):
+    """What SequenceDecoder runs for one token, in order: SeqPlan and AttnPlan entries.  Stacks the model's siblings
+    (fusion.fuse_siblings), which leaves its outputs as they were.  A prologue sequence qkv_0 = qkv(rmsnorm(embed)); per layer l its
+    attention, then one sequence o = o_proj(attn) + h, gu = gate_up(rmsnorm(o)), d = down(silu(g) u) + o and qkv_{l+1} = qkv(rmsnorm(d)),
+    the last layer's ending in lm_head(rmsnorm(d)) instead when lm_head is a QuantLinearLUT (else the final norm and lm_head run as
+    torch ops on its d)."""
+    from .fusion import fuse_siblings
+    from .quant import QuantLinearLUT
+    layers = _decoder_layout(model, max_len)
+    fuse_siblings(model)
+    qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3]) for layer in layers]
+    gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2]) for layer in layers]
+    H = model.config.hidden_size
+    plan = [SeqPlan("prologue", "embed", None, [PlanItem("qkv", qkv[0], ("x", 0, H), layers[0].input_layernorm)], ["qkv"])]
+    for i, layer in enumerate(layers):
+        prev = plan[-1].name
+        plan.append(AttnPlan(i, (prev, "qkv")))
+        I = layer.mlp.down_proj.infeatures
+        o_proj = layer.self_attn.o_proj
+        items = [PlanItem("o", o_proj, ("x", 0, o_proj.infeatures), residual=("h", 0, H)),
+                 PlanItem("gu", gate_up[i], ("o", 0, H), layer.post_attention_layernorm),
+                 PlanItem("d", layer.mlp.down_proj, ("gu", 0, I), up=("gu", I, I), residual=("o", 0, H))]
+        if i + 1 < len(layers):
+            items.append(PlanItem("qkv", qkv[i + 1], ("d", 0, H), layers[i + 1].input_layernorm))
+            outputs = ["d", "qkv"]
+        elif isinstance(model.lm_head, QuantLinearLUT):
+            items.append(PlanItem("logits", model.lm_head, ("d", 0, H), model.model.norm))
+            outputs = ["logits"]
+        else:
+            outputs = ["d"]
+        plan.append(SeqPlan(f"layer{i}", "attn", "embed" if i == 0 else (prev, "d"), items, outputs))
+    return plan
+
+
+class SequenceDecoder:
+    """Greedy batch-1 decode of a whole quantized LLaMA-family model (LlamaForCausalLM, MistralForCausalLM without an active sliding
+    window, Qwen2ForCausalLM without sliding window) on one GPU, in fp16 or bf16.  Its q/k/v/o/gate/up/down projections must be
+    QuantLinearLUT layers of one bit width (checkpoint.load_quantized / load_checkpoint, then .cuda()); lm_head may be dense or
+    QuantLinearLUT.
+
+        dec = SequenceDecoder(model, max_len=2048)
+        ids = dec.generate(input_ids, max_new_tokens=128, eos_token_id=tok.eos_token_id)
+
+    One token is one CUDA graph replay: the embedding gather from a device token id, the prologue sequence, then per layer the
+    attention kernel (quant_cuda.attn_decode: rotary, KV-cache append, attention) and the layer's DecodeSequence (decoder_plan), then
+    the final norm and lm_head, the argmax into the device token id and pos += 1.  Tokens follow each other with no host
+    synchronisation.  The prompt runs through the model's own forward (prefill), whose cache is copied into the decoder's static one.
+
+    The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
+    computes carries no gradient."""
+
+    CHECK_EVERY = 8  # generate() looks for EOS every this many tokens
+
+    def __init__(self, model, max_len):
+        from .quant import quant_cuda
+        _decoder_layout(model, max_len)
+        devs = {p.device for p in model.parameters()} | {b.device for b in model.buffers()}
+        if len(devs) != 1 or next(iter(devs)).type != "cuda":
+            raise ValueError(f"SequenceDecoder: the model must be on one GPU (its tensors are on {sorted(map(str, devs))})")
+        self.model, self.max_len = model, max_len
+        self.device = next(iter(devs))
+        self.dtype = model.model.embed_tokens.weight.dtype
+        self._qc = quant_cuda
+        cfg = model.config
+        attn = model.model.layers[0].self_attn
+        self.n_layers = cfg.num_hidden_layers
+        self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
+        self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
+        self.plan = decoder_plan(model, max_len)
+        dev, d = self.device, self.head_dim
+        with torch.cuda.device(dev), torch.no_grad():
+            self.pos = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.tok = torch.zeros(1, dtype=torch.int64, device=dev)
+            self.k_cache = torch.zeros(self.n_layers, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
+            self.v_cache = torch.zeros_like(self.k_cache)
+            self.attn_out = torch.zeros(self.n_heads * d, dtype=self.dtype, device=dev)
+            cos, sin = model.model.rotary_emb(torch.zeros(1, dtype=torch.float32, device=dev), torch.arange(max_len, device=dev)[None])
+            self.rope_cos = cos[0, :, :d // 2].float().contiguous()
+            self.rope_sin = sin[0, :, :d // 2].float().contiguous()
+            self._build()
+            self._pos = 0
+            self._capture()
+
+    def _build(self):
+        """The DecodeSequences of the plan, each reading its inputs in place: the attention output buffer, the previous sequence's d."""
+        self.sequences, self._run, out = [], [], {}
+        for step in self.plan:
+            if isinstance(step, AttnPlan):
+                self._run.append(("attn", step.layer, out[step.qkv]))
+                continue
+            x = self.attn_out if step.x == "attn" else None
+            first = step.items[0]
+            seq = DecodeSequence(first.x[2], self.device, dtype=self.dtype, x=x)
+            if step.x == "embed":
+                out["embed"] = seq.x
+            vecs = {"x": seq.input}
+            if step.h is not None:
+                vecs["h"], _ = seq.new_input(self.model.config.hidden_size, tensor=out[step.h])
+            for it in step.items:
+                kw = {}
+                if it.norm is not None:
+                    kw["norm"] = (it.norm.weight.detach(), float(it.norm.variance_epsilon))
+                if it.up is not None:
+                    kw["up"] = vecs[it.up[0]][it.up[1]:it.up[1] + it.up[2]]
+                if it.residual is not None:
+                    kw["residual"] = vecs[it.residual[0]][it.residual[1]:it.residual[1] + it.residual[2]]
+                vecs[it.name] = seq.matvec(it.layer, vecs[it.x[0]][it.x[1]:it.x[1] + it.x[2]], **kw)
+            seq.compile(outputs=[vecs[n] for n in step.outputs])
+            for n, t in zip(step.outputs, seq.outputs):
+                out[(step.name, n)] = t
+            self.sequences.append(seq)
+            self._run.append(("seq", seq))
+        last = self.plan[-1]
+        self._head_in = out[(last.name, last.outputs[0])]
+        self._quant_head = last.outputs == ["logits"]
+
+    def _token(self):
+        """One token on the current stream: what the graph holds."""
+        embed = self.sequences[0].x
+        torch.index_select(self.model.model.embed_tokens.weight, 0, self.tok, out=embed.view(1, -1))
+        for r in self._run:
+            if r[0] == "seq":
+                r[1].replay()
+            else:
+                _, layer, qkv = r
+                self._qc.attn_decode(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[layer], self.v_cache[layer],
+                                     self.attn_out, self.n_heads, self.n_kv, self.scale)
+        if self._quant_head:
+            logits = self._head_in
+        else:
+            logits = self.model.lm_head(self.model.model.norm(self._head_in.view(1, -1)))[0]
+        self.tok.copy_(logits.argmax().view(1))
+        self.pos.add_(1)
+        return logits
+
+    def _capture(self):
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            self._token()  # warm-up at position 0 (prefill overwrites what it wrote)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph, stream=side):
+            self.logits = self._token()
+        torch.cuda.synchronize()
+        self.reset()
+
+    def reset(self):
+        """Start a new prompt: position 0 (the cache's old slots are never read again)."""
+        self._pos = 0
+        self.pos.zero_()
+
+    @property
+    def position(self):
+        """The position the next step writes (host copy of the device counter)."""
+        return self._pos
+
+    def prefill(self, input_ids):
+        """Run the prompt [1, T] (or [T]) through the model's own forward, copy its KV cache into the static one and set the position
+        to T; returns the logits of the last position."""
+        ids = torch.as_tensor(input_ids).reshape(1, -1).to(self.device)
+        T = ids.shape[1]
+        if not 1 <= T <= self.max_len:
+            raise ValueError(f"SequenceDecoder.prefill: {T} prompt tokens, the cache holds 1 to {self.max_len}")
+        with torch.no_grad():
+            o = self.model(input_ids=ids, use_cache=True)
+            for i, layer in enumerate(o.past_key_values.layers):
+                self.k_cache[i, :, :T].copy_(layer.keys[0])
+                self.v_cache[i, :, :T].copy_(layer.values[0])
+        self.pos.fill_(T)
+        self._pos = T
+        return o.logits[0, -1]
+
+    def _replay(self):
+        if self._pos >= self.max_len:
+            raise RuntimeError(f"SequenceDecoder: the cache is full (max_len={self.max_len}); reset() or prefill() first")
+        self.graph.replay()
+        self._pos += 1
+
+    def step(self, token_id):
+        """Feed token_id (an int or a one-element device tensor) at the current position; returns the next-token logits, a static buffer
+        that the next step overwrites."""
+        if self._pos >= self.max_len:
+            raise RuntimeError(f"SequenceDecoder: the cache is full (max_len={self.max_len}); reset() or prefill() first")
+        if isinstance(token_id, torch.Tensor):
+            self.tok.copy_(token_id.reshape(1))
+        else:
+            self.tok.fill_(int(token_id))
+        self._replay()
+        return self.logits
+
+    def generate(self, input_ids, max_new_tokens, eos_token_id=None):
+        """Greedy: input_ids [1, T] followed by up to max_new_tokens tokens, ending after the first EOS (eos_token_id: an int or a list)
+        if one comes.  The prompt and max_new_tokens - 1 steps must fit in max_len."""
+        ids = torch.as_tensor(input_ids).reshape(1, -1)
+        if max_new_tokens < 1:
+            return ids
+        if ids.shape[1] + max_new_tokens - 1 > self.max_len:
+            raise ValueError(f"SequenceDecoder.generate: {ids.shape[1]} prompt tokens and {max_new_tokens} new ones need "
+                             f"{ids.shape[1] + max_new_tokens - 1} cache positions, max_len is {self.max_len}")
+        eos = set() if eos_token_id is None else {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
+        logits = self.prefill(ids)
+        out = torch.empty(max_new_tokens, dtype=torch.int64, device=self.device)
+        self.tok.copy_(logits.argmax().view(1))
+        out[0:1].copy_(self.tok)
+        n, seen = 1, 0
+        while True:
+            if eos and (n % self.CHECK_EVERY == 0 or n == max_new_tokens):
+                got = out[seen:n].tolist()
+                hit = next((seen + j for j, t in enumerate(got) if t in eos), None)
+                if hit is not None:
+                    n = hit + 1
+                    break
+                seen = n
+            if n == max_new_tokens:
+                break
+            self._replay()
+            out[n:n + 1].copy_(self.tok)
+            n += 1
+        for seq in self.sequences:
+            seq.check()
+        return torch.cat([ids.to(self.device), out[:n].view(1, -1)], dim=1)
