@@ -52,7 +52,7 @@ extern "C" {
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
                                  sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
-                                 sqllm_attn_decode_splits
+                                 sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -524,6 +524,42 @@ int sqllm_attn_decode(const sqllm_attn_decode_args *args, void *stream);
 /* CTAs per cluster of sqllm_attn_decode on a device of sm_count SMs: min(8, max(1, sm_count / (n_kv ceil(n_heads / n_kv / 8)))),
  * 0 for invalid arguments.  Independent of pos. */
 int sqllm_attn_decode_splits(int n_heads, int n_kv, int sm_count);
+
+/* Decode attention of B sequences at once: for each sequence b what sqllm_attn_decode does for one, at that sequence's own position
+ * pos[b], in its own cache, in ONE launch.
+ *   qkv       [batch][n_heads*d | n_kv*d | n_kv*d] of dtype: row b is sequence b's stacked q | k | v projection
+ *   pos       DEVICE int32 [batch]: the position of each sequence
+ *   rope_cos, rope_sin  fp32 [capacity][d/2], shared by the sequences
+ *   k_cache, v_cache    [batch][n_kv][capacity][d] of dtype: sequence b's cache is the [n_kv][capacity][d] block b
+ *   out       [batch][n_heads*d] of dtype
+ * Per row b, with pos[b] for pos, row b of qkv and out and block b of the caches, the numerics are exactly those of sqllm_attn_decode:
+ * the same rotary, the same stored k / v, the same fp32 online softmax and the same combine order.  A row computed with the same
+ * splits count (below) as a sqllm_attn_decode call on its slices is bitwise equal to that call's result.
+ * pos[b] outside [0, capacity): row b is idle - the call writes nothing of it, not its cache block and not its out row (a guard, not a
+ * mode: a decoder parks a free slot there).  No slot past pos[b] of block b is read, nor anything of another row.
+ * Launch shape: per (sequence, KV head, 8 query heads of a larger group) one thread-block cluster of
+ * sqllm_attn_decode_batch_splits(n_heads, n_kv, batch, SM count) CTAs (grid z = batch), which take the positions 0 .. pos[b] in
+ * blocks of 64 as sqllm_attn_decode's CTAs do.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_decode and batch in [1, 65535].
+ * No allocation, no host synchronisation: CUDA-graph capturable. */
+typedef struct sqllm_attn_decode_batch_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int batch;                /* sequences, 1 .. 65535 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions of each sequence's cache */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;
+    const int32_t *pos;       /* [batch] */
+    const float *rope_cos, *rope_sin;
+    void *k_cache, *v_cache;
+    void *out;
+} sqllm_attn_decode_batch_args;
+
+int sqllm_attn_decode_batch(const sqllm_attn_decode_batch_args *args, void *stream);
+/* CTAs per cluster of sqllm_attn_decode_batch on a device of sm_count SMs:
+ * min(8, max(1, sm_count / (batch n_kv ceil(n_heads / n_kv / 8)))), 0 for invalid arguments (batch outside [1, 65535] included).
+ * Independent of the positions; batch 1 gives sqllm_attn_decode_splits. */
+int sqllm_attn_decode_batch_splits(int n_heads, int n_kv, int batch, int sm_count);
 
 /* Test hook: unpack the packed indices on the GPU exactly as the GEMV kernels do
  * (idx uint8 [in, out]); lets tests prove the integer path bit-exact on its own. */

@@ -47,7 +47,7 @@ def ext_path():
 
 def build_lib(verbose=False):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    hdrs = [os.path.join(INCLUDE, "sqllm_b200.h")] + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h"))
+    hdrs = [os.path.join(INCLUDE, "sqllm_b200.h")] + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + glob.glob(os.path.join(CSRC, "*.inc"))
     os.makedirs(OBJ, exist_ok=True)
     objs, jobs = [], []
     for src in sorted(glob.glob(os.path.join(CSRC, "*.cu"))):

@@ -261,27 +261,27 @@ class AttnPlan(NamedTuple):
     qkv: tuple
 
 
-def _decoder_layout(model, max_len):
-    """The checks of SequenceDecoder that need no device, in the order they are made; raises ValueError naming the reason.  Returns
-    the model's decoder layers."""
+def _decoder_layout(model, max_len, who="SequenceDecoder"):
+    """The checks of SequenceDecoder (and BatchDecoder: `who`) that need no device, in the order they are made; raises ValueError
+    naming the reason.  Returns the model's decoder layers."""
     import transformers
     name = type(model).__name__
     if name not in DECODER_CLASSES or type(model) is not getattr(transformers, name):
-        raise ValueError(f"SequenceDecoder: {name} is not supported (only {', '.join(DECODER_CLASSES)})")
+        raise ValueError(f"{who}: {name} is not supported (only {', '.join(DECODER_CLASSES)})")
     if not isinstance(max_len, int) or max_len < 1:
-        raise ValueError(f"SequenceDecoder: max_len must be a positive int (got {max_len!r})")
+        raise ValueError(f"{who}: max_len must be a positive int (got {max_len!r})")
     cfg = model.config
     if "sliding_attention" in (getattr(cfg, "layer_types", None) or ()):
-        raise ValueError("SequenceDecoder: sliding-window attention is not supported (config.layer_types has sliding_attention layers)")
+        raise ValueError(f"{who}: sliding-window attention is not supported (config.layer_types has sliding_attention layers)")
     if name == "MistralForCausalLM" and cfg.sliding_window is not None and cfg.sliding_window < max_len:
-        raise ValueError(f"SequenceDecoder: sliding-window attention is not supported (sliding_window={cfg.sliding_window} < "
+        raise ValueError(f"{who}: sliding-window attention is not supported (sliding_window={cfg.sliding_window} < "
                          f"max_len={max_len})")
     if getattr(cfg, "hidden_act", "silu") != "silu":
-        raise ValueError(f"SequenceDecoder: hidden_act={cfg.hidden_act!r} is not silu")
+        raise ValueError(f"{who}: hidden_act={cfg.hidden_act!r} is not silu")
     layers = model.model.layers
     head_dim = layers[0].self_attn.head_dim
     if head_dim not in (64, 128):
-        raise ValueError(f"SequenceDecoder: head_dim={head_dim} is not 64 or 128")
+        raise ValueError(f"{who}: head_dim={head_dim} is not 64 or 128")
     from .quant import QuantLinearLUT
     quant = []
     for i, layer in enumerate(layers):
@@ -289,29 +289,43 @@ def _decoder_layout(model, max_len):
             for n in names:
                 m = getattr(getattr(layer, block), n)
                 if not isinstance(m, QuantLinearLUT):
-                    raise ValueError(f"SequenceDecoder: layers.{i}.{block}.{n} is a {type(m).__name__}, not a QuantLinearLUT")
+                    raise ValueError(f"{who}: layers.{i}.{block}.{n} is a {type(m).__name__}, not a QuantLinearLUT")
                 quant.append((f"layers.{i}.{block}.{n}", m))
     if isinstance(model.lm_head, QuantLinearLUT):
         quant.append(("lm_head", model.lm_head))
     bits = sorted({m.bits for _, m in quant})
     if len(bits) > 1:
-        raise ValueError(f"SequenceDecoder: mixed bit widths {bits}: the layers must share one")
+        raise ValueError(f"{who}: mixed bit widths {bits}: the layers must share one")
     for n, m in quant:
         if m._trained:
-            raise ValueError(f"SequenceDecoder: {n} is being trained (train_codebook: {', '.join(m._trained)})")
+            raise ValueError(f"{who}: {n} is being trained (train_codebook: {', '.join(m._trained)})")
     dtype = model.model.embed_tokens.weight.dtype
     if dtype not in (torch.float16, torch.bfloat16):
-        raise ValueError(f"SequenceDecoder: the model is {dtype}; only float16 and bfloat16 models are supported")
+        raise ValueError(f"{who}: the model is {dtype}; only float16 and bfloat16 models are supported")
     return layers
 
 
-def _stacked(module, names):
+def _stacked(module, names, who="SequenceDecoder"):
     """The stacked layer of the sibling group that holds exactly module.<names>, in that order."""
     ms = [getattr(module, n) for n in names]
     g = ms[0]._sibling_group
     if g is None or g[0].members != ms:
-        raise ValueError(f"SequenceDecoder: {', '.join(names)} are not one sibling group (fusion.fuse_siblings could not stack them)")
+        raise ValueError(f"{who}: {', '.join(names)} are not one sibling group (fusion.fuse_siblings could not stack them)")
     return g[0].layer
+
+
+def _model_device(model, who):
+    """The one GPU every tensor of the model is on; ValueError otherwise."""
+    devs = {p.device for p in model.parameters()} | {b.device for b in model.buffers()}
+    if len(devs) != 1 or next(iter(devs)).type != "cuda":
+        raise ValueError(f"{who}: the model must be on one GPU (its tensors are on {sorted(map(str, devs))})")
+    return next(iter(devs))
+
+
+def _rope_tables(model, max_len, head_dim, device):
+    """fp32 cos, sin [max_len, head_dim/2] of the model's own rotary embedding at positions 0 .. max_len-1 (any rope type)."""
+    cos, sin = model.model.rotary_emb(torch.zeros(1, dtype=torch.float32, device=device), torch.arange(max_len, device=device)[None])
+    return cos[0, :, :head_dim // 2].float().contiguous(), sin[0, :, :head_dim // 2].float().contiguous()
 
 
 def decoder_plan(model, max_len):
@@ -370,11 +384,8 @@ class SequenceDecoder:
     def __init__(self, model, max_len):
         from .quant import quant_cuda
         _decoder_layout(model, max_len)
-        devs = {p.device for p in model.parameters()} | {b.device for b in model.buffers()}
-        if len(devs) != 1 or next(iter(devs)).type != "cuda":
-            raise ValueError(f"SequenceDecoder: the model must be on one GPU (its tensors are on {sorted(map(str, devs))})")
+        self.device = _model_device(model, "SequenceDecoder")
         self.model, self.max_len = model, max_len
-        self.device = next(iter(devs))
         self.dtype = model.model.embed_tokens.weight.dtype
         self._qc = quant_cuda
         cfg = model.config
@@ -390,9 +401,7 @@ class SequenceDecoder:
             self.k_cache = torch.zeros(self.n_layers, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
             self.v_cache = torch.zeros_like(self.k_cache)
             self.attn_out = torch.zeros(self.n_heads * d, dtype=self.dtype, device=dev)
-            cos, sin = model.model.rotary_emb(torch.zeros(1, dtype=torch.float32, device=dev), torch.arange(max_len, device=dev)[None])
-            self.rope_cos = cos[0, :, :d // 2].float().contiguous()
-            self.rope_sin = sin[0, :, :d // 2].float().contiguous()
+            self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
             self._build()
             self._pos = 0
             self._capture()
@@ -537,3 +546,208 @@ class SequenceDecoder:
         for seq in self.sequences:
             seq.check()
         return torch.cat([ids.to(self.device), out[:n].view(1, -1)], dim=1)
+
+
+class BatchDecoder:
+    """Greedy decode of `batch` sequences at once (2 .. QuantLinearLUT.ROWS_MAX in fp16, 2 .. BF16_ROWS_MAX in bf16) through a whole
+    quantized LLaMA-family model on one GPU: the models SequenceDecoder takes, whose projections (stacked q/k/v, o, stacked gate/up,
+    down and a quantized lm_head) all fit the multi-row LUT-GEMV (QuantLinearLUT._rows_fits).
+
+        dec = BatchDecoder(model, max_len=2048, batch=8)
+        outs = dec.generate([ids_a, ids_b, ids_c], max_new_tokens=128, eos_token_id=tok.eos_token_id)
+
+    Each sequence has a slot: row b of every step, block b of the cache [n_layers, batch, n_kv, max_len, head_dim] and its own device
+    position pos[b], so prompts of different lengths need no padding and no mask.  A slot whose pos is -1 is idle: its row still goes
+    through the projections, but the attention writes nothing for it, and its logits and token mean nothing.  release() and prefill()
+    of a slot between steps while the others keep going is continuous batching.
+
+    One step is one CUDA graph replay: the embedding gather of the device tokens tok[batch]; per layer the model's input_layernorm, the
+    stacked q/k/v layer on [batch, hidden] (QuantLinearLUT.forward: the multi-row kernel), quant_cuda.attn_decode_batch on the layer's
+    cache, o_proj plus the residual, post_attention_layernorm, the stacked gate/up layer, silu(g) u, down plus the residual; the final
+    norm and lm_head, the argmax per row into tok and pos[b] += 1 for the active rows.  Steps follow each other with no host
+    synchronisation.  Every op of a step is row-wise, so a row's result does not depend on what the other rows hold.
+
+    The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
+    computes carries no gradient."""
+
+    CHECK_EVERY = 8  # generate() looks for EOS every this many steps
+
+    def __init__(self, model, max_len, batch):
+        import types
+
+        from .fusion import fuse_siblings
+        from .quant import FUSED_LIMITS, QuantLinearLUT, quant_cuda
+        layers = _decoder_layout(model, max_len, "BatchDecoder")
+        self.dtype = model.model.embed_tokens.weight.dtype
+        rows_max = QuantLinearLUT.ROWS_MAX if self.dtype == torch.float16 else QuantLinearLUT.BF16_ROWS_MAX
+        if not isinstance(batch, int) or not 2 <= batch <= rows_max:
+            hint = "; decode one sequence with SequenceDecoder" if batch == 1 else ""
+            raise ValueError(f"BatchDecoder: batch must be an int in 2..{rows_max} for a {self.dtype} model (got {batch!r}){hint}")
+        for i, layer in enumerate(layers):  # the shapes the step runs, stacked siblings included, before anything is stacked
+            at, mlp = layer.self_attn, layer.mlp
+            shapes = [("self_attn.q_proj|k_proj|v_proj", at.q_proj.infeatures,
+                       at.q_proj.outfeatures + at.k_proj.outfeatures + at.v_proj.outfeatures),
+                      ("self_attn.o_proj", at.o_proj.infeatures, at.o_proj.outfeatures),
+                      ("mlp.gate_proj|up_proj", mlp.gate_proj.infeatures, mlp.gate_proj.outfeatures + mlp.up_proj.outfeatures),
+                      ("mlp.down_proj", mlp.down_proj.infeatures, mlp.down_proj.outfeatures)]
+            if i == len(layers) - 1 and isinstance(model.lm_head, QuantLinearLUT):
+                shapes.append(("lm_head", model.lm_head.infeatures, model.lm_head.outfeatures))
+            for n, K, N in shapes:
+                if not QuantLinearLUT._rows_fits(types.SimpleNamespace(infeatures=K, outfeatures=N)):
+                    where = n if n == "lm_head" else f"layers.{i}.{n}"
+                    raise ValueError(f"BatchDecoder: {where} ({K} -> {N}) does not fit the multi-row LUT-GEMV (out_features a multiple "
+                                     f"of 4, in_features up to {FUSED_LIMITS['rows_max_in_features']})")
+        self.device = _model_device(model, "BatchDecoder")
+        self.model, self.max_len, self.batch = model, max_len, batch
+        self._qc = quant_cuda
+        cfg = model.config
+        attn = layers[0].self_attn
+        self.n_layers = cfg.num_hidden_layers
+        self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
+        self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
+        fuse_siblings(model)
+        self.qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3], "BatchDecoder") for layer in layers]
+        self.gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2], "BatchDecoder") for layer in layers]
+        dev, d = self.device, self.head_dim
+        with torch.cuda.device(dev), torch.no_grad():
+            self.pos = torch.full((batch,), -1, dtype=torch.int32, device=dev)
+            self.tok = torch.zeros(batch, dtype=torch.int64, device=dev)
+            self.k_cache = torch.zeros(self.n_layers, batch, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
+            self.v_cache = torch.zeros_like(self.k_cache)
+            self.attn_out = torch.zeros(batch, self.n_heads * d, dtype=self.dtype, device=dev)
+            self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
+            self._pos = [-1] * batch
+            self._capture()
+
+    def _proj(self, layer, x):
+        """layer(x) in the model's dtype (a batch's bias is added in the bias's dtype, fp32 for a checkpoint's bias)."""
+        y = layer(x)
+        return y if y.dtype == self.dtype else y.to(self.dtype)
+
+    def _step(self):
+        """One step on the current stream: what the graph holds."""
+        m = self.model.model
+        h = torch.index_select(m.embed_tokens.weight, 0, self.tok)
+        for i, layer in enumerate(m.layers):
+            qkv = self._proj(self.qkv[i], layer.input_layernorm(h))
+            self._qc.attn_decode_batch(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i], self.attn_out,
+                                       self.n_heads, self.n_kv, self.scale)
+            h = h + self._proj(layer.self_attn.o_proj, self.attn_out)
+            gu = self._proj(self.gate_up[i], layer.post_attention_layernorm(h))
+            I = gu.shape[1] // 2
+            h = h + self._proj(layer.mlp.down_proj, torch.nn.functional.silu(gu[:, :I]) * gu[:, I:])
+        logits = self.model.lm_head(m.norm(h))
+        self.tok.copy_(logits.argmax(dim=-1))
+        self.pos.add_((self.pos >= 0).to(torch.int32))
+        return logits
+
+    def _capture(self):
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            self._step()  # warm-up with every slot idle: no cache slot is written
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph, stream=side):
+            self.logits = self._step()
+        torch.cuda.synchronize()
+        self.reset()
+
+    def _slot(self, slot):
+        if not isinstance(slot, int) or not 0 <= slot < self.batch:
+            raise ValueError(f"BatchDecoder: slot must be an int in 0..{self.batch - 1} (got {slot!r})")
+        return slot
+
+    def reset(self):
+        """Release every slot."""
+        self.pos.fill_(-1)
+        self._pos = [-1] * self.batch
+
+    def release(self, slot):
+        """Make `slot` idle (pos -1): the steps write nothing for it from now on; its old cache slots are never read again."""
+        slot = self._slot(slot)
+        self.pos[slot] = -1
+        self._pos[slot] = -1
+
+    @property
+    def positions(self):
+        """The position each slot's next step writes, -1 for an idle slot (host copy of the device positions)."""
+        return list(self._pos)
+
+    def prefill(self, slot, input_ids):
+        """Run the prompt [1, T] (or [T]) alone through the model's own forward, copy its KV cache into `slot` and set the slot's
+        position to T; returns the logits of the last position."""
+        self._slot(slot)
+        ids = torch.as_tensor(input_ids).reshape(1, -1).to(self.device)
+        T = ids.shape[1]
+        if not 1 <= T <= self.max_len:
+            raise ValueError(f"BatchDecoder.prefill: {T} prompt tokens, the cache holds 1 to {self.max_len}")
+        with torch.no_grad():
+            o = self.model(input_ids=ids, use_cache=True)
+            for i, layer in enumerate(o.past_key_values.layers):
+                self.k_cache[i, slot, :, :T].copy_(layer.keys[0])
+                self.v_cache[i, slot, :, :T].copy_(layer.values[0])
+        self.pos[slot] = T
+        self._pos[slot] = T
+        return o.logits[0, -1]
+
+    def _replay(self):
+        full = [b for b, p in enumerate(self._pos) if p >= self.max_len]
+        if full:
+            raise RuntimeError(f"BatchDecoder: the cache of slot(s) {full} is full (max_len={self.max_len}); release() or prefill() them first")
+        self.graph.replay()
+        self._pos = [p + 1 if p >= 0 else p for p in self._pos]
+
+    def step(self, token_ids):
+        """Feed token_ids ([batch] ints or a device tensor; only the active slots' entries matter) at each active slot's position;
+        returns the next-token logits [batch, vocab], a static buffer that the next step overwrites."""
+        t = torch.as_tensor(token_ids)
+        if t.numel() != self.batch:
+            raise ValueError(f"BatchDecoder.step: {t.numel()} token ids for {self.batch} slots")
+        self.tok.copy_(t.reshape(self.batch))
+        self._replay()
+        return self.logits
+
+    def generate(self, prompts, max_new_tokens, eos_token_id=None):
+        """Greedy: each of the 1..batch prompts (1-D token ids, or [1, T]) followed by up to max_new_tokens tokens, ending after its
+        first EOS (eos_token_id: an int or a list) if one comes; prompt i runs in slot i, the other slots stay idle.  Every prompt and
+        max_new_tokens - 1 steps must fit in max_len.  Returns one 1-D tensor per prompt (prompt + new tokens), in order."""
+        prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
+        if not 1 <= len(prompts) <= self.batch:
+            raise ValueError(f"BatchDecoder.generate: {len(prompts)} prompts, the decoder takes 1 to {self.batch}")
+        if not isinstance(max_new_tokens, int) or max_new_tokens < 1:
+            raise ValueError(f"BatchDecoder.generate: max_new_tokens must be a positive int (got {max_new_tokens!r})")
+        for i, p in enumerate(prompts):
+            if p.numel() < 1:
+                raise ValueError(f"BatchDecoder.generate: prompt {i} is empty")
+            if p.numel() + max_new_tokens - 1 > self.max_len:
+                raise ValueError(f"BatchDecoder.generate: prompt {i} has {p.numel()} tokens and {max_new_tokens} new ones need "
+                                 f"{p.numel() + max_new_tokens - 1} cache positions, max_len is {self.max_len}")
+        eos = set() if eos_token_id is None else {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
+        R = len(prompts)
+        self.reset()
+        out = torch.zeros(self.batch, max_new_tokens, dtype=torch.int64, device=self.device)
+        for i, p in enumerate(prompts):
+            out[i, 0] = self.prefill(i, p).argmax()
+        self.tok.copy_(out[:, 0])
+        length = [None] * R  # new tokens of a finished row
+        n, seen = 1, 0
+        while True:
+            if eos and (n % self.CHECK_EVERY == 0 or n == max_new_tokens):
+                got = out[:R, seen:n].tolist()
+                for i in range(R):
+                    if length[i] is None:
+                        hit = next((seen + j for j, t in enumerate(got[i]) if t in eos), None)
+                        if hit is not None:
+                            length[i] = hit + 1
+                            self.release(i)
+                seen = n
+                if all(x is not None for x in length):
+                    break
+            if n == max_new_tokens:
+                break
+            self._replay()
+            out[:, n].copy_(self.tok)
+            n += 1
+        return [torch.cat([p.to(self.device), out[i, :length[i] if length[i] is not None else n]]) for i, p in enumerate(prompts)]
