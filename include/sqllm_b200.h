@@ -52,7 +52,8 @@ extern "C" {
                                  sqllm_lutgemm_fused_dt, sqllm_lutgemv_fused_dt, sqllm_lutgemv_rows_dt, sqllm_dequantize,
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
                                  sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
-                                 sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits
+                                 sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits,
+                                 sqllm_attn_extend, sqllm_attn_extend_splits
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -560,6 +561,49 @@ int sqllm_attn_decode_batch(const sqllm_attn_decode_batch_args *args, void *stre
  * min(8, max(1, sm_count / (batch n_kv ceil(n_heads / n_kv / 8)))), 0 for invalid arguments (batch outside [1, 65535] included).
  * Independent of the positions; batch 1 gives sqllm_attn_decode_splits. */
 int sqllm_attn_decode_batch_splits(int n_heads, int n_kv, int batch, int sm_count);
+
+/* Attention of a chunk of T new tokens of one sequence at positions start .. start+T-1 (a prompt, or more tokens appended to a sequence
+ * already in the cache): rotary on the chunk's q and k, the append of its k / v to the cache, and causal attention of every token over
+ * the cache up to its own position, with grouped KV heads.
+ *   qkv       [T][n_heads*d | n_kv*d | n_kv*d] of dtype: the stacked q | k | v projection of the chunk's tokens
+ *   start     host int: the position of the chunk's first token (slots 0 .. start-1 already hold the sequence's earlier k / v)
+ *   rope_cos, rope_sin  fp32 [capacity][d/2], as for sqllm_attn_decode
+ *   k_cache, v_cache    [n_kv][capacity][d] of dtype
+ *   out       [T][n_heads*d] of dtype
+ * Numerics, for token t at p = start + t (c = rope_cos[p], s = rope_sin[p], i < d/2, rotate-half convention):
+ *   k'_t  = the rotary of k_t in fp32, rounded to dtype once - the expression of sqllm_attn_decode, so the stored bits equal those
+ *           T successive sqllm_attn_decode calls at start .. start+T-1 store; k' at k_cache[kv][p], v_t unchanged at v_cache[kv][p],
+ *           the only cache elements the call writes
+ *   q'_t  = the rotary of q_t in fp32, split x = hi + lo (hi = dtype(x), lo = dtype(x - hi)) at x = q'/4
+ *   out[t, h] = round( sum_j 2^(z_j - M) V[j] / sum_j 2^(z_j - M) ),  z_j = scale log2(e) q'_{t,h} . K[j], j = 0 .. p,
+ *           kv = h / (n_heads / n_kv): both products on the tensor cores (mma m16n8k16, fp32 accumulation) with q' and the weights
+ *           2^(z_j - M) each as hi + lo in dtype; an online softmax in fp32 whose partial states are combined in a fixed order.
+ *           No cache slot at or past start + T is read or written.  Bit-reproducible: no atomics, no workspace.
+ * Launch shape: an append kernel (one CTA per token), then on the same stream the attention kernel: query tiles of 64 (token, query
+ * head) rows of one KV head's group, token-major; per tile one thread-block cluster of
+ * sqllm_attn_extend_splits(n_heads, n_kv, n_tokens, start, SM count) CTAs, which take the tile's keys 0 .. start + (its last token)
+ * in blocks of 64, ceil(blocks / splits) blocks per CTA.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_decode (dtype, head layout, head_dim,
+ * capacity, scale), n_tokens >= 1, start >= 0, start + n_tokens <= capacity, n_tokens * (n_heads / n_kv) <= 64 * 65535, n_kv <= 65535,
+ * every pointer non-null and 16-byte aligned.  No allocation, no host synchronisation: CUDA-graph capturable for a fixed start. */
+typedef struct sqllm_attn_extend_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions of the cache */
+    int start;                /* position of the chunk's first token */
+    int n_tokens;             /* T */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;
+    const float *rope_cos, *rope_sin;
+    void *k_cache, *v_cache;
+    void *out;
+} sqllm_attn_extend_args;
+
+int sqllm_attn_extend(const sqllm_attn_extend_args *args, void *stream);
+/* CTAs per cluster of sqllm_attn_extend on a device of sm_count SMs, with tiles = n_kv ceil(n_tokens (n_heads / n_kv) / 64):
+ * max(1, min(8, sm_count / tiles, ceil((start + n_tokens) / 64))); 0 for invalid arguments (a head layout that is not a positive
+ * multiple, n_tokens < 1, start < 0, sm_count < 1, start + n_tokens above INT_MAX, more than 65535 tiles per KV head). */
+int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int sm_count);
 
 /* Test hook: unpack the packed indices on the GPU exactly as the GEMV kernels do
  * (idx uint8 [in, out]); lets tests prove the integer path bit-exact on its own. */

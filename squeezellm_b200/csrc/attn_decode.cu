@@ -1,9 +1,12 @@
 // attn_decode.cu - decode attention with rotary and KV-cache append (attn_decode.cuh) behind sqllm_attn_decode (one sequence) and
-// sqllm_attn_decode_batch (several, each at its own position).
+// sqllm_attn_decode_batch (several, each at its own position); causal attention of a chunk of new tokens with the same rotary and
+// append (attn_extend.cuh) behind sqllm_attn_extend.
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 
 #include "attn_decode.cuh"
+#include "attn_extend.cuh"
 #include "host.h"
 
 using namespace sqllm;
@@ -30,6 +33,33 @@ KernelSmem attn_kernel_of(int G) {
 
 bool aligned16(const void *ptr) { return ptr && !(reinterpret_cast<uintptr_t>(ptr) & 15); }
 
+// the argument checks every attention entry point shares, in the order they run: the dtype, (the batch,) the head layout, head_dim,
+// capacity and scale, (the chunk,) the pointers
+int check_dtype(int dtype) {
+    if (dtype != SQLLM_DT_F16 && dtype != SQLLM_DT_BF16) return fail(SQLLM_EINVAL, "dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", dtype);
+    return SQLLM_OK;
+}
+
+template <typename Args>
+int check_heads(const Args *a) {
+    if (a->n_kv < 1 || a->n_heads < 1 || a->n_heads % a->n_kv)
+        return fail(SQLLM_EINVAL, "n_heads=%d must be a positive multiple of n_kv=%d", a->n_heads, a->n_kv);
+    if (a->head_dim != 64 && a->head_dim != 128) return fail(SQLLM_EINVAL, "head_dim=%d is not 64 or 128", a->head_dim);
+    if (a->capacity < 1) return fail(SQLLM_EINVAL, "capacity=%d must be >= 1", a->capacity);
+    if (!(isfinite(a->scale) && a->scale > 0.f)) return fail(SQLLM_EINVAL, "scale=%g must be finite and > 0", (double)a->scale);
+    return SQLLM_OK;
+}
+
+struct NamedPtr {
+    const void *p;
+    const char *name;
+};
+int check_ptrs(std::initializer_list<NamedPtr> ptrs) {
+    for (const NamedPtr &q : ptrs)
+        if (!aligned16(q.p)) return fail(SQLLM_EINVAL, "%s must be a non-null 16-byte aligned pointer", q.name);
+    return SQLLM_OK;
+}
+
 constexpr int MAX_BATCH = 65535;  // gridDim.z
 
 int splits(int n_heads, int n_kv, int batch, int sm_count) {
@@ -42,19 +72,12 @@ int splits(int n_heads, int n_kv, int batch, int sm_count) {
 // the checks and the launch of both entry points; `batch` sequences (the batch-1 entry: 1, on the batch-1 kernel)
 template <bool BATCH, typename Args>
 int attn_launch(const Args *a, int batch, void *stream) {
-    if (a->dtype != SQLLM_DT_F16 && a->dtype != SQLLM_DT_BF16)
-        return fail(SQLLM_EINVAL, "dtype=%d is not SQLLM_DT_F16 or SQLLM_DT_BF16", a->dtype);
+    if (int rc = check_dtype(a->dtype)) return rc;
     if (BATCH && (batch < 1 || batch > MAX_BATCH)) return fail(SQLLM_EINVAL, "batch=%d must be in [1, %d]", batch, MAX_BATCH);
-    if (a->n_kv < 1 || a->n_heads < 1 || a->n_heads % a->n_kv)
-        return fail(SQLLM_EINVAL, "n_heads=%d must be a positive multiple of n_kv=%d", a->n_heads, a->n_kv);
-    if (a->head_dim != 64 && a->head_dim != 128) return fail(SQLLM_EINVAL, "head_dim=%d is not 64 or 128", a->head_dim);
-    if (a->capacity < 1) return fail(SQLLM_EINVAL, "capacity=%d must be >= 1", a->capacity);
-    if (!(isfinite(a->scale) && a->scale > 0.f)) return fail(SQLLM_EINVAL, "scale=%g must be finite and > 0", (double)a->scale);
-    const struct { const void *p; const char *name; } ptrs[] = {{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"},
-                                                               {a->rope_sin, "rope_sin"}, {a->k_cache, "k_cache"},
-                                                               {a->v_cache, "v_cache"}, {a->out, "out"}};
-    for (const auto &q : ptrs)
-        if (!aligned16(q.p)) return fail(SQLLM_EINVAL, "%s must be a non-null 16-byte aligned pointer", q.name);
+    if (int rc = check_heads(a)) return rc;
+    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"},
+                             {a->k_cache, "k_cache"}, {a->v_cache, "v_cache"}, {a->out, "out"}}))
+        return rc;
     const int g = a->n_heads / a->n_kv, gc = std::min(g, attn::GMAX);
     const int G = gc <= 1 ? 1 : gc <= 2 ? 2 : gc <= 4 ? 4 : 8;
     const bool bf = a->dtype == SQLLM_DT_BF16;
@@ -78,6 +101,61 @@ int attn_launch(const Args *a, int batch, void *stream) {
     return SQLLM_OK;
 }
 
+template <typename T, int D>
+KernelSmem extend_kernel_of() { return {attn::attn_extend_kernel<T, D>, attn::ext_smem_bytes(D)}; }
+
+// the rows of the chunk's query tiles (T tokens x g heads of a group), 0 when they need more tiles than the grid holds
+long long ext_tiles(int n_heads, int n_kv, int T) {
+    const long long tiles = ((long long)T * (n_heads / n_kv) + attn::BM - 1) / attn::BM;
+    return tiles <= attn::MAX_TILES ? tiles : 0;
+}
+
+// CTAs per cluster of sqllm_attn_extend: 1 when the query tiles alone fill the SMs, else as many as the SMs left per tile allow, at
+// most MAX_CLUSTER and at most the key blocks of the longest tile (start + T keys)
+int ext_splits(int n_heads, int n_kv, int T, int start, int sm_count) {
+    if (n_kv < 1 || n_heads < n_kv || n_heads % n_kv || T < 1 || start < 0 || sm_count < 1 || (long long)start + T > INT_MAX) return 0;
+    const long long tiles = ext_tiles(n_heads, n_kv, T) * n_kv;
+    if (tiles == 0) return 0;
+    const long long blocks = ((long long)start + T + attn::BN - 1) / attn::BN;
+    return (int)std::max(1LL, std::min({(long long)attn::MAX_CLUSTER, sm_count / tiles, blocks}));
+}
+
+int extend_launch(const sqllm_attn_extend_args *a, void *stream) {
+    if (int rc = check_dtype(a->dtype)) return rc;
+    if (int rc = check_heads(a)) return rc;
+    if (a->n_tokens < 1) return fail(SQLLM_EINVAL, "n_tokens=%d must be >= 1", a->n_tokens);
+    if (a->start < 0) return fail(SQLLM_EINVAL, "start=%d must be >= 0", a->start);
+    if ((long long)a->start + a->n_tokens > a->capacity)
+        return fail(SQLLM_EINVAL, "start=%d + n_tokens=%d must be <= capacity=%d", a->start, a->n_tokens, a->capacity);
+    if (ext_tiles(a->n_heads, a->n_kv, a->n_tokens) == 0 || a->n_kv > 65535)
+        return fail(SQLLM_EINVAL, "n_tokens=%d x %d heads per KV head needs more than %d query tiles of %d, or n_kv=%d > 65535",
+                    a->n_tokens, a->n_heads / a->n_kv, attn::MAX_TILES, attn::BM, a->n_kv);
+    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->k_cache, "k_cache"},
+                             {a->v_cache, "v_cache"}, {a->out, "out"}}))
+        return rc;
+    const bool bf = a->dtype == SQLLM_DT_BF16;
+    const KernelSmem k = a->head_dim == 128 ? (bf ? extend_kernel_of<__nv_bfloat16, 128>() : extend_kernel_of<__half, 128>())
+                                            : (bf ? extend_kernel_of<__nv_bfloat16, 64>() : extend_kernel_of<__half, 64>());
+    int sm = 0;
+    int rc = dev_setup({k}, &sm);
+    if (rc) return rc;
+    attn::ExtParams p;
+    p.qkv = a->qkv; p.cos = a->rope_cos; p.sin = a->rope_sin; p.k_cache = a->k_cache; p.v_cache = a->v_cache; p.out = a->out;
+    p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = a->n_heads / a->n_kv; p.capacity = a->capacity; p.start = a->start; p.T = a->n_tokens;
+    p.qscale = a->scale * attn::LOG2E / attn::QPRE;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    void (*append)(attn::ExtParams) = a->head_dim == 128 ? (bf ? attn::attn_append_kernel<__nv_bfloat16, 128> : attn::attn_append_kernel<__half, 128>)
+                                                         : (bf ? attn::attn_append_kernel<__nv_bfloat16, 64> : attn::attn_append_kernel<__half, 64>);
+    append<<<a->n_tokens, attn::APPEND_THREADS, 0, st>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_extend append launch failed: %s", cudaGetErrorString(e));
+    const int S = ext_splits(a->n_heads, a->n_kv, a->n_tokens, a->start, sm);
+    const dim3 grid(S, (unsigned)ext_tiles(a->n_heads, a->n_kv, a->n_tokens), a->n_kv);
+    e = launch_ex(reinterpret_cast<void (*)(attn::ExtParams)>(const_cast<void *>(k.fn)), grid, attn::XTHREADS, k.bytes, st, cluster_of(S), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_extend launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -94,6 +172,15 @@ int sqllm_attn_decode(const sqllm_attn_decode_args *a, void *stream) {
 int sqllm_attn_decode_batch(const sqllm_attn_decode_batch_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
     return attn_launch<true>(a, a->batch, stream);
+}
+
+int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int sm_count) {
+    return ext_splits(n_heads, n_kv, n_tokens, start, sm_count);
+}
+
+int sqllm_attn_extend(const sqllm_attn_extend_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return extend_launch(a, stream);
 }
 
 }  // extern "C"

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -697,6 +697,52 @@ void attn_decode_batch(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_
     check_status(sqllm_attn_decode_batch(&a, cur_stream()), "quant_cuda.attn_decode_batch");
 }
 
+// Attention of a chunk of T new tokens at positions start .. start+T-1 (sqllm_attn_extend): the append of the chunk's rotated k and v
+// at slots start .. start+T-1 of the caches, causal attention of every token over the cache up to its own position into out, on the
+// current stream.  The same check order as attn_decode: the device-free checks first.
+void attn_extend(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
+                 torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
+                                                                  {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
+    for (const auto &t : all) {
+        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), "attn_extend: ", t.second, " must be a contiguous tensor");
+        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), "attn_extend: ", t.second, " must be 16-byte aligned");
+    }
+    const auto dt = qkv.scalar_type();
+    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, "attn_extend: dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
+    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, "attn_extend: n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
+    TORCH_CHECK(k_cache.dim() == 3 && k_cache.size(0) == n_kv, "attn_extend: k_cache must be [n_kv=", n_kv, ", capacity, head_dim] (got ",
+                k_cache.sizes(), ")");
+    const int64_t cap = k_cache.size(1), d = k_cache.size(2);
+    TORCH_CHECK(d == 64 || d == 128, "attn_extend: head_dim=", d, " is not 64 or 128");
+    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, "attn_extend: capacity=", cap, " must be >= 1");
+    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), "attn_extend: scale=", scale, " must be finite and > 0");
+    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt,
+                "attn_extend: k_cache, v_cache and out must have qkv's dtype ", dt);
+    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), "attn_extend: v_cache must have k_cache's shape ", k_cache.sizes(), " (got ", v_cache.sizes(), ")");
+    TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
+                (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+    const int64_t T = qkv.size(0);
+    TORCH_CHECK(T >= 1, "attn_extend: qkv has no rows (T=0)");
+    TORCH_CHECK(start >= 0, "attn_extend: start=", start, " must be >= 0");
+    TORCH_CHECK(start + T <= cap, "attn_extend: start=", start, " + T=", T, " must be <= capacity=", cap);
+    TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend: out must be [T=", T, ", n_heads head_dim=",
+                n_heads * d, "] (got ", out.sizes(), ")");
+    for (const torch::Tensor *t : {&rope_cos, &rope_sin})
+        TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->dim() == 2 && t->size(0) == cap && t->size(1) == d / 2,
+                    "attn_extend: rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
+    for (const auto &t : all)
+        TORCH_CHECK(t.first->is_cuda() && t.first->device() == qkv.device(), "attn_extend: ", t.second, " must be a CUDA tensor, on the device of qkv");
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    sqllm_attn_extend_args a;
+    a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
+    a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
+    a.start = (int)start; a.n_tokens = (int)T;
+    a.qkv = qkv.data_ptr(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
+    a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    check_status(sqllm_attn_extend(&a, cur_stream()), "quant_cuda.attn_extend");
+}
+
 torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
     need(qweight, "qweight", torch::kInt32, qweight);
@@ -847,6 +893,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               return sqllm_attn_decode_batch_splits(n_heads, n_kv, batch, sm);
           }, "CTAs per cluster of attn_decode_batch on the current device (independent of the positions)");
     m.def("unpack_indices", &unpack_indices,"GPU unpack of the packed indices -> uint8 [in, out] (test hook)");
+    m.def("attn_extend", &attn_extend, "attention of a chunk of T new tokens at positions start .. start+T-1: rotary, the append of k / v at "
+          "slots start .. start+T-1, causal attention over the cache (qkv [T, ...], start, rope_cos, rope_sin, k_cache, v_cache, out [T, ...], "
+          "n_heads, n_kv, scale)", py::arg("qkv"), py::arg("start"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_cache"),
+          py::arg("v_cache"), py::arg("out"), py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_extend_splits", [](int n_heads, int n_kv, int n_tokens, int start) {
+              const int sm = sqllm_device_sm_count();
+              TORCH_CHECK(sm > 0, "attn_extend_splits: ", sqllm_last_error());
+              return sqllm_attn_extend_splits(n_heads, n_kv, n_tokens, start, sm);
+          }, "CTAs per cluster of attn_extend on the current device");
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },
           "fused path: True = bit-reproducible fixed-order reduction, False (default) = red.add accumulation");

@@ -362,7 +362,59 @@ def decoder_plan(model, max_len):
     return plan
 
 
-class SequenceDecoder:
+class _DecoderBase:
+    """What SequenceDecoder and BatchDecoder share: the eager layer body on rows of tokens and `extend` on the decoder's own kernels.
+    A subclass holds model, dtype, device, the stacked q/k/v and gate/up layers (qkv, gate_up), the head layout, scale, max_len and
+    the rotary tables."""
+
+    EXTEND_CHUNK = 2048  # extend() runs a prompt in chunks of at most this many tokens: it bounds the activations of one chunk
+
+    def _proj(self, layer, x):
+        """layer(x) in the model's dtype (a batch's bias is added in the bias's dtype, fp32 for a checkpoint's bias)."""
+        y = layer(x)
+        return y if y.dtype == self.dtype else y.to(self.dtype)
+
+    def _layer(self, i, layer, h, attend):
+        """Decoder layer i on the rows h [rows, hidden]: input_layernorm, the stacked q/k/v, attend(qkv) -> the attention output
+        [rows, n_heads * head_dim], o_proj plus the residual, post_attention_layernorm, the stacked gate/up, silu(g) u, down plus the
+        residual."""
+        qkv = self._proj(self.qkv[i], layer.input_layernorm(h))
+        h = h + self._proj(layer.self_attn.o_proj, attend(qkv))
+        gu = self._proj(self.gate_up[i], layer.post_attention_layernorm(h))
+        I = gu.shape[1] // 2
+        return h + self._proj(layer.mlp.down_proj, torch.nn.functional.silu(gu[:, :I]) * gu[:, I:])
+
+    def _check_extend(self, who, input_ids, start):
+        """The prompt as a 1-D int64 device tensor; ValueError before anything is written when it is empty, not 1-D or does not fit."""
+        ids = torch.as_tensor(input_ids)
+        if ids.dim() != 1 or ids.numel() == 0:
+            raise ValueError(f"{who}: input_ids must be a non-empty 1-D tensor of token ids (got shape {tuple(ids.shape)})")
+        if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+            raise ValueError(f"{who}: input_ids must hold integer token ids (got {ids.dtype})")
+        if start + ids.numel() > self.max_len:
+            raise ValueError(f"{who}: {ids.numel()} tokens at position {start} need {start + ids.numel()} cache positions, "
+                             f"max_len is {self.max_len}")
+        return ids.to(device=self.device, dtype=torch.int64)
+
+    def _extend(self, ids, start, k_cache, v_cache):
+        """The tokens ids at positions start .. start+T-1 through every layer, EXTEND_CHUNK tokens at a time, with quant_cuda.attn_extend
+        on the caches k_cache[layer], v_cache[layer] ([n_kv, max_len, head_dim] each); the logits of the last token."""
+        m = self.model.model
+        with torch.no_grad():
+            for c0 in range(0, ids.numel(), self.EXTEND_CHUNK):
+                chunk = ids[c0:c0 + self.EXTEND_CHUNK]
+                out = torch.empty(chunk.numel(), self.n_heads * self.head_dim, dtype=self.dtype, device=self.device)
+                h = torch.index_select(m.embed_tokens.weight, 0, chunk)
+                for i, layer in enumerate(m.layers):
+                    def attend(qkv, i=i):
+                        self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, k_cache[i], v_cache[i], out, self.n_heads,
+                                             self.n_kv, self.scale)
+                        return out
+                    h = self._layer(i, layer, h, attend)
+            return self.model.lm_head(m.norm(h[-1:]))[0]
+
+
+class SequenceDecoder(_DecoderBase):
     """Greedy batch-1 decode of a whole quantized LLaMA-family model (LlamaForCausalLM, MistralForCausalLM without an active sliding
     window, Qwen2ForCausalLM without sliding window) on one GPU, in fp16 or bf16.  Its q/k/v/o/gate/up/down projections must be
     QuantLinearLUT layers of one bit width (checkpoint.load_quantized / load_checkpoint, then .cuda()); lm_head may be dense or
@@ -374,7 +426,8 @@ class SequenceDecoder:
     One token is one CUDA graph replay: the embedding gather from a device token id, the prologue sequence, then per layer the
     attention kernel (quant_cuda.attn_decode: rotary, KV-cache append, attention) and the layer's DecodeSequence (decoder_plan), then
     the final norm and lm_head, the argmax into the device token id and pos += 1.  Tokens follow each other with no host
-    synchronisation.  The prompt runs through the model's own forward (prefill), whose cache is copied into the decoder's static one.
+    synchronisation.  The prompt runs through the model's own forward (prefill), whose cache is copied into the decoder's static one, or
+on the decoder's own kernels (extend), which also appends a new turn to the sequence already in the cache.
 
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
@@ -394,6 +447,8 @@ class SequenceDecoder:
         self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
         self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
         self.plan = decoder_plan(model, max_len)
+        self.qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3]) for layer in model.model.layers]
+        self.gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2]) for layer in model.model.layers]
         dev, d = self.device, self.head_dim
         with torch.cuda.device(dev), torch.no_grad():
             self.pos = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -497,6 +552,18 @@ class SequenceDecoder:
         self._pos = T
         return o.logits[0, -1]
 
+    def extend(self, input_ids):
+        """Append the tokens input_ids (1-D) at the current position on the decoder's own kernels (quant_cuda.attn_extend between the
+        layers' projections, EXTEND_CHUNK tokens at a time), advance the position by T and return the logits of the last token.  After
+        reset() this is a prefill; after prefill(), steps or an earlier extend it continues the sequence (a new turn of a chat, say).
+        Raises ValueError, with nothing written, for an empty or non-1-D prompt or one that does not fit in max_len."""
+        start = self._pos
+        ids = self._check_extend("SequenceDecoder.extend", input_ids, start)
+        logits = self._extend(ids, start, self.k_cache, self.v_cache)
+        self.pos.fill_(start + ids.numel())
+        self._pos = start + ids.numel()
+        return logits
+
     def _replay(self):
         if self._pos >= self.max_len:
             raise RuntimeError(f"SequenceDecoder: the cache is full (max_len={self.max_len}); reset() or prefill() first")
@@ -548,7 +615,7 @@ class SequenceDecoder:
         return torch.cat([ids.to(self.device), out[:n].view(1, -1)], dim=1)
 
 
-class BatchDecoder:
+class BatchDecoder(_DecoderBase):
     """Greedy decode of `batch` sequences at once (2 .. QuantLinearLUT.ROWS_MAX in fp16, 2 .. BF16_ROWS_MAX in bf16) through a whole
     quantized LLaMA-family model on one GPU: the models SequenceDecoder takes, whose projections (stacked q/k/v, o, stacked gate/up,
     down and a quantized lm_head) all fit the multi-row LUT-GEMV (QuantLinearLUT._rows_fits).
@@ -619,23 +686,16 @@ class BatchDecoder:
             self._pos = [-1] * batch
             self._capture()
 
-    def _proj(self, layer, x):
-        """layer(x) in the model's dtype (a batch's bias is added in the bias's dtype, fp32 for a checkpoint's bias)."""
-        y = layer(x)
-        return y if y.dtype == self.dtype else y.to(self.dtype)
-
     def _step(self):
         """One step on the current stream: what the graph holds."""
         m = self.model.model
         h = torch.index_select(m.embed_tokens.weight, 0, self.tok)
         for i, layer in enumerate(m.layers):
-            qkv = self._proj(self.qkv[i], layer.input_layernorm(h))
-            self._qc.attn_decode_batch(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i], self.attn_out,
-                                       self.n_heads, self.n_kv, self.scale)
-            h = h + self._proj(layer.self_attn.o_proj, self.attn_out)
-            gu = self._proj(self.gate_up[i], layer.post_attention_layernorm(h))
-            I = gu.shape[1] // 2
-            h = h + self._proj(layer.mlp.down_proj, torch.nn.functional.silu(gu[:, :I]) * gu[:, I:])
+            def attend(qkv, i=i):
+                self._qc.attn_decode_batch(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i], self.attn_out,
+                                           self.n_heads, self.n_kv, self.scale)
+                return self.attn_out
+            h = self._layer(i, layer, h, attend)
         logits = self.model.lm_head(m.norm(h))
         self.tok.copy_(logits.argmax(dim=-1))
         self.pos.add_((self.pos >= 0).to(torch.int32))
@@ -691,6 +751,19 @@ class BatchDecoder:
         self.pos[slot] = T
         self._pos[slot] = T
         return o.logits[0, -1]
+
+    def extend(self, slot, input_ids):
+        """Append the tokens input_ids (1-D) to `slot` at its position (0 for an idle slot) on the decoder's own kernels, as
+        SequenceDecoder.extend does, advance the slot's position by T and return the logits of the last token.  It reads and writes
+        nothing of the other slots, so it may run between steps while they keep their state.  Raises ValueError, with nothing written,
+        for a bad slot, an empty or non-1-D prompt or one that does not fit in max_len."""
+        slot = self._slot(slot)
+        start = max(self._pos[slot], 0)
+        ids = self._check_extend("BatchDecoder.extend", input_ids, start)
+        logits = self._extend(ids, start, self.k_cache[:, slot], self.v_cache[:, slot])
+        self.pos[slot] = start + ids.numel()
+        self._pos[slot] = start + ids.numel()
+        return logits
 
     def _replay(self):
         full = [b for b, p in enumerate(self._pos) if p >= self.max_len]
