@@ -53,7 +53,7 @@ extern "C" {
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
                                  sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
                                  sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits,
-                                 sqllm_attn_extend, sqllm_attn_extend_splits
+                                 sqllm_attn_extend, sqllm_attn_extend_splits, sqllm_sample
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -604,6 +604,43 @@ int sqllm_attn_extend(const sqllm_attn_extend_args *args, void *stream);
  * max(1, min(8, sm_count / tiles, ceil((start + n_tokens) / 64))); 0 for invalid arguments (a head layout that is not a positive
  * multiple, n_tokens < 1, start < 0, sm_count < 1, start + n_tokens above INT_MAX, more than 65535 tiles per KV head). */
 int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int sm_count);
+
+/* ---------------------------------------------------------------------------------------------
+ * Token sampling: one token per row of logits, on the device (DESIGN.md section 3.20).  Row b (b < rows) holds x_i =
+ * logits[b * row_stride + i], i < vocab, of dtype SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, read as fp32, and has the
+ * parameters temperature[b], top_k[b], top_p[b], seed[b] and pos[b], the position the sampled token will occupy in its sequence.
+ *   1. pos[b] < 0: an idle row; nothing of it is written (the guard of sqllm_attn_decode_batch).
+ *   2. Greedy: temperature[b] <= 0 or NaN, or the maximum of z below is not finite (a NaN or +inf logit, no finite logit, or x / t
+ *      overflowing): out[b] = torch.argmax of the row, the smallest index of its maximum (NaN above every number), bitwise.
+ *   3. z_i = x_i / t in fp32 (t = temperature[b]).
+ *   4. Top-k, when 0 < top_k < vocab: keep i iff z_i >= the top_k-th largest z, counted with multiplicity (ties at the edge kept).
+ *   5. Top-p, when top_p < 1: p_i = softmax(z) over the tokens kept so far; keep i iff the sum of p_j over the kept j with z_j > z_i
+ *      is < top_p (ties kept: the maximum always survives; top_p <= 0 keeps the maximum alone).  top_p >= 1 or NaN: no top-p.
+ *   6. Draw: (w0, w1, w2, w3) = Philox4x32-10(key = (seed lo32, seed hi32), counter = (i / 4, pos[b], 0, 0)), w = w_(i mod 4);
+ *      u_i = ((w >> 9) + 0.5) 2^-23 (exact in fp32, in (0, 1)); g_i = -logf(-logf(u_i)) in fp32; out[b] = the kept i with the
+ *      largest z_i + g_i (fp32), ties to the lowest index: an exact sample of the softmax over the kept set (Gumbel-max).
+ * out[b] is always in [0, vocab), whatever the logits hold.  A row's token is a pure function of its logits, its four parameters
+ * and pos[b]: it does not depend on rows, on the other rows, on the stream or on the device's SM count.  The top-p masses are
+ * exp(z - z_max) rounded to multiples of 2^-44 and summed as integers, so the top-p boundary is exact up to fp32 expf and that
+ * rounding.  Parameter values are not checked on the device.
+ * Launch shape: one thread-block cluster of min(8, ceil(vocab / 16384)) CTAs per row; no allocation, no host synchronisation, no
+ * atomics whose order matters: bit-reproducible and CUDA-graph capturable.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): dtype as above, rows in [1, 65535], vocab in
+ * [1, 262144], row_stride >= vocab, every pointer non-null and aligned to its element size. */
+typedef struct sqllm_sample_args {
+    int dtype;                /* of logits: SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int rows, vocab;
+    int64_t row_stride;       /* elements from one row of logits to the next */
+    const void *logits;       /* [rows][row_stride], the first vocab of each row read */
+    const int32_t *pos;       /* [rows] */
+    const float *temperature; /* [rows] */
+    const int32_t *top_k;     /* [rows] */
+    const float *top_p;       /* [rows] */
+    const uint64_t *seed;     /* [rows] */
+    int64_t *out;             /* [rows] token ids */
+} sqllm_sample_args;
+
+int sqllm_sample(const sqllm_sample_args *args, void *stream);
 
 /* Test hook: unpack the packed indices on the GPU exactly as the GEMV kernels do
  * (idx uint8 [in, out]); lets tests prove the integer path bit-exact on its own. */

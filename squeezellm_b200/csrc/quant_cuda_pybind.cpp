@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `sample`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -22,6 +22,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "sqllm_b200.h"
@@ -743,6 +744,43 @@ void attn_extend(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch
     check_status(sqllm_attn_extend(&a, cur_stream()), "quant_cuda.attn_extend");
 }
 
+// One token per row of logits (sqllm_sample): greedy, or temperature / top-k / top-p filtering and a Gumbel-max draw keyed by seed[b]
+// and counted by pos[b], into out[b]; a row whose pos[b] < 0 writes nothing.  Current stream, no allocation: graph-capturable.  The
+// same check order as attn_extend: the device-free checks first.
+void sample(torch::Tensor logits, torch::Tensor pos, torch::Tensor temperature, torch::Tensor top_k, torch::Tensor top_p, torch::Tensor seed,
+            torch::Tensor out) {
+    const std::pair<const torch::Tensor *, const char *> all[] = {{&logits, "logits"}, {&pos, "pos"}, {&temperature, "temperature"},
+                                                                  {&top_k, "top_k"}, {&top_p, "top_p"}, {&seed, "seed"}, {&out, "out"}};
+    for (const auto &t : all) TORCH_CHECK(t.first->defined(), "sample: ", t.second, " is undefined");
+    const auto dt = logits.scalar_type();
+    TORCH_CHECK(dt == torch::kFloat32 || dt == torch::kFloat16 || dt == torch::kBFloat16,
+                "sample: dtype of logits must be torch.float32, torch.float16 or torch.bfloat16 (got ", dt, ")");
+    TORCH_CHECK(logits.dim() == 2 && logits.size(0) >= 1 && logits.size(1) >= 1, "sample: logits must be [rows, vocab] (got ", logits.sizes(), ")");
+    const int64_t R = logits.size(0), V = logits.size(1);
+    TORCH_CHECK(R <= 65535, "sample: rows=", R, " must be in [1, 65535]");
+    TORCH_CHECK(V <= 262144, "sample: vocab=", V, " must be in [1, 262144]");
+    TORCH_CHECK(logits.stride(1) == 1 || V == 1, "sample: logits must have unit last stride (got strides ", logits.strides(), ")");
+    const int64_t row_stride = R == 1 ? V : logits.stride(0);
+    TORCH_CHECK(row_stride >= V, "sample: logits' row stride ", logits.stride(0), " must be >= vocab=", V);
+    const std::tuple<const torch::Tensor *, const char *, c10::ScalarType> vecs[] = {
+        {&pos, "pos", torch::kInt32}, {&temperature, "temperature", torch::kFloat32}, {&top_k, "top_k", torch::kInt32},
+        {&top_p, "top_p", torch::kFloat32}, {&seed, "seed", torch::kInt64}, {&out, "out", torch::kInt64}};
+    for (const auto &v : vecs) {
+        const torch::Tensor &t = *std::get<0>(v);
+        TORCH_CHECK(t.scalar_type() == std::get<2>(v) && t.dim() == 1 && t.size(0) == R && t.is_contiguous(), "sample: ", std::get<1>(v),
+                    " must be a contiguous ", std::get<2>(v), " vector of rows=", R, " elements (got ", t.scalar_type(), " ", t.sizes(), ")");
+    }
+    for (const auto &t : all)
+        TORCH_CHECK(t.first->is_cuda() && t.first->device() == logits.device(), "sample: ", t.second, " must be a CUDA tensor, on the device of logits");
+    const at::cuda::OptionalCUDAGuard guard(device_of(logits));
+    sqllm_sample_args a;
+    a.dtype = dt == torch::kFloat32 ? SQLLM_DT_F32 : dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
+    a.rows = (int)R; a.vocab = (int)V; a.row_stride = row_stride;
+    a.logits = logits.data_ptr(); a.pos = pos.data_ptr<int32_t>(); a.temperature = temperature.data_ptr<float>(); a.top_k = top_k.data_ptr<int32_t>();
+    a.top_p = top_p.data_ptr<float>(); a.seed = reinterpret_cast<const uint64_t *>(seed.data_ptr<int64_t>()); a.out = out.data_ptr<int64_t>();
+    check_status(sqllm_sample(&a, cur_stream()), "quant_cuda.sample");
+}
+
 torch::Tensor unpack_indices(torch::Tensor qweight, int bits) {
     const at::cuda::OptionalCUDAGuard guard(device_of(qweight));
     need(qweight, "qweight", torch::kInt32, qweight);
@@ -902,6 +940,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               TORCH_CHECK(sm > 0, "attn_extend_splits: ", sqllm_last_error());
               return sqllm_attn_extend_splits(n_heads, n_kv, n_tokens, start, sm);
           }, "CTAs per cluster of attn_extend on the current device");
+    m.def("sample", &sample, "one token per row of logits [rows, vocab] (fp32, fp16 or bf16; unit last stride) into out int64 [rows]: greedy "
+          "when temperature[b] <= 0, else temperature, top_k[b] (0: off) and top_p[b] (1: off) filtering and a Gumbel-max draw from "
+          "Philox4x32-10 keyed by seed[b] (int64) at counter (i / 4, pos[b]); a row whose pos[b] (int32) < 0 writes nothing; current stream",
+          py::arg("logits"), py::arg("pos"), py::arg("temperature"), py::arg("top_k"), py::arg("top_p"), py::arg("seed"), py::arg("out"));
     m.def("abi_version", []() { return sqllm_abi_version(); });
     m.def("set_deterministic", [](bool on) { sqllm_set_deterministic(on ? 1 : 0); },
           "fused path: True = bit-reproducible fixed-order reduction, False (default) = red.add accumulation");

@@ -10,6 +10,8 @@ It exists because the reference drives the path from Python one launch at a time
 (llama.py:226-234, quant_cuda_kernel.cu:147), which costs more host time per call than the kernels take on an
 H100; our kernels launch on the current stream precisely so that they can be captured.
 """
+import math
+import numbers
 from typing import NamedTuple
 
 import torch
@@ -362,12 +364,69 @@ def decoder_plan(model, max_len):
     return plan
 
 
+def _sampling(who, n, temperature, top_k, top_p, seed):
+    """generate's sampling keywords as four lists of n values, one per prompt (temperature, top_k, top_p, seed), or None when every
+    temperature is 0 (greedy: generate then launches no sampler).  A scalar applies to every prompt, except a scalar seed s, which gives
+    prompt i the seed s + i, so that identical prompts of one call do not draw alike.  Raises ValueError, before anything runs, for a
+    temperature that is negative or not finite, a top_k that is not an int >= 0, a top_p outside (0, 1], a seed outside [0, 2^63) or a
+    list whose length is not n."""
+    def per_prompt(name, v):
+        if isinstance(v, (list, tuple)):
+            if len(v) != n:
+                raise ValueError(f"{who}: {name} has {len(v)} values for {n} prompt(s)")
+            return list(v)
+        return None
+
+    def real(v):
+        return isinstance(v, numbers.Real) and not isinstance(v, bool)
+
+    def integer(v):
+        return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+    temps = per_prompt("temperature", temperature) or [temperature] * n
+    ks = per_prompt("top_k", top_k) or [top_k] * n
+    ps = per_prompt("top_p", top_p) or [top_p] * n
+    seeds = per_prompt("seed", seed) or ([seed + i for i in range(n)] if integer(seed) else [seed] * n)
+    for t in temps:
+        if not real(t) or not math.isfinite(t) or t < 0:
+            raise ValueError(f"{who}: temperature must be a finite number >= 0 (got {t!r})")
+    for k in ks:
+        if not integer(k) or k < 0:
+            raise ValueError(f"{who}: top_k must be an int >= 0 (got {k!r})")
+    for p in ps:
+        if not real(p) or not 0 < p <= 1:
+            raise ValueError(f"{who}: top_p must be a number in (0, 1] (got {p!r})")
+    for s in seeds:
+        if not integer(s) or not 0 <= s < 2**63:
+            raise ValueError(f"{who}: seed must be an int in [0, 2^63) (got {s!r})")
+    if all(t == 0 for t in temps):
+        return None
+    return [float(t) for t in temps], [min(int(k), 2**31 - 1) for k in ks], [float(p) for p in ps], [int(s) for s in seeds]
+
+
 class _DecoderBase:
     """What SequenceDecoder and BatchDecoder share: the eager layer body on rows of tokens and `extend` on the decoder's own kernels.
     A subclass holds model, dtype, device, the stacked q/k/v and gate/up layers (qkv, gate_up), the head layout, scale, max_len and
     the rotary tables."""
 
     EXTEND_CHUNK = 2048  # extend() runs a prompt in chunks of at most this many tokens: it bounds the activations of one chunk
+
+    def _sampling_buffers(self, rows):
+        """The device parameters of quant_cuda.sample, one per row: temperature, top_k, top_p and seed (greedy until generate sets them)."""
+        self.temperature = torch.zeros(rows, dtype=torch.float32, device=self.device)
+        self.top_k = torch.zeros(rows, dtype=torch.int32, device=self.device)
+        self.top_p = torch.ones(rows, dtype=torch.float32, device=self.device)
+        self.seed = torch.zeros(rows, dtype=torch.int64, device=self.device)
+
+    def _set_sampling(self, params):
+        """Rows 0 .. n-1 of the sampling buffers from _sampling's lists of n values."""
+        for buf, vals in zip((self.temperature, self.top_k, self.top_p, self.seed), params):
+            buf[:len(vals)].copy_(torch.tensor(vals, dtype=buf.dtype))
+
+    def _sample(self, logits):
+        """tok[b] = quant_cuda.sample of logits row b at pos[b], for the rows of logits; a row whose pos is -1 keeps its token."""
+        n = logits.shape[0]
+        self._qc.sample(logits, self.pos[:n], self.temperature[:n], self.top_k[:n], self.top_p[:n], self.seed[:n], self.tok[:n])
 
     def _proj(self, layer, x):
         """layer(x) in the model's dtype (a batch's bias is added in the bias's dtype, fp32 for a checkpoint's bias)."""
@@ -415,19 +474,25 @@ class _DecoderBase:
 
 
 class SequenceDecoder(_DecoderBase):
-    """Greedy batch-1 decode of a whole quantized LLaMA-family model (LlamaForCausalLM, MistralForCausalLM without an active sliding
+    """Batch-1 decode of a whole quantized LLaMA-family model (LlamaForCausalLM, MistralForCausalLM without an active sliding
     window, Qwen2ForCausalLM without sliding window) on one GPU, in fp16 or bf16.  Its q/k/v/o/gate/up/down projections must be
     QuantLinearLUT layers of one bit width (checkpoint.load_quantized / load_checkpoint, then .cuda()); lm_head may be dense or
     QuantLinearLUT.
 
         dec = SequenceDecoder(model, max_len=2048)
-        ids = dec.generate(input_ids, max_new_tokens=128, eos_token_id=tok.eos_token_id)
+        ids = dec.generate(input_ids, max_new_tokens=128, eos_token_id=tok.eos_token_id)                   # greedy
+        ids = dec.generate(input_ids, 128, eos_token_id=tok.eos_token_id, temperature=0.7, top_p=0.9, seed=1)  # sampled
 
     One token is one CUDA graph replay: the embedding gather from a device token id, the prologue sequence, then per layer the
     attention kernel (quant_cuda.attn_decode: rotary, KV-cache append, attention) and the layer's DecodeSequence (decoder_plan), then
     the final norm and lm_head, the argmax into the device token id and pos += 1.  Tokens follow each other with no host
     synchronisation.  The prompt runs through the model's own forward (prefill), whose cache is copied into the decoder's static one, or
 on the decoder's own kernels (extend), which also appends a new turn to the sequence already in the cache.
+
+    Sampling (generate's temperature, top_k, top_p and seed) runs quant_cuda.sample after each replay, on the same stream: it overwrites
+    the graph's argmax in tok with a draw keyed by the seed and counted by the position, so tokens still follow each other with no host
+    synchronisation.  A step() user samples the same way: quant_cuda.sample(dec.logits.view(1, -1), dec.pos, dec.temperature, dec.top_k,
+    dec.top_p, dec.seed, dec.tok) after step() draws the token of position dec.position (fill the four parameter buffers first).
 
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
@@ -457,6 +522,7 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
             self.v_cache = torch.zeros_like(self.k_cache)
             self.attn_out = torch.zeros(self.n_heads * d, dtype=self.dtype, device=dev)
             self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
+            self._sampling_buffers(1)
             self._build()
             self._pos = 0
             self._capture()
@@ -582,9 +648,13 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         self._replay()
         return self.logits
 
-    def generate(self, input_ids, max_new_tokens, eos_token_id=None):
-        """Greedy: input_ids [1, T] followed by up to max_new_tokens tokens, ending after the first EOS (eos_token_id: an int or a list)
-        if one comes.  The prompt and max_new_tokens - 1 steps must fit in max_len."""
+    def generate(self, input_ids, max_new_tokens, eos_token_id=None, *, temperature=0.0, top_k=0, top_p=1.0, seed=0):
+        """input_ids [1, T] followed by up to max_new_tokens tokens, ending after the first EOS (eos_token_id: an int or a list) if one
+        comes.  The prompt and max_new_tokens - 1 steps must fit in max_len.  Greedy by default; temperature > 0 samples each token with
+        quant_cuda.sample: softmax(logits / temperature), restricted to the top_k largest (0: all) and then to the smallest set of mass
+        top_p (1: all), drawn with the random stream of `seed` at the token's position, so a call is reproducible.  Each keyword may also
+        be a one-element list.  Bad values raise ValueError before anything runs (see _sampling)."""
+        sampling = _sampling("SequenceDecoder.generate", 1, temperature, top_k, top_p, seed)
         ids = torch.as_tensor(input_ids).reshape(1, -1)
         if max_new_tokens < 1:
             return ids
@@ -594,7 +664,11 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         eos = set() if eos_token_id is None else {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
         logits = self.prefill(ids)
         out = torch.empty(max_new_tokens, dtype=torch.int64, device=self.device)
-        self.tok.copy_(logits.argmax().view(1))
+        if sampling:
+            self._set_sampling(sampling)
+            self._sample(logits.view(1, -1))
+        else:
+            self.tok.copy_(logits.argmax().view(1))
         out[0:1].copy_(self.tok)
         n, seen = 1, 0
         while True:
@@ -608,6 +682,8 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
             if n == max_new_tokens:
                 break
             self._replay()
+            if sampling:
+                self._sample(self.logits.view(1, -1))
             out[n:n + 1].copy_(self.tok)
             n += 1
         for seq in self.sequences:
@@ -616,12 +692,13 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
 
 
 class BatchDecoder(_DecoderBase):
-    """Greedy decode of `batch` sequences at once (2 .. QuantLinearLUT.ROWS_MAX in fp16, 2 .. BF16_ROWS_MAX in bf16) through a whole
+    """Decode of `batch` sequences at once (2 .. QuantLinearLUT.ROWS_MAX in fp16, 2 .. BF16_ROWS_MAX in bf16) through a whole
     quantized LLaMA-family model on one GPU: the models SequenceDecoder takes, whose projections (stacked q/k/v, o, stacked gate/up,
     down and a quantized lm_head) all fit the multi-row LUT-GEMV (QuantLinearLUT._rows_fits).
 
         dec = BatchDecoder(model, max_len=2048, batch=8)
         outs = dec.generate([ids_a, ids_b, ids_c], max_new_tokens=128, eos_token_id=tok.eos_token_id)
+        outs = dec.generate([ids_a, ids_b], 128, eos_token_id=tok.eos_token_id, temperature=0.7, top_p=0.9, seed=1)
 
     Each sequence has a slot: row b of every step, block b of the cache [n_layers, batch, n_kv, max_len, head_dim] and its own device
     position pos[b], so prompts of different lengths need no padding and no mask.  A slot whose pos is -1 is idle: its row still goes
@@ -633,6 +710,11 @@ class BatchDecoder(_DecoderBase):
     cache, o_proj plus the residual, post_attention_layernorm, the stacked gate/up layer, silu(g) u, down plus the residual; the final
     norm and lm_head, the argmax per row into tok and pos[b] += 1 for the active rows.  Steps follow each other with no host
     synchronisation.  Every op of a step is row-wise, so a row's result does not depend on what the other rows hold.
+
+    Sampling (generate's temperature, top_k, top_p and seed, per prompt) runs quant_cuda.sample after each replay, on the same stream: it
+    overwrites the active rows' argmax in tok with draws keyed by each row's seed and counted by its position, so a row's tokens do not
+    depend on the other rows either.  A step() user samples the same way: quant_cuda.sample(dec.logits, dec.pos, dec.temperature,
+    dec.top_k, dec.top_p, dec.seed, dec.tok) after step() (fill the four [batch] parameter buffers first).
 
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
@@ -683,6 +765,7 @@ class BatchDecoder(_DecoderBase):
             self.v_cache = torch.zeros_like(self.k_cache)
             self.attn_out = torch.zeros(batch, self.n_heads * d, dtype=self.dtype, device=dev)
             self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
+            self._sampling_buffers(batch)
             self._pos = [-1] * batch
             self._capture()
 
@@ -782,13 +865,17 @@ class BatchDecoder(_DecoderBase):
         self._replay()
         return self.logits
 
-    def generate(self, prompts, max_new_tokens, eos_token_id=None):
-        """Greedy: each of the 1..batch prompts (1-D token ids, or [1, T]) followed by up to max_new_tokens tokens, ending after its
-        first EOS (eos_token_id: an int or a list) if one comes; prompt i runs in slot i, the other slots stay idle.  Every prompt and
-        max_new_tokens - 1 steps must fit in max_len.  Returns one 1-D tensor per prompt (prompt + new tokens), in order."""
+    def generate(self, prompts, max_new_tokens, eos_token_id=None, *, temperature=0.0, top_k=0, top_p=1.0, seed=0):
+        """Each of the 1..batch prompts (1-D token ids, or [1, T]) followed by up to max_new_tokens tokens, ending after its first EOS
+        (eos_token_id: an int or a list) if one comes; prompt i runs in slot i, the other slots stay idle.  Every prompt and
+        max_new_tokens - 1 steps must fit in max_len.  Returns one 1-D tensor per prompt (prompt + new tokens), in order.
+        Greedy by default; temperature > 0 samples as SequenceDecoder.generate does.  Each keyword is a scalar or a list of one value
+        per prompt (temperature 0 keeps that prompt greedy); a scalar seed s gives prompt i the seed s + i.  A prompt's tokens depend on
+        its own prompt, parameters and seed only.  Bad values raise ValueError before anything runs (see _sampling)."""
         prompts = [torch.as_tensor(p).reshape(-1) for p in prompts]
         if not 1 <= len(prompts) <= self.batch:
             raise ValueError(f"BatchDecoder.generate: {len(prompts)} prompts, the decoder takes 1 to {self.batch}")
+        sampling = _sampling("BatchDecoder.generate", len(prompts), temperature, top_k, top_p, seed)
         if not isinstance(max_new_tokens, int) or max_new_tokens < 1:
             raise ValueError(f"BatchDecoder.generate: max_new_tokens must be a positive int (got {max_new_tokens!r})")
         for i, p in enumerate(prompts):
@@ -801,8 +888,13 @@ class BatchDecoder(_DecoderBase):
         R = len(prompts)
         self.reset()
         out = torch.zeros(self.batch, max_new_tokens, dtype=torch.int64, device=self.device)
-        for i, p in enumerate(prompts):
-            out[i, 0] = self.prefill(i, p).argmax()
+        if sampling:
+            self._set_sampling(sampling)
+            self._sample(torch.stack([self.prefill(i, p) for i, p in enumerate(prompts)]))
+            out[:R, 0].copy_(self.tok[:R])
+        else:
+            for i, p in enumerate(prompts):
+                out[i, 0] = self.prefill(i, p).argmax()
         self.tok.copy_(out[:, 0])
         length = [None] * R  # new tokens of a finished row
         n, seen = 1, 0
@@ -821,6 +913,8 @@ class BatchDecoder(_DecoderBase):
             if n == max_new_tokens:
                 break
             self._replay()
+            if sampling:
+                self._sample(self.logits)
             out[:, n].copy_(self.tok)
             n += 1
         return [torch.cat([p.to(self.device), out[i, :length[i] if length[i] is not None else n]]) for i, p in enumerate(prompts)]
