@@ -153,13 +153,13 @@ int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t 
 // =================================================================================================
 // v2 (lutgemv_v2.cuh): plan + launch.  One CTA per SM; all process-wide state behind one mutex / atomics.
 // =================================================================================================
-typedef void (*K2)(const v2::P2, const CUtensorMap, const CUtensorMap);
-struct K2Info { K2 fn; int tab, stage; };
+typedef void (*K2)(const v2::P2, const CUtensorMap, const CUtensorMap, const CUtensorMap);
+struct K2Info { K2 fn; int tab, stage, su, ring; };
 // fused: variant 0: exact, fp32 x ; 1: exact, fp16 x ; 2: fp16 pair table, fp16 x ; 3: exact, bf16 x.  Accumulate mode (the 12
 // symbols): variant 0 only.
 constexpr int K2_VARIANTS = 4;
 K2Info k2_lookup(int bits, int variant, bool fused) {
-#define K2E(B, M, XT, F) K2Info{v2::lutgemv2_kernel<B, M, XT, F>, v2::C2<B, M>::TAB, v2::C2<B, M>::STAGE}
+#define K2E(B, M, XT, F) K2Info{v2::lutgemv2_kernel<B, M, XT, F>, v2::G2<B, M>::TAB, v2::G2<B, M>::STAGE, v2::G2<B, M>::SU, v2::G2<B, M>::RING}
     if (bits == 4) {
         if (!fused) return K2E(4, 0, float, false);
         if (variant == 0) return K2E(4, 0, float, true);
@@ -197,11 +197,11 @@ int plan_layer(const sqllm_lutgemv_args &a, int sm, v2::P2 &p, int &G) {
     return SQLLM_OK;
 }
 
-// The two tensor maps over the packed matrix: 64 columns x (32 units | 2 units) boxes.
-int tensor_maps(const sqllm_lutgemv_args &a, CUtensorMap &big, CUtensorMap &small) {
+// The two tensor maps over the packed matrix: 64 columns x (su units per stage | 2 units) boxes.
+int tensor_maps(const sqllm_lutgemv_args &a, int su, CUtensorMap &big, CUtensorMap &small) {
     const int rows_per_unit = a.bits == 4 ? 1 : 3, qrows = a.in_features / 32 * a.bits;
     // (a matrix shorter than one full stage never issues the big box; its map is clamped so that the encoder accepts it)
-    const int rc = get_tensor_map(a.qweight, qrows, a.out_features, qrows < v2::SU2 * rows_per_unit ? 2 * rows_per_unit : v2::SU2 * rows_per_unit, big);
+    const int rc = get_tensor_map(a.qweight, qrows, a.out_features, qrows < su * rows_per_unit ? 2 * rows_per_unit : su * rows_per_unit, big);
     return rc ? rc : get_tensor_map(a.qweight, qrows, a.out_features, 2 * rows_per_unit, small);
 }
 
@@ -223,8 +223,8 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
     if (fused && G > MAX_GRID_V2) return fail(SQLLM_EINVAL, "grid of %d CTAs exceeds the mailbox area (%d)", G, MAX_GRID_V2);
     const unsigned base = (raw + 127u) & ~127u;
     const unsigned xbytes = (unsigned)((p.K * (variant == 0 ? 4 : 2) + 127) & ~127);  // this layer's x, in its own dtype
-    // one GEMV: the ring needs no more stages than the CTA's chunk fills
-    const int n = v2::Carve(base, xbytes, 0u, ki.tab, 2, ki.stage, 0).depth(raw, 227 * 1024, ki.stage, (p.chunk + v2::SU2 - 1) / v2::SU2 + 1);
+    // one GEMV: the ring needs no more stages than the CTA's chunk fills, and no more than the mode's limit
+    const int n = v2::Carve(base, xbytes, 0u, ki.tab, 2, ki.stage, 0).depth(raw, 227 * 1024, ki.stage, std::min((p.chunk + ki.su - 1) / ki.su + 1, ki.ring));
     if (n < 0) return fail(SQLLM_EINVAL, "in_features=%d does not fit the shared-memory carve-up of this table mode", p.K);
     if (n < 2) return fail(SQLLM_EINVAL, "in_features=%d leaves no room for a weight ring in shared memory", p.K);
     const int smem = (int)(v2::Carve(base, xbytes, 0u, ki.tab, 2, ki.stage, n).end - raw);
@@ -242,9 +242,11 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
         if (g_trace) g_trace += g_trace_stride;
         g_last_grid = G;
     }
-    CUtensorMap tm_big, tm_small;
-    if ((rc = tensor_maps(*a, tm_big, tm_small))) return rc;
-    const cudaError_t e = launch_ex(ki.fn, G, v2::THREADS2, smem, st, PDL, p, tm_big, tm_small);
+    CUtensorMap tm_big, tm_small, tm_mid{};
+    if ((rc = tensor_maps(*a, ki.su, tm_big, tm_small))) return rc;
+    // 64-unit stages: the first 32 units of a ragged stage (the other modes do not read this map)
+    if (ki.su > v2::SU2 && (rc = tensor_maps(*a, v2::SU2, tm_mid, tm_small))) return rc;
+    const cudaError_t e = launch_ex(ki.fn, G, v2::THREADS2, smem, st, PDL, p, tm_big, tm_small, tm_mid);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -505,7 +507,7 @@ extern "C" int sqllm_sequence_create_ops(const sqllm_seq_item *items, const sqll
         p.trace = opt->trace ? reinterpret_cast<unsigned long long *>(opt->trace) + (size_t)i * 1024 * 32 : nullptr;
         d.x_tag = it.x_from < 0 ? nullptr : reinterpret_cast<const uint32_t *>(static_cast<unsigned char *>(s->d_arena) + yoff[it.x_from]) + it.x_offset;
         d.y_off = yoff[i];
-        if ((rc = tensor_maps(a, d.tm_big, d.tm_small))) return seq_fail_free(s, rc);
+        if ((rc = tensor_maps(a, v2::SU2, d.tm_big, d.tm_small))) return seq_fail_free(s, rc);
     }
     std::vector<seq::SeqExport> ex(std::max(1, opt->n_export));
     for (int e = 0; e < opt->n_export; ++e) {

@@ -86,6 +86,20 @@ struct C2 {
     static constexpr int STAGE = SU2 * UNIT;                 // 8 KB / 24 KB
     static constexpr int NTB = TAB <= 16384 ? 4 : 2;         // sequence kernel: table buffers (and strip accumulators), 4 x 4 KB exact, 2 x 64 KB for the 4-bit pair table
 };
+// The one-GEMV kernel's plan (lutgemv2_kernel; the sequence kernel keeps C2's).  4-bit exact (ROT): a stage is 64 units, two positions per
+// consumer warp behind one full-barrier wait, and a table buffer holds the strip table twice - copy 0 for the even half-warps, copy 1
+// (4 KB above, entry of slot s at slot s ^ 16: bank-rotated by 16) for the odd ones, so that both read column t of their lane with
+// word t and still hit 32 different banks.  Every other mode: 32-unit stages and one copy, as C2.
+template <int BITS, int MODE>
+struct G2 : C2<BITS, MODE> {
+    static constexpr bool ROT = BITS == 4 && MODE == 0;
+    static constexpr int SU = ROT ? 2 * SU2 : SU2;           // units per stage
+    static constexpr int STAGE = SU * C2<BITS, MODE>::UNIT;  // 16 KB 4-bit exact ; 8 KB / 24 KB otherwise
+    static constexpr int TAB = (ROT ? 2 : 1) * C2<BITS, MODE>::TAB;
+    // ring depth limit.  ROT: 3 stages (48 KB per SM).  Measured on the 7B chain (DESIGN §6), a shallow ring is faster: with 132 SMs
+    // each holding 128 KB of requests at once, the launch's last CTAs finish later than with 48 KB.
+    static constexpr int RING = ROT ? 3 : MAXD;
+};
 
 // Shared-memory carve-up of lutgemv2_kernel and lutgemv_seq_kernel, from the 128-byte aligned base:
 //   [fixed OFF_X][x: xbytes][front][ring stages 0 .. n_lo)[ntab tables, each aligned to its own size][ring stages n_lo .. nstage)
@@ -209,7 +223,8 @@ __device__ __forceinline__ void lut_prefetch(const P2 &p, const uint32_t lutbuf,
     cp_async_commit();
 }
 
-template <int BITS, int MODE>
+// ROT (G2): also the bank-rotated second copy of the exact table, C2::TAB bytes above the first.
+template <int BITS, int MODE, bool ROT = false>
 __device__ __forceinline__ void build_table(const uint32_t tab, const uint32_t lutbuf, const int slot) {
     using C = C2<BITS, MODE>;
     const uint32_t row = lutbuf + slot * (C::L * 4 + 16);    // the staged LUT row of the column this slot serves (slot s <-> column (s & 15) * 4 + (s >> 4))
@@ -223,6 +238,11 @@ __device__ __forceinline__ void build_table(const uint32_t tab, const uint32_t l
     if constexpr (MODE == 0) {
 #pragma unroll
         for (int e = 0; e < C::L; ++e) sts_u32(a0 + e * (STRIP * 4), __float_as_uint(v[e]));
+        if constexpr (ROT) {
+            const uint32_t a1 = tab + C::TAB + ((slot ^ 16) << 2);
+#pragma unroll
+            for (int e = 0; e < C::L; ++e) sts_u32(a1 + e * (STRIP * 4), __float_as_uint(v[e]));
+        }
     } else {
         uint32_t H[C::L / 2];  // H[m] = half2(LUT[2m], LUT[2m+1])
 #pragma unroll
@@ -588,8 +608,9 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
 // ---------------------------------------------------------------------------------------------------------------------------
 template <int BITS, int MODE, typename XT, bool FUSED>
 __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const __grid_constant__ CUtensorMap tm_big,
-                                                               const __grid_constant__ CUtensorMap tm_small) {
-    using C = C2<BITS, MODE>;
+                                                               const __grid_constant__ CUtensorMap tm_small,
+                                                               const __grid_constant__ CUtensorMap tm_mid) {
+    using C = G2<BITS, MODE>;
     using Y16 = y16_t<XT>;
     static_assert(MODE == 0 || std::is_same<XT, __half>::value, "the pair table multiplies fp16 by fp16: it needs fp16 x");
     extern __shared__ unsigned char smem_raw[];
@@ -632,6 +653,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_big)) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_small)) : "memory");
+            if constexpr (C::ROT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_mid)) : "memory");
         }
         const int G = (int)gridDim.x;
         const size_t lut_lines = ((size_t)N * C::L * 4 + 127) / 128, per = (lut_lines + G - 1) / G;
@@ -648,7 +670,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
 
     if (warp == WARP_PROD) {
         // =========================== TMA producer: weights never depend on the previous kernel ===========================
-        // Stages never straddle a strip: segment `seg` (the CTA's part of strip s0+seg) is cut into stages of SU2 units from its own start.
+        // Stages never straddle a strip: segment `seg` (the CTA's part of strip s0+seg) is cut into stages of C::SU units from its own start.
         // (Also tried: cp.async.bulk.prefetch.tensor into L2 16-24 stages ahead of the ring - slower on every shape, like the
         // L2 prefetch experiment of round 1.)
         const uint64_t pol = l2_evict_first_policy();
@@ -660,18 +682,22 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             const int seglen = send - sstart;
             const int u0 = r0 + sstart - seg * R;  // unit-in-strip of the segment's first unit
             const int col0 = (s0 + seg) * STRIP;
-            for (int u = 0; u < seglen; u += SU2) {
+            for (int u = 0; u < seglen; u += C::SU) {
                 if (refill) mbar_wait(bar_u32 + 128 + 8 * slot, ph);
-                const int nu = min(SU2, seglen - u);
+                const int nu = min(C::SU, seglen - u);
                 const uint32_t full = bar_u32 + 8 * slot;
                 const uint32_t dst = (slot < n_lo ? lo_base : hi_base) + slot * C::STAGE;
                 const int row0 = (u0 + u) * C::ROWS;
                 if (lane == 0) mbar_expect_tx(full, (uint32_t)nu * C::UNIT);
                 __syncwarp();
-                if (nu == SU2) {
+                if (nu == C::SU) {
                     if (lane == 0) tma_tile2d_g2s(dst, &tm_big, col0, row0, full, pol);
-                } else if (2 * lane < nu) {
-                    tma_tile2d_g2s(dst + lane * 2 * C::UNIT, &tm_small, col0, row0 + lane * 2 * C::ROWS, full, pol);
+                } else {
+                    // ROT: a ragged stage of 32 units or more starts with one 32-unit box (tm_mid), so that it takes no more copies than
+                    // with 32-unit stages - the TMA unit retires small boxes slowly
+                    const int um = C::ROT && nu >= SU2 ? SU2 : 0;
+                    if (C::ROT && um && lane == 0) tma_tile2d_g2s(dst, &tm_mid, col0, row0, full, pol);
+                    if (2 * lane < nu - um) tma_tile2d_g2s(dst + (um + lane * 2) * C::UNIT, &tm_small, col0, row0 + (um + lane * 2) * C::ROWS, full, pol);
                 }
                 if (++slot == nstage) {
                     slot = 0;
@@ -726,7 +752,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             if (s + 1 < nseg) cp_async_wait_pending<1>();  // all but the newest group (the next strip's rows) have landed
             else cp_async_wait_all();
             named_bar_sync(3, NBT);  // the strip's LUT rows are in shared memory, all of them
-            build_table<BITS, MODE>(tab0 + b * C::TAB, lutbuf + b * LUTBUF, bt);
+            build_table<BITS, MODE, C::ROT>(tab0 + b * C::TAB, lutbuf + b * LUTBUF, bt);
             named_bar_sync(3, NBT);  // both warps are done reading the rows (and writing the table)
             if (lane == 0) mbar_arrive(bar_u32 + 256 + 8 * b);
             if (s + 2 < nseg) lut_prefetch<BITS>(p, lutbuf + b * LUTBUF, s0 + s + 2, bt);  // this buffer's next strip: long there when it is needed
@@ -977,7 +1003,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         const uint32_t sacc_lane = base + OFF_SACC + (4 * i16) * 4;
         const uint32_t lane_in_stage = (uint32_t)((2 * warp + jsel) * C::UNIT + i16 * 16);
         constexpr int XB = C::XU * (int)sizeof(XT);  // bytes of x per unit
-        constexpr int XBS = SU2 * XB;             // ... per stage
+        constexpr int XBS = SU2 * XB;             // ... per 32 units (a stage; ROT: half a stage)
 
         int slot = 0;
         uint32_t par = 0;
@@ -986,8 +1012,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         for (int seg = 0; seg < nseg; ++seg) {
             const int b = seg & 1;
             // slot addresses of this lane's 4 columns in table b: column (t ^ jsel) -> slot ((t ^ jsel) << 4 | i16); the table base bits above
-            // the row field come with them (exact 4-bit: bits 12..15 ride in segc instead, because byte 1 of the address is built by PRMT)
-            const uint32_t tab = tab0 + b * C::TAB;
+            // the row field come with them (exact 4-bit: bits 12..15 ride in segc instead, because byte 1 of the address is built by PRMT).
+            // ROT: the odd half-warp reads copy 1, where slot ((t ^ 1) << 4 | i16) holds ITS column t.
+            const uint32_t tab = tab0 + b * C::TAB + (C::ROT ? (uint32_t)jsel * (C::TAB / 2) : 0u);
             const uint32_t tb_hi = (MODE == 1 && BITS == 4) ? tab : (BITS == 4 ? (tab & 0xFFFF0000u) : tab);
             uint32_t l[4];
 #pragma unroll
@@ -1000,30 +1027,50 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             const int seglen = send - sstart;
             const int u0 = r0 + sstart - seg * R;
             uint32_t xaddr = xs_u32 + (uint32_t)((u0 + 2 * warp + jsel) * XB);
-            const int nstg = (seglen + SU2 - 1) / SU2;
-            const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;  // stages in which this warp has a pair
+            const int nstg = (seglen + C::SU - 1) / C::SU;
+            const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;  // positions (32-unit steps) in which this warp has a pair
 
             mbar_wait(bar_u32 + 256 + 8 * b, (uint32_t)((seg >> 1) & 1));  // table b holds this strip
             TRACE(16 + (seg < 7 ? seg : 7), tid == 0);
             // Every consumer warp walks every stage of the segment (the empty barriers count NWC arrivals); a warp whose pair lies past
-            // the end of a ragged last stage just releases it.  One stage per trip, no look-ahead: the smallest loop body.  (A two-stage
+            // the end of a ragged last stage just releases it.  One stage per trip, no look-ahead across stages.  (A two-stage
             // ping-pong variant that hides the word fetch behind the previous position's gathers doubles the body to ~290 instructions;
             // with 23 warps in five roles on the SM the instruction cache misses ate the gain - ncu showed many stall samples on
             // "no instruction".)
-            for (int k = 0; k < nstg; ++k) {
-                mbar_wait(bar_u32 + 8 * slot, par);
-                if (k < mine) {
-                    Fetch<BITS, XT> F;
-                    fetch2<BITS, XT>(F, stage_of(slot), xaddr);
-                    math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
+            if constexpr (C::ROT) {
+                // 64-unit stages: position p of stage k is unit 32p + 2 warp + jsel, so a lane meets its units in the same order as with
+                // 32-unit stages (same FMA order).  Both positions' words and x are read before the first gather; the second position's
+                // reads may run past a ragged stage's end (stale ring bytes, x past K: still inside the window), its math is skipped.
+                for (int k = 0; k < nstg; ++k) {
+                    mbar_wait(bar_u32 + 8 * slot, par);
+                    if (2 * k < mine) {
+                        Fetch<BITS, XT> F0, F1;
+                        fetch2<BITS, XT>(F0, stage_of(slot), xaddr);
+                        fetch2<BITS, XT>(F1, stage_of(slot) + SU2 * C::UNIT, xaddr + XBS);
+                        math2<BITS, MODE, XT>(F0, 0, l, segc, xaddr, A);
+                        if (2 * k + 1 < mine) math2<BITS, MODE, XT>(F1, 0, l, segc, xaddr, A);
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
+                    advance();
+                    xaddr += 2 * XBS;
                 }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
-                advance();
-                xaddr += XBS;
+            } else {
+                for (int k = 0; k < nstg; ++k) {
+                    mbar_wait(bar_u32 + 8 * slot, par);
+                    if (k < mine) {
+                        Fetch<BITS, XT> F;
+                        fetch2<BITS, XT>(F, stage_of(slot), xaddr);
+                        math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
+                    advance();
+                    xaddr += XBS;
+                }
             }
-            {   // this strip's sums: lane (i, j=1) holds column t^1 in slot t - hand it to lane (i, j=0), which adds both into the CTA's
-                // shared accumulator of the strip (16 warps x 64 red.shared.add; the builders move it on to global memory)
+            {   // this strip's sums: lane (i, j=1) holds column t^1 in slot t (ROT: column t) - hand it to lane (i, j=0), which adds both
+                // into the CTA's shared accumulator of the strip (16 warps x 64 red.shared.add; the builders move it on to global memory)
                 float s[4];
 #pragma unroll
                 for (int t = 0; t < 4; ++t) {
@@ -1032,10 +1079,11 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                     A.f[t] = 0.f;
                     A.f[t + 4] = 0.f;
                 }
-                const float v0 = __shfl_xor_sync(0xffffffffu, s[1], 16);
-                const float v1 = __shfl_xor_sync(0xffffffffu, s[0], 16);
-                const float v2 = __shfl_xor_sync(0xffffffffu, s[3], 16);
-                const float v3 = __shfl_xor_sync(0xffffffffu, s[2], 16);
+                constexpr int SW = C::ROT ? 0 : 1;
+                const float v0 = __shfl_xor_sync(0xffffffffu, s[0 ^ SW], 16);
+                const float v1 = __shfl_xor_sync(0xffffffffu, s[1 ^ SW], 16);
+                const float v2 = __shfl_xor_sync(0xffffffffu, s[2 ^ SW], 16);
+                const float v3 = __shfl_xor_sync(0xffffffffu, s[3 ^ SW], 16);
                 if (jsel == 0 && mine > 0) {
                     const uint32_t a = sacc_lane + b * (STRIP * 4);
                     asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(s[0] + v0) : "memory");
