@@ -71,7 +71,8 @@ __device__ __forceinline__ void unpack8(const uint4 w, float (&f)[8]) {
 // exp2(a - b) with exp2(-inf) = 0 whatever b is (an empty state or a masked position weighs nothing)
 __device__ __forceinline__ float wexp2(float a, float b) { return a == -INFINITY ? 0.f : exp2f(a - b); }
 
-// batch 1: one sequence at *p.pos
+// batch 1: one sequence at *p.pos.  Kept beside the batched kernel, which computes the same bits at batch 1 but up to 0.9 % slower
+// (DESIGN §3.18)
 template <typename T, int D, int G>
 __global__ void __launch_bounds__(THREADS, 1) attn_decode_kernel(const Params p) {
 #include "attn_decode_row.inc"

@@ -610,143 +610,109 @@ void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, 
                  "quant_cuda.fisher_accumulate");
 }
 
-// One layer's decode attention (sqllm_attn_decode): rotary, the append of k / v at slot *pos of the caches, attention over slots
-// 0..*pos into out, on the current stream.  The checks that need no device run first, on tensors of any device, so that a CPU caller
-// sees the same rejections; then every tensor must be a CUDA tensor on qkv's device.
-void attn_decode(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
-                 torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
-    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {&pos, "pos"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
+// The argument checks attn_decode, attn_decode_batch and attn_extend share, in the order they run, each message prefixed with `fn`:
+// every tensor contiguous and 16-byte aligned, qkv's dtype, the head layout, k_cache [batch (lead = 1 only), n_kv, capacity, head_dim],
+// the batch, head_dim, capacity, scale, the cache and out dtypes and v_cache's shape; then own(batch, capacity, head_dim), the binding's
+// own shape checks; then the rope tables.  The device checks come last, so that a CPU caller sees the same rejections.  pos: null for
+// attn_extend.  -> the sqllm args with the fields the three share.
+template <typename Args, typename Own>
+Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::Tensor *pos, const torch::Tensor &rope_cos,
+               const torch::Tensor &rope_sin, const torch::Tensor &k_cache, const torch::Tensor &v_cache, const torch::Tensor &out,
+               int64_t n_heads, int64_t n_kv, double scale, Own own) {
+    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {pos, "pos"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
                                                                   {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
     for (const auto &t : all) {
-        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), "attn_decode: ", t.second, " must be a contiguous tensor");
-        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), "attn_decode: ", t.second, " must be 16-byte aligned");
+        if (!t.first) continue;
+        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), fn, ": ", t.second, " must be a contiguous tensor");
+        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), fn, ": ", t.second, " must be 16-byte aligned");
     }
     const auto dt = qkv.scalar_type();
-    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, "attn_decode: dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
-    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, "attn_decode: n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
-    TORCH_CHECK(k_cache.dim() == 3 && k_cache.size(0) == n_kv, "attn_decode: k_cache must be [n_kv=", n_kv, ", capacity, head_dim] (got ",
-                k_cache.sizes(), ")");
-    const int64_t cap = k_cache.size(1), d = k_cache.size(2);
-    TORCH_CHECK(d == 64 || d == 128, "attn_decode: head_dim=", d, " is not 64 or 128");
-    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, "attn_decode: capacity=", cap, " must be >= 1");
-    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), "attn_decode: scale=", scale, " must be finite and > 0");
-    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt,
-                "attn_decode: k_cache, v_cache and out must have qkv's dtype ", dt);
-    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), "attn_decode: v_cache must have k_cache's shape ", k_cache.sizes(), " (got ", v_cache.sizes(), ")");
-    TORCH_CHECK(qkv.numel() == (n_heads + 2 * n_kv) * d, "attn_decode: qkv has ", qkv.numel(), " elements, want (n_heads + 2 n_kv) head_dim = ",
-                (n_heads + 2 * n_kv) * d);
-    TORCH_CHECK(out.numel() == n_heads * d, "attn_decode: out has ", out.numel(), " elements, want n_heads head_dim = ", n_heads * d);
-    TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.numel() == 1, "attn_decode: pos must be one int32 element");
+    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, fn, ": dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
+    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, fn, ": n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
+    TORCH_CHECK(k_cache.dim() == 3 + lead && k_cache.size(lead) == n_kv, fn, ": k_cache must be [", lead ? "batch, " : "", "n_kv=", n_kv,
+                ", capacity, head_dim] (got ", k_cache.sizes(), ")");
+    const int64_t B = lead ? k_cache.size(0) : 1, cap = k_cache.size(lead + 1), d = k_cache.size(lead + 2);
+    TORCH_CHECK(B >= 1 && B <= 65535, fn, ": batch=", B, " must be in [1, 65535]");
+    TORCH_CHECK(d == 64 || d == 128, fn, ": head_dim=", d, " is not 64 or 128");
+    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, fn, ": capacity=", cap, " must be >= 1");
+    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), fn, ": scale=", scale, " must be finite and > 0");
+    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt, fn,
+                ": k_cache, v_cache and out must have qkv's dtype ", dt);
+    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), fn, ": v_cache must have k_cache's shape ", k_cache.sizes(), " (got ", v_cache.sizes(), ")");
+    own(B, cap, d);
     for (const torch::Tensor *t : {&rope_cos, &rope_sin})
         TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->dim() == 2 && t->size(0) == cap && t->size(1) == d / 2,
-                    "attn_decode: rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
+                    fn, ": rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
     for (const auto &t : all)
-        TORCH_CHECK(t.first->is_cuda() && t.first->device() == qkv.device(), "attn_decode: ", t.second, " must be a CUDA tensor, on the device of qkv");
-    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
-    sqllm_attn_decode_args a;
+        TORCH_CHECK(!t.first || (t.first->is_cuda() && t.first->device() == qkv.device()), fn, ": ", t.second,
+                    " must be a CUDA tensor, on the device of qkv");
+    Args a;
     a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
     a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
-    a.qkv = qkv.data_ptr(); a.pos = pos.data_ptr<int32_t>(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
+    a.qkv = qkv.data_ptr(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
     a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    return a;
+}
+
+// One layer's decode attention (sqllm_attn_decode): rotary, the append of k / v at slot *pos of the caches, attention over slots
+// 0..*pos into out, on the current stream.
+void attn_decode(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
+                 torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_decode_args>("attn_decode", 0, qkv, &pos, rope_cos, rope_sin, k_cache, v_cache, out, n_heads, n_kv, scale,
+                                               [&](int64_t, int64_t, int64_t d) {
+        TORCH_CHECK(qkv.numel() == (n_heads + 2 * n_kv) * d, "attn_decode: qkv has ", qkv.numel(), " elements, want (n_heads + 2 n_kv) head_dim = ",
+                    (n_heads + 2 * n_kv) * d);
+        TORCH_CHECK(out.numel() == n_heads * d, "attn_decode: out has ", out.numel(), " elements, want n_heads head_dim = ", n_heads * d);
+        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.numel() == 1, "attn_decode: pos must be one int32 element");
+    });
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    a.pos = pos.data_ptr<int32_t>();
     check_status(sqllm_attn_decode(&a, cur_stream()), "quant_cuda.attn_decode");
 }
 
 // Decode attention of B sequences (sqllm_attn_decode_batch): for each row b what attn_decode does, at position pos[b] in cache block b;
-// a row whose pos[b] is outside the cache writes nothing.  The same check order as attn_decode: the device-free checks first.
+// a row whose pos[b] is outside the cache writes nothing.
 void attn_decode_batch(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
                        torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
-    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {&pos, "pos"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
-                                                                  {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
-    for (const auto &t : all) {
-        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), "attn_decode_batch: ", t.second, " must be a contiguous tensor");
-        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), "attn_decode_batch: ", t.second, " must be 16-byte aligned");
-    }
-    const auto dt = qkv.scalar_type();
-    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, "attn_decode_batch: dtype of qkv must be torch.float16 or torch.bfloat16 (got ",
-                dt, ")");
-    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, "attn_decode_batch: n_heads=", n_heads, " must be a positive multiple of n_kv=",
-                n_kv);
-    TORCH_CHECK(k_cache.dim() == 4 && k_cache.size(1) == n_kv, "attn_decode_batch: k_cache must be [batch, n_kv=", n_kv,
-                ", capacity, head_dim] (got ", k_cache.sizes(), ")");
-    const int64_t B = k_cache.size(0), cap = k_cache.size(2), d = k_cache.size(3);
-    TORCH_CHECK(B >= 1 && B <= 65535, "attn_decode_batch: batch=", B, " must be in [1, 65535]");
-    TORCH_CHECK(d == 64 || d == 128, "attn_decode_batch: head_dim=", d, " is not 64 or 128");
-    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, "attn_decode_batch: capacity=", cap, " must be >= 1");
-    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), "attn_decode_batch: scale=", scale, " must be finite and > 0");
-    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt,
-                "attn_decode_batch: k_cache, v_cache and out must have qkv's dtype ", dt);
-    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), "attn_decode_batch: v_cache must have k_cache's shape ", k_cache.sizes(), " (got ",
-                v_cache.sizes(), ")");
-    TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_decode_batch: qkv must be [batch=", B,
-                ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-    TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, "attn_decode_batch: out must be [batch=", B,
-                ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
-    TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, "attn_decode_batch: pos must be int32 [batch=", B,
-                "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
-    for (const torch::Tensor *t : {&rope_cos, &rope_sin})
-        TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->dim() == 2 && t->size(0) == cap && t->size(1) == d / 2,
-                    "attn_decode_batch: rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
-    for (const auto &t : all)
-        TORCH_CHECK(t.first->is_cuda() && t.first->device() == qkv.device(), "attn_decode_batch: ", t.second,
-                    " must be a CUDA tensor, on the device of qkv");
+    auto a = attn_args<sqllm_attn_decode_batch_args>("attn_decode_batch", 1, qkv, &pos, rope_cos, rope_sin, k_cache, v_cache, out, n_heads,
+                                                     n_kv, scale, [&](int64_t B, int64_t, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_decode_batch: qkv must be [batch=", B,
+                    ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, "attn_decode_batch: out must be [batch=", B,
+                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
+        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, "attn_decode_batch: pos must be int32 [batch=", B,
+                    "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
+    });
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
-    sqllm_attn_decode_batch_args a;
-    a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
-    a.batch = (int)B; a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
-    a.qkv = qkv.data_ptr(); a.pos = pos.data_ptr<int32_t>(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
-    a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    a.batch = (int)k_cache.size(0);
+    a.pos = pos.data_ptr<int32_t>();
     check_status(sqllm_attn_decode_batch(&a, cur_stream()), "quant_cuda.attn_decode_batch");
 }
 
 // Attention of a chunk of T new tokens at positions start .. start+T-1 (sqllm_attn_extend): the append of the chunk's rotated k and v
 // at slots start .. start+T-1 of the caches, causal attention of every token over the cache up to its own position into out, on the
-// current stream.  The same check order as attn_decode: the device-free checks first.
+// current stream.
 void attn_extend(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
                  torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
-    const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
-                                                                  {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
-    for (const auto &t : all) {
-        TORCH_CHECK(t.first->defined() && t.first->is_contiguous(), "attn_extend: ", t.second, " must be a contiguous tensor");
-        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(t.first->data_ptr()) & 15), "attn_extend: ", t.second, " must be 16-byte aligned");
-    }
-    const auto dt = qkv.scalar_type();
-    TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, "attn_extend: dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
-    TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, "attn_extend: n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
-    TORCH_CHECK(k_cache.dim() == 3 && k_cache.size(0) == n_kv, "attn_extend: k_cache must be [n_kv=", n_kv, ", capacity, head_dim] (got ",
-                k_cache.sizes(), ")");
-    const int64_t cap = k_cache.size(1), d = k_cache.size(2);
-    TORCH_CHECK(d == 64 || d == 128, "attn_extend: head_dim=", d, " is not 64 or 128");
-    TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, "attn_extend: capacity=", cap, " must be >= 1");
-    TORCH_CHECK(std::isfinite(scale) && scale > 0 && std::isfinite((float)scale), "attn_extend: scale=", scale, " must be finite and > 0");
-    TORCH_CHECK(k_cache.scalar_type() == dt && v_cache.scalar_type() == dt && out.scalar_type() == dt,
-                "attn_extend: k_cache, v_cache and out must have qkv's dtype ", dt);
-    TORCH_CHECK(v_cache.sizes() == k_cache.sizes(), "attn_extend: v_cache must have k_cache's shape ", k_cache.sizes(), " (got ", v_cache.sizes(), ")");
-    TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
-                (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-    const int64_t T = qkv.size(0);
-    TORCH_CHECK(T >= 1, "attn_extend: qkv has no rows (T=0)");
-    TORCH_CHECK(start >= 0, "attn_extend: start=", start, " must be >= 0");
-    TORCH_CHECK(start + T <= cap, "attn_extend: start=", start, " + T=", T, " must be <= capacity=", cap);
-    TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend: out must be [T=", T, ", n_heads head_dim=",
-                n_heads * d, "] (got ", out.sizes(), ")");
-    for (const torch::Tensor *t : {&rope_cos, &rope_sin})
-        TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->dim() == 2 && t->size(0) == cap && t->size(1) == d / 2,
-                    "attn_extend: rope_cos / rope_sin must be fp32 [capacity=", cap, ", head_dim/2=", d / 2, "] (got ", t->sizes(), ")");
-    for (const auto &t : all)
-        TORCH_CHECK(t.first->is_cuda() && t.first->device() == qkv.device(), "attn_extend: ", t.second, " must be a CUDA tensor, on the device of qkv");
+    auto a = attn_args<sqllm_attn_extend_args>("attn_extend", 0, qkv, nullptr, rope_cos, rope_sin, k_cache, v_cache, out, n_heads, n_kv, scale,
+                                               [&](int64_t, int64_t cap, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
+                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        const int64_t T = qkv.size(0);
+        TORCH_CHECK(T >= 1, "attn_extend: qkv has no rows (T=0)");
+        TORCH_CHECK(start >= 0, "attn_extend: start=", start, " must be >= 0");
+        TORCH_CHECK(start + T <= cap, "attn_extend: start=", start, " + T=", T, " must be <= capacity=", cap);
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend: out must be [T=", T, ", n_heads head_dim=",
+                    n_heads * d, "] (got ", out.sizes(), ")");
+    });
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
-    sqllm_attn_extend_args a;
-    a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
-    a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
-    a.start = (int)start; a.n_tokens = (int)T;
-    a.qkv = qkv.data_ptr(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
-    a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    a.start = (int)start; a.n_tokens = (int)qkv.size(0);
     check_status(sqllm_attn_extend(&a, cur_stream()), "quant_cuda.attn_extend");
 }
 
 // One token per row of logits (sqllm_sample): greedy, or temperature / top-k / top-p filtering and a Gumbel-max draw keyed by seed[b]
 // and counted by pos[b], into out[b]; a row whose pos[b] < 0 writes nothing.  Current stream, no allocation: graph-capturable.  The
-// same check order as attn_extend: the device-free checks first.
+// device-free checks run first, as in the attention bindings.
 void sample(torch::Tensor logits, torch::Tensor pos, torch::Tensor temperature, torch::Tensor top_k, torch::Tensor top_p, torch::Tensor seed,
             torch::Tensor out) {
     const std::pair<const torch::Tensor *, const char *> all[] = {{&logits, "logits"}, {&pos, "pos"}, {&temperature, "temperature"},

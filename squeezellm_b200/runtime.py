@@ -307,7 +307,7 @@ def _decoder_layout(model, max_len, who="SequenceDecoder"):
     return layers
 
 
-def _stacked(module, names, who="SequenceDecoder"):
+def _stacked(module, names, who):
     """The stacked layer of the sibling group that holds exactly module.<names>, in that order."""
     ms = [getattr(module, n) for n in names]
     g = ms[0]._sibling_group
@@ -336,12 +336,21 @@ def decoder_plan(model, max_len):
     attention, then one sequence o = o_proj(attn) + h, gu = gate_up(rmsnorm(o)), d = down(silu(g) u) + o and qkv_{l+1} = qkv(rmsnorm(d)),
     the last layer's ending in lm_head(rmsnorm(d)) instead when lm_head is a QuantLinearLUT (else the final norm and lm_head run as
     torch ops on its d)."""
-    from .fusion import fuse_siblings
-    from .quant import QuantLinearLUT
     layers = _decoder_layout(model, max_len)
+    return _plan(model, layers, *_stack_siblings(model, layers, "SequenceDecoder"))
+
+
+def _stack_siblings(model, layers, who):
+    """fusion.fuse_siblings(model), then the stacked q/k/v layers and the stacked gate/up layers of the decoder layers."""
+    from .fusion import fuse_siblings
     fuse_siblings(model)
-    qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3]) for layer in layers]
-    gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2]) for layer in layers]
+    return ([_stacked(layer.self_attn, _PROJ[0][1][:3], who) for layer in layers],
+            [_stacked(layer.mlp, _PROJ[1][1][:2], who) for layer in layers])
+
+
+def _plan(model, layers, qkv, gate_up):
+    """decoder_plan's list from the decoder layers and their stacked q/k/v and gate/up layers."""
+    from .quant import QuantLinearLUT
     H = model.config.hidden_size
     plan = [SeqPlan("prologue", "embed", None, [PlanItem("qkv", qkv[0], ("x", 0, H), layers[0].input_layernorm)], ["qkv"])]
     for i, layer in enumerate(layers):
@@ -404,19 +413,72 @@ def _sampling(who, n, temperature, top_k, top_p, seed):
     return [float(t) for t in temps], [min(int(k), 2**31 - 1) for k in ks], [float(p) for p in ps], [int(s) for s in seeds]
 
 
+def _eos_set(eos_token_id):
+    """generate's eos_token_id (None, an int or a list of ints) as a set of ints."""
+    if eos_token_id is None:
+        return set()
+    return {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
+
+
 class _DecoderBase:
-    """What SequenceDecoder and BatchDecoder share: the eager layer body on rows of tokens and `extend` on the decoder's own kernels.
-    A subclass holds model, dtype, device, the stacked q/k/v and gate/up layers (qkv, gate_up), the head layout, scale, max_len and
-    the rotary tables."""
+    """What SequenceDecoder and BatchDecoder share, for `slots` sequences (SequenceDecoder: one): the set-up, the graph capture, the
+    prompts (prefill and extend of one slot), the replay with its full-cache check and the generate loop.  Slot b is row b of pos, tok,
+    the attention output and the sampling buffers and block b of the caches [n_layers, slots, n_kv, max_len, head_dim]; _pos holds the
+    slots' host positions (-1: idle).  A subclass defines _step (one token of every slot on the current stream: what the graph holds) and
+    reset(), and names itself in CACHE_FULL."""
 
     EXTEND_CHUNK = 2048  # extend() runs a prompt in chunks of at most this many tokens: it bounds the activations of one chunk
+    CHECK_EVERY = 8      # generate() looks for EOS every this many steps
 
-    def _sampling_buffers(self, rows):
-        """The device parameters of quant_cuda.sample, one per row: temperature, top_k, top_p and seed (greedy until generate sets them)."""
-        self.temperature = torch.zeros(rows, dtype=torch.float32, device=self.device)
-        self.top_k = torch.zeros(rows, dtype=torch.int32, device=self.device)
-        self.top_p = torch.ones(rows, dtype=torch.float32, device=self.device)
-        self.seed = torch.zeros(rows, dtype=torch.int64, device=self.device)
+    def __init__(self, model, max_len, layers, slots, who):
+        """After the subclass's device-free checks (layers: _decoder_layout's): the one GPU, the head layout and scale, the stacked
+        siblings, then on the device the caches, the attention output, the rotary tables, pos, tok and the sampling buffers."""
+        from .quant import quant_cuda
+        self.device = _model_device(model, who)
+        self.model, self.max_len = model, max_len
+        self.dtype = model.model.embed_tokens.weight.dtype
+        self._qc = quant_cuda
+        cfg = model.config
+        attn = layers[0].self_attn
+        self.n_layers = cfg.num_hidden_layers
+        self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
+        self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
+        self.qkv, self.gate_up = _stack_siblings(model, layers, who)
+        dev, d = self.device, self.head_dim
+        with torch.cuda.device(dev), torch.no_grad():
+            self.pos = torch.zeros(slots, dtype=torch.int32, device=dev)
+            self.tok = torch.zeros(slots, dtype=torch.int64, device=dev)
+            self._k = torch.zeros(self.n_layers, slots, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
+            self._v = torch.zeros_like(self._k)
+            self.attn_out = torch.zeros(slots, self.n_heads * d, dtype=self.dtype, device=dev)
+            self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
+            # the device parameters of quant_cuda.sample, one per slot: temperature, top_k, top_p and seed (greedy until generate sets them)
+            self.temperature = torch.zeros(slots, dtype=torch.float32, device=dev)
+            self.top_k = torch.zeros(slots, dtype=torch.int32, device=dev)
+            self.top_p = torch.ones(slots, dtype=torch.float32, device=dev)
+            self.seed = torch.zeros(slots, dtype=torch.int64, device=dev)
+        self._pos = [0] * slots
+
+    def _capture(self):
+        """From reset(): _step once on a side stream (SequenceDecoder's writes position 0, which a prompt overwrites; BatchDecoder's has
+        every slot idle and writes nothing), then its capture as the graph, whose logits are self.logits; reset() again."""
+        self.reset()
+        with torch.cuda.device(self.device), torch.no_grad():
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._step()
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph, stream=side):
+                self.logits = self._step()
+            torch.cuda.synchronize()
+        self.reset()
+
+    def _set_pos(self, slot, p):
+        self.pos[slot] = p
+        self._pos[slot] = p
 
     def _set_sampling(self, params):
         """Rows 0 .. n-1 of the sampling buffers from _sampling's lists of n values."""
@@ -443,8 +505,26 @@ class _DecoderBase:
         I = gu.shape[1] // 2
         return h + self._proj(layer.mlp.down_proj, torch.nn.functional.silu(gu[:, :I]) * gu[:, I:])
 
-    def _check_extend(self, who, input_ids, start):
-        """The prompt as a 1-D int64 device tensor; ValueError before anything is written when it is empty, not 1-D or does not fit."""
+    def _prefill(self, who, slot, input_ids):
+        """The prompt [1, T] (or [T]) through the model's own forward, its KV cache copied into `slot`, whose position becomes T; the
+        logits of the last position."""
+        ids = torch.as_tensor(input_ids).reshape(1, -1).to(self.device)
+        T = ids.shape[1]
+        if not 1 <= T <= self.max_len:
+            raise ValueError(f"{who}: {T} prompt tokens, the cache holds 1 to {self.max_len}")
+        with torch.no_grad():
+            o = self.model(input_ids=ids, use_cache=True)
+            for i, layer in enumerate(o.past_key_values.layers):
+                self._k[i, slot, :, :T].copy_(layer.keys[0])
+                self._v[i, slot, :, :T].copy_(layer.values[0])
+        self._set_pos(slot, T)
+        return o.logits[0, -1]
+
+    def _extend(self, who, slot, input_ids):
+        """The tokens input_ids (1-D) at `slot`'s positions start .. start+T-1 (start: its position, 0 for an idle slot) through every
+        layer, EXTEND_CHUNK tokens at a time, with quant_cuda.attn_extend on the slot's caches; the slot's position becomes start + T.
+        The logits of the last token.  ValueError before anything is written when the prompt is empty, not 1-D or does not fit."""
+        start = max(self._pos[slot], 0)
         ids = torch.as_tensor(input_ids)
         if ids.dim() != 1 or ids.numel() == 0:
             raise ValueError(f"{who}: input_ids must be a non-empty 1-D tensor of token ids (got shape {tuple(ids.shape)})")
@@ -453,11 +533,7 @@ class _DecoderBase:
         if start + ids.numel() > self.max_len:
             raise ValueError(f"{who}: {ids.numel()} tokens at position {start} need {start + ids.numel()} cache positions, "
                              f"max_len is {self.max_len}")
-        return ids.to(device=self.device, dtype=torch.int64)
-
-    def _extend(self, ids, start, k_cache, v_cache):
-        """The tokens ids at positions start .. start+T-1 through every layer, EXTEND_CHUNK tokens at a time, with quant_cuda.attn_extend
-        on the caches k_cache[layer], v_cache[layer] ([n_kv, max_len, head_dim] each); the logits of the last token."""
+        ids = ids.to(device=self.device, dtype=torch.int64)
         m = self.model.model
         with torch.no_grad():
             for c0 in range(0, ids.numel(), self.EXTEND_CHUNK):
@@ -466,11 +542,61 @@ class _DecoderBase:
                 h = torch.index_select(m.embed_tokens.weight, 0, chunk)
                 for i, layer in enumerate(m.layers):
                     def attend(qkv, i=i):
-                        self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, k_cache[i], v_cache[i], out, self.n_heads,
-                                             self.n_kv, self.scale)
+                        self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i, slot], self._v[i, slot], out,
+                                             self.n_heads, self.n_kv, self.scale)
                         return out
                     h = self._layer(i, layer, h, attend)
-            return self.model.lm_head(m.norm(h[-1:]))[0]
+            logits = self.model.lm_head(m.norm(h[-1:]))[0]
+        self._set_pos(slot, start + ids.numel())
+        return logits
+
+    def _replay(self):
+        """One step of every active slot; RuntimeError, before it, when an active slot's cache is full."""
+        full = [b for b, p in enumerate(self._pos) if p >= self.max_len]
+        if full:
+            raise RuntimeError(self.CACHE_FULL.format(slots=full, max_len=self.max_len))
+        self.graph.replay()
+        self._pos = [p + 1 if p >= 0 else p for p in self._pos]
+
+    def _finished(self, row):
+        """generate's row `row` has come to its EOS."""
+
+    def _generate(self, who, prompts, max_new_tokens, eos, sampling):
+        """Prompt i (token ids) prefilled into slot i, then steps until every prompt has max_new_tokens new tokens or its first token in
+        the set `eos`, looked for every CHECK_EVERY steps, after which _finished(i).  Sampled with _sampling's lists `sampling`, else
+        greedy.  -> the new tokens [slots, max_new_tokens] (on the device) and each prompt's count of them."""
+        R = len(prompts)
+        out = torch.zeros(len(self._pos), max_new_tokens, dtype=torch.int64, device=self.device)
+        if sampling:
+            self._set_sampling(sampling)
+            self._sample(torch.stack([self._prefill(who, i, p) for i, p in enumerate(prompts)]))
+            out[:R, 0].copy_(self.tok[:R])
+        else:
+            for i, p in enumerate(prompts):
+                out[i, 0] = self._prefill(who, i, p).argmax()
+        self.tok.copy_(out[:, 0])
+        length = [None] * R  # new tokens of a finished row
+        n, seen = 1, 0
+        while True:
+            if eos and (n % self.CHECK_EVERY == 0 or n == max_new_tokens):
+                got = out[:R, seen:n].tolist()
+                for i in range(R):
+                    if length[i] is None:
+                        hit = next((seen + j for j, t in enumerate(got[i]) if t in eos), None)
+                        if hit is not None:
+                            length[i] = hit + 1
+                            self._finished(i)
+                seen = n
+                if all(x is not None for x in length):
+                    break
+            if n == max_new_tokens:
+                break
+            self._replay()
+            if sampling:
+                self._sample(self.logits.view(len(self._pos), -1))
+            out[:, n].copy_(self.tok)
+            n += 1
+        return out, [n if x is None else x for x in length]
 
 
 class SequenceDecoder(_DecoderBase):
@@ -497,35 +623,17 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
 
-    CHECK_EVERY = 8  # generate() looks for EOS every this many tokens
+    CACHE_FULL = "SequenceDecoder: the cache is full (max_len={max_len}); reset() or prefill() first"
 
     def __init__(self, model, max_len):
-        from .quant import quant_cuda
-        _decoder_layout(model, max_len)
-        self.device = _model_device(model, "SequenceDecoder")
-        self.model, self.max_len = model, max_len
-        self.dtype = model.model.embed_tokens.weight.dtype
-        self._qc = quant_cuda
-        cfg = model.config
-        attn = model.model.layers[0].self_attn
-        self.n_layers = cfg.num_hidden_layers
-        self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
-        self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
-        self.plan = decoder_plan(model, max_len)
-        self.qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3]) for layer in model.model.layers]
-        self.gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2]) for layer in model.model.layers]
-        dev, d = self.device, self.head_dim
-        with torch.cuda.device(dev), torch.no_grad():
-            self.pos = torch.zeros(1, dtype=torch.int32, device=dev)
-            self.tok = torch.zeros(1, dtype=torch.int64, device=dev)
-            self.k_cache = torch.zeros(self.n_layers, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
-            self.v_cache = torch.zeros_like(self.k_cache)
-            self.attn_out = torch.zeros(self.n_heads * d, dtype=self.dtype, device=dev)
-            self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
-            self._sampling_buffers(1)
+        layers = _decoder_layout(model, max_len)
+        super().__init__(model, max_len, layers, 1, "SequenceDecoder")
+        # the one slot's views: caches [n_layers, n_kv, max_len, head_dim], attention output [n_heads * head_dim]
+        self.k_cache, self.v_cache, self.attn_out = self._k[:, 0], self._v[:, 0], self.attn_out[0]
+        self.plan = _plan(model, layers, self.qkv, self.gate_up)
+        with torch.cuda.device(self.device), torch.no_grad():
             self._build()
-            self._pos = 0
-            self._capture()
+        self._capture()
 
     def _build(self):
         """The DecodeSequences of the plan, each reading its inputs in place: the attention output buffer, the previous sequence's d."""
@@ -560,7 +668,7 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         self._head_in = out[(last.name, last.outputs[0])]
         self._quant_head = last.outputs == ["logits"]
 
-    def _token(self):
+    def _step(self):
         """One token on the current stream: what the graph holds."""
         embed = self.sequences[0].x
         torch.index_select(self.model.model.embed_tokens.weight, 0, self.tok, out=embed.view(1, -1))
@@ -579,68 +687,31 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         self.pos.add_(1)
         return logits
 
-    def _capture(self):
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            self._token()  # warm-up at position 0 (prefill overwrites what it wrote)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=side):
-            self.logits = self._token()
-        torch.cuda.synchronize()
-        self.reset()
-
     def reset(self):
         """Start a new prompt: position 0 (the cache's old slots are never read again)."""
-        self._pos = 0
+        self._pos = [0]
         self.pos.zero_()
 
     @property
     def position(self):
         """The position the next step writes (host copy of the device counter)."""
-        return self._pos
+        return self._pos[0]
 
     def prefill(self, input_ids):
         """Run the prompt [1, T] (or [T]) through the model's own forward, copy its KV cache into the static one and set the position
         to T; returns the logits of the last position."""
-        ids = torch.as_tensor(input_ids).reshape(1, -1).to(self.device)
-        T = ids.shape[1]
-        if not 1 <= T <= self.max_len:
-            raise ValueError(f"SequenceDecoder.prefill: {T} prompt tokens, the cache holds 1 to {self.max_len}")
-        with torch.no_grad():
-            o = self.model(input_ids=ids, use_cache=True)
-            for i, layer in enumerate(o.past_key_values.layers):
-                self.k_cache[i, :, :T].copy_(layer.keys[0])
-                self.v_cache[i, :, :T].copy_(layer.values[0])
-        self.pos.fill_(T)
-        self._pos = T
-        return o.logits[0, -1]
+        return self._prefill("SequenceDecoder.prefill", 0, input_ids)
 
     def extend(self, input_ids):
         """Append the tokens input_ids (1-D) at the current position on the decoder's own kernels (quant_cuda.attn_extend between the
         layers' projections, EXTEND_CHUNK tokens at a time), advance the position by T and return the logits of the last token.  After
         reset() this is a prefill; after prefill(), steps or an earlier extend it continues the sequence (a new turn of a chat, say).
         Raises ValueError, with nothing written, for an empty or non-1-D prompt or one that does not fit in max_len."""
-        start = self._pos
-        ids = self._check_extend("SequenceDecoder.extend", input_ids, start)
-        logits = self._extend(ids, start, self.k_cache, self.v_cache)
-        self.pos.fill_(start + ids.numel())
-        self._pos = start + ids.numel()
-        return logits
-
-    def _replay(self):
-        if self._pos >= self.max_len:
-            raise RuntimeError(f"SequenceDecoder: the cache is full (max_len={self.max_len}); reset() or prefill() first")
-        self.graph.replay()
-        self._pos += 1
+        return self._extend("SequenceDecoder.extend", 0, input_ids)
 
     def step(self, token_id):
         """Feed token_id (an int or a one-element device tensor) at the current position; returns the next-token logits, a static buffer
         that the next step overwrites."""
-        if self._pos >= self.max_len:
-            raise RuntimeError(f"SequenceDecoder: the cache is full (max_len={self.max_len}); reset() or prefill() first")
         if isinstance(token_id, torch.Tensor):
             self.tok.copy_(token_id.reshape(1))
         else:
@@ -661,34 +732,10 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         if ids.shape[1] + max_new_tokens - 1 > self.max_len:
             raise ValueError(f"SequenceDecoder.generate: {ids.shape[1]} prompt tokens and {max_new_tokens} new ones need "
                              f"{ids.shape[1] + max_new_tokens - 1} cache positions, max_len is {self.max_len}")
-        eos = set() if eos_token_id is None else {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
-        logits = self.prefill(ids)
-        out = torch.empty(max_new_tokens, dtype=torch.int64, device=self.device)
-        if sampling:
-            self._set_sampling(sampling)
-            self._sample(logits.view(1, -1))
-        else:
-            self.tok.copy_(logits.argmax().view(1))
-        out[0:1].copy_(self.tok)
-        n, seen = 1, 0
-        while True:
-            if eos and (n % self.CHECK_EVERY == 0 or n == max_new_tokens):
-                got = out[seen:n].tolist()
-                hit = next((seen + j for j, t in enumerate(got) if t in eos), None)
-                if hit is not None:
-                    n = hit + 1
-                    break
-                seen = n
-            if n == max_new_tokens:
-                break
-            self._replay()
-            if sampling:
-                self._sample(self.logits.view(1, -1))
-            out[n:n + 1].copy_(self.tok)
-            n += 1
+        out, (n,) = self._generate("SequenceDecoder.prefill", [ids], max_new_tokens, _eos_set(eos_token_id), sampling)
         for seq in self.sequences:
             seq.check()
-        return torch.cat([ids.to(self.device), out[:n].view(1, -1)], dim=1)
+        return torch.cat([ids.to(self.device), out[:, :n]], dim=1)
 
 
 class BatchDecoder(_DecoderBase):
@@ -719,19 +766,18 @@ class BatchDecoder(_DecoderBase):
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
 
-    CHECK_EVERY = 8  # generate() looks for EOS every this many steps
+    CACHE_FULL = "BatchDecoder: the cache of slot(s) {slots} is full (max_len={max_len}); release() or prefill() them first"
 
     def __init__(self, model, max_len, batch):
         import types
 
-        from .fusion import fuse_siblings
-        from .quant import FUSED_LIMITS, QuantLinearLUT, quant_cuda
+        from .quant import FUSED_LIMITS, QuantLinearLUT
         layers = _decoder_layout(model, max_len, "BatchDecoder")
-        self.dtype = model.model.embed_tokens.weight.dtype
-        rows_max = QuantLinearLUT.ROWS_MAX if self.dtype == torch.float16 else QuantLinearLUT.BF16_ROWS_MAX
+        dtype = model.model.embed_tokens.weight.dtype
+        rows_max = QuantLinearLUT.ROWS_MAX if dtype == torch.float16 else QuantLinearLUT.BF16_ROWS_MAX
         if not isinstance(batch, int) or not 2 <= batch <= rows_max:
             hint = "; decode one sequence with SequenceDecoder" if batch == 1 else ""
-            raise ValueError(f"BatchDecoder: batch must be an int in 2..{rows_max} for a {self.dtype} model (got {batch!r}){hint}")
+            raise ValueError(f"BatchDecoder: batch must be an int in 2..{rows_max} for a {dtype} model (got {batch!r}){hint}")
         for i, layer in enumerate(layers):  # the shapes the step runs, stacked siblings included, before anything is stacked
             at, mlp = layer.self_attn, layer.mlp
             shapes = [("self_attn.q_proj|k_proj|v_proj", at.q_proj.infeatures,
@@ -746,28 +792,10 @@ class BatchDecoder(_DecoderBase):
                     where = n if n == "lm_head" else f"layers.{i}.{n}"
                     raise ValueError(f"BatchDecoder: {where} ({K} -> {N}) does not fit the multi-row LUT-GEMV (out_features a multiple "
                                      f"of 4, in_features up to {FUSED_LIMITS['rows_max_in_features']})")
-        self.device = _model_device(model, "BatchDecoder")
-        self.model, self.max_len, self.batch = model, max_len, batch
-        self._qc = quant_cuda
-        cfg = model.config
-        attn = layers[0].self_attn
-        self.n_layers = cfg.num_hidden_layers
-        self.n_heads, self.n_kv, self.head_dim = cfg.num_attention_heads, cfg.num_key_value_heads, attn.head_dim
-        self.scale = float(getattr(attn, "scaling", self.head_dim ** -0.5))
-        fuse_siblings(model)
-        self.qkv = [_stacked(layer.self_attn, _PROJ[0][1][:3], "BatchDecoder") for layer in layers]
-        self.gate_up = [_stacked(layer.mlp, _PROJ[1][1][:2], "BatchDecoder") for layer in layers]
-        dev, d = self.device, self.head_dim
-        with torch.cuda.device(dev), torch.no_grad():
-            self.pos = torch.full((batch,), -1, dtype=torch.int32, device=dev)
-            self.tok = torch.zeros(batch, dtype=torch.int64, device=dev)
-            self.k_cache = torch.zeros(self.n_layers, batch, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
-            self.v_cache = torch.zeros_like(self.k_cache)
-            self.attn_out = torch.zeros(batch, self.n_heads * d, dtype=self.dtype, device=dev)
-            self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
-            self._sampling_buffers(batch)
-            self._pos = [-1] * batch
-            self._capture()
+        super().__init__(model, max_len, layers, batch, "BatchDecoder")
+        self.batch = batch
+        self.k_cache, self.v_cache = self._k, self._v
+        self._capture()
 
     def _step(self):
         """One step on the current stream: what the graph holds."""
@@ -784,19 +812,6 @@ class BatchDecoder(_DecoderBase):
         self.pos.add_((self.pos >= 0).to(torch.int32))
         return logits
 
-    def _capture(self):
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            self._step()  # warm-up with every slot idle: no cache slot is written
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=side):
-            self.logits = self._step()
-        torch.cuda.synchronize()
-        self.reset()
-
     def _slot(self, slot):
         if not isinstance(slot, int) or not 0 <= slot < self.batch:
             raise ValueError(f"BatchDecoder: slot must be an int in 0..{self.batch - 1} (got {slot!r})")
@@ -809,9 +824,9 @@ class BatchDecoder(_DecoderBase):
 
     def release(self, slot):
         """Make `slot` idle (pos -1): the steps write nothing for it from now on; its old cache slots are never read again."""
-        slot = self._slot(slot)
-        self.pos[slot] = -1
-        self._pos[slot] = -1
+        self._set_pos(self._slot(slot), -1)
+
+    _finished = release
 
     @property
     def positions(self):
@@ -821,39 +836,14 @@ class BatchDecoder(_DecoderBase):
     def prefill(self, slot, input_ids):
         """Run the prompt [1, T] (or [T]) alone through the model's own forward, copy its KV cache into `slot` and set the slot's
         position to T; returns the logits of the last position."""
-        self._slot(slot)
-        ids = torch.as_tensor(input_ids).reshape(1, -1).to(self.device)
-        T = ids.shape[1]
-        if not 1 <= T <= self.max_len:
-            raise ValueError(f"BatchDecoder.prefill: {T} prompt tokens, the cache holds 1 to {self.max_len}")
-        with torch.no_grad():
-            o = self.model(input_ids=ids, use_cache=True)
-            for i, layer in enumerate(o.past_key_values.layers):
-                self.k_cache[i, slot, :, :T].copy_(layer.keys[0])
-                self.v_cache[i, slot, :, :T].copy_(layer.values[0])
-        self.pos[slot] = T
-        self._pos[slot] = T
-        return o.logits[0, -1]
+        return self._prefill("BatchDecoder.prefill", self._slot(slot), input_ids)
 
     def extend(self, slot, input_ids):
         """Append the tokens input_ids (1-D) to `slot` at its position (0 for an idle slot) on the decoder's own kernels, as
         SequenceDecoder.extend does, advance the slot's position by T and return the logits of the last token.  It reads and writes
         nothing of the other slots, so it may run between steps while they keep their state.  Raises ValueError, with nothing written,
         for a bad slot, an empty or non-1-D prompt or one that does not fit in max_len."""
-        slot = self._slot(slot)
-        start = max(self._pos[slot], 0)
-        ids = self._check_extend("BatchDecoder.extend", input_ids, start)
-        logits = self._extend(ids, start, self.k_cache[:, slot], self.v_cache[:, slot])
-        self.pos[slot] = start + ids.numel()
-        self._pos[slot] = start + ids.numel()
-        return logits
-
-    def _replay(self):
-        full = [b for b, p in enumerate(self._pos) if p >= self.max_len]
-        if full:
-            raise RuntimeError(f"BatchDecoder: the cache of slot(s) {full} is full (max_len={self.max_len}); release() or prefill() them first")
-        self.graph.replay()
-        self._pos = [p + 1 if p >= 0 else p for p in self._pos]
+        return self._extend("BatchDecoder.extend", self._slot(slot), input_ids)
 
     def step(self, token_ids):
         """Feed token_ids ([batch] ints or a device tensor; only the active slots' entries matter) at each active slot's position;
@@ -884,37 +874,7 @@ class BatchDecoder(_DecoderBase):
             if p.numel() + max_new_tokens - 1 > self.max_len:
                 raise ValueError(f"BatchDecoder.generate: prompt {i} has {p.numel()} tokens and {max_new_tokens} new ones need "
                                  f"{p.numel() + max_new_tokens - 1} cache positions, max_len is {self.max_len}")
-        eos = set() if eos_token_id is None else {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
-        R = len(prompts)
+        eos = _eos_set(eos_token_id)
         self.reset()
-        out = torch.zeros(self.batch, max_new_tokens, dtype=torch.int64, device=self.device)
-        if sampling:
-            self._set_sampling(sampling)
-            self._sample(torch.stack([self.prefill(i, p) for i, p in enumerate(prompts)]))
-            out[:R, 0].copy_(self.tok[:R])
-        else:
-            for i, p in enumerate(prompts):
-                out[i, 0] = self.prefill(i, p).argmax()
-        self.tok.copy_(out[:, 0])
-        length = [None] * R  # new tokens of a finished row
-        n, seen = 1, 0
-        while True:
-            if eos and (n % self.CHECK_EVERY == 0 or n == max_new_tokens):
-                got = out[:R, seen:n].tolist()
-                for i in range(R):
-                    if length[i] is None:
-                        hit = next((seen + j for j, t in enumerate(got[i]) if t in eos), None)
-                        if hit is not None:
-                            length[i] = hit + 1
-                            self.release(i)
-                seen = n
-                if all(x is not None for x in length):
-                    break
-            if n == max_new_tokens:
-                break
-            self._replay()
-            if sampling:
-                self._sample(self.logits)
-            out[:, n].copy_(self.tok)
-            n += 1
-        return [torch.cat([p.to(self.device), out[i, :length[i] if length[i] is not None else n]]) for i, p in enumerate(prompts)]
+        out, length = self._generate("BatchDecoder.prefill", prompts, max_new_tokens, eos, sampling)
+        return [torch.cat([p.to(self.device), out[i, :length[i]]]) for i, p in enumerate(prompts)]

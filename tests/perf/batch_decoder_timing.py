@@ -55,12 +55,8 @@ def decoder_for(model, B, max_len):
 
 
 def set_positions(dec, B, ctx):
-    if B == 1:
-        dec.pos.fill_(ctx)
-        dec._pos = ctx
-    else:
-        dec.pos.fill_(ctx)
-        dec._pos = [ctx] * B
+    dec.pos.fill_(ctx)
+    dec._pos = [ctx] * B
     dec.tok.fill_(1)
 
 

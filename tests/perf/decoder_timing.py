@@ -89,12 +89,12 @@ def capture(dec, qc):
         side.wait_stream(torch.cuda.current_stream())
         with torch.no_grad():
             with torch.cuda.stream(side):
-                dec._token()
+                dec._step()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=side):
-                logits = dec._token()
+                logits = dec._step()
         torch.cuda.synchronize()
     finally:
         dec._qc = real
@@ -145,7 +145,7 @@ def main():
     for ctx in contexts:
         def set_pos(ctx=ctx):
             dec.pos.fill_(ctx)
-            dec._pos = ctx
+            dec._pos = [ctx]
             dec.tok.fill_(1)
         g_sdpa, logits_sdpa = capture(dec, TorchAttention(quant_cuda, ctx + BLOCK + 1))
         # one token of each graph from the same state: the logits agree to the attention's rounding

@@ -83,7 +83,7 @@ def main():
 
     def back_to_history():
         dec.pos.fill_(HISTORY)
-        dec._pos = HISTORY
+        dec._pos = [HISTORY]
 
     def append():
         dec.extend(ids[HISTORY:])
