@@ -1,6 +1,7 @@
 // lutgemv_seq.cuh - the SEQUENCE kernel: one persistent launch runs a whole list of dependent LUT-GEMVs (a decode token's QuantLinear
 // matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Built on lutgemv_v2.cuh:
-// the per-position math, table builders, outlier warps (sparse3) and mailboxes are v2's (namespace v2), what is new is everything BETWEEN two GEMVs.
+// the per-position math, table builders, outlier warps (sparse3), mailboxes, CTA span (Span) and strip flush (flush_strip) are v2's
+// (namespace v2), what is new is everything BETWEEN two GEMVs.
 //
 // Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
 // carries a fixed cost (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
@@ -203,15 +204,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
     const uint32_t xwant = xtag << 16;
     const int ngemv = c.ngemv;
 
-    // the CTA's part of GEMV `p`: units [g0, g0 + len) of the strip-major [strip][unit] space
-#define SEQ_GEOMETRY(p)                                                                   \
-    const int N = (p).N, R = (p).R;                                                       \
-    const int g0 = min((int)blockIdx.x * (p).chunk, (p).T), g1 = min(g0 + (p).chunk, (p).T); \
-    const int len = g1 - g0;                                                              \
-    const int s0 = g0 / R, r0 = g0 - s0 * R;                                              \
-    const int nseg = len > 0 ? (g1 - 1) / R - s0 + 1 : 0;                                 \
-    (void)N; (void)r0; (void)s0; (void)nseg;
-
     if (warp == WARP_PROD) {
         // =========================== TMA producer: runs ahead of the consumers across GEMV boundaries ===========================
         const uint64_t pol = l2_evict_first_policy();
@@ -225,27 +217,18 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         for (int g = 0; g < ngemv; ++g) {
             const SeqDesc &d = c.descs[g];
             const P2 &p = d.p;
-            SEQ_GEOMETRY(p)
+            const int N = p.N, R = p.R;
+            const Span sp(p);
             if (lane == 0 && g + 1 < ngemv) {
                 asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&c.descs[g + 1].tm_big)) : "memory");
                 asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&c.descs[g + 1].tm_small)) : "memory");
             }
-            {   // a 1/grid slice of the GEMV's look-up table and row pointers -> L2, for everybody (cold otherwise: a token never finds them there)
-                const int G = (int)gridDim.x;
-                const size_t lut_lines = ((size_t)N * C::L * 4 + 127) / 128, per = (lut_lines + G - 1) / G;
-                for (size_t i = (size_t)blockIdx.x * per + lane; i < min(lut_lines, ((size_t)blockIdx.x + 1) * per); i += 32)
-                    asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.lut) + 128 * i));
-                if (p.rows) {
-                    const size_t row_lines = ((size_t)(N + 1) * 4 + 127) / 128, rper = (row_lines + G - 1) / G;
-                    for (size_t i = (size_t)blockIdx.x * rper + lane; i < min(row_lines, ((size_t)blockIdx.x + 1) * rper); i += 32)
-                        asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.rows) + 128 * i));
-                }
-            }
-            for (int seg = 0; seg < nseg; ++seg) {
-                const int sstart = seg == 0 ? 0 : seg * R - r0, send = min(len, (seg + 1) * R - r0);
+            warm_l2<BITS>(p, N, lane);  // (cold otherwise: a token never finds them in L2)
+            for (int seg = 0; seg < sp.nseg; ++seg) {
+                const int sstart = seg == 0 ? 0 : seg * R - sp.r0, send = min(sp.len, (seg + 1) * R - sp.r0);
                 const int seglen = send - sstart;
-                const int u0 = r0 + sstart - seg * R;
-                const int col0 = (s0 + seg) * STRIP;
+                const int u0 = sp.r0 + sstart - seg * R;
+                const int col0 = (sp.s0 + seg) * STRIP;
                 for (int u = 0; u < seglen; u += SU2) {
                     if (refill) mbar_wait(bar_u32 + 128 + 8 * slot, ph);
                     const int nu = min(SU2, seglen - u);
@@ -283,37 +266,25 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         for (int b = 0; b < NTB; ++b) sts_u32(sacc0 + 4 * (b * STRIP + bt), 0u);
         int *const err = c.err;
         int q0 = 0;  // segments of earlier GEMVs: segment s of this one uses table buffer / accumulator (q0 + s) % NTB
-        {
-            const P2 &p = c.descs[0].p;
-            SEQ_GEOMETRY(p)
-            if (nseg > 0) lut_prefetch<BITS>(p, lutbuf, s0, bt);
-            if (nseg > 1) lut_prefetch<BITS>(p, lutbuf + LUTBUF, s0 + 1, bt);
-        }
+        auto prefetch_first = [&](const P2 &p) {  // the raw LUT rows of a GEMV's first two strips
+            const Span sp(p);
+            if (sp.nseg > 0) lut_prefetch<BITS>(p, lutbuf, sp.s0, bt);
+            if (sp.nseg > 1) lut_prefetch<BITS>(p, lutbuf + LUTBUF, sp.s0 + 1, bt);
+        };
+        prefetch_first(c.descs[0].p);
         for (int g = 0; g < ngemv; ++g) {
             const SeqDesc &d = c.descs[g];
             const P2 &p = d.p;
-            SEQ_GEOMETRY(p)
+            const int N = p.N, R = p.R;
+            const Span sp(p);
+            const int s0 = sp.s0, r0 = sp.r0, nseg = sp.nseg;
             const uint32_t boxtag = (epoch << 10) | (uint32_t)(g + 1);
             float *const acc_out = p.ws_acc;
-            int *const flags = p.ws_cnt + 64;
             auto sacc_of = [&](int s) { return sacc0 + 4u * (uint32_t)(((q0 + s) % NTB) * STRIP + bt); };
             auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + 288 + 8 * ((q0 + s) % NTB), (uint32_t)(((q0 + s) / NTB) & 1)); };
-            // Strip sums of segment s go to the strip's owner: another CTA (mailbox row) if the strip started before our range, else ourselves -
-            // and then they never leave the SM: sown[u][column] for the u-th owned strip (a strip inside one CTA is exactly one segment).
-            // (v2 and the first sequence build sent them through the global accumulator - a RED and, in the finishing pass, a load that has to
-            // wait for it: L2 round trips on the critical path between the last weight and y.)
             const uint32_t sown = base + OFF_FIN;   // float [SOWN][64], as in lutgemv2_kernel
-            constexpr int SOWN = 8;
             const int ofs = r0 != 0 ? 1 : 0;        // segment s is owned strip s - ofs
-            auto flush = [&](int s) {
-                const uint32_t a = sacc_of(s);
-                const float v = lds_f32(a);
-                sts_u32(a, 0u);
-                const int col = (s0 + s) * STRIP + bt;
-                if (s == 0 && r0 != 0) st_relaxed_u64(p.ws_hbox + (size_t)blockIdx.x * STRIP + bt, box_word(v, boxtag));
-                else if (s - ofs < SOWN) sts_u32(sown + 4u * (uint32_t)((s - ofs) * STRIP + bt), __float_as_uint(v));
-                else if (col < N) atomicAdd(acc_out + col, v);
-            };
+            auto flush = [&](int s) { flush_strip<true>(p, sacc_of(s), s, ofs, sp, N, base, bt, acc_out, boxtag); };
             for (int s = 0; s < nseg; ++s) {
                 const int b = (q0 + s) % NTB;
                 if (s >= NTB) {
@@ -328,13 +299,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 if (lane == 0) mbar_arrive(bar_u32 + 256 + 8 * b);
                 if (s + 2 < nseg) lut_prefetch<BITS>(p, lutbuf + (s & 1) * LUTBUF, s0 + s + 2, bt);
             }
-            if (g + 1 < ngemv) {  // the next GEMV's first raw LUT rows travel while this one is being finished
-                const P2 &pn = c.descs[g + 1].p;
-                const int gn0 = min((int)blockIdx.x * pn.chunk, pn.T), gn1 = min(gn0 + pn.chunk, pn.T);
-                const int sn0 = gn0 / pn.R, nsegn = gn1 > gn0 ? (gn1 - 1) / pn.R - sn0 + 1 : 0;
-                if (nsegn > 0) lut_prefetch<BITS>(pn, lutbuf, sn0, bt);
-                if (nsegn > 1) lut_prefetch<BITS>(pn, lutbuf + LUTBUF, sn0 + 1, bt);
-            }
+            if (g + 1 < ngemv) prefetch_first(c.descs[g + 1].p);  // the next GEMV's rows travel while this one is being finished
             // ---- finish the strips this CTA owns (those that start in its range); see lutgemv_v2.cuh for the protocol ----
             TRACE(12, bt == 0);
             const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
@@ -578,7 +543,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         for (int g = 0; g < ngemv; ++g) {
             const SeqDesc &d = c.descs[g];
             const P2 &p = d.p;
-            SEQ_GEOMETRY(p)
+            const int R = p.R;
+            const Span sp(p);
             TRACE(2, tid == 0);
             if (g > 0) named_bar_sync(6, NCT + NSPW * 32);  // every consumer warp and the outlier warps are done with the previous x
             if (d.x_tag == nullptr) {
@@ -611,7 +577,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             }
             named_bar_sync(2, NCT + NSPW * 32);  // x visible to the consumers and the outlier warps
             TRACE(4, tid == 0);
-            for (int seg = 0; seg < nseg; ++seg) {
+            for (int seg = 0; seg < sp.nseg; ++seg) {
                 const int q = q0 + seg, b = q % NTB;
                 const uint32_t tab = tab0 + b * C::TAB;
                 const uint32_t tb_hi = (MODE == 1 && BITS == 4) ? tab : (BITS == 4 ? (tab & 0xFFFF0000u) : tab);
@@ -622,9 +588,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                     asm volatile("mov.u32 %0, %0;" : "+r"(l[t]));
                 }
                 const uint32_t segc = ((tab >> 8) & 0xF0u) * 0x01010101u;
-                const int sstart = seg == 0 ? 0 : seg * R - r0, send = min(len, (seg + 1) * R - r0);
+                const int sstart = seg == 0 ? 0 : seg * R - sp.r0, send = min(sp.len, (seg + 1) * R - sp.r0);
                 const int seglen = send - sstart;
-                const int u0 = r0 + sstart - seg * R;
+                const int u0 = sp.r0 + sstart - seg * R;
                 uint32_t xaddr = xs_u32 + (uint32_t)((u0 + 2 * warp + jsel) * XB);
                 const int nstg = (seglen + SU2 - 1) / SU2;
                 const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;
@@ -668,7 +634,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 TRACE(24 + (seg < 7 ? seg : 7), tid == 0);
             }
             TRACE(6, tid == 0);
-            q0 += nseg;
+            q0 += sp.nseg;
         }
         // exports: plain 16-bit copies of the vectors the caller asked for (on several GPUs this is also where the last exchange completes)
         for (int e = (int)blockIdx.x; e < c.nexport; e += (int)gridDim.x) {
@@ -678,7 +644,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             });
         }
     }
-#undef SEQ_GEOMETRY
 }
 
 }  // namespace seq

@@ -602,6 +602,66 @@ __device__ __forceinline__ void sparse3(const P2 &p, const uint32_t base, const 
     }
 }
 
+// The calling CTA's part of GEMV `p`: units [g0, g0 + len) of the strip-major [strip][unit] space, from unit r0 of strip s0, in nseg
+// segments (a segment is the CTA's part of one strip).
+struct Span {
+    int g0, len, s0, r0, nseg;
+    __device__ __forceinline__ explicit Span(const P2 &p) {
+        const int R = p.R;
+        g0 = min((int)blockIdx.x * p.chunk, p.T);
+        const int g1 = min(g0 + p.chunk, p.T);
+        len = g1 - g0;
+        s0 = g0 / R;
+        r0 = g0 - s0 * R;
+        nseg = len > 0 ? (g1 - 1) / R - s0 + 1 : 0;
+    }
+};
+
+// By one producer lane each: a 1/grid slice of the GEMV's look-up table and row pointers into L2.  A decode step finds none of a layer's
+// arrays there, and the CTAs of a launch start at different times, so the late ones find what the early ones asked for.
+template <int BITS>
+__device__ __forceinline__ void warm_l2(const P2 &p, const int N, const int lane) {
+    const int G = (int)gridDim.x;
+    const size_t lut_lines = ((size_t)N * (1 << BITS) * 4 + 127) / 128, per = (lut_lines + G - 1) / G;
+    for (size_t i = (size_t)blockIdx.x * per + lane; i < min(lut_lines, ((size_t)blockIdx.x + 1) * per); i += 32)
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.lut) + 128 * i));
+    if (p.rows) {
+        const size_t row_lines = ((size_t)(N + 1) * 4 + 127) / 128, rper = (row_lines + G - 1) / G;
+        for (size_t i = (size_t)blockIdx.x * rper + lane; i < min(row_lines, ((size_t)blockIdx.x + 1) * rper); i += 32)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.rows) + 128 * i));
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Strip finishing (fused mode), by the builder warps of lutgemv2_kernel and lutgemv_seq_kernel (thread bt = column bt of a strip).
+// A strip is finished (converted to y) by the CTA in whose range it STARTS.  A CTA that only holds a later part of it (that can only
+// be its first segment) hands its sums to that owner through its mailbox row (ws_hbox); the owner's own strip sums never leave the SM:
+// sown[u][column] for the u-th owned strip (a strip inside one CTA is exactly one segment), SOWN of them, the rest through the global
+// accumulator.  (The first round-2 build sent all of them through the global accumulator: a RED and, in the finishing pass, a load that
+// had to wait for it - two L2 round trips between the last weight and y when the last segment is short.)
+// A mailbox word carries the kernel's tag (box_word): 1 in lutgemv2_kernel, reset by the owner; the (token, GEMV) tag in the sequence
+// kernel, never reset.  The finishing pass itself is written out in each kernel (DESIGN §3.4).
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int SOWN = 8;
+
+// Strip sums of segment s (at `a` in shared memory, back to zero) -> the strip's owner; FUSED = false: one red.add per column.
+// ofs = sp.r0 != 0 (segment s is owned strip s - ofs), given by the caller: the sequence kernel has it once per GEMV.
+template <bool FUSED>
+__device__ __forceinline__ void flush_strip(const P2 &p, const uint32_t a, const int s, const int ofs, const Span &sp, const int N,
+                                            const uint32_t base, const int bt, float *const acc_out, const uint32_t tag) {
+    const float v = lds_f32(a);
+    sts_u32(a, 0u);
+    const int strip = sp.s0 + s, col = strip * STRIP + bt;
+    if constexpr (FUSED) {
+        const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
+        if (s == 0 && sp.r0 != 0) st_relaxed_u64(p.ws_hbox + (size_t)blockIdx.x * STRIP + bt, box_word(v, tag));
+        else if (s - ofs < SOWN) sts_u32(sown + 4u * (uint32_t)((s - ofs) * STRIP + bt), __float_as_uint(v));
+        else if (col < N) atomicAdd(acc_out + col, v);
+    } else {
+        if (col < N) atomicAdd(acc_out + col, v);
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------------------
 // The kernel.  MODE 0: exact fp32 table ; MODE 1: fp16 pair table (needs fp16 x).  XT: x's element type (float, __half or
 // __nv_bfloat16), in which it is given and staged; a 16-bit y (p.y_is_half) is y16_t<XT>.
@@ -628,10 +688,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int N = p.N, R = p.R;
-    const int g0 = min((int)blockIdx.x * p.chunk, p.T), g1 = min(g0 + p.chunk, p.T);
-    const int len = g1 - g0;
-    const int s0 = g0 / R, r0 = g0 - s0 * R;
-    const int nseg = len > 0 ? (g1 - 1) / R - s0 + 1 : 0;
+    const Span sp(p);
+    const int len = sp.len, s0 = sp.s0, r0 = sp.r0, nseg = sp.nseg;
 
     TRACE(0, tid == 0);
     if (tid == 0) {
@@ -647,23 +705,14 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     }
     pdl_launch_dependents();
     if (warp == WARP_PROD) {
-        // Cold-start latencies (a decode step finds none of a layer's arrays in L2): ask for the two tensor-map descriptors now, and let
-        // every CTA pull a 1/grid slice of the layer's look-up table and row pointers into L2 - the CTAs of a launch start at different
-        // times (they inherit their SM from the previous kernel's CTAs), so the late ones find what the early ones asked for.
+        // Cold-start latencies (a decode step finds none of a layer's arrays in L2): ask for the tensor-map descriptors now, and pull this
+        // CTA's slice of the look-up table and row pointers into L2 (the CTAs inherit their SM from the previous kernel's CTAs).
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_big)) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_small)) : "memory");
             if constexpr (C::ROT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_mid)) : "memory");
         }
-        const int G = (int)gridDim.x;
-        const size_t lut_lines = ((size_t)N * C::L * 4 + 127) / 128, per = (lut_lines + G - 1) / G;
-        for (size_t i = (size_t)blockIdx.x * per + lane; i < min(lut_lines, ((size_t)blockIdx.x + 1) * per); i += 32)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.lut) + 128 * i));
-        if (p.rows) {
-            const size_t row_lines = ((size_t)(N + 1) * 4 + 127) / 128, rper = (row_lines + G - 1) / G;
-            for (size_t i = (size_t)blockIdx.x * rper + lane; i < min(row_lines, ((size_t)blockIdx.x + 1) * rper); i += 32)
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(p.rows) + 128 * i));
-        }
+        warm_l2<BITS>(p, N, lane);
     }
     __syncthreads();
     float *const acc_out = FUSED ? p.ws_acc : reinterpret_cast<float *>(p.out);
@@ -720,25 +769,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         bool dep_ok = false;
         auto dep_wait = [&]() { if (!dep_ok) { pdl_wait(); dep_ok = true; } };  // builders never read x: they only need this before writing
         const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
-        constexpr int SOWN = 8;
-        auto flush = [&](int s) {  // strip sums of segment s -> one red.add per column, accumulator back to zero
-            const uint32_t a = sacc + 4 * ((s & 1) * STRIP + bt);
-            const float v = lds_f32(a);
-            sts_u32(a, 0u);
-            const int strip = s0 + s, col = strip * STRIP + bt;
-            if constexpr (FUSED) {
-                // A strip is finished (converted to y) by the CTA in whose range it STARTS; a CTA that only holds a later part of it
-                // (that can only be its first segment) hands its sums to that owner through its mailbox row.
-                // ... or to ourselves: then they never leave the SM (sown[u][column] for the u-th owned strip; a strip inside one CTA is exactly
-                // one segment).  Through the global accumulator (first round-2 build) that was a RED and, in the finishing pass, a load that had to
-                // wait for it - two L2 round trips between the last weight and y when the last segment is short.
-                if (s == 0 && r0 != 0) st_relaxed_u64(p.ws_hbox + (size_t)blockIdx.x * STRIP + bt, box_word(v));
-                else if (s - (r0 != 0 ? 1 : 0) < SOWN) sts_u32(sown + 4u * (uint32_t)((s - (r0 != 0 ? 1 : 0)) * STRIP + bt), __float_as_uint(v));
-                else if (col < N) atomicAdd(acc_out + col, v);
-            } else {
-                if (col < N) atomicAdd(acc_out + col, v);
-            }
-        };
+        auto flush = [&](int s) { flush_strip<FUSED>(p, sacc + 4 * ((s & 1) * STRIP + bt), s, r0 != 0 ? 1 : 0, sp, N, base, bt, acc_out, 1u); };
         // The raw LUT rows of the first two strips are requested at once (one cold round trip, not two); later strips two ahead.
         if (nseg > 0) lut_prefetch<BITS>(p, lutbuf, s0, bt);
         if (nseg > 1) lut_prefetch<BITS>(p, lutbuf + LUTBUF, s0 + 1, bt);
@@ -871,7 +902,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                             } else atomicAdd(acc_out + cc, v);
                         }
                     }
-                    named_bar_sync(3, NBT);  // (the list and the sums are reused by the next item; an idle CTA has no other barrier before that)
+                    named_bar_sync(3, NBT);  // (the sequence kernel's copy reuses the list and the sums for its next item; here nothing does)
                 }
                 const int w = p.xw_world ? N / p.xw_members : 0;
                 auto store_y = [&](int col, float yv) {
