@@ -64,10 +64,12 @@ const char *sqllm_last_error(void);
 int sqllm_device_sm_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * Workspace.  Used only by the *_fused entry point (cross-CTA accumulator, counters, deterministic-mode partials).
- * Must be zero-filled once after allocation (cudaMemset); the library keeps it consistent afterwards.  One
- * workspace serves layers of any shape, but must not be used by two streams concurrently.  A size returned in either
- * summation mode serves both.
+ * Workspace.  Used only by the *_fused entry point (cross-CTA accumulator, counters and mailboxes of the default summation mode;
+ * the deterministic mode reads none of it, but requires it all the same).  Must be zero-filled once after allocation
+ * (cudaMemset); the library keeps it consistent afterwards.  One workspace serves layers of any shape, but must not be used by
+ * two streams concurrently.  sqllm_workspace_bytes returns one fixed size for every shape the fused path takes, in either
+ * summation mode; 0 for bits other than 3 or 4, in_features not a positive multiple of 64, out_features <= 0 or
+ * out_features > SQLLM_FUSED_MAX_OUT.  topX does not change the size.
  * ------------------------------------------------------------------------------------------- */
 size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int topX);
 
@@ -98,8 +100,11 @@ int sqllm_lutgemv(const sqllm_lutgemv_args *args, void *stream);
 /* Fused-path summation mode (process-wide).
  *   0 (default; env SQLLM_DETERMINISTIC unset): contributions are added in the order they arrive (red.add.f32), like the
  *     reference's atomicAdd - results can differ in the last bits from run to run.
- *   1: per-strip partials reduced in a fixed order by the last-arriving contributor - bit-reproducible, 1.3-2x slower on
- *     layers with outliers. */
+ *   1: the multi-row kernel of sqllm_lutgemv_rows_dt at one row (fp32 x too): every output is written once, its K split over a
+ *     thread-block cluster whose leader adds the partial sums in a fixed order - bit-reproducible, and a row gets the bits it gets
+ *     inside a multi-row call.  About 1.8x the default mode's time on the four launches of a LLaMA-7B decoder layer (w4 and w3,
+ *     0.45 % outliers, 10 dense rows; measured on an H100 80GB HBM3 at a 700 W power limit).  The fused entry points keep their
+ *     limits and checks (the workspace included) in this mode; the exchange path refuses it. */
 void sqllm_set_deterministic(int on);
 
 /* Look-up-table precision of the fused path (process-wide; the 12 reference launchers below always use the exact table).

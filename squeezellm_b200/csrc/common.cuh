@@ -1,6 +1,6 @@
 // common.cuh - what every kernel of the library shares: the fused-path limits and the layout of the fused workspace header, the PTX
 // wrappers (shared-memory loads, cp.async, mbarrier, TMA, PDL, named barriers, cluster rank), fp32 pair math, the 16-bit conversions,
-// the 3-bit field decode of the exact-table GEMVs (v1 and v2) and the TRACE time stamps of -DSQLLM_TRACE builds.
+// the 3-bit field decode of the exact-table GEMVs and the TRACE time stamps of -DSQLLM_TRACE builds.
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
 #include <cuda_bf16.h>
@@ -16,14 +16,14 @@ namespace {
 
 constexpr int STRIP = 64;                 // output columns per strip (16 lanes x 4 columns)
 constexpr int MAX_TOPX_FUSED = SQLLM_FUSED_MAX_TOPX;
-constexpr int MAX_STRIPS = 16320;         // per-strip tickets in the workspace header (out_features <= 1,044,480)
+constexpr int MAX_STRIPS = 16320;         // per-strip flags of the sequence workspace; [256, 256 + 4*MAX_STRIPS) of the fused header stays reserved
 constexpr int MAX_N_FUSED = SQLLM_FUSED_MAX_OUT;  // fused path: the scratch accumulator lives at a fixed place in the workspace
 constexpr size_t WS_ACC_OFF = 65536;       // [64 KB, 64 KB + 4*MAX_N_FUSED): fp32 accumulator (zero between launches)
 constexpr int MAX_GRID_V2 = 256;           // v2 runs one CTA per SM
 constexpr size_t WS_HBOX_OFF = WS_ACC_OFF + (size_t)MAX_N_FUSED * 4;       // v2 mailboxes: [MAX_GRID_V2][64] x 8 bytes (partial strip sums)
 constexpr size_t WS_CBOX_OFF = WS_HBOX_OFF + (size_t)MAX_GRID_V2 * 64 * 8;  // ... and [MAX_N_FUSED] x 8 bytes (outlier row sums); zero between launches
 constexpr size_t WS_DBOX_OFF = WS_CBOX_OFF + (size_t)MAX_N_FUSED * 8;          // ... and [MAX_TOPX_FUSED][MAX_GRID_V2] x 8 bytes (dense-row parts, one per contributing CTA)
-constexpr size_t WS_HEADER = WS_DBOX_OFF + (size_t)MAX_TOPX_FUSED * MAX_GRID_V2 * 8;  // tickets + accumulator + mailboxes: never shared with data of any shape
+constexpr size_t WS_HEADER = WS_DBOX_OFF + (size_t)MAX_TOPX_FUSED * MAX_GRID_V2 * 8;  // error word + accumulator + mailboxes: the whole fused workspace
 
 // ---- small PTX helpers -------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -52,7 +52,8 @@ int det_mode() {
     if (g_det < 0) { const char *e = getenv("SQLLM_DETERMINISTIC"); g_det = (e && e[0] == '1') ? 1 : 0; }
     return g_det;
 }
-// g_det - fused mode: 1 = v1, deterministic per-strip tickets (SQLLM_DETERMINISTIC=1 or sqllm_set_deterministic), 0 = v2 (default)
+// g_det - fused mode: 1 = deterministic, the multi-row kernel at one row (SQLLM_DETERMINISTIC=1 or sqllm_set_deterministic);
+// 0 = v2 (default)
 int g_last_grid = 0;
 unsigned long long *g_trace = nullptr;
 size_t g_trace_stride = 0;

@@ -128,7 +128,8 @@ bool dt_valid(int dt);
 int check_layer(const sqllm_lutgemv_args *a, int k_mult, int n_mult);
 int check_common(const sqllm_lutgemv_args *a);
 
-// the fused mode (1: deterministic, v1) and the table mode (1: fp16 pair table), from the environment until set through the C ABI
+// the fused mode (1: deterministic, the multi-row kernel at one row) and the table mode (1: fp16 pair table), from the environment
+// until set through the C ABI
 int det_mode();
 int lut_mode();
 
@@ -142,5 +143,8 @@ int get_tensor_map(const void *qweight, int rows, int cols, int box_rows, CUtens
 
 // the *_batched symbols, and sqllm_lutgemv for batch >= 2 (lutgemv_rows.cu)
 int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st);
+// the multi-row LUT-GEMV (lutgemv_rows.cu) of a->batch rows of x, after the caller's argument checks: sqllm_lutgemv_rows_dt, and the
+// deterministic fused mode at one row, which also takes fp32 x (with fp32 or fp16 y)
+int launch_rows(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y, int y_dt, const float *bias, cudaStream_t st);
 
 }  // namespace sqllm

@@ -7,22 +7,21 @@
 //   DenseMatVecKernel[Batched]                       (:1092-1164)  topX dense rows
 // and the 12 host launchers (:132-738), behind the C ABI of include/sqllm_b200.h.
 //
-// lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default (fast) fused mode, the sequence
-// kernel (lutgemv_seq.cuh) a list of dependent GEMVs in one persistent launch, and lutgemv_kernel (lutgemv_v1.cuh) the deterministic
-// fused mode.  The other kernel families have translation units of their own: lutgemv_rows.cu (the batched symbols and a few
-// fp16 / bf16 rows on the CUDA cores), lutgemm_tc.cu (prefill-sized batches on the tensor cores), backward.cu (input and codebook
-// gradients, Fisher information) and tools.cu (dequantize, k-means, pack); host.cu holds the process-wide state.
+// lutgemv2_kernel (lutgemv_v2.cuh) runs every one-vector GEMV in the accumulate and the default (fast) fused mode, and the sequence
+// kernel (lutgemv_seq.cuh) a list of dependent GEMVs in one persistent launch; the deterministic fused mode runs the multi-row
+// kernel of lutgemv_rows.cu at one row (launch_rows).  The other kernel families have translation units of their own:
+// lutgemv_rows.cu (the batched symbols and a few rows on the CUDA cores), lutgemm_tc.cu (prefill-sized batches on the tensor
+// cores), backward.cu (input and codebook gradients, Fisher information) and tools.cu (dequantize, k-means, pack); host.cu holds
+// the process-wide state.
 #include <stdint.h>
 #include <string.h>
 
 #include <algorithm>
 #include <cmath>
-#include <unordered_map>
 #include <vector>
 
 #include "host.h"
 #include "lutgemv_seq.cuh"
-#include "lutgemv_v1.cuh"
 
 using namespace sqllm;
 
@@ -44,110 +43,6 @@ bool fused_dt_pair(int x_dt, int y_dt) {
 int fused_dt_fail(int x_dt, int y_dt) {
     return fail(SQLLM_EINVAL, "x_dtype=%d, y_dtype=%d: x must be SQLLM_DT_F32, SQLLM_DT_F16 or SQLLM_DT_BF16, y SQLLM_DT_F32 or the "
                               "16-bit type of x (SQLLM_DT_F16 for fp32 x)", x_dt, y_dt);
-}
-
-struct Plan {
-    int R, strips, T, chunk, G, maxc, hc, hrows, smem, maxseg, x_direct, xfloats;
-    size_t ws_cnt_off, ws_hyb_off, ws_part_off, ws_csr_off, ws_bytes;
-    int csr_rpc, has_stage;
-};
-
-// stage: bytes of the shared-memory staging buffer when the layer has CSR outliers or dense rows: STAGE for a launch (smaller only
-// in sqllm_workspace_bytes)
-int make_plan(int bits, int K, int N, int topX, bool has_csr_in, int stage, Plan &pl) {
-    std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);  // lazily initialised statics below
-    const bool has_csr = has_csr_in || topX > 0;  // from here on: "a staging buffer is needed"
-    pl.has_stage = has_csr ? stage : 0;
-    int sm = 0;
-    const int rc = dev_setup({{lutgemv_kernel<4>, 227 * 1024}, {lutgemv_kernel<3>, 227 * 1024}}, &sm);
-    if (rc) return rc;
-    const int XU = bits == 4 ? 8 : 32;
-    pl.R = bits == 4 ? K / 8 : K / 32;
-    pl.strips = (N + STRIP - 1) / STRIP;
-    const long long T = (long long)pl.strips * pl.R;
-    if (T > 0x3fffffff) return fail(SQLLM_EINVAL, "problem too large");
-    pl.T = (int)T;
-    if (pl.strips > MAX_STRIPS || N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the workspace header (max %d)", N, MAX_N_FUSED);
-
-    // One wave: a plan whose shared memory lets fewer than CTAS_PER_SM CTAs onto an SM would run a second one.  Plan for
-    // CTAS_PER_SM, ask the occupancy calculator, and fall back to fewer CTAs per SM if it disagrees.
-    int use_cps = CTAS_PER_SM;
-replan:
-    const int G0 = sm * use_cps;
-    int chunk = (int)(2 * ((T + 2LL * G0 - 1) / (2LL * G0)));  // an even number of units: a consumer warp's pair never straddles the end
-    if (chunk > 3 * pl.R) chunk = 3 * pl.R;  // a CTA may touch at most MAXSEG strips
-    if (chunk < 2) chunk = 2;
-    int maxseg = (chunk - 2) / pl.R + 2;      // worst case over start offsets (even offsets, even R)
-    if (maxseg > MAXSEG) maxseg = MAXSEG;
-    const bool direct = (long long)chunk * XU >= K;
-    const int xfl = direct ? K : chunk * XU;
-    pl.x_direct = direct ? 1 : 0;
-    const int smem = bits == 4 ? Cfg<4>::total(maxseg, xfl, pl.has_stage) : Cfg<3>::total(maxseg, xfl, pl.has_stage);
-    if (smem > 227 * 1024) return fail(SQLLM_EINVAL, "in_features=%d needs %d B of shared memory (> 227 KB)", K, smem);
-    {
-        static std::unordered_map<unsigned long long, int> occ_cache;
-        const unsigned long long key = ((unsigned long long)smem << 8) | (unsigned long long)bits;
-        int occ = -1;
-        auto it = occ_cache.find(key);
-        if (it != occ_cache.end()) occ = it->second;
-        if (occ < 0) {
-            const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, THREADS, smem);
-            if (e != cudaSuccess) return fail(SQLLM_ECUDA, "occupancy query failed: %s", cudaGetErrorString(e));
-            occ_cache[key] = occ;
-        }
-        if (occ < 1) return fail(SQLLM_EINVAL, "kernel does not fit an SM (shared memory %d B)", smem);
-        if (occ < use_cps) { use_cps = occ; goto replan; }
-    }
-    pl.smem = smem;
-    pl.maxseg = maxseg;
-    pl.xfloats = xfl;
-    pl.chunk = chunk;
-    pl.G = (int)((T + chunk - 1) / chunk);
-    pl.maxc = (pl.R - 1) / chunk + 2;
-    pl.hc = 0;
-    pl.hrows = 0;
-    int hc = 0;
-    if (topX > 0) {
-        // dense-row contributors: as few k-rows per CTA as the grid allows, down to what one warp requests before the dependency
-        // wait (HYB_R steps of 32/topX rows), and no more partials (hc*topX floats) than the 2*CSR_CH-float staging buffer of the
-        // finisher holds
-        const int rows_pre = HYB_R * (topX <= 32 ? 32 / topX : 1);
-        hc = std::min({pl.G, (K + rows_pre - 1) / rows_pre, 2 * CSR_CH / topX});
-        if (hc < 1) hc = 1;
-        pl.hrows = (K + hc - 1) / hc;
-        pl.hc = (K + pl.hrows - 1) / pl.hrows;
-    }
-    pl.csr_rpc = (N + pl.G - 1) / pl.G;
-    if (pl.csr_rpc < 1) pl.csr_rpc = 1;
-    // Fixed header: [256, 256+4*MAX_STRIPS) per-strip tickets.  Tickets must never share bytes with data regions of ANY shape
-    // (the workspace is reused across layers of different sizes).
-    size_t off = WS_HEADER;
-    pl.ws_cnt_off = 256;
-    pl.ws_hyb_off = off; off += (size_t)hc * topX * 4;
-    off = (off + 255) & ~(size_t)255;
-    pl.ws_part_off = off; off += (size_t)pl.strips * pl.maxc * STRIP * 4;
-    off = (off + 255) & ~(size_t)255;
-    pl.ws_csr_off = off; off += (size_t)N * 4;
-    pl.ws_bytes = off;
-    return SQLLM_OK;
-}
-
-int launch(const sqllm_lutgemv_args *a, const Plan &pl, Params &p, cudaStream_t st) {
-    std::lock_guard<std::recursive_mutex> state_lock(g_state_mu);
-    set_layer(p, *a);
-    p.K = a->in_features; p.N = a->out_features;
-    p.R = pl.R; p.strips = pl.strips; p.T = pl.T; p.chunk = pl.chunk;
-    p.maxseg = pl.maxseg; p.x_direct = pl.x_direct; p.xfloats = pl.xfloats;
-    p.hc = p.topX > 0 ? pl.hc : 0; p.hrows = pl.hrows; p.maxc = pl.maxc;
-    p.has_stage = pl.has_stage;
-    p.csr_rpc = pl.csr_rpc;
-    p.csr_al16 = (a->rows && ((reinterpret_cast<uintptr_t>(a->cols) | reinterpret_cast<uintptr_t>(a->vals)) & 15) == 0) ? 1 : 0;
-    p.trace = g_trace;
-    if (g_trace) g_trace += g_trace_stride;
-    g_last_grid = pl.G;
-    const cudaError_t e = launch_ex(a->bits == 4 ? lutgemv_kernel<4> : lutgemv_kernel<3>, pl.G, THREADS, pl.smem, st, PDL, p);
-    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
-    return SQLLM_OK;
 }
 
 // =================================================================================================
@@ -219,7 +114,6 @@ int launch2(const sqllm_lutgemv_args *a, int variant, bool fused, v2::P2 &p, cud
     if (rc) return rc;
     int G = 0;
     if ((rc = plan_layer(*a, sm, p, G))) return rc;
-    if (fused && p.N > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the fused accumulator (max %d)", p.N, MAX_N_FUSED);
     if (fused && G > MAX_GRID_V2) return fail(SQLLM_EINVAL, "grid of %d CTAs exceeds the mailbox area (%d)", G, MAX_GRID_V2);
     const unsigned base = (raw + 127u) & ~127u;
     const unsigned xbytes = (unsigned)((p.K * (variant == 0 ? 4 : 2) + 127) & ~127);  // this layer's x, in its own dtype
@@ -593,8 +487,8 @@ extern "C" void sqllm_sequence_destroy(sqllm_sequence *s) {
 
 namespace {
 
-// ---- fused GEMV: v2, or v1 in the deterministic mode; with an exchange descriptor (v2 only) the result goes to every rank's
-// arena instead of y ---------------------------------------------------------------------------------------------------------------
+// ---- fused GEMV: v2, or the multi-row kernel at one row in the deterministic mode; with an exchange descriptor (v2 only) the result
+// goes to every rank's arena instead of y ------------------------------------------------------------------------------------------
 // x_dt / y_dt: SQLLM_DT_* codes, a pair sqllm_lutgemv_fused_dt accepts
 int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y, int y_dt, const float *bias,
                   void *workspace, size_t workspace_bytes, const sqllm_exchange *xc, cudaStream_t st) {
@@ -619,9 +513,10 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y,
     }
     const bool hyb = a->full_rows && a->topX > 0;
     if (hyb && a->topX > MAX_TOPX_FUSED) return fail(SQLLM_EINVAL, "fused path supports topX <= %d", MAX_TOPX_FUSED);
+    if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
+    if (a->out_features > MAX_N_FUSED) return fail(SQLLM_EINVAL, "out_features=%d exceeds the fused accumulator (max %d)", a->out_features, MAX_N_FUSED);
     unsigned char *ws = static_cast<unsigned char *>(workspace);
     if (det == 0) {
-        if (!workspace || workspace_bytes < WS_HEADER) return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", (size_t)WS_HEADER, workspace_bytes);
         v2::P2 q;
         memset(&q, 0, sizeof(q));
         q.ws_cnt = reinterpret_cast<int *>(ws);
@@ -640,19 +535,10 @@ int lutgemv_fused(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y,
         const int variant = x_dt == SQLLM_DT_F16 ? (lut_mode() == 1 && a->out_features >= STRIP ? 2 : 1) : x_dt == SQLLM_DT_BF16 ? 3 : 0;
         return launch2(a, variant, true, q, st);
     }
-    Plan pl;
-    rc = make_plan(a->bits, a->in_features, a->out_features, hyb ? a->topX : 0, a->rows != nullptr, STAGE, pl);
-    if (rc) return rc;
-    if (!workspace || workspace_bytes < pl.ws_bytes)
-        return fail(SQLLM_EWORKSPACE, "workspace too small: need %zu bytes, got %zu", pl.ws_bytes, workspace_bytes);
-    Params p;
-    memset(&p, 0, sizeof(p));
-    p.ws_cnt = reinterpret_cast<int *>(ws + pl.ws_cnt_off);
-    p.ws_hyb = reinterpret_cast<float *>(ws + pl.ws_hyb_off);
-    p.ws_part = reinterpret_cast<float *>(ws + pl.ws_part_off);
-    p.ws_csr = reinterpret_cast<float *>(ws + pl.ws_csr_off);
-    p.x = x; p.x_dt = x_dt; p.out = y; p.y_dt = y_dt; p.bias = bias;
-    return launch(a, pl, p, st);
+    // a row of the multi-row kernel has the same bits at any M and is written once, in a fixed order: one row is a deterministic GEMV
+    sqllm_lutgemv_args one = *a;
+    one.batch = 1;
+    return launch_rows(&one, x, x_dt, y, y_dt, bias, st);
 }
 
 }  // namespace
@@ -669,17 +555,13 @@ int sqllm_workspace_error(const void *workspace, void *stream) {
 }
 
 size_t sqllm_workspace_bytes(int bits, int in_features, int out_features, int topX) {
-    Plan pl;
     if (bits != 3 && bits != 4) return 0;
     if (in_features <= 0 || in_features % 64 || out_features <= 0) return 0;
-    // CSR staging changes the shared-memory footprint, hence occupancy, grid and chunk: take the max of both plans.  The
-    // deterministic mode gets exactly what its kernel needs.  The default mode plans with the CSR cols / vals alone in the staging
-    // buffer: less shared memory, at least as many CTAs and strip partials, so a workspace sized in either mode serves both.
-    const int stage = det_mode() == 1 ? STAGE : CSR_CH * 8;
-    size_t b = 0;
-    for (int csr = 0; csr < 2; ++csr)
-        if (make_plan(bits, in_features, out_features, topX, csr != 0, stage, pl) == SQLLM_OK && pl.ws_bytes > b) b = pl.ws_bytes;
-    return b;
+    if (out_features > MAX_N_FUSED) {
+        fail(SQLLM_EINVAL, "out_features=%d exceeds the workspace header (max %d)", out_features, MAX_N_FUSED);
+        return 0;
+    }
+    return WS_HEADER;  // v2 keeps everything in the fixed header; the deterministic mode needs no workspace
 }
 
 int sqllm_lutgemv(const sqllm_lutgemv_args *a, void *stream) {

@@ -1,6 +1,6 @@
 // lutgemv_rows.cu - the GEMVs of several rows on the CUDA cores: the batched tile kernel and its outlier kernels behind the *_batched
-// symbols (lutgemm_batched.cuh), and the multi-row LUT-GEMV with a cluster split-K behind sqllm_lutgemv_rows_dt (lutgemv_rows.cuh),
-// which shares the batched kernel's table layout and decode.
+// symbols (lutgemm_batched.cuh), and the multi-row LUT-GEMV with a cluster split-K behind sqllm_lutgemv_rows_dt and the deterministic
+// fused mode (lutgemv_rows.cuh), which shares the batched kernel's table layout and decode.
 #include <stdint.h>
 #include <string.h>
 
@@ -54,7 +54,7 @@ int launch_batched(const sqllm_lutgemv_args *a, cudaStream_t st) {
 
 namespace {
 
-// ---- a few fp16 / bf16 rows (lutgemv_rows.cuh): plan + launch ------------------------------------------------------------------
+// ---- a few rows (lutgemv_rows.cuh): plan + launch ------------------------------------------------------------------------------
 // Slabs per strip S (the cluster size) from K, N and the SM count only - never from M, so that a row's result does not depend on
 // M: the smallest S in {1, 2, 4, 8} that gives at least two CTAs per SM and a slab of at most SLAB_GOAL inputs, with no more
 // slabs than units.  Rows per CTA RB from M: 2, 4 or 8 (a row computes the same bits whatever RB is).
@@ -82,9 +82,43 @@ KRows krows_lookup_t(int bits, int RB) {
     if (bits == 4) return RB == 2 ? lutgemv_rows_kernel<4, 2, XT> : RB == 4 ? lutgemv_rows_kernel<4, 4, XT> : lutgemv_rows_kernel<4, 8, XT>;
     return RB == 2 ? lutgemv_rows_kernel<3, 2, XT> : RB == 4 ? lutgemv_rows_kernel<3, 4, XT> : lutgemv_rows_kernel<3, 8, XT>;
 }
-KRows krows_lookup(int bits, int RB, bool bf16) { return bf16 ? krows_lookup_t<__nv_bfloat16>(bits, RB) : krows_lookup_t<__half>(bits, RB); }
+// fp32 x is instantiated at RB = 2 only: it comes from the deterministic fused mode, which runs one row
+KRows krows_lookup(int bits, int RB, int x_dt) {
+    using namespace rows;
+    if (x_dt == SQLLM_DT_F32) return RB != 2 ? nullptr : bits == 4 ? lutgemv_rows_kernel<4, 2, float> : lutgemv_rows_kernel<3, 2, float>;
+    return x_dt == SQLLM_DT_BF16 ? krows_lookup_t<__nv_bfloat16>(bits, RB) : krows_lookup_t<__half>(bits, RB);
+}
 
 }  // namespace
+
+namespace __attribute__((visibility("hidden"))) sqllm {
+
+int launch_rows(const sqllm_lutgemv_args *a, const void *x, int x_dt, void *y, int y_dt, const float *bias, cudaStream_t st) {
+    int sm = 0;
+    int rc = dev_setup({}, &sm);
+    if (rc) return rc;
+    RowsPlan pl;
+    if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
+    const KRows kern = krows_lookup(a->bits, pl.RB, x_dt);
+    if (!kern) return fail(SQLLM_EINVAL, "fp32 x is taken for one or two rows only (got batch=%d)", a->batch);
+    if ((rc = dev_setup({{kern, 227 * 1024}}))) return rc;
+    const int groups = (a->batch + pl.RB - 1) / pl.RB;
+    if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
+    rows::PR p;
+    memset(&p, 0, sizeof(p));
+    set_layer(p, *a);
+    p.x = x; p.y = y; p.y_16 = y_dt != SQLLM_DT_F32; p.bias = bias;
+    p.K = a->in_features; p.N = a->out_features; p.M = a->batch; p.R = a->bits == 4 ? p.K / 8 : p.K / 32;
+    p.ks = pl.ks; p.kpad = pl.kpad;
+    p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0;
+    // the S CTAs of a strip's cluster split its K
+    const cudaError_t e = launch_ex(kern, dim3(pl.S, (a->out_features + STRIP - 1) / STRIP, groups), rows::RTHREADS, pl.smem, st,
+                                    cluster_of(pl.S), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+}  // namespace sqllm
 
 extern "C" {
 
@@ -105,26 +139,7 @@ int sqllm_lutgemv_rows_dt(const sqllm_lutgemv_args *a, const void *x, int x_dtyp
         return fail(SQLLM_EINVAL, "qweight, lookup_table and bias must be 4-byte aligned");
     if (reinterpret_cast<uintptr_t>(x) & 15) return fail(SQLLM_EINVAL, "x must be 16-byte aligned");
     if (reinterpret_cast<uintptr_t>(y) & 15) return fail(SQLLM_EINVAL, "y must be 16-byte aligned");
-    int sm = 0;
-    if ((rc = dev_setup({}, &sm))) return rc;
-    RowsPlan pl;
-    if ((rc = rows_plan(a->bits, a->in_features, a->out_features, a->batch, sm, pl))) return rc;
-    const KRows kern = krows_lookup(a->bits, pl.RB, x_dtype == SQLLM_DT_BF16);
-    if ((rc = dev_setup({{kern, 227 * 1024}}))) return rc;
-    const int groups = (a->batch + pl.RB - 1) / pl.RB;
-    if (groups > 65535) return fail(SQLLM_EINVAL, "batch=%d is too large for one call (max %d)", a->batch, 65535 * pl.RB);
-    rows::PR p;
-    memset(&p, 0, sizeof(p));
-    set_layer(p, *a);
-    p.x = x; p.y = y; p.y_16 = y_dtype != SQLLM_DT_F32; p.bias = bias;
-    p.K = a->in_features; p.N = a->out_features; p.M = a->batch; p.R = a->bits == 4 ? p.K / 8 : p.K / 32;
-    p.ks = pl.ks; p.kpad = pl.kpad;
-    p.qw_al16 = (reinterpret_cast<uintptr_t>(a->qweight) & 15) == 0;
-    // the S CTAs of a strip's cluster split its K
-    const cudaError_t e = launch_ex(kern, dim3(pl.S, (a->out_features + STRIP - 1) / STRIP, groups), rows::RTHREADS, pl.smem,
-                                    static_cast<cudaStream_t>(stream), cluster_of(pl.S), p);
-    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "lutgemv_rows launch failed: %s", cudaGetErrorString(e));
-    return SQLLM_OK;
+    return launch_rows(a, x, x_dtype, y, y_dtype, bias, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

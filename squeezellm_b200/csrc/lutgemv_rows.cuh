@@ -1,14 +1,15 @@
 // lutgemv_rows.cuh - the multi-row LUT-GEMV behind sqllm_lutgemv_rows_dt: a few fp16 or bf16 rows (decode of several sequences,
-// speculative-decoding verification, short prompts) in ONE launch.  It shares the table layout, decode and row FMAs
-// (batched::unit_fma) of lutgemm_batched.cuh.
+// speculative-decoding verification, short prompts) in ONE launch, and the one row of the deterministic fused mode
+// (sqllm_set_deterministic), which also takes fp32 x.  It shares the table layout, decode and row FMAs (batched::unit_fma) of
+// lutgemm_batched.cuh.
 //
-//   y[m][c] = sum_k W[k][c] x[m][k] + CSR + dense rows (+ bias),  fp16 or bf16 x [M][K] (XT), y fp32 or x's type, exact fp32
-//   codebook, fp32 sums.
+//   y[m][c] = sum_k W[k][c] x[m][k] + CSR + dense rows (+ bias),  fp16, bf16 or fp32 x [M][K] (XT), y fp32 or 16-bit (bf16 for
+//   bf16 x, else fp16), exact fp32 codebook, fp32 sums.
 //
 // Tiling: a CTA owns one 64-column strip, one K-slab and one group of RB rows; grid (S, strips, ceil(M / RB)), launched as clusters of
 // (S, 1, 1): the S CTAs of a cluster split the strip's K.  S comes from K, N and the SM count only (rows_plan), never from M, and
 // every row runs the same instructions whatever RB is, so a row's result does not depend on M or on the other rows.
-//   * x: the CTA stages its slab of its rows, converted to fp32 (exact for both types), rows padded to an even number of units with
+//   * x: the CTA stages its slab of its rows, converted to fp32 (exact for every type), rows padded to an even number of units with
 //     zeros.  Nothing after the staging depends on x's type.
 //   * weights: each lane reads its 16 bytes per unit row straight from global memory, one position ahead (as lutgemm_batched_kernel),
 //     decodes its 4 columns x one unit once and runs them against all RB rows.
@@ -36,8 +37,8 @@ constexpr int MAX_SLABS = 8;          // S <= 8: portable cluster size
 struct PR {
     const uint32_t *qw;
     const float *lut;
-    const void *x;      // [M][K], fp16 or bf16 (the kernel's XT)
-    void *y;            // [M][N], fp32 or XT
+    const void *x;      // [M][K], fp16, bf16 or fp32 (the kernel's XT)
+    void *y;            // [M][N], fp32, or bf16 for bf16 x and fp16 otherwise
     const float *bias;  // may be null
     const int *rows, *cols;
     const float *vals;
@@ -47,7 +48,7 @@ struct PR {
     int K, N, M, R;     // R = units per strip
     int ks;             // units per slab
     int kpad;           // floats per staged x row: ks rounded up to an even number of units
-    int y_16;           // y is XT, not fp32
+    int y_16;           // y is 16-bit, not fp32
     int qw_al16;        // qweight is 16-byte aligned: 16-byte weight loads
 };
 
@@ -98,11 +99,17 @@ __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
             const int b = e / n8, q = e - b * n8;
             float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
             if (b0 + b < p.M && 8 * q < kn) {
-                const uint4 h = __ldg(reinterpret_cast<const uint4 *>(static_cast<const XT *>(p.x) + (size_t)(b0 + b) * p.K + k_lo + 8 * q));
-                const float2 f0 = x16x2_to_f32x2<XT>(h.x), f1 = x16x2_to_f32x2<XT>(h.y);
-                const float2 f2 = x16x2_to_f32x2<XT>(h.z), f3 = x16x2_to_f32x2<XT>(h.w);
-                lo = make_float4(f0.x, f0.y, f1.x, f1.y);
-                hi = make_float4(f2.x, f2.y, f3.x, f3.y);
+                const XT *src = static_cast<const XT *>(p.x) + (size_t)(b0 + b) * p.K + k_lo + 8 * q;
+                if constexpr (std::is_same<XT, float>::value) {
+                    lo = __ldg(reinterpret_cast<const float4 *>(src));
+                    hi = __ldg(reinterpret_cast<const float4 *>(src) + 1);
+                } else {
+                    const uint4 h = __ldg(reinterpret_cast<const uint4 *>(src));
+                    const float2 f0 = x16x2_to_f32x2<XT>(h.x), f1 = x16x2_to_f32x2<XT>(h.y);
+                    const float2 f2 = x16x2_to_f32x2<XT>(h.z), f3 = x16x2_to_f32x2<XT>(h.w);
+                    lo = make_float4(f0.x, f0.y, f1.x, f1.y);
+                    hi = make_float4(f2.x, f2.y, f3.x, f3.y);
+                }
             }
             float4 *dst = reinterpret_cast<float4 *>(sm + C::TAB + b * xpitch + 32 * q);
             dst[0] = lo;
@@ -249,7 +256,7 @@ __global__ void __launch_bounds__(RTHREADS, 2) lutgemv_rows_kernel(const PR p) {
                     v.x = *reinterpret_cast<const uint32_t *>(&h01);
                     v.y = *reinterpret_cast<const uint32_t *>(&h23);
                 }
-                *reinterpret_cast<uint2 *>(static_cast<XT *>(p.y) + o) = v;
+                *reinterpret_cast<uint2 *>(static_cast<uint16_t *>(p.y) + o) = v;
             } else {
                 *reinterpret_cast<float4 *>(static_cast<float *>(p.y) + o) = s;
             }

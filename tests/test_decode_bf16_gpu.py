@@ -1,5 +1,5 @@
 """bf16 decode on the fused kernels: one bf16 row through the one-GEMV kernels (`sqllm_lutgemv_fused_dt`, `quant_cuda.lutgemv_fused`;
-lutgemv2_kernel in the default mode, the round-1 kernel in the deterministic one) and 2 to QuantLinearLUT.BF16_ROWS_MAX bf16 rows
+lutgemv2_kernel in the default mode, the multi-row kernel at one row in the deterministic one) and 2 to QuantLinearLUT.BF16_ROWS_MAX bf16 rows
 through the multi-row GEMV (`sqllm_lutgemv_rows_dt`, `quant_cuda.lutgemv_rows_bf16`).  The truth is the fp64 oracle on the
 bf16-rounded activations; the metric is the per-element bound of tests/util.py (bound_ratio <= 1) beside rel_err < TIGHT_TOL, both
 with fp32 output.  Covered: the parity shapes at both bit widths, narrow and wide layers, dense-row and CSR edge cases in both

@@ -162,7 +162,7 @@ def test_dense_rows_every_mode(lib, topx, pattern):
 @pytest.mark.parametrize("pattern", ["chan0", "one-strip", "edges", "mixed"])
 @pytest.mark.parametrize("topx", [1, 17, 33, 128])
 def test_dense_rows_narrow_layer_every_mode(lib, topx, pattern):
-    """N = 60 < 64: one ragged strip in every mode; in the deterministic mode the round-1 kernel's hybrid_totals (tp <= 16 split)."""
+    """N = 60 < 64: one ragged strip in every mode; in the deterministic mode one strip of the multi-row kernel at one row."""
     _every_mode(lib, _layer(4, 512, 60, topx, pattern, sparsity=0.02, seed=topx + 500))
 
 
@@ -268,7 +268,7 @@ def test_wide_layer_dense_rows_in_late_owned_strips(lib, bits, K, N):
 # D. CSR arrays that are not 16-byte aligned (staged with 4-byte copies on another chunk grid)
 def _csr_with_long_row(K, N, long_len, rng):
     counts = rng.integers(0, 9, size=N)
-    counts[N // 3] = long_len  # longer than a staging chunk (v2: 256, round 1: 1024 elements)
+    counts[N // 3] = long_len  # longer than a staging chunk (v2: 256 elements)
     rows = np.zeros(N + 1, dtype=np.int32)
     rows[1:] = np.cumsum(counts)
     cols = np.concatenate([np.sort(rng.choice(K, size=c, replace=False)) for c in counts]).astype(np.int32)
