@@ -1,7 +1,7 @@
 // lutgemv_seq.cuh - the SEQUENCE kernel: one persistent launch runs a whole list of dependent LUT-GEMVs (a decode token's QuantLinear
 // matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Built on lutgemv_v2.cuh:
 // the per-position math, table builders, outlier warps (sparse3), mailboxes, CTA span (Span) and strip flush (flush_strip) are v2's
-// (namespace v2), what is new is everything BETWEEN two GEMVs.
+// (namespace v2), and so is the finishing pass (lutgemv_finish.inc); what is new is everything BETWEEN two GEMVs.
 //
 // Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
 // carries a fixed cost (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
@@ -264,7 +264,6 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         const uint32_t lutbuf = base + OFF_LUT;
 #pragma unroll
         for (int b = 0; b < NTB; ++b) sts_u32(sacc0 + 4 * (b * STRIP + bt), 0u);
-        int *const err = c.err;
         int q0 = 0;  // segments of earlier GEMVs: segment s of this one uses table buffer / accumulator (q0 + s) % NTB
         auto prefetch_first = [&](const P2 &p) {  // the raw LUT rows of a GEMV's first two strips
             const Span sp(p);
@@ -282,7 +281,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             float *const acc_out = p.ws_acc;
             auto sacc_of = [&](int s) { return sacc0 + 4u * (uint32_t)(((q0 + s) % NTB) * STRIP + bt); };
             auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + 288 + 8 * ((q0 + s) % NTB), (uint32_t)(((q0 + s) / NTB) & 1)); };
-            const uint32_t sown = base + OFF_FIN;   // float [SOWN][64], as in lutgemv2_kernel
+            const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
             const int ofs = r0 != 0 ? 1 : 0;        // segment s is owned strip s - ofs
             auto flush = [&](int s) { flush_strip<true>(p, sacc_of(s), s, ofs, sp, N, base, bt, acc_out, boxtag); };
             for (int s = 0; s < nseg; ++s) {
@@ -300,87 +299,29 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 if (s + 2 < nseg) lut_prefetch<BITS>(p, lutbuf + (s & 1) * LUTBUF, s0 + s + 2, bt);
             }
             if (g + 1 < ngemv) prefetch_first(c.descs[g + 1].p);  // the next GEMV's rows travel while this one is being finished
-            // ---- finish the strips this CTA owns (those that start in its range); see lutgemv_v2.cuh for the protocol ----
-            TRACE(12, bt == 0);
-            const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
-            const int so0 = (int)((cb0 + R - 1) / R), so1 = (int)((cb1 + R - 1) / R), nown = so1 - so0;
-            const bool last_owned = nseg >= 2 || r0 == 0;
-            constexpr int FAST = 4;
-            const int lidx = last_owned && nseg > 0 ? nown - 1 : -1;
-            const int nh = lidx >= 0 ? (int)((((long long)(so1 - 1) + 1) * R - 1) / p.chunk) - (int)blockIdx.x : 0;
-            // Dense rows whose channel lies in a strip we own: listed now (static), summed below.  sdj[i] = dense row, sden[i] = its sum.
-            int *const sdj = reinterpret_cast<int *>(sm + OFF_FIN + 2048);
-            const uint32_t sden = base + OFF_FIN + 2048 + 4 * 128, sdn_a = base + OFF_FIN + 2048 + 8 * 128;
-            if (p.full_rows) {
-                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads for the 30
-                //  dense rows of a stacked q/k/v layer - on every CTA, before its first mailbox row went out)
-                const int topX = p.topX;
-                if (bt == 0) sts_u32(sdn_a, 0u);
-                sts_u32(sden + 4 * bt, 0u);
-                sts_u32(sden + 4 * (bt + NBT), 0u);
-                named_bar_sync(3, NBT);
-                if (topX <= 32) {
-                    if (bt < 32) {
-                        const int cc = bt < topX ? __ldg(p.fri + bt) : -1 - bt;
-                        bool first = true;  // rows on the same channel were combined by the contributors: the first of them carries the sum
-                        for (int j2 = 0; j2 < topX; ++j2) {
-                            const int c2 = __shfl_sync(0xffffffffu, cc, j2);
-                            if (c2 == cc && j2 < bt) first = false;
-                        }
-                        const bool mine = bt < topX && first && cc >= 0 && cc < N && cc / STRIP >= so0 && cc / STRIP < so1;
-                        const unsigned m = __ballot_sync(0xffffffffu, mine);
-                        if (mine) sdj[__popc(m & ((1u << bt) - 1u))] = bt;
-                        if (bt == 0) sts_u32(sdn_a, (uint32_t)__popc(m));
-                    }
-                } else {
-                    for (int j = bt; j < topX; j += NBT) {
-                        const int cc = __ldg(p.fri + j);
-                        if (cc >= 0 && cc < N && cc / STRIP >= so0 && cc / STRIP < so1) {
-                            uint32_t at;
-                            asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(at) : "r"(sdn_a) : "memory");
-                            sdj[at] = j;
-                        }
-                    }
-                }
-                named_bar_sync(3, NBT);
-            }
-            const int sdn = p.full_rows ? (int)lds_u32(sdn_a) : 0;
-            for (int s = max(0, nseg - NTB); s < nseg - 1; ++s) {
-                tfree_wait(s);
-                flush(s);
-            }
-            TRACE(13, bt == 0);
-            {
-                unsigned long long cw[FAST], hw[3];
-#pragma unroll
-                for (int u = 0; u < FAST; ++u) {
-                    const int col = (so0 + u) * STRIP + bt;
-                    cw[u] = (p.rows && u < nown && col < N) ? ld_relaxed_u64(p.ws_cbox + col) : box_word(0.f, boxtag);
-                }
-#pragma unroll
-                for (int h = 0; h < 3; ++h)
-                    hw[h] = h < nh ? ld_relaxed_u64(p.ws_hbox + ((size_t)blockIdx.x + 1 + h) * STRIP + bt) : box_word(0.f, boxtag);
-                // OPS residual: one word per owned column, issued with the mailbox words.  An external vector's element is given the token's
-                // tag here; an earlier item's word is taken like x (read again until it carries the tag, bounded).  Column col reads the
-                // element of the full-length vector that store_y writes: col on one GPU, e below on several.
-                const uint32_t *res_tag = nullptr;
-                const XT *res_ext = nullptr;
+            // the finishing pass (lutgemv_finish.inc): mailbox words are never reset (a stale word carries an older tag); y is a tagged
+            // word in every rank's arena, and a plain XT copy if the item has one
+            constexpr bool box_keep = true;
+            auto err_word = [&]() { return c.err; };
+            // OPS residual: one word per owned column, issued with the mailbox words (res_load).  An external vector's element is given
+            // the token's tag here; an earlier item's word is taken like x (read again until it carries the tag, bounded).  Column col
+            // reads the element of the full-length vector that store_y writes: col on one GPU, e below on several.
+            const uint32_t *res_tag = nullptr;
+            const XT *res_ext = nullptr;
+            auto res_index = [&](int col) -> unsigned {
+                if constexpr (!MULTI) return (unsigned)col;
+                const int wm = N / p.xw_members, mm = col / wm;
+                return (unsigned)(mm * p.xw_nfull + c.rank * wm + (col - mm * wm));
+            };
+            auto res_word = [&](int col) -> uint32_t {
+                if (res_tag) return ld_relaxed_u32<MULTI>(res_tag + res_index(col));
+                if (res_ext) return xwant | (uint32_t)bits16(res_ext[res_index(col)]);
+                return 0u;
+            };
+            auto res_load = [&](uint32_t *rw, uint32_t &rlast, const int so0, const int nown, const int lidx) {
                 if constexpr (OPS) {
                     res_tag = c.ops[g].res_tag;
                     res_ext = static_cast<const XT *>(c.ops[g].res_ext);
-                }
-                auto res_index = [&](int col) -> unsigned {
-                    if constexpr (!MULTI) return (unsigned)col;
-                    const int wm = N / p.xw_members, mm = col / wm;
-                    return (unsigned)(mm * p.xw_nfull + c.rank * wm + (col - mm * wm));
-                };
-                auto res_word = [&](int col) -> uint32_t {
-                    if (res_tag) return ld_relaxed_u32<MULTI>(res_tag + res_index(col));
-                    if (res_ext) return xwant | (uint32_t)bits16(res_ext[res_index(col)]);
-                    return 0u;
-                };
-                uint32_t rw[FAST], rlast = 0u;
-                if constexpr (OPS) {
                     if (res_tag || res_ext) {
 #pragma unroll
                         for (int u = 0; u < FAST; ++u) {
@@ -390,51 +331,13 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                         const int lcol = (so0 + lidx) * STRIP + bt;
                         if (lidx >= 0 && lcol < N) rlast = res_word(lcol);
                     }
+                } else {
+                    for (int u = 0; u < FAST; ++u) rw[u] = 0u;
                 }
-                // dense rows: hc tagged words per listed row (one from every contributing CTA), four loads in flight per thread; row sums are
-                // collected in shared memory and added to the column they belong to by the thread that owns that column
-                float last_dense = 0.f;
-                if (sdn > 0) {
-                    const int hc = p.hc;
-                    unsigned long long *const dbox = p.ws_dbox;
-                    for (int j0 = 0; j0 < sdn; j0 += 4) {  // four rows x up to four words per thread in flight (hc <= MAX_GRID_V2 = 4 x NBT)
-                        unsigned long long dw[4][4];
-                        int row[4];
-#pragma unroll
-                        for (int a = 0; a < 4; ++a) {
-                            row[a] = j0 + a < sdn ? sdj[j0 + a] : -1;
-#pragma unroll
-                            for (int b = 0; b < 4; ++b)
-                                if (row[a] >= 0 && bt + b * NBT < hc) dw[a][b] = ld_relaxed_u64(dbox + (size_t)row[a] * MAX_GRID_V2 + bt + b * NBT);
-                        }
-#pragma unroll
-                        for (int a = 0; a < 4; ++a) {
-                            if (row[a] < 0) continue;  // (uniform)
-                            float v = 0.f;
-#pragma unroll
-                            for (int b = 0; b < 4; ++b)
-                                if (bt + b * NBT < hc) v += box_take(dw[a][b], dbox + (size_t)row[a] * MAX_GRID_V2 + bt + b * NBT, err, boxtag, true);
-                            v = warp_sum(v);
-                            if (lane == 0) asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sden + 4u * (uint32_t)(j0 + a)), "f"(v) : "memory");
-                        }
-                    }
-                    named_bar_sync(3, NBT);
-                    for (int i = 0; i < sdn; ++i) {
-                        const int cc = __ldg(p.fri + sdj[i]);
-                        if ((cc & (STRIP - 1)) == bt) {
-                            const int u = cc / STRIP - so0;
-                            const float v = lds_f32(sden + 4u * (uint32_t)i);
-                            if (u == lidx) last_dense += v;
-                            else if (u < SOWN) {
-                                const uint32_t a = sown + 4u * (uint32_t)(u * STRIP + bt);
-                                sts_u32(a, __float_as_uint(lds_f32(a) + v));
-                            } else atomicAdd(acc_out + cc, v);
-                        }
-                    }
-                    named_bar_sync(3, NBT);  // (the list and the sums are reused by the next item; an idle CTA has no other barrier before that)
-                }
+            };
+            auto make_store_y = [&]() {
                 const int w = MULTI ? N / p.xw_members : 0;
-                auto store_y = [&](int col, float yv, uint32_t rword = 0u) {
+                return [&, w](int col, float yv, uint32_t rword) {
                     if (p.bias) yv += __ldg(p.bias + col);
                     if constexpr (OPS) {
                         if (res_tag || res_ext) {  // y = round_XT(sum + bias + r): the residual too is inside the one rounding
@@ -445,7 +348,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                                 do {
                                     rword = ld_relaxed_u32<MULTI>(src);
                                     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                                    if (t1 - t0 > 2000000000ull) { *reinterpret_cast<volatile int *>(err) = 1; break; }
+                                    if (t1 - t0 > 2000000000ull) { *reinterpret_cast<volatile int *>(c.err) = 1; break; }
                                 } while ((rword ^ xwant) >> 16);
                             }
                             yv += x16x2_to_f32x2<XT>(rword & 0xFFFFu).x;
@@ -465,61 +368,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                     // (the same value as yh, converted again as before bf16 existed: reusing yh reschedules the fp16 MULTI instantiations)
                     if (p.out) reinterpret_cast<XT *>(p.out)[col] = f32_to<XT>(yv);
                 };
-                // per owned strip but the last segment's: [our own sums (+ dense rows), from shared memory] + [the column's outlier sum]
-                TRACE(14, bt == 0);
-                float last_others = last_dense;
-#pragma unroll
-                for (int u = 0; u < FAST; ++u) {
-                    const int col = (so0 + u) * STRIP + bt;
-                    if (u < nown && col < N) {
-                        float yv = 0.f;
-                        if (u != lidx && u < SOWN) yv = lds_f32(sown + 4u * (uint32_t)(u * STRIP + bt));
-                        if (p.rows) yv += box_take(cw[u], p.ws_cbox + col, err, boxtag, true);
-                        if (u == lidx) last_others += yv;
-                        else store_y(col, yv, OPS ? rw[u] : 0u);
-                    }
-                }
-                for (int i = FAST; i < nown; ++i) {  // (more owned strips than FAST; beyond SOWN the sums went through the global accumulator)
-                    const int col = (so0 + i) * STRIP + bt;
-                    if (col < N) {
-                        float yv = 0.f;
-                        if (i >= SOWN) { yv = __ldcg(p.ws_acc + col); p.ws_acc[col] = 0.f; }
-                        else if (i != lidx) yv = lds_f32(sown + 4u * (uint32_t)(i * STRIP + bt));
-                        if (p.rows) yv += box_take(0ull, p.ws_cbox + col, err, boxtag, true);
-                        if (i == lidx) last_others += yv;
-                        else store_y(col, yv, OPS ? res_word(col) : 0u);
-                    }
-                }
-                TRACE(15, bt == 0);
-#pragma unroll
-                for (int h = 0; h < 3; ++h)
-                    if (h < nh) last_others += box_take(hw[h], p.ws_hbox + ((size_t)blockIdx.x + 1 + h) * STRIP + bt, err, boxtag, true);
-                // (a strip that spans many CTAs - narrow column shards: 18 CTAs per strip for a 512-column shard of down_proj - has many such
-                //  words: eight reads in flight, not one round trip after the other)
-                for (int h0 = 3; h0 < nh; h0 += 8) {
-                    unsigned long long mw[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        if (h0 + k < nh) mw[k] = ld_relaxed_u64(p.ws_hbox + ((size_t)blockIdx.x + 1 + h0 + k) * STRIP + bt);
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        if (h0 + k < nh) last_others += box_take(mw[k], p.ws_hbox + ((size_t)blockIdx.x + 1 + h0 + k) * STRIP + bt, err, boxtag, true);
-                }
-                TRACE(8, bt == 0);
-                if (nseg > 0) {
-                    const int s = nseg - 1;
-                    tfree_wait(s);
-                    if (last_owned) {
-                        const uint32_t a = sacc_of(s);
-                        const float own = lds_f32(a);
-                        sts_u32(a, 0u);
-                        const int lcol = (s0 + s) * STRIP + bt;
-                        if (lcol < N) store_y(lcol, last_others + own, rlast);
-                    } else {
-                        flush(s);
-                    }
-                }
-            }
+            };
+#include "lutgemv_finish.inc"
             TRACE(9, bt == 0);
             q0 += nseg;
         }

@@ -640,9 +640,10 @@ __device__ __forceinline__ void warm_l2(const P2 &p, const int N, const int lane
 // accumulator.  (The first round-2 build sent all of them through the global accumulator: a RED and, in the finishing pass, a load that
 // had to wait for it - two L2 round trips between the last weight and y when the last segment is short.)
 // A mailbox word carries the kernel's tag (box_word): 1 in lutgemv2_kernel, reset by the owner; the (token, GEMV) tag in the sequence
-// kernel, never reset.  The finishing pass itself is written out in each kernel (DESIGN §3.4).
+// kernel, never reset.  The finishing pass itself is one text, lutgemv_finish.inc, #included by both kernels (DESIGN §3.4).
 // ---------------------------------------------------------------------------------------------------------------------------
 constexpr int SOWN = 8;
+constexpr int FAST = 4;  // owned strips whose outlier-sum words the finishing pass requests ahead, before it needs them
 
 // Strip sums of segment s (at `a` in shared memory, back to zero) -> the strip's owner; FUSED = false: one red.add per column.
 // ofs = sp.r0 != 0 (segment s is owned strip s - ofs), given by the caller: the sequence kernel has it once per GEMV.
@@ -769,7 +770,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         bool dep_ok = false;
         auto dep_wait = [&]() { if (!dep_ok) { pdl_wait(); dep_ok = true; } };  // builders never read x: they only need this before writing
         const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
-        auto flush = [&](int s) { flush_strip<FUSED>(p, sacc + 4 * ((s & 1) * STRIP + bt), s, r0 != 0 ? 1 : 0, sp, N, base, bt, acc_out, 1u); };
+        constexpr int NTB = 2;  // table buffers and strip accumulators
+        auto sacc_of = [&](int s) { return sacc + 4 * ((s & 1) * STRIP + bt); };
+        auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1)); };
+        auto flush = [&](int s) { flush_strip<FUSED>(p, sacc_of(s), s, r0 != 0 ? 1 : 0, sp, N, base, bt, acc_out, 1u); };
         // The raw LUT rows of the first two strips are requested at once (one cold round trip, not two); later strips two ahead.
         if (nseg > 0) lut_prefetch<BITS>(p, lutbuf, s0, bt);
         if (nseg > 1) lut_prefetch<BITS>(p, lutbuf + LUTBUF, s0 + 1, bt);
@@ -790,122 +794,21 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         }
         dep_wait();
         if constexpr (!FUSED) {
-            for (int s = max(0, nseg - 2); s < nseg; ++s) {  // the last two segments
-                mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1));
+            for (int s = max(0, nseg - NTB); s < nseg; ++s) {  // the last two segments
+                tfree_wait(s);
                 flush(s);
             }
         } else {
-            // ---- finish the strips this CTA owns (those that start in its range).  Every table is built, so the builders have time: while
-            //      the consumers are still in the last segment they collect the other contributors' mailbox words - the outlier row sums of
-            //      the strips' columns, the first-segment sums of the later CTAs that hold a part of the last owned strip, one tagged word
-            //      per (contributing CTA, dense row) if a dense-row channel lies in an owned strip - and add them to this CTA's own strip
-            //      sums, which never leave shared memory.  What is left for the very end is y = collected sums + own last segment (+ bias):
-            //      no round trip to L2 after the last weight, no grid-wide step; a CTA leaves as soon as its own strips are complete.
-            //      Waits are bounded (2 s, then the workspace error word is set).  The sequence kernel (lutgemv_seq.cuh) finishes the same way.
-            TRACE(12, bt == 0);
-            const long long cb0 = (long long)blockIdx.x * p.chunk, cb1 = min((long long)p.T, cb0 + p.chunk);
-            const int so0 = (int)((cb0 + R - 1) / R), so1 = (int)((cb1 + R - 1) / R), nown = so1 - so0;
-            const bool last_owned = nseg >= 2 || r0 == 0;
-            constexpr int FAST = 4;
-            const int lidx = last_owned && nseg > 0 ? nown - 1 : -1;
-            const int nh = lidx >= 0 ? (int)((((long long)(so1 - 1) + 1) * R - 1) / p.chunk) - (int)blockIdx.x : 0;
-            // Dense rows whose channel lies in a strip we own: listed now (static), summed below.  sdj[i] = dense row, sden[i] = its sum.
-            int *const err = p.ws_cnt + 16;
-            int *const sdj = reinterpret_cast<int *>(sm + OFF_FIN + 2048);
-            const uint32_t sden = base + OFF_FIN + 2048 + 4 * 128, sdn_a = base + OFF_FIN + 2048 + 8 * 128;
-            if (p.full_rows) {
-                // (one warp, registers and shuffles: a serial scan of full_row_indices by one thread cost 435 dependent loads for the 30
-                //  dense rows of a stacked q/k/v layer - on every CTA, before its first mailbox row went out)
-                const int topX = p.topX;
-                if (bt == 0) sts_u32(sdn_a, 0u);
-                sts_u32(sden + 4 * bt, 0u);
-                sts_u32(sden + 4 * (bt + NBT), 0u);
-                named_bar_sync(3, NBT);
-                if (topX <= 32) {
-                    if (bt < 32) {
-                        const int cc = bt < topX ? __ldg(p.fri + bt) : -1 - bt;
-                        bool first = true;  // rows on the same channel were combined by the contributors: the first of them carries the sum
-                        for (int j2 = 0; j2 < topX; ++j2) {
-                            const int c2 = __shfl_sync(0xffffffffu, cc, j2);
-                            if (c2 == cc && j2 < bt) first = false;
-                        }
-                        const bool mine = bt < topX && first && cc >= 0 && cc < N && cc / STRIP >= so0 && cc / STRIP < so1;
-                        const unsigned m = __ballot_sync(0xffffffffu, mine);
-                        if (mine) sdj[__popc(m & ((1u << bt) - 1u))] = bt;
-                        if (bt == 0) sts_u32(sdn_a, (uint32_t)__popc(m));
-                    }
-                } else {
-                    for (int j = bt; j < topX; j += NBT) {
-                        const int cc = __ldg(p.fri + j);
-                        if (cc >= 0 && cc < N && cc / STRIP >= so0 && cc / STRIP < so1) {
-                            uint32_t at;
-                            asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(at) : "r"(sdn_a) : "memory");
-                            sdj[at] = j;
-                        }
-                    }
-                }
-                named_bar_sync(3, NBT);
-            }
-            const int sdn = p.full_rows ? (int)lds_u32(sdn_a) : 0;
-            for (int s = max(0, nseg - 2); s < nseg - 1; ++s) {
-                mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1));
-                flush(s);
-            }
-            TRACE(13, bt == 0);
-            {
-                unsigned long long cw[FAST], hw[3];
-#pragma unroll
-                for (int u = 0; u < FAST; ++u) {
-                    const int col = (so0 + u) * STRIP + bt;
-                    cw[u] = (p.rows && u < nown && col < N) ? ld_relaxed_u64(p.ws_cbox + col) : box_word(0.f);
-                }
-#pragma unroll
-                for (int h = 0; h < 3; ++h)
-                    hw[h] = h < nh ? ld_relaxed_u64(p.ws_hbox + ((size_t)blockIdx.x + 1 + h) * STRIP + bt) : box_word(0.f);
-                // dense rows: hc tagged words per listed row (one from every contributing CTA), four loads in flight per thread; row sums are
-                // collected in shared memory and added to the column they belong to by the thread that owns that column
-                float last_dense = 0.f;
-                if (sdn > 0) {
-                    const int hc = p.hc;
-                    unsigned long long *const dbox = p.ws_dbox;
-                    for (int j0 = 0; j0 < sdn; j0 += 4) {  // four rows x up to four words per thread in flight (hc <= MAX_GRID_V2 = 4 x NBT)
-                        unsigned long long dw[4][4];
-                        int row[4];
-#pragma unroll
-                        for (int a = 0; a < 4; ++a) {
-                            row[a] = j0 + a < sdn ? sdj[j0 + a] : -1;
-#pragma unroll
-                            for (int b = 0; b < 4; ++b)
-                                if (row[a] >= 0 && bt + b * NBT < hc) dw[a][b] = ld_relaxed_u64(dbox + (size_t)row[a] * MAX_GRID_V2 + bt + b * NBT);
-                        }
-#pragma unroll
-                        for (int a = 0; a < 4; ++a) {
-                            if (row[a] < 0) continue;  // (uniform)
-                            float v = 0.f;
-#pragma unroll
-                            for (int b = 0; b < 4; ++b)
-                                if (bt + b * NBT < hc) v += box_take(dw[a][b], dbox + (size_t)row[a] * MAX_GRID_V2 + bt + b * NBT, err);
-                            v = warp_sum(v);
-                            if (lane == 0) asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sden + 4u * (uint32_t)(j0 + a)), "f"(v) : "memory");
-                        }
-                    }
-                    named_bar_sync(3, NBT);
-                    for (int i = 0; i < sdn; ++i) {
-                        const int cc = __ldg(p.fri + sdj[i]);
-                        if ((cc & (STRIP - 1)) == bt) {
-                            const int u = cc / STRIP - so0;
-                            const float v = lds_f32(sden + 4u * (uint32_t)i);
-                            if (u == lidx) last_dense += v;
-                            else if (u < SOWN) {
-                                const uint32_t a = sown + 4u * (uint32_t)(u * STRIP + bt);
-                                sts_u32(a, __float_as_uint(lds_f32(a) + v));
-                            } else atomicAdd(acc_out + cc, v);
-                        }
-                    }
-                    named_bar_sync(3, NBT);  // (the sequence kernel's copy reuses the list and the sums for its next item; here nothing does)
-                }
+            // the finishing pass (lutgemv_finish.inc): every mailbox word is written back to zero by its owner; no word per column
+            // besides the mailboxes'; y is fp32 or y16_t, in this rank's vector or, with the exchange, in every rank's
+            auto err_word = [&]() { return p.ws_cnt + 16; };
+            constexpr uint32_t boxtag = 1u;
+            constexpr bool box_keep = false;
+            auto res_load = [](uint32_t *rw, uint32_t &, int, int, int) { for (int u = 0; u < FAST; ++u) rw[u] = 0u; };
+            auto res_word = [](int) { return 0u; };
+            auto make_store_y = [&]() {
                 const int w = p.xw_world ? N / p.xw_members : 0;
-                auto store_y = [&](int col, float yv) {
+                return [&, w](int col, float yv, uint32_t) {
                     if (p.bias) yv += __ldg(p.bias + col);
                     if (p.xw_world == 0) {
                         if (p.y_is_half) reinterpret_cast<Y16 *>(p.out)[col] = f32_to<Y16>(yv);
@@ -922,61 +825,8 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
                         }
                     }
                 };
-                // per owned strip but the last segment's: [our own sums (+ dense rows), from shared memory] + [the column's outlier sum]
-                TRACE(14, bt == 0);
-                float last_others = last_dense;
-#pragma unroll
-                for (int u = 0; u < FAST; ++u) {
-                    const int col = (so0 + u) * STRIP + bt;
-                    if (u < nown && col < N) {
-                        float yv = 0.f;
-                        if (u != lidx && u < SOWN) yv = lds_f32(sown + 4u * (uint32_t)(u * STRIP + bt));
-                        if (p.rows) yv += box_take(cw[u], p.ws_cbox + col, err);
-                        if (u == lidx) last_others += yv;
-                        else store_y(col, yv);
-                    }
-                }
-                for (int i = FAST; i < nown; ++i) {  // (more owned strips than FAST; beyond SOWN the sums went through the global accumulator)
-                    const int col = (so0 + i) * STRIP + bt;
-                    if (col < N) {
-                        float yv = 0.f;
-                        if (i >= SOWN) { yv = __ldcg(p.ws_acc + col); p.ws_acc[col] = 0.f; }
-                        else if (i != lidx) yv = lds_f32(sown + 4u * (uint32_t)(i * STRIP + bt));
-                        if (p.rows) yv += box_take(0ull, p.ws_cbox + col, err);
-                        if (i == lidx) last_others += yv;
-                        else store_y(col, yv);
-                    }
-                }
-                TRACE(15, bt == 0);
-#pragma unroll
-                for (int h = 0; h < 3; ++h)
-                    if (h < nh) last_others += box_take(hw[h], p.ws_hbox + ((size_t)blockIdx.x + 1 + h) * STRIP + bt, err);
-                // (a strip that spans many CTAs - narrow column shards: 18 CTAs per strip for a 512-column shard of down_proj - has many such
-                //  words: eight reads in flight, not one round trip after the other)
-                for (int h0 = 3; h0 < nh; h0 += 8) {
-                    unsigned long long mw[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        if (h0 + k < nh) mw[k] = ld_relaxed_u64(p.ws_hbox + ((size_t)blockIdx.x + 1 + h0 + k) * STRIP + bt);
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)
-                        if (h0 + k < nh) last_others += box_take(mw[k], p.ws_hbox + ((size_t)blockIdx.x + 1 + h0 + k) * STRIP + bt, err);
-                }
-                TRACE(8, bt == 0);
-                if (nseg > 0) {
-                    const int s = nseg - 1;
-                    mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1));
-                    if (last_owned) {
-                        const uint32_t a = (sacc + 4 * ((s & 1) * STRIP + bt));
-                        const float own = lds_f32(a);
-                        sts_u32(a, 0u);
-                        const int lcol = (s0 + s) * STRIP + bt;
-                        if (lcol < N) store_y(lcol, last_others + own);
-                    } else {
-                        flush(s);
-                    }
-                }
-            }
+            };
+#include "lutgemv_finish.inc"
             if (p.xw_world) {
                 // exchange: every owning CTA publishes its stores on every rank (system-scope release); CTA 0 (it always owns strip 0)
                 // then holds the grid open until every owning CTA of every rank has published on ours: when this grid completes, the
