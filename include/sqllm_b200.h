@@ -53,7 +53,8 @@ extern "C" {
                                  sqllm_fisher_accumulate, sqllm_sequence_create_dt, sqllm_lutgemv_fused_exchange_dt,
                                  sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
                                  sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits,
-                                 sqllm_attn_extend, sqllm_attn_extend_splits, sqllm_sample
+                                 sqllm_attn_extend, sqllm_attn_extend_splits, sqllm_sample, sqllm_attn_verify,
+                                 sqllm_attn_verify_splits, sqllm_attn_verify_launch_splits
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -609,6 +610,54 @@ int sqllm_attn_extend(const sqllm_attn_extend_args *args, void *stream);
  * max(1, min(8, sm_count / tiles, ceil((start + n_tokens) / 64))); 0 for invalid arguments (a head layout that is not a positive
  * multiple, n_tokens < 1, start < 0, sm_count < 1, start + n_tokens above INT_MAX, more than 65535 tiles per KV head). */
 int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int sm_count);
+
+/* Decode attention of T <= 16 new tokens of one sequence at a device position (the verify step of speculative decoding): what T
+ * successive sqllm_attn_decode calls at *pos .. *pos+T-1 do, in ONE launch that reads the K / V cache once.
+ *   qkv       [T][n_heads*d | n_kv*d | n_kv*d] of dtype: the stacked q | k | v projection of the T tokens
+ *   pos       DEVICE int32: the first token's position (on the device so that a captured CUDA graph replays at a position that moves)
+ *   rope_cos, rope_sin  fp32 [capacity][d/2], as for sqllm_attn_decode
+ *   k_cache, v_cache    [n_kv][capacity][d] of dtype
+ *   out       [T][n_heads*d] of dtype
+ * Numerics, for token t at p_t = pos + t (c = rope_cos[p_t], s = rope_sin[p_t], i < d/2, rotate-half convention):
+ *   k'_t  = the rotary of k_t in fp32, rounded to dtype once - the expression of sqllm_attn_decode, so the stored bits equal those T
+ *           successive sqllm_attn_decode calls store; k' at k_cache[kv][p_t], v_t unchanged at v_cache[kv][p_t], the only cache
+ *           elements the call writes
+ *   q'_t  = the rotary of q_t in fp32, times scale * log2(e), not rounded
+ *   out[t, h] = round( sum_j 2^(z_j - M) V[j] / sum_j 2^(z_j - M) ),  z_j = q'_{t,h} . K[j] (fp32 FMAs), j = 0 .. p_t,
+ *           kv = h / (n_heads / n_kv), where K[p], V[p] for p >= pos are the call's own k', v: the fp32 online softmax of
+ *           sqllm_attn_decode, its partial states combined in a fixed order, rounded to dtype once.  Row t reads nothing of the qkv
+ *           rows after t.  No cache slot at or past pos + T is read.  Bit-reproducible: no atomics, no workspace.
+ * pos < 0 or pos + T > capacity: the call writes nothing at all (a guard, not a mode).
+ * Launch shape: per KV head and chunk of 8 of its group's T (n_heads / n_kv) (token, query head) rows, token-major, one
+ * thread-block cluster of S CTAs, which take the positions 0 .. pos+T-1 in blocks of 64 as sqllm_attn_decode's CTAs take 0 .. pos.
+ * S is sqllm_attn_verify_splits(n_heads, n_kv, n_tokens, SM count), lowered until every cluster of the launch is resident at once
+ * (the device's cudaOccupancyMaxActiveClusters for the kernel instance): sqllm_attn_verify_launch_splits.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_decode (dtype, head layout, head_dim,
+ * capacity, scale), n_tokens in [1, 16], n_kv ceil(n_tokens (n_heads / n_kv) / 8) <= 65535, every pointer non-null and 16-byte
+ * aligned.  No allocation, no host synchronisation: CUDA-graph capturable. */
+typedef struct sqllm_attn_verify_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions of the cache */
+    int n_tokens;             /* T, 1 .. 16 */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;
+    const int32_t *pos;
+    const float *rope_cos, *rope_sin;
+    void *k_cache, *v_cache;
+    void *out;
+} sqllm_attn_verify_args;
+
+int sqllm_attn_verify(const sqllm_attn_verify_args *args, void *stream);
+/* CTAs per cluster of sqllm_attn_verify on a device of sm_count SMs, with clusters = n_kv ceil(n_tokens (n_heads / n_kv) / 8):
+ * min(8, max(1, sm_count / clusters)); 0 for invalid arguments (a head layout that is not a positive multiple, n_tokens outside
+ * [1, 16], sm_count < 1, more than 65535 clusters).  Independent of pos; n_tokens 1 gives sqllm_attn_decode_splits.  An upper bound on
+ * the S a launch uses (below). */
+int sqllm_attn_verify_splits(int n_heads, int n_kv, int n_tokens, int sm_count);
+/* The S of a sqllm_attn_verify launch with these arguments on the current device: sqllm_attn_verify_splits lowered until all
+ * n_kv ceil(n_tokens (n_heads / n_kv) / 8) clusters of S CTAs of the kernel instance (dtype, head_dim, rows per CTA) can be resident at
+ * once; 1 when even S = 2 cannot.  0 for arguments sqllm_attn_verify rejects or when the device cannot be queried.  Independent of pos. */
+int sqllm_attn_verify_launch_splits(int dtype, int n_heads, int n_kv, int head_dim, int n_tokens);
 
 /* ---------------------------------------------------------------------------------------------
  * Token sampling: one token per row of logits, on the device (DESIGN.md section 3.20).  Row b (b < rows) holds x_i =

@@ -1,12 +1,18 @@
 // attn_decode.cu - decode attention with rotary and KV-cache append (attn_decode.cuh) behind sqllm_attn_decode (one sequence) and
 // sqllm_attn_decode_batch (several, each at its own position); causal attention of a chunk of new tokens with the same rotary and
-// append (attn_extend.cuh) behind sqllm_attn_extend.
+// append (attn_extend.cuh) behind sqllm_attn_extend; decode attention of up to 16 new tokens of one sequence at a device position
+// (attn_verify.cuh) behind sqllm_attn_verify.
 #include <limits.h>
 #include <math.h>
 #include <stdint.h>
+#include <string.h>
+
+#include <map>
+#include <tuple>
 
 #include "attn_decode.cuh"
 #include "attn_extend.cuh"
+#include "attn_verify.cuh"
 #include "host.h"
 
 using namespace sqllm;
@@ -156,6 +162,105 @@ int extend_launch(const sqllm_attn_extend_args *a, void *stream) {
     return SQLLM_OK;
 }
 
+template <typename T, int D>
+KernelSmem verify_kernel_of(int G) {
+    switch (G) {
+        case 1: return {attn::attn_verify_kernel<T, D, 1>, 0};
+        case 2: return {attn::attn_verify_kernel<T, D, 2>, 0};
+        case 4: return {attn::attn_verify_kernel<T, D, 4>, 0};
+        default: return {attn::attn_verify_kernel<T, D, 8>, 0};
+    }
+}
+
+// clusters per KV head of sqllm_attn_verify: chunks of GMAX of the T * g (token, query head) rows of its group
+int ver_chunks(int n_heads, int n_kv, int T) { return (T * (n_heads / n_kv) + attn::GMAX - 1) / attn::GMAX; }
+
+// the split rule of sqllm_attn_verify: as splits() for the n_kv * ver_chunks clusters, an upper bound on what a launch uses (below);
+// 0 for invalid arguments
+int ver_splits(int n_heads, int n_kv, int T, int sm_count) {
+    if (n_kv < 1 || n_heads < n_kv || n_heads % n_kv || sm_count < 1 || T < 1 || T > attn::VMAX) return 0;
+    const long long clusters = (long long)n_kv * ver_chunks(n_heads, n_kv, T);
+    if (clusters > MAX_BATCH) return 0;
+    return (int)std::max(1LL, std::min((long long)attn::MAX_CLUSTER, sm_count / clusters));
+}
+
+// the checks of a verify launch that need no pointers, in the order they run
+template <typename Args>
+int ver_check(const Args *a) {
+    if (int rc = check_dtype(a->dtype)) return rc;
+    if (int rc = check_heads(a)) return rc;
+    if (a->n_tokens < 1 || a->n_tokens > attn::VMAX) return fail(SQLLM_EINVAL, "n_tokens=%d must be in [1, %d]", a->n_tokens, attn::VMAX);
+    if ((long long)a->n_kv * ver_chunks(a->n_heads, a->n_kv, a->n_tokens) > MAX_BATCH)
+        return fail(SQLLM_EINVAL, "n_kv=%d x %d clusters per KV head exceeds %d", a->n_kv, ver_chunks(a->n_heads, a->n_kv, a->n_tokens),
+                    MAX_BATCH);
+    return SQLLM_OK;
+}
+
+// the kernel instance of a verify launch: G, the rows per CTA, is min(T g, GMAX) rounded up to a power of two
+KernelSmem ver_kernel(int n_heads, int n_kv, int T, int head_dim, int dtype) {
+    const int rows = std::min(T * (n_heads / n_kv), attn::GMAX);
+    const int G = rows <= 1 ? 1 : rows <= 2 ? 2 : rows <= 4 ? 4 : 8;
+    const bool bf = dtype == SQLLM_DT_BF16;
+    return head_dim == 128 ? (bf ? verify_kernel_of<__nv_bfloat16, 128>(G) : verify_kernel_of<__half, 128>(G))
+                           : (bf ? verify_kernel_of<__nv_bfloat16, 64>(G) : verify_kernel_of<__half, 64>(G));
+}
+
+// The CTAs per cluster a verify launch of `clusters` clusters of kernel `fn` uses on the current device: the rule's S, lowered until
+// every cluster is resident at once (cudaOccupancyMaxActiveClusters, asked once per device, kernel and S).  At 115 to 253 registers
+// per thread one or two CTAs of an instance fit an SM, and a cluster's CTAs must share a GPC, so the rule's S can leave clusters
+// for a second wave, which costs more than the longer position ranges of a smaller S.  S = 1 has no cluster constraint.
+int ver_launch_splits(const void *fn, int S, long long clusters, int *out) {
+    static std::map<std::tuple<int, const void *, int>, int> active;  // (device, kernel, S) -> max active clusters
+    std::lock_guard<std::recursive_mutex> lk(g_state_mu);
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return fail(SQLLM_ECUDA, "cudaGetDevice failed");
+    for (; S > 1; --S) {
+        auto it = active.find({dev, fn, S});
+        if (it == active.end()) {
+            cudaLaunchConfig_t cfg;
+            memset(&cfg, 0, sizeof(cfg));
+            cfg.gridDim = dim3(S, (unsigned)clusters);
+            cfg.blockDim = dim3(attn::THREADS);
+            cudaLaunchAttribute attr;
+            attr.id = cudaLaunchAttributeClusterDimension;
+            attr.val.clusterDim.x = S; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+            cfg.attrs = &attr;
+            cfg.numAttrs = 1;
+            int n = 0;
+            if (cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess)
+                return fail(SQLLM_ECUDA, "cudaOccupancyMaxActiveClusters failed: %s", cudaGetErrorString(cudaGetLastError()));
+            it = active.emplace(std::make_tuple(dev, fn, S), n).first;
+        }
+        if (it->second >= clusters) break;
+    }
+    *out = S;
+    return SQLLM_OK;
+}
+
+int verify_launch(const sqllm_attn_verify_args *a, void *stream) {
+    if (int rc = ver_check(a)) return rc;
+    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"},
+                             {a->k_cache, "k_cache"}, {a->v_cache, "v_cache"}, {a->out, "out"}}))
+        return rc;
+    const KernelSmem k = ver_kernel(a->n_heads, a->n_kv, a->n_tokens, a->head_dim, a->dtype);
+    int sm = 0;
+    int rc = dev_setup({}, &sm);
+    if (rc) return rc;
+    attn::VerParams p;
+    p.qkv = a->qkv; p.pos = a->pos; p.cos = a->rope_cos; p.sin = a->rope_sin;
+    p.k_cache = a->k_cache; p.v_cache = a->v_cache; p.out = a->out;
+    p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = a->n_heads / a->n_kv; p.chunks = ver_chunks(a->n_heads, a->n_kv, a->n_tokens);
+    p.capacity = a->capacity; p.T = a->n_tokens;
+    p.qscale = a->scale * attn::LOG2E;
+    int S = 0;
+    if ((rc = ver_launch_splits(k.fn, ver_splits(a->n_heads, a->n_kv, a->n_tokens, sm), (long long)a->n_kv * p.chunks, &S))) return rc;
+    const dim3 grid(S, a->n_kv * p.chunks);
+    const cudaError_t e = launch_ex(reinterpret_cast<void (*)(attn::VerParams)>(const_cast<void *>(k.fn)), grid, attn::THREADS, 0,
+                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_verify launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -181,6 +286,24 @@ int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int
 int sqllm_attn_extend(const sqllm_attn_extend_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
     return extend_launch(a, stream);
+}
+
+int sqllm_attn_verify_splits(int n_heads, int n_kv, int n_tokens, int sm_count) { return ver_splits(n_heads, n_kv, n_tokens, sm_count); }
+
+int sqllm_attn_verify_launch_splits(int dtype, int n_heads, int n_kv, int head_dim, int n_tokens) {
+    struct { int dtype, n_heads, n_kv, head_dim, capacity, n_tokens; float scale; } a = {dtype, n_heads, n_kv, head_dim, 1, n_tokens, 1.f};
+    if (ver_check(&a)) return 0;
+    int sm = 0, S = 0;
+    if (dev_setup({}, &sm)) return 0;
+    if (ver_launch_splits(ver_kernel(n_heads, n_kv, n_tokens, head_dim, dtype).fn, ver_splits(n_heads, n_kv, n_tokens, sm),
+                          (long long)n_kv * ver_chunks(n_heads, n_kv, n_tokens), &S))
+        return 0;
+    return S;
+}
+
+int sqllm_attn_verify(const sqllm_attn_verify_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return verify_launch(a, stream);
 }
 
 }  // extern "C"

@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `sample`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `attn_verify`, `sample`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -610,11 +610,11 @@ void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, 
                  "quant_cuda.fisher_accumulate");
 }
 
-// The argument checks attn_decode, attn_decode_batch and attn_extend share, in the order they run, each message prefixed with `fn`:
-// every tensor contiguous and 16-byte aligned, qkv's dtype, the head layout, k_cache [batch (lead = 1 only), n_kv, capacity, head_dim],
-// the batch, head_dim, capacity, scale, the cache and out dtypes and v_cache's shape; then own(batch, capacity, head_dim), the binding's
-// own shape checks; then the rope tables.  The device checks come last, so that a CPU caller sees the same rejections.  pos: null for
-// attn_extend.  -> the sqllm args with the fields the three share.
+// The argument checks attn_decode, attn_decode_batch, attn_extend and attn_verify share, in the order they run, each message prefixed
+// with `fn`: every tensor contiguous and 16-byte aligned, qkv's dtype, the head layout, k_cache [batch (lead = 1 only), n_kv, capacity,
+// head_dim], the batch, head_dim, capacity, scale, the cache and out dtypes and v_cache's shape; then own(batch, capacity, head_dim), the
+// binding's own shape checks; then the rope tables.  The device checks come last, so that a CPU caller sees the same rejections.  pos:
+// null for attn_extend.  -> the sqllm args with the fields the four share.
 template <typename Args, typename Own>
 Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::Tensor *pos, const torch::Tensor &rope_cos,
                const torch::Tensor &rope_sin, const torch::Tensor &k_cache, const torch::Tensor &v_cache, const torch::Tensor &out,
@@ -708,6 +708,26 @@ void attn_extend(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.start = (int)start; a.n_tokens = (int)qkv.size(0);
     check_status(sqllm_attn_extend(&a, cur_stream()), "quant_cuda.attn_extend");
+}
+
+// Decode attention of T <= 16 new tokens at positions *pos .. *pos+T-1 (sqllm_attn_verify): the append of their rotated k and v at those
+// slots, and per token attention over slots 0 .. its own position into out, on the current stream.
+void attn_verify(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
+                 torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_verify_args>("attn_verify", 0, qkv, &pos, rope_cos, rope_sin, k_cache, v_cache, out, n_heads, n_kv, scale,
+                                               [&](int64_t, int64_t, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_verify: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
+                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        const int64_t T = qkv.size(0);
+        TORCH_CHECK(T >= 1 && T <= 16, "attn_verify: qkv has ", T, " rows, want T in [1, 16]");
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_verify: out must be [T=", T, ", n_heads head_dim=",
+                    n_heads * d, "] (got ", out.sizes(), ")");
+        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.numel() == 1, "attn_verify: pos must be one int32 element");
+    });
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    a.n_tokens = (int)qkv.size(0);
+    a.pos = pos.data_ptr<int32_t>();
+    check_status(sqllm_attn_verify(&a, cur_stream()), "quant_cuda.attn_verify");
 }
 
 // One token per row of logits (sqllm_sample): greedy, or temperature / top-k / top-p filtering and a Gumbel-max draw keyed by seed[b]
@@ -906,6 +926,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               TORCH_CHECK(sm > 0, "attn_extend_splits: ", sqllm_last_error());
               return sqllm_attn_extend_splits(n_heads, n_kv, n_tokens, start, sm);
           }, "CTAs per cluster of attn_extend on the current device");
+    m.def("attn_verify", &attn_verify, "decode attention of T <= 16 new tokens at device positions pos .. pos+T-1: rotary, the append of k / "
+          "v at those slots, per token softmax(scale q K^T[0..p_t]) V[0..p_t] (qkv [T, ...], pos int32 [1], rope_cos, rope_sin, k_cache, "
+          "v_cache, out [T, ...], n_heads, n_kv, scale); pos < 0 or pos + T > capacity writes nothing; current stream",
+          py::arg("qkv"), py::arg("pos"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_cache"), py::arg("v_cache"), py::arg("out"),
+          py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_verify_splits", [](int n_heads, int n_kv, int n_tokens, int head_dim, at::ScalarType dtype) {
+              TORCH_CHECK(dtype == torch::kFloat16 || dtype == torch::kBFloat16, "attn_verify_splits: dtype must be torch.float16 or "
+                          "torch.bfloat16");
+              const int S = sqllm_attn_verify_launch_splits(dtype == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16, n_heads, n_kv,
+                                                            head_dim, n_tokens);
+              TORCH_CHECK(S > 0, "attn_verify_splits: ", sqllm_last_error());
+              return S;
+          }, "CTAs per cluster an attn_verify launch uses on the current device (independent of pos)", py::arg("n_heads"), py::arg("n_kv"),
+          py::arg("n_tokens"), py::arg("head_dim") = 128, py::arg("dtype") = torch::kFloat16);
     m.def("sample", &sample, "one token per row of logits [rows, vocab] (fp32, fp16 or bf16; unit last stride) into out int64 [rows]: greedy "
           "when temperature[b] <= 0, else temperature, top_k[b] (0: off) and top_p[b] (1: off) filtering and a Gumbel-max draw from "
           "Philox4x32-10 keyed by seed[b] (int64) at counter (i / 4, pos[b]); a row whose pos[b] (int32) < 0 writes nothing; current stream",

@@ -307,6 +307,29 @@ def _decoder_layout(model, max_len, who="SequenceDecoder"):
     return layers
 
 
+def _check_rows_fit(model, layers, who):
+    """ValueError naming the first projection of a multi-row step (stacked q/k/v, o, stacked gate/up, down and a quantized lm_head)
+    that does not fit the multi-row LUT-GEMV (QuantLinearLUT._rows_fits); the shapes are those of the stacked siblings, checked before
+    anything is stacked."""
+    import types
+
+    from .quant import FUSED_LIMITS, QuantLinearLUT
+    for i, layer in enumerate(layers):
+        at, mlp = layer.self_attn, layer.mlp
+        shapes = [("self_attn.q_proj|k_proj|v_proj", at.q_proj.infeatures,
+                   at.q_proj.outfeatures + at.k_proj.outfeatures + at.v_proj.outfeatures),
+                  ("self_attn.o_proj", at.o_proj.infeatures, at.o_proj.outfeatures),
+                  ("mlp.gate_proj|up_proj", mlp.gate_proj.infeatures, mlp.gate_proj.outfeatures + mlp.up_proj.outfeatures),
+                  ("mlp.down_proj", mlp.down_proj.infeatures, mlp.down_proj.outfeatures)]
+        if i == len(layers) - 1 and isinstance(model.lm_head, QuantLinearLUT):
+            shapes.append(("lm_head", model.lm_head.infeatures, model.lm_head.outfeatures))
+        for n, K, N in shapes:
+            if not QuantLinearLUT._rows_fits(types.SimpleNamespace(infeatures=K, outfeatures=N)):
+                where = n if n == "lm_head" else f"layers.{i}.{n}"
+                raise ValueError(f"{who}: {where} ({K} -> {N}) does not fit the multi-row LUT-GEMV (out_features a multiple "
+                                 f"of 4, in_features up to {FUSED_LIMITS['rows_max_in_features']})")
+
+
 def _stacked(module, names, who):
     """The stacked layer of the sibling group that holds exactly module.<names>, in that order."""
     ms = [getattr(module, n) for n in names]
@@ -420,6 +443,46 @@ def _eos_set(eos_token_id):
     return {int(e) for e in (eos_token_id if isinstance(eos_token_id, (list, tuple)) else [eos_token_id])}
 
 
+class PromptLookup:
+    """The built-in drafter of speculative generate: propose the tokens that followed the most recent earlier occurrence of the last
+    n tokens of the history, n = 3 first, then n = 2 (prompt-lookup decoding).  An n-gram -> the index after its last earlier
+    occurrence map is kept up to date as tokens arrive, so extend() and propose() cost O(n + k) on the host, not a scan."""
+
+    NGRAMS = (3, 2)
+
+    def __init__(self, tokens=(), k=1):
+        self.k = k
+        self.tokens = []
+        self._after = {}  # n-gram (tuple) -> index of the token after its most recent occurrence that has a token after it
+        self.extend(tokens)
+
+    def extend(self, tokens):
+        for t in tokens:
+            self.tokens.append(int(t))
+            i = len(self.tokens) - 1  # the n-grams ending at i - 1 now have a token after them
+            for n in self.NGRAMS:
+                if i >= n:
+                    self._after[tuple(self.tokens[i - n:i])] = i
+
+    def propose(self):
+        """Up to k ids (fewer when the occurrence is near the end of the history, none when no suffix n-gram occurred before)."""
+        for n in self.NGRAMS:
+            if len(self.tokens) > n:
+                j = self._after.get(tuple(self.tokens[-n:]))
+                if j is not None:
+                    return self.tokens[j:j + self.k]
+        return []
+
+
+def accept_length(drafts, draws):
+    """The speculative accept rule: the length n of the longest prefix with drafts[i] == draws[i] (draws[i]: the target's own token
+    for the position after drafts[i - 1]).  The tokens emitted are draws[0 .. n]."""
+    n = 0
+    while n < len(drafts) and drafts[n] == draws[n]:
+        n += 1
+    return n
+
+
 class _DecoderBase:
     """What SequenceDecoder and BatchDecoder share, for `slots` sequences (SequenceDecoder: one): the set-up, the graph capture, the
     prompts (prefill and extend of one slot), the replay with its full-cache check and the generate loop.  Slot b is row b of pos, tok,
@@ -463,18 +526,23 @@ class _DecoderBase:
         """From reset(): _step once on a side stream (SequenceDecoder's writes position 0, which a prompt overwrites; BatchDecoder's has
         every slot idle and writes nothing), then its capture as the graph, whose logits are self.logits; reset() again."""
         self.reset()
+        self.graph, self.logits = self._graph_of(self._step)
+        self.reset()
+
+    def _graph_of(self, fn):
+        """fn() once on a side stream, then its capture: (the graph, fn's result in the graph's memory)."""
         with torch.cuda.device(self.device), torch.no_grad():
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                self._step()
+                fn()
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph, stream=side):
-                self.logits = self._step()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=side):
+                out = fn()
             torch.cuda.synchronize()
-        self.reset()
+        return graph, out
 
     def _set_pos(self, slot, p):
         self.pos[slot] = p
@@ -620,13 +688,33 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
     synchronisation.  A step() user samples the same way: quant_cuda.sample(dec.logits.view(1, -1), dec.pos, dec.temperature, dec.top_k,
     dec.top_p, dec.seed, dec.tok) after step() draws the token of position dec.position (fill the four parameter buffers first).
 
+    Speculation (speculate=K in 1..15) adds a second graph, the verify step: T = K + 1 tokens at positions pos .. pos+K in one pass -
+    the embedding gather of the device ids, per layer the stacked projections on [T, hidden] (QuantLinearLUT.forward: the multi-row
+    kernel, so every projection must fit it) with quant_cuda.attn_verify on the decoder's cache, the final norm, lm_head and the argmax
+    of every row.  It reads pos from the device and does not advance it.  generate() then drafts up to K tokens per iteration (the
+    built-in PromptLookup, or a `draft` callable), verifies the pending token and the drafts in one replay and keeps the drafts up to the
+    first whose target token differs.  Each emitted token is the draw plain generate makes from the same logits at the same position
+    (greedy: the argmax; sampled: quant_cuda.sample keyed by the seed and the position), so speculation changes how many positions a
+    pass computes, never which token a position gets beyond the rounding of its logits.
+
     The model itself is changed only by the sibling stacking of fusion.fuse_siblings, which keeps its outputs.  Everything the decoder
     computes carries no gradient."""
 
     CACHE_FULL = "SequenceDecoder: the cache is full (max_len={max_len}); reset() or prefill() first"
 
-    def __init__(self, model, max_len):
+    def __init__(self, model, max_len, speculate=0):
+        """speculate: K, the drafted tokens one verify step checks (0: no speculation, no verify graph)."""
+        from .quant import QuantLinearLUT
         layers = _decoder_layout(model, max_len)
+        if not isinstance(speculate, int) or isinstance(speculate, bool) or not 0 <= speculate <= 15:
+            raise ValueError(f"SequenceDecoder: speculate must be an int in 0..15 (got {speculate!r})")
+        if speculate:
+            _check_rows_fit(model, layers, "SequenceDecoder")
+            dtype = model.model.embed_tokens.weight.dtype
+            rows_max = QuantLinearLUT.ROWS_MAX if dtype == torch.float16 else QuantLinearLUT.BF16_ROWS_MAX
+            if speculate + 1 > rows_max:
+                raise ValueError(f"SequenceDecoder: speculate={speculate} needs {speculate + 1} rows, the multi-row LUT-GEMV takes up to "
+                                 f"{rows_max} for a {dtype} model")
         super().__init__(model, max_len, layers, 1, "SequenceDecoder")
         # the one slot's views: caches [n_layers, n_kv, max_len, head_dim], attention output [n_heads * head_dim]
         self.k_cache, self.v_cache, self.attn_out = self._k[:, 0], self._v[:, 0], self.attn_out[0]
@@ -634,6 +722,36 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         with torch.cuda.device(self.device), torch.no_grad():
             self._build()
         self._capture()
+        self.speculate, self.spec_stats = speculate, None
+        if speculate:
+            T, dev = speculate + 1, self.device
+            with torch.cuda.device(dev), torch.no_grad():
+                self.vtok = torch.zeros(T, dtype=torch.int64, device=dev)     # the verify step's ids: pending token, drafts, padding
+                self.vdraw = torch.zeros(T, dtype=torch.int64, device=dev)    # row t's token: the argmax, or quant_cuda.sample's draw
+                self.vpos = torch.zeros(T, dtype=torch.int32, device=dev)     # row t's sampling position pos + t + 1
+                self._vstep = torch.arange(1, T + 1, dtype=torch.int32, device=dev)
+                self._vattn = torch.zeros(T, self.n_heads * self.head_dim, dtype=self.dtype, device=dev)
+                # quant_cuda.sample's parameters for the T rows (generate copies slot 0's into them)
+                self._vsampling = (torch.zeros(T, dtype=torch.float32, device=dev), torch.zeros(T, dtype=torch.int32, device=dev),
+                                   torch.ones(T, dtype=torch.float32, device=dev), torch.zeros(T, dtype=torch.int64, device=dev))
+            self.reset()
+            self.vgraph, self.vlogits = self._graph_of(self._verify_step)
+            self.reset()
+
+    def _verify_step(self):
+        """The verify step on the current stream: what the verify graph holds.  pos is read, not advanced."""
+        m = self.model.model
+        h = torch.index_select(m.embed_tokens.weight, 0, self.vtok)
+        for i, layer in enumerate(m.layers):
+            def attend(qkv, i=i):
+                self._qc.attn_verify(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i], self._vattn,
+                                     self.n_heads, self.n_kv, self.scale)
+                return self._vattn
+            h = self._layer(i, layer, h, attend)
+        logits = self.model.lm_head(m.norm(h))
+        self.vdraw.copy_(logits.argmax(dim=-1))
+        torch.add(self.pos, self._vstep, out=self.vpos)
+        return logits
 
     def _build(self):
         """The DecodeSequences of the plan, each reading its inputs in place: the attention output buffer, the previous sequence's d."""
@@ -719,23 +837,125 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         self._replay()
         return self.logits
 
-    def generate(self, input_ids, max_new_tokens, eos_token_id=None, *, temperature=0.0, top_k=0, top_p=1.0, seed=0):
+    def verify(self, token_ids):
+        """Feed the speculate + 1 token ids (ints or a device tensor) at positions p .. p + speculate in one verify replay; returns
+        their next-token logits [speculate + 1, vocab], a static buffer that the next verify overwrites, and advances the position by
+        speculate + 1 (rewind() takes it back to keep a prefix).  Raises ValueError, with nothing written, on a decoder without
+        speculation, for a wrong count or non-integer ids, or when the tokens do not fit in max_len."""
+        who = "SequenceDecoder.verify"
+        if not self.speculate:
+            raise ValueError(f"{who}: the decoder was built with speculate=0; pass speculate=K to SequenceDecoder")
+        T = self.speculate + 1
+        t = torch.as_tensor(token_ids)
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise ValueError(f"{who}: token_ids must hold integer token ids (got {t.dtype})")
+        if t.numel() != T:
+            raise ValueError(f"{who}: {t.numel()} token ids, the verify step takes speculate + 1 = {T}")
+        p = self._pos[0]
+        if p + T > self.max_len:
+            raise ValueError(f"{who}: {T} tokens at position {p} need {p + T} cache positions, max_len is {self.max_len}")
+        self.vtok.copy_(t.reshape(T))
+        self.vgraph.replay()
+        self._set_pos(0, p + T)
+        return self.vlogits
+
+    def rewind(self, position):
+        """Set the position back to `position` (0 .. the current one): the cache slots from there on are never read again, and the next
+        step or verify writes there.  Raises ValueError otherwise."""
+        if not isinstance(position, int) or isinstance(position, bool) or not 0 <= position <= self._pos[0]:
+            raise ValueError(f"SequenceDecoder.rewind: position must be an int in 0..{self._pos[0]} (got {position!r})")
+        self._set_pos(0, position)
+
+    def generate(self, input_ids, max_new_tokens, eos_token_id=None, *, temperature=0.0, top_k=0, top_p=1.0, seed=0, draft=None):
         """input_ids [1, T] followed by up to max_new_tokens tokens, ending after the first EOS (eos_token_id: an int or a list) if one
         comes.  The prompt and max_new_tokens - 1 steps must fit in max_len.  Greedy by default; temperature > 0 samples each token with
         quant_cuda.sample: softmax(logits / temperature), restricted to the top_k largest (0: all) and then to the smallest set of mass
         top_p (1: all), drawn with the random stream of `seed` at the token's position, so a call is reproducible.  Each keyword may also
-        be a one-element list.  Bad values raise ValueError before anything runs (see _sampling)."""
-        sampling = _sampling("SequenceDecoder.generate", 1, temperature, top_k, top_p, seed)
+        be a one-element list.  Bad values raise ValueError before anything runs (see _sampling).
+
+        On a decoder built with speculate=K > 0 generation speculates: `draft` is a callable (the tokens so far, prompt included, as a
+        list it must not change) -> a list of proposed next ids, of which the first K are used; None: the built-in PromptLookup.  A
+        proposal that is not a list of ints in [0, vocab) raises ValueError.  `draft` on a decoder without speculation raises ValueError.
+        spec_stats then holds the call's verify, drafted and accepted counts."""
+        who = "SequenceDecoder.generate"
+        sampling = _sampling(who, 1, temperature, top_k, top_p, seed)
+        if draft is not None and not self.speculate:
+            raise ValueError(f"{who}: draft needs a decoder built with speculate > 0")
+        if draft is not None and not callable(draft):
+            raise ValueError(f"{who}: draft must be a callable (tokens -> list of ids) or None (got {type(draft).__name__})")
         ids = torch.as_tensor(input_ids).reshape(1, -1)
         if max_new_tokens < 1:
             return ids
         if ids.shape[1] + max_new_tokens - 1 > self.max_len:
             raise ValueError(f"SequenceDecoder.generate: {ids.shape[1]} prompt tokens and {max_new_tokens} new ones need "
                              f"{ids.shape[1] + max_new_tokens - 1} cache positions, max_len is {self.max_len}")
-        out, (n,) = self._generate("SequenceDecoder.prefill", [ids], max_new_tokens, _eos_set(eos_token_id), sampling)
+        if self.speculate:
+            new = self._speculate("SequenceDecoder.prefill", ids, max_new_tokens, _eos_set(eos_token_id), sampling, draft)
+            out = torch.tensor([new], dtype=torch.int64, device=self.device)
+            n = len(new)
+        else:
+            out, (n,) = self._generate("SequenceDecoder.prefill", [ids], max_new_tokens, _eos_set(eos_token_id), sampling)
         for seq in self.sequences:
             seq.check()
         return torch.cat([ids.to(self.device), out[:, :n]], dim=1)
+
+    def _speculate(self, who, ids, max_new_tokens, eos, sampling, draft):
+        """generate's loop with speculation; -> the new tokens (a list).  One host synchronisation per iteration: the emitted tokens."""
+        K, vocab = self.speculate, self.vlogits.shape[-1]
+        if sampling:
+            self._set_sampling(sampling)
+            for buf, vals in zip(self._vsampling, sampling):
+                buf.fill_(vals[0])
+            self._sample(self._prefill(who, 0, ids).view(1, -1))
+            c = int(self.tok)
+        else:
+            c = int(self._prefill(who, 0, ids).argmax())
+        history = [int(t) for t in ids.reshape(-1).tolist()] + [c]
+        lookup = PromptLookup(history, K) if draft is None else None
+        new = [c]
+        self.spec_stats = {"verifies": 0, "drafted": 0, "accepted": 0}
+        while len(new) < max_new_tokens and c not in eos:
+            p = self._pos[0]
+            drafts = lookup.propose() if draft is None else self._check_draft(draft(history), vocab)[:K]
+            if not drafts or p + K >= self.max_len:  # one ordinary step, the position advanced by its graph
+                self.step(c)
+                if sampling:
+                    self._sample(self.logits.view(1, -1))
+                emitted = [int(self.tok)]
+            else:
+                m = len(drafts)
+                self.vtok.copy_(torch.tensor([c] + drafts + [c] * (K - m), dtype=torch.int64))
+                self.vgraph.replay()
+                if sampling:
+                    self._qc.sample(self.vlogits, self.vpos, *self._vsampling, self.vdraw)
+                y = self.vdraw.tolist()
+                n = accept_length(drafts, y)
+                emitted = y[:n + 1]
+                st = self.spec_stats
+                st["verifies"], st["drafted"], st["accepted"] = st["verifies"] + 1, st["drafted"] + m, st["accepted"] + n
+                for j, t in enumerate(emitted):  # EOS and max_new_tokens cut an accepted run
+                    if t in eos or len(new) + j + 1 == max_new_tokens:
+                        emitted = emitted[:j + 1]
+                        break
+                self._set_pos(0, p + len(emitted))  # the fed tokens c, d_1 .. d_j are kept; the rest of the slots is never read
+            new += emitted
+            history += emitted
+            if lookup is not None:
+                lookup.extend(emitted)
+            c = new[-1]
+        return new
+
+    @staticmethod
+    def _check_draft(d, vocab):
+        """A drafter's proposal as a list of ints in [0, vocab); ValueError otherwise."""
+        if isinstance(d, torch.Tensor):
+            d = d.tolist()
+        if not isinstance(d, (list, tuple)):
+            raise ValueError(f"SequenceDecoder.generate: draft must return a list of token ids (got {type(d).__name__})")
+        for t in d:
+            if not isinstance(t, numbers.Integral) or isinstance(t, bool) or not 0 <= t < vocab:
+                raise ValueError(f"SequenceDecoder.generate: draft returned {t!r}, not a token id in [0, {vocab})")
+        return [int(t) for t in d]
 
 
 class BatchDecoder(_DecoderBase):
@@ -769,29 +989,14 @@ class BatchDecoder(_DecoderBase):
     CACHE_FULL = "BatchDecoder: the cache of slot(s) {slots} is full (max_len={max_len}); release() or prefill() them first"
 
     def __init__(self, model, max_len, batch):
-        import types
-
-        from .quant import FUSED_LIMITS, QuantLinearLUT
+        from .quant import QuantLinearLUT
         layers = _decoder_layout(model, max_len, "BatchDecoder")
         dtype = model.model.embed_tokens.weight.dtype
         rows_max = QuantLinearLUT.ROWS_MAX if dtype == torch.float16 else QuantLinearLUT.BF16_ROWS_MAX
         if not isinstance(batch, int) or not 2 <= batch <= rows_max:
             hint = "; decode one sequence with SequenceDecoder" if batch == 1 else ""
             raise ValueError(f"BatchDecoder: batch must be an int in 2..{rows_max} for a {dtype} model (got {batch!r}){hint}")
-        for i, layer in enumerate(layers):  # the shapes the step runs, stacked siblings included, before anything is stacked
-            at, mlp = layer.self_attn, layer.mlp
-            shapes = [("self_attn.q_proj|k_proj|v_proj", at.q_proj.infeatures,
-                       at.q_proj.outfeatures + at.k_proj.outfeatures + at.v_proj.outfeatures),
-                      ("self_attn.o_proj", at.o_proj.infeatures, at.o_proj.outfeatures),
-                      ("mlp.gate_proj|up_proj", mlp.gate_proj.infeatures, mlp.gate_proj.outfeatures + mlp.up_proj.outfeatures),
-                      ("mlp.down_proj", mlp.down_proj.infeatures, mlp.down_proj.outfeatures)]
-            if i == len(layers) - 1 and isinstance(model.lm_head, QuantLinearLUT):
-                shapes.append(("lm_head", model.lm_head.infeatures, model.lm_head.outfeatures))
-            for n, K, N in shapes:
-                if not QuantLinearLUT._rows_fits(types.SimpleNamespace(infeatures=K, outfeatures=N)):
-                    where = n if n == "lm_head" else f"layers.{i}.{n}"
-                    raise ValueError(f"BatchDecoder: {where} ({K} -> {N}) does not fit the multi-row LUT-GEMV (out_features a multiple "
-                                     f"of 4, in_features up to {FUSED_LIMITS['rows_max_in_features']})")
+        _check_rows_fit(model, layers, "BatchDecoder")
         super().__init__(model, max_len, layers, batch, "BatchDecoder")
         self.batch = batch
         self.k_cache, self.v_cache = self._k, self._v
