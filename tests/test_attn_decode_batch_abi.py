@@ -73,7 +73,9 @@ def test_rejects_null_args():
                                               (32, 8, 4, 132, 4), (32, 8, 16, 132, 1), (8, 2, 5, 132, 8), (8, 2, 63, 132, 1),
                                               (4, 4, 8, 132, 4), (64, 8, 2, 132, 8), (128, 2, 1, 132, 8), (128, 2, 4, 132, 2), (128, 2, 8, 132, 1),
                                               (32, 32, 65535, 132, 1), (32, 32, 0, 132, 0), (32, 32, 65536, 132, 0),
-                                              (30, 8, 2, 132, 0), (8, 0, 2, 132, 0), (8, 2, 2, 0, 0)])
+                                              (30, 8, 2, 132, 0), (8, 0, 2, 132, 0), (8, 2, 2, 0, 0),
+                                              (71, 1, 5, 132, 2),   # ceil(71 / 8) = 9 clusters per sequence, 45 in all: 132 / 45 = 2
+                                              (48, 4, 4, 132, 4)])  # B 4 x n_kv 4 x ceil(12 / 8) = 32 clusters: 132 / 32 = 4
 def test_splits(nh, nkv, B, sm, want):
     assert load_lib().sqllm_attn_decode_batch_splits(nh, nkv, B, sm) == want
 

@@ -5,8 +5,10 @@ position in its own cache block, checked row by row with the single-row tests' c
   * idle rows (pos -1 and pos = capacity) between active ones leave their out row and their whole cache block bitwise untouched;
   * row b bitwise equal to quant_cuda.attn_decode on row b's slices wherever the two split counts agree;
   * repeated runs bitwise equal; a CUDA graph that advances the active rows' positions on the device bitwise equal to eager calls.
-Shapes: (n_heads, n_kv) in {(32, 32), (32, 8), (8, 2), (4, 4)}, head_dim 64 and 128, fp16 and bf16, B in {2, 5, 8, 63}; the rows
-take different positions from {0, 1, 63, 64, 65, 64S - 1, 64S, capacity - 1} (S: the batch's split count)."""
+Shapes: (n_heads, n_kv) in test_attn_decode_gpu.HEADS, head_dim 64 and 128, fp16 and bf16; B in {2, 5, 8, 63} for the layouts
+(32, 32), (32, 8), (8, 2) and (4, 4), and B in {5, 63} for the others (g = 2, 3, 5, 6, 7, 8, 12, 16 and 71), which bounds the module's
+time (on 132 SMs, B = 5 splits every one of them over 2 to 8 CTAs and B = 63 over one); the rows take different positions from
+{0, 1, 63, 64, 65, 64S - 1, 64S, capacity - 1} (S: the batch's split count)."""
 import pytest
 import torch
 
@@ -16,6 +18,9 @@ pytestmark = pytest.mark.gpu
 
 CAP = 1100  # not a multiple of 64: the last block of a full cache is partial
 BATCHES = [2, 5, 8, 63]
+# (nh, nkv, d, dtype, B): every B for the first four layouts, B = 5 and 63 for the others
+ROWS_GRID = [(nh, nkv, d, dt, B) for i, (nh, nkv) in enumerate(HEADS) for d in (64, 128) for dt in DTYPES
+             for B in (BATCHES if i < 4 else [5, 63])]
 
 
 def _quant_cuda():
@@ -59,10 +64,7 @@ def record(request):
     return lambda name, value: request.node.user_properties.append((name, value))
 
 
-@pytest.mark.parametrize("B", BATCHES)
-@pytest.mark.parametrize("dtype", list(DTYPES))
-@pytest.mark.parametrize("d", [64, 128])
-@pytest.mark.parametrize("nh,nkv", HEADS, ids=[f"{a}x{b}" for a, b in HEADS])
+@pytest.mark.parametrize("nh,nkv,d,dtype,B", ROWS_GRID, ids=[f"{a}x{b}-{d}-{dt}-{B}" for a, b, d, dt, B in ROWS_GRID])
 def test_rows_against_fp64(record, nh, nkv, d, dtype, B):
     bc = BatchCase(nh, nkv, d, DTYPES[dtype], ragged(nh, nkv, B, shift=B), seed=B)
     before = [(r.kbuf.clone(), r.vbuf.clone()) for r in bc.rows]

@@ -4,9 +4,12 @@ Per call, with the cache slots past `pos` filled with NaN (so any read of them w
   * the stored k within one rounding to the dtype (plus the fp32 rotary's terms) of the fp64 rotary of qkv's k;
   * the stored v bit-exact, every other cache slot bitwise unchanged;
   * the output within the bound of `out_bound`, reported as its ratio (<= 1 passes) like util.bound_ratio.
-Shapes: (n_heads, n_kv) in {(32, 32), (32, 8), (8, 2), (4, 4)}, head_dim 64 and 128, fp16 and bf16, pos at 0, 1, both sides of
-the first two split boundaries, 4095 and capacity - 1; one dominant score (+-1e4) and all-equal scores; repeated runs bitwise equal;
-N steps replayed in a CUDA graph that advances pos on the device bitwise equal to N eager calls; pos = capacity writes nothing."""
+Shapes: (n_heads, n_kv) in HEADS, with query heads per KV head g in {1, 2, 3, 4, 5, 6, 7, 8, 12, 16, 71} (every instance G in
+{1, 2, 4, 8}, padding rows for g = 3, 5, 6, 7, a group over several clusters for g > 8), head_dim 64 and 128, fp16 and bf16, pos at 0,
+1, both sides of the first two split boundaries, 4095 and capacity - 1; one dominant score (+-1e4) and all-equal scores (also at g = 7
+and at g = 71, whose group 0 spans nine clusters); repeated runs bitwise equal; N steps replayed in a CUDA graph that advances pos on
+the device bitwise equal to N eager calls (also at g = 12, where only the first cluster of a group appends); pos = capacity writes
+nothing."""
 import math
 
 import numpy as np
@@ -18,7 +21,10 @@ from util import OUT_ROUNDING
 pytestmark = pytest.mark.gpu
 
 CAP = 4160
-HEADS = [(32, 32), (32, 8), (8, 2), (4, 4)]
+# (n_heads, n_kv) of every kernel test of the four attention kernels: g = n_heads / n_kv at 1 and 4 (G = 1, 4), 2 (G = 2), 3, 5, 6
+# and 7 (padding rows in G = 4 or 8, and one token's heads split across verify chunks of 8 rows and extend tiles of 64), 8 (G = 8 with
+# U = 2), 12 and 16 (a group over two clusters, the last one partial at 12) and the MQA 71 x 1 (nine clusters, the last of 7 heads)
+HEADS = [(32, 32), (32, 8), (8, 2), (4, 4), (16, 8), (24, 8), (40, 8), (12, 2), (28, 4), (64, 8), (48, 4), (32, 2), (71, 1)]
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16}
 U = 2.0 ** -24
 E_SCORE = 2.0 ** -19  # fp32 terms of a score, relative to scale * sum_d |q-rotary terms| |k_d|: the rotary, the 8-term FMA chain, the
@@ -153,7 +159,7 @@ def test_against_fp64(record, nh, nkv, d, dtype):
 
 @pytest.mark.parametrize("mode", ["dominant", "equal"])
 @pytest.mark.parametrize("dtype", list(DTYPES))
-@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64), (28, 4, 128), (71, 1, 64)])
 def test_extreme_scores(record, nh, nkv, d, dtype, mode):
     worst = 0.0
     for pos in (2, 700, 4095):
@@ -182,7 +188,7 @@ def test_bitwise_reproducible(dtype):
         assert torch.equal(k.view(torch.int16), outs[0][1].view(torch.int16))
 
 
-@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64), (48, 4, 128)])
 def test_graph_replay_advances_pos_on_device(nh, nkv, d):
     """N steps of one captured call + pos += 1, each with new qkv, bitwise equal to N eager calls at the same positions."""
     N, p0 = 12, 250

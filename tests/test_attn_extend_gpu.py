@@ -4,10 +4,11 @@ Per call, with the cache slots before `start` random and the slots from `start` 
   * the stored cache bitwise equal to what T successive attn_decode calls at start .. start+T-1 leave (k' and v at the chunk's slots,
     every other slot and the guard band after the cache unchanged: the NaN slots past start + T stay NaN);
   * every output element within the bound of `out_bound`, reported as its ratio (<= 1 passes).
-Shapes: (n_heads, n_kv) in {(32, 32), (32, 8), (8, 2), (4, 4)}, head_dim 64 and 128, fp16 and bf16, (start, T) from one token at 0 to
-2048 tokens at 0, across the 64-key blocks and with a few tokens on a long history; scores at +-1e4 and all-equal scores; two calls
-bitwise equal; out row t independent of the qkv rows after t; a CUDA-graph replay bitwise equal to the eager call; T = 1 against
-attn_decode.
+Shapes: (n_heads, n_kv) in test_attn_decode_gpu.HEADS (g = n_heads / n_kv from 1 to 16 and 71: where g does not divide 64,
+a 64-row query tile of a group can start inside a token), head_dim 64 and 128, fp16 and bf16, (start, T) from one token at 0 to 2048 tokens
+at 0, across the 64-key blocks and with a few tokens on a long history; scores at +-1e4 and all-equal scores (also at g = 7 and 71);
+two calls bitwise equal; out row t independent of the qkv rows after t (also at g = 7, with token t split by a tile edge); a
+CUDA-graph replay bitwise equal to the eager call; T = 1 against attn_decode.
 
 The bound.  For token t at p = start + t and head h, with z_j = scale q'.K_j (natural-log units), A_j = scale sum_d |q'-terms| |K_jd|
 (the rotary's terms summed in magnitude, as in test_attn_decode_gpu) and the fp64 softmax weights w_j:
@@ -29,12 +30,12 @@ import numpy as np
 import pytest
 import torch
 
+from test_attn_decode_gpu import HEADS
 from util import OUT_ROUNDING
 
 pytestmark = pytest.mark.gpu
 
 CAP = 4160
-HEADS = [(32, 32), (32, 8), (8, 2), (4, 4)]
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16}
 CHUNKS = [(0, 1), (0, 17), (0, 64), (0, 65), (63, 2), (64, 64), (100, 300), (4000, 8), (0, 2048), (CAP - 5, 5)]
 U_SPLIT = {torch.float16: 2.0 ** -22, torch.bfloat16: 2.0 ** -16}
@@ -190,7 +191,7 @@ def test_against_fp64(record, nh, nkv, d, dtype):
 
 @pytest.mark.parametrize("mode", ["dominant", "equal"])
 @pytest.mark.parametrize("dtype", list(DTYPES))
-@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64), (28, 4, 128), (71, 1, 64)])
 def test_extreme_scores(record, nh, nkv, d, dtype, mode):
     worst = 0.0
     for start, T in ((5, 5), (700, 64), (4000, 100)):
@@ -221,9 +222,11 @@ def test_bitwise_reproducible(dtype, start, T):
         assert torch.equal(k.view(torch.int16), outs[0][1].view(torch.int16))
 
 
-@pytest.mark.parametrize("nh,nkv,d,start,T", [(32, 8, 128, 100, 300), (8, 2, 64, 4000, 8), (32, 32, 128, 0, 130)])
+@pytest.mark.parametrize("nh,nkv,d,start,T", [(32, 8, 128, 100, 300), (8, 2, 64, 4000, 8), (32, 32, 128, 0, 130),
+                                               (28, 4, 128, 100, 55)])
 def test_causal(nh, nkv, d, start, T):
-    """Changing the qkv rows after t leaves out rows 0..t bitwise unchanged."""
+    """Changing the qkv rows after t leaves out rows 0..t bitwise unchanged.  At g = 7 and T = 55, t = 27: token 27's rows 189 .. 195
+    straddle the tile edge at 192, so tile 3 holds heads of token 27 and of every token after it."""
     case = Case(nh, nkv, d, torch.float16, start, T, seed=3)
     case.run()
     first = case.out.clone()

@@ -72,6 +72,8 @@ def test_rejects_null_args():
     (8, 2, 1, 132, 8), (4, 4, 16, 132, 8), (4, 4, 2, 132, 8),
     (64, 8, 16, 132, 1),     # 8 x 16 clusters
     (32, 32, 1, 16, 1),
+    (71, 1, 16, 132, 1),     # 1 x ceil(16 x 71 / 8) = 142 clusters: 132 / 142 = 0, at least 1
+    (28, 4, 3, 132, 8),      # 4 x ceil(3 x 7 / 8) = 12 clusters: 132 / 12 = 11, at most 8
     (30, 8, 4, 132, 0), (8, 0, 4, 132, 0), (8, 2, 4, 0, 0), (8, 2, 0, 132, 0), (8, 2, 17, 132, 0), (65536, 65536, 1, 132, 0),
 ])
 def test_splits(nh, nkv, T, sm, want):

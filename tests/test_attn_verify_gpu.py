@@ -5,10 +5,12 @@ Per call, with the cache slots from pos on filled with NaN (so any read of a slo
   * k_cache and v_cache (and a guard band after them) bitwise equal to what T successive attn_decode calls at pos .. pos+T-1 leave:
     the same k' bits, v unchanged, every other slot untouched, NaN past pos + T still NaN;
   * every output element within the bound of test_attn_decode_gpu.out_bound (DESIGN section 3.17) with its own token's position p_t.
-Shapes: (n_heads, n_kv) in {(32, 32), (32, 8), (8, 2), (4, 4)}, head_dim 64 and 128, fp16 and bf16, T in {1, 2, 5, 8, 16}, pos at 0,
-1, 63 - T/2, 64, 64 S - 1, 64 S (S: the split count), 4095 - T and capacity - T.  Besides: one dominant score (+-1e4) and all-equal
-scores; row t unchanged when the qkv rows after t change, also to inf or NaN; the launched split count within 1 .. 8; reruns and a
-graph replay that advances the device pos bitwise equal to eager calls; pos < 0 and pos + T > capacity write nothing."""
+Shapes: (n_heads, n_kv) in test_attn_decode_gpu.HEADS (g = n_heads / n_kv from 1 to 16 and 71: where g does not divide 8, a chunk of
+8 rows can start inside a token, and padding rows fill the last chunk; 71 x 1 at T = 16 is 142 clusters, so S = 1), head_dim 64 and
+128, fp16 and bf16, T in {1, 2, 5, 8, 16}, pos at 0, 1, 63 - T/2, 64, 64 S - 1, 64 S (S: the split count), 4095 - T and
+capacity - T.  Besides: one dominant score (+-1e4) and all-equal scores (also at g = 7 and 71); row t unchanged when the qkv rows
+after t change, also to inf or NaN (also at g = 7, with token t split by a chunk edge); the launched split count within 1 .. 8; reruns
+and a graph replay that advances the device pos bitwise equal to eager calls; pos < 0 and pos + T > capacity write nothing."""
 import pytest
 import torch
 
@@ -133,7 +135,7 @@ def test_against_fp64_and_decode(record, nh, nkv, d, dtype):
 
 @pytest.mark.parametrize("mode", ["dominant", "equal"])
 @pytest.mark.parametrize("dtype", list(DTYPES))
-@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 8, 128), (8, 2, 64), (28, 4, 128), (71, 1, 64)])
 def test_extreme_scores(record, nh, nkv, d, dtype, mode):
     worst = 0.0
     for pos in (2, 700, 4090):
@@ -148,8 +150,9 @@ def test_extreme_scores(record, nh, nkv, d, dtype, mode):
     record("bound_ratio", worst)
 
 
-@pytest.mark.parametrize("nh,nkv,d", [(32, 32, 128), (32, 8, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 32, 128), (32, 8, 128), (8, 2, 64), (28, 4, 128)])
 def test_row_ignores_later_rows(nh, nkv, d):
+    """At g = 7, token t = 2's rows 14 .. 20 straddle the chunk edge at 16, and chunk 2 holds rows of token 3 as well."""
     T, t, pos = 8, 2, 777
     a = VCase(nh, nkv, d, torch.float16, pos, T, seed=4)
     b = VCase(nh, nkv, d, torch.float16, pos, T, seed=4)
@@ -162,9 +165,10 @@ def test_row_ignores_later_rows(nh, nkv, d):
 
 
 @pytest.mark.parametrize("bad", ["nan", "inf"])
-@pytest.mark.parametrize("nh,nkv,d", [(32, 32, 128), (8, 2, 64)])
+@pytest.mark.parametrize("nh,nkv,d", [(32, 32, 128), (8, 2, 64), (28, 4, 128)])
 def test_row_ignores_non_finite_later_rows(nh, nkv, d, bad):
-    """A later token's k and v that overflowed (inf) or are NaN leave the earlier rows' outputs bitwise as they were."""
+    """A later token's k and v that overflowed (inf) or are NaN leave the earlier rows' outputs bitwise as they were.  At g = 7, token
+    t = 3's rows 21 .. 27 straddle the chunk edge at 24, and chunk 3 holds rows of token 4 as well."""
     T, t, pos = 8, 3, 300
     a = VCase(nh, nkv, d, torch.float16, pos, T, seed=6)
     b = VCase(nh, nkv, d, torch.float16, pos, T, seed=6)

@@ -2,7 +2,8 @@
 test_decoder_gpu.py (same models, same banks of oracle layers, same criteria, applied per row).
 
 Kinds A4 (Llama, 8 heads / 2 KV heads), C (Qwen2 with q/k/v bias and a quantized lm_head) and H64 (head_dim 64), in fp16 and bf16 at
-batch 2 and 5, and the 7B-shaped layer B at batch 5; the rows hold prompts of different lengths (1, 9, 17, 5, 12 tokens):
+batch 2 and 5, the 7B-shaped layer B and G7 (7 query heads per KV head) at batch 5, and MQA (16 heads on one KV head) at batch 2;
+the rows hold prompts of different lengths (1, 9, 17, 5, 12 tokens):
   * teacher-forced decode for 40 steps: every row's logits at most twice as far (max norm) from the twin's as a dense model of the same
     dtype decoding the same tokens with HF's cache;
   * greedy generate matches the twin's greedy tokens, row by row, up to the twin's first near-tie;
@@ -24,7 +25,8 @@ pytestmark = pytest.mark.gpu
 MAX_LEN = 64
 STEPS = 40
 LENS = [1, 9, 17, 5, 12]
-CASES = [(k, dt, B) for k in ("A4", "C", "H64") for dt in DTYPES for B in (2, 5)] + [("B", dt, 5) for dt in DTYPES]
+CASES = ([(k, dt, B) for k in ("A4", "C", "H64") for dt in DTYPES for B in (2, 5)] + [("B", dt, 5) for dt in DTYPES]
+         + [(k, dt, B) for k, B in (("G7", 5), ("MQA", 2)) for dt in DTYPES])
 
 
 @pytest.fixture

@@ -2,7 +2,8 @@
 (quant_cuda.attn_extend between the projections), against the fp64 twin of test_decoder_gpu.py.
 
 Models, banks and the criterion are those of test_decoder_gpu.py: kinds A4 / A3 (Llama at 4 / 3 bits), C (Qwen2 with q/k/v bias and a
-quantized lm_head), M (Mistral), H64 (head_dim 64) and B (one 7B-shaped layer), each in fp16 and bf16.  Every logit row the decoder
+quantized lm_head), M (Mistral), H64 (head_dim 64), B (one 7B-shaped layer), G7 (Qwen2, 7 query heads per KV head) and MQA (16 heads
+on one KV head), each in fp16 and bf16.  Every logit row the decoder
 returns is at most twice as far (max norm) from the twin's as the logits of the dense model of the same dtype (the twin's weights
 rounded) run by HF on the same schedule (HF takes several tokens at once with a cache).  Schedules:
   * extend(17) after reset(), then 40 teacher-forced steps;

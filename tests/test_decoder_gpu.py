@@ -3,8 +3,10 @@
 Models are made as in test_model_gpu.py (random init from a config, eager attention, oracle.make_layer layers scaled to entries of about
 1 / sqrt(in_features), loaded through checkpoint.load_quantized, then .cuda()); the fp64 twin is the same HF class in float64 holding the
 dense fp64 weights W.T.  Kinds: A4 / A3 (Llama, hidden 1024, 8 heads, 2 KV heads, at 4 / 3 bits), C (Qwen2 with q/k/v bias and a
-quantized lm_head), M (Mistral with its window >= max_len), H64 (Llama with head_dim 64), B (one 7B-shaped Llama layer).  Each in fp16
-and bf16, after a prompt of 1 and of 17 tokens:
+quantized lm_head), M (Mistral with its window >= max_len), H64 (Llama with head_dim 64), B (one 7B-shaped Llama layer), G7 (Qwen2
+with the attention of Qwen2.5-0.5B: 14 heads of 64 on 2 KV heads, 7 query heads per KV head, and a quantized lm_head, at 4 bits) and
+MQA (Llama with 16 heads of 128 on one KV head: each group over two clusters of the attention kernels, at 3 bits).  Each in fp16 and
+bf16, after a prompt of 1 and of 17 tokens:
   * teacher-forced decode for 40 steps: at every step the decoder's logits are at most twice as far (max norm) from the twin's as the
     logits of a dense model of the same dtype (the twin's weights rounded) decoding the same tokens with HF's cache;
   * greedy generate matches the twin's greedy tokens up to the first step where the twin's top-2 margin is below twice the error
@@ -41,6 +43,10 @@ SPEC = {  # kind: (config class, config kwargs, bits, lm_head quantized)
                                 vocab_size=512), 4, False),
     "B": ("LlamaConfig", dict(hidden_size=4096, intermediate_size=11008, num_hidden_layers=1, num_attention_heads=32, num_key_value_heads=32,
                               vocab_size=256), 4, False),
+    "G7": ("Qwen2Config", dict(hidden_size=896, intermediate_size=2432, num_hidden_layers=2, num_attention_heads=14, num_key_value_heads=2,
+                               vocab_size=512), 4, True),
+    "MQA": ("LlamaConfig", dict(hidden_size=2048, intermediate_size=5504, num_hidden_layers=2, num_attention_heads=16, num_key_value_heads=1,
+                                vocab_size=512), 3, False),
 }
 MODEL_OF = {"LlamaConfig": "LlamaForCausalLM", "Qwen2Config": "Qwen2ForCausalLM", "MistralConfig": "MistralForCausalLM"}
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16}

@@ -1,6 +1,6 @@
 """Speculative decoding in SequenceDecoder (speculate=K) on the GPU, on the models of test_decoder_gpu.py (A4, A3, C with q/k/v bias and a
-quantized lm_head, M, H64 and the 7B-shaped B) in fp16 and bf16, K in {3, 15} on every kind and {1, 7} besides on A4, prompts of 1 and
-17 tokens, against the fp64 twin:
+quantized lm_head, M, H64, the 7B-shaped B, G7 with 7 query heads per KV head and MQA with one KV head) in fp16 and bf16, K in
+{3, 15} on every kind and {1, 7} besides on A4, prompts of 1 and 17 tokens, against the fp64 twin:
   * teacher-forced verify() chunks of K + 1 tokens: every logits row at most twice as far (max norm) from the twin's as the logits of
     the dense model of the same dtype decoding the same tokens with HF's cache (the criterion of test_decoder_gpu.py);
   * after each verify, quant_cuda.sample of every row at dec.vpos (= p + t + 1) passes the draw check of test_decoder_sample_gpu.py;
