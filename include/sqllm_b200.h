@@ -54,7 +54,8 @@ extern "C" {
                                  sqllm_lutgemm_fused_f32, sqllm_sequence_create_ops, sqllm_attn_decode,
                                  sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits,
                                  sqllm_attn_extend, sqllm_attn_extend_splits, sqllm_sample, sqllm_attn_verify,
-                                 sqllm_attn_verify_splits, sqllm_attn_verify_launch_splits
+                                 sqllm_attn_verify_splits, sqllm_attn_verify_launch_splits, sqllm_attn_decode_paged,
+                                 sqllm_attn_extend_paged
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -658,6 +659,67 @@ int sqllm_attn_verify_splits(int n_heads, int n_kv, int n_tokens, int sm_count);
  * n_kv ceil(n_tokens (n_heads / n_kv) / 8) clusters of S CTAs of the kernel instance (dtype, head_dim, rows per CTA) can be resident at
  * once; 1 when even S = 2 cannot.  0 for arguments sqllm_attn_verify rejects or when the device cannot be queried.  Independent of pos. */
 int sqllm_attn_verify_launch_splits(int dtype, int n_heads, int n_kv, int head_dim, int n_tokens);
+
+/* Paged KV caches: the decode and chunk attention above on a pool of pages shared by many sequences, so that a sequence holds memory
+ * for the positions it uses, not for its capacity.
+ *   page      64 consecutive positions of one sequence for every KV head of a layer; one layer's pool k_pages (and v_pages) is
+ *             [n_pages][n_kv][64][d] of dtype
+ *   table     a sequence's block table, int32 [table_width], table_width = ceil(capacity / 64): position t is row t % 64 of page
+ *             table[t / 64].  Entries a call does not reach are never read, so an unassigned entry may hold anything (-1 by convention).
+ * A call reads no page that the entries of blocks 0 .. (its last position) / 64 do not name, and no slot past a row's own position;
+ * it writes only the slots of the positions it appends.  Several rows may name the same page for reading (a shared prefix); keeping
+ * two active rows from appending to the same slot is the caller's duty.  capacity is the positions a sequence may use, which is also
+ * the rows of the rope tables. */
+
+/* Decode attention of B sequences in one page pool: row b is what sqllm_attn_decode_batch computes for it, at pos[b], through row b
+ * of block_table [batch][table_width], with the split rule of sqllm_attn_decode_batch_splits(n_heads, n_kv, batch, SM count) and the
+ * same combine order.  So a row is bitwise equal to sqllm_attn_decode_batch run on the row's pages gathered into a contiguous cache.
+ * Row b is idle - it reads no page and writes nothing - when pos[b] is outside [0, capacity) or an entry of its blocks
+ * 0 .. pos[b] / 64 is outside [0, n_pages); every CTA of the row checks those entries itself before any cluster barrier.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_decode_batch, n_pages >= 1,
+ * table_width = ceil(capacity / 64), k_pages, v_pages and the other pointers non-null and 16-byte aligned, block_table non-null and
+ * 4-byte aligned.  No workspace, no atomics, no allocation, no host synchronisation: CUDA-graph capturable. */
+typedef struct sqllm_attn_decode_paged_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int batch;                /* sequences, 1 .. 65535 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions a sequence may use: the rows of the rope tables */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;          /* [batch][n_heads*d | n_kv*d | n_kv*d] */
+    const int32_t *pos;       /* DEVICE [batch] */
+    const float *rope_cos, *rope_sin;
+    void *k_pages, *v_pages;  /* [n_pages][n_kv][64][d] */
+    int n_pages;
+    const int32_t *block_table; /* DEVICE [batch][table_width] */
+    int table_width;          /* ceil(capacity / 64) */
+    void *out;                /* [batch][n_heads*d] */
+} sqllm_attn_decode_paged_args;
+
+int sqllm_attn_decode_paged(const sqllm_attn_decode_paged_args *args, void *stream);
+
+/* The chunk attention of sqllm_attn_extend for one sequence in a page pool, through its block table row [table_width]: both launches
+ * (the append and the attention) take the table, with the split rule of sqllm_attn_extend_splits.  The output and the stored k / v
+ * are bitwise those of sqllm_attn_extend on the sequence's pages gathered into a contiguous cache.  If an entry of blocks
+ * 0 .. (start + n_tokens - 1) / 64 is outside [0, n_pages), neither launch reads a page or writes anything.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_extend, and the page arguments of
+ * sqllm_attn_decode_paged.  No allocation, no host synchronisation: CUDA-graph capturable for a fixed start. */
+typedef struct sqllm_attn_extend_paged_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions the sequence may use: the rows of the rope tables */
+    int start;                /* position of the chunk's first token */
+    int n_tokens;             /* T */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    const void *qkv;          /* [T][n_heads*d | n_kv*d | n_kv*d] */
+    const float *rope_cos, *rope_sin;
+    void *k_pages, *v_pages;  /* [n_pages][n_kv][64][d] */
+    int n_pages;
+    const int32_t *block_table; /* DEVICE [table_width]: the sequence's row */
+    int table_width;          /* ceil(capacity / 64) */
+    void *out;                /* [T][n_heads*d] */
+} sqllm_attn_extend_paged_args;
+
+int sqllm_attn_extend_paged(const sqllm_attn_extend_paged_args *args, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Token sampling: one token per row of logits, on the device (DESIGN.md section 3.20).  Row b (b < rows) holds x_i =

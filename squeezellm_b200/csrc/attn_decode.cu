@@ -1,7 +1,7 @@
-// attn_decode.cu - decode attention with rotary and KV-cache append (attn_decode.cuh) behind sqllm_attn_decode (one sequence) and
-// sqllm_attn_decode_batch (several, each at its own position); causal attention of a chunk of new tokens with the same rotary and
+// attn_decode.cu - decode attention with rotary and KV-cache append (attn_decode.cuh) behind sqllm_attn_decode (one sequence),
+// sqllm_attn_decode_batch (several, each at its own position) and sqllm_attn_decode_paged (several, in one pool of KV pages); causal attention of a chunk of new tokens with the same rotary and
 // append (attn_extend.cuh) behind sqllm_attn_extend; decode attention of up to 16 new tokens of one sequence at a device position
-// (attn_verify.cuh) behind sqllm_attn_verify.
+// (attn_verify.cuh) behind sqllm_attn_verify; the chunk attention on KV pages behind sqllm_attn_extend_paged.
 #include <limits.h>
 #include <math.h>
 #include <stdint.h>
@@ -108,7 +108,69 @@ int attn_launch(const Args *a, int batch, void *stream) {
 }
 
 template <typename T, int D>
-KernelSmem extend_kernel_of() { return {attn::attn_extend_kernel<T, D>, attn::ext_smem_bytes(D)}; }
+void *paged_kernel_of(int G) {
+    switch (G) {
+        case 1: return (void *)attn::attn_decode_paged_kernel<T, D, 1>;
+        case 2: return (void *)attn::attn_decode_paged_kernel<T, D, 2>;
+        case 4: return (void *)attn::attn_decode_paged_kernel<T, D, 4>;
+        default: return (void *)attn::attn_decode_paged_kernel<T, D, 8>;
+    }
+}
+
+// the checks of the page arguments both paged entry points share, after check_heads: the pool size, the table width against capacity,
+// the pointers of the pools and the table
+template <typename Args>
+int check_pages(const Args *a) {
+    if (a->n_pages < 1) return fail(SQLLM_EINVAL, "n_pages=%d must be >= 1", a->n_pages);
+    const int width = (a->capacity + attn::PAGE - 1) / attn::PAGE;
+    if (a->table_width != width)
+        return fail(SQLLM_EINVAL, "table_width=%d must be ceil(capacity=%d / %d) = %d", a->table_width, a->capacity, attn::PAGE, width);
+    if (int rc = check_ptrs({{a->k_pages, "k_pages"}, {a->v_pages, "v_pages"}})) return rc;
+    if (!a->block_table || (reinterpret_cast<uintptr_t>(a->block_table) & 3))
+        return fail(SQLLM_EINVAL, "block_table must be a non-null 4-byte aligned pointer");
+    return SQLLM_OK;
+}
+
+int paged_launch(const sqllm_attn_decode_paged_args *a, void *stream) {
+    if (int rc = check_dtype(a->dtype)) return rc;
+    if (a->batch < 1 || a->batch > MAX_BATCH) return fail(SQLLM_EINVAL, "batch=%d must be in [1, %d]", a->batch, MAX_BATCH);
+    if (int rc = check_heads(a)) return rc;
+    if (int rc = check_pages(a)) return rc;
+    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->out, "out"}}))
+        return rc;
+    const int g = a->n_heads / a->n_kv, gc = std::min(g, attn::GMAX);
+    const int G = gc <= 1 ? 1 : gc <= 2 ? 2 : gc <= 4 ? 4 : 8;
+    const bool bf = a->dtype == SQLLM_DT_BF16;
+    void *fn = a->head_dim == 128 ? (bf ? paged_kernel_of<__nv_bfloat16, 128>(G) : paged_kernel_of<__half, 128>(G))
+                                  : (bf ? paged_kernel_of<__nv_bfloat16, 64>(G) : paged_kernel_of<__half, 64>(G));
+    int sm = 0;
+    int rc = dev_setup({}, &sm);
+    if (rc) return rc;
+    attn::PagedParams p;
+    p.qkv = a->qkv; p.pos = a->pos; p.cos = a->rope_cos; p.sin = a->rope_sin;
+    p.k_cache = a->k_pages; p.v_cache = a->v_pages; p.out = a->out;
+    p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = g; p.hchunks = (g + attn::GMAX - 1) / attn::GMAX; p.capacity = a->capacity;
+    p.qscale = a->scale * attn::LOG2E;
+    p.table = a->block_table; p.width = a->table_width; p.n_pages = a->n_pages;
+    const int S = splits(a->n_heads, a->n_kv, a->batch, sm);   // the rule of sqllm_attn_decode_batch: the same bits per row
+    const dim3 grid(S, a->n_kv * p.hchunks, a->batch);
+    const cudaError_t e = launch_ex(reinterpret_cast<void (*)(attn::PagedParams)>(fn), grid, attn::THREADS, 0,
+                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_decode_paged launch failed: %s", cudaGetErrorString(e));
+    return SQLLM_OK;
+}
+
+template <typename T, int D, typename P>
+KernelSmem extend_kernel_of() {
+    if constexpr (attn::is_paged<P>) return {attn::attn_extend_paged_kernel<T, D>, attn::ext_smem_bytes(D)};
+    else return {attn::attn_extend_kernel<T, D>, attn::ext_smem_bytes(D)};
+}
+
+template <typename T, int D, typename P>
+auto append_kernel_of() {
+    if constexpr (attn::is_paged<P>) return attn::attn_append_paged_kernel<T, D>;
+    else return attn::attn_append_kernel<T, D>;
+}
 
 // the rows of the chunk's query tiles (T tokens x g heads of a group), 0 when they need more tiles than the grid holds
 long long ext_tiles(int n_heads, int n_kv, int T) {
@@ -126,7 +188,10 @@ int ext_splits(int n_heads, int n_kv, int T, int start, int sm_count) {
     return (int)std::max(1LL, std::min({(long long)attn::MAX_CLUSTER, sm_count / tiles, blocks}));
 }
 
-int extend_launch(const sqllm_attn_extend_args *a, void *stream) {
+// the checks and both launches of sqllm_attn_extend (P = ExtParams) and sqllm_attn_extend_paged (P = ExtPagedParams)
+template <typename P, typename Args>
+int extend_launch(const Args *a, void *stream) {
+    constexpr bool PAGED = attn::is_paged<P>;
     if (int rc = check_dtype(a->dtype)) return rc;
     if (int rc = check_heads(a)) return rc;
     if (a->n_tokens < 1) return fail(SQLLM_EINVAL, "n_tokens=%d must be >= 1", a->n_tokens);
@@ -136,29 +201,37 @@ int extend_launch(const sqllm_attn_extend_args *a, void *stream) {
     if (ext_tiles(a->n_heads, a->n_kv, a->n_tokens) == 0 || a->n_kv > 65535)
         return fail(SQLLM_EINVAL, "n_tokens=%d x %d heads per KV head needs more than %d query tiles of %d, or n_kv=%d > 65535",
                     a->n_tokens, a->n_heads / a->n_kv, attn::MAX_TILES, attn::BM, a->n_kv);
-    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->k_cache, "k_cache"},
-                             {a->v_cache, "v_cache"}, {a->out, "out"}}))
-        return rc;
+    P p;
+    if constexpr (PAGED) {
+        if (int rc = check_pages(a)) return rc;
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->out, "out"}})) return rc;
+        p.k_cache = a->k_pages; p.v_cache = a->v_pages; p.table = a->block_table; p.n_pages = a->n_pages;
+    } else {
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->k_cache, "k_cache"},
+                                 {a->v_cache, "v_cache"}, {a->out, "out"}}))
+            return rc;
+        p.k_cache = a->k_cache; p.v_cache = a->v_cache;
+    }
     const bool bf = a->dtype == SQLLM_DT_BF16;
-    const KernelSmem k = a->head_dim == 128 ? (bf ? extend_kernel_of<__nv_bfloat16, 128>() : extend_kernel_of<__half, 128>())
-                                            : (bf ? extend_kernel_of<__nv_bfloat16, 64>() : extend_kernel_of<__half, 64>());
+    const KernelSmem k = a->head_dim == 128 ? (bf ? extend_kernel_of<__nv_bfloat16, 128, P>() : extend_kernel_of<__half, 128, P>())
+                                            : (bf ? extend_kernel_of<__nv_bfloat16, 64, P>() : extend_kernel_of<__half, 64, P>());
     int sm = 0;
     int rc = dev_setup({k}, &sm);
     if (rc) return rc;
-    attn::ExtParams p;
-    p.qkv = a->qkv; p.cos = a->rope_cos; p.sin = a->rope_sin; p.k_cache = a->k_cache; p.v_cache = a->v_cache; p.out = a->out;
+    p.qkv = a->qkv; p.cos = a->rope_cos; p.sin = a->rope_sin; p.out = a->out;
     p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = a->n_heads / a->n_kv; p.capacity = a->capacity; p.start = a->start; p.T = a->n_tokens;
     p.qscale = a->scale * attn::LOG2E / attn::QPRE;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    void (*append)(attn::ExtParams) = a->head_dim == 128 ? (bf ? attn::attn_append_kernel<__nv_bfloat16, 128> : attn::attn_append_kernel<__half, 128>)
-                                                         : (bf ? attn::attn_append_kernel<__nv_bfloat16, 64> : attn::attn_append_kernel<__half, 64>);
+    void (*append)(P) = a->head_dim == 128 ? (bf ? append_kernel_of<__nv_bfloat16, 128, P>() : append_kernel_of<__half, 128, P>())
+                                           : (bf ? append_kernel_of<__nv_bfloat16, 64, P>() : append_kernel_of<__half, 64, P>());
+    const char *name = PAGED ? "attn_extend_paged" : "attn_extend";
     append<<<a->n_tokens, attn::APPEND_THREADS, 0, st>>>(p);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_extend append launch failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s append launch failed: %s", name, cudaGetErrorString(e));
     const int S = ext_splits(a->n_heads, a->n_kv, a->n_tokens, a->start, sm);
     const dim3 grid(S, (unsigned)ext_tiles(a->n_heads, a->n_kv, a->n_tokens), a->n_kv);
-    e = launch_ex(reinterpret_cast<void (*)(attn::ExtParams)>(const_cast<void *>(k.fn)), grid, attn::XTHREADS, k.bytes, st, cluster_of(S), p);
-    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_extend launch failed: %s", cudaGetErrorString(e));
+    e = launch_ex(reinterpret_cast<void (*)(P)>(const_cast<void *>(k.fn)), grid, attn::XTHREADS, k.bytes, st, cluster_of(S), p);
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
     return SQLLM_OK;
 }
 
@@ -285,7 +358,17 @@ int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int
 
 int sqllm_attn_extend(const sqllm_attn_extend_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
-    return extend_launch(a, stream);
+    return extend_launch<attn::ExtParams>(a, stream);
+}
+
+int sqllm_attn_decode_paged(const sqllm_attn_decode_paged_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return paged_launch(a, stream);
+}
+
+int sqllm_attn_extend_paged(const sqllm_attn_extend_paged_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return extend_launch<attn::ExtPagedParams>(a, stream);
 }
 
 int sqllm_attn_verify_splits(int n_heads, int n_kv, int n_tokens, int sm_count) { return ver_splits(n_heads, n_kv, n_tokens, sm_count); }

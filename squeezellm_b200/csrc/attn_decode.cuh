@@ -13,6 +13,10 @@
 // The CTA whose range holds `pos` takes the new k (rotated, rounded to the dtype) and v from its shared memory, where every CTA
 // computes them from qkv; one CTA stores them into the cache.  So no CTA reads a cache slot another CTA of the launch writes, and no
 // slot past `pos` is read.
+//
+// The paged kernel (sqllm_attn_decode_paged) is the batched kernel with the caches in a pool of PAGE-position pages: row b's position
+// t is row t % PAGE of page table[b][t / PAGE].  A CTA's range starts at a block of BLOCK_POS = PAGE positions, so each warp step
+// looks its page up once.
 #pragma once
 #include "common.cuh"
 
@@ -25,6 +29,8 @@ constexpr int MAX_CLUSTER = 8;   // portable cluster size
 constexpr int BLOCK_POS = 64;    // positions are dealt to the CTAs of a cluster in blocks of this many
 constexpr int GMAX = 8;          // query heads per CTA: a larger group is split over several clusters, each reading the K / V again
 constexpr float LOG2E = 1.4426950408889634f;
+constexpr int PAGE = 64;         // positions per KV page of the paged kernels: one page is one BLOCK_POS block of a CTA's range
+static_assert(PAGE == BLOCK_POS, "a KV page must be exactly one block of positions");
 
 struct Params {                // the batched kernel: each of qkv, pos, the caches and out [batch] times over
     const void *qkv;             // [n_heads*D | n_kv*D | n_kv*D]
@@ -35,6 +41,33 @@ struct Params {                // the batched kernel: each of qkv, pos, the cach
     int n_heads, n_kv, g, hchunks, capacity;
     float qscale;                // scale * log2(e): scores in base 2
 };
+
+// the paged batched kernel: the caches are page pools [n_pages][n_kv][PAGE][D] shared by the rows; row b's position t is row t % PAGE
+// of page table[b * width + t / PAGE]
+struct PagedParams : Params {
+    const int *table;            // [batch][width]
+    int width, n_pages;
+};
+
+// one row's block table, as attn_decode_row.inc reads it (the contiguous kernels pass an empty one they never read)
+struct Pages {
+    const int *table;
+    int n_pages;
+};
+
+// the CTA's verdict on a row at `pos`: every entry of blocks 0 .. pos / PAGE names a page of the pool.  Every thread takes part.
+__device__ __forceinline__ bool pages_valid(const Pages pg, int pos) {
+    bool bad = false;
+    for (int i = threadIdx.x; i <= pos / PAGE; i += blockDim.x) {
+        const int id = pg.table[i];
+        bad |= id < 0 || id >= pg.n_pages;
+    }
+    return !__syncthreads_or(bad);
+}
+
+// element offset of page `id`'s rows of KV head kvh in a pool [n_pages][n_kv][PAGE][D]
+template <int D>
+__device__ __forceinline__ size_t page_base(int id, int n_kv, int kvh) { return ((size_t)id * n_kv + kvh) * PAGE * D; }
 
 // positions [p0, p1) of CTA `rank` of S for pos + 1 positions: blocks of BLOCK_POS, ceil(blocks / S) per CTA
 __device__ __forceinline__ void cta_range(int pos, int rank, int S, int &p0, int &p1) {
@@ -75,6 +108,8 @@ __device__ __forceinline__ float wexp2(float a, float b) { return a == -INFINITY
 // (DESIGN §3.18)
 template <typename T, int D, int G>
 __global__ void __launch_bounds__(THREADS, 1) attn_decode_kernel(const Params p) {
+    constexpr bool PAGED = false;
+    const Pages pg{};
 #include "attn_decode_row.inc"
 }
 
@@ -90,6 +125,23 @@ __global__ void __launch_bounds__(THREADS, 1) attn_decode_batch_kernel(const Par
     p.k_cache = static_cast<T *>(all.k_cache) + cache;
     p.v_cache = static_cast<T *>(all.v_cache) + cache;
     p.out = static_cast<T *>(all.out) + (size_t)b * all.n_heads * D;
+    constexpr bool PAGED = false;
+    const Pages pg{};
+#include "attn_decode_row.inc"
+}
+
+// gridDim.z sequences in one page pool: sequence b = blockIdx.z at all.pos[b] through row b of the block table, with its own qkv and out
+// rows; a row with an entry outside [0, n_pages) among the blocks it reads or writes is idle.  The same code as the batched kernel but
+// for the addressing, so a row is bitwise what the batched kernel computes on the row's pages gathered into a contiguous cache.
+template <typename T, int D, int G>
+__global__ void __launch_bounds__(THREADS, 1) attn_decode_paged_kernel(const PagedParams all) {
+    const int b = blockIdx.z;
+    Params p = all;
+    p.qkv = static_cast<const T *>(all.qkv) + (size_t)b * (all.n_heads + 2 * all.n_kv) * D;
+    p.pos = all.pos + b;
+    p.out = static_cast<T *>(all.out) + (size_t)b * all.n_heads * D;
+    constexpr bool PAGED = true;
+    const Pages pg{all.table + (size_t)b * all.width, all.n_pages};
 #include "attn_decode_row.inc"
 }
 

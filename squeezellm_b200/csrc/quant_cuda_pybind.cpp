@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `attn_verify`, `sample`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `attn_verify`, `attn_decode_paged`, `attn_extend_paged`, `sample`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -615,10 +615,13 @@ void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, 
 // head_dim], the batch, head_dim, capacity, scale, the cache and out dtypes and v_cache's shape; then own(batch, capacity, head_dim), the
 // binding's own shape checks; then the rope tables.  The device checks come last, so that a CPU caller sees the same rejections.  pos:
 // null for attn_extend.  -> the sqllm args with the fields the four share.
+// table: the block table of attn_decode_paged ([batch, width], lead = 1) and attn_extend_paged ([width], lead = 0), null for the
+// others.  With a table the caches are page pools [n_pages, n_kv, 64, head_dim], capacity is the rope tables' rows, the batch is the
+// table's rows, and the table must be int32, contiguous and 4-byte aligned with width = ceil(capacity / 64).
 template <typename Args, typename Own>
 Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::Tensor *pos, const torch::Tensor &rope_cos,
                const torch::Tensor &rope_sin, const torch::Tensor &k_cache, const torch::Tensor &v_cache, const torch::Tensor &out,
-               int64_t n_heads, int64_t n_kv, double scale, Own own) {
+               int64_t n_heads, int64_t n_kv, double scale, Own own, const torch::Tensor *table = nullptr) {
     const std::pair<const torch::Tensor *, const char *> all[] = {{&qkv, "qkv"}, {pos, "pos"}, {&rope_cos, "rope_cos"}, {&rope_sin, "rope_sin"},
                                                                   {&k_cache, "k_cache"}, {&v_cache, "v_cache"}, {&out, "out"}};
     for (const auto &t : all) {
@@ -629,9 +632,24 @@ Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::
     const auto dt = qkv.scalar_type();
     TORCH_CHECK(dt == torch::kFloat16 || dt == torch::kBFloat16, fn, ": dtype of qkv must be torch.float16 or torch.bfloat16 (got ", dt, ")");
     TORCH_CHECK(n_kv >= 1 && n_heads >= 1 && n_heads % n_kv == 0, fn, ": n_heads=", n_heads, " must be a positive multiple of n_kv=", n_kv);
-    TORCH_CHECK(k_cache.dim() == 3 + lead && k_cache.size(lead) == n_kv, fn, ": k_cache must be [", lead ? "batch, " : "", "n_kv=", n_kv,
-                ", capacity, head_dim] (got ", k_cache.sizes(), ")");
-    const int64_t B = lead ? k_cache.size(0) : 1, cap = k_cache.size(lead + 1), d = k_cache.size(lead + 2);
+    int64_t B, cap, d;
+    if (table) {
+        TORCH_CHECK(table->defined() && table->is_contiguous() && table->scalar_type() == torch::kInt32, fn,
+                    ": block_table must be a contiguous int32 tensor");
+        TORCH_CHECK(!(reinterpret_cast<uintptr_t>(table->data_ptr()) & 3), fn, ": block_table must be 4-byte aligned");
+        TORCH_CHECK(k_cache.dim() == 4 && k_cache.size(1) == n_kv && k_cache.size(2) == 64 && k_cache.size(0) >= 1 &&
+                    k_cache.size(0) <= INT32_MAX, fn, ": k_pages must be [n_pages, n_kv=", n_kv, ", 64, head_dim] (got ", k_cache.sizes(), ")");
+        cap = rope_cos.dim() == 2 ? rope_cos.size(0) : 0;
+        const int64_t width = (cap + 63) / 64;
+        TORCH_CHECK(table->dim() == 1 + lead && table->size(lead) == width, fn, ": block_table must be [", lead ? "batch, " : "",
+                    "ceil(capacity=", cap, " / 64)=", width, "] (got ", table->sizes(), ")");
+        B = lead ? table->size(0) : 1;
+        d = k_cache.size(3);
+    } else {
+        TORCH_CHECK(k_cache.dim() == 3 + lead && k_cache.size(lead) == n_kv, fn, ": k_cache must be [", lead ? "batch, " : "", "n_kv=", n_kv,
+                    ", capacity, head_dim] (got ", k_cache.sizes(), ")");
+        B = lead ? k_cache.size(0) : 1; cap = k_cache.size(lead + 1); d = k_cache.size(lead + 2);
+    }
     TORCH_CHECK(B >= 1 && B <= 65535, fn, ": batch=", B, " must be in [1, 65535]");
     TORCH_CHECK(d == 64 || d == 128, fn, ": head_dim=", d, " is not 64 or 128");
     TORCH_CHECK(cap >= 1 && cap <= INT32_MAX, fn, ": capacity=", cap, " must be >= 1");
@@ -646,11 +664,18 @@ Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::
     for (const auto &t : all)
         TORCH_CHECK(!t.first || (t.first->is_cuda() && t.first->device() == qkv.device()), fn, ": ", t.second,
                     " must be a CUDA tensor, on the device of qkv");
+    TORCH_CHECK(!table || (table->is_cuda() && table->device() == qkv.device()), fn, ": block_table must be a CUDA tensor, on the device of qkv");
     Args a;
     a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
     a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
     a.qkv = qkv.data_ptr(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
-    a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+    if constexpr (std::is_same<Args, sqllm_attn_decode_paged_args>::value || std::is_same<Args, sqllm_attn_extend_paged_args>::value) {
+        a.k_pages = k_cache.data_ptr(); a.v_pages = v_cache.data_ptr(); a.n_pages = (int)k_cache.size(0);
+        a.block_table = table->data_ptr<int32_t>(); a.table_width = (int)table->size(lead);
+    } else {
+        a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr();
+    }
+    a.out = out.data_ptr();
     return a;
 }
 
@@ -728,6 +753,45 @@ void attn_verify(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, t
     a.n_tokens = (int)qkv.size(0);
     a.pos = pos.data_ptr<int32_t>();
     check_status(sqllm_attn_verify(&a, cur_stream()), "quant_cuda.attn_verify");
+}
+
+// Decode attention of B sequences in one page pool (sqllm_attn_decode_paged): for each row b what attn_decode_batch does, at position
+// pos[b], through row b of block_table; a row whose pos[b] is outside the cache or whose table names a page outside the pool writes
+// nothing.
+void attn_decode_paged(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_pages,
+                       torch::Tensor v_pages, torch::Tensor block_table, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_decode_paged_args>("attn_decode_paged", 1, qkv, &pos, rope_cos, rope_sin, k_pages, v_pages, out, n_heads,
+                                                     n_kv, scale, [&](int64_t B, int64_t, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_decode_paged: qkv must be [batch=", B,
+                    ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, "attn_decode_paged: out must be [batch=", B,
+                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
+        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, "attn_decode_paged: pos must be int32 [batch=", B,
+                    "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
+    }, &block_table);
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    a.batch = (int)block_table.size(0);
+    a.pos = pos.data_ptr<int32_t>();
+    check_status(sqllm_attn_decode_paged(&a, cur_stream()), "quant_cuda.attn_decode_paged");
+}
+
+// The chunk attention of attn_extend for one sequence in a page pool (sqllm_attn_extend_paged), through its block table row.
+void attn_extend_paged(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_pages,
+                       torch::Tensor v_pages, torch::Tensor block_table_row, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_extend_paged_args>("attn_extend_paged", 0, qkv, nullptr, rope_cos, rope_sin, k_pages, v_pages, out, n_heads,
+                                                     n_kv, scale, [&](int64_t, int64_t cap, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend_paged: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
+                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        const int64_t T = qkv.size(0);
+        TORCH_CHECK(T >= 1, "attn_extend_paged: qkv has no rows (T=0)");
+        TORCH_CHECK(start >= 0, "attn_extend_paged: start=", start, " must be >= 0");
+        TORCH_CHECK(start + T <= cap, "attn_extend_paged: start=", start, " + T=", T, " must be <= capacity=", cap);
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend_paged: out must be [T=", T,
+                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
+    }, &block_table_row);
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    a.start = (int)start; a.n_tokens = (int)qkv.size(0);
+    check_status(sqllm_attn_extend_paged(&a, cur_stream()), "quant_cuda.attn_extend_paged");
 }
 
 // One token per row of logits (sqllm_sample): greedy, or temperature / top-k / top-p filtering and a Gumbel-max draw keyed by seed[b]
@@ -926,6 +990,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               TORCH_CHECK(sm > 0, "attn_extend_splits: ", sqllm_last_error());
               return sqllm_attn_extend_splits(n_heads, n_kv, n_tokens, start, sm);
           }, "CTAs per cluster of attn_extend on the current device");
+    m.def("attn_decode_paged", &attn_decode_paged, "attn_decode_batch on KV page pools [n_pages, n_kv, 64, head_dim]: row b at position "
+          "pos[b] through row b of block_table [batch, ceil(capacity / 64)]; a row with pos outside the cache or a table entry outside the "
+          "pool writes nothing", py::arg("qkv"), py::arg("pos"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_pages"),
+          py::arg("v_pages"), py::arg("block_table"), py::arg("out"), py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_extend_paged", &attn_extend_paged, "attn_extend for one sequence on KV page pools [n_pages, n_kv, 64, head_dim] through "
+          "its block table row [ceil(capacity / 64)]; an entry outside the pool among the chunk's blocks writes nothing", py::arg("qkv"),
+          py::arg("start"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_pages"), py::arg("v_pages"), py::arg("block_table_row"),
+          py::arg("out"), py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
     m.def("attn_verify", &attn_verify, "decode attention of T <= 16 new tokens at device positions pos .. pos+T-1: rotary, the append of k / "
           "v at those slots, per token softmax(scale q K^T[0..p_t]) V[0..p_t] (qkv [T, ...], pos int32 [1], rope_cos, rope_sin, k_cache, "
           "v_cache, out [T, ...], n_heads, n_kv, scale); pos < 0 or pos + T > capacity writes nothing; current stream",

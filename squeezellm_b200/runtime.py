@@ -483,17 +483,105 @@ def accept_length(drafts, draws):
     return n
 
 
+PAGE = 64  # positions per KV page of a paged decoder: attn::PAGE of the paged attention kernels
+
+
+class PagePool:
+    """The host side of a pool of n_pages KV pages shared by `slots` sequences of up to `width` pages each (no device): the free list,
+    each page's reference count and each slot's block table, a list of `width` page ids with -1 where no page is assigned.  A page is
+    referenced by every slot whose table names it; it returns to the free list when the last one lets it go.  Every method that can
+    fail raises before it changes anything."""
+
+    def __init__(self, n_pages, slots, width):
+        self.n_pages, self.width = n_pages, width
+        self._free = list(range(n_pages - 1, -1, -1))  # pop() takes the lowest id
+        self.refs = [0] * n_pages
+        self.tables = [[-1] * width for _ in range(slots)]
+
+    @property
+    def free(self):
+        """Pages on the free list."""
+        return len(self._free)
+
+    def held(self, slot):
+        """The number of leading blocks of `slot` that have a page."""
+        t = self.tables[slot]
+        return next((j for j, x in enumerate(t) if x < 0), len(t))
+
+    def need(self, slot, blocks, fresh=False):
+        """Pages assign(slot, blocks, fresh) takes from the free list, net of the pages it gives back."""
+        if fresh:
+            return blocks - sum(1 for x in self.tables[slot] if x >= 0 and self.refs[x] == 1)
+        return max(0, blocks - self.held(slot))
+
+    def assign(self, slot, blocks, fresh=False):
+        """Give `slot` pages for its blocks 0 .. blocks-1 (fresh: drop its pages first, so that none of them is shared); RuntimeError
+        when the free list is short.  -> [(block, page)] newly assigned."""
+        h = 0 if fresh else self.held(slot)
+        self.reserve({slot: (blocks, fresh)})
+        return [(j, self.tables[slot][j]) for j in range(h, blocks)]
+
+    def reserve(self, want):
+        """assign() for several slots at once, {slot: (blocks, fresh)}: all of them or, with RuntimeError naming the slots, none."""
+        if sum(max(0, self.need(b, n, f)) for b, (n, f) in want.items()) > len(self._free):
+            raise RuntimeError(f"KV page pool: no free page for slot(s) {sorted(want)} ({len(self._free)} of {self.n_pages} pages "
+                               f"free); release a slot first")
+        for b, (n, f) in want.items():
+            if f:
+                self.release(b)
+            for j in range(self.held(b), n):
+                self.tables[b][j] = p = self._free.pop()
+                self.refs[p] = 1
+
+    def release(self, slot):
+        """Let go of every page of `slot`; its table becomes all -1."""
+        t = self.tables[slot]
+        for x in t:
+            if x >= 0 and self.refs[x] < 1:
+                raise ValueError(f"KV page pool: page {x} of slot {slot} is already free")
+        for j, x in enumerate(t):
+            if x >= 0:
+                self.refs[x] -= 1
+                if self.refs[x] == 0:
+                    self._free.append(x)
+                t[j] = -1
+
+    def fork(self, src, dst, pos):
+        """dst (holding no page) starts as src at position pos: the full pages of src before pos are shared, the partly filled one
+        (pos % PAGE != 0) is replaced by a fresh page.  RuntimeError without a free page for it.  -> (src's page, dst's page) to
+        copy, or None at a page boundary."""
+        if any(x >= 0 for x in self.tables[dst]):
+            raise ValueError(f"KV page pool: slot {dst} already holds pages")
+        full, part = divmod(pos, PAGE)
+        if part and not self._free:
+            raise RuntimeError(f"KV page pool: no free page for the fork into slot {dst} (0 of {self.n_pages} pages free)")
+        for j in range(full):
+            x = self.tables[src][j]
+            self.tables[dst][j] = x
+            self.refs[x] += 1
+        if not part:
+            return None
+        self.tables[dst][full] = p = self._free.pop()
+        self.refs[p] = 1
+        return self.tables[src][full], p
+
+
 class _DecoderBase:
     """What SequenceDecoder and BatchDecoder share, for `slots` sequences (SequenceDecoder: one): the set-up, the graph capture, the
     prompts (prefill and extend of one slot), the replay with its full-cache check and the generate loop.  Slot b is row b of pos, tok,
-    the attention output and the sampling buffers and block b of the caches [n_layers, slots, n_kv, max_len, head_dim]; _pos holds the
-    slots' host positions (-1: idle).  A subclass defines _step (one token of every slot on the current stream: what the graph holds) and
-    reset(), and names itself in CACHE_FULL."""
+    the attention output and the sampling buffers; _pos holds the slots' host positions (-1: idle).  The caches have one of two layouts:
+      contiguous (pages=None)  [n_layers, slots, n_kv, max_len, head_dim]: slot b owns block b, max_len positions for its whole life;
+      paged (pages=P)          [n_layers, P, n_kv, PAGE, head_dim]: a pool of P pages of PAGE positions (a page id names the same page in
+                               every layer), and block_table [slots, ceil(max_len / PAGE)] int32 on the device: position t of slot b is
+                               row t % PAGE of page block_table[b, t // PAGE], -1 where no page is assigned.  _pages (a PagePool)
+                               holds the host copy; pages are assigned on the host before anything writes their positions.
+    A subclass defines _step (one token of every slot on the current stream: what the graph holds) and reset(), and names itself in
+    CACHE_FULL."""
 
     EXTEND_CHUNK = 2048  # extend() runs a prompt in chunks of at most this many tokens: it bounds the activations of one chunk
     CHECK_EVERY = 8      # generate() looks for EOS every this many steps
 
-    def __init__(self, model, max_len, layers, slots, who):
+    def __init__(self, model, max_len, layers, slots, who, pages=None):
         """After the subclass's device-free checks (layers: _decoder_layout's): the one GPU, the head layout and scale, the stacked
         siblings, then on the device the caches, the attention output, the rotary tables, pos, tok and the sampling buffers."""
         from .quant import quant_cuda
@@ -511,7 +599,14 @@ class _DecoderBase:
         with torch.cuda.device(dev), torch.no_grad():
             self.pos = torch.zeros(slots, dtype=torch.int32, device=dev)
             self.tok = torch.zeros(slots, dtype=torch.int64, device=dev)
-            self._k = torch.zeros(self.n_layers, slots, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
+            if pages is None:
+                self._k = torch.zeros(self.n_layers, slots, self.n_kv, max_len, d, dtype=self.dtype, device=dev)
+                self._pages = None
+            else:
+                width = -(-max_len // PAGE)
+                self._k = torch.zeros(self.n_layers, pages, self.n_kv, PAGE, d, dtype=self.dtype, device=dev)
+                self.block_table = torch.full((slots, width), -1, dtype=torch.int32, device=dev)
+                self._pages = PagePool(pages, slots, width)
             self._v = torch.zeros_like(self._k)
             self.attn_out = torch.zeros(slots, self.n_heads * d, dtype=self.dtype, device=dev)
             self.rope_cos, self.rope_sin = _rope_tables(model, max_len, d, dev)
@@ -548,6 +643,27 @@ class _DecoderBase:
         self.pos[slot] = p
         self._pos[slot] = p
 
+    def _reserve(self, want):
+        """Paged: pages for {slot: (positions, fresh)} - the slot's positions 0 .. positions-1, fresh: none shared with another slot,
+        none kept from before - all or none (RuntimeError naming the slots, nothing changed), and the new entries into block_table.
+        Nothing for a contiguous cache."""
+        if self._pages is None:
+            return
+        held = {b: 0 if f else self._pages.held(b) for b, (n, f) in want.items()}
+        self._pages.reserve({b: (-(-n // PAGE), f) for b, (n, f) in want.items()})
+        for b, (n, f) in want.items():
+            t = self._pages.tables[b]
+            if f:
+                self.block_table[b].fill_(-1)
+            for j in range(held[b], -(-n // PAGE)):
+                self.block_table[b, j] = t[j]
+
+    def _drop_pages(self, slot):
+        """Paged: `slot`'s pages back to the pool and its block_table row to -1."""
+        if self._pages is not None and self._pages.held(slot):
+            self._pages.release(slot)
+            self.block_table[slot].fill_(-1)
+
     def _set_sampling(self, params):
         """Rows 0 .. n-1 of the sampling buffers from _sampling's lists of n values."""
         for buf, vals in zip((self.temperature, self.top_k, self.top_p, self.seed), params):
@@ -580,11 +696,18 @@ class _DecoderBase:
         T = ids.shape[1]
         if not 1 <= T <= self.max_len:
             raise ValueError(f"{who}: {T} prompt tokens, the cache holds 1 to {self.max_len}")
+        self._reserve({slot: (T, True)})
         with torch.no_grad():
             o = self.model(input_ids=ids, use_cache=True)
             for i, layer in enumerate(o.past_key_values.layers):
-                self._k[i, slot, :, :T].copy_(layer.keys[0])
-                self._v[i, slot, :, :T].copy_(layer.values[0])
+                if self._pages is None:
+                    self._k[i, slot, :, :T].copy_(layer.keys[0])
+                    self._v[i, slot, :, :T].copy_(layer.values[0])
+                    continue
+                for j in range(-(-T // PAGE)):
+                    page, n = self._pages.tables[slot][j], min(PAGE, T - j * PAGE)
+                    self._k[i, page, :, :n].copy_(layer.keys[0][:, j * PAGE:j * PAGE + n])
+                    self._v[i, page, :, :n].copy_(layer.values[0][:, j * PAGE:j * PAGE + n])
         self._set_pos(slot, T)
         return o.logits[0, -1]
 
@@ -601,6 +724,7 @@ class _DecoderBase:
         if start + ids.numel() > self.max_len:
             raise ValueError(f"{who}: {ids.numel()} tokens at position {start} need {start + ids.numel()} cache positions, "
                              f"max_len is {self.max_len}")
+        self._reserve({slot: (start + ids.numel(), False)})
         ids = ids.to(device=self.device, dtype=torch.int64)
         m = self.model.model
         with torch.no_grad():
@@ -610,8 +734,12 @@ class _DecoderBase:
                 h = torch.index_select(m.embed_tokens.weight, 0, chunk)
                 for i, layer in enumerate(m.layers):
                     def attend(qkv, i=i):
-                        self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i, slot], self._v[i, slot], out,
-                                             self.n_heads, self.n_kv, self.scale)
+                        if self._pages is None:
+                            self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i, slot], self._v[i, slot], out,
+                                                 self.n_heads, self.n_kv, self.scale)
+                        else:
+                            self._qc.attn_extend_paged(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i], self._v[i],
+                                                       self.block_table[slot], out, self.n_heads, self.n_kv, self.scale)
                         return out
                     h = self._layer(i, layer, h, attend)
             logits = self.model.lm_head(m.norm(h[-1:]))[0]
@@ -619,10 +747,13 @@ class _DecoderBase:
         return logits
 
     def _replay(self):
-        """One step of every active slot; RuntimeError, before it, when an active slot's cache is full."""
+        """One step of every active slot; RuntimeError, before it, when an active slot's cache is full or (paged) when the pool has no
+        page for an active slot whose position starts a new page."""
         full = [b for b, p in enumerate(self._pos) if p >= self.max_len]
         if full:
             raise RuntimeError(self.CACHE_FULL.format(slots=full, max_len=self.max_len))
+        if self._pages is not None:
+            self._reserve({b: (p + 1, False) for b, p in enumerate(self._pos) if p >= 0 and self._pages.held(b) <= p // PAGE})
         self.graph.replay()
         self._pos = [p + 1 if p >= 0 else p for p in self._pos]
 
@@ -967,8 +1098,19 @@ class BatchDecoder(_DecoderBase):
         outs = dec.generate([ids_a, ids_b, ids_c], max_new_tokens=128, eos_token_id=tok.eos_token_id)
         outs = dec.generate([ids_a, ids_b], 128, eos_token_id=tok.eos_token_id, temperature=0.7, top_p=0.9, seed=1)
 
-    Each sequence has a slot: row b of every step, block b of the cache [n_layers, batch, n_kv, max_len, head_dim] and its own device
-    position pos[b], so prompts of different lengths need no padding and no mask.  A slot whose pos is -1 is idle: its row still goes
+    Each sequence has a slot: row b of every step, its own device position pos[b] and its own cache, so prompts of different lengths need
+    no padding and no mask.  The cache has one of two layouts:
+      pages=None  block b of k_cache / v_cache [n_layers, batch, n_kv, max_len, head_dim]: every slot holds max_len positions for its
+                  whole life, idle or not.
+      pages=P     k_cache / v_cache are a pool of P pages of 64 positions, [n_layers, P, n_kv, 64, head_dim], and block_table
+                  [batch, ceil(max_len / 64)] (int32, on the device, -1 where no page is assigned) maps slot b's position t to row t % 64
+                  of page block_table[b, t // 64].  A slot holds pages for the positions it has used: prefill() and extend() assign
+                  the pages of the positions they write, a step assigns one when an active slot's position starts a new page (on the
+                  host, before the replay), and release(), reset() and an EOS in generate() give them back; free_pages counts what is
+                  left.  When the pool runs dry the call raises RuntimeError naming the slots, with nothing run or changed.  fork(src,
+                  dst) starts dst from src's state, sharing src's full pages.  Each row computes the same bits in both layouts.
+
+        dec = BatchDecoder(model, max_len=4096, batch=32, pages=2400)   # 2400 x 64 positions shared by 32 slots  A slot whose pos is -1 is idle: its row still goes
     through the projections, but the attention writes nothing for it, and its logits and token mean nothing.  release() and prefill()
     of a slot between steps while the others keep going is continuous batching.
 
@@ -988,7 +1130,7 @@ class BatchDecoder(_DecoderBase):
 
     CACHE_FULL = "BatchDecoder: the cache of slot(s) {slots} is full (max_len={max_len}); release() or prefill() them first"
 
-    def __init__(self, model, max_len, batch):
+    def __init__(self, model, max_len, batch, pages=None):
         from .quant import QuantLinearLUT
         layers = _decoder_layout(model, max_len, "BatchDecoder")
         dtype = model.model.embed_tokens.weight.dtype
@@ -996,8 +1138,11 @@ class BatchDecoder(_DecoderBase):
         if not isinstance(batch, int) or not 2 <= batch <= rows_max:
             hint = "; decode one sequence with SequenceDecoder" if batch == 1 else ""
             raise ValueError(f"BatchDecoder: batch must be an int in 2..{rows_max} for a {dtype} model (got {batch!r}){hint}")
+        most = batch * -(-max_len // PAGE)
+        if pages is not None and (not isinstance(pages, int) or isinstance(pages, bool) or not 1 <= pages <= most):
+            raise ValueError(f"BatchDecoder: pages must be None or an int in 1..{most} (batch x ceil(max_len / {PAGE})) (got {pages!r})")
         _check_rows_fit(model, layers, "BatchDecoder")
-        super().__init__(model, max_len, layers, batch, "BatchDecoder")
+        super().__init__(model, max_len, layers, batch, "BatchDecoder", pages)
         self.batch = batch
         self.k_cache, self.v_cache = self._k, self._v
         self._capture()
@@ -1008,8 +1153,12 @@ class BatchDecoder(_DecoderBase):
         h = torch.index_select(m.embed_tokens.weight, 0, self.tok)
         for i, layer in enumerate(m.layers):
             def attend(qkv, i=i):
-                self._qc.attn_decode_batch(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i], self.attn_out,
-                                           self.n_heads, self.n_kv, self.scale)
+                if self._pages is None:
+                    self._qc.attn_decode_batch(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i],
+                                               self.attn_out, self.n_heads, self.n_kv, self.scale)
+                else:
+                    self._qc.attn_decode_paged(qkv, self.pos, self.rope_cos, self.rope_sin, self.k_cache[i], self.v_cache[i],
+                                               self.block_table, self.attn_out, self.n_heads, self.n_kv, self.scale)
                 return self.attn_out
             h = self._layer(i, layer, h, attend)
         logits = self.model.lm_head(m.norm(h))
@@ -1026,12 +1175,41 @@ class BatchDecoder(_DecoderBase):
         """Release every slot."""
         self.pos.fill_(-1)
         self._pos = [-1] * self.batch
+        for b in range(self.batch):
+            self._drop_pages(b)
 
     def release(self, slot):
-        """Make `slot` idle (pos -1): the steps write nothing for it from now on; its old cache slots are never read again."""
+        """Make `slot` idle (pos -1): the steps write nothing for it from now on; its old cache slots are never read again (paged: its
+        pages go back to the pool)."""
         self._set_pos(self._slot(slot), -1)
+        self._drop_pages(slot)
 
     _finished = release
+
+    @property
+    def free_pages(self):
+        """Pages left in the pool (paged), None for the contiguous layout."""
+        return None if self._pages is None else self._pages.free
+
+    def fork(self, src, dst):
+        """Start idle slot `dst` from active slot `src`'s current state without recomputing it (n samples of one prompt, one system
+        prompt under several conversations): dst takes src's position; src's full pages before it are shared (writes only go to
+        positions at or past a slot's own, so a shared full page is never written) and its partly filled last page is copied into a
+        fresh page in every layer.  Paged decoders only.  ValueError for bad slots, RuntimeError (nothing changed) without a free page
+        for the copy."""
+        if self._pages is None:
+            raise ValueError("BatchDecoder.fork: needs the paged layout (BatchDecoder(..., pages=P))")
+        src, dst = self._slot(src), self._slot(dst)
+        if self._pos[src] < 0 or self._pos[dst] >= 0 or src == dst:
+            raise ValueError(f"BatchDecoder.fork: src must be active and dst idle (positions {self._pos[src]} and {self._pos[dst]})")
+        p = self._pos[src]
+        copy = self._pages.fork(src, dst, p)
+        with torch.no_grad():
+            if copy is not None:
+                self._k[:, copy[1]].copy_(self._k[:, copy[0]])
+                self._v[:, copy[1]].copy_(self._v[:, copy[0]])
+            self.block_table[dst].copy_(torch.tensor(self._pages.tables[dst], dtype=torch.int32))
+        self._set_pos(dst, p)
 
     @property
     def positions(self):
