@@ -9,6 +9,7 @@
 
 #include <map>
 #include <tuple>
+#include <type_traits>
 
 #include "attn_decode.cuh"
 #include "attn_extend.cuh"
@@ -19,22 +20,55 @@ using namespace sqllm;
 
 namespace {
 
-template <typename T, int D, bool BATCH>
-KernelSmem attn_kernel_of(int G) {
-    if (BATCH) {
-        switch (G) {
-            case 1: return {attn::attn_decode_batch_kernel<T, D, 1>, 0};
-            case 2: return {attn::attn_decode_batch_kernel<T, D, 2>, 0};
-            case 4: return {attn::attn_decode_batch_kernel<T, D, 4>, 0};
-            default: return {attn::attn_decode_batch_kernel<T, D, 8>, 0};
-        }
+// The kernel templates, one tag each: Tag::of<T, D, G>() is the instance for dtype T, head_dim D and G rows per CTA (the chunk kernels
+// have no G and ignore it).
+struct Decode {
+    template <typename T, int D, int G> static auto of() { return attn::attn_decode_kernel<T, D, G>; }
+};
+struct DecodeBatch {
+    template <typename T, int D, int G> static auto of() { return attn::attn_decode_batch_kernel<T, D, G>; }
+};
+struct DecodePaged {
+    template <typename T, int D, int G> static auto of() { return attn::attn_decode_paged_kernel<T, D, G>; }
+};
+struct Verify {
+    template <typename T, int D, int G> static auto of() { return attn::attn_verify_kernel<T, D, G>; }
+};
+template <typename P> struct Extend {
+    template <typename T, int D, int> static auto of() {
+        if constexpr (attn::is_paged<P>) return attn::attn_extend_paged_kernel<T, D>;
+        else return attn::attn_extend_kernel<T, D>;
     }
+};
+template <typename P> struct Append {
+    template <typename T, int D, int> static auto of() {
+        if constexpr (attn::is_paged<P>) return attn::attn_append_paged_kernel<T, D>;
+        else return attn::attn_append_kernel<T, D>;
+    }
+};
+
+template <typename K, typename T, int D>
+auto instance_g(int G) {
     switch (G) {
-        case 1: return {attn::attn_decode_kernel<T, D, 1>, 0};
-        case 2: return {attn::attn_decode_kernel<T, D, 2>, 0};
-        case 4: return {attn::attn_decode_kernel<T, D, 4>, 0};
-        default: return {attn::attn_decode_kernel<T, D, 8>, 0};
+        case 1: return K::template of<T, D, 1>();
+        case 2: return K::template of<T, D, 2>();
+        case 4: return K::template of<T, D, 4>();
+        default: return K::template of<T, D, 8>();
     }
+}
+
+// the instance of kernel template K for a launch's dtype (SQLLM_DT_F16 or SQLLM_DT_BF16), head_dim (64 or 128) and G (group_of)
+template <typename K>
+auto instance(int dtype, int head_dim, int G = 1) {
+    const bool bf = dtype == SQLLM_DT_BF16;
+    return head_dim == 128 ? (bf ? instance_g<K, __nv_bfloat16, 128>(G) : instance_g<K, __half, 128>(G))
+                           : (bf ? instance_g<K, __nv_bfloat16, 64>(G) : instance_g<K, __half, 64>(G));
+}
+
+// G of a CTA of `rows` query rows: rows, at most GMAX, rounded up to the instances' 1, 2, 4 or 8
+int group_of(int rows) {
+    rows = std::min(rows, attn::GMAX);
+    return rows <= 1 ? 1 : rows <= 2 ? 2 : rows <= 4 ? 4 : 8;
 }
 
 bool aligned16(const void *ptr) { return ptr && !(reinterpret_cast<uintptr_t>(ptr) & 15); }
@@ -75,48 +109,6 @@ int splits(int n_heads, int n_kv, int batch, int sm_count) {
     return (int)std::max(1LL, std::min((long long)attn::MAX_CLUSTER, sm_count / clusters));
 }
 
-// the checks and the launch of both entry points; `batch` sequences (the batch-1 entry: 1, on the batch-1 kernel)
-template <bool BATCH, typename Args>
-int attn_launch(const Args *a, int batch, void *stream) {
-    if (int rc = check_dtype(a->dtype)) return rc;
-    if (BATCH && (batch < 1 || batch > MAX_BATCH)) return fail(SQLLM_EINVAL, "batch=%d must be in [1, %d]", batch, MAX_BATCH);
-    if (int rc = check_heads(a)) return rc;
-    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"},
-                             {a->k_cache, "k_cache"}, {a->v_cache, "v_cache"}, {a->out, "out"}}))
-        return rc;
-    const int g = a->n_heads / a->n_kv, gc = std::min(g, attn::GMAX);
-    const int G = gc <= 1 ? 1 : gc <= 2 ? 2 : gc <= 4 ? 4 : 8;
-    const bool bf = a->dtype == SQLLM_DT_BF16;
-    const KernelSmem k = a->head_dim == 128
-                             ? (bf ? attn_kernel_of<__nv_bfloat16, 128, BATCH>(G) : attn_kernel_of<__half, 128, BATCH>(G))
-                             : (bf ? attn_kernel_of<__nv_bfloat16, 64, BATCH>(G) : attn_kernel_of<__half, 64, BATCH>(G));
-    int sm = 0;
-    int rc = dev_setup({}, &sm);
-    if (rc) return rc;
-    attn::Params p;
-    p.qkv = a->qkv; p.pos = a->pos; p.cos = a->rope_cos; p.sin = a->rope_sin;
-    p.k_cache = a->k_cache; p.v_cache = a->v_cache; p.out = a->out;
-    p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = g; p.hchunks = (g + attn::GMAX - 1) / attn::GMAX; p.capacity = a->capacity;
-    p.qscale = a->scale * attn::LOG2E;
-    const int S = splits(a->n_heads, a->n_kv, batch, sm);
-    const dim3 grid(S, a->n_kv * p.hchunks, batch);
-    const cudaError_t e = launch_ex(reinterpret_cast<void (*)(attn::Params)>(const_cast<void *>(k.fn)), grid, attn::THREADS, 0,
-                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
-    if (e != cudaSuccess)
-        return fail(SQLLM_ECUDA, "%s launch failed: %s", BATCH ? "attn_decode_batch" : "attn_decode", cudaGetErrorString(e));
-    return SQLLM_OK;
-}
-
-template <typename T, int D>
-void *paged_kernel_of(int G) {
-    switch (G) {
-        case 1: return (void *)attn::attn_decode_paged_kernel<T, D, 1>;
-        case 2: return (void *)attn::attn_decode_paged_kernel<T, D, 2>;
-        case 4: return (void *)attn::attn_decode_paged_kernel<T, D, 4>;
-        default: return (void *)attn::attn_decode_paged_kernel<T, D, 8>;
-    }
-}
-
 // the checks of the page arguments both paged entry points share, after check_heads: the pool size, the table width against capacity,
 // the pointers of the pools and the table
 template <typename Args>
@@ -131,45 +123,42 @@ int check_pages(const Args *a) {
     return SQLLM_OK;
 }
 
-int paged_launch(const sqllm_attn_decode_paged_args *a, void *stream) {
+// the checks and the launch of sqllm_attn_decode (P = Params, one sequence on the batch-1 kernel), sqllm_attn_decode_batch (Params,
+// BATCH: `batch` sequences) and sqllm_attn_decode_paged (PagedParams, BATCH)
+template <typename P, bool BATCH, typename Args>
+int attn_launch(const Args *a, int batch, void *stream) {
+    constexpr bool PAGED = std::is_same<P, attn::PagedParams>::value;
+    using K = std::conditional_t<PAGED, DecodePaged, std::conditional_t<BATCH, DecodeBatch, Decode>>;
     if (int rc = check_dtype(a->dtype)) return rc;
-    if (a->batch < 1 || a->batch > MAX_BATCH) return fail(SQLLM_EINVAL, "batch=%d must be in [1, %d]", a->batch, MAX_BATCH);
+    if (BATCH && (batch < 1 || batch > MAX_BATCH)) return fail(SQLLM_EINVAL, "batch=%d must be in [1, %d]", batch, MAX_BATCH);
     if (int rc = check_heads(a)) return rc;
-    if (int rc = check_pages(a)) return rc;
-    if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->out, "out"}}))
-        return rc;
-    const int g = a->n_heads / a->n_kv, gc = std::min(g, attn::GMAX);
-    const int G = gc <= 1 ? 1 : gc <= 2 ? 2 : gc <= 4 ? 4 : 8;
-    const bool bf = a->dtype == SQLLM_DT_BF16;
-    void *fn = a->head_dim == 128 ? (bf ? paged_kernel_of<__nv_bfloat16, 128>(G) : paged_kernel_of<__half, 128>(G))
-                                  : (bf ? paged_kernel_of<__nv_bfloat16, 64>(G) : paged_kernel_of<__half, 64>(G));
+    P p;
+    if constexpr (PAGED) {
+        if (int rc = check_pages(a)) return rc;
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->out, "out"}}))
+            return rc;
+        p.k_cache = a->k_pages; p.v_cache = a->v_pages; p.table = a->block_table; p.width = a->table_width; p.n_pages = a->n_pages;
+    } else {
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"},
+                                 {a->k_cache, "k_cache"}, {a->v_cache, "v_cache"}, {a->out, "out"}}))
+            return rc;
+        p.k_cache = a->k_cache; p.v_cache = a->v_cache;
+    }
+    const int g = a->n_heads / a->n_kv;
+    const auto fn = instance<K>(a->dtype, a->head_dim, group_of(g));
     int sm = 0;
     int rc = dev_setup({}, &sm);
     if (rc) return rc;
-    attn::PagedParams p;
-    p.qkv = a->qkv; p.pos = a->pos; p.cos = a->rope_cos; p.sin = a->rope_sin;
-    p.k_cache = a->k_pages; p.v_cache = a->v_pages; p.out = a->out;
+    p.qkv = a->qkv; p.pos = a->pos; p.cos = a->rope_cos; p.sin = a->rope_sin; p.out = a->out;
     p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = g; p.hchunks = (g + attn::GMAX - 1) / attn::GMAX; p.capacity = a->capacity;
     p.qscale = a->scale * attn::LOG2E;
-    p.table = a->block_table; p.width = a->table_width; p.n_pages = a->n_pages;
-    const int S = splits(a->n_heads, a->n_kv, a->batch, sm);   // the rule of sqllm_attn_decode_batch: the same bits per row
-    const dim3 grid(S, a->n_kv * p.hchunks, a->batch);
-    const cudaError_t e = launch_ex(reinterpret_cast<void (*)(attn::PagedParams)>(fn), grid, attn::THREADS, 0,
-                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
-    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_decode_paged launch failed: %s", cudaGetErrorString(e));
+    const int S = splits(a->n_heads, a->n_kv, batch, sm);   // the paged kernel: the rule of sqllm_attn_decode_batch, the same bits per row
+    const dim3 grid(S, a->n_kv * p.hchunks, batch);
+    const cudaError_t e = launch_ex(fn, grid, attn::THREADS, 0, static_cast<cudaStream_t>(stream), cluster_of(S), p);
+    if (e != cudaSuccess)
+        return fail(SQLLM_ECUDA, "%s launch failed: %s", PAGED ? "attn_decode_paged" : BATCH ? "attn_decode_batch" : "attn_decode",
+                    cudaGetErrorString(e));
     return SQLLM_OK;
-}
-
-template <typename T, int D, typename P>
-KernelSmem extend_kernel_of() {
-    if constexpr (attn::is_paged<P>) return {attn::attn_extend_paged_kernel<T, D>, attn::ext_smem_bytes(D)};
-    else return {attn::attn_extend_kernel<T, D>, attn::ext_smem_bytes(D)};
-}
-
-template <typename T, int D, typename P>
-auto append_kernel_of() {
-    if constexpr (attn::is_paged<P>) return attn::attn_append_paged_kernel<T, D>;
-    else return attn::attn_append_kernel<T, D>;
 }
 
 // the rows of the chunk's query tiles (T tokens x g heads of a group), 0 when they need more tiles than the grid holds
@@ -212,37 +201,25 @@ int extend_launch(const Args *a, void *stream) {
             return rc;
         p.k_cache = a->k_cache; p.v_cache = a->v_cache;
     }
-    const bool bf = a->dtype == SQLLM_DT_BF16;
-    const KernelSmem k = a->head_dim == 128 ? (bf ? extend_kernel_of<__nv_bfloat16, 128, P>() : extend_kernel_of<__half, 128, P>())
-                                            : (bf ? extend_kernel_of<__nv_bfloat16, 64, P>() : extend_kernel_of<__half, 64, P>());
+    const auto fn = instance<Extend<P>>(a->dtype, a->head_dim);
+    const int bytes = attn::ext_smem_bytes(a->head_dim);
     int sm = 0;
-    int rc = dev_setup({k}, &sm);
+    int rc = dev_setup({KernelSmem(fn, bytes)}, &sm);
     if (rc) return rc;
     p.qkv = a->qkv; p.cos = a->rope_cos; p.sin = a->rope_sin; p.out = a->out;
     p.n_heads = a->n_heads; p.n_kv = a->n_kv; p.g = a->n_heads / a->n_kv; p.capacity = a->capacity; p.start = a->start; p.T = a->n_tokens;
     p.qscale = a->scale * attn::LOG2E / attn::QPRE;
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    void (*append)(P) = a->head_dim == 128 ? (bf ? append_kernel_of<__nv_bfloat16, 128, P>() : append_kernel_of<__half, 128, P>())
-                                           : (bf ? append_kernel_of<__nv_bfloat16, 64, P>() : append_kernel_of<__half, 64, P>());
+    const auto append = instance<Append<P>>(a->dtype, a->head_dim);
     const char *name = PAGED ? "attn_extend_paged" : "attn_extend";
     append<<<a->n_tokens, attn::APPEND_THREADS, 0, st>>>(p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s append launch failed: %s", name, cudaGetErrorString(e));
     const int S = ext_splits(a->n_heads, a->n_kv, a->n_tokens, a->start, sm);
     const dim3 grid(S, (unsigned)ext_tiles(a->n_heads, a->n_kv, a->n_tokens), a->n_kv);
-    e = launch_ex(reinterpret_cast<void (*)(P)>(const_cast<void *>(k.fn)), grid, attn::XTHREADS, k.bytes, st, cluster_of(S), p);
+    e = launch_ex(fn, grid, attn::XTHREADS, bytes, st, cluster_of(S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
     return SQLLM_OK;
-}
-
-template <typename T, int D>
-KernelSmem verify_kernel_of(int G) {
-    switch (G) {
-        case 1: return {attn::attn_verify_kernel<T, D, 1>, 0};
-        case 2: return {attn::attn_verify_kernel<T, D, 2>, 0};
-        case 4: return {attn::attn_verify_kernel<T, D, 4>, 0};
-        default: return {attn::attn_verify_kernel<T, D, 8>, 0};
-    }
 }
 
 // clusters per KV head of sqllm_attn_verify: chunks of GMAX of the T * g (token, query head) rows of its group
@@ -269,13 +246,9 @@ int ver_check(const Args *a) {
     return SQLLM_OK;
 }
 
-// the kernel instance of a verify launch: G, the rows per CTA, is min(T g, GMAX) rounded up to a power of two
-KernelSmem ver_kernel(int n_heads, int n_kv, int T, int head_dim, int dtype) {
-    const int rows = std::min(T * (n_heads / n_kv), attn::GMAX);
-    const int G = rows <= 1 ? 1 : rows <= 2 ? 2 : rows <= 4 ? 4 : 8;
-    const bool bf = dtype == SQLLM_DT_BF16;
-    return head_dim == 128 ? (bf ? verify_kernel_of<__nv_bfloat16, 128>(G) : verify_kernel_of<__half, 128>(G))
-                           : (bf ? verify_kernel_of<__nv_bfloat16, 64>(G) : verify_kernel_of<__half, 64>(G));
+// the kernel instance of a verify launch: a CTA's rows are T g, at most GMAX
+auto ver_kernel(int n_heads, int n_kv, int T, int head_dim, int dtype) {
+    return instance<Verify>(dtype, head_dim, group_of(T * (n_heads / n_kv)));
 }
 
 // The CTAs per cluster a verify launch of `clusters` clusters of kernel `fn` uses on the current device: the rule's S, lowered until
@@ -315,7 +288,7 @@ int verify_launch(const sqllm_attn_verify_args *a, void *stream) {
     if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->pos, "pos"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"},
                              {a->k_cache, "k_cache"}, {a->v_cache, "v_cache"}, {a->out, "out"}}))
         return rc;
-    const KernelSmem k = ver_kernel(a->n_heads, a->n_kv, a->n_tokens, a->head_dim, a->dtype);
+    const auto fn = ver_kernel(a->n_heads, a->n_kv, a->n_tokens, a->head_dim, a->dtype);
     int sm = 0;
     int rc = dev_setup({}, &sm);
     if (rc) return rc;
@@ -326,10 +299,10 @@ int verify_launch(const sqllm_attn_verify_args *a, void *stream) {
     p.capacity = a->capacity; p.T = a->n_tokens;
     p.qscale = a->scale * attn::LOG2E;
     int S = 0;
-    if ((rc = ver_launch_splits(k.fn, ver_splits(a->n_heads, a->n_kv, a->n_tokens, sm), (long long)a->n_kv * p.chunks, &S))) return rc;
+    if ((rc = ver_launch_splits((const void *)fn, ver_splits(a->n_heads, a->n_kv, a->n_tokens, sm), (long long)a->n_kv * p.chunks, &S)))
+        return rc;
     const dim3 grid(S, a->n_kv * p.chunks);
-    const cudaError_t e = launch_ex(reinterpret_cast<void (*)(attn::VerParams)>(const_cast<void *>(k.fn)), grid, attn::THREADS, 0,
-                                    static_cast<cudaStream_t>(stream), cluster_of(S), p);
+    const cudaError_t e = launch_ex(fn, grid, attn::THREADS, 0, static_cast<cudaStream_t>(stream), cluster_of(S), p);
     if (e != cudaSuccess) return fail(SQLLM_ECUDA, "attn_verify launch failed: %s", cudaGetErrorString(e));
     return SQLLM_OK;
 }
@@ -344,12 +317,12 @@ int sqllm_attn_decode_batch_splits(int n_heads, int n_kv, int batch, int sm_coun
 
 int sqllm_attn_decode(const sqllm_attn_decode_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
-    return attn_launch<false>(a, 1, stream);
+    return attn_launch<attn::Params, false>(a, 1, stream);
 }
 
 int sqllm_attn_decode_batch(const sqllm_attn_decode_batch_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
-    return attn_launch<true>(a, a->batch, stream);
+    return attn_launch<attn::Params, true>(a, a->batch, stream);
 }
 
 int sqllm_attn_extend_splits(int n_heads, int n_kv, int n_tokens, int start, int sm_count) {
@@ -363,7 +336,7 @@ int sqllm_attn_extend(const sqllm_attn_extend_args *a, void *stream) {
 
 int sqllm_attn_decode_paged(const sqllm_attn_decode_paged_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
-    return paged_launch(a, stream);
+    return attn_launch<attn::PagedParams, true>(a, a->batch, stream);
 }
 
 int sqllm_attn_extend_paged(const sqllm_attn_extend_paged_args *a, void *stream) {
@@ -378,7 +351,7 @@ int sqllm_attn_verify_launch_splits(int dtype, int n_heads, int n_kv, int head_d
     if (ver_check(&a)) return 0;
     int sm = 0, S = 0;
     if (dev_setup({}, &sm)) return 0;
-    if (ver_launch_splits(ver_kernel(n_heads, n_kv, n_tokens, head_dim, dtype).fn, ver_splits(n_heads, n_kv, n_tokens, sm),
+    if (ver_launch_splits((const void *)ver_kernel(n_heads, n_kv, n_tokens, head_dim, dtype), ver_splits(n_heads, n_kv, n_tokens, sm),
                           (long long)n_kv * ver_chunks(n_heads, n_kv, n_tokens), &S))
         return 0;
     return S;

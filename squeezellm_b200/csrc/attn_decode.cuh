@@ -104,6 +104,15 @@ __device__ __forceinline__ void unpack8(const uint4 w, float (&f)[8]) {
 // exp2(a - b) with exp2(-inf) = 0 whatever b is (an empty state or a masked position weighs nothing)
 __device__ __forceinline__ float wexp2(float a, float b) { return a == -INFINITY ? 0.f : exp2f(a - b); }
 
+// rotary (rotate-half) in fp32: element i of the rotated x, from the pair (a, b) = (x[j], x[j + D/2]) and the row (cs, sn) of the
+// cos / sin tables at x's position, j = i % (D/2).  Every kernel rotates q and k with this one expression, so a cache slot holds the
+// same bits whichever kernel wrote it (decode, batched, paged, verify or append), and q' is the same whichever kernel attends with it.
+template <int D>
+__device__ __forceinline__ float rope(float a, float b, const float *cs, const float *sn, int i) {
+    const int j = i % (D / 2);
+    return i < D / 2 ? a * cs[j] - b * sn[j] : b * cs[j] + a * sn[j];
+}
+
 // batch 1: one sequence at *p.pos.  Kept beside the batched kernel, which computes the same bits at batch 1 but up to 0.9 % slower
 // (DESIGN §3.18)
 template <typename T, int D, int G>

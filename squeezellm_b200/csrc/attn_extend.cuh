@@ -2,8 +2,8 @@
 // (sqllm_attn_extend): the append of the chunk's rotated k and its v at slots start .. start+T-1 of the KV cache, then causal
 // softmax(scale q'.K^T[0..p]) V[0..p] for every token (p = start + t) and query head, with grouped KV heads.  Two launches on one stream:
 //
-//   attn_append_kernel   one CTA per token: k' = rotary(k) in fp32 rounded to the dtype once - the expression of attn_decode_row.inc,
-//                        so a slot holds the same bits whichever kernel wrote it - and v unchanged.
+//   attn_append_kernel   one CTA per token: k' = rotary(k) in fp32 rounded to the dtype once - rope() of attn_decode.cuh, so a slot
+//                        holds the same bits whichever kernel wrote it - and v unchanged.
 //   attn_extend_kernel   FlashAttention-2 style, K / V read from the cache only (so no CTA reads a slot written in the same launch).
 //
 // Shape of attn_extend_kernel.  A query tile is BM = 64 (token, query head) rows of one KV head's group, token-major (row r of the
@@ -123,7 +123,7 @@ __device__ __forceinline__ void append_body(const P &p) {
         size_t slot;
         if constexpr (is_paged<P>) slot = page_base<D>(p.table[pos / PAGE], p.n_kv, kvh) + (size_t)(pos % PAGE) * D + i;
         else slot = ((size_t)kvh * p.capacity + pos) * D + i;
-        static_cast<T *>(p.k_cache)[slot] = f32_to<T>(i < D / 2 ? a * cs[j] - b * sn[j] : b * cs[j] + a * sn[j]);
+        static_cast<T *>(p.k_cache)[slot] = f32_to<T>(rope<D>(a, b, cs, sn, i));
         static_cast<T *>(p.v_cache)[slot] = qkv[(size_t)(p.n_heads + p.n_kv) * D + (size_t)kvh * D + i];
     }
 }

@@ -5,11 +5,11 @@
 // (KV head, chunk of up to GMAX rows), so every K / V row a CTA loads serves all the rows of its chunk: at g = 1 and T = 8 one chunk per
 // KV head, the K / V bytes of one decode call.  The positions 0 .. pos+T-1 are dealt to the S CTAs in blocks of BLOCK_POS (cta_range),
 // and inside a CTA to its warps exactly as in the decode kernel.  Row r's own causal limit pos + r/g masks only positions of the last
-// T, which lie in the last block.  Every CTA computes the T rotated k' (rounded to the dtype once, the expression of attn_decode_row.inc)
-// and the T v into shared memory, takes positions >= pos from there and reads the cache only below pos; one CTA per KV head stores
-// them.  So no CTA reads a slot written in the same launch, and no slot at or past pos + T is read.  Partial states are combined as in
-// the decode kernel: row slots by an xor tree, warps in warp order, CTAs in rank order over distributed shared memory.  No workspace, no
-// atomics: bit-reproducible.  A position range outside the cache (pos < 0 or pos + T > capacity) writes nothing.
+// T, which lie in the last block.  Every CTA computes the T rotated k' (rounded to the dtype once, rope() of attn_decode.cuh) and the
+// T v into shared memory, takes positions >= pos from there and reads the cache only below pos; one CTA per KV head stores them.  So
+// no CTA reads a slot written in the same launch, and no slot at or past pos + T is read.  Partial states are combined by the decode
+// kernel's text (attn_combine.inc): row slots by an xor tree, warps in warp order, CTAs in rank order over distributed shared memory.
+// No workspace, no atomics: bit-reproducible.  A position range outside the cache (pos < 0 or pos + T > capacity) writes nothing.
 #pragma once
 #include "attn_decode.cuh"
 
@@ -48,6 +48,11 @@ __global__ void __launch_bounds__(THREADS, 1) attn_verify_kernel(const VerParams
     const int kvh = blockIdx.y / p.chunks, ch = blockIdx.y % p.chunks;
     const int r0 = ch * GMAX;                           // first (token, head) row of this CTA in the group's T*g rows
     const int gc = min(GMAX, p.T * p.g - r0);           // rows of this CTA (<= G)
+    T *const out = static_cast<T *>(p.out);
+    const auto store_out = [&](int h, int i, float v) {  // for attn_combine.inc: row h is token t's query head `head`
+        const int t = (r0 + h) / p.g, head = kvh * p.g + (r0 + h) % p.g;
+        out[(size_t)t * p.n_heads * D + (size_t)head * D + i] = f32_to<T>(v);
+    };
     const size_t row_elems = (size_t)(p.n_heads + 2 * p.n_kv) * D;
     const T *qkv = static_cast<const T *>(p.qkv);
 
@@ -61,7 +66,7 @@ __global__ void __launch_bounds__(THREADS, 1) attn_verify_kernel(const VerParams
             const float *cs = p.cos + (size_t)(pos + t) * (D / 2), *sn = p.sin + (size_t)(pos + t) * (D / 2);
             const T *q = qkv + t * row_elems + (size_t)h * D;
             const float a = to_f32(q[j]), b = to_f32(q[j + D / 2]);
-            v = (i < D / 2 ? a * cs[j] - b * sn[j] : b * cs[j] + a * sn[j]) * p.qscale;
+            v = rope<D>(a, b, cs, sn, i) * p.qscale;
         }
         qc[r][i] = v;
     }
@@ -70,7 +75,7 @@ __global__ void __launch_bounds__(THREADS, 1) attn_verify_kernel(const VerParams
         const float *cs = p.cos + (size_t)(pos + t) * (D / 2), *sn = p.sin + (size_t)(pos + t) * (D / 2);
         const T *k = qkv + t * row_elems + (size_t)p.n_heads * D + (size_t)kvh * D;
         const float a = to_f32(k[j]), b = to_f32(k[j + D / 2]);
-        knew[t][i] = f32_to<T>(i < D / 2 ? a * cs[j] - b * sn[j] : b * cs[j] + a * sn[j]);
+        knew[t][i] = f32_to<T>(rope<D>(a, b, cs, sn, i));
         vnew[t][i] = qkv[t * row_elems + (size_t)(p.n_heads + p.n_kv) * D + (size_t)kvh * D + i];
     }
     __syncthreads();
@@ -160,71 +165,8 @@ __global__ void __launch_bounds__(THREADS, 1) attn_verify_kernel(const VerParams
         }
     }
 
-    // the row slots of the warp: xor tree over the lanes LPR apart
-#pragma unroll
-    for (int o = LPR; o < 32; o <<= 1) {
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-            const float mo = __shfl_xor_sync(0xffffffffu, m[h], o), lo = __shfl_xor_sync(0xffffffffu, l[h], o);
-            const float mx = fmaxf(m[h], mo);
-            const float a = wexp2(m[h], mx), b = wexp2(mo, mx);
-            l[h] = l[h] * a + lo * b;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float ao = __shfl_xor_sync(0xffffffffu, acc[h][j], o);
-                acc[h][j] = acc[h][j] * a + ao * b;
-            }
-            m[h] = mx;
-        }
-    }
-    if (sub == 0) {
-#pragma unroll
-        for (int h = 0; h < G; ++h) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) wacc[warp][h][e + j] = acc[h][j];
-            if (lane == 0) { wm[warp][h] = m[h]; wl[warp][h] = l[h]; }
-        }
-    }
-    __syncthreads();
-    // the warps of the CTA, in warp order (into qc: every warp read its q' before the barrier above)
-    for (int idx = tid; idx < G * D; idx += THREADS) {
-        const int h = idx / D, i = idx % D;
-        float mx = -INFINITY;
-#pragma unroll
-        for (int w = 0; w < WARPS; ++w) mx = fmaxf(mx, wm[w][h]);
-        float L = 0.f, A = 0.f;
-#pragma unroll
-        for (int w = 0; w < WARPS; ++w) {
-            const float c = wexp2(wm[w][h], mx);
-            L += wl[w][h] * c;
-            A += wacc[w][h][i] * c;
-        }
-        qc[h][i] = A;
-        if (i == 0) { cm[h] = mx; cl[h] = L; }
-    }
-    asm volatile("barrier.cluster.arrive.release;\nbarrier.cluster.wait.acquire;" ::: "memory");
-    // the CTAs of the cluster, in rank order; CTA r finishes the outputs r, r + S*THREADS, ... of its rows
-    T *out = static_cast<T *>(p.out);
-    for (int idx = rank * THREADS + tid; idx < gc * D; idx += S * THREADS) {
-        const int h = idx / D, i = idx % D;
-        float mr[MAX_CLUSTER], mx = -INFINITY;
-#pragma unroll
-        for (int r = 0; r < MAX_CLUSTER; ++r) {
-            if (r < S) { mr[r] = ld_cluster_f32(&cm[h], r); mx = fmaxf(mx, mr[r]); }
-        }
-        float L = 0.f, A = 0.f;
-#pragma unroll
-        for (int r = 0; r < MAX_CLUSTER; ++r) {
-            if (r < S) {
-                const float c = wexp2(mr[r], mx);
-                L += ld_cluster_f32(&cl[h], r) * c;
-                A += ld_cluster_f32(&qc[h][i], r) * c;
-            }
-        }
-        const int t = (r0 + h) / p.g, head = kvh * p.g + (r0 + h) % p.g;
-        out[(size_t)t * p.n_heads * D + (size_t)head * D + i] = f32_to<T>(A / L);
-    }
-    asm volatile("barrier.cluster.arrive.relaxed;\nbarrier.cluster.wait;" ::: "memory");  // the peers' partials stay alive until read
+    float (&cacc)[G][D] = qc;  // the CTA's combined sums go to qc: every warp read its q' into registers before the combine's barrier
+#include "attn_combine.inc"
 }
 
 }  // namespace attn

@@ -679,6 +679,35 @@ Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::
     return a;
 }
 
+// The own shape checks of attn_decode_batch and attn_decode_paged (attn_args' `own`), messages prefixed with `fn`: qkv [batch,
+// (n_heads + 2 n_kv) head_dim], out [batch, n_heads head_dim], pos int32 [batch].
+auto batch_shapes(const char *fn, const torch::Tensor &qkv, const torch::Tensor &pos, const torch::Tensor &out, int64_t n_heads,
+                  int64_t n_kv) {
+    return [=, &qkv, &pos, &out](int64_t B, int64_t, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, fn, ": qkv must be [batch=", B,
+                    ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, fn, ": out must be [batch=", B,
+                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
+        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, fn, ": pos must be int32 [batch=", B,
+                    "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
+    };
+}
+
+// The own shape checks of attn_extend and attn_extend_paged, messages prefixed with `fn`: qkv [T >= 1, (n_heads + 2 n_kv) head_dim],
+// start + T <= capacity, out [T, n_heads head_dim].
+auto chunk_shapes(const char *fn, const torch::Tensor &qkv, int64_t start, const torch::Tensor &out, int64_t n_heads, int64_t n_kv) {
+    return [=, &qkv, &out](int64_t, int64_t cap, int64_t d) {
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, fn, ": qkv must be [T, (n_heads + 2 n_kv) head_dim=",
+                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        const int64_t T = qkv.size(0);
+        TORCH_CHECK(T >= 1, fn, ": qkv has no rows (T=0)");
+        TORCH_CHECK(start >= 0, fn, ": start=", start, " must be >= 0");
+        TORCH_CHECK(start + T <= cap, fn, ": start=", start, " + T=", T, " must be <= capacity=", cap);
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, fn, ": out must be [T=", T, ", n_heads head_dim=",
+                    n_heads * d, "] (got ", out.sizes(), ")");
+    };
+}
+
 // One layer's decode attention (sqllm_attn_decode): rotary, the append of k / v at slot *pos of the caches, attention over slots
 // 0..*pos into out, on the current stream.
 void attn_decode(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
@@ -700,14 +729,7 @@ void attn_decode(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, t
 void attn_decode_batch(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
                        torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
     auto a = attn_args<sqllm_attn_decode_batch_args>("attn_decode_batch", 1, qkv, &pos, rope_cos, rope_sin, k_cache, v_cache, out, n_heads,
-                                                     n_kv, scale, [&](int64_t B, int64_t, int64_t d) {
-        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_decode_batch: qkv must be [batch=", B,
-                    ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-        TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, "attn_decode_batch: out must be [batch=", B,
-                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
-        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, "attn_decode_batch: pos must be int32 [batch=", B,
-                    "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
-    });
+                                                     n_kv, scale, batch_shapes("attn_decode_batch", qkv, pos, out, n_heads, n_kv));
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.batch = (int)k_cache.size(0);
     a.pos = pos.data_ptr<int32_t>();
@@ -720,16 +742,7 @@ void attn_decode_batch(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_
 void attn_extend(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache,
                  torch::Tensor v_cache, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
     auto a = attn_args<sqllm_attn_extend_args>("attn_extend", 0, qkv, nullptr, rope_cos, rope_sin, k_cache, v_cache, out, n_heads, n_kv, scale,
-                                               [&](int64_t, int64_t cap, int64_t d) {
-        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
-                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-        const int64_t T = qkv.size(0);
-        TORCH_CHECK(T >= 1, "attn_extend: qkv has no rows (T=0)");
-        TORCH_CHECK(start >= 0, "attn_extend: start=", start, " must be >= 0");
-        TORCH_CHECK(start + T <= cap, "attn_extend: start=", start, " + T=", T, " must be <= capacity=", cap);
-        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend: out must be [T=", T, ", n_heads head_dim=",
-                    n_heads * d, "] (got ", out.sizes(), ")");
-    });
+                                               chunk_shapes("attn_extend", qkv, start, out, n_heads, n_kv));
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.start = (int)start; a.n_tokens = (int)qkv.size(0);
     check_status(sqllm_attn_extend(&a, cur_stream()), "quant_cuda.attn_extend");
@@ -761,14 +774,8 @@ void attn_verify(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, t
 void attn_decode_paged(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_pages,
                        torch::Tensor v_pages, torch::Tensor block_table, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
     auto a = attn_args<sqllm_attn_decode_paged_args>("attn_decode_paged", 1, qkv, &pos, rope_cos, rope_sin, k_pages, v_pages, out, n_heads,
-                                                     n_kv, scale, [&](int64_t B, int64_t, int64_t d) {
-        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == B && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_decode_paged: qkv must be [batch=", B,
-                    ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-        TORCH_CHECK(out.dim() == 2 && out.size(0) == B && out.size(1) == n_heads * d, "attn_decode_paged: out must be [batch=", B,
-                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
-        TORCH_CHECK(pos.scalar_type() == torch::kInt32 && pos.dim() == 1 && pos.size(0) == B, "attn_decode_paged: pos must be int32 [batch=", B,
-                    "] (got ", pos.scalar_type(), " ", pos.sizes(), ")");
-    }, &block_table);
+                                                     n_kv, scale, batch_shapes("attn_decode_paged", qkv, pos, out, n_heads, n_kv),
+                                                     &block_table);
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.batch = (int)block_table.size(0);
     a.pos = pos.data_ptr<int32_t>();
@@ -779,16 +786,8 @@ void attn_decode_paged(torch::Tensor qkv, torch::Tensor pos, torch::Tensor rope_
 void attn_extend_paged(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_pages,
                        torch::Tensor v_pages, torch::Tensor block_table_row, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
     auto a = attn_args<sqllm_attn_extend_paged_args>("attn_extend_paged", 0, qkv, nullptr, rope_cos, rope_sin, k_pages, v_pages, out, n_heads,
-                                                     n_kv, scale, [&](int64_t, int64_t cap, int64_t d) {
-        TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == (n_heads + 2 * n_kv) * d, "attn_extend_paged: qkv must be [T, (n_heads + 2 n_kv) head_dim=",
-                    (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
-        const int64_t T = qkv.size(0);
-        TORCH_CHECK(T >= 1, "attn_extend_paged: qkv has no rows (T=0)");
-        TORCH_CHECK(start >= 0, "attn_extend_paged: start=", start, " must be >= 0");
-        TORCH_CHECK(start + T <= cap, "attn_extend_paged: start=", start, " + T=", T, " must be <= capacity=", cap);
-        TORCH_CHECK(out.dim() == 2 && out.size(0) == T && out.size(1) == n_heads * d, "attn_extend_paged: out must be [T=", T,
-                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
-    }, &block_table_row);
+                                                     n_kv, scale, chunk_shapes("attn_extend_paged", qkv, start, out, n_heads, n_kv),
+                                                     &block_table_row);
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.start = (int)start; a.n_tokens = (int)qkv.size(0);
     check_status(sqllm_attn_extend_paged(&a, cur_stream()), "quant_cuda.attn_extend_paged");
