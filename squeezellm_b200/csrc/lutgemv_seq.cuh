@@ -1,7 +1,9 @@
 // lutgemv_seq.cuh - the SEQUENCE kernel: one persistent launch runs a whole list of dependent LUT-GEMVs (a decode token's QuantLinear
 // matvecs: llama.py:226-234 calls them one by one, 224 launches per LLaMA-7B token).  Built on lutgemv_v2.cuh:
 // the per-position math, table builders, outlier warps (sparse3), mailboxes, CTA span (Span) and strip flush (flush_strip) are v2's
-// (namespace v2), and so is the finishing pass (lutgemv_finish.inc); what is new is everything BETWEEN two GEMVs.
+// (namespace v2), and so are the texts of the warp roles' per-segment work: the producer's stream of a segment (lutgemv_stream.inc),
+// the builders' loop (lutgemv_tables.inc) and finishing pass (lutgemv_finish.inc), and the consumers' segment (lutgemv_segment.inc),
+// here with C2's 32-unit stages.  What is new is everything BETWEEN two GEMVs.
 //
 // Why: with one launch per GEMV (v2 + PDL + CUDA graph) a 4096x4096 layer takes several times its HBM time in the chain: every launch
 // carries a fixed cost (CTA exit -> grid completion -> dependency release -> CTA start, barrier init, tensor
@@ -172,6 +174,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
     static_assert(std::is_same<XT, __half>::value || std::is_same<XT, __nv_bfloat16>::value, "x is fp16 or bf16");
     static_assert(MODE == 0 || std::is_same<XT, __half>::value, "the pair table multiplies fp16 by fp16: it needs fp16 x");
     constexpr int NTB = C::NTB;
+    constexpr int TFREE = 288;   // tfree[b] at bar_u32 + TFREE + 8b (after up to four tfull barriers)
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     if (raw != c.smem_raw) __trap();
@@ -194,7 +197,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         }
         for (int b = 0; b < NTB; ++b) {
             mbar_init(bar_u32 + 256 + 8 * b, NBW);
-            mbar_init(bar_u32 + 288 + 8 * b, NWC);
+            mbar_init(bar_u32 + TFREE + 8 * b, NWC);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -224,30 +227,11 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
                 asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&c.descs[g + 1].tm_small)) : "memory");
             }
             warm_l2<BITS>(p, N, lane);  // (cold otherwise: a token never finds them in L2)
+            const int len = sp.len, s0 = sp.s0, r0 = sp.r0;
             for (int seg = 0; seg < sp.nseg; ++seg) {
-                const int sstart = seg == 0 ? 0 : seg * R - sp.r0, send = min(sp.len, (seg + 1) * R - sp.r0);
-                const int seglen = send - sstart;
-                const int u0 = sp.r0 + sstart - seg * R;
-                const int col0 = (sp.s0 + seg) * STRIP;
-                for (int u = 0; u < seglen; u += SU2) {
-                    if (refill) mbar_wait(bar_u32 + 128 + 8 * slot, ph);
-                    const int nu = min(SU2, seglen - u);
-                    const uint32_t full = bar_u32 + 8 * slot;
-                    const uint32_t dst = (slot < n_lo ? lo_base : hi_base) + slot * C::STAGE;
-                    const int row0 = (u0 + u) * C::ROWS;
-                    if (lane == 0) mbar_expect_tx(full, (uint32_t)nu * C::UNIT);
-                    __syncwarp();
-                    if (nu == SU2) {
-                        if (lane == 0) tma_tile2d_g2s(dst, &d.tm_big, col0, row0, full, pol);
-                    } else if (2 * lane < nu) {
-                        tma_tile2d_g2s(dst + lane * 2 * C::UNIT, &d.tm_small, col0, row0 + lane * 2 * C::ROWS, full, pol);
-                    }
-                    if (++slot == nstage) {
-                        slot = 0;
-                        if (refill) ph ^= 1u;
-                        refill = true;
-                    }
-                }
+                // (inside the loop: taken ahead of it, the descriptor's address is computed before the nseg test; C2 has no mid box)
+                const CUtensorMap *const tmap_big = &d.tm_big, *const tmap_small = &d.tm_small, *const tmap_mid = nullptr;
+#include "lutgemv_stream.inc"
             }
         }
     } else if (warp >= WARP_SP) {
@@ -265,6 +249,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
 #pragma unroll
         for (int b = 0; b < NTB; ++b) sts_u32(sacc0 + 4 * (b * STRIP + bt), 0u);
         int q0 = 0;  // segments of earlier GEMVs: segment s of this one uses table buffer / accumulator (q0 + s) % NTB
+        auto tab_of = [&](int s) { return (q0 + s) % NTB; };
         auto prefetch_first = [&](const P2 &p) {  // the raw LUT rows of a GEMV's first two strips
             const Span sp(p);
             if (sp.nseg > 0) lut_prefetch<BITS>(p, lutbuf, sp.s0, bt);
@@ -279,25 +264,13 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             const int s0 = sp.s0, r0 = sp.r0, nseg = sp.nseg;
             const uint32_t boxtag = (epoch << 10) | (uint32_t)(g + 1);
             float *const acc_out = p.ws_acc;
-            auto sacc_of = [&](int s) { return sacc0 + 4u * (uint32_t)(((q0 + s) % NTB) * STRIP + bt); };
-            auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + 288 + 8 * ((q0 + s) % NTB), (uint32_t)(((q0 + s) / NTB) & 1)); };
+            auto sacc_of = [&](int s) { return sacc0 + 4u * (uint32_t)(tab_of(s) * STRIP + bt); };
+            auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + TFREE + 8 * tab_of(s), (uint32_t)(((q0 + s) / NTB) & 1)); };
+            auto reuse_wait = [&](int s) { tfree_wait(s - NTB); };
             const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
             const int ofs = r0 != 0 ? 1 : 0;        // segment s is owned strip s - ofs
             auto flush = [&](int s) { flush_strip<true>(p, sacc_of(s), s, ofs, sp, N, base, bt, acc_out, boxtag); };
-            for (int s = 0; s < nseg; ++s) {
-                const int b = (q0 + s) % NTB;
-                if (s >= NTB) {
-                    tfree_wait(s - NTB);
-                    flush(s - NTB);
-                }
-                if (s + 1 < nseg) cp_async_wait_pending<1>();
-                else cp_async_wait_all();
-                named_bar_sync(3, NBT);
-                build_table<BITS, MODE>(tab0 + b * C::TAB, lutbuf + (s & 1) * LUTBUF, bt);
-                named_bar_sync(3, NBT);
-                if (lane == 0) mbar_arrive(bar_u32 + 256 + 8 * b);
-                if (s + 2 < nseg) lut_prefetch<BITS>(p, lutbuf + (s & 1) * LUTBUF, s0 + s + 2, bt);
-            }
+#include "lutgemv_tables.inc"
             if (g + 1 < ngemv) prefetch_first(c.descs[g + 1].p);  // the next GEMV's rows travel while this one is being finished
             // the finishing pass (lutgemv_finish.inc): mailbox words are never reset (a stale word carries an older tag); y is a tagged
             // word in every rank's arena, and a plain XT copy if the item has one
@@ -384,10 +357,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
         const uint32_t slotb[4] = {(uint32_t)((((0 ^ jsel) << 4) | i16) << 2), (uint32_t)((((1 ^ jsel) << 4) | i16) << 2),
                                    (uint32_t)((((2 ^ jsel) << 4) | i16) << 2), (uint32_t)((((3 ^ jsel) << 4) | i16) << 2)};
         const uint32_t lane_in_stage = (uint32_t)((2 * warp + jsel) * C::UNIT + i16 * 16);
-        constexpr int XB = C::XU * 2;
-        constexpr int XBS = SU2 * XB;
         int slot = 0, q0 = 0;
         uint32_t par = 0;
+        auto sacc_row = [&](int b) { return sacc0 + (uint32_t)(b * STRIP + 4 * i16) * 4u; };
         auto stage_of = [&](int sl) { return (sl < n_lo ? lo_base : hi_base) + sl * C::STAGE + lane_in_stage; };
         auto advance = [&]() { if (++slot == nstage) { slot = 0; par ^= 1u; } };
         for (int g = 0; g < ngemv; ++g) {
@@ -395,6 +367,11 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             const P2 &p = d.p;
             const int R = p.R;
             const Span sp(p);
+            const int len = sp.len, r0 = sp.r0;
+            // (q0 by value: captured by reference, it changes the order in which q0, slot and par are promoted to registers, and with
+            // it the register allocation)
+            auto tab_of = [q0](int s) { return (q0 + s) % NTB; };
+            auto tab_phase = [q0](int s) { return (uint32_t)(((q0 + s) / NTB) & 1); };
             TRACE(2, tid == 0);
             if (g > 0) named_bar_sync(6, NCT + NSPW * 32);  // every consumer warp and the outlier warps are done with the previous x
             if (d.x_tag == nullptr) {
@@ -428,60 +405,7 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv_seq_kernel(const SeqCfg c
             named_bar_sync(2, NCT + NSPW * 32);  // x visible to the consumers and the outlier warps
             TRACE(4, tid == 0);
             for (int seg = 0; seg < sp.nseg; ++seg) {
-                const int q = q0 + seg, b = q % NTB;
-                const uint32_t tab = tab0 + b * C::TAB;
-                const uint32_t tb_hi = (MODE == 1 && BITS == 4) ? tab : (BITS == 4 ? (tab & 0xFFFF0000u) : tab);
-                uint32_t l[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    l[t] = tb_hi | slotb[t];
-                    asm volatile("mov.u32 %0, %0;" : "+r"(l[t]));
-                }
-                const uint32_t segc = ((tab >> 8) & 0xF0u) * 0x01010101u;
-                const int sstart = seg == 0 ? 0 : seg * R - sp.r0, send = min(sp.len, (seg + 1) * R - sp.r0);
-                const int seglen = send - sstart;
-                const int u0 = sp.r0 + sstart - seg * R;
-                uint32_t xaddr = xs_u32 + (uint32_t)((u0 + 2 * warp + jsel) * XB);
-                const int nstg = (seglen + SU2 - 1) / SU2;
-                const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;
-                mbar_wait(bar_u32 + 256 + 8 * b, (uint32_t)((q / NTB) & 1));
-                TRACE(16 + (seg < 7 ? seg : 7), tid == 0);
-                for (int k = 0; k < nstg; ++k) {
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (k < mine) {
-                        Fetch<BITS, XT> F;
-                        fetch2<BITS, XT>(F, stage_of(slot), xaddr);
-                        math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
-                    advance();
-                    xaddr += XBS;
-                }
-                {
-                    float s[4];
-#pragma unroll
-                    for (int t = 0; t < 4; ++t) {
-                        s[t] = MODE == 0 ? sum2(A.a[t]) : A.f[t] + A.f[t + 4];
-                        A.a[t] = 0ull;
-                        A.f[t] = 0.f;
-                        A.f[t + 4] = 0.f;
-                    }
-                    const float v0 = __shfl_xor_sync(0xffffffffu, s[1], 16);
-                    const float v1 = __shfl_xor_sync(0xffffffffu, s[0], 16);
-                    const float v2 = __shfl_xor_sync(0xffffffffu, s[3], 16);
-                    const float v3 = __shfl_xor_sync(0xffffffffu, s[2], 16);
-                    if (jsel == 0 && mine > 0) {
-                        const uint32_t a = sacc0 + (uint32_t)(b * STRIP + 4 * i16) * 4u;
-                        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(s[0] + v0) : "memory");
-                        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 4), "f"(s[1] + v1) : "memory");
-                        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 8), "f"(s[2] + v2) : "memory");
-                        asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 12), "f"(s[3] + v3) : "memory");
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_u32 + 288 + 8 * b);
-                }
-                TRACE(24 + (seg < 7 ? seg : 7), tid == 0);
+#include "lutgemv_segment.inc"
             }
             TRACE(6, tid == 0);
             q0 += sp.nseg;

@@ -18,6 +18,9 @@
 //     exact products (fhfma2; tests/perf/microbench2.cu measures the loop).  The only rounding is LUT -> fp16 (2^-11 relative per centroid); it needs fp16 x.
 //   * x is staged whole in its own type (fp32, fp16 or bf16: the XT template parameter; 16-bit pairs are widened to fp32 in registers),
 //     the sparse warps gather it from shared memory (sparse3: nothing else of theirs goes through shared memory).
+// The warp roles' per-segment work is text #included by this kernel and the sequence kernel (lutgemv_seq.cuh), each text opening with
+// the names its includer defines: the producer's lutgemv_stream.inc, the builders' lutgemv_tables.inc and lutgemv_finish.inc, the
+// consumers' lutgemv_segment.inc (DESIGN §3.4).
 #pragma once
 #include "common.cuh"
 
@@ -83,6 +86,8 @@ struct C2 {
     static constexpr int ROWS = BITS == 4 ? 1 : 3;           // packed rows per unit
     static constexpr int XU = BITS == 4 ? 8 : 32;            // inputs per unit
     static constexpr int UNIT = ROWS * STRIP * 4;            // bytes of one unit in a stage
+    static constexpr int SU = SU2;                           // units per stage
+    static constexpr bool ROT = false;                       // no 64-unit stages (G2), so the sequence kernel runs 32-unit ones
     static constexpr int STAGE = SU2 * UNIT;                 // 8 KB / 24 KB
     static constexpr int NTB = TAB <= 16384 ? 4 : 2;         // sequence kernel: table buffers (and strip accumulators), 4 x 4 KB exact, 2 x 64 KB for the 4-bit pair table
 };
@@ -683,7 +688,10 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
     const uint32_t bar_u32 = base + OFF_BAR;
     const uint32_t xs_u32 = base + OFF_X;
     const int nstage = p.nstage;
-    const Carve cv(base, (uint32_t)((p.K * (int)sizeof(XT) + 127) & ~127), 0u, C::TAB, 2, C::STAGE, nstage);
+    constexpr int NTB = 2;       // table buffers and strip accumulators: segment s uses s & 1
+    constexpr int TFREE = 272;   // tfree[b] at bar_u32 + TFREE + 8b
+    auto tab_of = [](int s) { return s & 1; };
+    const Carve cv(base, (uint32_t)((p.K * (int)sizeof(XT) + 127) & ~127), 0u, C::TAB, NTB, C::STAGE, nstage);
     const uint32_t lo_base = cv.lo_base, tab0 = cv.tab0, hi_base = cv.hi_base;
     const int n_lo = cv.n_lo;
 
@@ -698,9 +706,9 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
             mbar_init(bar_u32 + 8 * s, 1);          // full: the producer's arrive.expect_tx
             mbar_init(bar_u32 + 128 + 8 * s, NWC);  // empty: one arrive per consumer warp
         }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(bar_u32 + 256 + 8 * b, NBW);  // tfull: table b is built (one arrive per builder warp)
-            mbar_init(bar_u32 + 272 + 8 * b, NWC);  // tfree: every consumer warp is done with table b and has deposited its strip sums
+        for (int b = 0; b < NTB; ++b) {
+            mbar_init(bar_u32 + 256 + 8 * b, NBW);    // tfull: table b is built (one arrive per builder warp)
+            mbar_init(bar_u32 + TFREE + 8 * b, NWC);  // tfree: every consumer warp is done with table b and has deposited its strip sums
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -720,49 +728,22 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
 
     if (warp == WARP_PROD) {
         // =========================== TMA producer: weights never depend on the previous kernel ===========================
-        // Stages never straddle a strip: segment `seg` (the CTA's part of strip s0+seg) is cut into stages of C::SU units from its own start.
         // (Also tried: cp.async.bulk.prefetch.tensor into L2 16-24 stages ahead of the ring - slower on every shape, like the
         // L2 prefetch experiment of round 1.)
         const uint64_t pol = l2_evict_first_policy();
+        const CUtensorMap *const tmap_big = &tm_big, *const tmap_small = &tm_small, *const tmap_mid = &tm_mid;
         int slot = 0;
         uint32_t ph = 0;
         bool refill = false;
         for (int seg = 0; seg < nseg; ++seg) {
-            const int sstart = seg == 0 ? 0 : seg * R - r0, send = min(len, (seg + 1) * R - r0);
-            const int seglen = send - sstart;
-            const int u0 = r0 + sstart - seg * R;  // unit-in-strip of the segment's first unit
-            const int col0 = (s0 + seg) * STRIP;
-            for (int u = 0; u < seglen; u += C::SU) {
-                if (refill) mbar_wait(bar_u32 + 128 + 8 * slot, ph);
-                const int nu = min(C::SU, seglen - u);
-                const uint32_t full = bar_u32 + 8 * slot;
-                const uint32_t dst = (slot < n_lo ? lo_base : hi_base) + slot * C::STAGE;
-                const int row0 = (u0 + u) * C::ROWS;
-                if (lane == 0) mbar_expect_tx(full, (uint32_t)nu * C::UNIT);
-                __syncwarp();
-                if (nu == C::SU) {
-                    if (lane == 0) tma_tile2d_g2s(dst, &tm_big, col0, row0, full, pol);
-                } else {
-                    // ROT: a ragged stage of 32 units or more starts with one 32-unit box (tm_mid), so that it takes no more copies than
-                    // with 32-unit stages - the TMA unit retires small boxes slowly
-                    const int um = C::ROT && nu >= SU2 ? SU2 : 0;
-                    if (C::ROT && um && lane == 0) tma_tile2d_g2s(dst, &tm_mid, col0, row0, full, pol);
-                    if (2 * lane < nu - um) tma_tile2d_g2s(dst + (um + lane * 2) * C::UNIT, &tm_small, col0, row0 + (um + lane * 2) * C::ROWS, full, pol);
-                }
-                if (++slot == nstage) {
-                    slot = 0;
-                    if (refill) ph ^= 1u;
-                    refill = true;
-                }
-            }
+#include "lutgemv_stream.inc"
         }
     } else if (warp >= WARP_SP) {
         sparse3<XT, FUSED>(p, base, warp - WARP_SP, lane, acc_out, 1u);
         TRACE(10, lane == 0);
     } else if (warp >= WARP_BLD) {
         // =========================== table builders (2 warps, thread = column slot) ===========================
-        // Segment s uses table buffer s & 1 and strip accumulator s & 1.  For every segment: wait until the consumers are done with the
-        // buffer's previous user (segment s-2), flush that segment's sums to global memory, build the new table, signal tfull.
+        // Segment s uses table buffer s & 1 and strip accumulator s & 1; the loop over the segments is lutgemv_tables.inc.
         const int bt = tid - WARP_BLD * 32;
         const uint32_t lutbuf = base + OFF_LUT, sacc = base + OFF_SACC;
         sts_u32(sacc + 4 * bt, 0u);
@@ -770,28 +751,17 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         bool dep_ok = false;
         auto dep_wait = [&]() { if (!dep_ok) { pdl_wait(); dep_ok = true; } };  // builders never read x: they only need this before writing
         const uint32_t sown = base + OFF_FIN;   // float [SOWN][64]
-        constexpr int NTB = 2;  // table buffers and strip accumulators
         auto sacc_of = [&](int s) { return sacc + 4 * ((s & 1) * STRIP + bt); };
-        auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + 272 + 8 * (s & 1), (uint32_t)((s >> 1) & 1)); };
+        auto tfree_wait = [&](int s) { mbar_wait(bar_u32 + TFREE + 8 * (s & 1), (uint32_t)((s >> 1) & 1)); };
+        auto reuse_wait = [&](int s) {  // the previous user of segment s's buffer: segment s - 2
+            dep_wait();                 // from here on we write global memory: the previous kernel must be done
+            mbar_wait(bar_u32 + TFREE + 8 * (s & 1), (uint32_t)(((s >> 1) - 1) & 1));
+        };
         auto flush = [&](int s) { flush_strip<FUSED>(p, sacc_of(s), s, r0 != 0 ? 1 : 0, sp, N, base, bt, acc_out, 1u); };
         // The raw LUT rows of the first two strips are requested at once (one cold round trip, not two); later strips two ahead.
         if (nseg > 0) lut_prefetch<BITS>(p, lutbuf, s0, bt);
         if (nseg > 1) lut_prefetch<BITS>(p, lutbuf + LUTBUF, s0 + 1, bt);
-        for (int s = 0; s < nseg; ++s) {
-            const int b = s & 1;
-            if (s >= 2) {
-                dep_wait();  // from here on we write global memory: the previous kernel must be done
-                mbar_wait(bar_u32 + 272 + 8 * b, (uint32_t)(((s >> 1) - 1) & 1));
-                flush(s - 2);
-            }
-            if (s + 1 < nseg) cp_async_wait_pending<1>();  // all but the newest group (the next strip's rows) have landed
-            else cp_async_wait_all();
-            named_bar_sync(3, NBT);  // the strip's LUT rows are in shared memory, all of them
-            build_table<BITS, MODE, C::ROT>(tab0 + b * C::TAB, lutbuf + b * LUTBUF, bt);
-            named_bar_sync(3, NBT);  // both warps are done reading the rows (and writing the table)
-            if (lane == 0) mbar_arrive(bar_u32 + 256 + 8 * b);
-            if (s + 2 < nseg) lut_prefetch<BITS>(p, lutbuf + b * LUTBUF, s0 + s + 2, bt);  // this buffer's next strip: long there when it is needed
-        }
+#include "lutgemv_tables.inc"
         dep_wait();
         if constexpr (!FUSED) {
             for (int s = max(0, nseg - NTB); s < nseg; ++s) {  // the last two segments
@@ -882,100 +852,15 @@ __global__ void __launch_bounds__(THREADS2, 1) lutgemv2_kernel(const P2 p, const
         const uint32_t slotb[4] = {(uint32_t)((((0 ^ jsel) << 4) | i16) << 2), (uint32_t)((((1 ^ jsel) << 4) | i16) << 2),
                                    (uint32_t)((((2 ^ jsel) << 4) | i16) << 2), (uint32_t)((((3 ^ jsel) << 4) | i16) << 2)};
         const uint32_t sacc_lane = base + OFF_SACC + (4 * i16) * 4;
+        auto sacc_row = [&](int b) { return sacc_lane + b * (STRIP * 4); };
+        auto tab_phase = [](int s) { return (uint32_t)((s >> 1) & 1); };
         const uint32_t lane_in_stage = (uint32_t)((2 * warp + jsel) * C::UNIT + i16 * 16);
-        constexpr int XB = C::XU * (int)sizeof(XT);  // bytes of x per unit
-        constexpr int XBS = SU2 * XB;             // ... per 32 units (a stage; ROT: half a stage)
-
         int slot = 0;
         uint32_t par = 0;
         auto stage_of = [&](int sl) { return (sl < n_lo ? lo_base : hi_base) + sl * C::STAGE + lane_in_stage; };
         auto advance = [&]() { if (++slot == nstage) { slot = 0; par ^= 1u; } };
         for (int seg = 0; seg < nseg; ++seg) {
-            const int b = seg & 1;
-            // slot addresses of this lane's 4 columns in table b: column (t ^ jsel) -> slot ((t ^ jsel) << 4 | i16); the table base bits above
-            // the row field come with them (exact 4-bit: bits 12..15 ride in segc instead, because byte 1 of the address is built by PRMT).
-            // ROT: the odd half-warp reads copy 1, where slot ((t ^ 1) << 4 | i16) holds ITS column t.
-            const uint32_t tab = tab0 + b * C::TAB + (C::ROT ? (uint32_t)jsel * (C::TAB / 2) : 0u);
-            const uint32_t tb_hi = (MODE == 1 && BITS == 4) ? tab : (BITS == 4 ? (tab & 0xFFFF0000u) : tab);
-            uint32_t l[4];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-                l[t] = tb_hi | slotb[t];
-                asm volatile("mov.u32 %0, %0;" : "+r"(l[t]));
-            }
-            const uint32_t segc = ((tab >> 8) & 0xF0u) * 0x01010101u;
-            const int sstart = seg == 0 ? 0 : seg * R - r0, send = min(len, (seg + 1) * R - r0);
-            const int seglen = send - sstart;
-            const int u0 = r0 + sstart - seg * R;
-            uint32_t xaddr = xs_u32 + (uint32_t)((u0 + 2 * warp + jsel) * XB);
-            const int nstg = (seglen + C::SU - 1) / C::SU;
-            const int mine = 2 * warp < seglen ? (seglen - 2 * warp + SU2 - 1) / SU2 : 0;  // positions (32-unit steps) in which this warp has a pair
-
-            mbar_wait(bar_u32 + 256 + 8 * b, (uint32_t)((seg >> 1) & 1));  // table b holds this strip
-            TRACE(16 + (seg < 7 ? seg : 7), tid == 0);
-            // Every consumer warp walks every stage of the segment (the empty barriers count NWC arrivals); a warp whose pair lies past
-            // the end of a ragged last stage just releases it.  One stage per trip, no look-ahead across stages.  (A two-stage
-            // ping-pong variant that hides the word fetch behind the previous position's gathers doubles the body to ~290 instructions;
-            // with 23 warps in five roles on the SM the instruction cache misses ate the gain - ncu showed many stall samples on
-            // "no instruction".)
-            if constexpr (C::ROT) {
-                // 64-unit stages: position p of stage k is unit 32p + 2 warp + jsel, so a lane meets its units in the same order as with
-                // 32-unit stages (same FMA order).  Both positions' words and x are read before the first gather; the second position's
-                // reads may run past a ragged stage's end (stale ring bytes, x past K: still inside the window), its math is skipped.
-                for (int k = 0; k < nstg; ++k) {
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (2 * k < mine) {
-                        Fetch<BITS, XT> F0, F1;
-                        fetch2<BITS, XT>(F0, stage_of(slot), xaddr);
-                        fetch2<BITS, XT>(F1, stage_of(slot) + SU2 * C::UNIT, xaddr + XBS);
-                        math2<BITS, MODE, XT>(F0, 0, l, segc, xaddr, A);
-                        if (2 * k + 1 < mine) math2<BITS, MODE, XT>(F1, 0, l, segc, xaddr, A);
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
-                    advance();
-                    xaddr += 2 * XBS;
-                }
-            } else {
-                for (int k = 0; k < nstg; ++k) {
-                    mbar_wait(bar_u32 + 8 * slot, par);
-                    if (k < mine) {
-                        Fetch<BITS, XT> F;
-                        fetch2<BITS, XT>(F, stage_of(slot), xaddr);
-                        math2<BITS, MODE, XT>(F, jsel, l, segc, xaddr, A);
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_u32 + 128 + 8 * slot);
-                    advance();
-                    xaddr += XBS;
-                }
-            }
-            {   // this strip's sums: lane (i, j=1) holds column t^1 in slot t (ROT: column t) - hand it to lane (i, j=0), which adds both
-                // into the CTA's shared accumulator of the strip (16 warps x 64 red.shared.add; the builders move it on to global memory)
-                float s[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    s[t] = MODE == 0 ? sum2(A.a[t]) : A.f[t] + A.f[t + 4];
-                    A.a[t] = 0ull;
-                    A.f[t] = 0.f;
-                    A.f[t + 4] = 0.f;
-                }
-                constexpr int SW = C::ROT ? 0 : 1;
-                const float v0 = __shfl_xor_sync(0xffffffffu, s[0 ^ SW], 16);
-                const float v1 = __shfl_xor_sync(0xffffffffu, s[1 ^ SW], 16);
-                const float v2 = __shfl_xor_sync(0xffffffffu, s[2 ^ SW], 16);
-                const float v3 = __shfl_xor_sync(0xffffffffu, s[3 ^ SW], 16);
-                if (jsel == 0 && mine > 0) {
-                    const uint32_t a = sacc_lane + b * (STRIP * 4);
-                    asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a), "f"(s[0] + v0) : "memory");
-                    asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 4), "f"(s[1] + v1) : "memory");
-                    asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 8), "f"(s[2] + v2) : "memory");
-                    asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(a + 12), "f"(s[3] + v3) : "memory");
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_u32 + 272 + 8 * b);  // done with table b, sums deposited
-            }
-            TRACE(24 + (seg < 7 ? seg : 7), tid == 0);
+#include "lutgemv_segment.inc"
         }
         TRACE(6, tid == 0);
     }
