@@ -9,20 +9,28 @@ import torch
 from util import orc, rel_err, to_torch, REL_TOL
 
 FLAG, STATE, ERROR, DATA = 0, 64, 128, 4096
+EXCHANGE_LAYERS = [(4, 1024, 1024, 2, 0.01, 4), (3, 512, 256, 1, 0.0, 0), (4, 4096, 4096, 3, 0.0045, 10),
+                   (4, 256, 32, 1, 0.02, 4),  # narrower than one strip: one ragged strip
+                   (3, 1024, 512, 3, 0.01, 40)]  # more than 32 dense rows: the general dense-row branch
+EXCHANGE_IDS = ["w4-2x1024", "w3-1x256", "w4-qkv", "w4-1x32", "w3-3x512-t40"]
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("bits,K,w,members,sp,topx", [(4, 1024, 1024, 2, 0.01, 4), (3, 512, 256, 1, 0.0, 0), (4, 4096, 4096, 3, 0.0045, 10),
-                                                      (4, 256, 32, 1, 0.02, 4),  # narrower than one strip: one ragged strip
-                                                      (3, 1024, 512, 3, 0.01, 40)],  # more than 32 dense rows: the general dense-row branch
-                         ids=["w4-2x1024", "w3-1x256", "w4-qkv", "w4-1x32", "w3-3x512-t40"])
-def test_exchange_world1_matches_oracle_and_counts_arrivals(bits, K, w, members, sp, topx):
-    from squeezellm_b200 import quant as Q
-    qc = Q.quant_cuda
+def exchange_layer(bits, K, w, members, sp, topx):
+    """The oracle layer of `members` stacked shards of width w (EXCHANGE_LAYERS), with a bias."""
     N = members * w
     L = orc.make_layer(bits, K, N, sparsity=sp, topX=topx, seed=K + N, nonzero_full_rows=True, bias=True)
     if topx and sp == 0:
         L["full_rows"] = L["full_row_indices"] = None
+    return L
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("bits,K,w,members,sp,topx", EXCHANGE_LAYERS, ids=EXCHANGE_IDS)
+def test_exchange_world1_matches_oracle_and_counts_arrivals(bits, K, w, members, sp, topx):
+    from squeezellm_b200 import quant as Q
+    qc = Q.quant_cuda
+    N = members * w
+    L = exchange_layer(bits, K, w, members, sp, topx)
     T = to_torch(L)
     x = orc.make_vec(K, seed=6)
     xt = torch.from_numpy(x).cuda().reshape(-1).half()
