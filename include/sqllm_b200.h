@@ -55,7 +55,7 @@ extern "C" {
                                  sqllm_attn_decode_splits, sqllm_attn_decode_batch, sqllm_attn_decode_batch_splits,
                                  sqllm_attn_extend, sqllm_attn_extend_splits, sqllm_sample, sqllm_attn_verify,
                                  sqllm_attn_verify_splits, sqllm_attn_verify_launch_splits, sqllm_attn_decode_paged,
-                                 sqllm_attn_extend_paged
+                                 sqllm_attn_extend_paged, sqllm_attn_extend_batch, sqllm_attn_extend_batch_paged
                                  (backward compatible, same version) */
 
 int sqllm_abi_version(void);
@@ -720,6 +720,73 @@ typedef struct sqllm_attn_extend_paged_args {
 } sqllm_attn_extend_paged_args;
 
 int sqllm_attn_extend_paged(const sqllm_attn_extend_paged_args *args, void *stream);
+
+/* The chunk attention of sqllm_attn_extend for several sequences in one call: n_segments segments, segment i the chunk of n_tokens[i]
+ * new tokens of the sequence in slot slots[i] at positions starts[i] .. starts[i] + n_tokens[i] - 1.  Its rows are rows
+ * row0_i .. row0_i + n_tokens[i] - 1 of qkv and out, row0_i = n_tokens[0] + ... + n_tokens[i-1] (the caller's order).
+ *   qkv       [sum n_tokens][n_heads*d | n_kv*d | n_kv*d] of dtype
+ *   slots, starts, n_tokens   HOST int32 [n_segments]
+ *   k_cache, v_cache    [n_slots][n_kv][capacity][d] of dtype: slot b is block b, laid out as sqllm_attn_extend's cache
+ *   out       [sum n_tokens][n_heads*d] of dtype
+ * Segment i's out rows and the k / v it stores are bitwise what sqllm_attn_extend computes for slot slots[i] alone with (starts[i],
+ * n_tokens[i]), so they depend neither on the other segments nor on their order.  The call writes only positions starts[i] ..
+ * starts[i] + n_tokens[i] - 1 of each segment's slot, and reads nothing of a slot that no segment names.
+ * Launch shape: one append launch with one CTA per row of every segment; then the attention: segment i splits its tiles' keys over
+ * S_i = sqllm_attn_extend_splits(n_heads, n_kv, n_tokens[i], starts[i], SM count) CTAs per cluster, as sqllm_attn_extend does, and
+ * since a cluster has one size per launch, one attention launch per distinct S_i (at most 8), holding the tiles of its segments
+ * ordered by starts[i] + n_tokens[i], longest first, each segment's tiles last-first.  The segment table travels in the kernel
+ * parameters: no allocation, no upload, no host synchronisation; CUDA-graph capturable for fixed segments.
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_extend (dtype, head layout, head_dim,
+ * capacity, scale, n_kv <= 65535), n_segments in [1, SQLLM_ATTN_EXTEND_MAX_SEGMENTS], n_slots >= 1, slots, starts and n_tokens
+ * non-null; per segment a slot in [0, n_slots) that no other segment names, n_tokens >= 1, start >= 0, start + n_tokens <= capacity;
+ * the query tiles of all segments together, sum ceil(n_tokens[i] (n_heads / n_kv) / 64), at most 65535 (so every launch's fit);
+ * every device pointer non-null and 16-byte aligned. */
+#define SQLLM_ATTN_EXTEND_MAX_SEGMENTS 128
+
+typedef struct sqllm_attn_extend_batch_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions of a slot */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    int n_segments;           /* 1 .. SQLLM_ATTN_EXTEND_MAX_SEGMENTS */
+    const int32_t *slots;     /* HOST [n_segments] */
+    const int32_t *starts;    /* HOST [n_segments] */
+    const int32_t *n_tokens;  /* HOST [n_segments] */
+    int n_slots;              /* slots of the caches */
+    const void *qkv;          /* [sum n_tokens][n_heads*d | n_kv*d | n_kv*d] */
+    const float *rope_cos, *rope_sin;
+    void *k_cache, *v_cache;  /* [n_slots][n_kv][capacity][d] */
+    void *out;                /* [sum n_tokens][n_heads*d] */
+} sqllm_attn_extend_batch_args;
+
+int sqllm_attn_extend_batch(const sqllm_attn_extend_batch_args *args, void *stream);
+
+/* sqllm_attn_extend_batch in a page pool: segment i through row slots[i] of block_table [n_slots][table_width], bitwise what
+ * sqllm_attn_extend_paged computes for it alone with that row.  A segment with an entry of its blocks 0 .. (starts[i] + n_tokens[i] - 1)
+ * / 64 outside [0, n_pages) reads no page and writes nothing (every CTA of the segment checks those entries itself before any cluster
+ * barrier); the other segments are unaffected.  Several segments' rows may name the same page for reading (a shared prefix).
+ * Requirements (checked, SQLLM_EINVAL otherwise, before any device access): those of sqllm_attn_extend_batch, and the page arguments
+ * of sqllm_attn_decode_paged. */
+typedef struct sqllm_attn_extend_batch_paged_args {
+    int dtype;                /* SQLLM_DT_F16 or SQLLM_DT_BF16 */
+    int n_heads, n_kv, head_dim;
+    int capacity;             /* positions a sequence may use: the rows of the rope tables */
+    float scale;              /* softmax scale, usually 1/sqrt(head_dim) */
+    int n_segments;           /* 1 .. SQLLM_ATTN_EXTEND_MAX_SEGMENTS */
+    const int32_t *slots;     /* HOST [n_segments]: rows of block_table */
+    const int32_t *starts;    /* HOST [n_segments] */
+    const int32_t *n_tokens;  /* HOST [n_segments] */
+    int n_slots;              /* rows of block_table */
+    const void *qkv;          /* [sum n_tokens][n_heads*d | n_kv*d | n_kv*d] */
+    const float *rope_cos, *rope_sin;
+    void *k_pages, *v_pages;  /* [n_pages][n_kv][64][d] */
+    int n_pages;
+    const int32_t *block_table; /* DEVICE [n_slots][table_width] */
+    int table_width;          /* ceil(capacity / 64) */
+    void *out;                /* [sum n_tokens][n_heads*d] */
+} sqllm_attn_extend_batch_paged_args;
+
+int sqllm_attn_extend_batch_paged(const sqllm_attn_extend_batch_paged_args *args, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Token sampling: one token per row of logits, on the device (DESIGN.md section 3.20).  Row b (b < rows) holds x_i =

@@ -1,7 +1,8 @@
 // attn_decode.cu - decode attention with rotary and KV-cache append (attn_decode.cuh) behind sqllm_attn_decode (one sequence),
 // sqllm_attn_decode_batch (several, each at its own position) and sqllm_attn_decode_paged (several, in one pool of KV pages); causal attention of a chunk of new tokens with the same rotary and
 // append (attn_extend.cuh) behind sqllm_attn_extend; decode attention of up to 16 new tokens of one sequence at a device position
-// (attn_verify.cuh) behind sqllm_attn_verify; the chunk attention on KV pages behind sqllm_attn_extend_paged.
+// (attn_verify.cuh) behind sqllm_attn_verify; the chunk attention on KV pages behind sqllm_attn_extend_paged; the chunk attention of
+// several sequences in one call behind sqllm_attn_extend_batch and sqllm_attn_extend_batch_paged.
 #include <limits.h>
 #include <math.h>
 #include <stdint.h>
@@ -44,6 +45,18 @@ template <typename P> struct Append {
     template <typename T, int D, int> static auto of() {
         if constexpr (attn::is_paged<P>) return attn::attn_append_paged_kernel<T, D>;
         else return attn::attn_append_kernel<T, D>;
+    }
+};
+
+template <bool PAGED> struct ExtendBatch {
+    template <typename T, int D, int> static auto of() {
+        if constexpr (PAGED) return attn::attn_extend_batch_paged_kernel<T, D>;
+        else return attn::attn_extend_batch_kernel<T, D>;
+    }
+};
+template <bool PAGED> struct AppendBatch {
+    template <typename T, int D, int> static auto of() {
+        return attn::attn_append_batch_kernel<T, D, std::conditional_t<PAGED, attn::ExtPagedParams, attn::ExtParams>>;
     }
 };
 
@@ -222,6 +235,93 @@ int extend_launch(const Args *a, void *stream) {
     return SQLLM_OK;
 }
 
+static_assert(attn::MAX_SEGMENTS == SQLLM_ATTN_EXTEND_MAX_SEGMENTS, "one segment limit for the kernels and the header");
+
+// the checks and the launches of sqllm_attn_extend_batch (Args = sqllm_attn_extend_batch_args) and sqllm_attn_extend_batch_paged: the
+// append of every segment's rows, then one attention launch per distinct split S_i, its segments by key range start + T longest first
+template <bool PAGED, typename Args>
+int extend_batch_launch(const Args *a, void *stream) {
+    if (int rc = check_dtype(a->dtype)) return rc;
+    if (int rc = check_heads(a)) return rc;
+    const int n = a->n_segments;
+    if (n < 1 || n > attn::MAX_SEGMENTS) return fail(SQLLM_EINVAL, "n_segments=%d must be in [1, %d]", n, attn::MAX_SEGMENTS);
+    if (a->n_slots < 1) return fail(SQLLM_EINVAL, "n_slots=%d must be >= 1", a->n_slots);
+    if (!a->slots || !a->starts || !a->n_tokens) return fail(SQLLM_EINVAL, "slots, starts and n_tokens must be non-null host arrays");
+    if (a->n_kv > 65535) return fail(SQLLM_EINVAL, "n_kv=%d > 65535", a->n_kv);
+    long long tiles = 0;
+    for (int i = 0; i < n; ++i) {
+        const int slot = a->slots[i], start = a->starts[i], T = a->n_tokens[i];
+        if (slot < 0 || slot >= a->n_slots) return fail(SQLLM_EINVAL, "slots[%d]=%d must be in [0, n_slots=%d)", i, slot, a->n_slots);
+        for (int j = 0; j < i; ++j)
+            if (a->slots[j] == slot) return fail(SQLLM_EINVAL, "slots[%d]=%d repeats slots[%d]", i, slot, j);
+        if (T < 1) return fail(SQLLM_EINVAL, "n_tokens[%d]=%d must be >= 1", i, T);
+        if (start < 0) return fail(SQLLM_EINVAL, "starts[%d]=%d must be >= 0", i, start);
+        if ((long long)start + T > a->capacity)
+            return fail(SQLLM_EINVAL, "starts[%d]=%d + n_tokens[%d]=%d must be <= capacity=%d", i, start, i, T, a->capacity);
+        tiles += ((long long)T * (a->n_heads / a->n_kv) + attn::BM - 1) / attn::BM;
+    }
+    if (tiles > attn::MAX_TILES)
+        return fail(SQLLM_EINVAL, "the segments need %lld query tiles of %d per KV head, more than %d", tiles, attn::BM, attn::MAX_TILES);
+    attn::ExtBatchParams b;
+    if constexpr (PAGED) {
+        if (int rc = check_pages(a)) return rc;
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->out, "out"}})) return rc;
+        b.k_cache = a->k_pages; b.v_cache = a->v_pages; b.table = a->block_table; b.width = a->table_width; b.n_pages = a->n_pages;
+    } else {
+        if (int rc = check_ptrs({{a->qkv, "qkv"}, {a->rope_cos, "rope_cos"}, {a->rope_sin, "rope_sin"}, {a->k_cache, "k_cache"},
+                                 {a->v_cache, "v_cache"}, {a->out, "out"}}))
+            return rc;
+        b.k_cache = a->k_cache; b.v_cache = a->v_cache; b.table = nullptr; b.width = 0; b.n_pages = 0;
+    }
+    const auto fn = instance<ExtendBatch<PAGED>>(a->dtype, a->head_dim);
+    const int bytes = attn::ext_smem_bytes(a->head_dim);
+    int sm = 0;
+    int rc = dev_setup({KernelSmem(fn, bytes)}, &sm);
+    if (rc) return rc;
+    b.qkv = a->qkv; b.cos = a->rope_cos; b.sin = a->rope_sin; b.out = a->out;
+    b.n_heads = a->n_heads; b.n_kv = a->n_kv; b.g = a->n_heads / a->n_kv; b.capacity = a->capacity; b.start = 0; b.T = 0;
+    b.qscale = a->scale * attn::LOG2E / attn::QPRE;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const char *name = PAGED ? "attn_extend_batch_paged" : "attn_extend_batch";
+
+    // the append: every segment's rows in the caller's order
+    b.n = n;
+    int rows = 0, S[attn::MAX_SEGMENTS];
+    attn::ExtSegment all[attn::MAX_SEGMENTS];
+    for (int i = 0; i < n; ++i) {
+        all[i] = {a->slots[i], a->starts[i], a->n_tokens[i], rows};
+        b.first[i] = rows;
+        b.seg[i] = all[i];
+        rows += a->n_tokens[i];
+        S[i] = ext_splits(a->n_heads, a->n_kv, a->n_tokens[i], a->starts[i], sm);
+    }
+    const auto append = instance<AppendBatch<PAGED>>(a->dtype, a->head_dim);
+    append<<<rows, attn::APPEND_THREADS, 0, st>>>(b);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s append launch failed: %s", name, cudaGetErrorString(e));
+
+    // the attention: per split, its segments by key range, longest first (ties in the caller's order)
+    for (int s = attn::MAX_CLUSTER; s >= 1; --s) {
+        int order[attn::MAX_SEGMENTS], m = 0;
+        for (int i = 0; i < n; ++i)
+            if (S[i] == s) order[m++] = i;
+        if (m == 0) continue;
+        std::stable_sort(order, order + m, [&](int x, int y) {
+            return (long long)all[x].start + all[x].T > (long long)all[y].start + all[y].T;
+        });
+        int tiles_s = 0;
+        for (int k = 0; k < m; ++k) {
+            b.first[k] = tiles_s;
+            b.seg[k] = all[order[k]];
+            tiles_s += (int)ext_tiles(a->n_heads, a->n_kv, all[order[k]].T);
+        }
+        b.n = m;
+        e = launch_ex(fn, dim3(s, tiles_s, a->n_kv), attn::XTHREADS, bytes, st, cluster_of(s), b);
+        if (e != cudaSuccess) return fail(SQLLM_ECUDA, "%s launch failed: %s", name, cudaGetErrorString(e));
+    }
+    return SQLLM_OK;
+}
+
 // clusters per KV head of sqllm_attn_verify: chunks of GMAX of the T * g (token, query head) rows of its group
 int ver_chunks(int n_heads, int n_kv, int T) { return (T * (n_heads / n_kv) + attn::GMAX - 1) / attn::GMAX; }
 
@@ -342,6 +442,16 @@ int sqllm_attn_decode_paged(const sqllm_attn_decode_paged_args *a, void *stream)
 int sqllm_attn_extend_paged(const sqllm_attn_extend_paged_args *a, void *stream) {
     if (!a) return fail(SQLLM_EINVAL, "null args");
     return extend_launch<attn::ExtPagedParams>(a, stream);
+}
+
+int sqllm_attn_extend_batch(const sqllm_attn_extend_batch_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return extend_batch_launch<false>(a, stream);
+}
+
+int sqllm_attn_extend_batch_paged(const sqllm_attn_extend_batch_paged_args *a, void *stream) {
+    if (!a) return fail(SQLLM_EINVAL, "null args");
+    return extend_batch_launch<true>(a, stream);
 }
 
 int sqllm_attn_verify_splits(int n_heads, int n_kv, int n_tokens, int sm_count) { return ver_splits(n_heads, n_kv, n_tokens, sm_count); }

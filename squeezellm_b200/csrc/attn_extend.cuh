@@ -19,6 +19,9 @@
 //
 // Paged (sqllm_attn_extend_paged): attn_append_paged_kernel and attn_extend_paged_kernel are the same code with the cache addressed
 // through the sequence's block table (ExtPagedParams): key block kb is page table[kb] of the pools, so a K / V block is one page.
+//
+// Several sequences (sqllm_attn_extend_batch, _paged): attn_append_batch_kernel, attn_extend_batch_kernel and
+// attn_extend_batch_paged_kernel run the same code per segment of a segment table in the kernel parameters (below).
 #pragma once
 #include "attn_decode.cuh"
 
@@ -109,11 +112,11 @@ __device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t &r0, uint32_t 
 template <int D>
 __device__ __forceinline__ int swz(int row, int chunk) { return row * D + ((chunk ^ (row & 7)) << 3); }
 
-// one CTA per token t: k' and v of every KV head into slot start + t.  P: ExtParams (a contiguous cache) or ExtPagedParams (pools).
+// the CTA of token t: k' and v of every KV head into slot start + t.  P: ExtParams (a contiguous cache) or ExtPagedParams (pools).
 template <typename T, int D, typename P>
-__device__ __forceinline__ void append_body(const P &p) {
+__device__ __forceinline__ void append_body(const P &p, int t) {
     if (!ext_pages_valid(p)) return;
-    const int t = blockIdx.x, pos = p.start + t;
+    const int pos = p.start + t;
     const T *qkv = static_cast<const T *>(p.qkv) + (size_t)t * (p.n_heads + 2 * p.n_kv) * D;
     const float *cs = p.cos + (size_t)pos * (D / 2), *sn = p.sin + (size_t)pos * (D / 2);
     for (int idx = threadIdx.x; idx < p.n_kv * D; idx += APPEND_THREADS) {
@@ -129,14 +132,15 @@ __device__ __forceinline__ void append_body(const P &p) {
 }
 
 template <typename T, int D>
-__global__ void __launch_bounds__(APPEND_THREADS) attn_append_kernel(const ExtParams p) { append_body<T, D>(p); }
+__global__ void __launch_bounds__(APPEND_THREADS) attn_append_kernel(const ExtParams p) { append_body<T, D>(p, blockIdx.x); }
 template <typename T, int D>
-__global__ void __launch_bounds__(APPEND_THREADS) attn_append_paged_kernel(const ExtPagedParams p) { append_body<T, D>(p); }
+__global__ void __launch_bounds__(APPEND_THREADS) attn_append_paged_kernel(const ExtPagedParams p) { append_body<T, D>(p, blockIdx.x); }
 
 template <typename T, int D>
 __global__ void __launch_bounds__(XTHREADS, 1) attn_extend_kernel(const ExtParams p) {
     constexpr bool PAGED = false;
     const Pages pg{};
+    const int tile = gridDim.y - 1 - blockIdx.y;   // last-first
 #include "attn_extend_tile.inc"
 }
 
@@ -145,6 +149,88 @@ template <typename T, int D>
 __global__ void __launch_bounds__(XTHREADS, 1) attn_extend_paged_kernel(const ExtPagedParams p) {
     constexpr bool PAGED = true;
     const Pages pg{p.table, p.n_pages};
+    const int tile = gridDim.y - 1 - blockIdx.y;
+#include "attn_extend_tile.inc"
+}
+
+// ---- several sequences' chunks in one launch (sqllm_attn_extend_batch, sqllm_attn_extend_batch_paged) ----
+//
+// Segment i of a call is the chunk (slot_i, start_i, T_i): rows row0_i .. row0_i + T_i - 1 of qkv and out, row0_i = the sum of T_j over
+// the segments before it in the caller's order.  Each kernel finds its segment by binary search over `first`, the launch's first unit
+// (a row of the append, a query tile of the attention) of each segment, and then runs the single-sequence kernel's code on the segment
+// alone: the segment's qkv and out rows and, contiguous, its slot's caches; paged, its slot's block table row.  So a segment's bits are
+// those of the single-sequence launches with (start_i, T_i) on its slot, whatever the other segments are.
+constexpr int MAX_SEGMENTS = 128;  // SQLLM_ATTN_EXTEND_MAX_SEGMENTS
+
+struct ExtSegment {
+    int slot, start, T, row0;
+};
+
+struct ExtBatchParams : ExtParams {  // qkv [sum T][...], out [sum T][...]; k_cache / v_cache [n_slots][n_kv][capacity][D] or page pools
+    const int *table;                // paged: [n_slots][width]
+    int width, n_pages;
+    int n;                           // segments in this launch
+    int first[MAX_SEGMENTS];         // ascending: segment i's units are first[i] .. first[i + 1] - 1
+    ExtSegment seg[MAX_SEGMENTS];
+};
+static_assert(sizeof(ExtBatchParams) <= 4096, "the segment table travels in the kernel parameters, at most 4 KB");
+
+// the segment of unit u: the last i with first[i] <= u
+__device__ __forceinline__ int segment_of(const ExtBatchParams &b, int u) {
+    int lo = 0, hi = b.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (b.first[mid] <= u) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// the parameters of the single-sequence kernels for segment s alone (P: ExtParams or ExtPagedParams)
+template <typename T, int D, typename P>
+__device__ __forceinline__ P segment_params(const ExtBatchParams &b, const ExtSegment &s) {
+    P p;
+    static_cast<ExtParams &>(p) = b;
+    p.qkv = static_cast<const T *>(b.qkv) + (size_t)s.row0 * (b.n_heads + 2 * b.n_kv) * D;
+    p.out = static_cast<T *>(b.out) + (size_t)s.row0 * b.n_heads * D;
+    p.start = s.start;
+    p.T = s.T;
+    if constexpr (is_paged<P>) {
+        p.table = b.table + (size_t)s.slot * b.width;
+        p.n_pages = b.n_pages;
+    } else {
+        const size_t cache = (size_t)s.slot * b.n_kv * b.capacity * D;
+        p.k_cache = static_cast<T *>(b.k_cache) + cache;
+        p.v_cache = static_cast<T *>(b.v_cache) + cache;
+    }
+    return p;
+}
+
+// one CTA per row of every segment (first[i] = row0_i)
+template <typename T, int D, typename P>
+__global__ void __launch_bounds__(APPEND_THREADS) attn_append_batch_kernel(const ExtBatchParams b) {
+    const ExtSegment s = b.seg[segment_of(b, blockIdx.x)];
+    append_body<T, D>(segment_params<T, D, P>(b, s), (int)blockIdx.x - s.row0);
+}
+
+// grid (S, the launch's tiles, n_kv): the segments of one split S, each segment's tiles last-first from first[i] on
+template <typename T, int D>
+__global__ void __launch_bounds__(XTHREADS, 1) attn_extend_batch_kernel(const ExtBatchParams b) {
+    const int i = segment_of(b, blockIdx.y);
+    const ExtParams p = segment_params<T, D, ExtParams>(b, b.seg[i]);
+    constexpr bool PAGED = false;
+    const Pages pg{};
+    const int tile = (p.T * p.g + BM - 1) / BM - 1 - ((int)blockIdx.y - b.first[i]);
+#include "attn_extend_tile.inc"
+}
+
+template <typename T, int D>
+__global__ void __launch_bounds__(XTHREADS, 1) attn_extend_batch_paged_kernel(const ExtBatchParams b) {
+    const int i = segment_of(b, blockIdx.y);
+    const ExtPagedParams p = segment_params<T, D, ExtPagedParams>(b, b.seg[i]);
+    constexpr bool PAGED = true;
+    const Pages pg{p.table, p.n_pages};
+    const int tile = (p.T * p.g + BM - 1) / BM - 1 - ((int)blockIdx.y - b.first[i]);
 #include "attn_extend_tile.inc"
 }
 

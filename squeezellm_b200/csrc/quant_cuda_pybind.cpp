@@ -10,7 +10,7 @@
 //     stream, quant_cuda_kernel.cu:147,172,...), so the calls are CUDA-graph capturable;
 //   * `*_balanced_*` is not exported, exactly as in the reference (quant.py:238,282 reference a
 //     symbol that quant_cuda.cpp never defines).
-// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `attn_verify`, `attn_decode_paged`, `attn_extend_paged`, `sample`, `unpack_indices`, `abi_version`,
+// Extra, not in the reference: `lutgemv_fused`, `lutgemm_fused`, `lutgemv_rows`, `lutgemv_rows_bf16`, `lutgemm_t`, `lut_grad`, `dequantize`, `fisher_accumulate`, `attn_decode`, `attn_decode_batch`, `attn_extend`, `attn_verify`, `attn_decode_paged`, `attn_extend_paged`, `attn_extend_batch`, `attn_extend_batch_paged`, `sample`, `unpack_indices`, `abi_version`,
 // `fused_limits`.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -615,8 +615,8 @@ void fisher_accumulate(torch::Tensor x, torch::Tensor dy, torch::Tensor fisher, 
 // head_dim], the batch, head_dim, capacity, scale, the cache and out dtypes and v_cache's shape; then own(batch, capacity, head_dim), the
 // binding's own shape checks; then the rope tables.  The device checks come last, so that a CPU caller sees the same rejections.  pos:
 // null for attn_extend.  -> the sqllm args with the fields the four share.
-// table: the block table of attn_decode_paged ([batch, width], lead = 1) and attn_extend_paged ([width], lead = 0), null for the
-// others.  With a table the caches are page pools [n_pages, n_kv, 64, head_dim], capacity is the rope tables' rows, the batch is the
+// table: the block table of attn_decode_paged and attn_extend_batch_paged ([batch, width], lead = 1) and attn_extend_paged ([width],
+// lead = 0), null for the others.  With a table the caches are page pools [n_pages, n_kv, 64, head_dim], capacity is the rope tables' rows, the batch is the
 // table's rows, and the table must be int32, contiguous and 4-byte aligned with width = ceil(capacity / 64).
 template <typename Args, typename Own>
 Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::Tensor *pos, const torch::Tensor &rope_cos,
@@ -669,7 +669,8 @@ Args attn_args(const char *fn, int lead, const torch::Tensor &qkv, const torch::
     a.dtype = dt == torch::kFloat16 ? SQLLM_DT_F16 : SQLLM_DT_BF16;
     a.n_heads = (int)n_heads; a.n_kv = (int)n_kv; a.head_dim = (int)d; a.capacity = (int)cap; a.scale = (float)scale;
     a.qkv = qkv.data_ptr(); a.rope_cos = rope_cos.data_ptr<float>(); a.rope_sin = rope_sin.data_ptr<float>();
-    if constexpr (std::is_same<Args, sqllm_attn_decode_paged_args>::value || std::is_same<Args, sqllm_attn_extend_paged_args>::value) {
+    if constexpr (std::is_same<Args, sqllm_attn_decode_paged_args>::value || std::is_same<Args, sqllm_attn_extend_paged_args>::value ||
+                  std::is_same<Args, sqllm_attn_extend_batch_paged_args>::value) {
         a.k_pages = k_cache.data_ptr(); a.v_pages = v_cache.data_ptr(); a.n_pages = (int)k_cache.size(0);
         a.block_table = table->data_ptr<int32_t>(); a.table_width = (int)table->size(lead);
     } else {
@@ -707,6 +708,48 @@ auto chunk_shapes(const char *fn, const torch::Tensor &qkv, int64_t start, const
                     n_heads * d, "] (got ", out.sizes(), ")");
     };
 }
+
+// The own shape checks of attn_extend_batch and attn_extend_batch_paged, messages prefixed with `fn`, the segment checks of
+// sqllm_attn_extend_batch made here too so that a CPU caller sees them: 1 to 128 segments, the three lists of one length, each slot in
+// [0, n_slots) and named once, T >= 1, start >= 0, start + T <= capacity, the query tiles of all segments within 65535; qkv
+// [sum T, (n_heads + 2 n_kv) head_dim] and out [sum T, n_heads head_dim].
+auto segment_shapes(const char *fn, const torch::Tensor &qkv, const std::vector<int64_t> &slots, const std::vector<int64_t> &starts,
+                    const std::vector<int64_t> &n_tokens, const torch::Tensor &out, int64_t n_heads, int64_t n_kv) {
+    return [=, &qkv, &slots, &starts, &n_tokens, &out](int64_t n_slots, int64_t cap, int64_t d) {
+        const int64_t n = (int64_t)slots.size();
+        TORCH_CHECK(n >= 1 && n <= SQLLM_ATTN_EXTEND_MAX_SEGMENTS, fn, ": n_segments=", n, " must be in [1, ",
+                    SQLLM_ATTN_EXTEND_MAX_SEGMENTS, "]");
+        TORCH_CHECK((int64_t)starts.size() == n && (int64_t)n_tokens.size() == n, fn, ": slots, starts and n_tokens must have one length (got ",
+                    n, ", ", starts.size(), ", ", n_tokens.size(), ")");
+        int64_t rows = 0, tiles = 0;
+        for (int64_t i = 0; i < n; ++i) {
+            TORCH_CHECK(slots[i] >= 0 && slots[i] < n_slots, fn, ": slots[", i, "]=", slots[i], " must be in [0, n_slots=", n_slots, ")");
+            for (int64_t j = 0; j < i; ++j) TORCH_CHECK(slots[j] != slots[i], fn, ": slots[", i, "]=", slots[i], " repeats slots[", j, "]");
+            TORCH_CHECK(n_tokens[i] >= 1, fn, ": n_tokens[", i, "]=", n_tokens[i], " must be >= 1");
+            TORCH_CHECK(starts[i] >= 0, fn, ": starts[", i, "]=", starts[i], " must be >= 0");
+            TORCH_CHECK(starts[i] + n_tokens[i] <= cap, fn, ": starts[", i, "]=", starts[i], " + n_tokens[", i, "]=", n_tokens[i],
+                        " must be <= capacity=", cap);
+            rows += n_tokens[i];
+            tiles += (n_tokens[i] * (n_heads / n_kv) + 63) / 64;
+        }
+        TORCH_CHECK(tiles <= 65535, fn, ": the segments need ", tiles, " query tiles of 64 per KV head, more than 65535");
+        TORCH_CHECK(qkv.dim() == 2 && qkv.size(0) == rows && qkv.size(1) == (n_heads + 2 * n_kv) * d, fn, ": qkv must be [sum n_tokens=",
+                    rows, ", (n_heads + 2 n_kv) head_dim=", (n_heads + 2 * n_kv) * d, "] (got ", qkv.sizes(), ")");
+        TORCH_CHECK(out.dim() == 2 && out.size(0) == rows && out.size(1) == n_heads * d, fn, ": out must be [sum n_tokens=", rows,
+                    ", n_heads head_dim=", n_heads * d, "] (got ", out.sizes(), ")");
+    };
+}
+
+// the segment lists of an attn_extend_batch call as int32, checked by segment_shapes
+struct Segments {
+    std::vector<int32_t> slots, starts, n_tokens;
+    Segments(const std::vector<int64_t> &s, const std::vector<int64_t> &st, const std::vector<int64_t> &t)
+        : slots(s.begin(), s.end()), starts(st.begin(), st.end()), n_tokens(t.begin(), t.end()) {}
+    template <typename Args>
+    void into(Args &a) const {
+        a.n_segments = (int)slots.size(); a.slots = slots.data(); a.starts = starts.data(); a.n_tokens = n_tokens.data();
+    }
+};
 
 // One layer's decode attention (sqllm_attn_decode): rotary, the append of k / v at slot *pos of the caches, attention over slots
 // 0..*pos into out, on the current stream.
@@ -791,6 +834,35 @@ void attn_extend_paged(torch::Tensor qkv, int64_t start, torch::Tensor rope_cos,
     const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
     a.start = (int)start; a.n_tokens = (int)qkv.size(0);
     check_status(sqllm_attn_extend_paged(&a, cur_stream()), "quant_cuda.attn_extend_paged");
+}
+
+// The chunk attention of attn_extend for several sequences in one call (sqllm_attn_extend_batch): segment i is n_tokens[i] tokens of
+// slot slots[i] at starts[i] .. , rows row0_i .. of qkv and out in the lists' order, on caches [n_slots, n_kv, capacity, head_dim].
+void attn_extend_batch(torch::Tensor qkv, std::vector<int64_t> slots, std::vector<int64_t> starts, std::vector<int64_t> n_tokens,
+                       torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor out,
+                       int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_extend_batch_args>("attn_extend_batch", 1, qkv, nullptr, rope_cos, rope_sin, k_cache, v_cache, out,
+                                                     n_heads, n_kv, scale,
+                                                     segment_shapes("attn_extend_batch", qkv, slots, starts, n_tokens, out, n_heads, n_kv));
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    const Segments seg(slots, starts, n_tokens);
+    seg.into(a);
+    a.n_slots = (int)k_cache.size(0);
+    check_status(sqllm_attn_extend_batch(&a, cur_stream()), "quant_cuda.attn_extend_batch");
+}
+
+// attn_extend_batch in a page pool (sqllm_attn_extend_batch_paged): segment i through row slots[i] of block_table [n_slots, width].
+void attn_extend_batch_paged(torch::Tensor qkv, std::vector<int64_t> slots, std::vector<int64_t> starts, std::vector<int64_t> n_tokens,
+                             torch::Tensor rope_cos, torch::Tensor rope_sin, torch::Tensor k_pages, torch::Tensor v_pages,
+                             torch::Tensor block_table, torch::Tensor out, int64_t n_heads, int64_t n_kv, double scale) {
+    auto a = attn_args<sqllm_attn_extend_batch_paged_args>(
+        "attn_extend_batch_paged", 1, qkv, nullptr, rope_cos, rope_sin, k_pages, v_pages, out, n_heads, n_kv, scale,
+        segment_shapes("attn_extend_batch_paged", qkv, slots, starts, n_tokens, out, n_heads, n_kv), &block_table);
+    const at::cuda::OptionalCUDAGuard guard(device_of(qkv));
+    const Segments seg(slots, starts, n_tokens);
+    seg.into(a);
+    a.n_slots = (int)block_table.size(0);
+    check_status(sqllm_attn_extend_batch_paged(&a, cur_stream()), "quant_cuda.attn_extend_batch_paged");
 }
 
 // One token per row of logits (sqllm_sample): greedy, or temperature / top-k / top-p filtering and a Gumbel-max draw keyed by seed[b]
@@ -997,6 +1069,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "its block table row [ceil(capacity / 64)]; an entry outside the pool among the chunk's blocks writes nothing", py::arg("qkv"),
           py::arg("start"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_pages"), py::arg("v_pages"), py::arg("block_table_row"),
           py::arg("out"), py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_extend_batch", &attn_extend_batch, "attn_extend for several sequences in one call: segment i is n_tokens[i] tokens of "
+          "slot slots[i] at positions starts[i] .. (int lists), rows of qkv [sum T, ...] and out [sum T, ...] in the lists' order, on caches "
+          "[n_slots, n_kv, capacity, head_dim]; each segment bitwise what attn_extend computes for its slot alone", py::arg("qkv"),
+          py::arg("slots"), py::arg("starts"), py::arg("n_tokens"), py::arg("rope_cos"), py::arg("rope_sin"), py::arg("k_cache"),
+          py::arg("v_cache"), py::arg("out"), py::arg("n_heads"), py::arg("n_kv"), py::arg("scale"));
+    m.def("attn_extend_batch_paged", &attn_extend_batch_paged, "attn_extend_batch on KV page pools [n_pages, n_kv, 64, head_dim]: segment i "
+          "through row slots[i] of block_table [n_slots, ceil(capacity / 64)]; a segment with a table entry outside the pool among its "
+          "blocks writes nothing", py::arg("qkv"), py::arg("slots"), py::arg("starts"), py::arg("n_tokens"), py::arg("rope_cos"),
+          py::arg("rope_sin"), py::arg("k_pages"), py::arg("v_pages"), py::arg("block_table"), py::arg("out"), py::arg("n_heads"),
+          py::arg("n_kv"), py::arg("scale"));
     m.def("attn_verify", &attn_verify, "decode attention of T <= 16 new tokens at device positions pos .. pos+T-1: rotary, the append of k / "
           "v at those slots, per token softmax(scale q K^T[0..p_t]) V[0..p_t] (qkv [T, ...], pos int32 [1], rope_cos, rope_sin, k_cache, "
           "v_cache, out [T, ...], n_heads, n_kv, scale); pos < 0 or pos + T > capacity writes nothing; current stream",

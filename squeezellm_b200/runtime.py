@@ -10,6 +10,7 @@ It exists because the reference drives the path from Python one launch at a time
 (llama.py:226-234, quant_cuda_kernel.cu:147), which costs more host time per call than the kernels take on an
 H100; our kernels launch on the current stream precisely so that they can be captured.
 """
+import itertools
 import math
 import numbers
 from typing import NamedTuple
@@ -711,39 +712,69 @@ class _DecoderBase:
         self._set_pos(slot, T)
         return o.logits[0, -1]
 
-    def _extend(self, who, slot, input_ids):
-        """The tokens input_ids (1-D) at `slot`'s positions start .. start+T-1 (start: its position, 0 for an idle slot) through every
-        layer, EXTEND_CHUNK tokens at a time, with quant_cuda.attn_extend on the slot's caches; the slot's position becomes start + T.
-        The logits of the last token.  ValueError before anything is written when the prompt is empty, not 1-D or does not fit."""
-        start = max(self._pos[slot], 0)
-        ids = torch.as_tensor(input_ids)
-        if ids.dim() != 1 or ids.numel() == 0:
-            raise ValueError(f"{who}: input_ids must be a non-empty 1-D tensor of token ids (got shape {tuple(ids.shape)})")
-        if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
-            raise ValueError(f"{who}: input_ids must hold integer token ids (got {ids.dtype})")
-        if start + ids.numel() > self.max_len:
-            raise ValueError(f"{who}: {ids.numel()} tokens at position {start} need {start + ids.numel()} cache positions, "
-                             f"max_len is {self.max_len}")
-        self._reserve({slot: (start + ids.numel(), False)})
-        ids = ids.to(device=self.device, dtype=torch.int64)
+    def _extend(self, who, prompts, named=False):
+        """The prompts [(slot, input_ids (1-D))], each at its slot's positions start .. start+T-1 (start: its position, 0 for an idle
+        slot), through every layer; the slots must be distinct.  A pass takes the next EXTEND_CHUNK tokens of the prompts in the given
+        order, so a prompt may span passes; a pass's segments are (slot, its position so far, its tokens in the pass).  A pass of one
+        segment attends with quant_cuda.attn_extend (or attn_extend_paged) on the slot's caches, one of several with
+        quant_cuda.attn_extend_batch (or attn_extend_batch_paged).  Each slot's position becomes start + T.  -> the logits of each
+        prompt's last token [len(prompts), vocab].  ValueError before anything is written when a prompt is empty, not 1-D or does not
+        fit (named: the message names the prompt's index); paged, RuntimeError with nothing changed when the pool lacks pages."""
+        work = []  # (slot, start, ids)
+        for k, (slot, input_ids) in enumerate(prompts):
+            what = f"{who}: prompt {k}" if named else who
+            start = max(self._pos[slot], 0)
+            ids = torch.as_tensor(input_ids)
+            if ids.dim() != 1 or ids.numel() == 0:
+                raise ValueError(f"{what}: input_ids must be a non-empty 1-D tensor of token ids (got shape {tuple(ids.shape)})")
+            if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+                raise ValueError(f"{what}: input_ids must hold integer token ids (got {ids.dtype})")
+            if start + ids.numel() > self.max_len:
+                raise ValueError(f"{what}: {ids.numel()} tokens at position {start} need {start + ids.numel()} cache positions, "
+                                 f"max_len is {self.max_len}")
+            work.append((slot, start, ids))
+        self._reserve({slot: (start + ids.numel(), False) for slot, start, ids in work})
+        ids = torch.cat([x.to(device=self.device, dtype=torch.int64) for _, _, x in work])
+        ends = list(itertools.accumulate(x.numel() for _, _, x in work))  # prompt k is tokens begins[k] .. ends[k]-1 of ids
+        begins = [e - x.numel() for e, (_, _, x) in zip(ends, work)]
+        last = [None] * len(work)
         m = self.model.model
         with torch.no_grad():
             for c0 in range(0, ids.numel(), self.EXTEND_CHUNK):
-                chunk = ids[c0:c0 + self.EXTEND_CHUNK]
-                out = torch.empty(chunk.numel(), self.n_heads * self.head_dim, dtype=self.dtype, device=self.device)
-                h = torch.index_select(m.embed_tokens.weight, 0, chunk)
+                c1 = min(ids.numel(), c0 + self.EXTEND_CHUNK)
+                segs = []  # (prompt, slot, start, tokens) of the pass
+                for k, (slot, start, _) in enumerate(work):
+                    a, b = max(c0, begins[k]), min(c1, ends[k])
+                    if a < b:
+                        segs.append((k, slot, start + a - begins[k], b - a))
+                out = torch.empty(c1 - c0, self.n_heads * self.head_dim, dtype=self.dtype, device=self.device)
+                h = torch.index_select(m.embed_tokens.weight, 0, ids[c0:c1])
                 for i, layer in enumerate(m.layers):
                     def attend(qkv, i=i):
+                        if len(segs) == 1:
+                            _, slot, start, _ = segs[0]
+                            if self._pages is None:
+                                self._qc.attn_extend(qkv, start, self.rope_cos, self.rope_sin, self._k[i, slot], self._v[i, slot], out,
+                                                     self.n_heads, self.n_kv, self.scale)
+                            else:
+                                self._qc.attn_extend_paged(qkv, start, self.rope_cos, self.rope_sin, self._k[i], self._v[i],
+                                                           self.block_table[slot], out, self.n_heads, self.n_kv, self.scale)
+                            return out
+                        slots, starts, counts = ([s[j] for s in segs] for j in (1, 2, 3))
                         if self._pages is None:
-                            self._qc.attn_extend(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i, slot], self._v[i, slot], out,
-                                                 self.n_heads, self.n_kv, self.scale)
+                            self._qc.attn_extend_batch(qkv, slots, starts, counts, self.rope_cos, self.rope_sin, self._k[i], self._v[i],
+                                                       out, self.n_heads, self.n_kv, self.scale)
                         else:
-                            self._qc.attn_extend_paged(qkv, start + c0, self.rope_cos, self.rope_sin, self._k[i], self._v[i],
-                                                       self.block_table[slot], out, self.n_heads, self.n_kv, self.scale)
+                            self._qc.attn_extend_batch_paged(qkv, slots, starts, counts, self.rope_cos, self.rope_sin, self._k[i],
+                                                             self._v[i], self.block_table, out, self.n_heads, self.n_kv, self.scale)
                         return out
                     h = self._layer(i, layer, h, attend)
-            logits = self.model.lm_head(m.norm(h[-1:]))[0]
-        self._set_pos(slot, start + ids.numel())
+                for k, *_ in segs:
+                    if ends[k] <= c1:
+                        last[k] = h[ends[k] - 1 - c0:ends[k] - c0]
+            logits = self.model.lm_head(m.norm(torch.cat(last)))
+        for slot, start, x in work:
+            self._set_pos(slot, start + x.numel())
         return logits
 
     def _replay(self):
@@ -956,7 +987,7 @@ on the decoder's own kernels (extend), which also appends a new turn to the sequ
         layers' projections, EXTEND_CHUNK tokens at a time), advance the position by T and return the logits of the last token.  After
         reset() this is a prefill; after prefill(), steps or an earlier extend it continues the sequence (a new turn of a chat, say).
         Raises ValueError, with nothing written, for an empty or non-1-D prompt or one that does not fit in max_len."""
-        return self._extend("SequenceDecoder.extend", 0, input_ids)
+        return self._extend("SequenceDecoder.extend", [(0, input_ids)])[0]
 
     def step(self, token_id):
         """Feed token_id (an int or a one-element device tensor) at the current position; returns the next-token logits, a static buffer
@@ -1226,7 +1257,28 @@ class BatchDecoder(_DecoderBase):
         SequenceDecoder.extend does, advance the slot's position by T and return the logits of the last token.  It reads and writes
         nothing of the other slots, so it may run between steps while they keep their state.  Raises ValueError, with nothing written,
         for a bad slot, an empty or non-1-D prompt or one that does not fit in max_len."""
-        return self._extend("BatchDecoder.extend", self._slot(slot), input_ids)
+        return self._extend("BatchDecoder.extend", [(self._slot(slot), input_ids)])[0]
+
+    def extend_many(self, slots, prompts):
+        """Append prompts[i] (1-D token ids) to slots[i] at its position (0 for an idle slot) for every i in one run through the model,
+        advance each slot's position by its prompt's length and return the logits of each prompt's last token, [len(slots), vocab] in
+        the given order.  This is extend() for several slots at once: the prompts' tokens go through the projections together,
+        EXTEND_CHUNK rows per pass (a prompt may span passes), and each layer's attention runs every prompt's rows of the pass in one
+        quant_cuda.attn_extend_batch call (a pass with one prompt's rows runs attn_extend, as extend() does).  A slot's cache ends up
+        bitwise as extend() would leave it, and its logits are those of its own prompt (the projections of a row do not depend on the
+        other rows' values, though the kernel that runs them depends on how many rows a pass holds).  Slots not named are neither
+        read nor written, so the others keep their state; forked slots may take different turns.  Admitting several short prompts
+        this way reads the weights once per pass instead of once per prompt.
+        Raises ValueError, with nothing written, unless slots and prompts have one length in 1..batch, the slots are distinct valid
+        slots, and every prompt is a non-empty 1-D integer tensor that fits in max_len at its slot's position (the message names the
+        prompt's index); paged, RuntimeError naming the slots, with nothing changed, when the pool cannot hold every prompt's pages."""
+        slots, prompts = list(slots), list(prompts)
+        if len(slots) != len(prompts) or not 1 <= len(slots) <= self.batch:
+            raise ValueError(f"BatchDecoder.extend_many: {len(slots)} slots and {len(prompts)} prompts; want one length in 1..{self.batch}")
+        slots = [self._slot(s) for s in slots]
+        if len(set(slots)) != len(slots):
+            raise ValueError(f"BatchDecoder.extend_many: the slots must be distinct (got {slots})")
+        return self._extend("BatchDecoder.extend_many", list(zip(slots, prompts)), named=True)
 
     def step(self, token_ids):
         """Feed token_ids ([batch] ints or a device tensor; only the active slots' entries matter) at each active slot's position;
